@@ -1,5 +1,5 @@
 """Drop-in namespace: `from basic_pitch import ICASSP_2022_MODEL_PATH`, `from basic_pitch.inference import predict`
-keep working unchanged on top of the B200 implementation (package `basic_pitch_b200`).
+keep working unchanged on top of the H100 implementation (package `basic_pitch_b200`).
 Mirrors the public names of reference: basic_pitch/__init__.py:74-95."""
 from basic_pitch_b200 import (  # noqa: F401
     ICASSP_2022_MODEL_PATH,

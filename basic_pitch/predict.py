@@ -1,5 +1,5 @@
 """Drop-in for reference: basic_pitch/predict.py (the `basic-pitch` console entry point): `python -m basic_pitch.predict`
-forwards to the B200 command line (same flags)."""
+forwards to the command line of basic_pitch_b200 (same flags)."""
 from basic_pitch_b200.predict import main  # noqa: F401
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""basic-pitch hot path, Blackwell-native: audio -> harmonic CQT -> CNN -> note events on sm_100a.
+"""basic-pitch hot path, Hopper-native: audio -> harmonic CQT -> CNN -> note events on sm_90a.
 
 Public names mirror the reference package root (reference: basic_pitch/__init__.py:74-95):
 `FilenameSuffix`, `build_icassp_2022_model_path`, `ICASSP_2022_MODEL_PATH`.  There is exactly one

@@ -1,6 +1,6 @@
-"""ctypes binding of the C ABI declared in include/bp_b200.h (libbp_b200.so, sm_100a).
+"""ctypes binding of the C ABI declared in include/bp_b200.h (libbp_b200.so, sm_90a).
 
-There is no fallback of any kind: if the shared library is missing or no B200 is visible, loading or
+There is no fallback of any kind: if the shared library is missing or no H100 is visible, loading or
 model creation raises.  Build the library with `python -c "import __graft_entry__ as g; g.build()"`
 or `make -C basic_pitch_b200/csrc`.
 """

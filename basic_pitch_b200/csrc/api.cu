@@ -141,8 +141,8 @@ struct bp_model {
   double* d_gauss = nullptr;
   CnnWeights cw{};
   int chunk = 206;  // windows per launch sequence: the M-tiles of every tensor-core layer fill whole waves (bp_model_create)
-  int path = 1;  // 0 = FP32 FFMA everywhere, 1 = tcgen05 with fused epilogues, 2 = tcgen05 keeping the contour activations
-  int n_sms = 148;
+  int path = 1;  // 0 = FP32 FFMA everywhere, 1 = tensor cores with fused epilogues, 2 = tensor cores keeping the contour activations
+  int n_sms = 132;
   struct TcLayer {
     TcConvPlan plan;
     TcConvDev dev{};
@@ -317,7 +317,7 @@ int derive(bp_model* m, cudaStream_t st) {
     CK(cudaMemcpyAsync(L.tiles.p, pl.tiles.data(), pl.tiles.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
     std::vector<uint16_t> b2;
-    tc_build_b2(l, w2src[l], b2);
+    tc_build_b2_full(l, w2src[l], b2);
     CK(L.b2.reserve(b2.size()));
     CK(cudaMemcpyAsync(L.b2.p, b2.data(), b2.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
@@ -579,9 +579,9 @@ int bp_model_create(const void* blob, size_t nbytes, int device, bp_model_t** ou
   DeviceGuard g(device);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
+  if (prop.major != 9 || prop.minor != 0)
     return fail(BP_E_CUDA, std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major) +
-                               std::to_string(prop.minor) + "; this library is built for sm_100a only");
+                               std::to_string(prop.minor) + "; this library is built for sm_90a only");
   bp_model* m = new bp_model();
   m->device = device;
   rc = model_init(m, params, prop);
@@ -625,9 +625,9 @@ static int model_init(bp_model* m, const std::vector<float>& params, const cudaD
   }
   cqt_tc_setup();
   m->n_sms = prop.multiProcessorCount;
-  // largest chunk whose M-tiles make at most two per SM in every layer.  M-tiles advance by 128 - (KH2 - 1) rows (they
-  // overlap by the time taps of the fused conv2): 122 rows of 175 per window in the note layer, 124 / 126 of 174 in the
-  // contour / onset layers -> 206 windows on 148 SMs
+  // chunk of windows: as many as make 2 * n_sms spans of 122 rows in the note layer (175 rows per window), i.e. about four
+  // M-tiles per SM in every layer (M-tiles advance by 64 - (KH2 - 1) rows: they overlap by the time taps of the fused
+  // conv2) -> 184 windows on 132 SMs
   {
     const TcConvSpec ns = tc_note_spec();
     m->chunk = std::max(1, 2 * m->n_sms * (128 - (ns.KH2 - 1)) / ns.rows_per_window);
@@ -701,7 +701,7 @@ int bp_model_refresh(bp_model_t* m) {
 int bp_model_set_path(bp_model_t* m, int path) {
   if (!m) return fail(BP_E_INVALID, "bp_model_set_path: null model");
   if (path < 0 || path > 2)
-    return fail(BP_E_INVALID, "bp_model_set_path: path must be 0 (FP32 FFMA), 1 (tcgen05, fused epilogues) or 2 (tcgen05, "
+    return fail(BP_E_INVALID, "bp_model_set_path: path must be 0 (FP32 FFMA), 1 (tensor cores, fused epilogues) or 2 (tensor cores, "
                               "contour activations kept)");
   m->path = path;
   return BP_OK;

@@ -1,4 +1,4 @@
-// Shared definitions for the sm_100a kernels of the basic-pitch hot path.
+// Shared definitions for the sm_90a kernels of the basic-pitch hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -12,11 +12,16 @@
 //                    10*log10(p + 1e-10), per-window min/max (atomics)       (1 launch per chunk)
 //   lognorm_kernel   (L - min) / (max - min) * bn_scale + bn_bias            (1 launch per chunk)
 #include "kernels.cuh"
-#include "tc_ptx.cuh"
 
 namespace bp {
 
-// Low-pass taps as pairs for the packed FMAs: c_lp2[k] = (h[k - 12], h[k - 14]), zero outside the 256 taps.  A thread that
+// d.{x,y} += o * w.{x,y}: two FMAs whose tap pair is read from constant memory once (Hopper has no packed FP32 FMA)
+__device__ __forceinline__ void ffma2(float2& d, float o, float2 w) {
+  d.x = fmaf(o, w.x, d.x);
+  d.y = fmaf(o, w.y, d.y);
+}
+
+// Low-pass taps as pairs: c_lp2[k] = (h[k - 12], h[k - 14]), zero outside the 256 taps.  A thread that
 // owns outputs 8t .. 8t+7 feeds sample u of its input run into the output pairs (0,1), (2,3), (4,5), (6,7) with
 // c_lp2[u + 12], c_lp2[u + 8], c_lp2[u + 4], c_lp2[u].
 constexpr int kLp2 = kTaps + 14;
@@ -37,7 +42,7 @@ void upload_lowpass(const float* h_lp, cudaStream_t st) {
 // Half-band FIR + decimate by 2:  x_{o+1}[n] = sum_k LP[k] * x_o[2n + k - 127].
 // Input runs live in shared memory de-interleaved into 16 phases (sample li at ph[(li & 15) * S + (li >> 4)], S == 2
 // mod 32: conflict-free scatter and gather); thread t owns outputs 8t .. 8t+7, so every loaded sample feeds up to 8
-// FMAs, issued as 4 packed FMAs (FFMA2) whose tap pairs are uniform-register operands from constant memory.  Each
+// FMAs whose tap pairs are uniform-register operands from constant memory.  Each
 // output still accumulates its 256 products in tap order.
 //   decimate_kernel       stages 0-3: one CTA = 1024 outputs of one window
 //   decimate_tail_kernel  stages 4-7 (2740 -> 171 samples): one CTA per window runs the four stages back to back through

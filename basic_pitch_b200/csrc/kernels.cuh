@@ -38,7 +38,7 @@ void launch_onset2(const float* note, const float* o1, const CnnWeights& w, floa
                    cudaStream_t st);
 
 
-// ---- tc_conv.cu (tcgen05 path of the three wide convolutions, each with its following conv fused) ------------
+// ---- tc_conv.cu (tensor-core path of the three wide convolutions, each with its following conv fused) --------
 struct TcConvSpec {
   int KH, KW, SF, PT, PL, COUT, FLT, WOUT;  // taps, frequency stride, pads, channels, bins per 128-column tile, output bins
   int n_ci;                                 // input channels (harmonics of y, or 1 for the contour posteriorgram)
@@ -64,7 +64,7 @@ struct TcConvPlan {  // host side: weight tiles + the per-group MMA programs
 struct TcConvDev {
   TcConvSpec spec;
   const uint16_t* tiles;
-  const uint16_t* b2;  // conv2 weight tiles of the fused epilogue (tc_build_b2)
+  const uint16_t* b2;  // conv2 weight matrix of the fused epilogue (tc_build_b2_full)
   int n_groups;
   int layer;  // index of the program in constant memory (0 contour, 1 onset, 2 note)
 };
@@ -73,6 +73,8 @@ void tc_upload_epilogue(const float* contour1_b, const float* onset1_b, const fl
                         const float* contour2_b, const float* onset2_b, const float* note2_b, cudaStream_t st);
 // bf16 hi/lo weight tiles of the fused second conv (epi: 0 contour, 1 onset, 2 note; w2 = that conv's weights), see TcB2
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out);
+// the same tiles placed into the K = 128 x N = width conv2 weight matrix the kernel reads (tc_conv.cu)
+void tc_build_b2_full(int epi, const float* w2, std::vector<uint16_t>& out);
 int tc_rows_total(int n_windows, int rows_per_window);
 size_t tc_edge_floats(const TcConvSpec& spec, int n_windows);  // size of the edge buffer of a fused layer
 int tc_setup();  // 0 on success
@@ -116,7 +118,7 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
 void launch_contour2_tc(const float* c1_nhwc, const CnnWeights& w, float* contour, __nv_bfloat16* chl, int rows_total,
                         int n_windows, cudaStream_t st);
 
-// ---- cqt_tc.cu (tcgen05 path of the constant-Q projection, three-way bf16 split) ----------------------------
+// ---- cqt_tc.cu (tensor-core path of the constant-Q projection, three-way bf16 split) ------------------------
 void build_cqt_tc_weights(const float* cqt_real, const float* cqt_imag, std::vector<uint16_t>& out);
 void cqt_tc_setup();
 void launch_cqt_tc(const float* audio, const WinDesc* desc, const float* chain, const uint16_t* wtc, const float* scale,

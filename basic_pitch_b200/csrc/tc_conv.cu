@@ -1,7 +1,7 @@
 // The three wide convolutions — contour (8 -> 8 channels, 3 x 39 taps, 65 % of the model's FLOPs), onset
 // (8 -> 32 channels, 5 x 5 taps, frequency stride 3, 18 %) and note (1 -> 32 channels, 7 x 7, stride 3, 4.5 %) —
-// on the 5th-gen tensor cores: tcgen05.mma (kind::f16, bf16 operands, fp32 accumulators in TMEM), operands staged in shared
-// memory by bulk async copies (UBLKCP) signalled through mbarriers, warp-specialised roles.
+// on the Hopper tensor cores: warpgroup MMAs (wgmma, bf16 operands, fp32 accumulators in registers), operands staged in
+// shared memory by bulk async copies (UBLKCP) signalled through mbarriers, warp-specialised roles.
 //
 // Replaces nodes 231/232 (contour conv + ReLU, reference: basic_pitch/models.py:241-250) and 230/243 (onset
 // conv + ReLU, reference: basic_pitch/models.py:295-304) of the deployed graph, and the harmonic stacking in
@@ -11,12 +11,12 @@
 // the FOLLOWING single-output convolution (onset conv2 models.py:305-313, note conv2 :282-290, contour conv2 :254-262)
 // completely, so neither the 8- / 32-channel activations nor any partial sums of them reach HBM:
 //   * channels and frequency taps are reduced by a SECOND tensor-core contraction whose A operand is bias + ReLU of the
-//     accumulator, split to bf16 hi/lo and written back into the same tensor-memory columns (TS-form MMAs, see TcB2),
-//   * the time taps are summed across the lanes of the warp (the 32 lanes hold 32 consecutive frames: shuffles) and
-//     across the four epilogue warps of an accumulator slot through a small shared-memory exchange; M-tiles overlap
-//     by KH2 - 1 rows, so every frame is complete in exactly one tile.  The thread of tile row r finishes the output
-//     frame r - H (H = KH2 / 2), so every tap comes from a lane at or below its own: each lane adds its taps in the
-//     same order whatever its position in the tile, and a frame's value does not depend on the batch around it,
+//     conv1 accumulator, split to bf16 hi/lo straight in the registers (the accumulator fragment of wgmma is the A
+//     register fragment of the next K = 16 step), against a conv2 weight matrix in shared memory (TcB2),
+//   * its sums go through a small shared-memory staging area, where the thread of each tile row adds the time taps of
+//     the rows below it; M-tiles overlap by KH2 - 1 rows, so every frame is complete in exactly one tile.  The thread
+//     of tile row r finishes the output frame r - H (H = KH2 / 2) and adds its taps in the same order whatever its
+//     position in the tile, so a frame's value does not depend on the batch around it,
 //   * the frequency halo between neighbouring tiles is a register carry: a slot walks its frequency tiles in ascending
 //     order; only where two tile RANGES meet (slot 0 | slot 1, or the group splits of a small batch) the two partial
 //     sums go to a small edge buffer and edge_fix_kernel finishes those 4 (contour) / 2 bins,
@@ -37,29 +37,23 @@
 //            N = FLT output bins x COUT channels = 128 (contour 16 x 8, onset / note 4 x 32); a tile depends on
 //            (dt, 8c - SF*FLT*ft), so frequency tiles SF*FLT*d = 8*j bins apart share tiles (de-duplicated by
 //            content)
-//   every (ft, dt, c) with a non-empty tile is one K=16 MMA step of shape 128 x 128 x 16
+//   every (ft, dt, c) with a non-empty tile is one K=16 MMA step of shape 64 x 128 x 16
 // Precision: both operands are split x = hi + lo (bf16 each) and three products are accumulated
 // (hi*hi + hi*lo + lo*hi) in fp32, which keeps the posteriorgrams within ~1e-5 of the FP32 path
 // (SURVEY.md Appendix C.4); a single bf16 product would miss the 1e-3 bar.
 //
-// Work decomposition: item = (M-tile of 128 rows, split s of S over the frequency groups); group g = the two
-// frequency tiles {g, g + G0} (two accumulator slots; shared weight tiles where their content is equal).  Tensor memory:
-// three 128-column conv1 accumulator regions used as a ring + the conv2 accumulators.  A CTA (1 per SM, persistent) walks items
-// i = blockIdx.x, +gridDim.x, ...:
-//   warp 8      producer: bulk-copies the (128+KH-1) x 320 bf16 hi/lo data tile (k-chunk-major) once per item and
-//               streams the weight tiles of each group's program (8 KB each) through a 7- / 9-stage ring
-//   warps 9, 10 MMA issuers, one per accumulator slot of the group (instruction issue, not the tensor pipe, limits
-//               a single issuing warp at this MMA size): program words from constant memory, descriptors are
-//               base + precomputed offset, 3 x tcgen05.mma per step by one elected lane, tcgen05.commit frees the
-//               weight stage / publishes the accumulators
-//   warp 11     conv2 MMA issuer (A operand in tensor memory)
-//   warps 0-3, 4-7  epilogue, one warpgroup-like set of 4 warps (= the 4 TMEM lane quadrants) per accumulator slot:
-//               tcgen05.ld the accumulator columns, + bias, ReLU, split, tcgen05.st; then the conv2 sums as described above
+// Work decomposition: item = (M-tile of 64 rows, split s of S over the frequency groups); group g = the two
+// frequency tiles {g, g + G0} (two accumulator slots; shared weight tiles where their content is equal).  A CTA (1 per
+// SM, persistent) walks items i = blockIdx.x, +gridDim.x, ...:
+//   warp 8      producer: bulk-copies the (64+KH-1) x 320 bf16 hi/lo data tile (k-chunk-major) once per item and
+//               streams the weight tiles of each group's program (8 KB each) through a ring of stages
+//   warps 0-3, 4-7  one warpgroup per accumulator slot of the group: program words from constant memory, 3 x wgmma
+//               m64n128k16 per step (the stage is released once they completed), then the epilogue of the slot's tile
+//               from the accumulator registers: bias, ReLU, split, the conv2 MMAs, time taps, finish (see above)
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 
 #include <algorithm>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <unordered_map>
@@ -71,46 +65,62 @@
 namespace bp {
 
 namespace tc {
-constexpr int kMTile = 128;
+constexpr int kMTile = 64;
 constexpr int kTileBytes = 8192;                                 // weight tile: [plane 2][kchunk 2][128][8] bf16
 constexpr int kMaxSteps = 1024;                                  // program steps per layer (constant memory)
 constexpr int kMaxGroups = 15;
-constexpr int kThreads = 384;  // 12 warps: 2 x 4 epilogue warps, producer, 2 conv1 MMA issuers, the conv2 MMA issuer
-// The issue arbiter of an SM sub-partition prefers the highest warp id, so the latency-critical single-thread roles
-// (producer, MMA issuers) get the highest ids and are never starved by the epilogue warps.
-constexpr int kProducerWarp = 8, kMmaWarp0 = 9, kMmaWarp1 = 10, kMma2Warp = 11;
-// time-halo exchange between the four epilogue warps of a slot: [slot 2][buffer 2][warp 3][kXchgFloats] (warps 0..2 of a
-// slot publish their top lanes for the warp above; the last warp has nobody to publish to)
-// Shared memory is laid out per layer: the data tile, then as many weight-tile stages as fit.  The weight ring is what
-// bounds the conv1 MMAs (one 8 KB tile per step, about 2 000 cycles from the request to the release of its stage, most
-// steps used by one slot only = 192 tensor cycles), so every KB goes to stages: contour / onset 7, note 9.
+constexpr int kConsumerWarps = 8;  // two warpgroups, one per accumulator slot
+constexpr int kProducerWarp = 8;
+constexpr int kThreads = 32 * kConsumerWarps + 32;
+}  // namespace tc
+
+// ------------------------------------------------------------------------------------------------
+// The fused second convolution as a second tensor-core contraction.
+// After bias + ReLU the conv1 accumulator row (element k = accumulator column k = fl * COUT + c) is split to bf16
+// hi/lo.  A K = 16 step therefore covers
+//   contour: 2 bins x 8 channels        (step ks = bins 2 ks, 2 ks + 1)
+//   onset / note: half the channels of one bin   (step ks = bin ks / 2, channels 16 (ks % 2) ..)
+// and it contributes to the partial sums P[j][dt] of only a few output offsets j (frequency taps) of the tile:
+//   contour: j = bl + 4 - df  in [2 ks, 2 ks + 5]      onset / note: j = fl + 2 - df in [fl, fl + 2]
+// With the conv2 accumulator laid out j-major (column j * JS + dt, JS >= KH2) those are a contiguous WINDOW of columns,
+// the same for every step up to its start column: every step multiplies by the same small weight tile
+//   B2[kk][j' * JS + dt] = w2[c(kk)][dt][df(kk, j')]          (N = 32 columns; onset 16)
+// placed at the window's start column (contour 10 ks, note 8 fl, onset 4 fl) of a K = 128 x N = width matrix
+// (tc_build_b2_full), which the MMAs read from shared memory.
+// ------------------------------------------------------------------------------------------------
+struct TcB2 {
+  int n_tiles, n2, kh2, js, width;  // weight tiles, their N, time taps, columns per output offset j, accumulator columns
+};
+__host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour, 1 onset, 2 note
+  return epi == 1 ? TcB2{2, 16, 3, 4, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64} : TcB2{1, 32, 5, 5, 104};
+}
+
+namespace tc {
+// Shared memory is laid out per layer: the data tile, as many weight-tile stages as fit, and for the fused layers the
+// conv2 weight matrix and the staging of the conv2 sums.
 struct TcSmem {
-  int data_bytes;   // [2 planes][chunks][128 + KH - 1 rows][16 B], rounded up to 1 KB
-  int xchg_floats;  // per publishing warp (contour 10 lane values x 20 offsets, note 21 x 6, onset 3 x 6)
-  int b2_bytes;     // conv2 weight tiles (TcB2)
+  int data_bytes;   // [2 planes][chunks][64 + KH - 1 rows][16 B], rounded up to 1 KB
+  int b2_bytes;     // conv2 weight matrix [2 planes][128][width] bf16
+  int p_bytes;      // conv2 sums [2 slots][64 rows][width + 1] fp32
   int stages;
-  __host__ __device__ constexpr int xchg_bytes() const { return 2 * 2 * 3 * xchg_floats * 4; }
-  __host__ __device__ constexpr int total() const { return data_bytes + stages * kTileBytes + xchg_bytes() + b2_bytes + 512; }
+  __host__ __device__ constexpr int total() const { return data_bytes + stages * kTileBytes + b2_bytes + p_bytes + 512; }
 };
 constexpr int kMaxSmem = 232448;  // 227 KB opt-in per CTA
-__host__ __device__ constexpr TcSmem tc_smem(int epi) {  // epi: 0 / 3 contour, 1 onset, 2 note
+constexpr int kMaxStages = 12;
+__host__ __device__ constexpr TcSmem tc_smem(int epi) {  // epi: 0 contour (activations), 1 onset, 2 note, 3 contour (fused)
   TcSmem s{};
   const int chunks = epi == 2 ? 33 : 39, rows = kMTile + (epi == 1 ? 4 : epi == 2 ? 6 : 2);
+  const int width = tc_b2_spec(epi).width;
   s.data_bytes = (2 * chunks * rows * 16 + 1023) / 1024 * 1024;
-  s.xchg_floats = epi == 1 ? 32 : epi == 2 ? 128 : 200;
-  s.b2_bytes = epi == 2 ? 4096 : 2048;
-  s.stages = (kMaxSmem - 512 - s.data_bytes - s.xchg_bytes() - s.b2_bytes) / kTileBytes;
+  s.b2_bytes = epi == 0 ? 0 : 2 * 128 * width * 2;
+  s.p_bytes = epi == 0 ? 0 : 2 * 64 * (width + 1) * 4;
+  const int st = (kMaxSmem - 512 - s.data_bytes - s.b2_bytes - s.p_bytes) / kTileBytes;
+  s.stages = st < kMaxStages ? st : kMaxStages;
   return s;
 }
-static_assert(tc_smem(0).stages == 7 && tc_smem(1).stages == 7 && tc_smem(2).stages == 9, "weight ring depth");
-constexpr int kMaxStages = 9;
 // step word of a slot: [0,14) A start-address offset >> 4, [15] first MMA into that accumulator; kNoUse = the
 // slot's frequency tile does not use this step's weight tile
 constexpr uint32_t kUseFirstAcc = 1u << 15, kNoUse = 0xffffffffu;
-// Tensor memory (512 columns): three 128-column conv1 accumulators used as a ring by the frequency tiles in program order,
-// then the conv2 accumulators (per-layer widths in TcB2).
-constexpr int kRegions = 3;
-constexpr uint32_t kD2Base = kRegions * 128;
 }  // namespace tc
 
 // ------------------------------------------------------------------------------------------------
@@ -316,30 +326,6 @@ void tc_upload_epilogue(const float* contour1_b, const float* onset1_b, const fl
   cudaStreamSynchronize(st);
 }
 
-// ------------------------------------------------------------------------------------------------
-// The fused second convolution as a second tensor-core contraction (A operand in tensor memory).
-// After bias + ReLU the epilogue threads write relu(conv1) of their frame back into the accumulator's own 128 columns as
-// a bf16 hi/lo split (two elements per column: per 32-column chunk 16 columns hi, 16 columns lo); element k of the row is
-// the accumulator column k = fl * COUT + c.  A K = 16 step therefore covers
-//   contour: 2 bins x 8 channels        (step ks = bins 2 ks, 2 ks + 1)
-//   onset / note: half the channels of one bin   (step ks = bin ks / 2, channels 16 (ks % 2) ..)
-// and it contributes to the partial sums P[j][dt] of only a few output offsets j (frequency taps) of the tile:
-//   contour: j = bl + 4 - df  in [2 ks, 2 ks + 5]      onset / note: j = fl + 2 - df in [fl, fl + 2]
-// With the conv2 accumulator laid out j-major (column j * JS + dt, JS >= KH2) those are a contiguous WINDOW of columns,
-// the same for every step up to its start column: every step multiplies by the same small weight tile
-//   B2[kk][j' * JS + dt] = w2[c(kk)][dt][df(kk, j')]          (N = 32 columns; onset 16)
-// and only the D start column moves (contour 10 ks, note 8 fl, onset 4 fl) — tcgen05.mma takes any EVEN start column.  The
-// windows overlap, so all products accumulate into an accumulator the epilogue zeroes after reading it.
-// What is left for the CUDA cores is bias / ReLU / split (5 instructions per value) and the time taps (shuffles).
-// ------------------------------------------------------------------------------------------------
-struct TcB2 {
-  int n_tiles, n2, kh2, js, width;  // weight tiles, their N, time taps, columns per output offset j, accumulator columns
-};
-// (the D start column of an MMA must be even — an odd one raises a misaligned-address fault — hence js = 4 / 8, not 3 / 7)
-__host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour, 1 onset, 2 note
-  return epi == 1 ? TcB2{2, 16, 3, 4, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64} : TcB2{1, 32, 5, 5, 104};
-}
-
 // tiles: [tile][plane hi/lo][k-chunk 2][n N2][8] bf16 (canonical K-major no-swizzle: LBO = N2 * 16 B, SBO = 128 B)
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
   const TcB2 sp = tc_b2_spec(epi);
@@ -378,6 +364,24 @@ int tc_upload_program(int layer, const TcConvPlan& pl, cudaStream_t st) {
   cudaMemcpyToSymbolAsync(c_group_ft, pl.group_ft.data(), pl.group_ft.size() * 4, (size_t)layer * 2 * tc::kMaxGroups * 4,
                           cudaMemcpyHostToDevice, st);
   return cudaStreamSynchronize(st) == cudaSuccess ? 0 : -1;
+}
+
+// The small tiles expanded into the K = 128 x N = width matrix the conv2 MMAs read:
+// [plane hi/lo][k-chunk 16][n width][8] bf16 (K-major no-swizzle: LBO = width * 16 B, SBO = 128 B)
+void tc_build_b2_full(int epi, const float* w2, std::vector<uint16_t>& out) {
+  const TcB2 sp = tc_b2_spec(epi);
+  std::vector<uint16_t> small;
+  tc_build_b2(epi, w2, small);
+  const size_t tile_elems = (size_t)2 * 16 * sp.n2, plane = (size_t)128 * sp.width;
+  out.assign(2 * plane, 0);
+  for (int ks = 0; ks < 8; ++ks) {
+    const int col0 = (epi == 0 || epi == 3) ? 10 * ks : sp.js * (ks >> 1), tl = (epi == 0 || epi == 3) ? 0 : ks & 1;
+    for (int pl = 0; pl < 2; ++pl)
+      for (int kk = 0; kk < 16; ++kk)
+        for (int n = 0; n < sp.n2; ++n)
+          out[pl * plane + ((size_t)(2 * ks + (kk >> 3)) * sp.width + col0 + n) * 8 + (kk & 7)] =
+              small[(size_t)tl * tile_elems + pl * 16 * sp.n2 + (size_t)(kk >> 3) * sp.n2 * 8 + (size_t)n * 8 + (kk & 7)];
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -455,64 +459,29 @@ struct TcArgs {
   int use_tmap;                 // 0: the encoder was not available, the tile is fetched chunk by chunk with 1-D bulk copies
   const __nv_bfloat16* data;    // [2][chunks8][rows_total][8]
   const uint16_t* tiles;        // [n_tiles][8192 B]
-  const uint16_t* b2;           // conv2 weight tiles (tc_build_b2), fused layers
-  int dbg_skip_loads;           // -DBP_TC_TRACE builds: the producer only pretends to load weight tiles (timing experiment)
-  long long* trace;             // -DBP_TC_TRACE builds: [tile][8] clock64 stamps of CTA 0 (see tc_trace)
+  const uint16_t* b2;           // conv2 weight matrix (tc_build_b2_full), fused layers
   TcOut o;                      // where the results go (kernels.cuh)
   int edge_rows;                // row stride of o.edge: [edge slot][side 2][KE][edge_rows]
   int layer;                    // which constant-memory program (0 contour, 1 onset, 2 note)
   int rows_total, n_mtiles, n_windows;
   int n_groups, n_split;        // an item covers groups [s*n_groups/n_split, (s+1)*n_groups/n_split)
-  int data_rows, row0;          // tile rows (128 + KH - 1); first data row of M-tile 0
-  int ms, h2;                   // M-tile stride (128 - 2*h2) and time halo of the fused conv2
+  int data_rows, row0;          // tile rows (64 + KH - 1); first data row of M-tile 0
+  int ms, h2;                   // M-tile stride (64 - 2*h2) and time halo of the fused conv2
   int chunks8, rows_per_window;
   int cout, flt, wout, n_ft, g0;
 };
 
-// Pipeline trace (debug builds with -DBP_TC_TRACE and BP_TC_TRACE=1 in the environment): CTA 0 stamps, per frequency tile n,
-// 0 conv1 region acquired, 1 conv1 MMAs issued, 2 epilogue saw the accumulator, 3 split written back, 4 conv2 MMA warp
-// released, 5 conv2 MMAs issued, 6 epilogue saw the conv2 sums, 7 tile finished.
-#ifdef BP_TC_TRACE
-#define TC_TRACE(n, ev)                                                                                       \
-  do {                                                                                                        \
-    if (a.trace && blockIdx.x == 0 && (n) < 256u && lane == 0) a.trace[(n) * 8u + (ev)] = clock64();            \
-  } while (0)
-#else
-#define TC_TRACE(n, ev) \
-  do {                  \
-  } while (0)
-#endif
-
 __device__ __forceinline__ float sigmoidf_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 
-__device__ __forceinline__ void slot_barrier(int slot) {  // the four epilogue warps of one accumulator slot
+__device__ __forceinline__ void slot_barrier(int slot) {  // the four warps (one warpgroup) of one accumulator slot
   asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
-}
-
-// Time taps of the fused conv2 across frames.  The thread of tile row r finishes output frame q = r - H of the tile's row
-// space: out[q] = sum_dt P_dt[q + dt - H] = sum_a P_{2H-a}[row r - a], a = 0 .. 2H, i.e. every source is `a` lanes BELOW the
-// thread.  Sources inside the warp come by shuffle; lanes < a of warps 1..3 take them from the values the previous warp
-// published (lanes 32-a .. 31 -> entries a(a-1)/2 + lane - (32-a)) after the slot barrier (time_edges).  A lane adds
-// a = 0, 1, .., 2H in this order in both places, so the rounding of a frame does not depend on its row in the tile.
-// (The in-warp part is written out in pitch_tile_taps / contour_tile, the cross-warp part is time_edges.)
-template <int H, int NJ>
-__device__ __forceinline__ void time_edges(float (&S)[NJ], int quad, int lane, const float* xb /* [3][XF] */, int XF) {
-  if (quad == 0) return;
-#pragma unroll
-  for (int a = 1; a <= 2 * H; ++a) {
-    if (lane < a) {  // source `a` rows below: lane 32 - a + lane of the previous warp
-      const float* e = xb + (quad - 1) * XF + (a * (a - 1) / 2 + lane) * NJ;
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) S[j] += e[j];
-    }
-  }
 }
 
 // Edge-buffer slot of the tile range that slot `s` of split `q` walks (it starts at tile g0(q) + s * G0): s * n_split + q.
 // The range that ENDS below it is slot s of split q - 1, or, for (s, q) = (1, 0), slot 0 of the last split.
 
-// What the epilogue thread of one frame knows about where its results go.  All stores are coalesced: the 32 lanes of a
-// warp hold 32 consecutive frames, and every layout below has the frame index fastest.
+// What the thread that finishes one frame knows about where its results go.  The threads of a warp hold consecutive
+// frames, and every layout below has the frame index fastest.
 //   pitch layers (note / onset)  pitch-major planes  [pitch][frame]
 //   contour                      chunk-major         [8-bin chunk][frame][8]  (fp32), same shape as the bf16 hi/lo
 //                                split layout [plane][chunk][row][8] that the note conv reads
@@ -526,75 +495,6 @@ struct RowOut {
   bool ok;       // live output frame whose time taps are complete in this M-tile
   int e_lo, e_hi;  // edge slots of this range's start and of the range above its end (-1: none)
 };
-
-// relu(conv1 + bias) of one accumulator row -> bf16 hi/lo split written back IN PLACE: the A operand of the conv2 MMAs
-// (TcB2).  Per 32-column chunk q (elements k = 32 q .. 32 q + 31 of the row): columns [32 q, 32 q + 16) hold the hi
-// halves, [32 q + 16, 32 q + 32) the lo halves, two elements per column (element 2 c in the low 16 bits).  Rows that are
-// not live frames and the bins >= 264 of the last contour tile become zeros.
-template <int LAYER>
-__device__ __forceinline__ void convert_tile(uint32_t taddr, bool live, int n_valid) {
-#pragma unroll 1
-  for (int q = 0; q < 4; ++q) {
-    uint32_t v[32];
-    tmem_ld32_nowait(taddr + q * 32, v);
-    tmem_ld_wait();
-    const bool ok = live && q * 32 < n_valid;  // n_valid is a multiple of 32 (contour: 64 in the last tile, else 128)
-    uint32_t hi[16], lo[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int c0 = LAYER == 0 ? ((2 * i) & 7) : 2 * i;  // channel of accumulator column 32 q + 2 i
-      const float o0 = ok ? fmaxf(__uint_as_float(v[2 * i]) + c_bias1[LAYER][c0], 0.f) : 0.f;
-      const float o1 = ok ? fmaxf(__uint_as_float(v[2 * i + 1]) + c_bias1[LAYER][c0 + 1], 0.f) : 0.f;
-      const __nv_bfloat162 h = __floats2bfloat162_rn(o0, o1);
-      const uint32_t hu = *reinterpret_cast<const uint32_t*>(&h);
-      const __nv_bfloat162 l = __floats2bfloat162_rn(o0 - __uint_as_float(hu << 16), o1 - __uint_as_float(hu & 0xffff0000u));
-      hi[i] = hu;
-      lo[i] = *reinterpret_cast<const uint32_t*>(&l);
-    }
-    tmem_st16(taddr + q * 32, hi);
-    tmem_st16(taddr + q * 32 + 16, lo);
-  }
-  tmem_st_wait();
-}
-
-// Onset / note layers after the conv2 MMAs: the conv2 accumulator holds, for the thread's frame, P[j][dt] (column
-// j * JS + dt) = sum over channels and frequency taps for output offset j = 0 .. 5 (bins 4 ft - 1 + j) and time tap dt.
-// Reads them, zeroes the accumulator and hands it back, then sums the time taps: S[j] = sum_dt P[j][dt][frame + dt - H],
-// sources inside the warp by shuffle, the top lanes published for the next warp (see time_edges).
-template <int KH2>
-__device__ __forceinline__ void pitch_tile_taps(uint32_t d2, int lane, int quad, float* pub, uint64_t* d2_empty, float (&S)[6]) {
-  const int pub_from = quad < 3 ? 32 : 64;  // the last warp of a slot publishes nothing
-  constexpr int JS = KH2 == 7 ? 8 : 4;  // columns per output offset (TcB2::js)
-  uint32_t d[48];
-  tmem_ld32_nowait(d2, reinterpret_cast<uint32_t(&)[32]>(d[0]));
-  if constexpr (KH2 == 7) tmem_ld16_nowait(d2 + 32, reinterpret_cast<uint32_t(&)[16]>(d[32]));
-  tmem_ld_wait();
-  tmem_zero<32>(d2);
-  if constexpr (KH2 == 7) {
-    tmem_zero<16>(d2 + 32);
-    tmem_zero<8>(d2 + 48);
-  }
-  tmem_st_wait();
-  tc_fence_before();
-  __syncwarp();
-  if (lane == 0) mbar_arrive(d2_empty);
-#pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    float s = 0.f;
-#pragma unroll
-    for (int a = 0; a < KH2; ++a) {
-      const float p = __uint_as_float(d[j * JS + (KH2 - 1 - a)]);
-      if (a == 0) {
-        s += p;
-      } else {
-        const float v = __shfl_up_sync(0xffffffffu, p, a);
-        if (lane >= a) s += v;
-        if (lane >= pub_from - a) pub[(a * (a - 1) / 2 + lane - (32 - a)) * 6 + j] = p;
-      }
-    }
-    S[j] = s;
-  }
-}
 
 // Frequency halo + finish for the onset / note layers (FLT = 4, halo 1): S[j] is the time-complete sum for bin 4 ft - 1 + j.
 template <int EPI>
@@ -616,7 +516,7 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
   const int jhi = (ft == a.n_ft - 1) ? 5 : 4;  // the last tile also finishes its top bin (no tile above)
   if (ro.ok) {
     float nv[3][6];
-    if constexpr (EPI == 1) {  // note frames t-1 .. t+1, pitches 4 ft - 2 .. 4 ft + 3 (zero outside the image); lanes run along t
+    if constexpr (EPI == 1) {  // note frames t-1 .. t+1, pitches 4 ft - 2 .. 4 ft + 3 (zero outside the image)
 #pragma unroll
       for (int c = 0; c < 6; ++c) {
         const int f = 4 * ft - 2 + c;
@@ -670,90 +570,14 @@ __device__ __forceinline__ void store_contour_chunk(const TcArgs& a, const RowOu
   }
 }
 
-// Contour layer after the conv2 MMAs (8 -> 1 channels, 5 x 5 taps, models.py:252-259): the conv2 accumulator holds
-//   P[j][dt] (column j * 5 + dt) = sum_{c, df} relu(conv1)[c][t][16 ft + j + df - 4] * w2[c][dt][df]     j = 0 .. 19
-// for output bins 16 ft - 2 + j of the thread's frame.  Time taps by shuffles (see time_edges), frequency halo by register
-// carry, then sigmoid and the stores.
-__device__ __forceinline__ void contour_tile(const TcArgs& a, const RowOut& ro, uint32_t d2, uint64_t* d2_empty, int ft,
-                                             bool first, bool last, int quad, int lane, int slot, float* xb,
-                                             float (&carry)[4], float (&hold)[6]) {
-  float S[20];
-  float* pub = xb + quad * tc::tc_smem(3).xchg_floats;
-  const int pub_from = quad < 3 ? 32 : 64;  // the last warp of a slot publishes nothing
-  // one output offset: its five partial sums p[dt] -> time taps (see time_edges for the cross-warp part)
-  auto taps = [&](int j, const float (&p)[5]) {
-    float s = 0.f;
-#pragma unroll
-    for (int ta = 0; ta < 5; ++ta) {  // source row `ta` below the thread's: time tap dt = 4 - ta
-      const float x = p[4 - ta];
-      if (ta == 0) {
-        s += x;
-      } else {
-        const float v = __shfl_up_sync(0xffffffffu, x, ta);
-        if (lane >= ta) s += v;
-        if (lane >= pub_from - ta) pub[(ta * (ta - 1) / 2 + lane - (32 - ta)) * 20 + j] = x;
-      }
-    }
-    S[j] = s;
-  };
-  // tensor-memory loads want their column naturally aligned: columns 0 .. 63 first (j = 0 .. 11 and four values of
-  // j = 12), then 64 .. 103
-  uint32_t keep[4];
-  {
-    uint32_t d[64];
-    tmem_ld32_nowait(d2, reinterpret_cast<uint32_t(&)[32]>(d[0]));
-    tmem_ld32_nowait(d2 + 32, reinterpret_cast<uint32_t(&)[32]>(d[32]));
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 12; ++j) {
-      float p[5];
-#pragma unroll
-      for (int dt = 0; dt < 5; ++dt) p[dt] = __uint_as_float(d[j * 5 + dt]);
-      taps(j, p);
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) keep[k] = d[60 + k];
-  }
-  {
-    uint32_t d[40];
-    tmem_ld32_nowait(d2 + 64, reinterpret_cast<uint32_t(&)[32]>(d[0]));
-    {
-      uint32_t t8[8];
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                   : "=r"(t8[0]), "=r"(t8[1]), "=r"(t8[2]), "=r"(t8[3]), "=r"(t8[4]), "=r"(t8[5]), "=r"(t8[6]), "=r"(t8[7])
-                   : "r"(d2 + 96));
-#pragma unroll
-      for (int k = 0; k < 8; ++k) d[32 + k] = t8[k];
-    }
-    tmem_ld_wait();
-    // everything is in registers: zero the accumulator and hand it back to the conv2 MMA warp
-    tmem_zero<32>(d2);
-    tmem_zero<32>(d2 + 32);
-    tmem_zero<32>(d2 + 64);
-    tmem_zero<8>(d2 + 96);
-    tmem_st_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(d2_empty);
-#pragma unroll
-    for (int j = 12; j < 20; ++j) {
-      float p[5];
-#pragma unroll
-      for (int dt = 0; dt < 5; ++dt) {
-        const int c = j * 5 + dt;  // column 60 .. 99
-        p[dt] = __uint_as_float(c < 64 ? keep[c - 60] : d[c - 64]);
-      }
-      taps(j, p);
-    }
-  }
-  __syncwarp();
-  slot_barrier(slot);
-  time_edges<2, 20>(S, quad, lane, xb, tc::tc_smem(3).xchg_floats);
-  // frequency halo: S[j] <-> bin 16 ft - 2 + j; bins 16 ft - 2 .. 16 ft + 1 also get the top four sums of the tile below.
-  // Finished bins leave in aligned 8-bin chunks: chunk 2 ft - 1 = the six bins held back from the previous tile + j = 0, 1;
-  // chunk 2 ft = j = 2 .. 9; j = 10 .. 15 are held for the next tile.  Where a range starts / ends, the four partial sums
-  // AND the six finished bins next to them go to the edge buffer (10 values per side); edge_fix_kernel assembles the two
-  // chunks around the boundary.
+// Contour layer (8 -> 1 channels, 5 x 5 taps, models.py:252-259): S[j] = the time-complete sum for output bin 16 ft - 2 + j
+// of the thread's frame.  Frequency halo by register carry, then sigmoid and the stores.
+__device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOut& ro, float (&S)[20], int ft, bool first,
+                                                    bool last, float (&carry)[4], float (&hold)[6]) {
+  // Bins 16 ft - 2 .. 16 ft + 1 also get the top four sums of the tile below.  Finished bins leave in aligned 8-bin chunks:
+  // chunk 2 ft - 1 = the six bins held back from the previous tile + j = 0, 1; chunk 2 ft = j = 2 .. 9; j = 10 .. 15 are
+  // held for the next tile.  Where a range starts / ends, the four partial sums AND the six finished bins next to them go
+  // to the edge buffer (10 values per side); edge_fix_kernel assembles the two chunks around the boundary.
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
@@ -793,40 +617,56 @@ __device__ __forceinline__ void contour_tile(const TcArgs& a, const RowOut& ro, 
   }
 }
 
+// The conv2 MMAs of one tile: A = relu(conv1 + bias) of the warpgroup's 64 rows as bf16 hi / lo register fragments
+// (ah / al: per K = 16 step four registers), B = the conv2 weight matrix in shared memory; three split products per step.
+template <int NW>
+__device__ __forceinline__ void conv2_mma(float (&p)[NW / 2], const uint32_t (&ah)[32], const uint32_t (&al)[32], uint32_t b2) {
+  constexpr uint32_t kPlane = 128u * NW * 2u;  // bytes of one bf16 plane of the weight matrix
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) {
+    const uint64_t bh = make_desc(b2 + (uint32_t)(2 * ks * NW * 16), NW * 16, 128);
+    const uint64_t bl = make_desc(b2 + kPlane + (uint32_t)(2 * ks * NW * 16), NW * 16, 128);
+    const uint32_t xh[4] = {ah[4 * ks], ah[4 * ks + 1], ah[4 * ks + 2], ah[4 * ks + 3]};
+    const uint32_t xl[4] = {al[4 * ks], al[4 * ks + 1], al[4 * ks + 2], al[4 * ks + 3]};
+    if constexpr (NW == 104) {
+      wgmma_rs_n104(p, xh, bh, ks ? 1u : 0u);
+      wgmma_rs_n104(p, xh, bl, 1u);
+      wgmma_rs_n104(p, xl, bh, 1u);
+    } else if constexpr (NW == 64) {
+      wgmma_rs_n64(p, xh, bh, ks ? 1u : 0u);
+      wgmma_rs_n64(p, xh, bl, 1u);
+      wgmma_rs_n64(p, xl, bh, 1u);
+    } else {
+      wgmma_rs_n32(p, xh, bh, ks ? 1u : 0u);
+      wgmma_rs_n32(p, xh, bl, 1u);
+      wgmma_rs_n32(p, xl, bh, 1u);
+    }
+  }
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using namespace tc;
   constexpr bool kFused = EPI != 0;
   constexpr int LAYER = EPI == 3 ? 0 : EPI;  // index into the constant banks
   constexpr TcB2 B2 = tc_b2_spec(EPI);
-  constexpr int ND2 = 512 - (int)kD2Base >= 2 * B2.width ? 2 : 1;  // conv2 accumulators that fit behind the ring
+  constexpr int NW = B2.width, PS = NW + 1;  // conv2 accumulator columns; row pitch of their staging
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr TcSmem SM = tc_smem(EPI);
-  constexpr int kStages = SM.stages, kXchgFloats = SM.xchg_floats;
-  static_assert(SM.total() <= kMaxSmem && kStages <= kMaxStages, "dynamic shared memory per CTA");
+  constexpr int kStages = SM.stages;
+  static_assert(SM.total() <= kMaxSmem && kStages <= kMaxStages && kStages >= 4, "dynamic shared memory per CTA");
   unsigned char* s_data = smem;                    // [2 planes][chunks][data_rows][16 B]
   unsigned char* s_w = smem + SM.data_bytes;       // [kStages][8192]
-  float* s_x = reinterpret_cast<float*>(s_w + kStages * kTileBytes);  // [slot][buf][warp 3][kXchgFloats]
-  unsigned char* s_b2 = reinterpret_cast<unsigned char*>(s_x) + SM.xchg_bytes();  // conv2 weight tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_b2 + SM.b2_bytes);
+  unsigned char* s_b2 = s_w + kStages * kTileBytes;  // conv2 weight matrix [plane 2][k-chunk 16][NW][16 B]
+  float* s_p = reinterpret_cast<float*>(s_b2 + SM.b2_bytes);  // conv2 sums [slot 2][64 rows][PS]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(s_p) + SM.p_bytes);
   uint64_t* full_w = bars;             // [kStages]
-  uint64_t* empty_w = bars + kStages;  // [kStages]
+  uint64_t* empty_w = bars + kStages;  // [kStages] one arrival per consumer warp
   uint64_t* data_full = bars + 2 * kStages;
-  uint64_t* data_empty = data_full + 1;
-  // Parity waits are only safe when whoever waits for phase k + 1 of a barrier has seen phase k complete.  The regions
-  // (and a shared conv2 accumulator) alternate between the two slots irregularly (single-tile groups), so the barriers
-  // the epilogue warps wait on are per slot: tmem_full[region][slot], d2_full[slot]; each has one committing warp, one
-  // set of waiters and at most one phase outstanding.  The others have a single waiting warp that walks the tiles in order.
-  uint64_t* tmem_full = data_full + 2;            // [kRegions][2 slots] conv1 accumulator complete
-  uint64_t* tmem_empty = tmem_full + 2 * kRegions;  // [kRegions] region may be overwritten by the next conv1 tile
-  uint64_t* a2_full = tmem_empty + kRegions;  // [kRegions] relu(conv1) split written back: conv2 MMAs may start
-  uint64_t* d2_full = a2_full + kRegions;     // [2 slots] conv2 partial sums of the slot's current tile complete
-  uint64_t* d2_empty = d2_full + 2;           // [2 buffers] conv2 accumulator read and zeroed again
-  uint64_t* b2_full = d2_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b2_full + 1);
+  uint64_t* data_empty = data_full + 1;  // one arrival per consumer warp
+  uint64_t* b2_full = data_empty + 1;
 
-  // Broadcasting the warp index lets the compiler keep the role branches and the producer / MMA loop state in uniform
-  // registers (no R2UR before every UTCHMMA: ~40 instead of ~60 instructions per step).
+  // Broadcasting the warp index keeps the role branches and the producer loop state in uniform registers.
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const uint32_t lbo = (uint32_t)a.data_rows * 16u;
@@ -835,56 +675,23 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_w + s, 1);
-      mbar_init(empty_w + s, 2);  // one arrival per conv1 MMA warp
+      mbar_init(empty_w + s, kConsumerWarps);
     }
     mbar_init(data_full, 1);
-    mbar_init(data_empty, 2);
-    for (int i = 0; i < kRegions; ++i) {
-      mbar_init(tmem_full + 2 * i, 1);
-      mbar_init(tmem_full + 2 * i + 1, 1);
-      mbar_init(tmem_empty + i, kFused ? 1 : 4);  // fused: the commit behind the conv2 MMAs; else the four epilogue warps
-      mbar_init(a2_full + i, 4);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(d2_full + i, 1);
-      mbar_init(d2_empty + i, 4);
-    }
+    mbar_init(data_empty, kConsumerWarps);
     mbar_init(b2_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  if constexpr (kFused) {  // the conv2 accumulators start out zero (the MMAs only ever accumulate into them)
-    if (warp < 8 && (warp >> 2) < ND2) {
-      const uint32_t d2 = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + kD2Base + (uint32_t)(warp >> 2) * B2.width;
-#pragma unroll
-      for (int c = 0; c + 8 <= B2.width; c += 8) tmem_zero<8>(d2 + c);
-      tmem_st_wait();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-  }
 
   const int n_items = a.n_mtiles * a.n_split;
 
   if (warp == kProducerWarp) {
     // ------------------------------ producer ------------------------------
     // The whole warp walks the loop with warp-uniform state; the arrive / copy instructions are predicated on the elected
-    // lane.  (With `if (lane == 0)` the compiler put an elect loop and three R2UR around every UBLKCP; the weight ring is
-    // paced by this loop's latency per step — adding a division to it slowed the contour kernel by 70 %.)
+    // lane (no elect loop and R2UR around every UBLKCP: the weight ring is paced by this loop's latency per step).
     const uint32_t leader = elect_one() ? 1u : 0u;
-    if constexpr (kFused) {
-      constexpr uint32_t b2_bytes = (uint32_t)B2.n_tiles * 2u * 16u * B2.n2 * 2u;
-      static_assert(b2_bytes <= (uint32_t)SM.b2_bytes, "conv2 weight tiles");
-      bulk_g2s_expect_pred(s_b2, a.b2, b2_bytes, b2_full, leader);
-    }
+    if constexpr (kFused) bulk_g2s_expect_pred(s_b2, a.b2, (uint32_t)SM.b2_bytes, b2_full, leader);
     uint32_t stage = 0, ph_w = 0, ph_d = 0;
     const size_t plane_elems = (size_t)a.chunks8 * a.rows_total * 8;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
@@ -910,13 +717,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       for (int s = s0; s < s1; ++s) {
         const int tile_next = c_tile_seq[a.layer][s + 1];  // (one past the end is inside the array)
         mbar_wait_wd(empty_w + stage, ph_w ^ 1, 2);
-#ifdef BP_TC_TRACE
-        if (a.dbg_skip_loads) {
-          if (leader) mbar_arrive(full_w + stage);
-        } else
-#endif
-          bulk_g2s_expect_pred(s_w + stage * kTileBytes, a.tiles + (size_t)tile * (kTileBytes / 2), kTileBytes, full_w + stage,
-                               leader);
+        bulk_g2s_expect_pred(s_w + stage * kTileBytes, a.tiles + (size_t)tile * (kTileBytes / 2), kTileBytes, full_w + stage,
+                             leader);
         if (++stage == kStages) {
           stage = 0;
           ph_w ^= 1;
@@ -924,127 +726,51 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         tile = tile_next;
       }
     }
-  } else if (warp == kMmaWarp0 || warp == kMmaWarp1) {
-    // ------------------------------ conv1 MMA issuers: one warp per accumulator slot ---------------------
-    constexpr uint32_t idesc = make_idesc(128, 128);
-    const int slot = (warp == kMmaWarp0) ? 0 : 1;
-    const uint32_t leader = elect_one() ? 1u : 0u;
-    uint32_t stage = 0, ph_w = 0, ph_d = 0;
-    uint32_t n = 0;  // frequency tiles issued so far by this CTA (both slots, program order) -> region n % 3
-    // descriptor words: low = start >> 4 | (LBO >> 4) << 16 ; high = SBO >> 4 | version 1 << 14 (shared by all)
-    const uint32_t desc_hi32 = (128u >> 4) | (1u << 14);
-    const uint32_t a_hi_base = ((smem_u32(s_data) >> 4) & 0x3fffu) | ((uint32_t)a.data_rows << 16);
-    const uint32_t a_lo_base = a_hi_base + (plane_bytes >> 4);
-    const uint32_t b_base = ((smem_u32(s_w) >> 4) & 0x3fffu) | ((2048u >> 4) << 16);
-    const uint32_t* prog = c_prog[a.layer][slot];
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const int sp = it % a.n_split;
-      const int g0 = sp * a.n_groups / a.n_split, g1 = (sp + 1) * a.n_groups / a.n_split;
-      mbar_wait_wd(data_full, ph_d, 3);
-      ph_d ^= 1;
-      for (int g = g0; g < g1; ++g) {
-        const bool two = c_group_ft[a.layer][2 * g + 1] >= 0;
-        const bool mine = slot == 0 || two;
-        const uint32_t nm = n + (uint32_t)slot, r = nm % kRegions, u = nm / kRegions;
-        bool acquired = !mine;  // the region is acquired at this slot's first use of the group (see TcConvPlan::build)
-        const int s0 = c_group_step_off[a.layer][g], s1 = c_group_step_off[a.layer][g + 1];
-        const uint32_t d = tmem_base + r * 128u;
-        uint32_t w = prog[s0];
-        for (int s = s0; s < s1; ++s) {
-          const uint32_t w_next = prog[s + 1];  // (one word past the end is inside the array)
-          mbar_wait_wd(full_w + stage, ph_w, 5);
-          if (w != kNoUse) {
-            if (!acquired) {
-              mbar_wait_wd(tmem_empty + r, (u & 1u) ^ 1u, 4);
-              acquired = true;
-              TC_TRACE(nm, 0);
-            }
-            tc_fence_after();
-            const uint32_t off = w & 0x3fffu;
-            const uint32_t bl = b_base + stage * (kTileBytes >> 4);
-            umma_bf16_x3(d, a_hi_base + off, a_lo_base + off, bl, bl + 256u, desc_hi32, idesc,
-                         (w & kUseFirstAcc) ? 0u : 1u, leader);
-            umma_commit_pred(empty_w + stage, leader);
-          } else if (leader) {
-            mbar_arrive(empty_w + stage);
-          }
-          if (++stage == kStages) {
-            stage = 0;
-            ph_w ^= 1;
-          }
-          w = w_next;
-        }
-        if (mine) umma_commit_pred(tmem_full + 2 * r + slot, leader);  // this tile's conv1 accumulator is complete
-        if (mine) TC_TRACE(nm, 1);
-        n += two ? 2u : 1u;
-      }
-      umma_commit_pred(data_empty, leader);  // the data tile may be overwritten
-    }
-  } else if (warp == kMma2Warp) {
-    // ------------------------------ conv2 MMA issuer (A operand = the split relu(conv1) in tensor memory) ----------
-    if constexpr (kFused) {
-      constexpr uint32_t idesc2 = make_idesc(128, B2.n2);
-      constexpr uint32_t tile16 = (2u * 16u * B2.n2 * 2u) >> 4;  // bytes >> 4 of one weight tile (hi + lo planes)
-      const uint32_t leader = elect_one() ? 1u : 0u;
-      const uint32_t desc_hi32 = (128u >> 4) | (1u << 14);
-      const uint32_t b2_base = ((smem_u32(s_b2) >> 4) & 0x3fffu) | ((uint32_t)B2.n2 << 16);  // LBO = N2 * 16 bytes
-      uint32_t n = 0;
-      mbar_wait_wd(b2_full, 0, 6);
-      for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-        const int sp = it % a.n_split;
-        const int g0 = sp * a.n_groups / a.n_split, g1 = (sp + 1) * a.n_groups / a.n_split;
-        for (int g = g0; g < g1; ++g) {
-          const int n_here = c_group_ft[a.layer][2 * g + 1] >= 0 ? 2 : 1;
-          for (int sl = 0; sl < n_here; ++sl, ++n) {
-            const uint32_t r = n % kRegions, u = n / kRegions, b = n % ND2, v = n / ND2;
-            mbar_wait_wd(a2_full + r, u & 1u, 7);
-            mbar_wait_wd(d2_empty + b, (v & 1u) ^ 1u, 8);
-            tc_fence_after();
-            TC_TRACE(n, 4);
-            const uint32_t areg = tmem_base + r * 128u, dacc = tmem_base + kD2Base + b * (uint32_t)B2.width;
+  } else if (warp < kConsumerWarps) {
+    // ------------------------------ consumers: one warpgroup per accumulator slot ------------------------------
+    // conv1: the slot's frequency tile of the 64-row M-tile as m64n128k16 MMAs, accumulators in registers.  Fragment of a
+    // thread (warp w of the group, lane = 4 gq + qd): rows 16 w + gq and 16 w + gq + 8, columns 8 i + 2 qd + {0, 1}.
+    const int slot = warp >> 2, wq = warp & 3, gq = lane >> 2, qd = lane & 3;
+    const int tid = threadIdx.x & 127;
+    const int fr0 = 16 * wq + gq;  // first of the thread's two fragment rows (the other is fr0 + 8)
+    // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is 2 qd + e (COUT 8) or
+    // 8 (i % 4) + 2 qd + e (COUT 32)
+    float bz[4][2];
 #pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-              const uint32_t ah = areg + (uint32_t)((ks >> 1) * 32 + (ks & 1) * 8);
-              // window of conv2 accumulator columns this K step contributes to, and its weight tile (TcB2)
-              const uint32_t dcol = EPI == 3 ? 10u * ks : (uint32_t)(B2.js * (ks >> 1));
-              const uint32_t bt = b2_base + (EPI == 3 ? 0u : (uint32_t)(ks & 1) * tile16);
-              umma_ts_bf16_x3(dacc + dcol, ah, ah + 16u, bt, bt + (tile16 >> 1), desc_hi32, idesc2, leader);
-            }
-            umma_commit_pred(d2_full + sl, leader);    // conv2 partial sums of this tile are complete
-            umma_commit_pred(tmem_empty + r, leader);  // and its region may take the next conv1 tile
-            TC_TRACE(n, 5);
-          }
-        }
-      }
-    }
-  } else {
-    // ------------------------------ epilogue (warps 0..3 -> slot 0, warps 4..7 -> slot 1) ------------------------------
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    const int slot = warp >> 2;
-    const int row = quad * 32 + lane;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(quad * 32) << 16);
-    uint32_t n = 0;
-    uint32_t full_bits = 0;  // bit r: parity of the next phase of tmem_full[r][slot]
-    uint32_t my_tiles = 0;   // tiles of this slot so far: parity of d2_full[slot]
-    uint32_t xbuf = 0;  // exchange buffer of this slot, toggled per tile
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) bz[i][e] = c_bias1[LAYER][LAYER == 0 ? 2 * qd + e : 8 * i + 2 * qd + e];
+    uint32_t stage = 0, ph_w = 0, ph_d = 0;
+    const uint32_t a_hi = smem_u32(s_data), a_lo = a_hi + plane_bytes, w_base = smem_u32(s_w);
+    const uint32_t* prog = c_prog[a.layer][slot];
+    float* sp_rows = s_p + slot * 64 * PS;
+    if constexpr (kFused) mbar_wait_wd(b2_full, 0, 6);
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const int mt = it / a.n_split, sp = it % a.n_split;
-      const int g0 = sp * a.n_groups / a.n_split, g1 = (sp + 1) * a.n_groups / a.n_split;
-      // conv1 row of this thread (it provides relu(conv1) of that frame to the fused conv2) ...
-      const int m = mt * a.ms - a.h2 + row;  // row of the (window, frame) space: m = b * rows_per_window + t
-      const int b1 = m >= 0 ? m / a.rows_per_window : 0, t1 = m - b1 * a.rows_per_window;
-      const bool live = m >= 0 && (b1 < a.n_windows) && (t1 < kFrames);
-      // ... and the output frame it finishes: h2 rows earlier (all time taps of the fused conv2 then lie at or below the
-      // thread's own row, see time_edges); rows < 2 h2 of the tile are finished by the previous tile
-      const int q = m - a.h2;
-      const int b = q >= 0 ? q / a.rows_per_window : 0, t = q - b * a.rows_per_window;
+      const int mt = it / a.n_split, spl = it % a.n_split;
+      const int g0 = spl * a.n_groups / a.n_split, g1 = (spl + 1) * a.n_groups / a.n_split;
+      // conv1 rows of the thread's fragment (relu(conv1) of a row that is not a live frame is the zero padding in time)
+      bool live[2];
+      int rb[2], rt[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = mt * a.ms - a.h2 + fr0 + 8 * rr;  // row of the (window, frame) space: m = b * rows_per_window + t
+        rb[rr] = m >= 0 ? m / a.rows_per_window : 0;
+        rt[rr] = m - rb[rr] * a.rows_per_window;
+        live[rr] = m >= 0 && (rb[rr] < a.n_windows) && (rt[rr] < kFrames);
+      }
+      // Fused layers: threads 0..63 of the group each finish the output frame of one tile row, h2 rows earlier than the
+      // conv1 row (all time taps of the fused conv2 then lie at or below the row); rows < 2 h2 are finished by the
+      // previous M-tile
       RowOut ro{};
       float carry[4] = {0.f, 0.f, 0.f, 0.f};
       float hold[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
       if constexpr (kFused) {
-        ro.e_lo = slot * a.n_split + sp;
-        ro.e_hi = (sp + 1 < a.n_split) ? slot * a.n_split + sp + 1 : (slot == 0 ? a.n_split : -1);
-        ro.ok = row >= 2 * a.h2 && q >= 0 && b < a.n_windows && t < kFrames;
+        const int row = tid;
+        const int q = mt * a.ms - 2 * a.h2 + row;
+        const int b = q >= 0 ? q / a.rows_per_window : 0, t = q - b * a.rows_per_window;
+        ro.e_lo = slot * a.n_split + spl;
+        ro.e_hi = (spl + 1 < a.n_split) ? slot * a.n_split + spl + 1 : (slot == 0 ? a.n_split : -1);
+        ro.ok = row < 64 && row >= 2 * a.h2 && q >= 0 && b < a.n_windows && t < kFrames;
         ro.t = t;
         if (ro.ok) {
           ro.edge = a.o.edge + q;
@@ -1065,88 +791,134 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
           }
         }
       }
+      mbar_wait_wd(data_full, ph_d, 3);
+      ph_d ^= 1;
       for (int g = g0; g < g1; ++g) {
-        const bool two = c_group_ft[a.layer][2 * g + 1] >= 0;
         const int ft = c_group_ft[a.layer][2 * g + slot];
-        const uint32_t nm = n + (uint32_t)slot;
-        n += two ? 2u : 1u;
+        const int s0 = c_group_step_off[a.layer][g], s1 = c_group_step_off[a.layer][g + 1];
+        float acc[64];
+        int pend = -1;  // stage read by the MMA group still in flight
+        uint32_t w = prog[s0];
+        for (int s = s0; s < s1; ++s) {
+          const uint32_t w_next = prog[s + 1];  // (one word past the end is inside the array)
+          mbar_wait_wd(full_w + stage, ph_w, 5);
+          if (w != kNoUse) {
+            const uint32_t off = (w & 0x3fffu) << 4;  // chunk c8, row dt of the data tile
+            const uint32_t bw = w_base + stage * kTileBytes;
+            const uint64_t dah = make_desc(a_hi + off, lbo, 128), dal = make_desc(a_lo + off, lbo, 128);
+            const uint64_t dbh = make_desc(bw, 2048, 128), dbl = make_desc(bw + 4096, 2048, 128);
+            wgmma_fence();
+            wgmma_ss_n128(acc, dah, dbh, (w & kUseFirstAcc) ? 0u : 1u);
+            wgmma_ss_n128(acc, dah, dbl, 1u);
+            wgmma_ss_n128(acc, dal, dbh, 1u);
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous step's MMAs are done: its weight stage may be refilled
+            if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
+            pend = (int)stage;
+          } else {
+            // a run of steps of the other slot may be longer than the ring: release the held stage before passing on
+            if (pend >= 0) {
+              wgmma_wait<0>();
+              if (lane == 0) mbar_arrive(empty_w + pend);
+              pend = -1;
+            }
+            if (lane == 0) mbar_arrive(empty_w + stage);
+          }
+          if (++stage == kStages) {
+            stage = 0;
+            ph_w ^= 1;
+          }
+          w = w_next;
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
+        if (g == g1 - 1 && lane == 0) mbar_arrive(data_empty);  // this warp's MMAs no longer read the data tile
         if (ft < 0) continue;
-        const uint32_t r = nm % kRegions;
-        mbar_wait_wd(tmem_full + 2 * r + slot, (full_bits >> r) & 1u, 9);
-        full_bits ^= 1u << r;
-        tc_fence_after();
-        if (quad == 0) TC_TRACE(nm, 2);
-        const uint32_t taddr = lane_base + r * 128u;
         // first / last tile of this slot's ascending range inside the item
         const bool first = (g == g0);
         const bool last = (g == g1 - 1) || (ft == a.n_ft - 1);
+        const int n_valid = min(a.flt, a.wout - ft * a.flt) * a.cout;  // a multiple of 32 (contour: 64 in the last tile)
         if constexpr (EPI == 0) {
           // contour: 16 bins x 8 channels, bias + ReLU, channels-last rows of 128 contiguous floats
-          const int n_valid = min(a.flt, a.wout - ft * a.flt) * a.cout;
-          float* dst = a.o.act + ((size_t)b * kFrames + t) * ((size_t)a.wout * a.cout) + (size_t)ft * 128;
-#pragma unroll 1
-          for (int c4 = 0; c4 < 4; ++c4) {
-            uint32_t v[32];
-            tmem_ld32_nowait(taddr + c4 * 32, v);
-            tmem_ld_wait();
-            if (live) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                float4 o;
-                o.x = fmaxf(__uint_as_float(v[4 * i + 0]) + c_bias1[0][(4 * i + 0) & 7], 0.f);
-                o.y = fmaxf(__uint_as_float(v[4 * i + 1]) + c_bias1[0][(4 * i + 1) & 7], 0.f);
-                o.z = fmaxf(__uint_as_float(v[4 * i + 2]) + c_bias1[0][(4 * i + 2) & 7], 0.f);
-                o.w = fmaxf(__uint_as_float(v[4 * i + 3]) + c_bias1[0][(4 * i + 3) & 7], 0.f);
-                if (c4 * 32 + 4 * i < n_valid) reinterpret_cast<float4*>(dst + c4 * 32)[i] = o;
-              }
+          for (int rr = 0; rr < 2; ++rr) {
+            if (!live[rr]) continue;
+            float* dst = a.o.act + ((size_t)rb[rr] * kFrames + rt[rr]) * ((size_t)a.wout * a.cout) + (size_t)ft * 128;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              const int col = 8 * i + 2 * qd;
+              if (col < n_valid)
+                *reinterpret_cast<float2*>(dst + col) = make_float2(fmaxf(acc[4 * i + 2 * rr] + bz[i & 3][0], 0.f),
+                                                                    fmaxf(acc[4 * i + 2 * rr + 1] + bz[i & 3][1], 0.f));
             }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tmem_empty + r);
         } else {
-          // bias + ReLU + split in place, then the conv2 MMAs take over (kMma2Warp) ...
-          const int n_valid = min(a.flt, a.wout - ft * a.flt) * a.cout;
-          convert_tile<LAYER>(taddr, live, n_valid);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(a2_full + r);
-          if (quad == 0) TC_TRACE(nm, 3);
-          // ... and hand back P[j][dt] in the conv2 accumulator
-          const uint32_t bb = nm % ND2;
-          mbar_wait_wd(d2_full + slot, my_tiles & 1u, 10);
-          ++my_tiles;
-          tc_fence_after();
-          if (quad == 0) TC_TRACE(nm, 6);
-          const uint32_t d2 = lane_base + kD2Base + bb * (uint32_t)B2.width;
-          float* xb = s_x + (slot * 2 + xbuf) * 3 * kXchgFloats;
-          xbuf ^= 1u;
-          if constexpr (EPI == 3) {
-            contour_tile(a, ro, d2, d2_empty + bb, ft, first, last, quad, lane, slot, xb, carry, hold);
-          } else {
-            constexpr int KH2 = (EPI == 1) ? 3 : 7, H = KH2 / 2;
-            float S[6];
-            pitch_tile_taps<KH2>(d2, lane, quad, xb + quad * kXchgFloats, d2_empty + bb, S);
-            __syncwarp();
-            slot_barrier(slot);
-            time_edges<H, 6>(S, quad, lane, xb, kXchgFloats);
-            float c2[2] = {carry[0], carry[1]};
-            finish_pitch_tile<EPI>(a, ro, S, c2, ft, first, last);
-            carry[0] = c2[0];
-            carry[1] = c2[1];
+          // relu(conv1 + bias) -> bf16 hi / lo A fragments of the conv2 MMAs.  The conv1 accumulator fragment is the A
+          // register layout of a K = 16 step (registers: rows gq / gq + 8 x columns 2 qd / 8 + 2 qd of the step), so
+          // columns 16 ks .. 16 ks + 15 form step ks: register 4 ks + 2 (i & 1) + rr holds accumulator block i = 2 ks + (i & 1)
+          uint32_t ah[32], al[32];
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              const bool ok = live[rr] && 8 * i < n_valid;
+              const float o0 = ok ? fmaxf(acc[4 * i + 2 * rr] + bz[i & 3][0], 0.f) : 0.f;
+              const float o1 = ok ? fmaxf(acc[4 * i + 2 * rr + 1] + bz[i & 3][1], 0.f) : 0.f;
+              const __nv_bfloat162 hh = __floats2bfloat162_rn(o0, o1);
+              const uint32_t hu = *reinterpret_cast<const uint32_t*>(&hh);
+              const __nv_bfloat162 ll =
+                  __floats2bfloat162_rn(o0 - __uint_as_float(hu << 16), o1 - __uint_as_float(hu & 0xffff0000u));
+              const int r = 4 * (i >> 1) + 2 * (i & 1) + rr;
+              ah[r] = hu;
+              al[r] = *reinterpret_cast<const uint32_t*>(&ll);
+            }
+          // P[row][j * JS + dt] = sum over channels and frequency taps for output offset j and time tap dt (TcB2)
+          float p[NW / 2];
+          wgmma_fence();
+          conv2_mma<NW>(p, ah, al, smem_u32(s_b2));
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(p);
+          slot_barrier(slot);  // the previous tile's sums have been read
+#pragma unroll
+          for (int i = 0; i < NW / 8; ++i)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              float* d = sp_rows + (fr0 + 8 * rr) * PS + 8 * i + 2 * qd;
+              d[0] = p[4 * i + 2 * rr];
+              d[1] = p[4 * i + 2 * rr + 1];
+            }
+          slot_barrier(slot);
+          if (tid < 64) {
+            // time taps: the frame of tile row r takes P_dt from row r - (KH2 - 1 - dt), taps added from the own row down
+            // (the same order for every row: a frame's value does not depend on where the M-tile starts)
+            constexpr int KH2 = B2.kh2, JS = B2.js;
+            constexpr int NJ = EPI == 3 ? 20 : 6;
+            float S[NJ];
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+              float s = 0.f;
+#pragma unroll
+              for (int ta = 0; ta < KH2; ++ta)
+                if (tid - ta >= 0) s += sp_rows[(tid - ta) * PS + j * JS + (KH2 - 1 - ta)];
+              S[j] = s;
+            }
+            if constexpr (EPI == 3) {
+              finish_contour_tile(a, ro, S, ft, first, last, carry, hold);
+            } else {
+              float c2[2] = {carry[0], carry[1]};
+              finish_pitch_tile<EPI>(a, ro, S, c2, ft, first, last);
+              carry[0] = c2[0];
+              carry[1] = c2[1];
+            }
           }
-          if (quad == 0) TC_TRACE(nm, 7);
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
 }
+
 
 // ------------------------------------------------------------------------------------------------
 // Where two tile ranges meet (frequency tile ft_b = first tile of a range, ft_b > 0) the 2 * HALO bins
@@ -1231,7 +1003,6 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
   if (a.o.raw) a.o.raw[(size_t)f * a.o.raw_rows + (size_t)b * kFrames + t] = v;
   if (uf >= 0) a.o.unwrapped[(size_t)f * a.o.frame_stride + uf] = v;
 }
-
 // ------------------------------------------------------------------------------------------------
 int tc_rows_total(int n_windows, int rows_per_window) {
   // lead rows + the rows of the windows + what the last (overlapping) M-tile and its time taps may touch
@@ -1313,12 +1084,11 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
         fn = nullptr;
       return reinterpret_cast<EncodeFn>(fn);
     }();
-    // The data tile can be fetched by ONE tensor-map TMA (cp.async.bulk.tensor.4d -> UTMALDG) or by 78 1-D bulk copies
-    // (one per plane and chunk).  Measured on the same B200 (tools/stage_times.py, A/B in one run): the tensor-map form is
-    // 1.6 % slower on the conv kernels (contour 0.990 vs 0.974, onset 1.390 vs 1.368 us/window) — its innermost box
-    // dimension is only 16 bytes, and one box is walked by one TMA pipeline while the bulk copies proceed in parallel
-    // (splitting the box is not possible: a chunk is 130 rows x 16 B = 2 080 B, not a multiple of the 128-byte shared-
-    // memory alignment a box needs).  Default = bulk copies; BP_B200_TMAP=1 selects the tensor map (GPU-tested).
+    // The data tile can be fetched by ONE tensor-map TMA (cp.async.bulk.tensor.4d -> UTMALDG) or by 1-D bulk copies (one
+    // per plane and chunk).  The tensor map's innermost box dimension is only 16 bytes, and one box is walked by one TMA
+    // pipeline while the bulk copies proceed in parallel (splitting the box is not possible: a chunk is 66 rows x 16 B =
+    // 1 056 B, not a multiple of the 128-byte shared-memory alignment a box needs).  Default = bulk copies;
+    // BP_B200_TMAP=1 selects the tensor map (GPU-tested).
     a.use_tmap = 0;
     static const bool want_tmap = getenv("BP_B200_TMAP") != nullptr;
     if (encode && want_tmap) {
@@ -1332,16 +1102,6 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
         a.use_tmap = 1;
     }
   }
-#ifdef BP_TC_TRACE
-  static long long* d_trace = nullptr;
-  const bool tracing = getenv("BP_TC_TRACE") != nullptr;
-  if (tracing) {
-    if (!d_trace) cudaMalloc(&d_trace, 256 * 8 * sizeof(long long));
-    cudaMemsetAsync(d_trace, 0, 256 * 8 * sizeof(long long), st);
-    a.trace = d_trace;
-  }
-  a.dbg_skip_loads = getenv("BP_TC_SKIP_LOADS") != nullptr;
-#endif
   if (sp.epi == 0 && fuse_next)
     conv_tc_kernel<3><<<grid, tc::kThreads, tc::tc_smem(3).total(), st>>>(a);
   else if (sp.epi == 0)
@@ -1350,20 +1110,6 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
     conv_tc_kernel<1><<<grid, tc::kThreads, tc::tc_smem(1).total(), st>>>(a);
   else
     conv_tc_kernel<2><<<grid, tc::kThreads, tc::tc_smem(2).total(), st>>>(a);
-#ifdef BP_TC_TRACE
-  if (tracing) {
-    static long long h[256 * 8];
-    cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, st);
-    cudaStreamSynchronize(st);
-    long long t0 = h[0];
-    fprintf(stderr, "tc_trace layer %d n_items %d split %d grid %d\n", dev.layer, n_items, a.n_split, grid);
-    for (int n = 0; n < 256 && h[n * 8 + 1]; ++n) {
-      fprintf(stderr, "tile %3d:", n);
-      for (int e = 0; e < 8; ++e) fprintf(stderr, " %8lld", h[n * 8 + e] ? h[n * 8 + e] - t0 : -1);
-      fprintf(stderr, "\n");
-    }
-  }
-#endif
   if (fused) {  // slot s of split q covers tiles [g0(q) + s*G0, g1(q) + s*G0): edge slot s*split + q
     EdgeFixArgs ef{};
     ef.o = o;

@@ -1,5 +1,5 @@
-// Inline-PTX helpers shared by the tcgen05 kernels (tc_conv.cu, cqt_tc.cu): mbarriers, bulk async copies (UBLKCP),
-// UMMA shared-memory / instruction descriptors, tcgen05.mma / commit / fences, TMEM loads.
+// Inline-PTX helpers shared by the tensor-core kernels (tc_conv.cu, cqt_tc.cu): mbarriers, bulk async copies (UBLKCP),
+// wgmma shared-memory descriptors, warpgroup MMAs (wgmma.mma_async) with their fences, commits and waits.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -67,7 +67,7 @@ __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity, int
 }
 #else
 // Production form: the whole spin loop is one asm block (a C++ loop on the returned predicate makes the compiler treat the
-// issuing warps' loop state as divergent, which takes the MMA loops off the uniform datapath: R2UR before every UTCHMMA),
+// issuing warps' loop state as divergent, which takes the MMA loops off the uniform datapath: R2UR before every WGMMA),
 // bounded by a spin count (each try_wait suspends for a hardware-defined time first) and ending in a trap.
 // Build with -DBP_MBAR_DEBUG to get the message with the wait site instead.
 __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity, int /*tag*/) {
@@ -128,227 +128,71 @@ __device__ __forceinline__ void bulk_g2s_expect_pred(void* smem_dst, const void*
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "r"(leader)
       : "memory");
 }
-// K-major, no-swizzle shared-memory matrix descriptor (SM100 "version 1"):
-//   [0,14) start >> 4, [16,30) leading-dimension byte offset >> 4 (between the two 8-element k-chunks),
-//   [32,46) stride byte offset >> 4 (between 8-row groups), [46,48) = 1, layout type [61,64) = 0.
+// K-major, no-swizzle wgmma shared-memory matrix descriptor (core matrices of 8 rows x 16 B, rows 16 B apart):
+//   [0,14) start >> 4, [16,30) leading-dimension byte offset >> 4 (between the two 8-element k-chunks of a K = 16 step),
+//   [32,46) stride byte offset >> 4 (between 8-row groups), base offset 0, layout type [62,64) = 0 (no swizzle).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 46);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
-// instruction descriptor, kind::f16: D = f32 (bit 4), A = B = bf16 (bits 7, 10), both K-major, N>>3 @17, M>>4 @24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// The three split-precision products of one program use, issued by the elected lane only (PTX predication, no
-// branch): D (+)= Ahi*Bhi ; D += Ahi*Blo ; D += Alo*Bhi.  Descriptors are passed as (low word, shared high word).
-__device__ __forceinline__ void umma_bf16_x3(uint32_t tmem_d, uint32_t a_hi_lo32, uint32_t a_lo_lo32, uint32_t b_hi_lo32,
-                                             uint32_t b_lo_lo32, uint32_t desc_hi32, uint32_t idesc, uint32_t accumulate,
-                                             uint32_t leader) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q, t;\n\t"
-      ".reg .b64 dah, dal, dbh, dbl;\n\t"
-      "setp.ne.b32 p, %7, 0;\n\t"
-      "setp.ne.b32 q, %8, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 dah, {%1, %5};\n\t"
-      "mov.b64 dal, {%2, %5};\n\t"
-      "mov.b64 dbh, {%3, %5};\n\t"
-      "mov.b64 dbl, {%4, %5};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dah, dbh, %6, p;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dah, dbl, %6, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dal, dbh, %6, t;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_hi_lo32), "r"(a_lo_lo32), "r"(b_hi_lo32), "r"(b_lo_lo32), "r"(desc_hi32), "r"(idesc), "r"(accumulate),
-      "r"(leader)
-      : "memory");
-}
-// The six products of a three-way split (a = h + m + l, b likewise): D (+)= Ah*Bh ; += Ah*Bm ; += Am*Bh ; += Ah*Bl ; += Al*Bh ; += Am*Bm,
-// issued by the elected lane only.  Descriptors as (low word, shared high word), see umma_bf16_x3.
-__device__ __forceinline__ void umma_bf16_x6(uint32_t tmem_d, uint32_t a_h, uint32_t a_m, uint32_t a_l, uint32_t b_h,
-                                             uint32_t b_m, uint32_t b_l, uint32_t desc_hi32, uint32_t idesc,
-                                             uint32_t accumulate, uint32_t leader) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q, t;\n\t"
-      ".reg .b64 dah, dam, dal, dbh, dbm, dbl;\n\t"
-      "setp.ne.b32 p, %9, 0;\n\t"
-      "setp.ne.b32 q, %10, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 dah, {%1, %7};\n\t"
-      "mov.b64 dam, {%2, %7};\n\t"
-      "mov.b64 dal, {%3, %7};\n\t"
-      "mov.b64 dbh, {%4, %7};\n\t"
-      "mov.b64 dbm, {%5, %7};\n\t"
-      "mov.b64 dbl, {%6, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dah, dbh, %8, p;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dah, dbm, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dam, dbh, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dah, dbl, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dal, dbh, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], dam, dbm, %8, t;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_h), "r"(a_m), "r"(a_l), "r"(b_h), "r"(b_m), "r"(b_l), "r"(desc_hi32), "r"(idesc), "r"(accumulate), "r"(leader)
-      : "memory");
-}
-// Six products of a three-way split with the A operand in tensor memory (TS form): a_* are tensor-memory addresses (K = 16 ->
-// 8 columns each), b_* descriptor low words.  D (+)= Ah*Bh ; += Ah*Bm ; += Am*Bh ; += Ah*Bl ; += Al*Bh ; += Am*Bm.
-__device__ __forceinline__ void umma_ts_bf16_x6(uint32_t tmem_d, uint32_t a_h, uint32_t a_m, uint32_t a_l, uint32_t b_h,
-                                                uint32_t b_m, uint32_t b_l, uint32_t desc_hi32, uint32_t idesc,
-                                                uint32_t accumulate, uint32_t leader) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, q, t;\n\t"
-      ".reg .b64 dbh, dbm, dbl;\n\t"
-      "setp.ne.b32 p, %9, 0;\n\t"
-      "setp.ne.b32 q, %10, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 dbh, {%4, %7};\n\t"
-      "mov.b64 dbm, {%5, %7};\n\t"
-      "mov.b64 dbl, {%6, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], dbh, %8, p;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], dbm, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], dbh, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], dbl, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%3], dbh, %8, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], dbm, %8, t;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_h), "r"(a_m), "r"(a_l), "r"(b_h), "r"(b_m), "r"(b_l), "r"(desc_hi32), "r"(idesc), "r"(accumulate), "r"(leader)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void umma_commit_pred(uint64_t* bar, uint32_t leader) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred q;\n\t"
-      "setp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(leader)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Packed FP32 FMA (FFMA2): d.{x,y} += o * w.{x,y}.  One issue slot for two FMAs; with the scalar broadcast in a register and
-// the weight pair in a uniform register (constant memory, static offset) the epilogue FMA streams need half the issue
-// slots of scalar FFMAs — what the fused epilogues compete for with the MMA-issuing warps.
-__device__ __forceinline__ void ffma2(float2& d, float o, float2 w) {
-  unsigned long long dd, oo, ww;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(dd) : "f"(d.x), "f"(d.y));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(oo) : "f"(o));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ww) : "f"(w.x), "f"(w.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(dd) : "l"(oo), "l"(ww));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(dd));
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-
-// ---- A operand in tensor memory (tcgen05.mma "TS" form) -------------------------------------------------------------
-// kind::f16, M = 128: row = TMEM lane, two 16-bit elements per 32-bit column (element 2c in the low half), so a K = 16 step
-// reads 8 columns starting at the given column (measured with tools/ubench/umma_ts.cu, which also shows that the D
-// operand of a small-N MMA may start at ANY column).  The three split-precision products, all accumulating:
-//   D += Ahi*Bhi ; D += Ahi*Blo ; D += Alo*Bhi        (issued by the elected lane only)
-__device__ __forceinline__ void umma_ts_bf16_x3(uint32_t tmem_d, uint32_t tmem_a_hi, uint32_t tmem_a_lo, uint32_t b_hi_lo32,
-                                                uint32_t b_lo_lo32, uint32_t desc_hi32, uint32_t idesc, uint32_t leader) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred q, t;\n\t"
-      ".reg .b64 dbh, dbl;\n\t"
-      "setp.ne.b32 q, %7, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 dbh, {%3, %5};\n\t"
-      "mov.b64 dbl, {%4, %5};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], dbh, %6, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], dbl, %6, t;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], dbh, %6, t;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a_hi), "r"(tmem_a_lo), "r"(b_hi_lo32), "r"(b_lo_lo32), "r"(desc_hi32), "r"(idesc), "r"(leader)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld2_nowait(uint32_t taddr, uint32_t (&v)[2]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(v[0]), "=r"(v[1]) : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-// zero `N` consecutive columns of the calling warp's 32 lanes (N = 8, 16 or 32)
+// Register operands of in-flight wgmmas must not be touched: fence before the first MMA that reads registers written by
+// ordinary instructions, commit the issued MMAs as one group, wait until at most N groups are pending.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void tmem_zero(uint32_t taddr) {
-  static_assert(N == 8 || N == 16 || N == 32, "tmem_zero");
-  const uint32_t z = 0u;
-  if constexpr (N == 8) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr), "r"(z) : "memory");
-  } else if constexpr (N == 16) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr),
-        "r"(z)
-        : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, "
-        "%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr),
-        "r"(z)
-        : "memory");
-  }
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D (+)= A * B, m64n128k16, bf16 operands from shared memory (descriptors), fp32 accumulators d[64]
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// D (+)= A * B, m64n80k16, bf16 operands from shared memory (descriptors), fp32 accumulators d[40]
+__device__ __forceinline__ void wgmma_ss_n80(float (&d)[40], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// D (+)= A * B, m64n104k16, A from registers (a[4]: bf16 pairs in the accumulator fragment layout), B from shared memory
+__device__ __forceinline__ void wgmma_rs_n104(float (&d)[52], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %57, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n104k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51}, {%52, %53, %54, %55}, %56, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+
+// D (+)= A * B, m64n32k16, A from registers (a[4]: bf16 pairs in the accumulator fragment layout), B from shared memory
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+
+// D (+)= A * B, m64n64k16, A from registers (a[4]: bf16 pairs in the accumulator fragment layout), B from shared memory
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 
 }  // namespace bp

@@ -5,7 +5,7 @@ module (`Model`, `predict`, `predict_and_save`, `run_inference`, `window_audio_f
 `get_audio_input`, `unwrap_output`, `OutputExtensions`, `verify_*`, `build_output_path`,
 `save_note_events`, `DEFAULT_*`).  What differs is what sits behind `Model`: instead of dispatching
 to TensorFlow / CoreML / TFLite / onnxruntime (reference: inference.py:78-182) there is one runtime —
-the hand-written sm_100a kernels in `csrc/` reached through the C ABI of include/bp_b200.h — and no
+the hand-written sm_90a kernels in `csrc/` reached through the C ABI of include/bp_b200.h — and no
 CPU fallback.  Batch entry points (`Model.transcribe_arrays`, `predict_batch`) are additions.
 """
 from __future__ import annotations
@@ -114,12 +114,12 @@ def _default_device() -> int:
 
 
 class Model:
-    """A loaded network bound to one B200 (reference: inference.py:71-182).
+    """A loaded network bound to one H100 (reference: inference.py:71-182).
 
     `model_path` may be the packed blob shipped with this package (`ICASSP_2022_MODEL_PATH`) or an
     `.onnx` export of the same graph (e.g. the reference's `saved_models/icassp_2022/nmp.onnx`).
     Raises ValueError if the file is not a basic-pitch model (like the reference, inference.py:148-154)
-    and `_lib.BpError` / ImportError if the CUDA library or a B200 is missing.
+    and `_lib.BpError` / ImportError if the CUDA library or an H100 is missing.
     """
 
     class MODEL_TYPES(enum.Enum):
@@ -155,8 +155,8 @@ class Model:
         return self._h
 
     def set_path(self, path: int) -> None:
-        """0 = FP32 FFMA kernels everywhere (on-device accuracy reference), 1 = tcgen05 tensor-core kernels with fused
-        epilogues (default), 2 = tcgen05 kernels keeping the 8-channel contour activations (for activation-level tests)."""
+        """0 = FP32 FFMA kernels everywhere (on-device accuracy reference), 1 = tensor-core (wgmma) kernels with fused
+        epilogues (default), 2 = tensor-core kernels keeping the 8-channel contour activations (for activation-level tests)."""
         self._lib.bp_model_set_path(self._h, int(path))
 
     @property

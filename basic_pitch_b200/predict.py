@@ -12,7 +12,7 @@ import traceback
 def main() -> None:
     from . import ICASSP_2022_MODEL_PATH
 
-    p = argparse.ArgumentParser(description="Predict MIDI from audio on a B200.")
+    p = argparse.ArgumentParser(description="Predict MIDI from audio on an H100.")
     p.add_argument("output_dir", type=str, help="directory to save outputs")
     p.add_argument("audio_paths", type=str, nargs="+", help="audio file(s) to transcribe")
     p.add_argument("--model-path", type=str, default=str(ICASSP_2022_MODEL_PATH), help="packed .bpw blob or .onnx export")

@@ -2,6 +2,7 @@
 """Benchmark of the hot path: audio -> HCQT -> CNN -> note events, audio-seconds per second.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank per GPU)
+  python bench.py ... --dump-outputs DIR                    (also write the last timed step's note events as .npy)
   python bench.py --impl reference ...                      (CPU baseline arm: the oracle port on host cores)
 
 Workload (BASELINE.json configs[3], the configuration the 1/2/4/8-GPU metric is quoted on): 10 s synthetic
@@ -19,7 +20,7 @@ one pass of the path over that batch.
   parity       the oracle run on a fixed sample of THIS step's clips (BASELINE.md §5)
   cpu_baseline the oracle port timed on the host cores (same clips, windows batched across clips)
 
-Inputs per step (1.1 GB) exceed the 126 MB L2, so no explicit L2 flush is needed between iterations.
+Inputs per step (1.1 GB) exceed the 50 MB L2 of an H100, so no explicit L2 flush is needed between iterations.
 """
 import argparse
 import ctypes as C
@@ -44,11 +45,11 @@ FLOP_PER_WINDOW = 1_048_159_296  # SURVEY.md §8(d)
 DECODE_BYTES_PER_FRAME = 1760  # note + onset + contour rows, fp32 (SURVEY.md §8d)
 # kernel families the library can time (bp_model_profile): algorithmic FLOP per window of the tensor-core ones
 FAMILIES = {
-    0: ("contour conv 8->8 3x39 + fused conv2 8->1 5x5 (conv_tc_kernel<3>, tcgen05 split-bf16, conv2 as TS-form MMAs)", 680_030_208 + 18_163_200),
-    1: ("onset conv 8->32 5x5/3 + fused conv2 33->1 3x3 (conv_tc_kernel<1>, tcgen05 split-bf16, conv2 as TS-form MMAs)", 193_740_800 + 8_990_784),
-    2: ("constant-Q projection + log-normalise (cqt_tc_kernel, tcgen05 3-way bf16 split)", 57_065_472),
-    3: ("decimation chain (FFMA2)", 22_359_552),
-    4: ("note conv 1->32 7x7/3 + fused conv2 32->1 7x3 (conv_tc_kernel<2>, tcgen05 split-bf16, conv2 as TS-form MMAs)", 47_466_496 + 20_342_784),
+    0: ("contour conv 8->8 3x39 + fused conv2 8->1 5x5 (conv_tc_kernel<3>, wgmma split-bf16, conv2 with A from registers)", 680_030_208 + 18_163_200),
+    1: ("onset conv 8->32 5x5/3 + fused conv2 33->1 3x3 (conv_tc_kernel<1>, wgmma split-bf16, conv2 with A from registers)", 193_740_800 + 8_990_784),
+    2: ("constant-Q projection + log-normalise (cqt_tc_kernel, wgmma 3-way bf16 split)", 57_065_472),
+    3: ("decimation chain (FP32 FMA)", 22_359_552),
+    4: ("note conv 1->32 7x7/3 + fused conv2 32->1 7x3 (conv_tc_kernel<2>, wgmma split-bf16, conv2 with A from registers)", 47_466_496 + 20_342_784),
     5: ("decode: prep / candidates / sequential loops", 0),
     6: ("decode: amplitude + pitch bends", 0),
 }
@@ -88,12 +89,12 @@ def workload_config(clips_per_gpu: int, world: int):
         "workload": WORKLOAD, "clips_per_gpu_per_step": clips_per_gpu, "clip_seconds": CLIP_SECONDS,
         "clip_seeds": "3 + 100000*rank + i (all clips distinct)", "windows_per_gpu_per_step": windows * clips_per_gpu,
         "frames_per_gpu_per_step": frames * clips_per_gpu, "parallelism": f"files x{world}, no data-path collective",
-        "l2": f"inputs {clips_per_gpu * n * 4 / 1e6:.0f} MB per step > 126 MB L2 (no flush needed)",
+        "l2": f"inputs {clips_per_gpu * n * 4 / 1e6:.0f} MB per step > 50 MB L2 (no flush needed)",
     }  # fmt: skip
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -260,6 +261,35 @@ def parity_report(model, clips, sample_idx, threads: int):
     }  # fmt: skip
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname: str, out) -> None:
+    """The note events of the last step as float64 .npy files, trimmed to what the step produced: what
+    bp_transcribe_device hands its caller (per-file note offsets, frame offsets, start / end frame, MIDI pitch,
+    amplitude, per-note bend offsets and the bends).  Arrays that would push the total past 64 MB are replaced by a
+    fixed, seeded sample of their elements, written with the sample's indices (<name>_index.npy)."""
+    os.makedirs(dirname, exist_ok=True)
+    a = out.a
+    n_files = out.n_files
+    n = int(a["note_off"][n_files])
+    nb = int(a["bend_off"][n])
+    arrays = {"note_off": a["note_off"][: n_files + 1], "frame_off": a["frame_off"][: n_files + 1], "start": a["start"][:n],
+              "end": a["end"][:n], "pitch": a["pitch"][:n], "amp": a["amp"][:n], "bend_off": a["bend_off"][: n + 1],
+              "bends": a["bends"][:nb]}  # fmt: skip
+    budget = DUMP_LIMIT_BYTES
+    for name in sorted(arrays, key=lambda k: arrays[k].size):  # small arrays whole, the largest one sampled if need be
+        v = np.asarray(arrays[name], dtype=np.float64)
+        if v.nbytes > budget:
+            keep = max(1, budget // 16)  # value + index
+            idx = np.sort(np.random.default_rng(0).choice(v.size, size=min(keep, v.size), replace=False))
+            np.save(os.path.join(dirname, f"{name}_index.npy"), idx.astype(np.float64))
+            v = v[idx]
+            budget -= idx.size * 8
+        np.save(os.path.join(dirname, f"{name}.npy"), v)
+        budget -= v.nbytes
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -270,6 +300,8 @@ def main():
     ap.add_argument("--cpu-clips", type=int, default=2 * CPU_GROUP, help="clips of the cpu_baseline sample")
     ap.add_argument("--parity-clips", type=int, default=6, help="clips of the step checked against the oracle")
     ap.add_argument("--python-steps", type=int, default=2, help="timed predict_batch() passes for e2e_python")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the note events of the last timed step as DIR/<name>.npy (float64, rank 0)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -337,6 +369,8 @@ def main():
     ms = timed(dev_step, args.steps)
     launches = model.launch_count - l0
     n_notes = out.n_notes()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     for _ in range(2):
         host_step()
     ms_e2e = timed(host_step, args.steps)
@@ -390,9 +424,9 @@ def main():
                 peaks = json.load(fh)
         except OSError:
             pass
-        peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
-        peak_bw = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained / hbm_gbs)" if peaks else "fallback (B200_PROFILING.md)"
+        peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
+        peak_bw = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained / hbm_gbs)" if peaks else "H100 SXM data sheet (dense BF16, HBM3)"
         dom = max((0, 1, 2, 4), key=lambda k: fam[k]["ms_per_step"])
         f_ms, f_groups, f_win = fam[dom]["ms_per_step"], max(1, fam[dom]["launch_groups"]), fam[dom]["windows"]
         achieved = FAMILIES[dom][1] * f_win / (f_ms * 1e-3) / 1e12 if f_ms > 0 else None

@@ -1,5 +1,5 @@
 /*
- * bp_b200.h — C ABI of the Blackwell-native basic-pitch hot path (libbp_b200.so, sm_100a).
+ * bp_b200.h — C ABI of the Hopper-native basic-pitch hot path (libbp_b200.so, sm_90a).
  *
  * The reference has no FFI: its boundary is a Python API in front of a third-party ML runtime
  * (SURVEY.md §8b).  Each entry point below names the reference interface it stands in for
@@ -168,7 +168,7 @@ int bp_pitch_bends_host(bp_model_t* m, const float* h_contour, int64_t n_frames,
  * Only valid when the batch fitted in one internal chunk (n <= bp_model_chunk_windows). */
 int bp_debug_activation(bp_model_t* m, int which, float* h_out, int64_t n_windows);
 int64_t bp_model_chunk_windows(const bp_model_t* m);
-/* Selects the arithmetic path: 0 = FP32 FFMA kernels everywhere; 1 = tensor-core kernels (tcgen05, split-bf16
+/* Selects the arithmetic path: 0 = FP32 FFMA kernels everywhere; 1 = tensor-core kernels (wgmma, split-bf16
  * operands, FP32 accumulate) for the constant-Q projection and the three wide convolutions, each with the following
  * single-output convolution reduced in its epilogue (default); 2 = as 1 but the contour convolution stores its
  * 8-channel activations (bp_debug_activation which = 1). */

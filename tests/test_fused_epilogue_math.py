@@ -1,18 +1,17 @@
 """CPU: the index arithmetic of the fused second convolutions in the epilogues of the tensor-core kernels
-(csrc/tc_conv.cu: convert_tile + the TS-form conv2 MMAs, contour_tile, pitch_tile_taps, time_edges, finish_pitch_tile,
-edge_fix_kernel),
+(csrc/tc_conv.cu: the conv2 MMAs with their weight matrix, the time taps from the staged sums, finish_pitch_tile,
+finish_contour_tile, edge_fix_kernel),
 restated in NumPy with the SAME structure and compared with the direct convolution of the oracle:
 
   * per frequency tile of FLT bins the thread of a frame reduces relu(conv1) over channels and frequency taps into
     P[dt][j], j = 0 .. FLT + 2*HALO - 1 (output bin FLT*ft - HALO + j),
   * time taps: the thread of tile row r finishes output row r - H, which takes P[dt] of row r - (2H - dt): always a row
-    at or below its own — from a lower lane inside the warp (32 consecutive rows), from the published top lanes of the
-    previous warp otherwise; M-tiles advance by 128 - 2H rows, rows 2H .. 127 of a tile finish an output row,
+    at or below its own, read from the staged sums of the tile; M-tiles advance by 64 - 2H rows, rows 2H .. 63 of a
+    tile finish an output row,
   * frequency halo: a slot walks its tile range in ascending order carrying the top 2*HALO sums; where two ranges meet
     (slot 0 | slot 1, group splits) both sides go to the edge buffer and the fix-up adds them.
 
-This pins the halo bookkeeping, lane / entry formulas, tile ranges and zero padding; the GPU tests then only have to
-prove the kernels."""
+This pins the halo bookkeeping, tile ranges and zero padding; the GPU tests then only have to prove the kernels."""
 import numpy as np
 import pytest
 import torch
@@ -24,6 +23,7 @@ CASES = {  # name: (weights key, C_in, KH2, KW, FLT, HALO, W, rows_per_window, G
     "onset2": ("onset2_w", 32, 3, 3, 4, 1, 88, 174, 12),  # channels 1..32 of the 33-channel conv; channel 0 is the note input
 }
 T = 172
+MT = 64  # rows of an M-tile
 
 
 def _thread_partials(x, w2, KH2, KW, FLT, HALO, W):
@@ -46,37 +46,20 @@ def _thread_partials(x, w2, KH2, KW, FLT, HALO, W):
 
 
 def _time_sum_tile(Ptile, H):
-    """Ptile [KH2][J][128] (conv1 rows of one M-tile) -> S [J][128] exactly like time_tap + time_edges: 4 warps of 32
-    lanes; the thread of tile row r finishes output row r - H, so tap dt comes from `a = 2H - dt` rows below it."""
+    """Ptile [KH2][J][MT] (conv1 rows of one M-tile) -> S [J][MT] like the kernel: the thread of tile row r finishes
+    output row r - H and adds tap dt from `a = 2H - dt` rows below it, a = 0 .. 2H in this order."""
     KH2, J, _ = Ptile.shape
-    S = np.zeros((J, 128))
-    n_pub = H * (2 * H + 1)
-    pub = np.full((4, n_pub, J), np.nan)  # published entries per warp
-    for quad in range(4):
-        for lane in range(32):
-            row = quad * 32 + lane
-            for a in range(2 * H + 1):
-                dt = 2 * H - a
-                if a == 0:
-                    S[:, row] += Ptile[dt, :, row]
-                    continue
-                if lane >= a:
-                    S[:, row] += Ptile[dt, :, row - a]
-                if lane >= 32 - a:
-                    pub[quad, a * (a - 1) // 2 + lane - (32 - a)] = Ptile[dt, :, row]
-    for quad in range(1, 4):
-        for lane in range(32):
-            row = quad * 32 + lane
-            for a in range(1, 2 * H + 1):
-                if lane < a:
-                    S[:, row] += pub[quad - 1, a * (a - 1) // 2 + lane]
+    S = np.zeros((J, MT))
+    for row in range(MT):
+        for a in range(min(2 * H, row) + 1):
+            S[:, row] += Ptile[2 * H - a, :, row - a]
     return S
 
 
 def _fused_layer(x_rows, w2, bias, KH2, KW, FLT, HALO, W, rpw, G0, n_windows, n_split, extra=None):
     """Emulates conv_tc_kernel's fused epilogue + edge_fix_kernel for all M-tiles; returns out [n_windows][T][W]."""
     H = (KH2 - 1) // 2
-    MS = 128 - 2 * H
+    MS = MT - 2 * H
     KE = 2 * HALO
     n_rows = n_windows * rpw
     n_mtiles = (n_rows + MS - 1) // MS
@@ -101,16 +84,16 @@ def _fused_layer(x_rows, w2, bias, KH2, KW, FLT, HALO, W, rpw, G0, n_windows, n_
             for slot in range(2):
                 e_lo = slot * n_split + q
                 e_hi = slot * n_split + q + 1 if q + 1 < n_split else (n_split if slot == 0 else -1)
-                carry = np.zeros((KE, 128))
+                carry = np.zeros((KE, MT))
                 for g in range(g0, g1):
                     ft = g + slot * G0
                     if ft >= n_ft:
                         continue
                     first, last = g == g0, (g == g1 - 1) or (ft == n_ft - 1)
-                    S = _time_sum_tile(P[ft][:, :, m0 + pad : m0 + pad + 128], H)
+                    S = _time_sum_tile(P[ft][:, :, m0 + pad : m0 + pad + MT], H)
                     lower = ft > 0
                     rows_ok = []
-                    for row in range(2 * H, 128):
+                    for row in range(2 * H, MT):
                         m = m0 + row - H  # output row of this thread
                         b, t = divmod(m, rpw) if m >= 0 else (0, -1)
                         if m >= 0 and b < n_windows and t < T:

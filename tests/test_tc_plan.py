@@ -56,7 +56,7 @@ def test_tc_program_reproduces_convolution(weights_np, which):
     ypad[PT : PT + n_t, :bins] = y
     n_ft = (WOUT + FLT - 1) // FLT
     out = np.zeros((n_t, n_ft * 128))
-    lbo16 = 128 + KH - 1  # the program is built for 128-row M-tiles
+    lbo16 = 64 + KH - 1  # the program is built for 64-row M-tiles
     seen_ft = set()
     used = 0
     for g in range(n_groups):

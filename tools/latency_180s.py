@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE configs[1]: one 180 s 22 050 Hz clip end to end on one B200 (audio in host memory -> note events),
+"""BASELINE configs[1]: one 180 s 22 050 Hz clip end to end on one GPU (audio in host memory -> note events),
 with a per-stage breakdown and the event agreement against the oracle decode on the same posteriorgrams."""
 import json
 import sys

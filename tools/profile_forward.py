@@ -1,5 +1,5 @@
-"""Runs the forward pass (HCQT + CNN) on one full internal chunk of windows a few times; the target of the ncu captures
-under profiles/ (`ncu --set full -k regex:<kernel> ... python tools/profile_forward.py`)."""
+"""Runs the forward pass (HCQT + CNN) on one full internal chunk of windows a few times: a short, steady target for a
+profiler (for instance `ncu --set full -k regex:<kernel> ... python tools/profile_forward.py`)."""
 import argparse
 import sys
 from pathlib import Path

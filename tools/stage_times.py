@@ -9,7 +9,7 @@ from pathlib import Path
 
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 
-FAMILIES = {0: "contour conv (tcgen05, fused conv2)", 1: "onset conv (tcgen05)", 2: "CQT + log-normalise",
+FAMILIES = {0: "contour conv (wgmma, fused conv2)", 1: "onset conv (wgmma)", 2: "CQT + log-normalise",
             3: "decimation chain", 4: "note conv + tap sums + contour tap sum", 5: "decode prep/cand/seq",
             6: "note finish (amplitude, bends)"}
 
