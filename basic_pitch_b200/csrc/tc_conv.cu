@@ -36,7 +36,7 @@
 //            K-steps per time tap and frequency tile).
 //            N = FLT output bins x COUT channels = 128 (contour 16 x 8, onset / note 4 x 32); a tile depends on
 //            (dt, 8c - SF*FLT*ft), so frequency tiles SF*FLT*d = 8*j bins apart share tiles (de-duplicated by
-//            content)
+//            structure: equal sets of summed weights, whatever their values)
 //   every (ft, dt, c) with a non-empty tile is one K=16 MMA step of shape 64 x 128 x 16
 // Precision: both operands are split x = hi + lo (bf16 each) and three products are accumulated
 // (hi*hi + hi*lo + lo*hi) in fp32, which keeps the posteriorgrams within ~1e-5 of the FP32 path
@@ -163,10 +163,15 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   // (the fused epilogue carries the frequency halo of the next conv from tile to tile in registers)
   const int stride = sp.G0;
 
-  // weight tiles are de-duplicated by content (boundary clipping makes otherwise equal keys differ and vice versa)
+  // Weight tiles are de-duplicated by STRUCTURE, not by value: two steps share a tile when every element of the two
+  // sums the same weights.  The program (tile ids, their count, which steps of a group's two slots merge) then depends on
+  // the layer geometry alone, so it is the same for every model, and the __constant__ bank that holds it can be shared.
+  // A key word per element: 0 = no term, else 1 + (dt, d = u - SF * f, mask of the contributing channels), which names
+  // the summed weights W[co][ci][dt][d - shift_ci + PL] (co is the element's column) one to one.
   std::unordered_map<uint64_t, std::vector<int>> by_hash;
   int n_keys = 0;
   std::vector<uint16_t> scratch(kTileBytes / 2);
+  std::vector<uint32_t> key(16 * 128), keys;  // keys: [tile][16 * 128]
   // The n_ci input channels are shifted views of ONE image (harmonic stacking, nn.py:69-88), so the stack conv is a
   // single-channel conv of y with the merged kernel  Wm[co][dt][u] = sum_ci W[co][ci][dt][u - shift_ci + PL]  wherever
   // the stacked pixel exists (0 <= g = u_abs - shift_ci < 264): the contour taps of the 8 harmonics (8 x 39 = 312)
@@ -176,6 +181,7 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   auto find_or_add = [&](int dt, int c, int ft, int clip_lo) -> int {
     bool any = false;
     std::fill(scratch.begin(), scratch.end(), (uint16_t)0);
+    std::fill(key.begin(), key.end(), 0u);
     for (int kk = clip_lo; kk < 16; ++kk) {
       const int u = 8 * c + kk;  // bin of y
       if (u >= sp.data_bins) continue;
@@ -183,15 +189,16 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
         const int fl = n / sp.COUT, co = n % sp.COUT;
         const int f = ft * sp.FLT + fl;  // (columns f >= WOUT are computed like the others and dropped by the epilogue)
         double acc = 0.0;
-        bool hit = false;
+        uint32_t mask = 0;
         for (int ci = 0; ci < sp.n_ci; ++ci) {
           const int gg = u - sp.shifts[ci];  // bin of the stacked image
           const int df = gg - sp.SF * f + sp.PL;
           if (df < 0 || df >= sp.KW || gg < 0 || gg >= kContourBins) continue;
           acc += (double)W[((co * sp.n_ci + ci) * sp.KH + dt) * sp.KW + df];
-          hit = true;
+          mask |= 1u << ci;
         }
-        if (!hit) continue;
+        if (!mask) continue;
+        key[kk * 128 + n] = 1u + (((uint32_t)(dt * 1024 + (u - sp.SF * f + 512)) << 8) | mask);  // |d| < 512, n_ci <= 8
         const float w = (float)acc;
         const uint16_t hi = f2bf(w);
         const uint16_t lo = f2bf(w - bf2f(hi));
@@ -203,10 +210,11 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
     }
     if (!any) return -1;
     uint64_t h = 1469598103934665603ull;
-    for (uint16_t v : scratch) h = (h ^ v) * 1099511628211ull;
+    for (uint32_t v : key) h = (h ^ v) * 1099511628211ull;
     for (int id : by_hash[h])
-      if (std::memcmp(tiles.data() + (size_t)id * (kTileBytes / 2), scratch.data(), kTileBytes) == 0) return id;
+      if (std::memcmp(keys.data() + (size_t)id * key.size(), key.data(), key.size() * 4) == 0) return id;
     tiles.insert(tiles.end(), scratch.begin(), scratch.end());
+    keys.insert(keys.end(), key.begin(), key.end());
     by_hash[h].push_back(n_keys);
     return n_keys++;
   };
@@ -303,7 +311,8 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
 
 // The MMA programs live in constant memory: the issuing warp indexes them with warp-uniform values, so the words,
 // the descriptors derived from them and the loop state stay in uniform registers (no per-use R2UR traffic).
-// They depend only on the layer geometry (TcConvSpec), not on the weights.
+// They depend only on the layer geometry (TcConvSpec), not on the weights (tiles are de-duplicated by structure, see
+// TcConvPlan::build), so one upload serves every model of the process; the weight tiles they index are per model.
 __constant__ uint32_t c_prog[3][2][tc::kMaxSteps];  // [layer][slot][step]
 __constant__ int c_tile_seq[3][tc::kMaxSteps];       // [layer][step] -> weight tile id
 __constant__ int c_group_step_off[3][tc::kMaxGroups + 1];

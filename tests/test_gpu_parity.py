@@ -442,15 +442,20 @@ def test_predict_batch_and_error_paths(model, tmp_path):
 
 
 def test_two_models_with_different_weights_do_not_interfere(model, weights_np, tmp_path):
-    """Weight-dependent constants live in __constant__ memory shared by all models of a process on one device; the library
-    re-uploads them when the active model changes (the reference allows loading several model files side by side)."""
+    """Weight-dependent constants and the MMA programs live in __constant__ memory shared by all models of a process on
+    one device; the library re-uploads the constants when the active model changes, and the programs are the same for
+    every model (the reference allows loading several model files side by side).  The second model's conv1 weights
+    differ in which taps are zero, so content-based tile de-duplication would have given it a different program."""
     from basic_pitch_b200 import synth, weights
     from basic_pitch_b200.inference import Model
+    from oracle import model_ref
 
     w2 = {k: v.copy() for k, v in weights_np.items()}
     w2["onset1_b"] = w2["onset1_b"] + 0.25
     w2["note2_w"] = w2["note2_w"] * 0.5
     w2["lowpass"] = w2["lowpass"][::-1].copy() * 0.9
+    w2["contour1_w"][:, :, :, ::2] = 0.0
+    w2["onset1_w"][:, 1::2] = 0.0
     path = tmp_path / "other.bpw"
     path.write_bytes(weights.pack(w2))
     other = Model(path)
@@ -463,6 +468,11 @@ def test_two_models_with_different_weights_do_not_interfere(model, weights_np, t
         np.testing.assert_array_equal(a0[k], a1[k])
         np.testing.assert_array_equal(b0[k], b1[k])
     assert np.abs(a0["note"] - b0["note"]).max() > 1e-3 and np.abs(a0["onset"] - b0["onset"]).max() > 1e-3
+    for got, w in ((a0, weights_np), (b0, w2)):  # each against the oracle under its own weights
+        ref = model_ref.forward(x, w)
+        for k in ("note", "onset", "contour"):
+            err = np.abs(got[k] - ref[k]).max()
+            assert err < POST_TOL, f"{k}: max-abs {err:.3e}"
 
 
 @pytest.mark.gpu

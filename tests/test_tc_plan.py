@@ -8,6 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import model_ref
+from tests import weightsets
 
 SPECS = {  # which: (weights key, KH, KW, SF, PT, PL, COUT, FLT, WOUT)
     0: ("contour1_w", 3, 39, 1, 1, 19, 8, 16, 264),
@@ -40,8 +41,19 @@ def _plan(which, w):
 
 @pytest.mark.parametrize("which", [0, 1, 2])
 def test_tc_program_reproduces_convolution(weights_np, which):
+    _check_program_reproduces_convolution(which, weights_np[SPECS[which][0]])
+
+
+@pytest.mark.parametrize("wset", [n for n in weightsets.NAMES if n != "trained"])
+@pytest.mark.parametrize("which", [0, 1, 2])
+def test_tc_program_reproduces_convolution_synthetic_weights(which, wset):
+    """The same emulation under the synthetic weight sets: every tap non-zero (dense), only the outermost taps
+    (edge_taps), one centre tap per channel pair (sparse, whose tiles used to de-duplicate into a different program)."""
+    _check_program_reproduces_convolution(which, weightsets.get(wset)[SPECS[which][0]])
+
+
+def _check_program_reproduces_convolution(which, w):
     key, KH, KW, SF, PT, PL, COUT, FLT, WOUT = SPECS[which]
-    w = weights_np[key]
     tiles, tile_seq, slot_words, gso, gft, n_uses = _plan(which, w)
     n_groups = len(gft)
     assert gso[0] == 0 and gso[-1] == len(tile_seq) < 1023 and n_groups <= 15  # constant-memory program area
@@ -97,3 +109,23 @@ def test_tc_program_statistics(weights_np):
         assert (tile_seq >= 0).all() and (tile_seq < len(tiles)).all()
         print(which, "tiles", len(tiles), "steps", len(tile_seq), "uses", n_uses)
         assert len(tiles) < 700 and n_uses < 2200
+
+
+def test_tc_program_is_independent_of_the_weights():
+    """The MMA programs live in process-wide __constant__ memory that every model shares, so they must be a function of
+    the layer geometry alone: tile ids, tile count, step sequence, slot words, group offsets and group tiles are the same
+    under every weight set.  (`sparse` gives all (co, ci) pairs the same weight pattern: de-duplicating tiles by value
+    used to merge many of them and produce a different, smaller program.)"""
+    for which in (0, 1, 2):
+        key = SPECS[which][0]
+        ref = None
+        for wset in weightsets.NAMES:
+            tiles, tile_seq, slot_words, gso, gft, n_uses = _plan(which, weightsets.get(wset)[key])
+            prog = (len(tiles), tile_seq, slot_words, gso, gft, n_uses)
+            if ref is None:
+                ref = prog
+                continue
+            assert prog[0] == ref[0], (which, wset, "n_tiles", prog[0], ref[0])
+            assert prog[5] == ref[5], (which, wset, "n_uses")
+            for name, a, b in zip(("tile_seq", "slot_words", "group_step_off", "group_ft"), prog[1:5], ref[1:5]):
+                np.testing.assert_array_equal(a, b, err_msg=f"layer {which}, {wset}: {name}")
