@@ -1531,6 +1531,15 @@ int bp_debug_tc_b2(int which, const float* w2, int32_t* sizes, uint16_t* tiles) 
   return BP_OK;
 }
 
+int bp_debug_tc_clocks(bp_model_t* m, int which, uint64_t* cycles, int reset) {
+  if (!m || !cycles || which < 0 || which > 2) return fail(BP_E_INVALID, "bp_debug_tc_clocks: bad argument");
+  DeviceGuard g(m->device);
+  CK(cudaDeviceSynchronize());
+  if (tc_read_clocks(which, reinterpret_cast<unsigned long long*>(cycles), reset != 0) != 0)
+    return fail(BP_E_INVALID, "bp_debug_tc_clocks: the library was built without -DBP_TC_CLOCKS");
+  return BP_OK;
+}
+
 int bp_model_profile(bp_model_t* m, int which) {
   if (!m) return fail(BP_E_INVALID, "bp_model_profile: null model");
   if (which < -1 || which > 6) return fail(BP_E_INVALID, "bp_model_profile: unknown kernel family");

@@ -78,6 +78,9 @@ void tc_build_b2_full(int epi, const float* w2, std::vector<uint16_t>& out);
 int tc_rows_total(int n_windows, int rows_per_window);
 size_t tc_edge_floats(const TcConvSpec& spec, int n_windows);  // size of the edge buffer of a fused layer
 int tc_setup();  // 0 on success
+// cycle sums by role of one layer's conv_tc_kernel launches (tc::TcClk order), optionally reset; -1 unless the library
+// was built with -DBP_TC_CLOCKS
+int tc_read_clocks(int layer, unsigned long long* out, bool reset);
 // Where window w's centre frames go in the unwrapped (per-file) posteriorgrams (reference: inference.py:247-279).
 struct UnwrapDesc {
   long long dst_base;  // first output frame this window contributes to

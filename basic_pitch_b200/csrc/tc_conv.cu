@@ -70,8 +70,14 @@ constexpr int kTileBytes = 8192;                                 // weight tile:
 constexpr int kMaxSteps = 1024;                                  // program steps per layer (constant memory)
 constexpr int kMaxGroups = 15;
 constexpr int kConsumerWarps = 8;  // two warpgroups, one per accumulator slot
-constexpr int kProducerWarp = 8;
-constexpr int kThreads = 32 * kConsumerWarps + 32;
+constexpr int kProducerWarp = 8;   // the first warp of the third warpgroup; its other three warps only hand back registers
+constexpr int kThreads = 32 * kConsumerWarps + 128;
+// Registers per thread: the launch gives every warpgroup 168 (65 536 / 384, rounded down to 8); the producer warpgroup
+// drops to 24 so that the MMA warpgroups can take 240 (24 + 2 x 240 = 3 x 168, the CTA's pool).  With 168 the consumers
+// spill and ptxas serialises their wgmmas (C7512); the contour epilogue still spills at 232.
+constexpr int kProducerRegs = 24;
+constexpr int kConsumerRegs = 240;
+static_assert(kProducerRegs + 2 * kConsumerRegs <= 3 * 168, "register pool of the CTA");
 }  // namespace tc
 
 // ------------------------------------------------------------------------------------------------
@@ -90,9 +96,11 @@ constexpr int kThreads = 32 * kConsumerWarps + 32;
 // ------------------------------------------------------------------------------------------------
 struct TcB2 {
   int n_tiles, n2, kh2, js, width;  // weight tiles, their N, time taps, columns per output offset j, accumulator columns
+  int pass;  // accumulator columns staged in shared memory at a time (a multiple of 8 and of js: whole output offsets)
 };
 __host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour, 1 onset, 2 note
-  return epi == 1 ? TcB2{2, 16, 3, 4, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64} : TcB2{1, 32, 5, 5, 104};
+  // contour: 3 passes of 8 output offsets (40 columns), which frees 32 KB of staging for four more weight stages
+  return epi == 1 ? TcB2{2, 16, 3, 4, 32, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64, 64} : TcB2{1, 32, 5, 5, 104, 40};
 }
 
 namespace tc {
@@ -101,7 +109,7 @@ namespace tc {
 struct TcSmem {
   int data_bytes;   // [2 planes][chunks][64 + KH - 1 rows][16 B], rounded up to 1 KB
   int b2_bytes;     // conv2 weight matrix [2 planes][128][width] bf16
-  int p_bytes;      // conv2 sums [2 slots][64 rows][width + 1] fp32
+  int p_bytes;      // conv2 sums [2 slots][64 rows][pass + 1] fp32
   int stages;
   __host__ __device__ constexpr int total() const { return data_bytes + stages * kTileBytes + b2_bytes + p_bytes + 512; }
 };
@@ -110,14 +118,17 @@ constexpr int kMaxStages = 12;
 __host__ __device__ constexpr TcSmem tc_smem(int epi) {  // epi: 0 contour (activations), 1 onset, 2 note, 3 contour (fused)
   TcSmem s{};
   const int chunks = epi == 2 ? 33 : 39, rows = kMTile + (epi == 1 ? 4 : epi == 2 ? 6 : 2);
-  const int width = tc_b2_spec(epi).width;
+  const TcB2 b2 = tc_b2_spec(epi);
   s.data_bytes = (2 * chunks * rows * 16 + 1023) / 1024 * 1024;
-  s.b2_bytes = epi == 0 ? 0 : 2 * 128 * width * 2;
-  s.p_bytes = epi == 0 ? 0 : 2 * 64 * (width + 1) * 4;
+  s.b2_bytes = epi == 0 ? 0 : 2 * 128 * b2.width * 2;
+  s.p_bytes = epi == 0 ? 0 : 2 * 64 * (b2.pass + 1) * 4;
   const int st = (kMaxSmem - 512 - s.data_bytes - s.b2_bytes - s.p_bytes) / kTileBytes;
   s.stages = st < kMaxStages ? st : kMaxStages;
   return s;
 }
+// weight stages per layer (DESIGN §4.1): contour activations, onset, note, contour fused
+static_assert(tc_smem(0).stages == 12 && tc_smem(1).stages == 12 && tc_smem(2).stages == 11 && tc_smem(3).stages == 9,
+              "weight-ring depth per layer");
 // step word of a slot: [0,14) A start-address offset >> 4, [15] first MMA into that accumulator; kNoUse = the
 // slot's frequency tile does not use this step's weight tile
 constexpr uint32_t kUseFirstAcc = 1u << 15, kNoUse = 0xffffffffu;
@@ -285,9 +296,9 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
       i = j;
     }
     // Software skew between the two slots of a group: the steps only slot 0 uses come first, then the shared ones, then
-    // those only slot 1 uses.  Slot 1's next accumulator region is the one slot 0's previous tile still occupies until
-    // its conv2 MMAs are done (three regions for four tiles in flight); this way slot 0's tile finishes — and frees its
-    // region — early, and slot 1 needs its region late (the issuing warp acquires it at its first use), so neither waits.
+    // those only slot 1 uses.  The slots move through the weight ring independently (a slot skips the steps it does not
+    // use), so slot 0 runs its epilogue while slot 1 works through its own steps, and slot 1 runs its epilogue while
+    // slot 0 starts on the next group's.
     std::stable_sort(steps.begin(), steps.end(), [](const Step& a, const Step& b) {
       auto cls = [](const Step& s) { return s.w[1] == kNoUse ? 0 : (s.w[0] == kNoUse ? 2 : 1); };
       return cls(a) < cls(b);
@@ -482,6 +493,66 @@ struct TcArgs {
 
 __device__ __forceinline__ float sigmoidf_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 
+// Cycle accounting by role, compiled in with -DBP_TC_CLOCKS only (tools/tc_clocks.py): every thread cuts its time into
+// consecutive clock64 spans and adds each span to one bucket; lane 0 of every warp adds its sums to g_tc_clocks[layer]
+// when the CTA ends.  Without the flag the calls are empty.
+namespace tc {
+enum TcClk {
+  kClkFull,       // consumers: waiting on full_w (the weight tile of the step)
+  kClkMma,        // consumers: issuing the step's MMAs and waiting for the previous step's
+  kClkEpi,        // consumers: the epilogue of a tile (after the last MMA of the group)
+  kClkData,       // consumers: waiting on data_full (the item's data tile)
+  kClkConsOther,  // consumers: everything else (program reads, skipped steps, row set-up)
+  kClkEmpty,      // producer: waiting on empty_w (a free weight stage)
+  kClkDataEmpty,  // producer: waiting on data_empty (both slots done with the previous item's data tile)
+  kClkProdOther,  // producer: everything else (issuing the copies)
+  kNumClk
+};
+}  // namespace tc
+#ifdef BP_TC_CLOCKS
+__device__ unsigned long long g_tc_clocks[3][tc::kNumClk];
+struct TcClocks {
+  long long t, c[tc::kNumClk];
+  __device__ __forceinline__ TcClocks() {
+    t = clock64();
+#pragma unroll
+    for (int k = 0; k < tc::kNumClk; ++k) c[k] = 0;
+  }
+  __device__ __forceinline__ void lap(int k) {
+    const long long n = clock64();
+    c[k] += n - t;
+    t = n;
+  }
+  __device__ __forceinline__ void flush(int layer) {
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+      for (int k = 0; k < tc::kNumClk; ++k) atomicAdd(&g_tc_clocks[layer][k], (unsigned long long)c[k]);
+  }
+};
+#else
+struct TcClocks {
+  __device__ __forceinline__ void lap(int) {}
+  __device__ __forceinline__ void flush(int) {}
+};
+#endif
+
+int tc_read_clocks(int layer, unsigned long long* out, bool reset) {
+#ifdef BP_TC_CLOCKS
+  if (layer < 0 || layer > 2) return -1;
+  if (cudaMemcpyFromSymbol(out, g_tc_clocks, tc::kNumClk * sizeof(unsigned long long),
+                           (size_t)layer * tc::kNumClk * sizeof(unsigned long long)) != cudaSuccess)
+    return -1;
+  if (reset) {
+    static const unsigned long long zero[tc::kNumClk] = {};
+    if (cudaMemcpyToSymbol(g_tc_clocks, zero, sizeof(zero), (size_t)layer * sizeof(zero)) != cudaSuccess) return -1;
+  }
+  return 0;
+#else
+  (void)layer, (void)out, (void)reset;
+  return -1;
+#endif
+}
+
 __device__ __forceinline__ void slot_barrier(int slot) {  // the four warps (one warpgroup) of one accumulator slot
   asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
 }
@@ -659,7 +730,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   constexpr bool kFused = EPI != 0;
   constexpr int LAYER = EPI == 3 ? 0 : EPI;  // index into the constant banks
   constexpr TcB2 B2 = tc_b2_spec(EPI);
-  constexpr int NW = B2.width, PS = NW + 1;  // conv2 accumulator columns; row pitch of their staging
+  constexpr int NW = B2.width, PC = B2.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
+  static_assert(PC % 8 == 0 && PC % B2.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr TcSmem SM = tc_smem(EPI);
   constexpr int kStages = SM.stages;
@@ -674,6 +746,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   uint64_t* data_full = bars + 2 * kStages;
   uint64_t* data_empty = data_full + 1;  // one arrival per consumer warp
   uint64_t* b2_full = data_empty + 1;
+  uint32_t* issued = reinterpret_cast<uint32_t*>(b2_full + 1);  // weight fills the producer has issued so far
 
   // Broadcasting the warp index keeps the role branches and the producer loop state in uniform registers.
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -689,24 +762,32 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     mbar_init(data_full, 1);
     mbar_init(data_empty, kConsumerWarps);
     mbar_init(b2_full, 1);
+    *issued = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   const int n_items = a.n_mtiles * a.n_split;
+  TcClocks clk;
 
-  if (warp == kProducerWarp) {
+  if (warp >= kConsumerWarps) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp != kProducerWarp) return;
     // ------------------------------ producer ------------------------------
     // The whole warp walks the loop with warp-uniform state; the arrive / copy instructions are predicated on the elected
     // lane (no elect loop and R2UR around every UBLKCP: the weight ring is paced by this loop's latency per step).
+    // For a step that one slot does not use, the producer also arrives on the stage's empty_w for that slot's four warps,
+    // so the two slots move through the ring independently (see the consumers).
     const uint32_t leader = elect_one() ? 1u : 0u;
     if constexpr (kFused) bulk_g2s_expect_pred(s_b2, a.b2, (uint32_t)SM.b2_bytes, b2_full, leader);
-    uint32_t stage = 0, ph_w = 0, ph_d = 0;
+    uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;
     const size_t plane_elems = (size_t)a.chunks8 * a.rows_total * 8;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       const int mt = it / a.n_split, sp = it % a.n_split;
       const int g0 = sp * a.n_groups / a.n_split, g1 = (sp + 1) * a.n_groups / a.n_split;
+      clk.lap(kClkProdOther);
       mbar_wait_wd(data_empty, ph_d ^ 1, 1);
+      clk.lap(kClkDataEmpty);
       const size_t row = (size_t)mt * a.ms + a.row0;
       if (leader) {
         mbar_expect_tx(data_full, 2 * plane_bytes);
@@ -725,9 +806,15 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       int tile = c_tile_seq[a.layer][s0];
       for (int s = s0; s < s1; ++s) {
         const int tile_next = c_tile_seq[a.layer][s + 1];  // (one past the end is inside the array)
+        clk.lap(kClkProdOther);
         mbar_wait_wd(empty_w + stage, ph_w ^ 1, 2);
+        clk.lap(kClkEmpty);
         bulk_g2s_expect_pred(s_w + stage * kTileBytes, a.tiles + (size_t)tile * (kTileBytes / 2), kTileBytes, full_w + stage,
                              leader);
+        // every step has at least one user, so at most one slot skips it
+        const bool skip = c_prog[a.layer][0][s] == kNoUse || c_prog[a.layer][1][s] == kNoUse;
+        mbar_arrive_cnt_pred(empty_w + stage, kConsumerWarps / 2, skip ? leader : 0u);
+        counter_publish(issued, ++n_fill);
         if (++stage == kStages) {
           stage = 0;
           ph_w ^= 1;
@@ -735,7 +822,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         tile = tile_next;
       }
     }
-  } else if (warp < kConsumerWarps) {
+    clk.lap(kClkProdOther);
+    clk.flush(a.layer);
+  } else {
+    setmaxnreg_inc<kConsumerRegs>();
     // ------------------------------ consumers: one warpgroup per accumulator slot ------------------------------
     // conv1: the slot's frequency tile of the 64-row M-tile as m64n128k16 MMAs, accumulators in registers.  Fragment of a
     // thread (warp w of the group, lane = 4 gq + qd): rows 16 w + gq and 16 w + gq + 8, columns 8 i + 2 qd + {0, 1}.
@@ -749,7 +839,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int e = 0; e < 2; ++e) bz[i][e] = c_bias1[LAYER][LAYER == 0 ? 2 * qd + e : 8 * i + 2 * qd + e];
-    uint32_t stage = 0, ph_w = 0, ph_d = 0;
+    uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;  // n_fill: index of the current step's weight fill in the CTA
     const uint32_t a_hi = smem_u32(s_data), a_lo = a_hi + plane_bytes, w_base = smem_u32(s_w);
     const uint32_t* prog = c_prog[a.layer][slot];
     float* sp_rows = s_p + slot * 64 * PS;
@@ -800,18 +890,36 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
           }
         }
       }
+      clk.lap(kClkConsOther);
       mbar_wait_wd(data_full, ph_d, 3);
+      clk.lap(kClkData);
       ph_d ^= 1;
       for (int g = g0; g < g1; ++g) {
         const int ft = c_group_ft[a.layer][2 * g + slot];
         const int s0 = c_group_step_off[a.layer][g], s1 = c_group_step_off[a.layer][g + 1];
         float acc[64];
         int pend = -1;  // stage read by the MMA group still in flight
+        uint32_t pend_fill = 0;  // and its fill index
         uint32_t w = prog[s0];
-        for (int s = s0; s < s1; ++s) {
+        // A slot skips the steps it does not use (kNoUse) completely: no wait on full_w, no arrival on empty_w (the
+        // producer arrives for it).  So it does not see every phase of a stage, and its parity wait for fill f (the
+        // stage's phase f / kStages) is only exact if the stage is at most one phase off when it waits:
+        //   * not ahead: it first waits until the producer has ISSUED fill f.  That happened after the release of fill
+        //     f - kStages, whose user(s) waited for it to land, so the previous phase is complete;
+        //   * not behind: fill f + kStages cannot land before this slot's own arrival for fill f gates the refill.
+        for (int s = s0; s < s1; ++s, ++n_fill) {
           const uint32_t w_next = prog[s + 1];  // (one word past the end is inside the array)
-          mbar_wait_wd(full_w + stage, ph_w, 5);
           if (w != kNoUse) {
+            if (pend >= 0 && n_fill - pend_fill >= kStages) {
+              // fill f is issued after the release of fill f - kStages, which may be the stage still held
+              wgmma_wait<0>();
+              if (lane == 0) mbar_arrive(empty_w + pend);
+              pend = -1;
+            }
+            clk.lap(kClkConsOther);
+            counter_wait_above(issued, n_fill);
+            mbar_wait_wd(full_w + stage, ph_w, 5);
+            clk.lap(kClkFull);
             const uint32_t off = (w & 0x3fffu) << 4;  // chunk c8, row dt of the data tile
             const uint32_t bw = w_base + stage * kTileBytes;
             const uint64_t dah = make_desc(a_hi + off, lbo, 128), dal = make_desc(a_lo + off, lbo, 128);
@@ -824,14 +932,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
             wgmma_wait<1>();  // the previous step's MMAs are done: its weight stage may be refilled
             if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
             pend = (int)stage;
-          } else {
-            // a run of steps of the other slot may be longer than the ring: release the held stage before passing on
-            if (pend >= 0) {
-              wgmma_wait<0>();
-              if (lane == 0) mbar_arrive(empty_w + pend);
-              pend = -1;
-            }
-            if (lane == 0) mbar_arrive(empty_w + stage);
+            pend_fill = n_fill;
+            clk.lap(kClkMma);
           }
           if (++stage == kStages) {
             stage = 0;
@@ -839,8 +941,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
           }
           w = w_next;
         }
+        clk.lap(kClkConsOther);
         wgmma_wait<0>();
         reg_fence(acc);
+        clk.lap(kClkMma);
         if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
         if (g == g1 - 1 && lane == 0) mbar_arrive(data_empty);  // this warp's MMAs no longer read the data tile
         if (ft < 0) continue;
@@ -889,30 +993,38 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
           wgmma_commit();
           wgmma_wait<0>();
           reg_fence(p);
-          slot_barrier(slot);  // the previous tile's sums have been read
+          // time taps: the frame of tile row r takes P_dt from row r - (KH2 - 1 - dt), taps added from the own row down
+          // (the same order for every row: a frame's value does not depend on where the M-tile starts).  The sums go
+          // through the staging area PC columns (PC / JS output offsets j) at a time.
+          constexpr int KH2 = B2.kh2, JS = B2.js, JP = PC / JS;
+          constexpr int NJ = EPI == 3 ? 20 : 6;
+          float S[NJ];
 #pragma unroll
-          for (int i = 0; i < NW / 8; ++i)
+          for (int q = 0; q * JP < NJ; ++q) {
+            slot_barrier(slot);  // the previous pass's (or tile's) sums have been read
 #pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-              float* d = sp_rows + (fr0 + 8 * rr) * PS + 8 * i + 2 * qd;
-              d[0] = p[4 * i + 2 * rr];
-              d[1] = p[4 * i + 2 * rr + 1];
+            for (int i = 0; i < NW / 8; ++i) {
+              if (8 * i < q * PC || 8 * i >= (q + 1) * PC) continue;
+#pragma unroll
+              for (int rr = 0; rr < 2; ++rr) {
+                float* d = sp_rows + (fr0 + 8 * rr) * PS + 8 * i - q * PC + 2 * qd;
+                d[0] = p[4 * i + 2 * rr];
+                d[1] = p[4 * i + 2 * rr + 1];
+              }
             }
-          slot_barrier(slot);
+            slot_barrier(slot);
+            if (tid < 64) {
+#pragma unroll
+              for (int j = q * JP; j < NJ && j < (q + 1) * JP; ++j) {
+                float s = 0.f;
+#pragma unroll
+                for (int ta = 0; ta < KH2; ++ta)
+                  if (tid - ta >= 0) s += sp_rows[(tid - ta) * PS + j * JS - q * PC + (KH2 - 1 - ta)];
+                S[j] = s;
+              }
+            }
+          }
           if (tid < 64) {
-            // time taps: the frame of tile row r takes P_dt from row r - (KH2 - 1 - dt), taps added from the own row down
-            // (the same order for every row: a frame's value does not depend on where the M-tile starts)
-            constexpr int KH2 = B2.kh2, JS = B2.js;
-            constexpr int NJ = EPI == 3 ? 20 : 6;
-            float S[NJ];
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-              float s = 0.f;
-#pragma unroll
-              for (int ta = 0; ta < KH2; ++ta)
-                if (tid - ta >= 0) s += sp_rows[(tid - ta) * PS + j * JS + (KH2 - 1 - ta)];
-              S[j] = s;
-            }
             if constexpr (EPI == 3) {
               finish_contour_tile(a, ro, S, ft, first, last, carry, hold);
             } else {
@@ -923,8 +1035,11 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
             }
           }
         }
+        clk.lap(kClkEpi);
       }
     }
+    clk.lap(kClkConsOther);
+    clk.flush(a.layer);
   }
 }
 

@@ -22,6 +22,52 @@ __device__ __forceinline__ void mbar_expect_tx_only(uint64_t* bar, uint32_t byte
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// `count` arrivals at once, by the elected lane only (PTX predication, like bulk_g2s_expect_pred): one thread arriving
+// on behalf of several warps
+__device__ __forceinline__ void mbar_arrive_cnt_pred(uint64_t* bar, uint32_t count, uint32_t leader) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred q;\n\t"
+      "setp.ne.b32 q, %2, 0;\n\t"
+      "@q mbarrier.arrive.shared::cta.b64 _, [%0], %1;\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(count), "r"(leader)
+      : "memory");
+}
+// A 32-bit counter in shared memory that one warp advances and others wait on (release / acquire at CTA scope)
+__device__ __forceinline__ void counter_publish(uint32_t* ctr, uint32_t value) {
+  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(ctr)), "r"(value) : "memory");
+}
+// spin until the counter exceeds `value`; bounded like mbar_wait_wd (a protocol error traps instead of hanging)
+__device__ __forceinline__ void counter_wait_above(const uint32_t* ctr, uint32_t value) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p, q;\n\t"
+      ".reg .u32 v, spins;\n\t"
+      "mov.u32 spins, 0;\n\t"
+      "CTR_LOOP:\n\t"
+      "ld.acquire.cta.shared::cta.u32 v, [%0];\n\t"
+      "setp.gt.u32 p, v, %1;\n\t"
+      "@p bra CTR_DONE;\n\t"
+      "add.u32 spins, spins, 1;\n\t"
+      "setp.lt.u32 q, spins, 0x10000000;\n\t"
+      "@q bra CTR_LOOP;\n\t"
+      "trap;\n\t"
+      "CTR_DONE:\n\t"
+      "}\n" ::"r"(smem_u32(ctr)),
+      "r"(value)
+      : "memory");
+}
+// Per-warpgroup register budget (all four warps of the warpgroup execute it): the producer warpgroup gives registers
+// back, the MMA warpgroups take them
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t"

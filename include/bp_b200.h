@@ -243,6 +243,13 @@ int bp_debug_tc_b2(int which, const float* w2, int32_t* sizes, uint16_t* tiles);
 int bp_model_profile(bp_model_t* m, int which);
 int bp_model_profile_read(bp_model_t* m, double* total_ms, int64_t* n_intervals, int64_t* n_windows);
 
+/* Cycle accounting of the tensor-core conv kernels (tools/tc_clocks.py), available only in a library built with
+ * -DBP_TC_CLOCKS (BP_E_INVALID otherwise).  Synchronises the device and copies the SM cycles summed over all warps of
+ * all launches of layer `which` (0 contour, 1 onset, 2 note) since the last reset: cycles[8] = consumers waiting on a
+ * weight stage, issuing / waiting for MMAs, in the epilogue, waiting on the data tile, other; producer waiting on a free
+ * stage, waiting on the data tile to be released, other.  reset != 0 zeroes the sums after the copy. */
+int bp_debug_tc_clocks(bp_model_t* m, int which, uint64_t* cycles, int reset);
+
 #ifdef __cplusplus
 }
 #endif
