@@ -7,7 +7,6 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
-#include <mutex>
 #include <thread>
 #include <string>
 #include <vector>
@@ -149,8 +148,7 @@ struct bp_model {
     DevBuf<uint16_t> tiles, b2;
   } tc_contour, tc_onset, tc_note;
   DevBuf<__nv_bfloat16> yhl, chl;
-  std::vector<float> h_params;  // host copy of the parameter block (weight-dependent __constant__ data is re-uploaded
-                                // from it whenever another model used the device's constant bank in between)
+  Lowpass2 lp2{};  // decimation FIR taps, a parameter of every decimation launch
   DevBuf<uint16_t> cqt_wtc;  // three-way bf16 split of the CQT kernel matrix (tensor-core path)
   size_t chl_zeroed = 0;  // elements of chl known to hold zeros in every row/bin the kernels never write
   int64_t launches = 0;
@@ -199,15 +197,7 @@ struct bp_model {
 
 namespace {
 
-// Weight-dependent data in __constant__ memory (FIR taps, conv1 biases, fused conv2 weights) is shared by all models
-// of a process on one device; remember whose values are resident.
-// The bank is guarded per device: a launch sequence that depends on it (forward_chunk) holds the device's mutex while
-// it enqueues, and a change of owner first drains the device so that kernels of the previous owner that are still in
-// flight never see the new values.  Models with different weights may therefore be used from several host threads;
-// they serialise at chunk granularity.
 thread_local int64_t g_need_notes = 0, g_need_bends = 0;  // bp_last_required
-const bp_model* g_const_owner[64] = {};
-std::mutex g_const_mu[64];
 
 struct DeviceGuard {
   int prev = -1;
@@ -280,33 +270,26 @@ int parse_blob(const void* blob, size_t nbytes, std::vector<float>& params) {
   return BP_OK;
 }
 
-int upload_constants(bp_model* m, cudaStream_t st) {
-  const float* hp = m->h_params.data();
-  if (m->device >= 0 && m->device < 64 && g_const_owner[m->device] && g_const_owner[m->device] != m)
-    CK(cudaDeviceSynchronize());  // kernels of the previous owner may still be reading the bank
-  upload_lowpass(hp + ParamLayout::lowpass, st);
-  tc_upload_epilogue(hp + ParamLayout::contour1_b, hp + ParamLayout::onset1_b, hp + ParamLayout::note1_b,
-                     hp + ParamLayout::onset2_w, hp + ParamLayout::contour2_b, hp + ParamLayout::onset2_b, hp + ParamLayout::note2_b, st);
-  CKL();
-  if (m->device >= 0 && m->device < 64) g_const_owner[m->device] = m;
-  return BP_OK;
-}
-
 int derive(bp_model* m, cudaStream_t st) {
   derive_kernel<<<(256 * 72 + 255) / 256, 256, 0, st>>>(m->d_params, m->d_derived);
   CKL();
   m->launches += 1;
-  // tensor-core plans: split-bf16 Toeplitz weight tiles + MMA programs (host-built from the parameter block)
-  m->h_params.resize(ParamLayout::total);
-  std::vector<float>& hp = m->h_params;
+  // host-built from the parameter block: the decimation taps, the tensor-core plans (split-bf16 Toeplitz weight tiles +
+  // MMA programs) and the epilogue values of the tensor-core convs
+  std::vector<float> hp(ParamLayout::total);
   CK(cudaMemcpyAsync(hp.data(), m->d_params, sizeof(float) * ParamLayout::total, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  m->lp2 = lowpass_pairs(hp.data() + ParamLayout::lowpass);
   const TcConvSpec specs[3] = {tc_contour_spec(), tc_onset_spec(), tc_note_spec()};
   bp_model::TcLayer* layers[3] = {&m->tc_contour, &m->tc_onset, &m->tc_note};
   const float* wsrc[3] = {hp.data() + ParamLayout::contour1_w, hp.data() + ParamLayout::onset1_w,
                           hp.data() + ParamLayout::note1_w};
   const float* w2src[3] = {hp.data() + ParamLayout::contour2_w, hp.data() + ParamLayout::onset2_w,
                            hp.data() + ParamLayout::note2_w};
+  const float* b1src[3] = {hp.data() + ParamLayout::contour1_b, hp.data() + ParamLayout::onset1_b,
+                           hp.data() + ParamLayout::note1_b};
+  const float* b2src[3] = {hp.data() + ParamLayout::contour2_b, hp.data() + ParamLayout::onset2_b,
+                           hp.data() + ParamLayout::note2_b};
   for (int l = 0; l < 3; ++l) {
     bp_model::TcLayer& L = *layers[l];
     L.plan.build(specs[l], wsrc[l]);
@@ -322,6 +305,9 @@ int derive(bp_model* m, cudaStream_t st) {
     CK(cudaMemcpyAsync(L.b2.p, b2.data(), b2.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
     L.dev = TcConvDev{pl.spec, L.tiles.p, L.b2.p, pl.n_groups, l};
+    std::copy_n(b1src[l], pl.spec.COUT, L.dev.bias1);
+    L.dev.bias2 = *b2src[l];
+    if (l == 1) std::copy_n(hp.data() + ParamLayout::onset2_w, 9, L.dev.note_w);  // channel 0: the note input
   }
   {
     std::vector<uint16_t> wtc;
@@ -330,9 +316,7 @@ int derive(bp_model* m, cudaStream_t st) {
     CK(cudaMemcpyAsync(m->cqt_wtc.p, wtc.data(), wtc.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
   }
-  std::unique_lock<std::mutex> const_lock;
-  if (m->device >= 0 && m->device < 64) const_lock = std::unique_lock<std::mutex>(g_const_mu[m->device]);
-  return upload_constants(m, st);
+  return BP_OK;
 }
 
 int ensure_forward_ws(bp_model* m, int nb) {
@@ -403,15 +387,9 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
                   float* contour, cudaStream_t st, const UnwrapDesc* ud = nullptr, const PostI* u = nullptr) {
   float* chain = m->chain.p;
   if (m->profile_which >= 0) m->prof_windows += nb;
-  std::unique_lock<std::mutex> const_lock;
-  if (m->device >= 0 && m->device < 64) const_lock = std::unique_lock<std::mutex>(g_const_mu[m->device]);
-  if (m->device >= 0 && m->device < 64 && g_const_owner[m->device] != m) {
-    int rc = upload_constants(m, st);
-    if (rc) return rc;
-  }
   {
     ProfScope ps(m, 3, st);
-    for (int s = 0; s < 8; ++s) launch_decimate(audio, desc, chain, s, nb, st);
+    for (int s = 0; s < 8; ++s) launch_decimate(m->lp2, audio, desc, chain, s, nb, st);
   }
   const TcConvSpec cs = tc_contour_spec(), ns = tc_note_spec();
   const int ystride = tc_rows_total(m->chunk, cs.rows_per_window), cstride = tc_rows_total(m->chunk, ns.rows_per_window);
@@ -642,10 +620,6 @@ void bp_model_destroy(bp_model_t* m) {
   if (!m) return;
   DeviceGuard g(m->device);
   cudaDeviceSynchronize();
-  if (m->device >= 0 && m->device < 64) {
-    std::lock_guard<std::mutex> lk(g_const_mu[m->device]);
-    if (g_const_owner[m->device] == m) g_const_owner[m->device] = nullptr;
-  }
   m->chain.release(); m->y.release(); m->c1.release(); m->n1.release(); m->o1.release();
   m->raw_note.release(); m->raw_onset.release(); m->raw_contour.release(); m->minmax.release(); m->edge.release();
   m->i_note.release(); m->i_onset.release(); m->i_contour.release(); m->u_note.release(); m->u_onset.release();

@@ -21,44 +21,41 @@ __device__ __forceinline__ void ffma2(float2& d, float o, float2 w) {
   d.y = fmaf(o, w.y, d.y);
 }
 
-// Low-pass taps as pairs: c_lp2[k] = (h[k - 12], h[k - 14]), zero outside the 256 taps.  A thread that
-// owns outputs 8t .. 8t+7 feeds sample u of its input run into the output pairs (0,1), (2,3), (4,5), (6,7) with
-// c_lp2[u + 12], c_lp2[u + 8], c_lp2[u + 4], c_lp2[u].
-constexpr int kLp2 = kTaps + 14;
-__constant__ float2 c_lp2[kLp2];
-
-void upload_lowpass(const float* h_lp, cudaStream_t st) {
-  float2 tab[kLp2];  // (the copy is synchronised below)
+// Low-pass taps as pairs: t[k] = (h[k - 12], h[k - 14]), zero outside the 256 taps.  A thread that owns outputs
+// 8t .. 8t+7 feeds sample u of its input run into the output pairs (0,1), (2,3), (4,5), (6,7) with t[u + 12],
+// t[u + 8], t[u + 4], t[u].
+Lowpass2 lowpass_pairs(const float* h_lp) {
+  Lowpass2 lp;
   for (int k = 0; k < kLp2; ++k) {
     const int u = k - 12;
-    tab[k].x = (u >= 0 && u < kTaps) ? h_lp[u] : 0.f;
-    tab[k].y = (u - 2 >= 0 && u - 2 < kTaps) ? h_lp[u - 2] : 0.f;
+    lp.t[k].x = (u >= 0 && u < kTaps) ? h_lp[u] : 0.f;
+    lp.t[k].y = (u - 2 >= 0 && u - 2 < kTaps) ? h_lp[u - 2] : 0.f;
   }
-  cudaMemcpyToSymbolAsync(c_lp2, tab, sizeof(tab), 0, cudaMemcpyHostToDevice, st);
-  cudaStreamSynchronize(st);
+  return lp;
 }
 
 // ------------------------------------------------------------------------------------------------
 // Half-band FIR + decimate by 2:  x_{o+1}[n] = sum_k LP[k] * x_o[2n + k - 127].
 // Input runs live in shared memory de-interleaved into 16 phases (sample li at ph[(li & 15) * S + (li >> 4)], S == 2
 // mod 32: conflict-free scatter and gather); thread t owns outputs 8t .. 8t+7, so every loaded sample feeds up to 8
-// FMAs whose tap pairs are uniform-register operands from constant memory.  Each
-// output still accumulates its 256 products in tap order.
+// FMAs whose tap pairs are uniform-register operands from the kernel parameters (constant bank 0; fir8 reads them
+// through a reference to the __grid_constant__ parameter, so they are never copied).  Each output still accumulates its
+// 256 products in tap order.
 //   decimate_kernel       stages 0-3: one CTA = 1024 outputs of one window
 //   decimate_tail_kernel  stages 4-7 (2740 -> 171 samples): one CTA per window runs the four stages back to back through
 //                         shared memory (as four launches they were latency-bound: 25 % of the chain's time for 6 % of
 //                         its work)
 // ------------------------------------------------------------------------------------------------
 template <int S>
-__device__ __forceinline__ void fir8(const float* __restrict__ ph, int t, float (&out)[8]) {
+__device__ __forceinline__ void fir8(const Lowpass2& lp, const float* __restrict__ ph, int t, float (&out)[8]) {
   float2 a01 = make_float2(0.f, 0.f), a23 = a01, a45 = a01, a67 = a01;
 #pragma unroll
-  for (int u = 0; u < kTaps + 14; ++u) {
+  for (int u = 0; u < kLp2; ++u) {
     const float v = ph[(u & 15) * S + t + (u >> 4)];
-    if (u < kTaps + 2) ffma2(a01, v, c_lp2[u + 12]);
-    if (u >= 4 && u < kTaps + 6) ffma2(a23, v, c_lp2[u + 8]);
-    if (u >= 8 && u < kTaps + 10) ffma2(a45, v, c_lp2[u + 4]);
-    if (u >= 12) ffma2(a67, v, c_lp2[u]);
+    if (u < kTaps + 2) ffma2(a01, v, lp.t[u + 12]);
+    if (u >= 4 && u < kTaps + 6) ffma2(a23, v, lp.t[u + 8]);
+    if (u >= 8 && u < kTaps + 10) ffma2(a45, v, lp.t[u + 4]);
+    if (u >= 12) ffma2(a67, v, lp.t[u]);
   }
   out[0] = a01.x, out[1] = a01.y, out[2] = a23.x, out[3] = a23.y;
   out[4] = a45.x, out[5] = a45.y, out[6] = a67.x, out[7] = a67.y;
@@ -68,7 +65,8 @@ constexpr int kDecTile = 1024;
 constexpr int kDecThreads = 128;
 constexpr int kDecS = 162;  // positions per phase: (2 * 1024 + 270) / 16 = 145 -> next value == 2 (mod 32)
 
-__global__ void __launch_bounds__(kDecThreads) decimate_kernel(const float* __restrict__ audio,
+__global__ void __launch_bounds__(kDecThreads) decimate_kernel(const __grid_constant__ Lowpass2 lp,
+                                                               const float* __restrict__ audio,
                                                                const WinDesc* __restrict__ desc,  // stage 0 only
                                                                const float* __restrict__ src,     // chain, stage >= 1
                                                                float* __restrict__ dst, int src_off, int dst_off,
@@ -104,7 +102,7 @@ __global__ void __launch_bounds__(kDecThreads) decimate_kernel(const float* __re
   const int n = n0 + 8 * t;
   if (n >= len_out) return;
   float o[8];
-  fir8<kDecS>(ph, t, o);
+  fir8<kDecS>(lp, ph, t, o);
   float* d = dst + (size_t)b * kChainStride + dst_off;
   if (n + 7 < len_out) {
     *reinterpret_cast<float4*>(d + n) = make_float4(o[0], o[1], o[2], o[3]);
@@ -121,7 +119,8 @@ constexpr int kTailThreads = 256;
 constexpr int kTailS = 194;       // (2740 + 127 + 270) / 16 = 197 positions would be needed for reads past the last output's run;
                                   // active threads (8t < 1370) read positions <= 171 + 16, 194 == 2 (mod 32)
 
-__global__ void __launch_bounds__(kTailThreads) decimate_tail_kernel(float* __restrict__ chain) {
+__global__ void __launch_bounds__(kTailThreads) decimate_tail_kernel(const __grid_constant__ Lowpass2 lp,
+                                                                     float* __restrict__ chain) {
   __shared__ float buf[2][16 * kTailS];
   float* c = chain + (size_t)blockIdx.x * kChainStride;
   const int tid = threadIdx.x;
@@ -143,7 +142,7 @@ __global__ void __launch_bounds__(kTailThreads) decimate_tail_kernel(float* __re
     const int n = 8 * tid;
     if (n < len_out) {
       float o[8];
-      fir8<kTailS>(buf[cur], tid, o);
+      fir8<kTailS>(lp, buf[cur], tid, o);
       float* d = c + chain_off_rt(stage + 1);
 #pragma unroll
       for (int i = 0; i < 8; ++i)
@@ -158,17 +157,17 @@ __global__ void __launch_bounds__(kTailThreads) decimate_tail_kernel(float* __re
   }
 }
 
-void launch_decimate(const float* audio, const WinDesc* desc, float* chain, int stage, int n_windows,
+void launch_decimate(const Lowpass2& lp, const float* audio, const WinDesc* desc, float* chain, int stage, int n_windows,
                      cudaStream_t st) {
   if (stage > kTailFirst) return;  // done by the tail launch
   if (stage == kTailFirst) {
-    decimate_tail_kernel<<<n_windows, kTailThreads, 0, st>>>(chain);
+    decimate_tail_kernel<<<n_windows, kTailThreads, 0, st>>>(lp, chain);
     return;
   }
   // stage s: x_s -> x_{s+1}
   const int len_in = octave_len(stage), len_out = octave_len(stage + 1);
   dim3 grid((len_out + kDecTile - 1) / kDecTile, n_windows);
-  decimate_kernel<<<grid, kDecThreads, 0, st>>>(audio, desc, chain, chain, stage ? chain_off(stage) : 0,
+  decimate_kernel<<<grid, kDecThreads, 0, st>>>(lp, audio, desc, chain, chain, stage ? chain_off(stage) : 0,
                                                  chain_off(stage + 1), len_in, len_out, stage == 0);
 }
 

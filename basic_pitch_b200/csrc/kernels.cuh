@@ -11,8 +11,15 @@ namespace bp {
 
 // ---- hcqt.cu ------------------------------------------------------------------------------------
 void hcqt_setup();  // per device: shared-memory opt-in of the FP32 CQT kernel
-void upload_lowpass(const float* h_lp, cudaStream_t st);  // host taps -> __constant__ tap pairs
-void launch_decimate(const float* audio, const WinDesc* desc, float* chain, int stage, int n_windows, cudaStream_t st);
+// The decimation low-pass taps as the zero-padded pairs the FIR reads (hcqt.cu); every decimation launch takes them as
+// a kernel parameter (2.2 KB).
+constexpr int kLp2 = kTaps + 14;
+struct Lowpass2 {
+  float2 t[kLp2];
+};
+Lowpass2 lowpass_pairs(const float* h_lp /* host: the 256 taps of the parameter block */);
+void launch_decimate(const Lowpass2& lp, const float* audio, const WinDesc* desc, float* chain, int stage, int n_windows,
+                     cudaStream_t st);
 void launch_cqt(const float* audio, const WinDesc* desc, const float* chain, const float* wt, const float* scale,
                 float* logmag, unsigned int* minmax, int n_windows, cudaStream_t st);
 void launch_lognorm(float* y, const unsigned int* minmax, const float* bn /* device: scale, bias */, int n_windows,
@@ -67,10 +74,13 @@ struct TcConvDev {
   const uint16_t* b2;  // conv2 weight matrix of the fused epilogue (tc_build_b2_full)
   int n_groups;
   int layer;  // index of the program in constant memory (0 contour, 1 onset, 2 note)
+  // epilogue values, passed with every launch: conv1 bias (COUT used), conv2 bias, and for the onset layer the conv2
+  // weights of its note input channel (models.py:305: concat[note, onset1]) [dt][df]
+  float bias1[32];
+  float bias2;
+  float note_w[9];
 };
 int tc_upload_program(int layer, const TcConvPlan& plan, cudaStream_t st);  // 0 on success
-void tc_upload_epilogue(const float* contour1_b, const float* onset1_b, const float* note1_b, const float* onset2_w,
-                        const float* contour2_b, const float* onset2_b, const float* note2_b, cudaStream_t st);
 // bf16 hi/lo weight tiles of the fused second conv (epi: 0 contour, 1 onset, 2 note; w2 = that conv's weights), see TcB2
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out);
 // the same tiles placed into the K = 128 x N = width conv2 weight matrix the kernel reads (tc_conv.cu)

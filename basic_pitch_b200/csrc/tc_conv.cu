@@ -328,23 +328,6 @@ __constant__ uint32_t c_prog[3][2][tc::kMaxSteps];  // [layer][slot][step]
 __constant__ int c_tile_seq[3][tc::kMaxSteps];       // [layer][step] -> weight tile id
 __constant__ int c_group_step_off[3][tc::kMaxGroups + 1];
 __constant__ int c_group_ft[3][2 * tc::kMaxGroups];
-// epilogue constants: conv1 bias, conv2 bias
-__constant__ float c_bias1[3][32];
-__constant__ float c_bias2[3];
-// channel 0 of the onset conv2 multiplies the note posteriorgram (models.py:305: concat[note, onset1]): [dt][df]
-__constant__ float c_onset_note_w[9];
-
-void tc_upload_epilogue(const float* contour1_b, const float* onset1_b, const float* note1_b, const float* onset2_w,
-                        const float* contour2_b, const float* onset2_b, const float* note2_b, cudaStream_t st) {
-  float b[3][32] = {};
-  for (int i = 0; i < 8; ++i) b[0][i] = contour1_b[i];
-  for (int i = 0; i < 32; ++i) b[1][i] = onset1_b[i], b[2][i] = note1_b[i];
-  const float b2[3] = {contour2_b[0], onset2_b[0], note2_b[0]};
-  cudaMemcpyToSymbolAsync(c_bias1, b, sizeof(b), 0, cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_bias2, b2, sizeof(b2), 0, cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_onset_note_w, onset2_w, 9 * sizeof(float), 0, cudaMemcpyHostToDevice, st);
-  cudaStreamSynchronize(st);
-}
 
 // tiles: [tile][plane hi/lo][k-chunk 2][n N2][8] bf16 (canonical K-major no-swizzle: LBO = N2 * 16 B, SBO = 128 B)
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
@@ -489,6 +472,7 @@ struct TcArgs {
   int ms, h2;                   // M-tile stride (64 - 2*h2) and time halo of the fused conv2
   int chunks8, rows_per_window;
   int cout, flt, wout, n_ft, g0;
+  float bias1[32], bias2, note_w[9];  // the layer's epilogue values (TcConvDev)
 };
 
 __device__ __forceinline__ float sigmoidf_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
@@ -580,7 +564,6 @@ struct RowOut {
 template <int EPI>
 __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut& ro, float (&S)[6], float (&carry)[2], int ft,
                                                   bool first, bool last) {
-  constexpr int L = EPI == 1 ? 1 : 2;
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
@@ -611,13 +594,13 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
     for (int j = 0; j < 5; ++j) {
       if (j < jlo || j >= jhi) continue;
       const int f = 4 * ft - 1 + j;
-      float x = S[j] + c_bias2[L];
+      float x = S[j] + a.bias2;
       if constexpr (EPI == 1) {
 #pragma unroll
         for (int r = 0; r < 3; ++r)
 #pragma unroll
           for (int df = 0; df < 3; ++df)
-            if (j + df < 6) x = fmaf(nv[r][j + df], c_onset_note_w[r * 3 + df], x);  // pitch f + df - 1 = 4 ft - 2 + (j + df)
+            if (j + df < 6) x = fmaf(nv[r][j + df], a.note_w[r * 3 + df], x);  // pitch f + df - 1 = 4 ft - 2 + (j + df)
       }
       const float v = sigmoidf_fast(x);
       if (ro.raw) ro.raw[(size_t)f * a.o.raw_rows] = v;
@@ -665,7 +648,7 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
 #pragma unroll
       for (int k = 0; k < 4; ++k) e[(size_t)k * a.edge_rows] = S[k];
 #pragma unroll
-      for (int k = 0; k < 6; ++k) e[(size_t)(4 + k) * a.edge_rows] = sigmoidf_fast(S[4 + k] + c_bias2[0]);  // bins 16 ft + 2 .. + 7
+      for (int k = 0; k < 6; ++k) e[(size_t)(4 + k) * a.edge_rows] = sigmoidf_fast(S[4 + k] + a.bias2);  // bins 16 ft + 2 .. + 7
     }
   } else {
 #pragma unroll
@@ -673,7 +656,7 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
   }
   float fin[16];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) fin[j] = sigmoidf_fast(S[j] + c_bias2[0]);
+  for (int j = 0; j < 16; ++j) fin[j] = sigmoidf_fast(S[j] + a.bias2);
   if (ro.ok) {
     if (!first) {  // chunk 2 ft - 1: bins 16 ft - 8 .. 16 ft - 1
       const float v[8] = {hold[0], hold[1], hold[2], hold[3], hold[4], hold[5], fin[0], fin[1]};
@@ -728,7 +711,6 @@ template <int EPI>
 __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using namespace tc;
   constexpr bool kFused = EPI != 0;
-  constexpr int LAYER = EPI == 3 ? 0 : EPI;  // index into the constant banks
   constexpr TcB2 B2 = tc_b2_spec(EPI);
   constexpr int NW = B2.width, PC = B2.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
   static_assert(PC % 8 == 0 && PC % B2.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
@@ -838,7 +820,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) bz[i][e] = c_bias1[LAYER][LAYER == 0 ? 2 * qd + e : 8 * i + 2 * qd + e];
+      for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[EPI == 0 || EPI == 3 ? 2 * qd + e : 8 * i + 2 * qd + e];
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;  // n_fill: index of the current step's weight fill in the CTA
     const uint32_t a_hi = smem_u32(s_data), a_lo = a_hi + plane_bytes, w_base = smem_u32(s_w);
     const uint32_t* prog = c_prog[a.layer][slot];
@@ -1055,6 +1037,7 @@ struct EdgeFixArgs {
   int n_edges;                  // 2 * n_split slots: slot e = s * n_split + q starts at tile q * n_groups / n_split + s * G0
   int n_split, n_groups, g0, n_ft;
   int layer, wout, rows_per_window, n_windows;
+  float bias2, note_w[9];  // the layer's conv2 bias; onset: the conv2 weights of the note input channel
 };
 
 __global__ void edge_fix_kernel(const EdgeFixArgs a) {
@@ -1082,7 +1065,7 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
     float fx[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q)  // (S + carry) + bias, the order of the in-kernel carry
-      fx[q] = sigmoidf_fast((lo[(size_t)q * a.edge_rows] + hi[(size_t)q * a.edge_rows]) + c_bias2[0]);
+      fx[q] = sigmoidf_fast((lo[(size_t)q * a.edge_rows] + hi[(size_t)q * a.edge_rows]) + a.bias2);
     float va[8], vb[8];
 #pragma unroll
     for (int q = 0; q < 6; ++q) {
@@ -1112,7 +1095,7 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
   const int f = 4 * ft_b - 1 + k;
   if (f < 0 || f >= a.wout) return;
   float x = (a.o.edge[((size_t)(e * 2 + 0) * 2 + k) * a.edge_rows + R] +
-             a.o.edge[((size_t)(e * 2 + 1) * 2 + k) * a.edge_rows + R]) + c_bias2[a.layer];  // (S + carry) + bias
+             a.o.edge[((size_t)(e * 2 + 1) * 2 + k) * a.edge_rows + R]) + a.bias2;  // (S + carry) + bias
   if (a.o.note_raw) {
 #pragma unroll
     for (int dt = 0; dt < 3; ++dt)
@@ -1120,7 +1103,7 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
       for (int df = 0; df < 3; ++df) {
         const int tt = t + dt - 1, ff = f + df - 1;
         if ((unsigned)tt < (unsigned)kFrames && (unsigned)ff < (unsigned)kPitches)
-          x = fmaf(__ldg(a.o.note_raw + (size_t)ff * a.o.raw_rows + (size_t)b * kFrames + tt), c_onset_note_w[dt * 3 + df], x);
+          x = fmaf(__ldg(a.o.note_raw + (size_t)ff * a.o.raw_rows + (size_t)b * kFrames + tt), a.note_w[dt * 3 + df], x);
       }
   }
   const float v = sigmoidf_fast(x);
@@ -1193,6 +1176,9 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   a.wout = sp.WOUT;
   a.n_ft = (sp.WOUT + sp.FLT - 1) / sp.FLT;
   a.g0 = sp.G0;
+  std::copy_n(dev.bias1, 32, a.bias1);
+  a.bias2 = dev.bias2;
+  std::copy_n(dev.note_w, 9, a.note_w);
   const int n_items = a.n_mtiles * a.n_split;
   const int grid = n_items < n_sms ? n_items : n_sms;
   {
@@ -1244,10 +1230,12 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
     ef.n_groups = dev.n_groups;
     ef.g0 = sp.G0;
     ef.n_ft = a.n_ft;
-    ef.layer = sp.epi;  // c_bias2 index: 0 contour, 1 onset, 2 note
+    ef.layer = sp.epi;  // 0 contour, 1 onset, 2 note
     ef.wout = sp.WOUT;
     ef.rows_per_window = sp.rows_per_window;
     ef.n_windows = n_windows;
+    ef.bias2 = dev.bias2;
+    std::copy_n(dev.note_w, 9, ef.note_w);
     const long long total = (long long)ef.n_rows * ef.n_edges * (sp.epi == 0 ? 1 : 2);
     edge_fix_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ef);
   }

@@ -442,10 +442,10 @@ def test_predict_batch_and_error_paths(model, tmp_path):
 
 
 def test_two_models_with_different_weights_do_not_interfere(model, weights_np, tmp_path):
-    """Weight-dependent constants and the MMA programs live in __constant__ memory shared by all models of a process on
-    one device; the library re-uploads the constants when the active model changes, and the programs are the same for
-    every model (the reference allows loading several model files side by side).  The second model's conv1 weights
-    differ in which taps are zero, so content-based tile de-duplication would have given it a different program."""
+    """The MMA programs live in __constant__ memory shared by all models of a process on one device and are the same for
+    every model; the weight-dependent values (low-pass taps, biases) travel with each launch (the reference allows
+    loading several model files side by side).  The second model's conv1 weights differ in which taps are zero, so
+    content-based tile de-duplication would have given it a different program."""
     from basic_pitch_b200 import synth, weights
     from basic_pitch_b200.inference import Model
     from oracle import model_ref

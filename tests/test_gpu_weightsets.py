@@ -217,9 +217,9 @@ def test_run_inference_arrays_under_dense_weights(models):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("order", [("sparse", "trained", "dense"), ("dense", "trained", "sparse")])
 def test_models_with_different_weights_in_one_process(blob_paths, windows, order):
-    """The MMA programs and the weight-dependent constants live in __constant__ memory shared by every model of the
-    process.  Models created in either order, called interleaved, must each compute the oracle under their OWN weights,
-    and give the same bits on every call."""
+    """The MMA programs live in __constant__ memory shared by every model of the process; the weight-dependent values
+    are kernel parameters of each model's launches.  Models created in either order, called interleaved, must each
+    compute the oracle under their OWN weights, and give the same bits on every call."""
     from basic_pitch_b200.inference import Model
 
     x = windows[[0, 1, 6, 8, 12]]
@@ -233,6 +233,44 @@ def test_models_with_different_weights_in_one_process(blob_paths, windows, order
     finally:
         ms.clear()
         gc.collect()
+
+
+def test_models_with_different_weights_run_concurrently(models, windows):
+    """bp_forward_device only enqueues on the caller's stream (bp_b200.h).  Model A's call is queued on stream S1 behind
+    a ~0.5 s sleep; model B, with other weights, is then called on stream S2 and must return while A's work is still
+    pending: no call drains the device for another model.  Both results must be the bits of each model's own serial
+    call, which matches the oracle under that model's weights."""
+    import torch
+
+    x = windows[[0, 1, 6, 8, 12]]
+    n = len(x)
+    pair = {"trained": models["trained"], "dense": models["dense"]}
+    ref = {name: _check_forward(m, name, x, 1, "concurrent", label=" (serial)") for name, m in pair.items()}
+    dev = torch.device("cuda", pair["trained"].device)
+    d_x = torch.from_numpy(x).to(dev)
+    outs = {name: [torch.empty((n, 172, w), dtype=torch.float32, device=dev) for w in (88, 88, 264)] for name in pair}
+    streams = {"trained": torch.cuda.Stream(dev), "dense": torch.cuda.Stream(dev)}
+
+    def forward(name):
+        m, o = pair[name], outs[name]
+        m._lib.bp_forward_device(m.handle, d_x.data_ptr(), n, o[0].data_ptr(), o[1].data_ptr(), o[2].data_ptr(),
+                                 streams[name].cuda_stream)
+
+    for name in pair:  # both workspaces at this batch size: no allocation below
+        forward(name)
+    torch.cuda.synchronize(dev)
+    a_done = torch.cuda.Event()
+    with torch.cuda.stream(streams["trained"]):
+        torch.cuda._sleep(1_000_000_000)  # SM clock cycles: about 0.5 s
+    forward("trained")
+    a_done.record(streams["trained"])
+    forward("dense")
+    a_pending = not a_done.query()
+    torch.cuda.synchronize(dev)
+    assert a_pending, "model B's bp_forward_device waited for model A's work on another stream"
+    for name in pair:
+        for k, t in zip(POSTS, outs[name]):
+            np.testing.assert_array_equal(t.cpu().numpy(), ref[name][k], err_msg=f"{name} {k}, concurrent call")
 
 
 def test_refresh_with_other_weights_and_restore(blob_paths, windows):
