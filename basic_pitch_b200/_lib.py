@@ -24,7 +24,7 @@ EXPORTS = [
     "bp_model_create", "bp_model_destroy", "bp_model_device", "bp_model_param_block", "bp_model_refresh",
     "bp_model_launch_count", "bp_forward_device", "bp_forward_host", "bp_run_inference_device",
     "bp_run_inference_host", "bp_decode_device", "bp_decode_host", "bp_transcribe_host", "bp_transcribe_device",
-    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files",
+    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host",
 ]  # fmt: skip
 
 
@@ -126,6 +126,7 @@ def load() -> C.CDLL:
     lib.bp_debug_resample_filter.argtypes = [i32, i32, vp, i64]
     lib.bp_debug_resample_filter.restype = i64
     lib.bp_write_note_files.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, C.c_double, i32]
+    lib.bp_sonify_notes_host.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, i64]
     lib.bp_model_profile.argtypes = [vp, C.c_int]
     lib.bp_model_profile_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64), C.POINTER(i64)]
     for name in EXPORTS:

@@ -28,6 +28,7 @@ int fail(int code, const std::string& msg) {
 }  // namespace
 namespace bp {
 int writer_fail(int code, const std::string& msg) { return fail(code, msg); }  // writers.cu reports through bp_last_error
+int sonify_fail(int code, const std::string& msg) { return fail(code, msg); }  // sonify.cu likewise
 }
 namespace {
 
@@ -1088,6 +1089,22 @@ int bp_pitch_bends_host(bp_model_t* m, const float* h_contour, int64_t n_frames,
   CK(cudaMemcpyAsync(h_bends, m->d_bends.p, sizeof(int) * (size_t)total, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
+}
+
+int bp_sonify_notes_host(bp_model_t* m, int32_t n_files, const int32_t* note_off, const double* start_s,
+                         const double* end_s, const int32_t* pitch_midi, const float* amplitude, const int32_t* bend_off,
+                         const int32_t* bends, int32_t multiple_pitch_bends, int32_t sample_rate, int64_t* h_sample_off,
+                         double* h_audio, int64_t capacity) {
+  if (!m) return fail(BP_E_INVALID, "bp_sonify_notes_host: bad argument");
+  if (!h_audio)  // size query: host only
+    return sonify_notes(nullptr, nullptr, n_files, note_off, start_s, end_s, pitch_midi, amplitude, bend_off, bends,
+                        multiple_pitch_bends, sample_rate, h_sample_off, nullptr, capacity);
+  DeviceGuard g(m->device);
+  long long launches = 0;
+  const int rc = sonify_notes(m->stream, &launches, n_files, note_off, start_s, end_s, pitch_midi, amplitude, bend_off,
+                              bends, multiple_pitch_bends, sample_rate, h_sample_off, h_audio, capacity);
+  m->launches += launches;
+  return rc;
 }
 
 int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,

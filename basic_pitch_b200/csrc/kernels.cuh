@@ -186,4 +186,11 @@ void launch_note_finish(const float* note, const float* contour, const long long
                         int* bends, int n_notes, int with_bends, const double* gauss /*[51] device*/,
                         cudaStream_t st);
 
+// ---- sonify.cu: bp_sonify_notes_host on the given stream of the current device (h_audio == NULL: size query, no CUDA
+// call); adds its kernel launches to *launches ---------------------------------------------------------------------------
+int sonify_notes(cudaStream_t st, long long* launches, int32_t n_files, const int32_t* note_off, const double* start_s,
+                 const double* end_s, const int32_t* pitch_midi, const float* amplitude, const int32_t* bend_off,
+                 const int32_t* bends, int32_t multiple_pitch_bends, int32_t sample_rate, int64_t* h_sample_off,
+                 double* h_audio, int64_t capacity);
+
 }  // namespace bp

@@ -15,45 +15,13 @@
 #include <vector>
 
 #include "bp_b200.h"
+#include "midi_events.h"
 
 namespace bp {
 int writer_fail(int code, const std::string& msg);  // api.cu: sets bp_last_error
 }
 
 namespace {
-
-struct Ev {  // one note event of a file, bends as a range of the batch's flat array
-  double start, end;
-  long long pitch;
-  float amp;
-  const int32_t* bends;  // nullptr = dropped / none
-  int n_bends;
-};
-
-// Python's tuple comparison of (start, end, pitch, amplitude, [bends]) as used by sorted() in drop_overlapping_pitch_bends
-bool ev_less(const Ev& a, const Ev& b) {
-  if (a.start != b.start) return a.start < b.start;
-  if (a.end != b.end) return a.end < b.end;
-  if (a.pitch != b.pitch) return a.pitch < b.pitch;
-  if (a.amp != b.amp) return a.amp < b.amp;
-  const int n = std::min(a.n_bends, b.n_bends);
-  for (int i = 0; i < n; ++i)
-    if (a.bends[i] != b.bends[i]) return a.bends[i] < b.bends[i];
-  return a.n_bends < b.n_bends;
-}
-
-// reference: note_creation.py:274-286
-void drop_overlapping_pitch_bends(std::vector<Ev>& ev) {
-  std::stable_sort(ev.begin(), ev.end(), ev_less);
-  for (size_t i = 0; i + 1 < ev.size(); ++i)
-    for (size_t j = i + 1; j < ev.size(); ++j) {
-      if (ev[j].start >= ev[i].end) break;
-      ev[i].bends = nullptr, ev[i].n_bends = 0;
-      ev[j].bends = nullptr, ev[j].n_bends = 0;
-    }
-}
-
-inline int velocity_of(float amp) { return (int)std::nearbyintf(127.0f * amp); }  // int(np.round(127 * np.float32))
 
 void put_vlq(std::string& out, long long n) {
   unsigned char buf[10];
@@ -82,20 +50,11 @@ struct MidiMsg {
 };
 
 // midi.PrettyMIDI.write for the object note_events_to_midi builds (resolution 220, one tempo)
-std::string midi_bytes(std::vector<Ev> ev, bool multiple_pitch_bends, double tempo) {
-  if (!multiple_pitch_bends) drop_overlapping_pitch_bends(ev);
+std::string midi_bytes(std::vector<bp::Ev> ev, bool multiple_pitch_bends, double tempo) {
+  if (!multiple_pitch_bends) bp::drop_overlapping_pitch_bends(ev);
   const double resolution = 220.0;
   auto tick_of = [&](double t) { return (long long)std::nearbyint(t * resolution * tempo / 60.0); };
-  // instruments in order of first use: one per pitch with multiple_pitch_bends, else a single one
-  std::vector<long long> inst_key;
-  std::vector<std::vector<int>> inst_events;
-  for (int i = 0; i < (int)ev.size(); ++i) {
-    const long long key = multiple_pitch_bends ? ev[i].pitch : 0;
-    size_t k = 0;
-    while (k < inst_key.size() && inst_key[k] != key) ++k;
-    if (k == inst_key.size()) inst_key.push_back(key), inst_events.emplace_back();
-    inst_events[k].push_back(i);
-  }
+  const bp::Instruments inst = bp::group_instruments(ev, multiple_pitch_bends);
   std::vector<std::string> tracks;
   {
     std::string meta;
@@ -109,33 +68,23 @@ std::string midi_bytes(std::vector<Ev> ev, bool multiple_pitch_bends, double tem
     tracks.push_back(meta);
   }
   const int program = 4;  // "Electric Piano 1"
-  for (size_t idx = 0; idx < inst_key.size(); ++idx) {
+  for (size_t idx = 0; idx < inst.key.size(); ++idx) {
     static const int channels[15] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 11, 12, 13, 14, 15};
     const int ch = channels[idx % 15];
     std::vector<MidiMsg> msgs;
     msgs.push_back({0, 0, {(unsigned char)(0xC0 | ch), (unsigned char)(program & 0x7F), 0}, 2});
-    for (int i : inst_events[idx]) {
-      const Ev& e = ev[i];
-      const int vel = std::max(0, std::min(127, velocity_of(e.amp)));
+    for (int i : inst.events[idx]) {
+      const bp::Ev& e = ev[i];
+      const int vel = std::max(0, std::min(127, bp::velocity_of(e.amp)));
       msgs.push_back({tick_of(e.start), 2, {(unsigned char)(0x90 | ch), (unsigned char)(e.pitch & 0x7F), (unsigned char)vel}, 3});
       msgs.push_back({tick_of(e.end), 1, {(unsigned char)(0x90 | ch), (unsigned char)(e.pitch & 0x7F), 0}, 3});
     }
-    for (int i : inst_events[idx]) {
-      const Ev& e = ev[i];
+    for (int i : inst.events[idx]) {
+      const bp::Ev& e = ev[i];
       if (e.n_bends <= 0) continue;
-      // np.linspace(start, end, n): i * step + start, the last one exactly `end`
-      const double step = e.n_bends > 1 ? (e.end - e.start) / (double)(e.n_bends - 1) : 0.0;
       for (int b = 0; b < e.n_bends; ++b) {
-        double t;
-        if (e.n_bends == 1)
-          t = e.start;
-        else if (b == e.n_bends - 1)
-          t = e.end;
-        else
-          t = (step != 0.0) ? (double)b * step + e.start : (double)b * (e.end - e.start) / (double)(e.n_bends - 1) + e.start;
-        long long v = (long long)std::nearbyint((double)e.bends[b] * 4096.0 / 3.0);  // PITCH_BEND_SCALE / bins per semitone
-        v = std::max(-8192LL, std::min(8191LL, v)) + 8192;
-        msgs.push_back({tick_of(t), 0, {(unsigned char)(0xE0 | ch), (unsigned char)(v & 0x7F), (unsigned char)((v >> 7) & 0x7F)}, 3});
+        const long long v = bp::bend_tick(e.bends[b]) + 8192;
+        msgs.push_back({tick_of(bp::bend_time(e, b)), 0, {(unsigned char)(0xE0 | ch), (unsigned char)(v & 0x7F), (unsigned char)((v >> 7) & 0x7F)}, 3});
       }
     }
     std::stable_sort(msgs.begin(), msgs.end(),
@@ -186,17 +135,17 @@ void put_float_repr(std::string& out, double x) {
   }
 }
 
-std::string csv_bytes(const std::vector<Ev>& ev) {
+std::string csv_bytes(const std::vector<bp::Ev>& ev) {
   std::string out = "start_time_s,end_time_s,pitch_midi,velocity,pitch_bend\r\n";
   char buf[32];
-  for (const Ev& e : ev) {
+  for (const bp::Ev& e : ev) {
     put_float_repr(out, e.start);
     out.push_back(',');
     put_float_repr(out, e.end);
     out.push_back(',');
     out.append(buf, std::to_chars(buf, buf + sizeof(buf), e.pitch).ptr);
     out.push_back(',');
-    out.append(buf, std::to_chars(buf, buf + sizeof(buf), velocity_of(e.amp)).ptr);
+    out.append(buf, std::to_chars(buf, buf + sizeof(buf), bp::velocity_of(e.amp)).ptr);
     for (int b = 0; b < e.n_bends; ++b) {
       out.push_back(',');
       out.append(buf, std::to_chars(buf, buf + sizeof(buf), e.bends[b]).ptr);
@@ -226,11 +175,7 @@ extern "C" int bp_write_note_files(int32_t n_files, const char* const* midi_path
   std::vector<int> failed(n_threads, -1);
   auto work = [&](int t) {
     for (int i = t; i < n_files; i += n_threads) {
-      std::vector<Ev> ev;
-      for (int j = note_off[i]; j < note_off[i + 1]; ++j) {
-        const int nb = bend_off ? bend_off[j + 1] - bend_off[j] : 0;
-        ev.push_back({start_s[j], end_s[j], pitch_midi[j], amplitude[j], nb > 0 ? bends + bend_off[j] : nullptr, nb});
-      }
+      const std::vector<bp::Ev> ev = bp::file_events(i, note_off, start_s, end_s, pitch_midi, amplitude, bend_off, bends);
       bool ok = true;
       if (csv_paths && csv_paths[i]) ok = write_file(csv_paths[i], csv_bytes(ev)) && ok;
       if (midi_paths && midi_paths[i]) ok = write_file(midi_paths[i], midi_bytes(ev, multiple_pitch_bends != 0, midi_tempo)) && ok;

@@ -685,8 +685,9 @@ def predict_and_save(
     """reference: inference.py:509-604 — same files, names and failure behaviour (print, then re-raise).
 
     Several files without `debug_file` go through the batch path: one device pass per `BATCH_FILES` files
-    (`predict_batch`: GPU ingest, one library call) and one `bp_write_note_files` call for their MIDI / CSV files
-    (csrc/writers.cu) instead of a Python loop over files and notes."""
+    (`predict_batch`: GPU ingest, one library call), one `bp_write_note_files` call for their MIDI / CSV files
+    (csrc/writers.cu) and, for `sonify_midi` with the bundled MIDI stand-in, one `bp_sonify_notes_host` call for their
+    WAV samples (csrc/sonify.cu) instead of a Python loop over files and notes."""
 
     def _saved(kind: str, path) -> None:
         print(f"  ✅ Saved {kind.lower().replace('_', ' ')} to {path}")
@@ -696,6 +697,10 @@ def predict_and_save(
 
     paths = list(audio_path_list)
     if len(paths) > 1 and debug_file is None:
+        from scipy.io import wavfile
+
+        from . import midi as bundled_midi
+
         model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
         BATCH_FILES = 64
         for c0 in range(0, len(paths), BATCH_FILES):
@@ -704,6 +709,10 @@ def predict_and_save(
                 print(f"\nPredicting MIDI for {q}...")
             results = predict_batch([pathlib.Path(q) for q in chunk], model, onset_threshold, frame_threshold, minimum_note_length,
                                     minimum_frequency, maximum_frequency, multiple_pitch_bends, melodia_trick, midi_tempo)
+            # the GPU renders the bundled stand-in's synthesiser; with the real pretty_midi installed, its own synthesiser
+            # makes the file, one by one
+            gpu_sonify = sonify_midi and infer.pretty_midi is bundled_midi
+            sonified: Optional[List[np.ndarray]] = None
             midi_paths: List[Optional[pathlib.Path]] = [None] * len(chunk)
             csv_paths: List[Optional[pathlib.Path]] = [None] * len(chunk)
             for i, (audio_path, (model_output, midi_data, _events)) in enumerate(zip(chunk, results)):
@@ -720,7 +729,13 @@ def predict_and_save(
                 if sonify_midi:
                     path = build_output_path(audio_path, output_directory, OutputExtensions.MIDI_SONIFICATION)
                     try:
-                        infer.sonify_midi(midi_data, path, sr=sonification_samplerate)
+                        if gpu_sonify:  # the whole chunk rendered in one library call, when the first file needs it
+                            if sonified is None:
+                                sonified = infer.sonify_batch([r[2] for r in results], sonification_samplerate,
+                                                              multiple_pitch_bends, model)
+                            wavfile.write(path, sonification_samplerate, sonified[i])
+                        else:
+                            infer.sonify_midi(midi_data, path, sr=sonification_samplerate)
                         _saved(OutputExtensions.MIDI_SONIFICATION.name, path)
                     except Exception:
                         _failed(OutputExtensions.MIDI_SONIFICATION.name, path)

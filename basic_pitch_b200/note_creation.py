@@ -221,16 +221,10 @@ def note_events_batch(arrs: Dict[str, np.ndarray], n_files: int, include_pitch_b
     return out if lazy else [e.to_list() for e in out]
 
 
-def write_note_files(event_lists: Sequence[Sequence], midi_paths: Optional[Sequence], csv_paths: Optional[Sequence],
-                     multiple_pitch_bends: bool = False, midi_tempo: float = 120, n_threads: int = 0) -> None:
-    """One MIDI file and / or one note-event CSV per file of a batch in a single library call (`bp_write_note_files`,
-    csrc/writers.cu: host threads over the files, no per-note Python objects).  Same bytes as
-    `note_events_to_midi(events, ...).write(path)` with this package's MIDI writer and `inference.save_note_events`.
-    event_lists: one `NoteEventList` (or list of event tuples) per file; paths: one per file, None entries are skipped."""
-    import ctypes as C
-
-    from . import _lib
-
+def _pack_note_events(event_lists: Sequence[Sequence]):
+    """The events of a batch as the concatenated arrays of the batch entry points (include/bp_b200.h: bp_write_note_files,
+    bp_sonify_notes_host) -> (note_off int32, start_s f64, end_s f64, pitch int32, amplitude f32, bend_off int32, bends
+    int32).  event_lists: one `NoteEventList` (or list of event tuples) per file."""
     n_files = len(event_lists)
     per = []
     for ev in event_lists:
@@ -260,6 +254,21 @@ def write_note_files(event_lists: Sequence[Sequence], midi_paths: Optional[Seque
         a, b = int(noff[i]), int(noff[i + 1])
         boff[a : b + 1] = p[4] + base
         base += int(p[4][-1])
+    return noff, st, en, pitch, amp, boff, flat
+
+
+def write_note_files(event_lists: Sequence[Sequence], midi_paths: Optional[Sequence], csv_paths: Optional[Sequence],
+                     multiple_pitch_bends: bool = False, midi_tempo: float = 120, n_threads: int = 0) -> None:
+    """One MIDI file and / or one note-event CSV per file of a batch in a single library call (`bp_write_note_files`,
+    csrc/writers.cu: host threads over the files, no per-note Python objects).  Same bytes as
+    `note_events_to_midi(events, ...).write(path)` with this package's MIDI writer and `inference.save_note_events`.
+    event_lists: one `NoteEventList` (or list of event tuples) per file; paths: one per file, None entries are skipped."""
+    import ctypes as C
+
+    from . import _lib
+
+    n_files = len(event_lists)
+    noff, st, en, pitch, amp, boff, flat = _pack_note_events(event_lists)
 
     def c_paths(paths):
         if paths is None:
@@ -270,6 +279,29 @@ def write_note_files(event_lists: Sequence[Sequence], midi_paths: Optional[Seque
     _lib.load().bp_write_note_files(n_files, c_paths(midi_paths), c_paths(csv_paths), noff.ctypes.data, st.ctypes.data,
                                     en.ctypes.data, pitch.ctypes.data, amp.ctypes.data, boff.ctypes.data, flat.ctypes.data,
                                     int(bool(multiple_pitch_bends)), float(midi_tempo), int(n_threads))
+
+
+def sonify_batch(event_lists: Sequence[Sequence], sr: int = 44100, multiple_pitch_bends: bool = False,
+                 model=None) -> List[np.ndarray]:
+    """`note_events_to_midi(events, multiple_pitch_bends).synthesize(sr)` of the bundled `midi` stand-in for every file
+    of a batch, rendered on the GPU in one library call (`bp_sonify_notes_host`, csrc/sonify.cu).  Returns one float64
+    array per file (empty for a file without notes), views of one page-locked block.  The samples differ from the
+    stand-in's only by the rounding of the phase (DESIGN.md §4.4).  event_lists: one `NoteEventList` (or list of event
+    tuples) per file."""
+    from .inference import default_model
+
+    mdl = model if model is not None else default_model()
+    n_files = len(event_lists)
+    noff, st, en, pitch, amp, boff, flat = _pack_note_events(event_lists)
+    soff = np.zeros(n_files + 1, np.int64)
+    args = (n_files, noff.ctypes.data, st.ctypes.data, en.ctypes.data, pitch.ctypes.data, amp.ctypes.data,
+            boff.ctypes.data, flat.ctypes.data, int(bool(multiple_pitch_bends)), int(sr), soff.ctypes.data)
+    mdl._lib.bp_sonify_notes_host(mdl.handle, *args, None, 0)  # size query
+    total = int(soff[-1])
+    out = mdl._pinned.array((total,), np.float64)
+    mdl._lib.bp_sonify_notes_host(mdl.handle, *args, out.ctypes.data, total)
+    offs = soff.tolist()
+    return [out[a:b] for a, b in zip(offs[:-1], offs[1:])]
 
 
 def drop_overlapping_pitch_bends(note_events_with_pitch_bends: List[NoteEvent]) -> List[NoteEvent]:
@@ -405,7 +437,8 @@ def get_infered_onsets(onsets, frames, n_diff: int = 2, model=None):
 
 
 __all__ = [
-    "model_output_to_notes", "output_to_notes_polyphonic", "note_events_to_midi", "write_note_files", "note_events_batch",
+    "model_output_to_notes", "output_to_notes_polyphonic", "note_events_to_midi", "write_note_files", "sonify_batch",
+    "note_events_batch",
     "NoteEventList", "LazyPrettyMIDI", "drop_overlapping_pitch_bends",
     "model_frames_to_time", "constrain_frequency", "midi_pitch_to_contour_bin", "sonify_midi", "sonify_salience",
     "get_pitch_bends", "get_infered_onsets", "SONIFY_FS",

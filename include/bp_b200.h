@@ -216,6 +216,21 @@ int bp_write_note_files(int32_t n_files, const char* const* midi_paths, const ch
                         const float* amplitude, const int32_t* bend_off, const int32_t* bends,
                         int32_t multiple_pitch_bends, double midi_tempo, int32_t n_threads);
 
+/* MIDI sonification of a batch of files on the GPU: for file i the float64 samples of
+ * note_events_to_midi(events_i, multiple_pitch_bends).synthesize(sample_rate) with this package's additive stand-in
+ * synthesiser (basic_pitch_b200/midi.py: PrettyMIDI.synthesize), which stands in for the reference's sonify_midi
+ * (basic_pitch/note_creation.py:119-128, called by inference.py:586-592).  The note arrays are those of
+ * bp_write_note_files (times in seconds, finite and >= 0; bend_off may be NULL).  h_sample_off[n_files + 1] is always
+ * written: file i's samples are h_audio[h_sample_off[i] .. h_sample_off[i+1]), none for a file without notes.
+ * h_audio == NULL is a size query (host only, no device work); otherwise `capacity` (in samples) must hold them all
+ * (BP_E_CAPACITY).  sample_rate <= 0 or malformed offsets: BP_E_INVALID.  Synchronous on the model's device; the
+ * device buffers are sized per call (about 8 bytes per output sample), and a file is never split, so one very long
+ * file is one unit of work.  Samples match the stand-in except for the rounding of the phase (DESIGN.md §4.4). */
+int bp_sonify_notes_host(bp_model_t* m, int32_t n_files, const int32_t* note_off, const double* start_s,
+                         const double* end_s, const int32_t* pitch_midi, const float* amplitude, const int32_t* bend_off,
+                         const int32_t* bends, int32_t multiple_pitch_bends, int32_t sample_rate, int64_t* h_sample_off,
+                         double* h_audio, int64_t capacity);
+
 /* Host-only: the low-pass of the ingest resampler for the reduced ratio up / down (unit DC gain, before the gain `up`);
  * returns the number of taps, copies them if capacity allows.  Tests pin it against scipy.signal.firwin. */
 int64_t bp_debug_resample_filter(int32_t up, int32_t down, double* taps, int64_t capacity);
