@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <thread>
 #include <string>
 #include <vector>
@@ -134,7 +135,7 @@ __global__ void compact_notes_kernel(const long long* __restrict__ frame_off, co
 struct bp_model {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t copy_stream = nullptr;  // host->device audio copies of bp_transcribe_host run ahead of the compute stream
+  cudaStream_t copy_stream = nullptr;  // host->device audio copies of the host entry points run ahead of the compute stream
   std::vector<cudaEvent_t> copy_ev;
   float* d_params = nullptr;
   float* d_derived = nullptr;
@@ -166,8 +167,8 @@ struct bp_model {
   // staging for the host entry points
   DevBuf<float> st_audio, st_note, st_onset, st_contour;
   DevBuf<unsigned char> st_pcm;  // bp_load_pcm_host
-  // bp_transcribe_files_host: pinned gather buffers (one sub-batch of audio each), the device->host stream of the
-  // posteriorgrams and its events
+  // pinned gather buffers of per-file input (one sub-batch of audio each); the device->host stream of the posteriorgrams
+  // and its events
   float* gather[3] = {nullptr, nullptr, nullptr};
   size_t gather_cap = 0;  // floats per buffer
   cudaStream_t d2h_stream = nullptr;
@@ -349,6 +350,23 @@ int ensure_forward_ws(bp_model* m, int nb) {
       CK(cudaMemset(m->chl.p, 0, m->chl.cap * sizeof(__nv_bfloat16)));
       m->chl_zeroed = m->chl.cap;
     }
+  }
+  return BP_OK;
+}
+
+// Row-major posteriorgram staging of the model (st_note / st_onset / st_contour) for `n_frames` frames.
+int reserve_rows(bp_model* m, int64_t n_frames) {
+  CK(m->st_note.reserve((size_t)n_frames * kPitches + 4));
+  CK(m->st_onset.reserve((size_t)n_frames * kPitches + 4));
+  CK(m->st_contour.reserve((size_t)n_frames * kContourBins + 4));
+  return BP_OK;
+}
+
+int ensure_events(std::vector<cudaEvent_t>& ev, size_t n) {
+  while (ev.size() < n) {
+    cudaEvent_t e;
+    CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    ev.push_back(e);
   }
   return BP_OK;
 }
@@ -706,12 +724,11 @@ int bp_forward_host(bp_model_t* m, const float* h_audio, int64_t n_windows, floa
   if (n_windows < 0) return fail(BP_E_INVALID, "bp_forward_host: negative window count");
   DeviceGuard g(m->device);
   CK(m->st_audio.reserve((size_t)n_windows * kWinSamples));
-  CK(m->st_note.reserve((size_t)n_windows * kFrames * kPitches));
-  CK(m->st_onset.reserve((size_t)n_windows * kFrames * kPitches));
-  CK(m->st_contour.reserve((size_t)n_windows * kFrames * kContourBins));
+  int rc = reserve_rows(m, n_windows * kFrames);
+  if (rc) return rc;
   cudaStream_t st = m->stream;
   CK(cudaMemcpyAsync(m->st_audio.p, h_audio, sizeof(float) * n_windows * kWinSamples, cudaMemcpyHostToDevice, st));
-  int rc = bp_forward_device(m, m->st_audio.p, n_windows, m->st_note.p, m->st_onset.p, m->st_contour.p, st);
+  rc = bp_forward_device(m, m->st_audio.p, n_windows, m->st_note.p, m->st_onset.p, m->st_contour.p, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(h_note, m->st_note.p, sizeof(float) * n_windows * kFrames * kPitches, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(h_onset, m->st_onset.p, sizeof(float) * n_windows * kFrames * kPitches, cudaMemcpyDeviceToHost, st));
@@ -802,22 +819,247 @@ static int run_inference_internal(bp_model* m, const float* d_audio, const int64
   return BP_OK;
 }
 
-// internal posteriorgram buffers of the model for `total_frames` frames
-static int reserve_internal(bp_model* m, int64_t total_frames, PostI* u) {
-  const size_t F = (size_t)((total_frames + 31) / 32 * 32 + 32);
-  CK(m->u_note.reserve(kPitches * F));
-  CK(m->u_onset.reserve(kPitches * F));
-  CK(m->u_contour.reserve((size_t)kContourBins * F));
-  *u = PostI{m->u_note.p, m->u_onset.p, m->u_contour.p, (long long)F};
+namespace {
+// Host threads that copy the files of one sub-batch after the other into pinned staging buffers, running ahead of the
+// caller: worker t copies its share of sub-batch k as soon as the caller has released that buffer (`released` counts the
+// sub-batches whose buffer may be overwritten) and reports it in done[k].  The threads live for one call.
+struct Gatherer {
+  const float* const* audio;
+  const int64_t* rel;        // [n_files + 1] sample offsets
+  const int* cut;            // [n_sub + 1] file index where each sub-batch starts
+  int n_sub, n_threads;
+  float* const* stage;       // 3 staging buffers
+  std::atomic<int> released{0};
+  std::vector<std::atomic<int>> done;
+  std::vector<std::thread> threads;
+  std::atomic<bool> abort{false};
+
+  Gatherer(const float* const* a, const int64_t* r, const int* c, int ns, int nt, float* const* st)
+      : audio(a), rel(r), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
+    for (auto& d : done) d.store(0);
+    for (int t = 0; t < n_threads; ++t) threads.emplace_back([this, t] { run(t); });
+  }
+  ~Gatherer() {
+    abort.store(true);
+    for (auto& x : threads) x.join();
+  }
+  void run(int t) {
+    for (int k = 0; k < n_sub; ++k) {
+      for (int spins = 0; released.load(std::memory_order_acquire) <= k; ++spins) {  // buffer k % 3 still holds k - 3
+        if (abort.load()) return;
+        if (spins < 64)
+          std::this_thread::yield();
+        else
+          std::this_thread::sleep_for(std::chrono::microseconds(50));  // do not fight the enqueueing thread for cores
+      }
+      const int f0 = cut[k], f1 = cut[k + 1];
+      const int64_t base = rel[f0], total = rel[f1] - base;
+      float* dst = stage[k % 3];
+      // thread t copies samples [lo, hi) of the sub-batch: whole files where possible, split files otherwise
+      const int64_t lo = base + total * t / n_threads, hi = base + total * (t + 1) / n_threads;
+      if (hi > lo) {
+        int i = (int)(std::upper_bound(rel + f0, rel + f1 + 1, lo) - rel) - 1;
+        for (; i < f1 && rel[i] < hi; ++i) {
+          const int64_t a = std::max(lo, rel[i]), b = std::min(hi, rel[i + 1]);
+          if (b > a) std::memcpy(dst + (a - base), audio[i] + (a - rel[i]), sizeof(float) * (size_t)(b - a));
+        }
+      }
+      done[k].fetch_add(1, std::memory_order_release);
+    }
+  }
+  void release_upto(int k) { released.store(k, std::memory_order_release); }  // sub-batches < k may be gathered
+  void wait(int k) {
+    while (done[k].load(std::memory_order_acquire) < n_threads) std::this_thread::yield();
+  }
+};
+
+// A batch of whole files as an entry point received it: packed back to back (`audio`, in device memory if `on_device`,
+// else in host memory) or one host pointer per file (`files`).
+struct Batch {
+  const char* api;             // the calling entry point, prefix of every message
+  const float* audio;          // packed: the caller's array; describe_batch moves it to the first file's samples
+  bool on_device;
+  const float* const* files;
+  std::vector<int64_t> rel{};  // [n_files + 1] sample offsets from the first file (describe_batch)
+  int64_t total_frames = 0;    // frames of the posteriorgrams (describe_batch)
+  int n_files() const { return (int)rel.size() - 1; }
+};
+
+struct Rows {
+  float *note, *onset, *contour;
+};
+}  // namespace
+
+// Validates the files of `b` (packed: sample_off [n_files + 1]; per file: n_samples [n_files]) and fills in their
+// offsets relative to the first file and the frames of the batch.
+static int describe_batch(Batch& b, const int64_t* sample_off, const int64_t* n_samples, int32_t n_files) {
+  const std::string api = b.api;
+  if (sample_off && b.audio) b.audio += sample_off[0];
+  b.rel.assign(n_files + 1, 0);
+  b.total_frames = 0;
+  for (int i = 0; i < n_files; ++i) {
+    const int64_t n = sample_off ? sample_off[i + 1] - sample_off[i] : n_samples[i];
+    if (n < 0 && sample_off) return fail(BP_E_INVALID, api + ": sample offsets must be non-decreasing");
+    if (n < 0) return fail(BP_E_INVALID, api + ": file " + std::to_string(i) + " has a negative length");
+    if (n > 0 && !(b.files ? b.files[i] : b.audio))
+      return fail(BP_E_INVALID, api + ": null audio for file " + std::to_string(i));
+    b.rel[i + 1] = b.rel[i] + n;
+    b.total_frames += bp_num_frames(n);
+  }
   return BP_OK;
 }
 
-// internal -> the row-major arrays of the C ABI (any of the destinations may be null)
-static void internal_to_rows(bp_model* m, const PostI& u, int64_t total_frames, float* d_note, float* d_onset,
-                             float* d_contour, cudaStream_t st) {
-  if (d_note) launch_pm_to_rows(u.note, u.stride, 0, total_frames, kPitches, d_note, st), m->launches += 1;
-  if (d_onset) launch_pm_to_rows(u.onset, u.stride, 0, total_frames, kPitches, d_onset, st), m->launches += 1;
-  if (d_contour) launch_cm_to_rows(u.contour, u.stride, 0, total_frames, d_contour, st), m->launches += 1;
+// Sub-batches of whole files, as the index of each one's first file plus n_files.  Device input is one sub-batch.  On
+// host input the first two hold at most one chunk of windows (their uploads are the ones the kernels cannot hide), the
+// next two at most two and the rest at most four; two for per-file input, whose three pinned staging buffers each hold
+// a whole sub-batch, so that the cap bounds their size.
+static std::vector<int> cut_sub_batches(const Batch& b, int64_t chunk) {
+  const int n_files = b.n_files();
+  if (b.on_device) return {0, n_files};
+  const int64_t cap = b.files ? 2 : 4;
+  std::vector<int> cut{0};
+  int64_t w = 0;
+  for (int i = 0; i < n_files; ++i) {
+    const size_t k = cut.size() - 1;
+    const int64_t limit = std::min<int64_t>(k < 2 ? 1 : (k < 4 ? 2 : 4), cap) * chunk;
+    const int64_t nw = bp_num_windows(b.rel[i + 1] - b.rel[i]);
+    if (w > 0 && w + nw > limit) {
+      cut.push_back(i);
+      w = 0;
+    }
+    w += nw;
+  }
+  cut.push_back(n_files);
+  return cut;
+}
+
+// The whole-file pipeline of every bp_run_inference_* / bp_transcribe_* entry point: windows -> forward -> unwrap ->
+// row-major posteriorgrams in `rows` (device memory; the model's staging when null), sub-batch by sub-batch
+// (cut_sub_batches).  Host input is uploaded on the copy stream ahead of the kernels, and the posteriorgrams of each
+// sub-batch go to `host` (any may be null) on the device->host stream while later ones compute.  Then the decode, if
+// `params` is given.  Device input only enqueues on `st` (the decode synchronises it); host input returns synchronised.
+static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, const bp_decode_params_t* params,
+                     bp_notes_t* notes, int64_t* h_frame_off, cudaStream_t st) {
+  const int n_files = b.n_files();
+  int rc = rows ? BP_OK : reserve_rows(m, b.total_frames);
+  if (rc) return rc;
+  const Rows d = rows ? *rows : Rows{m->st_note.p, m->st_onset.p, m->st_contour.p};
+  // internal (frame-fastest) posteriorgrams of the whole batch
+  const size_t F = (size_t)((b.total_frames + 31) / 32 * 32 + 32);
+  CK(m->u_note.reserve(kPitches * F));
+  CK(m->u_onset.reserve(kPitches * F));
+  CK(m->u_contour.reserve((size_t)kContourBins * F));
+  const PostI u{m->u_note.p, m->u_onset.p, m->u_contour.p, (long long)F};
+  const std::vector<int> cut = cut_sub_batches(b, m->chunk);
+  const int n_sub = (int)cut.size() - 1;
+  const bool from_host = !b.on_device, to_host = host.note || host.onset || host.contour;
+  if (from_host) {
+    CK(m->st_audio.reserve((size_t)std::max<int64_t>(b.rel[n_files], 1)));
+    if ((rc = ensure_events(m->copy_ev, n_sub))) return rc;
+  }
+  if (to_host) {
+    if (!m->d2h_stream) CK(cudaStreamCreateWithFlags(&m->d2h_stream, cudaStreamNonBlocking));
+    if ((rc = ensure_events(m->conv_ev, n_sub))) return rc;
+  }
+  int n_threads = 0;
+  if (b.files) {
+    size_t max_sub = 1;
+    for (int k = 0; k < n_sub; ++k) max_sub = std::max<size_t>(max_sub, (size_t)(b.rel[cut[k + 1]] - b.rel[cut[k]]));
+    if (max_sub > m->gather_cap) {
+      for (float*& g : m->gather) {
+        if (g) cudaFreeHost(g);
+        g = nullptr;
+      }
+      m->gather_cap = 0;
+      const size_t want = max_sub + max_sub / 8;
+      for (float*& g : m->gather) CK(cudaHostAlloc(&g, want * sizeof(float), cudaHostAllocDefault));
+      m->gather_cap = want;
+    }
+    n_threads = (int)std::max(1u, std::min(16u, std::thread::hardware_concurrency() > 2 ? std::thread::hardware_concurrency() - 1 : 1u));
+  }
+  const bool timing = from_host && getenv("BP_B200_TIMING") != nullptr;  // host-side breakdown of this call on stderr
+  auto now = [] { return std::chrono::steady_clock::now(); };
+  auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(now() - t).count(); };
+  const auto t_call = now();
+  double t_gather = 0, t_wait = 0, t_launch = 0;
+  if (from_host) CK(cudaStreamSynchronize(st));  // st_audio / st_note.. may still be in use by earlier work on the compute stream
+  std::unique_ptr<Gatherer> gatherer;
+  if (b.files) {
+    gatherer.reset(new Gatherer(b.files, b.rel.data(), cut.data(), n_sub, n_threads, m->gather));
+    gatherer->release_upto(std::min(3, n_sub));  // the three buffers are free: the workers start at once
+  }
+  h_frame_off[0] = 0;
+  // Iteration k queues sub-batch k, then copies the posteriorgrams of k - 1 to the host: a copy into pageable memory
+  // returns only once it is done, so the kernels of the next sub-batch must already be queued to keep the device busy.
+  for (int k = 0; k <= n_sub; ++k) {
+    auto t0 = now();
+    if (k < n_sub) {
+      const int f0 = cut[k], f1 = cut[k + 1];
+      const int64_t s0 = b.rel[f0], s1 = b.rel[f1];
+      if (from_host) {
+        if (gatherer) {
+          gatherer->wait(k);  // sub-batch k is in its staging buffer (gathered while earlier sub-batches were enqueued)
+          t_gather += ms_since(t0);
+          t0 = now();
+        }
+        const float* src = gatherer ? m->gather[k % 3] : b.audio + s0;
+        if (s1 > s0)
+          CK(cudaMemcpyAsync(m->st_audio.p + s0, src, sizeof(float) * (size_t)(s1 - s0), cudaMemcpyHostToDevice, m->copy_stream));
+        CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
+        CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
+      }
+      const int64_t base = h_frame_off[f0];  // run_inference_internal writes the offsets relative to it
+      rc = run_inference_internal(m, from_host ? m->st_audio.p : b.audio, b.rel.data() + f0, f1 - f0, u, base,
+                                  h_frame_off + f0, st);
+      if (rc) return rc;
+      for (int i = f0; i <= f1; ++i) h_frame_off[i] += base;
+      if (gatherer && k >= 1) {  // buffer (k - 1) % 3 = (k + 2) % 3 is free once the upload of sub-batch k - 1 has left the host
+        const auto tw = now();
+        CK(cudaEventSynchronize(m->copy_ev[k - 1]));
+        t_wait += ms_since(tw);
+        gatherer->release_upto(std::min(k + 3, n_sub));
+      }
+      const int64_t nf = h_frame_off[f1] - base;
+      if (nf > 0) {  // this sub-batch's posteriorgrams: internal -> row-major
+        launch_pm_to_rows(u.note, u.stride, base, nf, kPitches, d.note + base * kPitches, st);
+        launch_pm_to_rows(u.onset, u.stride, base, nf, kPitches, d.onset + base * kPitches, st);
+        launch_cm_to_rows(u.contour, u.stride, base, nf, d.contour + base * kContourBins, st);
+        m->launches += 3;
+        CKL();
+        if (to_host) CK(cudaEventRecord(m->conv_ev[k], st));
+      }
+    }
+    if (to_host && k >= 1) {
+      const int64_t f0 = h_frame_off[cut[k - 1]], nf = h_frame_off[cut[k]] - f0;
+      if (nf > 0) {
+        CK(cudaStreamWaitEvent(m->d2h_stream, m->conv_ev[k - 1], 0));
+        if (host.note)
+          CK(cudaMemcpyAsync(host.note + f0 * kPitches, d.note + f0 * kPitches, sizeof(float) * nf * kPitches,
+                             cudaMemcpyDeviceToHost, m->d2h_stream));
+        if (host.onset)
+          CK(cudaMemcpyAsync(host.onset + f0 * kPitches, d.onset + f0 * kPitches, sizeof(float) * nf * kPitches,
+                             cudaMemcpyDeviceToHost, m->d2h_stream));
+        if (host.contour)
+          CK(cudaMemcpyAsync(host.contour + f0 * kContourBins, d.contour + f0 * kContourBins,
+                             sizeof(float) * nf * kContourBins, cudaMemcpyDeviceToHost, m->d2h_stream));
+      }
+    }
+    t_launch += ms_since(t0);
+  }
+  const auto t_dec = now();
+  rc = params ? bp_decode_device(m, d.note, d.onset, d.contour, h_frame_off, n_files, params, notes, st) : BP_OK;
+  if (!from_host) return rc;
+  const double ms_dec = ms_since(t_dec);
+  const auto t_d2h = now();
+  const cudaError_t e1 = to_host ? cudaStreamSynchronize(m->d2h_stream) : cudaSuccess;
+  if (timing)
+    fprintf(stderr, "%s: %d files, %d sub-batches, %d gather threads: gather %.1f ms, staging waits %.1f ms, enqueue %.1f ms, "
+            "decode (incl. waiting for the forward pass) %.1f ms, tail of the posteriorgram copies %.1f ms, total %.1f ms\n",
+            b.api, n_files, n_sub, n_threads, t_gather, t_wait, t_launch, ms_dec, ms_since(t_d2h), ms_since(t_call));
+  if (rc) return rc;
+  CK(e1);
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
@@ -827,49 +1069,26 @@ int bp_run_inference_device(bp_model_t* m, const float* d_audio, const int64_t* 
   if (!m || !h_sample_off || !h_frame_off || n_files < 0)
     return fail(BP_E_INVALID, "bp_run_inference_device: bad argument");
   DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int64_t total_frames = 0;
-  for (int i = 0; i < n_files; ++i) total_frames += bp_num_frames(h_sample_off[i + 1] - h_sample_off[i]);
-  if (total_frames > 0 && (!d_audio || !d_note || !d_onset || !d_contour))
+  Batch b{"bp_run_inference_device", d_audio, true, nullptr};
+  int rc = describe_batch(b, h_sample_off, nullptr, n_files);
+  if (rc) return rc;
+  if (b.total_frames > 0 && (!d_note || !d_onset || !d_contour))
     return fail(BP_E_INVALID, "bp_run_inference_device: null buffer");
   if (!aligned16(d_contour)) return fail(BP_E_INVALID, "bp_run_inference_device: d_contour must be 16-byte aligned");
-  PostI u;
-  int rc = reserve_internal(m, total_frames, &u);
-  if (rc) return rc;
-  rc = run_inference_internal(m, d_audio, h_sample_off, n_files, u, 0, h_frame_off, st);
-  if (rc) return rc;
-  internal_to_rows(m, u, total_frames, d_note, d_onset, d_contour, st);
-  CKL();
-  return BP_OK;
+  const Rows rows{d_note, d_onset, d_contour};
+  return run_batch(m, b, &rows, Rows{}, nullptr, nullptr, h_frame_off, static_cast<cudaStream_t>(stream));
 }
 
 int bp_run_inference_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
                           float* h_note, float* h_onset, float* h_contour, int64_t* h_frame_off) {
   if (!m || !h_sample_off || !h_frame_off || n_files < 0) return fail(BP_E_INVALID, "bp_run_inference_host: bad argument");
   DeviceGuard g(m->device);
-  const int64_t n_samples = h_sample_off[n_files] - h_sample_off[0];
-  int64_t total_frames = 0;
-  for (int i = 0; i < n_files; ++i) total_frames += bp_num_frames(h_sample_off[i + 1] - h_sample_off[i]);
-  cudaStream_t st = m->stream;
-  CK(m->st_audio.reserve((size_t)std::max<int64_t>(n_samples, 1)));
-  CK(m->st_note.reserve((size_t)total_frames * kPitches + 1));
-  CK(m->st_onset.reserve((size_t)total_frames * kPitches + 1));
-  CK(m->st_contour.reserve((size_t)total_frames * kContourBins + 1));
-  if (n_samples > 0)
-    CK(cudaMemcpyAsync(m->st_audio.p, h_audio + h_sample_off[0], sizeof(float) * n_samples, cudaMemcpyHostToDevice, st));
-  std::vector<int64_t> rel(n_files + 1);
-  for (int i = 0; i <= n_files; ++i) rel[i] = h_sample_off[i] - h_sample_off[0];
-  int rc = bp_run_inference_device(m, m->st_audio.p, rel.data(), n_files, m->st_note.p, m->st_onset.p, m->st_contour.p,
-                                   h_frame_off, st);
+  Batch b{"bp_run_inference_host", h_audio, false, nullptr};
+  int rc = describe_batch(b, h_sample_off, nullptr, n_files);
   if (rc) return rc;
-  if (total_frames > 0) {
-    if (!h_note || !h_onset || !h_contour) return fail(BP_E_INVALID, "bp_run_inference_host: null output");
-    CK(cudaMemcpyAsync(h_note, m->st_note.p, sizeof(float) * total_frames * kPitches, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_onset, m->st_onset.p, sizeof(float) * total_frames * kPitches, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_contour, m->st_contour.p, sizeof(float) * total_frames * kContourBins, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  return BP_OK;
+  if (b.total_frames > 0 && (!h_note || !h_onset || !h_contour))
+    return fail(BP_E_INVALID, "bp_run_inference_host: null output");
+  return run_batch(m, b, nullptr, Rows{h_note, h_onset, h_contour}, nullptr, nullptr, h_frame_off, m->stream);
 }
 
 int bp_decode_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
@@ -1019,8 +1238,8 @@ int bp_infer_onsets_host(bp_model_t* m, const float* h_onset, const float* h_not
   DeviceGuard g(m->device);
   cudaStream_t st = m->stream;
   const size_t cells = (size_t)n_frames * kPitches;
-  CK(m->st_note.reserve(cells + 1));
-  CK(m->st_onset.reserve(cells + 1));
+  const int rc = reserve_rows(m, n_frames);
+  if (rc) return rc;
   CK(m->energy.reserve(cells + 1));
   CK(m->candbits.reserve(cells / 32 + 2));
   CK(m->max_onset.reserve(1));
@@ -1066,8 +1285,8 @@ int bp_pitch_bends_host(bp_model_t* m, const float* h_contour, int64_t n_frames,
   if (!h_bends) return fail(BP_E_INVALID, "bp_pitch_bends_host: bends array missing");
   DeviceGuard g(m->device);
   cudaStream_t st = m->stream;
-  CK(m->st_contour.reserve((size_t)n_frames * kContourBins + 1));
-  CK(m->st_note.reserve((size_t)n_frames * kPitches + 1));  // the kernel also averages the note posteriorgram: zeros here
+  const int rc = reserve_rows(m, n_frames);  // the kernel also averages the note posteriorgram: zeros in st_note
+  if (rc) return rc;
   CK(m->d_start.reserve(n_notes));
   CK(m->d_end.reserve(n_notes));
   CK(m->d_pitch.reserve(n_notes));
@@ -1113,9 +1332,8 @@ int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, con
   DeviceGuard g(m->device);
   const int64_t total = h_frame_off[n_files];
   cudaStream_t st = m->stream;
-  CK(m->st_note.reserve((size_t)total * kPitches + 1));
-  CK(m->st_onset.reserve((size_t)total * kPitches + 1));
-  CK(m->st_contour.reserve((size_t)total * kContourBins + 1));
+  const int rc = reserve_rows(m, total);
+  if (rc) return rc;
   if (total > 0) {
     if (!h_note || !h_onset || !h_contour) return fail(BP_E_INVALID, "bp_decode_host: null posteriorgram");
     CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
@@ -1131,20 +1349,10 @@ int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_s
   int rc = validate_params(params);
   if (rc) return rc;
   DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int64_t total_frames = 0;
-  for (int i = 0; i < n_files; ++i) total_frames += bp_num_frames(h_sample_off[i + 1] - h_sample_off[i]);
-  CK(m->st_note.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_onset.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_contour.reserve((size_t)total_frames * kContourBins + 4));
-  PostI u;
-  rc = reserve_internal(m, total_frames, &u);
+  Batch b{"bp_transcribe_device", d_audio, true, nullptr};
+  rc = describe_batch(b, h_sample_off, nullptr, n_files);
   if (rc) return rc;
-  rc = run_inference_internal(m, d_audio, h_sample_off, n_files, u, 0, h_frame_off, st);
-  if (rc) return rc;
-  internal_to_rows(m, u, total_frames, m->st_note.p, m->st_onset.p, m->st_contour.p, st);
-  CKL();
-  return bp_decode_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, notes, stream);
+  return run_batch(m, b, nullptr, Rows{}, params, notes, h_frame_off, static_cast<cudaStream_t>(stream));
 }
 
 int bp_transcribe_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
@@ -1154,81 +1362,10 @@ int bp_transcribe_host(bp_model_t* m, const float* h_audio, const int64_t* h_sam
   int rc = validate_params(params);
   if (rc) return rc;
   DeviceGuard g(m->device);
-  const int64_t n_samples = h_sample_off[n_files] - h_sample_off[0];
-  cudaStream_t st = m->stream;
-  CK(m->st_audio.reserve((size_t)std::max<int64_t>(n_samples, 1)));
-  if (n_samples > 0 && !h_audio) return fail(BP_E_INVALID, "bp_transcribe_host: null audio");
-  std::vector<int64_t> rel(n_files + 1);
-  int64_t total_frames = 0;
-  for (int i = 0; i <= n_files; ++i) rel[i] = h_sample_off[i] - h_sample_off[0];
-  for (int i = 0; i < n_files; ++i) {
-    if (rel[i + 1] < rel[i]) return fail(BP_E_INVALID, "bp_transcribe_host: sample offsets must be non-decreasing");
-    total_frames += bp_num_frames(rel[i + 1] - rel[i]);
-  }
-  CK(m->st_note.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_onset.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_contour.reserve((size_t)total_frames * kContourBins + 4));
-  PostI u;
-  rc = reserve_internal(m, total_frames, &u);
+  Batch b{"bp_transcribe_host", h_audio, false, nullptr};
+  rc = describe_batch(b, h_sample_off, nullptr, n_files);
   if (rc) return rc;
-
-  // Sub-batches of files (about 4 internal chunks of windows each): all host->device copies are queued on the copy
-  // stream up front, the compute stream waits for sub-batch k only, so the PCIe transfer of k+1.. overlaps the kernels.
-  std::vector<int> cut{0};
-  {
-    // Sub-batches end on file boundaries and do not spill a few windows into an extra internal chunk: the first two
-    // hold at most one chunk of windows (their copies are the ones that cannot be hidden), the next two at most two,
-    // the rest at most four.
-    int64_t w = 0;
-    for (int i = 0; i < n_files; ++i) {
-      const size_t k = cut.size() - 1;
-      const int64_t limit = (k < 2 ? 1 : (k < 4 ? 2 : 4)) * (int64_t)m->chunk;
-      const int64_t nw = bp_num_windows(rel[i + 1] - rel[i]);
-      if (w > 0 && w + nw > limit) {
-        cut.push_back(i);
-        w = 0;
-      }
-      w += nw;
-    }
-    cut.push_back(n_files);
-  }
-  const size_t n_sub = cut.size() - 1;
-  while (m->copy_ev.size() < n_sub) {
-    cudaEvent_t e;
-    CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    m->copy_ev.push_back(e);
-  }
-  CK(cudaStreamSynchronize(st));  // st_audio may still be read by earlier work on the compute stream
-  for (size_t k = 0; k < n_sub; ++k) {
-    const int64_t s0 = rel[cut[k]], s1 = rel[cut[k + 1]];
-    if (s1 > s0)
-      CK(cudaMemcpyAsync(m->st_audio.p + s0, h_audio + h_sample_off[0] + s0, sizeof(float) * (s1 - s0),
-                         cudaMemcpyHostToDevice, m->copy_stream));
-    CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
-  }
-  h_frame_off[0] = 0;
-  std::vector<int64_t> sub_off;
-  for (size_t k = 0; k < n_sub; ++k) {
-    const int f0 = cut[k], f1 = cut[k + 1];
-    CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
-    sub_off.assign(f1 - f0 + 1, 0);
-    const int64_t base = h_frame_off[f0];
-    rc = run_inference_internal(m, m->st_audio.p, rel.data() + f0, f1 - f0, u, base, sub_off.data(), st);
-    if (rc) return rc;
-    for (int i = f0; i < f1; ++i) h_frame_off[i + 1] = base + sub_off[i - f0 + 1];
-  }
-  internal_to_rows(m, u, total_frames, m->st_note.p, m->st_onset.p, m->st_contour.p, st);
-  CKL();
-  rc = bp_decode_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, notes, st);
-  if (rc) return rc;
-  if (total_frames > 0) {
-    if (h_note) CK(cudaMemcpyAsync(h_note, m->st_note.p, sizeof(float) * total_frames * kPitches, cudaMemcpyDeviceToHost, st));
-    if (h_onset) CK(cudaMemcpyAsync(h_onset, m->st_onset.p, sizeof(float) * total_frames * kPitches, cudaMemcpyDeviceToHost, st));
-    if (h_contour)
-      CK(cudaMemcpyAsync(h_contour, m->st_contour.p, sizeof(float) * total_frames * kContourBins, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  return BP_OK;
+  return run_batch(m, b, nullptr, Rows{h_note, h_onset, h_contour}, params, notes, h_frame_off, m->stream);
 }
 
 void bp_last_required(int64_t* notes, int64_t* bends) {
@@ -1250,61 +1387,6 @@ void bp_host_free(void* p) {
   if (p) cudaFreeHost(p);
 }
 
-namespace {
-// Host threads that copy the files of one sub-batch after the other into pinned staging buffers, running ahead of the
-// caller: worker t copies its share of sub-batch k as soon as the caller has released that buffer (`released` counts the
-// sub-batches whose buffer may be overwritten) and reports it in done[k].  The threads live for one call.
-struct Gatherer {
-  const float* const* audio;
-  const int64_t* rel;        // [n_files + 1] sample offsets
-  const int* cut;            // [n_sub + 1] file index where each sub-batch starts
-  int n_sub, n_threads;
-  float* const* stage;       // 3 staging buffers
-  std::atomic<int> released{0};
-  std::vector<std::atomic<int>> done;
-  std::vector<std::thread> threads;
-  std::atomic<bool> abort{false};
-
-  Gatherer(const float* const* a, const int64_t* r, const int* c, int ns, int nt, float* const* st)
-      : audio(a), rel(r), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
-    for (auto& d : done) d.store(0);
-    for (int t = 0; t < n_threads; ++t) threads.emplace_back([this, t] { run(t); });
-  }
-  ~Gatherer() {
-    abort.store(true);
-    for (auto& x : threads) x.join();
-  }
-  void run(int t) {
-    for (int k = 0; k < n_sub; ++k) {
-      for (int spins = 0; released.load(std::memory_order_acquire) <= k; ++spins) {  // buffer k % 3 still holds k - 3
-        if (abort.load()) return;
-        if (spins < 64)
-          std::this_thread::yield();
-        else
-          std::this_thread::sleep_for(std::chrono::microseconds(50));  // do not fight the enqueueing thread for cores
-      }
-      const int f0 = cut[k], f1 = cut[k + 1];
-      const int64_t base = rel[f0], total = rel[f1] - base;
-      float* dst = stage[k % 3];
-      // thread t copies samples [lo, hi) of the sub-batch: whole files where possible, split files otherwise
-      const int64_t lo = base + total * t / n_threads, hi = base + total * (t + 1) / n_threads;
-      if (hi > lo) {
-        int i = (int)(std::upper_bound(rel + f0, rel + f1 + 1, lo) - rel) - 1;
-        for (; i < f1 && rel[i] < hi; ++i) {
-          const int64_t a = std::max(lo, rel[i]), b = std::min(hi, rel[i + 1]);
-          if (b > a) std::memcpy(dst + (a - base), audio[i] + (a - rel[i]), sizeof(float) * (size_t)(b - a));
-        }
-      }
-      done[k].fetch_add(1, std::memory_order_release);
-    }
-  }
-  void release_upto(int k) { released.store(k, std::memory_order_release); }  // sub-batches < k may be gathered
-  void wait(int k) {
-    while (done[k].load(std::memory_order_acquire) < n_threads) std::this_thread::yield();
-  }
-};
-}  // namespace
-
 int bp_transcribe_files_host(bp_model_t* m, const float* const* audio, const int64_t* n_samples, int32_t n_files,
                              const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
                              int64_t* h_frame_off, bp_notes_t* notes) {
@@ -1313,132 +1395,10 @@ int bp_transcribe_files_host(bp_model_t* m, const float* const* audio, const int
   int rc = validate_params(params);
   if (rc) return rc;
   DeviceGuard g(m->device);
-  cudaStream_t st = m->stream;
-  std::vector<int64_t> rel(n_files + 1, 0);
-  int64_t total_frames = 0;
-  for (int i = 0; i < n_files; ++i) {
-    if (n_samples[i] < 0 || (n_samples[i] > 0 && !audio[i]))
-      return fail(BP_E_INVALID, "bp_transcribe_files_host: file " + std::to_string(i) + ": null audio or negative length");
-    rel[i + 1] = rel[i] + n_samples[i];
-    total_frames += bp_num_frames(n_samples[i]);
-  }
-  const int64_t total_samples = rel[n_files];
-  CK(m->st_audio.reserve((size_t)std::max<int64_t>(total_samples, 1)));
-  CK(m->st_note.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_onset.reserve((size_t)total_frames * kPitches + 4));
-  CK(m->st_contour.reserve((size_t)total_frames * kContourBins + 4));
-  PostI u;
-  rc = reserve_internal(m, total_frames, &u);
+  Batch b{"bp_transcribe_files_host", nullptr, false, audio};
+  rc = describe_batch(b, nullptr, n_samples, n_files);
   if (rc) return rc;
-  // sub-batches of whole files, about two internal chunks of windows each (the first ones one chunk, so that the
-  // kernels start early)
-  std::vector<int> cut{0};
-  {
-    int64_t w = 0;
-    for (int i = 0; i < n_files; ++i) {
-      const size_t k = cut.size() - 1;
-      const int64_t limit = (k < 2 ? 1 : 2) * (int64_t)m->chunk;
-      const int64_t nw = bp_num_windows(n_samples[i]);
-      if (w > 0 && w + nw > limit) {
-        cut.push_back(i);
-        w = 0;
-      }
-      w += nw;
-    }
-    cut.push_back(n_files);
-  }
-  const size_t n_sub = cut.size() - 1;
-  size_t max_sub = 1;
-  for (size_t k = 0; k < n_sub; ++k) max_sub = std::max<size_t>(max_sub, (size_t)(rel[cut[k + 1]] - rel[cut[k]]));
-  if (max_sub > m->gather_cap) {
-    for (float*& b : m->gather) {
-      if (b) cudaFreeHost(b);
-      b = nullptr;
-    }
-    m->gather_cap = 0;
-    const size_t want = max_sub + max_sub / 8;
-    for (float*& b : m->gather) CK(cudaHostAlloc(&b, want * sizeof(float), cudaHostAllocDefault));
-    m->gather_cap = want;
-  }
-  if (!m->d2h_stream) CK(cudaStreamCreateWithFlags(&m->d2h_stream, cudaStreamNonBlocking));
-  while (m->copy_ev.size() < n_sub || m->conv_ev.size() < n_sub) {
-    cudaEvent_t e;
-    CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    (m->copy_ev.size() < n_sub ? m->copy_ev : m->conv_ev).push_back(e);
-  }
-  int n_threads = (int)std::max(1u, std::min(16u, std::thread::hardware_concurrency() > 2 ? std::thread::hardware_concurrency() - 1 : 1u));
-  if (const char* e = getenv("BP_B200_GATHER_THREADS")) n_threads = std::max(1, std::min(64, atoi(e)));
-  const bool timing = getenv("BP_B200_TIMING") != nullptr;  // host-side breakdown of this call on stderr
-  auto now = [] { return std::chrono::steady_clock::now(); };
-  auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(now() - t).count(); };
-  const auto t_call = now();
-  double t_gather = 0, t_wait = 0, t_launch = 0;
-  CK(cudaStreamSynchronize(st));  // st_audio / st_note.. may still be in use by earlier work on the compute stream
-  h_frame_off[0] = 0;
-  std::vector<int64_t> sub_off;
-  Gatherer gatherer(audio, rel.data(), cut.data(), (int)n_sub, n_threads, m->gather);
-  gatherer.release_upto(std::min<int>(3, (int)n_sub));  // the three buffers are free: the workers start at once
-  for (size_t k = 0; k < n_sub; ++k) {
-    const int f0 = cut[k], f1 = cut[k + 1];
-    const int64_t s0 = rel[f0], s1 = rel[f1];
-    float* stage = m->gather[k % 3];
-    auto t0 = now();
-    gatherer.wait((int)k);  // sub-batch k is in its staging buffer (gathered while earlier sub-batches were enqueued)
-    t_gather += ms_since(t0);
-    t0 = now();
-    if (s1 > s0)
-      CK(cudaMemcpyAsync(m->st_audio.p + s0, stage, sizeof(float) * (size_t)(s1 - s0), cudaMemcpyHostToDevice, m->copy_stream));
-    CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
-    CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
-    sub_off.assign(f1 - f0 + 1, 0);
-    const int64_t base = h_frame_off[f0];
-    rc = run_inference_internal(m, m->st_audio.p, rel.data() + f0, f1 - f0, u, base, sub_off.data(), st);
-    if (rc) return rc;
-    if (k >= 1) {  // buffer (k - 1) % 3 = (k + 2) % 3 is free once the upload of sub-batch k - 1 has left the host
-      auto tw = now();
-      CK(cudaEventSynchronize(m->copy_ev[k - 1]));
-      t_wait += ms_since(tw);
-      gatherer.release_upto((int)std::min<size_t>(k + 3, n_sub));
-    }
-    for (int i = f0; i < f1; ++i) h_frame_off[i + 1] = base + sub_off[i - f0 + 1];
-    // this sub-batch's posteriorgrams: internal -> row-major, then to the host on their own stream while the next
-    // sub-batches compute
-    const int64_t nf = h_frame_off[f1] - base;
-    if (nf > 0) {
-      launch_pm_to_rows(u.note, u.stride, base, nf, kPitches, m->st_note.p + base * kPitches, st);
-      launch_pm_to_rows(u.onset, u.stride, base, nf, kPitches, m->st_onset.p + base * kPitches, st);
-      launch_cm_to_rows(u.contour, u.stride, base, nf, m->st_contour.p + base * kContourBins, st);
-      m->launches += 3;
-      CKL();
-      CK(cudaEventRecord(m->conv_ev[k], st));
-      if (h_note || h_onset || h_contour) {
-        CK(cudaStreamWaitEvent(m->d2h_stream, m->conv_ev[k], 0));
-        if (h_note)
-          CK(cudaMemcpyAsync(h_note + base * kPitches, m->st_note.p + base * kPitches, sizeof(float) * nf * kPitches,
-                             cudaMemcpyDeviceToHost, m->d2h_stream));
-        if (h_onset)
-          CK(cudaMemcpyAsync(h_onset + base * kPitches, m->st_onset.p + base * kPitches, sizeof(float) * nf * kPitches,
-                             cudaMemcpyDeviceToHost, m->d2h_stream));
-        if (h_contour)
-          CK(cudaMemcpyAsync(h_contour + base * kContourBins, m->st_contour.p + base * kContourBins,
-                             sizeof(float) * nf * kContourBins, cudaMemcpyDeviceToHost, m->d2h_stream));
-      }
-    }
-    t_launch += ms_since(t0);
-  }
-  const auto t_dec = now();
-  rc = bp_decode_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, notes, st);
-  const double ms_dec = ms_since(t_dec);
-  const auto t_d2h = now();
-  cudaError_t e1 = cudaStreamSynchronize(m->d2h_stream);
-  if (timing)
-    fprintf(stderr, "bp_transcribe_files_host: %d files, %zu sub-batches, %d gather threads: gather %.1f ms, staging waits %.1f ms, "
-            "enqueue %.1f ms, decode (incl. waiting for the forward pass) %.1f ms, tail of the posteriorgram copies %.1f ms, total %.1f ms\n",
-            n_files, n_sub, n_threads, t_gather, t_wait, t_launch, ms_dec, ms_since(t_d2h), ms_since(t_call));
-  if (rc) return rc;
-  CK(e1);
-  CK(cudaStreamSynchronize(st));
-  return BP_OK;
+  return run_batch(m, b, nullptr, Rows{h_note, h_onset, h_contour}, params, notes, h_frame_off, m->stream);
 }
 
 int64_t bp_resampled_length(int64_t n_frames, int32_t sample_rate) { return ingest_output_length(n_frames, sample_rate); }

@@ -118,7 +118,10 @@ int bp_forward_host(bp_model_t* m, const float* h_audio, int64_t n_windows, floa
  * audio: the files' samples back to back; sample_off[n_files+1] gives each file's range.
  * Outputs: unwrapped posteriorgrams of all files back to back; file i has
  * bp_num_frames(len_i) frames starting at frame_off[i] (frame_off[n_files+1] is written by the
- * call; host array in both variants).  Output arrays must hold sum_i bp_num_frames(len_i) frames. */
+ * call; host array in both variants).  Output arrays must hold sum_i bp_num_frames(len_i) frames.
+ * _host, like every host entry point for a batch of files, runs it in sub-batches of whole files: the upload of each
+ * overlaps the kernels of the one before, and its posteriorgrams come back while later ones compute (page-locked
+ * outputs from bp_host_alloc make that copy asynchronous). */
 int bp_run_inference_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,
                             float* d_note, float* d_onset, float* d_contour, int64_t* h_frame_off, void* stream);
 int bp_run_inference_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
@@ -140,7 +143,8 @@ int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, con
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
- * them on the device only).  `h_frame_off` [n_files+1] is always written. */
+ * them on the device only).  `h_frame_off` [n_files+1] is always written.  bp_transcribe_host uploads the audio and
+ * returns the posteriorgrams sub-batch by sub-batch, overlapped with the kernels, like bp_run_inference_host. */
 int bp_transcribe_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
                        const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
                        int64_t* h_frame_off, bp_notes_t* notes);
@@ -177,10 +181,10 @@ int bp_model_set_path(bp_model_t* m, int path);
 /* `bp_transcribe_host` for audio that is NOT packed: file i is audio[i][0 .. n_samples[i]) in ordinary (pageable) host
  * memory — what a caller holding one array per file has (reference: basic_pitch/inference.py:509-604, `predict_and_save`
  * loops `predict` over `audio_path_list`).  The library gathers the files sub-batch by sub-batch into pinned staging with
- * a few host threads, so that the gather and upload of sub-batch k+1 overlap the kernels of k, and streams the
- * posteriorgrams of each finished sub-batch back (h_note / h_onset / h_contour, row-major [total_frames][88 | 88 | 264],
- * any may be NULL) while later sub-batches compute; buffers from bp_host_alloc make that copy asynchronous.
- * Everything else (h_frame_off, notes, errors) as bp_transcribe_host. */
+ * a few host threads, so that the gather and upload of sub-batch k+1 overlap the kernels of k; sub-batches are at most
+ * two chunks of windows (four for packed input), which bounds that staging.  Everything else (the posteriorgrams
+ * h_note / h_onset / h_contour, row-major [total_frames][88 | 88 | 264], any may be NULL, coming back per sub-batch;
+ * h_frame_off, notes, errors) as bp_transcribe_host. */
 int bp_transcribe_files_host(bp_model_t* m, const float* const* audio, const int64_t* n_samples, int32_t n_files,
                              const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
                              int64_t* h_frame_off, bp_notes_t* notes);

@@ -311,38 +311,97 @@ def test_transcribe_batch_equals_per_file(model):
 
 
 def test_transcribe_host_sub_batches_equal_device_path(model):
-    """bp_transcribe_host splits a large batch into sub-batches on file boundaries (copies overlap the kernels) and runs
-    partial internal chunks; its note events must equal those of one bp_transcribe_device call on the same audio, and the
-    ragged file lengths exercise windows that cross sub-batch / chunk boundaries."""
+    """The host entry points split a batch into sub-batches on file boundaries (1, 1, 2, 2 chunks of windows, then 4 for
+    packed and 2 for per-file input; uploads and posteriorgram copies overlap the kernels) and run partial internal
+    chunks; the device entry points run it in one.  On a batch of more than 8 chunks of windows with ragged lengths and
+    an empty file, the posteriorgrams of bp_run_inference_host, bp_transcribe_host and bp_transcribe_files_host must be
+    the bits of bp_run_inference_device's, and the note events and frame offsets of the host transcribe calls those of
+    one bp_transcribe_device call."""
+    import ctypes as C
+
     import torch
 
     from basic_pitch_b200 import engine, synth
 
-    chunk = int(model._lib.bp_model_chunk_windows(model.handle))
-    base = [synth.random_notes_clip(4.0 + 0.7 * (i % 5), seed=100 + i) for i in range(10)]
-    clips = [base[i % len(base)] for i in range(160)]  # ~ 3 windows each -> several sub-batches of 1, 1, 2 chunks
-    n_windows = sum(int(model._lib.bp_num_windows(len(c))) for c in clips)
-    assert n_windows > 2 * chunk
+    lib = model._lib
+    chunk = int(lib.bp_model_chunk_windows(model.handle))
+    base = [synth.random_notes_clip(0.3 + 0.8 * i, seed=100 + i) for i in range(12)]  # 1 .. 6 windows
+    keys = [i % len(base) for i in range(480)]
+    keys.insert(200, None)
+    clips = [np.zeros(0, np.float32) if k is None else base[k] for k in keys]
+    n = len(clips)
+    n_windows = sum(int(lib.bp_num_windows(len(c))) for c in clips)
+    assert n_windows > 8 * chunk
+    n_frames = sum(int(lib.bp_num_frames(len(c))) for c in clips)
+    flat, offs = model._pack_audio(clips)  # pageable, like run_inference_arrays'
+    p = engine.default_params(model)
+
+    def note_buffers():
+        return engine.NoteBuffers(n, max(4096, 2 * n_frames), max(65536, 24 * n_frames))
+
+    def posteriorgrams():  # NaN wherever a copy is missing
+        return [np.full((n_frames, w), np.nan, np.float32) for w in (88, 88, 264)]
+
+    def ptrs(arrays):
+        return [a.ctypes.data for a in arrays]
+
+    # reference: one device call
     packed = engine.PackedAudio(clips, pinned=True)
-    n_frames = sum(int(model._lib.bp_num_frames(len(c))) for c in clips)
-    out_h = engine.NoteBuffers(len(clips), max(4096, 2 * n_frames), max(65536, 24 * n_frames))
-    out_d = engine.NoteBuffers(len(clips), max(4096, 2 * n_frames), max(65536, 24 * n_frames))
-    nh = engine.transcribe_packed_host(model, packed, out_h)
     d_audio = packed.to_device(model.device)
+    d_post = [torch.empty((n_frames, w), dtype=torch.float32, device=d_audio.device) for w in (88, 88, 264)]
+    foff_d = np.zeros(n + 1, np.int64)
+    st = torch.cuda.current_stream(d_audio.device).cuda_stream
+    lib.bp_run_inference_device(model.handle, d_audio.data_ptr(), packed.offsets.ctypes.data, n,
+                                *[t.data_ptr() for t in d_post], foff_d.ctypes.data, st)
+    out_d = note_buffers()
     nd = engine.transcribe_packed_device(model, d_audio, packed.offsets, out_d)
     torch.cuda.synchronize()
-    assert nh == nd > 200
-    for k in ("note_off", "frame_off"):
-        np.testing.assert_array_equal(out_h.a[k][: len(clips) + 1], out_d.a[k][: len(clips) + 1], err_msg=k)
-    for k in ("start", "end", "pitch", "amp"):
-        np.testing.assert_array_equal(out_h.a[k][:nh], out_d.a[k][:nh], err_msg=k)
-    nb = int(out_h.a["bend_off"][nh])
-    np.testing.assert_array_equal(out_h.a["bend_off"][: nh + 1], out_d.a["bend_off"][: nh + 1])
-    np.testing.assert_array_equal(out_h.a["bends"][:nb], out_d.a["bends"][:nb])
+    ref = [t.cpu().numpy() for t in d_post]
+    del d_post
+    np.testing.assert_array_equal(foff_d, np.cumsum([0] + [int(lib.bp_num_frames(len(c))) for c in clips]))
+    assert nd > 200
+
+    def check_posteriorgrams(got, foff, name):
+        np.testing.assert_array_equal(foff, foff_d, err_msg=f"{name} frame_off")
+        for k, g, r in zip(("note", "onset", "contour"), got, ref):
+            np.testing.assert_array_equal(g, r, err_msg=f"{name} {k}")
+
+    def check_notes(out, name):
+        for k in ("note_off", "frame_off"):
+            np.testing.assert_array_equal(out.a[k][: n + 1], out_d.a[k][: n + 1], err_msg=f"{name} {k}")
+        for k in ("start", "end", "pitch", "amp"):
+            np.testing.assert_array_equal(out.a[k][:nd], out_d.a[k][:nd], err_msg=f"{name} {k}")
+        nb = int(out_d.a["bend_off"][nd])
+        np.testing.assert_array_equal(out.a["bend_off"][: nd + 1], out_d.a["bend_off"][: nd + 1], err_msg=name)
+        np.testing.assert_array_equal(out.a["bends"][:nb], out_d.a["bends"][:nb], err_msg=name)
+
+    post, foff = posteriorgrams(), np.zeros(n + 1, np.int64)
+    lib.bp_run_inference_host(model.handle, flat.ctypes.data, offs.ctypes.data, n, *ptrs(post), foff.ctypes.data)
+    check_posteriorgrams(post, foff, "bp_run_inference_host")
+
+    out, post = note_buffers(), posteriorgrams()
+    lib.bp_transcribe_host(model.handle, flat.ctypes.data, offs.ctypes.data, n, C.byref(p), *ptrs(post),
+                           out.a["frame_off"].ctypes.data, C.byref(out.notes))
+    check_posteriorgrams(post, out.a["frame_off"][: n + 1], "bp_transcribe_host")
+    check_notes(out, "bp_transcribe_host")
+
+    out, post = note_buffers(), posteriorgrams()
+    files = (C.c_void_p * n)(*[c.ctypes.data for c in clips])
+    lens = np.array([len(c) for c in clips], np.int64)
+    lib.bp_transcribe_files_host(model.handle, files, lens.ctypes.data, n, C.byref(p), *ptrs(post),
+                                 out.a["frame_off"].ctypes.data, C.byref(out.notes))
+    check_posteriorgrams(post, out.a["frame_off"][: n + 1], "bp_transcribe_files_host")
+    check_notes(out, "bp_transcribe_files_host")
+    del post
+
+    out_h = note_buffers()  # pinned audio, no posteriorgrams back (bench.py's e2e)
+    assert engine.transcribe_packed_host(model, packed, out_h) == nd
+    check_notes(out_h, "bp_transcribe_host (pinned, no posteriorgrams)")
     # identical clips give identical events wherever they sit in the batch
     no = out_h.a["note_off"]
-    for i in range(len(base), len(clips)):
-        j = i % len(base)
+    first = {}
+    for i, k in enumerate(keys):
+        j = first.setdefault(k, i)
         assert no[i + 1] - no[i] == no[j + 1] - no[j]
         np.testing.assert_array_equal(out_h.a["start"][no[i] : no[i + 1]], out_h.a["start"][no[j] : no[j + 1]])
         np.testing.assert_array_equal(out_h.a["amp"][no[i] : no[i + 1]], out_h.a["amp"][no[j] : no[j + 1]])
