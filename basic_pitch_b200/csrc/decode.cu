@@ -468,8 +468,10 @@ __global__ void __launch_bounds__(kSeqThreads) decode_seq_kernel(
             s_pick[0] = tm;
             s_pick[1] = f;
             // zeroed on three columns: [backward exit + 1, forward exit), i.e. within energy_tol of the note's ends
-            s_pick[3] = max(0, min(t_start - p.energy_tol, tm));
-            s_pick[4] = min(T - 1, max(t_end + p.energy_tol, tm));
+            // (64-bit: energy_tol may be up to INT_MAX, and t_end + energy_tol must not wrap below tm)
+            const long long tol = p.energy_tol;
+            s_pick[3] = (int)max(0LL, min((long long)t_start - tol, (long long)tm));
+            s_pick[4] = (int)min((long long)T - 1, max((long long)t_end + tol, (long long)tm));
           }
         }
         if (lane == 0) s_pick[2] = go ? 0 : 1;

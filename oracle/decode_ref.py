@@ -45,13 +45,19 @@ def midi_to_hz(m):
     return 440.0 * (2.0 ** ((np.asanyarray(m) - 69.0) / 12.0))
 
 
-def constrain_frequency(onsets, frames, max_freq: Optional[float], min_freq: Optional[float]):
-    """Zero (IN PLACE, like the reference) pitch columns outside [min_freq, max_freq)."""
+def constrain_frequency(onsets, frames, max_freq: Optional[float], min_freq: Optional[float],
+                        lo_col: Optional[int] = None, hi_col: Optional[int] = None):
+    """Zero (IN PLACE, like the reference) pitch columns outside [min_freq, max_freq).  `lo_col` / `hi_col` give the
+    column range directly (the library's min_pitch_idx / max_pitch_idx) and take precedence over the frequencies."""
     lo, hi = 0, onsets.shape[1]
     if min_freq is not None:
         lo = int(np.round(hz_to_midi(min_freq) - MIDI_OFFSET))
     if max_freq is not None:
         hi = int(np.round(hz_to_midi(max_freq) - MIDI_OFFSET))
+    if lo_col is not None:
+        lo = int(lo_col)
+    if hi_col is not None:
+        hi = int(hi_col)
     for m in (onsets, frames):
         m[:, :lo] = 0
         m[:, hi:] = 0
@@ -95,9 +101,11 @@ def output_to_notes_polyphonic(
     min_freq: Optional[float],
     melodia_trick: bool = True,
     energy_tol: int = 11,
+    lo_col: Optional[int] = None,
+    hi_col: Optional[int] = None,
 ) -> List[Tuple[int, int, int, np.float32]]:
     n_t = frames.shape[0]
-    onsets, frames = constrain_frequency(onsets, frames, max_freq, min_freq)
+    onsets, frames = constrain_frequency(onsets, frames, max_freq, min_freq, lo_col, hi_col)
     if infer_onsets_flag:
         onsets = infer_onsets(onsets, frames)
 
@@ -194,11 +202,15 @@ def model_output_to_note_events(
     max_freq: Optional[float] = None,
     include_pitch_bends: bool = True,
     melodia_trick: bool = True,
+    energy_tol: int = 11,
+    lo_col: Optional[int] = None,
+    hi_col: Optional[int] = None,
 ):
     """Returns (frame-indexed notes with bends, second-indexed note events)."""
     frames, onsets, contours = output["note"], output["onset"], output["contour"]
     notes = output_to_notes_polyphonic(
-        frames, onsets, onset_thresh, frame_thresh, min_note_len, infer_onsets_flag, max_freq, min_freq, melodia_trick
+        frames, onsets, onset_thresh, frame_thresh, min_note_len, infer_onsets_flag, max_freq, min_freq, melodia_trick,
+        energy_tol, lo_col, hi_col,
     )
     if include_pitch_bends:
         with_bends = pitch_bends(contours, notes)

@@ -6,7 +6,8 @@ satisfied by oracle/ref_shims (librosa / pretty_midi / mir_eval / resampy stand-
 `onnxruntime` stand-in whose arithmetic is oracle/model_ref.py), so every line of the reference's
 `inference.py` host logic and `note_creation.py` decode executes as shipped.
 
-    python oracle/make_golden.py            # rewrites tests/golden/*.npz
+    python oracle/make_golden.py                  # rewrites tests/golden/*.npz
+    python oracle/make_golden.py decode_edges     # rewrites tests/golden/decode_edges.npz only (byte-reproducible)
 
 Fixtures written (all small, committed):
   vocadito10_pcm44k.npz the same clip as stored in the reference's test resources (44.1 kHz int16 mono): ingest tests
@@ -16,6 +17,7 @@ Fixtures written (all small, committed):
   decode_cases.npz      posteriorgram inputs (uint16-quantised) + reference decode outputs
   host_cases.npz        window counts / unwrap lengths from the reference's windowing code
   predict_2s.npz        config-1 clip: int16 audio + reference predict() outputs (fake-ORT oracle model)
+  decode_edges.npz      reference decode outputs on the adversarial posteriorgram sets of tests/postsets.py
 """
 import hashlib
 import io
@@ -289,9 +291,107 @@ def main() -> None:
     print(f"config-1 clip: {out['note'].shape[0]} frames, {len(events)} events")
     np.savez_compressed(GOLD / "predict_2s.npz", **store)
 
+    decode_edges()
     for f in sorted(GOLD.glob("*.npz")):
         print(f"{f.name}: {f.stat().st_size} B")
 
 
+def save_npz_reproducible(path: pathlib.Path, store) -> None:
+    """np.savez_compressed with fixed member timestamps: the same arrays give the same bytes on every run."""
+    import zipfile
+
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED) as zf:
+        for key in sorted(store):
+            info = zipfile.ZipInfo(key + ".npy", date_time=(1980, 1, 1, 0, 0, 0))
+            info.compress_type = zipfile.ZIP_DEFLATED
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, np.asanyarray(store[key]), allow_pickle=False)
+            zf.writestr(info, buf.getvalue())
+
+
+def column_range_as_freqs(lo: int, hi: int):
+    """(min_freq, max_freq) that the reference's constrain_frequency turns into pitch columns [lo, hi)."""
+    min_freq = None if lo == 0 else float(librosa_midi_to_hz(21 + lo))
+    max_freq = None if hi == 88 else float(librosa_midi_to_hz(21 + hi))
+    for f, col in ((min_freq, lo), (max_freq, hi)):
+        assert f is None or int(np.round(ref_nc.librosa.hz_to_midi(f) - 21)) == col, (f, col)
+    return min_freq, max_freq
+
+
+def librosa_midi_to_hz(m):
+    return ref_nc.librosa.midi_to_hz(m)
+
+
+def decode_edges() -> None:
+    """tests/golden/decode_edges.npz: the reference decode (`output_to_notes_polyphonic` with `energy_tol`,
+    `get_pitch_bends`, `model_frames_to_time`) on every file and parameter set of tests/postsets.py.  The inputs are
+    regenerated from tests/postsets.py (seeded) and identified by a SHA-256 per file; the outputs are stored per set and
+    parameter set, concatenated over the files of the set (note_off[i] .. note_off[i + 1] are file i's notes), in the
+    narrowest exact dtypes: start / end / pitch frames int16, bends int8 (|bend| <= 25), amplitudes float32.  Every note has end - start
+    bends, so the bend offsets follow from the frames.  Frame times depend on the frame index only: one array for the
+    longest file serves every file.
+
+        python oracle/make_golden.py decode_edges     # this fixture only
+    """
+    from tests import postsets
+
+    store = {}
+    max_t = 0
+    for name in postsets.NAMES:
+        files, grid = postsets.get(name)
+        store[f"{name}/sha"] = np.stack([np.frombuffer(postsets.file_sha(f), np.uint8) for f in files])
+        store[f"{name}/T"] = np.array([f[0].shape[0] for f in files], np.int64)
+        max_t = max([max_t] + [f[0].shape[0] for f in files])
+        for j, p in enumerate(grid):
+            min_freq, max_freq = column_range_as_freqs(p["lo_col"], p["hi_col"])
+            frames, amp, flat, noff = [], [], [], [0]
+            for note, onset, contour in postsets.get(name)[0]:
+                notes = []
+                if note.shape[0] > 0:  # the reference cannot take an empty file (np.max of nothing); it has no notes
+                    with warnings.catch_warnings():
+                        warnings.simplefilter("ignore")
+                        notes = ref_nc.output_to_notes_polyphonic(
+                            note, onset, onset_thresh=p["onset_thresh"], frame_thresh=p["frame_thresh"],
+                            min_note_len=p["min_note_len"], infer_onsets=p["infer_onsets"], max_freq=max_freq,
+                            min_freq=min_freq, melodia_trick=p["melodia_trick"], energy_tol=p["energy_tol"],
+                        )
+                        notes = ref_nc.get_pitch_bends(contour, notes)
+                for a, b, pitch, am, bends in notes:
+                    assert len(bends) == b - a
+                    frames.append((a, b, pitch))
+                    amp.append(am)
+                    flat.extend(int(v) for v in bends)
+                noff.append(len(frames))
+            key = f"{name}/p{j}"
+            store[f"{key}/params"] = np.array(
+                [p["onset_thresh"], p["frame_thresh"], p["min_note_len"], p["energy_tol"], p["infer_onsets"],
+                 p["melodia_trick"], p["lo_col"], p["hi_col"]], np.float64)  # fmt: skip
+            fr = narrow(np.array(frames, np.int64).reshape(-1, 3), np.int16)
+            for c, k in enumerate(("start", "end", "pitch")):  # one array per column: each compresses on its own
+                store[f"{key}/{k}"] = np.ascontiguousarray(fr[:, c])
+            store[f"{key}/amp"] = np.array(amp, np.float32)
+            store[f"{key}/bend_flat"] = narrow(np.array(flat, np.int64), np.int8)
+            store[f"{key}/note_off"] = np.array(noff, np.int32)
+            print(f"  {key}: {np.diff(noff).tolist()} notes")
+    store["times"] = np.asarray(ref_nc.model_frames_to_time(max_t), np.float64)
+    # get_pitch_bends alone on the notes of pitch_edges (bp_pitch_bends_host)
+    contour = postsets.get("pitch_edges")[0][0][2]
+    wb = ref_nc.get_pitch_bends(contour, [(a, b, p, 0.5) for a, b, p in postsets.edge_notes()])
+    store["pitch_edges/direct/bend_flat"] = narrow(np.array([int(v) for e in wb for v in e[4]], np.int64), np.int8)
+    path = GOLD / "decode_edges.npz"
+    save_npz_reproducible(path, store)
+    print(f"{path.name}: {path.stat().st_size} B")
+
+
+def narrow(a: np.ndarray, dtype) -> np.ndarray:
+    """`a` in a narrower integer dtype, which must hold every value exactly."""
+    out = a.astype(dtype)
+    assert np.array_equal(out, a), dtype
+    return out
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["decode_edges"]:
+        decode_edges()
+    else:
+        main()

@@ -55,3 +55,14 @@ def assert_events_equal(got, exp, amp_atol=0.0, ctx=""):
         np.testing.assert_array_equal(got["amp"], exp["amp"], err_msg=f"{ctx}: amplitude")
     else:
         np.testing.assert_allclose(got["amp"], exp["amp"], rtol=0, atol=amp_atol, err_msg=f"{ctx}: amplitude")
+
+
+def edges_case(z, key):
+    """The reference's notes for one set and parameter set of decode_edges.npz (`key` = "<set>/p<j>"), concatenated over
+    the set's files: int32 start / end / pitch, float32 amp, int32 bends, the bend offsets (every note has end - start
+    bends) and the per-file note offsets."""
+    start, end, pitch = (z[f"{key}/{k}"].astype(np.int32) for k in ("start", "end", "pitch"))
+    return {
+        "start": start, "end": end, "pitch": pitch, "amp": z[f"{key}/amp"], "bends": z[f"{key}/bend_flat"].astype(np.int32),
+        "bend_off": np.concatenate([[0], np.cumsum(end - start)]).astype(np.int32), "note_off": z[f"{key}/note_off"],
+    }  # fmt: skip

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 from oracle import decode_ref, host_ref, model_ref
-from tests.golden_util import assert_events_equal, case_expected, case_params, dequant, events_to_arrays
+from tests.golden_util import assert_events_equal, case_expected, case_params, dequant, edges_case, events_to_arrays
 
 
 def test_model_restatement_vs_reference_golden(golden_dir, weights_np):
@@ -98,3 +98,46 @@ def test_host_restatement_vs_reference(golden_dir):
     wins = host_ref.window_audio(ramp)
     assert wins.shape[0] == int(z["ramp_n_windows"])
     assert hashlib.sha256(wins.tobytes()).digest() == z["ramp_windows_sha"].tobytes()
+
+
+def test_decode_restatement_vs_reference_run_edges(golden_dir):
+    """decode_ref (with energy_tol and the lo_col / hi_col column range) against the unmodified reference decode on every
+    file and parameter set of tests/postsets.py (fixture decode_edges.npz; the reference was given the column range as
+    min_freq / max_freq)."""
+    from tests import postsets
+
+    z = np.load(golden_dir / "decode_edges.npz")
+    for name in postsets.NAMES:
+        files, grid = postsets.get(name)
+        for i, f in enumerate(files):
+            assert postsets.file_sha(f) == z[f"{name}/sha"][i].tobytes(), f"{name} file {i}: inputs differ from the fixture"
+        for j, p in enumerate(grid):
+            key = f"{name}/p{j}"
+            stored = z[f"{key}/params"]
+            assert list(stored) == [p[k] for k in ("onset_thresh", "frame_thresh", "min_note_len", "energy_tol", "infer_onsets",
+                                                   "melodia_trick", "lo_col", "hi_col")], key
+            c = edges_case(z, key)
+            noff, boff, amp, flat = c["note_off"], c["bend_off"], c["amp"], c["bends"]
+            fr = np.stack([c["start"], c["end"], c["pitch"]], axis=1)
+            for i, (note, onset, contour) in enumerate(postsets.get(name)[0]):
+                a, b = int(noff[i]), int(noff[i + 1])
+                if note.shape[0] == 0:
+                    assert a == b
+                    continue
+                with np.errstate(all="ignore"):
+                    wb, ev = decode_ref.model_output_to_note_events(
+                        {"note": note, "onset": onset, "contour": contour}, p["onset_thresh"], p["frame_thresh"],
+                        p["infer_onsets"], p["min_note_len"], melodia_trick=p["melodia_trick"], energy_tol=p["energy_tol"],
+                        lo_col=p["lo_col"], hi_col=p["hi_col"])  # fmt: skip
+                ctx = f"{key} file {i}"
+                got = np.array([e[:3] for e in wb], np.int32).reshape(-1, 3)
+                np.testing.assert_array_equal(got, fr[a:b], err_msg=ctx)
+                np.testing.assert_array_equal(np.array([e[3] for e in wb], np.float32).view(np.uint32), amp[a:b].view(np.uint32),
+                                              err_msg=f"{ctx}: amplitude bytes")
+                np.testing.assert_array_equal([int(v) for e in wb for v in e[4]], flat[boff[a] : boff[b]], err_msg=ctx)
+                np.testing.assert_array_equal(np.cumsum([0] + [len(e[4]) for e in wb]), boff[a : b + 1] - boff[a], err_msg=ctx)
+                times = z["times"][: note.shape[0]]  # frame times depend on the frame index only
+                np.testing.assert_array_equal([e[0] for e in ev], times[fr[a:b, 0]], err_msg=f"{ctx}: start times")
+                np.testing.assert_array_equal([e[1] for e in ev], times[fr[a:b, 1]], err_msg=f"{ctx}: end times")
+    wb = decode_ref.pitch_bends(postsets.get("pitch_edges")[0][0][2], [(a, b, p, 0.5) for a, b, p in postsets.edge_notes()])
+    np.testing.assert_array_equal([int(v) for e in wb for v in e[4]], z["pitch_edges/direct/bend_flat"])
