@@ -147,7 +147,7 @@ struct bp_model {
   struct TcLayer {
     TcConvPlan plan;
     TcConvDev dev{};
-    DevBuf<uint16_t> tiles, b2;
+    DevBuf<uint16_t> tiles, b1, b2;  // tiles: contour only; b1: onset / note only
   } tc_contour, tc_onset, tc_note;
   DevBuf<__nv_bfloat16> yhl, chl;
   Lowpass2 lp2{};  // decimation FIR taps, a parameter of every decimation launch
@@ -294,20 +294,29 @@ int derive(bp_model* m, cudaStream_t st) {
                            hp.data() + ParamLayout::note2_b};
   for (int l = 0; l < 3; ++l) {
     bp_model::TcLayer& L = *layers[l];
-    L.plan.build(specs[l], wsrc[l]);
-    const TcConvPlan& pl = L.plan;
-    if (tc_upload_program(l, pl, st) != 0)
-      return fail(BP_E_INVALID, "tensor-core program does not fit its constant-memory area");
-    CK(L.tiles.reserve(pl.tiles.size()));
-    CK(cudaMemcpyAsync(L.tiles.p, pl.tiles.data(), pl.tiles.size() * 2, cudaMemcpyHostToDevice, st));
+    int n_groups = specs[l].G0;
+    if (l == 0) {  // the contour conv: Toeplitz weight tiles + the MMA program
+      L.plan.build(specs[l], wsrc[l]);
+      const TcConvPlan& pl = L.plan;
+      if (tc_upload_program(pl, st) != 0)
+        return fail(BP_E_INVALID, "tensor-core program does not fit its constant-memory area");
+      CK(L.tiles.reserve(pl.tiles.size()));
+      CK(cudaMemcpyAsync(L.tiles.p, pl.tiles.data(), pl.tiles.size() * 2, cudaMemcpyHostToDevice, st));
+      n_groups = pl.n_groups;
+    } else {  // onset / note: the two B matrices of the gathered conv1
+      std::vector<uint16_t> b1;
+      tc_build_b1(l, wsrc[l], b1);
+      CK(L.b1.reserve(b1.size()));
+      CK(cudaMemcpyAsync(L.b1.p, b1.data(), b1.size() * 2, cudaMemcpyHostToDevice, st));
+    }
     CK(cudaStreamSynchronize(st));
     std::vector<uint16_t> b2;
     tc_build_b2_full(l, w2src[l], b2);
     CK(L.b2.reserve(b2.size()));
     CK(cudaMemcpyAsync(L.b2.p, b2.data(), b2.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
-    L.dev = TcConvDev{pl.spec, L.tiles.p, L.b2.p, pl.n_groups, l};
-    std::copy_n(b1src[l], pl.spec.COUT, L.dev.bias1);
+    L.dev = TcConvDev{specs[l], L.tiles.p, L.b1.p, L.b2.p, n_groups, l};
+    std::copy_n(b1src[l], specs[l].COUT, L.dev.bias1);
     L.dev.bias2 = *b2src[l];
     if (l == 1) std::copy_n(hp.data() + ParamLayout::onset2_w, 9, L.dev.note_w);  // channel 0: the note input
   }
@@ -652,7 +661,7 @@ void bp_model_destroy(bp_model_t* m) {
   m->yhl.release();
   m->chl.release();
   m->cqt_wtc.release();
-  for (bp_model::TcLayer* L : {&m->tc_contour, &m->tc_onset, &m->tc_note}) L->tiles.release(), L->b2.release();
+  for (bp_model::TcLayer* L : {&m->tc_contour, &m->tc_onset, &m->tc_note}) L->tiles.release(), L->b1.release(), L->b2.release();
   if (m->d_params) cudaFree(m->d_params);
   if (m->d_derived) cudaFree(m->d_derived);
   if (m->d_gauss) cudaFree(m->d_gauss);
@@ -1465,6 +1474,23 @@ int bp_debug_tc_plan(int which, const float* w, int32_t* sizes, uint16_t* tiles,
   }
   if (group_step_off) std::memcpy(group_step_off, pl.group_step_off.data(), pl.group_step_off.size() * 4);
   if (group_ft) std::memcpy(group_ft, pl.group_ft.data(), pl.group_ft.size() * 4);
+  return BP_OK;
+}
+
+int bp_debug_tc_gather(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* starts, int32_t* ranges) {
+  if (!w || !sizes || which < 1 || which > 2) return fail(BP_E_INVALID, "bp_debug_tc_gather: bad argument");
+  const TcGatherGeom g = tc_gather_geometry(which);
+  sizes[0] = g.K;
+  sizes[1] = g.n_ci;
+  sizes[2] = g.KH;
+  sizes[3] = g.wout;
+  if (b1) {
+    std::vector<uint16_t> m;
+    tc_build_b1(which, w, m);
+    std::memcpy(b1, m.data(), m.size() * 2);
+  }
+  if (starts) std::copy(g.starts.begin(), g.starts.end(), starts);
+  if (ranges) std::copy(g.ranges.begin(), g.ranges.end(), ranges);
   return BP_OK;
 }
 

@@ -58,7 +58,9 @@ struct TcConvSpec {
 TcConvSpec tc_contour_spec();
 TcConvSpec tc_onset_spec();
 TcConvSpec tc_note_spec();
-struct TcConvPlan {  // host side: weight tiles + the per-group MMA programs
+// Host side: weight tiles + the per-group MMA programs of the Toeplitz form.  The kernels run it for the contour conv
+// only; the onset and note convs gather their A operand instead (tc_build_b1), and their plans only serve the tests.
+struct TcConvPlan {
   TcConvSpec spec{};
   std::vector<uint16_t> tiles;          // n_tiles x 4096 bf16 : [plane hi/lo][k-chunk 2][n 128][8]
   std::vector<int> tile_seq;            // per step: tile id
@@ -70,17 +72,27 @@ struct TcConvPlan {  // host side: weight tiles + the per-group MMA programs
 };
 struct TcConvDev {
   TcConvSpec spec;
-  const uint16_t* tiles;
-  const uint16_t* b2;  // conv2 weight matrix of the fused epilogue (tc_build_b2_full)
+  const uint16_t* tiles;  // contour: Toeplitz weight tiles (the program is in constant memory)
+  const uint16_t* b1;     // onset / note: conv1 B matrices (tc_build_b1)
+  const uint16_t* b2;     // conv2 weight matrix of the fused epilogue (tc_build_b2_full)
   int n_groups;
-  int layer;  // index of the program in constant memory (0 contour, 1 onset, 2 note)
+  int layer;  // 0 contour, 1 onset, 2 note
   // epilogue values, passed with every launch: conv1 bias (COUT used), conv2 bias, and for the onset layer the conv2
   // weights of its note input channel (models.py:305: concat[note, onset1]) [dt][df]
   float bias1[32];
   float bias2;
   float note_w[9];
 };
-int tc_upload_program(int layer, const TcConvPlan& plan, cudaStream_t st);  // 0 on success
+int tc_upload_program(const TcConvPlan& contour_plan, cudaStream_t st);  // 0 on success
+// conv1 of the onset (epi 1, w = [32][8][5][5]) / note (epi 2, w = [32][1][7][7]) layer as the kernel gathers it: its two
+// B matrices [parity 2][plane hi/lo][K / 8][32][8] bf16, and the geometry of the gather (window start of every output
+// bin and channel, [wout][n_ci]; the bins [lo, hi) of every channel that hold input, [n_ci][2])
+void tc_build_b1(int epi, const float* w, std::vector<uint16_t>& out);
+struct TcGatherGeom {
+  int K, n_ci, KH, wout;
+  std::vector<int> starts, ranges;
+};
+TcGatherGeom tc_gather_geometry(int epi);
 // bf16 hi/lo weight tiles of the fused second conv (epi: 0 contour, 1 onset, 2 note; w2 = that conv's weights), see TcB2
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out);
 // the same tiles placed into the K = 128 x N = width conv2 weight matrix the kernel reads (tc_conv.cu)

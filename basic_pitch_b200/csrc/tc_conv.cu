@@ -23,7 +23,8 @@
 //   * bias, sigmoid (+ the note input channel of the onset conv2, + unwrap inference.py:247-279) and the store.
 // EPI 0 stores the contour activations channels-last (path 2, activation-level tests).
 //
-// Formulation ("Toeplitz along frequency on aligned chunks")
+// Formulation of the contour conv1 ("Toeplitz along frequency on aligned chunks"; the onset and note conv1 gather instead,
+// see below)
 //   rows  m = b*174 + t            time frames of all windows of the chunk, two zero rows between windows
 //   D[m][(fl,co)] (+)= A[m+dt][8c .. 8c+15] x T(dt,off)[16][(fl,co)]
 //     A      the normalised CQT y itself (NOT the 8-channel stack), rows shifted by the time tap dt; K = 16 bins that
@@ -42,14 +43,27 @@
 // (hi*hi + hi*lo + lo*hi) in fp32, which keeps the posteriorgrams within ~1e-5 of the FP32 path
 // (SURVEY.md Appendix C.4); a single bf16 product would miss the 1e-3 bar.
 //
+// Formulation of the onset and note conv1 (EPI 1 / 2: 5 or 7 frequency taps at stride 3, where a Toeplitz tile would be
+// mostly zeros): an implicit GEMM per output bin f,
+//   D_f[m][co] = sum over K = (dt, ci, j < 8) of x[m + dt][s(f, ci) + j] * B_{f & 1}[(dt, ci, j)][co]      (m64 n32)
+//   s(f, ci)   the even bin at or below the first tap u0 = SF*f - PL + shift_ci, so the taps sit at j = (u0 & 1) + df
+//   B_p        [K = KH * n_ci * 8, padded to 16][32 channels]: the weights at those positions for f & 1 = p (TcGather)
+// The A operand is GATHERED from the data tile into wgmma A registers: a register holds the bins s + 2 qd, s + 2 qd + 1
+// of one row, one aligned 32-bit shared load, masked to zero where the reference has no input (outside the CQT / the
+// contour posteriorgram, outside the stacked image).  The two B matrices stay resident in shared memory.  The four bins of
+// a frequency tile go to four m64n32 accumulators that, side by side, are the m64n128 fragment of the Toeplitz form, so
+// the epilogue is the same for all layers.
+//
 // Work decomposition: item = (M-tile of 64 rows, split s of S over the frequency groups); group g = the two
 // frequency tiles {g, g + G0} (two accumulator slots; shared weight tiles where their content is equal).  A CTA (1 per
 // SM, persistent) walks items i = blockIdx.x, +gridDim.x, ...:
 //   warp 8      producer: bulk-copies the (64+KH-1) x 320 bf16 hi/lo data tile (k-chunk-major) once per item and
-//               streams the weight tiles of each group's program (8 KB each) through a ring of stages
-//   warps 0-3, 4-7  one warpgroup per accumulator slot of the group: program words from constant memory, 3 x wgmma
-//               m64n128k16 per step (the stage is released once they completed), then the epilogue of the slot's tile
-//               from the accumulator registers: bias, ReLU, split, the conv2 MMAs, time taps, finish (see above)
+//               (contour) streams the weight tiles of each group's program (8 KB each) through a ring of stages;
+//               (onset / note) copies the conv1 B matrices once per CTA
+//   warps 0-3, 4-7  one warpgroup per accumulator slot of the group: contour: program words from constant memory, 3 x
+//               wgmma m64n128k16 per step (the stage is released once they completed); onset / note: the gather and
+//               3 x wgmma m64n32k16 per K-step and bin.  Then the epilogue of the slot's tile from the accumulator
+//               registers: bias, ReLU, split, the conv2 MMAs, time taps, finish (see above)
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 
@@ -103,15 +117,43 @@ __host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour,
   return epi == 1 ? TcB2{2, 16, 3, 4, 32, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64, 64} : TcB2{1, 32, 5, 5, 104, 40};
 }
 
+// ------------------------------------------------------------------------------------------------
+// The gathered conv1 of the onset (EPI 1) and note (EPI 2) layers, 32 output channels at frequency stride 3 (see the
+// header).  K runs over (time tap dt, channel ci, 8-bin window j): k = 8 (dt * n_ci + ci) + j, padded to whole K = 16 steps.
+//   onset: 5 dt x 8 harmonics x 8 = 320 (20 steps, 62.5 % of the rows hold a tap); note: 7 dt x 1 x 8 = 56 -> 64 (4 steps)
+// ------------------------------------------------------------------------------------------------
+struct TcGather {
+  int KH, KW, PL, n_ci;  // time / frequency taps, frequency pad, input channels (frequency stride 3, 32 output channels)
+  int data_bins;         // bins of the input rows (the CQT, or the contour posteriorgram)
+  int tile_bins;         // bins the data tile holds (8 x its chunks)
+  int shifts[8];         // harmonic shift of every input channel
+  __host__ __device__ constexpr int ksteps() const { return (KH * n_ci * 8 + 15) / 16; }
+};
+__host__ __device__ constexpr TcGather tc_gather_spec(int epi) {  // epi 1 onset, 2 note (the geometry of tc_*_spec)
+  return epi == 1 ? TcGather{5, 5, 1, 8, kCqtBins, 312, {-36, 0, 36, 57, 72, 84, 93, 101}}
+                  : TcGather{7, 7, 2, 1, kContourBins, 264, {0, 0, 0, 0, 0, 0, 0, 0}};
+}
+// first bin of the 8-bin window of output bin f, channel ci: the even bin at or below its first tap
+__host__ __device__ constexpr int tc_gather_start(TcGather g, int f, int ci) { return (3 * f - g.PL + g.shifts[ci]) & ~1; }
+// the bins u of channel ci that hold input: inside the row (u < data_bins) and inside the stacked image
+// (0 <= u - shift < 264, the zero fill of HarmonicStacking); the gather supplies zero everywhere else
+__host__ __device__ constexpr int tc_gather_lo(TcGather g, int ci) { return g.shifts[ci] > 0 ? g.shifts[ci] : 0; }
+__host__ __device__ constexpr int tc_gather_hi(TcGather g, int ci) {
+  return g.data_bins < kContourBins + g.shifts[ci] ? g.data_bins : kContourBins + g.shifts[ci];
+}
+
 namespace tc {
-// Shared memory is laid out per layer: the data tile, as many weight-tile stages as fit, and for the fused layers the
-// conv2 weight matrix and the staging of the conv2 sums.
+// Shared memory is laid out per layer: the data tile; contour: as many weight-tile stages as fit; onset / note: the two
+// conv1 B matrices; for the fused layers the conv2 weight matrix and the staging of the conv2 sums.
 struct TcSmem {
   int data_bytes;   // [2 planes][chunks][64 + KH - 1 rows][16 B], rounded up to 1 KB
+  int b1_bytes;     // onset / note conv1 B matrices [parity 2][plane 2][K / 8][32][8] bf16
   int b2_bytes;     // conv2 weight matrix [2 planes][128][width] bf16
   int p_bytes;      // conv2 sums [2 slots][64 rows][pass + 1] fp32
-  int stages;
-  __host__ __device__ constexpr int total() const { return data_bytes + stages * kTileBytes + b2_bytes + p_bytes + 512; }
+  int stages;       // contour weight-tile stages
+  __host__ __device__ constexpr int total() const {
+    return data_bytes + stages * kTileBytes + b1_bytes + b2_bytes + p_bytes + 512;
+  }
 };
 constexpr int kMaxSmem = 232448;  // 227 KB opt-in per CTA
 constexpr int kMaxStages = 12;
@@ -119,16 +161,18 @@ __host__ __device__ constexpr TcSmem tc_smem(int epi) {  // epi: 0 contour (acti
   TcSmem s{};
   const int chunks = epi == 2 ? 33 : 39, rows = kMTile + (epi == 1 ? 4 : epi == 2 ? 6 : 2);
   const TcB2 b2 = tc_b2_spec(epi);
+  const bool gather = epi == 1 || epi == 2;
   s.data_bytes = (2 * chunks * rows * 16 + 1023) / 1024 * 1024;
+  s.b1_bytes = gather ? 2 * 2 * 16 * tc_gather_spec(epi).ksteps() * 32 * 2 : 0;
   s.b2_bytes = epi == 0 ? 0 : 2 * 128 * b2.width * 2;
   s.p_bytes = epi == 0 ? 0 : 2 * 64 * (b2.pass + 1) * 4;
-  const int st = (kMaxSmem - 512 - s.data_bytes - s.b2_bytes - s.p_bytes) / kTileBytes;
-  s.stages = st < kMaxStages ? st : kMaxStages;
+  const int st = (kMaxSmem - 512 - s.data_bytes - s.b1_bytes - s.b2_bytes - s.p_bytes) / kTileBytes;
+  s.stages = gather ? 0 : st < kMaxStages ? st : kMaxStages;
   return s;
 }
-// weight stages per layer (DESIGN §4.1): contour activations, onset, note, contour fused
-static_assert(tc_smem(0).stages == 12 && tc_smem(1).stages == 12 && tc_smem(2).stages == 11 && tc_smem(3).stages == 9,
-              "weight-ring depth per layer");
+// weight stages of the contour layer (DESIGN §4.1): activations, fused
+static_assert(tc_smem(0).stages == 12 && tc_smem(3).stages == 9, "weight-ring depth per layer");
+static_assert(tc_smem(1).total() <= kMaxSmem && tc_smem(2).total() <= kMaxSmem, "onset / note shared memory");
 // step word of a slot: [0,14) A start-address offset >> 4, [15] first MMA into that accumulator; kNoUse = the
 // slot's frequency tile does not use this step's weight tile
 constexpr uint32_t kUseFirstAcc = 1u << 15, kNoUse = 0xffffffffu;
@@ -320,14 +364,15 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   n_groups = (int)group_ft.size() / 2;
 }
 
-// The MMA programs live in constant memory: the issuing warp indexes them with warp-uniform values, so the words,
-// the descriptors derived from them and the loop state stay in uniform registers (no per-use R2UR traffic).
-// They depend only on the layer geometry (TcConvSpec), not on the weights (tiles are de-duplicated by structure, see
-// TcConvPlan::build), so one upload serves every model of the process; the weight tiles they index are per model.
-__constant__ uint32_t c_prog[3][2][tc::kMaxSteps];  // [layer][slot][step]
-__constant__ int c_tile_seq[3][tc::kMaxSteps];       // [layer][step] -> weight tile id
-__constant__ int c_group_step_off[3][tc::kMaxGroups + 1];
-__constant__ int c_group_ft[3][2 * tc::kMaxGroups];
+// The contour layer's MMA program lives in constant memory: the issuing warp indexes it with warp-uniform values, so the
+// words, the descriptors derived from them and the loop state stay in uniform registers (no per-use R2UR traffic).
+// It depends only on the layer geometry (TcConvSpec), not on the weights (tiles are de-duplicated by structure, see
+// TcConvPlan::build), so one upload serves every model of the process; the weight tiles it indexes are per model.
+// (The onset and note layers gather their A operand and need no program.)
+__constant__ uint32_t c_prog[2][tc::kMaxSteps];  // [slot][step]
+__constant__ int c_tile_seq[tc::kMaxSteps];       // [step] -> weight tile id
+__constant__ int c_group_step_off[tc::kMaxGroups + 1];
+__constant__ int c_group_ft[2 * tc::kMaxGroups];
 
 // tiles: [tile][plane hi/lo][k-chunk 2][n N2][8] bf16 (canonical K-major no-swizzle: LBO = N2 * 16 B, SBO = 128 B)
 void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
@@ -355,18 +400,57 @@ void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
       }
 }
 
-int tc_upload_program(int layer, const TcConvPlan& pl, cudaStream_t st) {
-  if (layer < 0 || layer > 2 || (int)pl.tile_seq.size() > tc::kMaxSteps - 1 || pl.n_groups > tc::kMaxGroups) return -1;
+int tc_upload_program(const TcConvPlan& pl, cudaStream_t st) {
+  if (pl.spec.epi != 0 || (int)pl.tile_seq.size() > tc::kMaxSteps - 1 || pl.n_groups > tc::kMaxGroups) return -1;
   for (int sl = 0; sl < 2; ++sl)
-    cudaMemcpyToSymbolAsync(c_prog, pl.slot_words[sl].data(), pl.slot_words[sl].size() * 4,
-                            ((size_t)layer * 2 + sl) * tc::kMaxSteps * 4, cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_tile_seq, pl.tile_seq.data(), pl.tile_seq.size() * 4, (size_t)layer * tc::kMaxSteps * 4,
+    cudaMemcpyToSymbolAsync(c_prog, pl.slot_words[sl].data(), pl.slot_words[sl].size() * 4, (size_t)sl * tc::kMaxSteps * 4,
+                            cudaMemcpyHostToDevice, st);
+  cudaMemcpyToSymbolAsync(c_tile_seq, pl.tile_seq.data(), pl.tile_seq.size() * 4, 0, cudaMemcpyHostToDevice, st);
+  cudaMemcpyToSymbolAsync(c_group_step_off, pl.group_step_off.data(), pl.group_step_off.size() * 4, 0,
                           cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_group_step_off, pl.group_step_off.data(), pl.group_step_off.size() * 4,
-                          (size_t)layer * (tc::kMaxGroups + 1) * 4, cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_group_ft, pl.group_ft.data(), pl.group_ft.size() * 4, (size_t)layer * 2 * tc::kMaxGroups * 4,
-                          cudaMemcpyHostToDevice, st);
+  cudaMemcpyToSymbolAsync(c_group_ft, pl.group_ft.data(), pl.group_ft.size() * 4, 0, cudaMemcpyHostToDevice, st);
   return cudaStreamSynchronize(st) == cudaSuccess ? 0 : -1;
+}
+
+// The two conv1 B matrices of the onset / note layer, f even and f odd (TcGather), in the layout the MMAs read:
+// [parity 2][plane hi/lo][k-chunk K / 8][n 32][8] bf16 (K-major no-swizzle: LBO = 32 * 16 B, SBO = 128 B).
+// B_p[8 (dt * n_ci + ci) + j][co] = W[co][ci][dt][j - o], o = the first tap's offset in its window for f & 1 = p.
+void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<uint16_t>& out) {
+  const TcGather g = tc_gather_spec(epi);
+  const size_t plane = (size_t)16 * g.ksteps() * 32;
+  out.assign(4 * plane, 0);
+  for (int p = 0; p < 2; ++p)
+    for (int dt = 0; dt < g.KH; ++dt)
+      for (int ci = 0; ci < g.n_ci; ++ci) {
+        const int o = 3 * p - g.PL + g.shifts[ci] - tc_gather_start(g, p, ci);
+        for (int j = 0; j < 8; ++j) {
+          const int df = j - o, k = 8 * (dt * g.n_ci + ci) + j;
+          if (df < 0 || df >= g.KW) continue;
+          for (int co = 0; co < 32; ++co) {
+            const float w = W[((co * g.n_ci + ci) * g.KH + dt) * g.KW + df];
+            const uint16_t hi = f2bf(w), lo = f2bf(w - bf2f(hi));
+            const size_t e = ((size_t)(k >> 3) * 32 + co) * 8 + (k & 7);
+            out[(2 * p) * plane + e] = hi;
+            out[(2 * p + 1) * plane + e] = lo;
+          }
+        }
+      }
+}
+
+TcGatherGeom tc_gather_geometry(int epi) {
+  const TcGather g = tc_gather_spec(epi);
+  TcGatherGeom r;
+  r.K = 16 * g.ksteps();
+  r.n_ci = g.n_ci;
+  r.KH = g.KH;
+  r.wout = kPitches;
+  for (int f = 0; f < kPitches; ++f)
+    for (int ci = 0; ci < g.n_ci; ++ci) r.starts.push_back(tc_gather_start(g, f, ci));
+  for (int ci = 0; ci < g.n_ci; ++ci) {
+    r.ranges.push_back(tc_gather_lo(g, ci));
+    r.ranges.push_back(tc_gather_hi(g, ci));
+  }
+  return r;
 }
 
 // The small tiles expanded into the K = 128 x N = width matrix the conv2 MMAs read:
@@ -461,11 +545,12 @@ struct TcArgs {
   CUtensorMap data_map;         // 4-D tensor map of `data`: (8 elements, rows_total, chunks8, 2 planes); box = one data tile
   int use_tmap;                 // 0: the encoder was not available, the tile is fetched chunk by chunk with 1-D bulk copies
   const __nv_bfloat16* data;    // [2][chunks8][rows_total][8]
-  const uint16_t* tiles;        // [n_tiles][8192 B]
+  const uint16_t* tiles;        // contour: [n_tiles][8192 B]
+  const uint16_t* b1;           // onset / note: the conv1 B matrices (tc_build_b1)
   const uint16_t* b2;           // conv2 weight matrix (tc_build_b2_full), fused layers
   TcOut o;                      // where the results go (kernels.cuh)
   int edge_rows;                // row stride of o.edge: [edge slot][side 2][KE][edge_rows]
-  int layer;                    // which constant-memory program (0 contour, 1 onset, 2 note)
+  int layer;                    // 0 contour, 1 onset, 2 note (cycle accounting)
   int rows_total, n_mtiles, n_windows;
   int n_groups, n_split;        // an item covers groups [s*n_groups/n_split, (s+1)*n_groups/n_split)
   int data_rows, row0;          // tile rows (64 + KH - 1); first data row of M-tile 0
@@ -482,12 +567,12 @@ __device__ __forceinline__ float sigmoidf_fast(float x) { return __fdividef(1.f,
 // when the CTA ends.  Without the flag the calls are empty.
 namespace tc {
 enum TcClk {
-  kClkFull,       // consumers: waiting on full_w (the weight tile of the step)
+  kClkFull,       // consumers: contour: waiting on full_w (the weight tile of the step); onset / note: the gather
   kClkMma,        // consumers: issuing the step's MMAs and waiting for the previous step's
   kClkEpi,        // consumers: the epilogue of a tile (after the last MMA of the group)
   kClkData,       // consumers: waiting on data_full (the item's data tile)
   kClkConsOther,  // consumers: everything else (program reads, skipped steps, row set-up)
-  kClkEmpty,      // producer: waiting on empty_w (a free weight stage)
+  kClkEmpty,      // producer: waiting on empty_w (a free weight stage; contour only)
   kClkDataEmpty,  // producer: waiting on data_empty (both slots done with the previous item's data tile)
   kClkProdOther,  // producer: everything else (issuing the copies)
   kNumClk
@@ -496,14 +581,16 @@ enum TcClk {
 #ifdef BP_TC_CLOCKS
 __device__ unsigned long long g_tc_clocks[3][tc::kNumClk];
 struct TcClocks {
-  long long t, c[tc::kNumClk];
+  // 32-bit sums (a thread's share of one launch stays far below 2^32 cycles) keep the instrumented consumers within
+  // their register budget
+  uint32_t t, c[tc::kNumClk];
   __device__ __forceinline__ TcClocks() {
-    t = clock64();
+    t = (uint32_t)clock();
 #pragma unroll
     for (int k = 0; k < tc::kNumClk; ++k) c[k] = 0;
   }
   __device__ __forceinline__ void lap(int k) {
-    const long long n = clock64();
+    const uint32_t n = (uint32_t)clock();
     c[k] += n - t;
     t = n;
   }
@@ -707,20 +794,114 @@ __device__ __forceinline__ void conv2_mma(float (&p)[NW / 2], const uint32_t (&a
   }
 }
 
+// conv1 of frequency tile ft of the onset / note layer (EPI 1 / 2), gathered (see the header): for each bin f = 4 ft + fl
+// the K-steps of TcGather, three split products m64n32k16 each, into acc[16 fl ..] (= columns 32 fl .. of the m64n128
+// fragment).  The A registers of the next step are loaded while the current step's MMAs run (two register buffers).
+// Every output sums its steps in the same order whatever the item: a value depends only on f and the layer.
+template <int EPI>
+struct GatherRegs {
+  static constexpr TcGather G = tc_gather_spec(EPI);
+  // per channel: byte offset of the thread's bin pair (row fr0) in the data tile in bits [0, 24), and in bits 24 / 25
+  // whether its first / second bf16 half holds input (one register per channel keeps the consumers within budget)
+  uint32_t om[G.n_ci];
+  // the window of output bin f for the thread (lane qd of its quad, rows fr0 / fr0 + 8)
+  __device__ __forceinline__ void setup(int f, int fr0, int qd) {
+#pragma unroll
+    for (int ci = 0; ci < G.n_ci; ++ci) {
+      const int u = tc_gather_start(G, f, ci) + 2 * qd;
+      const int lo = tc_gather_lo(G, ci), hi = tc_gather_hi(G, ci);
+      const int uc = min(max(u, 0), G.tile_bins - 2);  // a pair outside the tile is masked; read one inside it
+      om[ci] = (uint32_t)((uc >> 3) * ((tc::kMTile + G.KH - 1) * 16) + (uc & 7) * 2 + fr0 * 16) |
+               (u >= lo && u < hi ? 1u << 24 : 0u) | (u + 1 >= lo && u + 1 < hi ? 1u << 25 : 0u);
+    }
+  }
+  __device__ __forceinline__ uint32_t mask(int ci) const {  // bits 24 / 25 -> 0x0000ffff / 0xffff0000
+    const uint32_t m = om[ci] >> 24;
+    return ((m | (m << 15)) & 0x10001u) * 0xffffu;
+  }
+  // the A registers of K-step ks, x[0..3] hi, x[4..7] lo: (window 2 ks, row fr0), (2 ks, fr0 + 8), (2 ks + 1, fr0),
+  // (2 ks + 1, fr0 + 8)
+  template <int KS>
+  __device__ __forceinline__ void load(const unsigned char* s_data, uint32_t (&x)[8]) const {
+    constexpr int kPlane = G.tile_bins / 8 * (tc::kMTile + G.KH - 1) * 16;  // bytes of one plane of the data tile
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      constexpr int NW = G.KH * G.n_ci;  // 8-bin windows holding taps; the rest of the last step is K padding
+      const int wi = 2 * KS + h, dt = wi / G.n_ci, ci = wi % G.n_ci;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (wi < NW) {
+          const unsigned char* p = s_data + (om[ci] & 0xffffffu) + dt * 16 + rr * 128;
+          x[2 * h + rr] = *reinterpret_cast<const uint32_t*>(p) & mask(ci);
+          x[4 + 2 * h + rr] = *reinterpret_cast<const uint32_t*>(p + kPlane) & mask(ci);
+        } else {
+          x[2 * h + rr] = 0u;
+          x[4 + 2 * h + rr] = 0u;
+        }
+      }
+    }
+  }
+};
+
+template <int EPI, int I>
+__device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& gr, uint32_t (&x)[2][8], const unsigned char* s_data,
+                                             uint64_t d0, int ft, int fr0, int qd, TcClocks& clk) {
+  using namespace tc;
+  constexpr int KS = tc_gather_spec(EPI).ksteps(), NST = 4 * KS;
+  constexpr int fl = I / KS, ks = I % KS;
+  constexpr uint32_t kB1Plane = 16 * KS * 32 * 2;  // bytes of one B plane
+  float(&d)[16] = *reinterpret_cast<float(*)[16]>(acc + 16 * fl);
+  // B_{f & 1}, K-step ks (f & 1 = fl & 1: a tile starts on an even bin)
+  const uint64_t bh = d0 + (uint64_t)(((fl & 1) * 2 * kB1Plane + ks * 2 * 32 * 16) >> 4), bl = bh + (kB1Plane >> 4);
+  const uint32_t xh[4] = {x[I & 1][0], x[I & 1][1], x[I & 1][2], x[I & 1][3]};
+  const uint32_t xl[4] = {x[I & 1][4], x[I & 1][5], x[I & 1][6], x[I & 1][7]};
+  wgmma_fence();
+  wgmma_rs_n32(d, xh, bh, ks ? 1u : 0u);
+  wgmma_rs_n32(d, xh, bl, 1u);
+  wgmma_rs_n32(d, xl, bh, 1u);
+  wgmma_commit();
+  if constexpr (I + 1 < NST) {
+    wgmma_wait<1>();  // the previous step's MMAs are done: its A registers may be refilled
+    clk.lap(kClkMma);
+    if constexpr ((I + 1) % KS == 0) gr.setup(4 * ft + (I + 1) / KS, fr0, qd);
+    gr.template load<(I + 1) % KS>(s_data, x[(I + 1) & 1]);
+    clk.lap(kClkFull);
+    gather_steps<EPI, I + 1>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
+  }
+}
+
+template <int EPI>
+__device__ __forceinline__ void gather_conv1(float (&acc)[64], const unsigned char* s_data, uint32_t b1, int ft, int fr0, int qd,
+                                             TcClocks& clk) {
+  using namespace tc;
+  GatherRegs<EPI> gr;
+  const uint64_t d0 = make_desc(b1, 32 * 16, 128);
+  uint32_t x[2][8];
+  gr.setup(4 * ft, fr0, qd);
+  gr.template load<0>(s_data, x[0]);
+  clk.lap(kClkFull);
+  gather_steps<EPI, 0>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
+  wgmma_wait<0>();
+  reg_fence(acc);
+  clk.lap(kClkMma);
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using namespace tc;
   constexpr bool kFused = EPI != 0;
+  constexpr bool kGather = EPI == 1 || EPI == 2;  // onset / note: gathered conv1, no weight ring
   constexpr TcB2 B2 = tc_b2_spec(EPI);
   constexpr int NW = B2.width, PC = B2.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
   static_assert(PC % 8 == 0 && PC % B2.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr TcSmem SM = tc_smem(EPI);
   constexpr int kStages = SM.stages;
-  static_assert(SM.total() <= kMaxSmem && kStages <= kMaxStages && kStages >= 4, "dynamic shared memory per CTA");
+  static_assert(SM.total() <= kMaxSmem && kStages <= kMaxStages && (kGather || kStages >= 4), "dynamic shared memory per CTA");
   unsigned char* s_data = smem;                    // [2 planes][chunks][data_rows][16 B]
-  unsigned char* s_w = smem + SM.data_bytes;       // [kStages][8192]
-  unsigned char* s_b2 = s_w + kStages * kTileBytes;  // conv2 weight matrix [plane 2][k-chunk 16][NW][16 B]
+  unsigned char* s_w = smem + SM.data_bytes;       // contour: [kStages][8192]
+  unsigned char* s_b1 = s_w + kStages * kTileBytes;  // onset / note: conv1 B matrices (tc_build_b1)
+  unsigned char* s_b2 = s_b1 + SM.b1_bytes;          // conv2 weight matrix [plane 2][k-chunk 16][NW][16 B]
   float* s_p = reinterpret_cast<float*>(s_b2 + SM.b2_bytes);  // conv2 sums [slot 2][64 rows][PS]
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(s_p) + SM.p_bytes);
   uint64_t* full_w = bars;             // [kStages]
@@ -728,7 +909,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   uint64_t* data_full = bars + 2 * kStages;
   uint64_t* data_empty = data_full + 1;  // one arrival per consumer warp
   uint64_t* b2_full = data_empty + 1;
-  uint32_t* issued = reinterpret_cast<uint32_t*>(b2_full + 1);  // weight fills the producer has issued so far
+  uint64_t* b1_full = b2_full + 1;
+  uint32_t* issued = reinterpret_cast<uint32_t*>(b1_full + 1);  // weight fills the producer has issued so far
 
   // Broadcasting the warp index keeps the role branches and the producer loop state in uniform registers.
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -744,6 +926,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     mbar_init(data_full, 1);
     mbar_init(data_empty, kConsumerWarps);
     mbar_init(b2_full, 1);
+    mbar_init(b1_full, 1);
     *issued = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -759,9 +942,11 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     // The whole warp walks the loop with warp-uniform state; the arrive / copy instructions are predicated on the elected
     // lane (no elect loop and R2UR around every UBLKCP: the weight ring is paced by this loop's latency per step).
     // For a step that one slot does not use, the producer also arrives on the stage's empty_w for that slot's four warps,
-    // so the two slots move through the ring independently (see the consumers).
+    // so the two slots move through the ring independently (see the consumers).  The onset / note layers have no ring:
+    // their producer copies the B matrices once and then only the data tile of every item.
     const uint32_t leader = elect_one() ? 1u : 0u;
     if constexpr (kFused) bulk_g2s_expect_pred(s_b2, a.b2, (uint32_t)SM.b2_bytes, b2_full, leader);
+    if constexpr (kGather) bulk_g2s_expect_pred(s_b1, a.b1, (uint32_t)SM.b1_bytes, b1_full, leader);
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;
     const size_t plane_elems = (size_t)a.chunks8 * a.rows_total * 8;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
@@ -784,17 +969,18 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       }
       __syncwarp();
       ph_d ^= 1;
-      const int s0 = c_group_step_off[a.layer][g0], s1 = c_group_step_off[a.layer][g1];
-      int tile = c_tile_seq[a.layer][s0];
+      if constexpr (kGather) continue;
+      const int s0 = c_group_step_off[g0], s1 = c_group_step_off[g1];
+      int tile = c_tile_seq[s0];
       for (int s = s0; s < s1; ++s) {
-        const int tile_next = c_tile_seq[a.layer][s + 1];  // (one past the end is inside the array)
+        const int tile_next = c_tile_seq[s + 1];  // (one past the end is inside the array)
         clk.lap(kClkProdOther);
         mbar_wait_wd(empty_w + stage, ph_w ^ 1, 2);
         clk.lap(kClkEmpty);
         bulk_g2s_expect_pred(s_w + stage * kTileBytes, a.tiles + (size_t)tile * (kTileBytes / 2), kTileBytes, full_w + stage,
                              leader);
         // every step has at least one user, so at most one slot skips it
-        const bool skip = c_prog[a.layer][0][s] == kNoUse || c_prog[a.layer][1][s] == kNoUse;
+        const bool skip = c_prog[0][s] == kNoUse || c_prog[1][s] == kNoUse;
         mbar_arrive_cnt_pred(empty_w + stage, kConsumerWarps / 2, skip ? leader : 0u);
         counter_publish(issued, ++n_fill);
         if (++stage == kStages) {
@@ -823,9 +1009,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[EPI == 0 || EPI == 3 ? 2 * qd + e : 8 * i + 2 * qd + e];
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;  // n_fill: index of the current step's weight fill in the CTA
     const uint32_t a_hi = smem_u32(s_data), a_lo = a_hi + plane_bytes, w_base = smem_u32(s_w);
-    const uint32_t* prog = c_prog[a.layer][slot];
+    const uint32_t* prog = c_prog[slot];
     float* sp_rows = s_p + slot * 64 * PS;
     if constexpr (kFused) mbar_wait_wd(b2_full, 0, 6);
+    if constexpr (kGather) mbar_wait_wd(b1_full, 0, 7);
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       const int mt = it / a.n_split, spl = it % a.n_split;
       const int g0 = spl * a.n_groups / a.n_split, g1 = (spl + 1) * a.n_groups / a.n_split;
@@ -877,58 +1064,64 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       clk.lap(kClkData);
       ph_d ^= 1;
       for (int g = g0; g < g1; ++g) {
-        const int ft = c_group_ft[a.layer][2 * g + slot];
-        const int s0 = c_group_step_off[a.layer][g], s1 = c_group_step_off[a.layer][g + 1];
         float acc[64];
-        int pend = -1;  // stage read by the MMA group still in flight
-        uint32_t pend_fill = 0;  // and its fill index
-        uint32_t w = prog[s0];
-        // A slot skips the steps it does not use (kNoUse) completely: no wait on full_w, no arrival on empty_w (the
-        // producer arrives for it).  So it does not see every phase of a stage, and its parity wait for fill f (the
-        // stage's phase f / kStages) is only exact if the stage is at most one phase off when it waits:
-        //   * not ahead: it first waits until the producer has ISSUED fill f.  That happened after the release of fill
-        //     f - kStages, whose user(s) waited for it to land, so the previous phase is complete;
-        //   * not behind: fill f + kStages cannot land before this slot's own arrival for fill f gates the refill.
-        for (int s = s0; s < s1; ++s, ++n_fill) {
-          const uint32_t w_next = prog[s + 1];  // (one word past the end is inside the array)
-          if (w != kNoUse) {
-            if (pend >= 0 && n_fill - pend_fill >= kStages) {
-              // fill f is issued after the release of fill f - kStages, which may be the stage still held
-              wgmma_wait<0>();
-              if (lane == 0) mbar_arrive(empty_w + pend);
-              pend = -1;
+        int ft;
+        if constexpr (kGather) {
+          ft = g + slot * a.g0 < a.n_ft ? g + slot * a.g0 : -1;
+          if (ft >= 0) gather_conv1<EPI>(acc, s_data, smem_u32(s_b1), ft, fr0, qd, clk);
+        } else {
+          ft = c_group_ft[2 * g + slot];
+          const int s0 = c_group_step_off[g], s1 = c_group_step_off[g + 1];
+          int pend = -1;  // stage read by the MMA group still in flight
+          uint32_t pend_fill = 0;  // and its fill index
+          uint32_t w = prog[s0];
+          // A slot skips the steps it does not use (kNoUse) completely: no wait on full_w, no arrival on empty_w (the
+          // producer arrives for it).  So it does not see every phase of a stage, and its parity wait for fill f (the
+          // stage's phase f / kStages) is only exact if the stage is at most one phase off when it waits:
+          //   * not ahead: it first waits until the producer has ISSUED fill f.  That happened after the release of fill
+          //     f - kStages, whose user(s) waited for it to land, so the previous phase is complete;
+          //   * not behind: fill f + kStages cannot land before this slot's own arrival for fill f gates the refill.
+          for (int s = s0; s < s1; ++s, ++n_fill) {
+            const uint32_t w_next = prog[s + 1];  // (one word past the end is inside the array)
+            if (w != kNoUse) {
+              if (pend >= 0 && n_fill - pend_fill >= kStages) {
+                // fill f is issued after the release of fill f - kStages, which may be the stage still held
+                wgmma_wait<0>();
+                if (lane == 0) mbar_arrive(empty_w + pend);
+                pend = -1;
+              }
+              clk.lap(kClkConsOther);
+              counter_wait_above(issued, n_fill);
+              mbar_wait_wd(full_w + stage, ph_w, 5);
+              clk.lap(kClkFull);
+              const uint32_t off = (w & 0x3fffu) << 4;  // chunk c8, row dt of the data tile
+              const uint32_t bw = w_base + stage * kTileBytes;
+              const uint64_t dah = make_desc(a_hi + off, lbo, 128), dal = make_desc(a_lo + off, lbo, 128);
+              const uint64_t dbh = make_desc(bw, 2048, 128), dbl = make_desc(bw + 4096, 2048, 128);
+              wgmma_fence();
+              wgmma_ss_n128(acc, dah, dbh, (w & kUseFirstAcc) ? 0u : 1u);
+              wgmma_ss_n128(acc, dah, dbl, 1u);
+              wgmma_ss_n128(acc, dal, dbh, 1u);
+              wgmma_commit();
+              wgmma_wait<1>();  // the previous step's MMAs are done: its weight stage may be refilled
+              if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
+              pend = (int)stage;
+              pend_fill = n_fill;
+              clk.lap(kClkMma);
             }
-            clk.lap(kClkConsOther);
-            counter_wait_above(issued, n_fill);
-            mbar_wait_wd(full_w + stage, ph_w, 5);
-            clk.lap(kClkFull);
-            const uint32_t off = (w & 0x3fffu) << 4;  // chunk c8, row dt of the data tile
-            const uint32_t bw = w_base + stage * kTileBytes;
-            const uint64_t dah = make_desc(a_hi + off, lbo, 128), dal = make_desc(a_lo + off, lbo, 128);
-            const uint64_t dbh = make_desc(bw, 2048, 128), dbl = make_desc(bw + 4096, 2048, 128);
-            wgmma_fence();
-            wgmma_ss_n128(acc, dah, dbh, (w & kUseFirstAcc) ? 0u : 1u);
-            wgmma_ss_n128(acc, dah, dbl, 1u);
-            wgmma_ss_n128(acc, dal, dbh, 1u);
-            wgmma_commit();
-            wgmma_wait<1>();  // the previous step's MMAs are done: its weight stage may be refilled
-            if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
-            pend = (int)stage;
-            pend_fill = n_fill;
-            clk.lap(kClkMma);
+            if (++stage == kStages) {
+              stage = 0;
+              ph_w ^= 1;
+            }
+            w = w_next;
           }
-          if (++stage == kStages) {
-            stage = 0;
-            ph_w ^= 1;
-          }
-          w = w_next;
+          clk.lap(kClkConsOther);
+          wgmma_wait<0>();
+          reg_fence(acc);
+          clk.lap(kClkMma);
+          if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
         }
-        clk.lap(kClkConsOther);
-        wgmma_wait<0>();
-        reg_fence(acc);
-        clk.lap(kClkMma);
-        if (pend >= 0 && lane == 0) mbar_arrive(empty_w + pend);
-        if (g == g1 - 1 && lane == 0) mbar_arrive(data_empty);  // this warp's MMAs no longer read the data tile
+        if (g == g1 - 1 && lane == 0) mbar_arrive(data_empty);  // this warp no longer reads the data tile
         if (ft < 0) continue;
         // first / last tile of this slot's ascending range inside the item
         const bool first = (g == g0);
@@ -1146,6 +1339,7 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   TcArgs a{};
   a.data = data;
   a.tiles = dev.tiles;
+  a.b1 = dev.b1;
   a.b2 = dev.b2;
   a.o = o;
   a.layer = dev.layer;

@@ -243,9 +243,17 @@ int64_t bp_debug_resample_filter(int32_t up, int32_t down, double* taps, int64_t
  * programs, csrc/tc_conv.cu) of the contour conv (which = 0, w = [8][8][3][39]), the onset conv (which = 1,
  * w = [32][8][5][5]) or the note conv (which = 2, w = [32][1][7][7]) so that tests can emulate the program on the CPU.  sizes[4] = {n_tiles, n_steps, n_uses,
  * n_groups}; pass NULL arrays to query sizes first.  tiles: n_tiles x 4096 bf16 ([plane hi/lo][k-chunk 2][n 128][8]);
- * slot_words: [2][n_steps]; group_step_off has n_groups + 1 entries, group_ft n_groups x 2. */
+ * slot_words: [2][n_steps]; group_step_off has n_groups + 1 entries, group_ft n_groups x 2.  The kernels run the
+ * contour plan only; the onset and note plans pin the planner on stride-3 geometry (see bp_debug_tc_gather). */
 int bp_debug_tc_plan(int which, const float* w, int32_t* sizes, uint16_t* tiles, int32_t* tile_seq, uint32_t* slot_words,
                      int32_t* group_step_off, int32_t* group_ft);
+
+/* Host-only: the conv1 of the onset (which = 1, w = [32][8][5][5]) or note (which = 2, w = [32][1][7][7]) layer as the
+ * kernel computes it, an implicit GEMM with a gathered A operand (csrc/tc_conv.cu, TcGather).  sizes[4] = {K, n_ci, KH,
+ * wout}; b1 (may be NULL): the two B matrices, [parity of the output bin 2][plane hi/lo][K / 8][32][8] bf16, row
+ * k = 8 (dt * n_ci + ci) + j; starts (may be NULL): [wout][n_ci] first input bin of the 8-bin window of output bin f and
+ * channel ci; ranges (may be NULL): [n_ci][2] the input bins [lo, hi) of each channel that hold data (zero elsewhere). */
+int bp_debug_tc_gather(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* starts, int32_t* ranges);
 
 /* Host-only: the bf16 hi/lo weight tiles of the fused SECOND convolution of a tensor-core layer (csrc/tc_conv.cu, TcB2):
  * which = 0 contour conv2 (w2 = [1][8][5][5], reference models.py:254-262), 1 onset conv2 ([1][33][3][3], models.py:305-313),

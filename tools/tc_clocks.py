@@ -1,7 +1,8 @@
 """Cycle accounting of the three tensor-core conv kernels (conv_tc_kernel, 1 GPU): builds the library with
 -DBP_TC_CLOCKS into a temporary directory (or loads --lib), runs the bench workload and prints, per layer, where the
-warps' SM cycles go as JSON: the consumer warpgroups (waiting on a weight stage, MMAs, epilogue, waiting on the data
-tile) and the producer warp (waiting on a free stage, waiting on the data tile to be released)."""
+warps' SM cycles go as JSON: the consumer warpgroups (contour: waiting on a weight stage; onset / note: gathering the A
+registers; then MMAs, epilogue, waiting on the data tile) and the producer warp (contour: waiting on a free stage; all:
+waiting on the data tile to be released)."""
 import argparse
 import ctypes as C
 import json
@@ -18,6 +19,8 @@ sys.path.insert(0, str(ROOT))
 LAYERS = {0: "contour", 1: "onset", 2: "note"}
 CONSUMER = ["wait_weight_stage", "mma", "epilogue", "wait_data_tile", "other"]
 PRODUCER = ["wait_free_stage", "wait_data_release", "other"]
+# the onset and note kernels gather their A operand and have no weight ring: the first consumer bucket is the gather
+CONSUMER_GATHER = ["gather"] + CONSUMER[1:]
 
 
 def build_clocks_lib(dst: Path) -> Path:
@@ -72,7 +75,8 @@ def main() -> None:
             c = [int(v) for v in cyc]
             cons, prod = c[:5], c[5:]
             res["layers"][name] = {
-                "consumer_share": {k: round(v / max(1, sum(cons)), 4) for k, v in zip(CONSUMER, cons)},
+                "consumer_share": {k: round(v / max(1, sum(cons)), 4)
+                                   for k, v in zip(CONSUMER if layer == 0 else CONSUMER_GATHER, cons)},
                 "producer_share": {k: round(v / max(1, sum(prod)), 4) for k, v in zip(PRODUCER, prod)},
                 "consumer_warp_cycles_per_step": sum(cons) // a.steps,
             }
