@@ -1486,11 +1486,24 @@ int bp_debug_tc_gather(int which, const float* w, int32_t* sizes, uint16_t* b1, 
   sizes[3] = g.wout;
   if (b1) {
     std::vector<uint16_t> m;
-    tc_build_b1(which, w, m);
+    tc_build_b1(which, w, m, true);
     std::memcpy(b1, m.data(), m.size() * 2);
   }
   if (starts) std::copy(g.starts.begin(), g.starts.end(), starts);
   if (ranges) std::copy(g.ranges.begin(), g.ranges.end(), ranges);
+  return BP_OK;
+}
+
+int bp_debug_tc_gather_packed(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* kmap) {
+  if (!w || !sizes || which < 1 || which > 2) return fail(BP_E_INVALID, "bp_debug_tc_gather_packed: bad argument");
+  const TcGatherGeom g = tc_gather_geometry(which);
+  sizes[0] = g.K_packed;
+  if (b1) {
+    std::vector<uint16_t> m;
+    tc_build_b1(which, w, m);
+    std::memcpy(b1, m.data(), m.size() * 2);
+  }
+  if (kmap) std::copy(g.kmap.begin(), g.kmap.end(), kmap);
   return BP_OK;
 }
 

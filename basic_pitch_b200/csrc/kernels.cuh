@@ -86,11 +86,14 @@ struct TcConvDev {
 int tc_upload_program(const TcConvPlan& contour_plan, cudaStream_t st);  // 0 on success
 // conv1 of the onset (epi 1, w = [32][8][5][5]) / note (epi 2, w = [32][1][7][7]) layer as the kernel gathers it: its two
 // B matrices [parity 2][plane hi/lo][K / 8][32][8] bf16, and the geometry of the gather (window start of every output
-// bin and channel, [wout][n_ci]; the bins [lo, hi) of every channel that hold input, [n_ci][2])
-void tc_build_b1(int epi, const float* w, std::vector<uint16_t>& out);
+// bin and channel, [wout][n_ci]; the bins [lo, hi) of every channel that hold input, [n_ci][2]).  window8: B in the
+// 8-bin-window form (K rows 8 (dt * n_ci + ci) + j) instead of the K order the kernel uses (kmap).
+void tc_build_b1(int epi, const float* w, std::vector<uint16_t>& out, bool window8 = false);
 struct TcGatherGeom {
-  int K, n_ci, KH, wout;
+  int K, n_ci, KH, wout;  // K of the 8-bin-window form
+  int K_packed;           // K the kernel runs
   std::vector<int> starts, ranges;
+  std::vector<int> kmap;  // [K_packed][3]: (dt, ci, window bin j) of every row of the kernel's B, -1 for padding
 };
 TcGatherGeom tc_gather_geometry(int epi);
 // bf16 hi/lo weight tiles of the fused second conv (epi: 0 contour, 1 onset, 2 note; w2 = that conv's weights), see TcB2

@@ -119,20 +119,49 @@ __host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour,
 
 // ------------------------------------------------------------------------------------------------
 // The gathered conv1 of the onset (EPI 1) and note (EPI 2) layers, 32 output channels at frequency stride 3 (see the
-// header).  K runs over (time tap dt, channel ci, 8-bin window j): k = 8 (dt * n_ci + ci) + j, padded to whole K = 16 steps.
-//   onset: 5 dt x 8 harmonics x 8 = 320 (20 steps, 62.5 % of the rows hold a tap); note: 7 dt x 1 x 8 = 56 -> 64 (4 steps)
+// header).  K runs over (time tap dt, channel ci, window bin j < W), padded to whole K = 16 steps (tc_gather_k):
+//   onset: 5 dt x 8 harmonics x 6 = 240 (15 steps, 83 % of the rows hold a tap): the window's first tap is at j = 0 or 1
+//          and KW = 5, so every tap lies in j < 6; k = 48 dt + 2 P + (j & 1) with the slot P of pair (ci, j / 2)
+//   note:  7 dt x 1 x 8 = 56 -> 64 (4 steps): k = 8 (dt * n_ci + ci) + j
 // ------------------------------------------------------------------------------------------------
 struct TcGather {
   int KH, KW, PL, n_ci;  // time / frequency taps, frequency pad, input channels (frequency stride 3, 32 output channels)
   int data_bins;         // bins of the input rows (the CQT, or the contour posteriorgram)
   int tile_bins;         // bins the data tile holds (8 x its chunks)
   int shifts[8];         // harmonic shift of every input channel
-  __host__ __device__ constexpr int ksteps() const { return (KH * n_ci * 8 + 15) / 16; }
+  int W;                 // window width in K: 8, or 6 where the KW taps fit 6 bins at either parity (onset, KW = 5)
+  // W = 6: K slot pair P of a time tap (k = 48 dt + 2 P + {0, 1}) -> bin pair 3 ci + jp of window ci.  Lane qd of a
+  // quad loads slot 4 e + qd of register word e; the order keeps the bank conflicts at their minimum (DESIGN §4.1)
+  int slot[24];
+  __host__ __device__ constexpr int ksteps() const { return (KH * n_ci * W + 15) / 16; }
 };
 __host__ __device__ constexpr TcGather tc_gather_spec(int epi) {  // epi 1 onset, 2 note (the geometry of tc_*_spec)
-  return epi == 1 ? TcGather{5, 5, 1, 8, kCqtBins, 312, {-36, 0, 36, 57, 72, 84, 93, 101}}
-                  : TcGather{7, 7, 2, 1, kContourBins, 264, {0, 0, 0, 0, 0, 0, 0, 0}};
+  return epi == 1 ? TcGather{5, 5, 1, 8, kCqtBins, 312, {-36, 0, 36, 57, 72, 84, 93, 101}, 6,
+                             {9, 10, 21, 22, 14, 4, 2, 1, 16, 3, 6, 13, 5, 17, 18, 20, 19, 23, 7, 0, 8, 15, 12, 11}}
+                  : TcGather{7, 7, 2, 1, kContourBins, 264, {0, 0, 0, 0, 0, 0, 0, 0}, 8, {}};
 }
+// row k of B for time tap dt, channel ci, window bin j
+__host__ __device__ constexpr int tc_gather_k(TcGather g, int dt, int ci, int j) {
+  if (g.W == 8) return 8 * (dt * g.n_ci + ci) + j;
+  int P = 0;
+  while (g.slot[P] != 3 * ci + j / 2) ++P;
+  return g.n_ci * g.W * dt + 2 * P + (j & 1);
+}
+__host__ __device__ constexpr bool tc_gather_slots_ok(TcGather g) {  // W = 6: the slots are a permutation of the pairs
+  if (g.W == 8) return true;
+  if (g.W != 6 || g.n_ci != 8) return false;
+  for (int p = 0; p < 24; ++p) {
+    int n = 0;
+    for (int P = 0; P < 24; ++P) n += g.slot[P] == p;
+    if (n != 1) return false;
+  }
+  return true;
+}
+// W = 6: shift of the channel, and bin pair in its window, that K slot P holds
+__host__ __device__ constexpr int tc_gather_slot_shift(TcGather g, int P) { return g.shifts[g.slot[P] / 3]; }
+__host__ __device__ constexpr int tc_gather_slot_pair(TcGather g, int P) { return g.slot[P] % 3; }
+static_assert(tc_gather_slots_ok(tc_gather_spec(1)) && tc_gather_slots_ok(tc_gather_spec(2)), "K slot map of the gather");
+static_assert(tc_gather_spec(1).ksteps() == 15 && tc_gather_spec(2).ksteps() == 4, "K-steps per output bin");
 // first bin of the 8-bin window of output bin f, channel ci: the even bin at or below its first tap
 __host__ __device__ constexpr int tc_gather_start(TcGather g, int f, int ci) { return (3 * f - g.PL + g.shifts[ci]) & ~1; }
 // the bins u of channel ci that hold input: inside the row (u < data_bins) and inside the stacked image
@@ -414,17 +443,19 @@ int tc_upload_program(const TcConvPlan& pl, cudaStream_t st) {
 
 // The two conv1 B matrices of the onset / note layer, f even and f odd (TcGather), in the layout the MMAs read:
 // [parity 2][plane hi/lo][k-chunk K / 8][n 32][8] bf16 (K-major no-swizzle: LBO = 32 * 16 B, SBO = 128 B).
-// B_p[8 (dt * n_ci + ci) + j][co] = W[co][ci][dt][j - o], o = the first tap's offset in its window for f & 1 = p.
-void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<uint16_t>& out) {
+// B_p[tc_gather_k(dt, ci, j)][co] = W[co][ci][dt][j - o], o = the first tap's offset in its window for f & 1 = p.
+// window8: the same weights in the 8-bin-window form k = 8 (dt * n_ci + ci) + j, whatever W (bp_debug_tc_gather).
+void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<uint16_t>& out, bool window8) {
   const TcGather g = tc_gather_spec(epi);
-  const size_t plane = (size_t)16 * g.ksteps() * 32;
+  const int wn = window8 ? 8 : g.W;
+  const size_t plane = (size_t)16 * ((g.KH * g.n_ci * wn + 15) / 16) * 32;
   out.assign(4 * plane, 0);
   for (int p = 0; p < 2; ++p)
     for (int dt = 0; dt < g.KH; ++dt)
       for (int ci = 0; ci < g.n_ci; ++ci) {
         const int o = 3 * p - g.PL + g.shifts[ci] - tc_gather_start(g, p, ci);
-        for (int j = 0; j < 8; ++j) {
-          const int df = j - o, k = 8 * (dt * g.n_ci + ci) + j;
+        for (int j = 0; j < wn; ++j) {
+          const int df = j - o, k = window8 ? 8 * (dt * g.n_ci + ci) + j : tc_gather_k(g, dt, ci, j);
           if (df < 0 || df >= g.KW) continue;
           for (int co = 0; co < 32; ++co) {
             const float w = W[((co * g.n_ci + ci) * g.KH + dt) * g.KW + df];
@@ -440,7 +471,16 @@ void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<u
 TcGatherGeom tc_gather_geometry(int epi) {
   const TcGather g = tc_gather_spec(epi);
   TcGatherGeom r;
-  r.K = 16 * g.ksteps();
+  r.K = 16 * ((g.KH * g.n_ci * 8 + 15) / 16);  // of the 8-bin-window form
+  r.K_packed = 16 * g.ksteps();
+  for (int k = 0; k < r.K_packed; ++k) {  // which (dt, ci, j) the kernel puts at row k (-1: K padding)
+    int hit[3] = {-1, -1, -1};
+    for (int dt = 0; dt < g.KH; ++dt)
+      for (int ci = 0; ci < g.n_ci; ++ci)
+        for (int j = 0; j < g.W; ++j)
+          if (tc_gather_k(g, dt, ci, j) == k) hit[0] = dt, hit[1] = ci, hit[2] = j;
+    r.kmap.insert(r.kmap.end(), hit, hit + 3);
+  }
   r.n_ci = g.n_ci;
   r.KH = g.KH;
   r.wout = kPitches;
@@ -796,44 +836,70 @@ __device__ __forceinline__ void conv2_mma(float (&p)[NW / 2], const uint32_t (&a
 
 // conv1 of frequency tile ft of the onset / note layer (EPI 1 / 2), gathered (see the header): for each bin f = 4 ft + fl
 // the K-steps of TcGather, three split products m64n32k16 each, into acc[16 fl ..] (= columns 32 fl .. of the m64n128
-// fragment).  The A registers of the next step are loaded while the current step's MMAs run (two register buffers).
+// fragment).  The A registers are loaded two steps ahead of the MMAs that read them (three register buffers, gather_steps).
 // Every output sums its steps in the same order whatever the item: a value depends only on f and the layer.
 template <int EPI>
 struct GatherRegs {
   static constexpr TcGather G = tc_gather_spec(EPI);
-  // per channel: byte offset of the thread's bin pair (row fr0) in the data tile in bits [0, 24), and in bits 24 / 25
-  // whether its first / second bf16 half holds input (one register per channel keeps the consumers within budget)
-  uint32_t om[G.n_ci];
-  // the window of output bin f for the thread (lane qd of its quad, rows fr0 / fr0 + 8)
+  static_assert(G.W == 8 || (G.W == 6 && G.n_ci * G.W == 48), "W = 6: a time tap is 3 whole K-steps, 6 register words");
+  // per register word (W = 8: per channel; W = 6: per slot group e, lane qd loads slot 4 e + qd): byte offset of the
+  // thread's bin pair (row fr0) in the data tile in bits [0, 24), and in bits 24 / 25 whether its first / second bf16
+  // half holds input (one register per word keeps the consumers within budget)
+  static constexpr int NWD = G.W == 8 ? G.n_ci : 6;
+  uint32_t om[NWD];
+  __device__ __forceinline__ static uint32_t word(int u, int lo, int hi, int fr0) {
+    const int uc = min(max(u, 0), G.tile_bins - 2);  // a pair outside the tile is masked; read one inside it
+    return (uint32_t)((uc >> 3) * ((tc::kMTile + G.KH - 1) * 16) + (uc & 7) * 2 + fr0 * 16) |
+           (u >= lo && u < hi ? 1u << 24 : 0u) | (u + 1 >= lo && u + 1 < hi ? 1u << 25 : 0u);
+  }
+  // the windows of output bin f for the thread (lane qd of its quad, rows fr0 / fr0 + 8)
   __device__ __forceinline__ void setup(int f, int fr0, int qd) {
+    if constexpr (G.W == 8) {
 #pragma unroll
-    for (int ci = 0; ci < G.n_ci; ++ci) {
-      const int u = tc_gather_start(G, f, ci) + 2 * qd;
-      const int lo = tc_gather_lo(G, ci), hi = tc_gather_hi(G, ci);
-      const int uc = min(max(u, 0), G.tile_bins - 2);  // a pair outside the tile is masked; read one inside it
-      om[ci] = (uint32_t)((uc >> 3) * ((tc::kMTile + G.KH - 1) * 16) + (uc & 7) * 2 + fr0 * 16) |
-               (u >= lo && u < hi ? 1u << 24 : 0u) | (u + 1 >= lo && u + 1 < hi ? 1u << 25 : 0u);
+      for (int ci = 0; ci < G.n_ci; ++ci)
+        om[ci] = word(tc_gather_start(G, f, ci) + 2 * qd, tc_gather_lo(G, ci), tc_gather_hi(G, ci), fr0);
+    } else {
+      setup_word<0>(f, fr0, qd);
+      setup_word<1>(f, fr0, qd);
+      setup_word<2>(f, fr0, qd);
+      setup_word<3>(f, fr0, qd);
+      setup_word<4>(f, fr0, qd);
+      setup_word<5>(f, fr0, qd);
     }
   }
-  __device__ __forceinline__ uint32_t mask(int ci) const {  // bits 24 / 25 -> 0x0000ffff / 0xffff0000
-    const uint32_t m = om[ci] >> 24;
+  // W = 6: word e = the lane's slot 4 e + qd, bin pair jp of the window of the channel with shift sh (immediates picked
+  // by qd, so that the spec's tables are not indexed at run time)
+  template <int E>
+  __device__ __forceinline__ void setup_word(int f, int fr0, int qd) {
+    constexpr int s0 = tc_gather_slot_shift(G, 4 * E), s1 = tc_gather_slot_shift(G, 4 * E + 1),
+                  s2 = tc_gather_slot_shift(G, 4 * E + 2), s3 = tc_gather_slot_shift(G, 4 * E + 3);
+    constexpr int j0 = tc_gather_slot_pair(G, 4 * E), j1 = tc_gather_slot_pair(G, 4 * E + 1),
+                  j2 = tc_gather_slot_pair(G, 4 * E + 2), j3 = tc_gather_slot_pair(G, 4 * E + 3);
+    const int sh = qd == 0 ? s0 : qd == 1 ? s1 : qd == 2 ? s2 : s3;
+    const int jp = qd == 0 ? j0 : qd == 1 ? j1 : qd == 2 ? j2 : j3;
+    const int u = ((3 * f - G.PL + sh) & ~1) + 2 * jp;  // tc_gather_start + 2 jp
+    om[E] = word(u, sh > 0 ? sh : 0, G.data_bins < kContourBins + sh ? G.data_bins : kContourBins + sh, fr0);
+  }
+  __device__ __forceinline__ uint32_t mask(int i) const {  // bits 24 / 25 -> 0x0000ffff / 0xffff0000
+    const uint32_t m = om[i] >> 24;
     return ((m | (m << 15)) & 0x10001u) * 0xffffu;
   }
-  // the A registers of K-step ks, x[0..3] hi, x[4..7] lo: (window 2 ks, row fr0), (2 ks, fr0 + 8), (2 ks + 1, fr0),
-  // (2 ks + 1, fr0 + 8)
+  // the A registers of K-step ks, x[0..3] hi, x[4..7] lo: (half 0, row fr0), (half 0, fr0 + 8), (half 1, fr0),
+  // (half 1, fr0 + 8).  W = 8: half h is window 2 ks + h; W = 6: time tap ks / 3, word 2 (ks % 3) + h
   template <int KS>
   __device__ __forceinline__ void load(const unsigned char* s_data, uint32_t (&x)[8]) const {
     constexpr int kPlane = G.tile_bins / 8 * (tc::kMTile + G.KH - 1) * 16;  // bytes of one plane of the data tile
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      constexpr int NW = G.KH * G.n_ci;  // 8-bin windows holding taps; the rest of the last step is K padding
-      const int wi = 2 * KS + h, dt = wi / G.n_ci, ci = wi % G.n_ci;
+      constexpr int NW = G.W == 8 ? G.KH * G.n_ci : 2 * G.ksteps();  // halves holding taps; the rest is K padding
+      const int wi = 2 * KS + h;
+      const int dt = G.W == 8 ? wi / G.n_ci : KS / 3, i = G.W == 8 ? wi % G.n_ci : 2 * (KS % 3) + h;
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         if (wi < NW) {
-          const unsigned char* p = s_data + (om[ci] & 0xffffffu) + dt * 16 + rr * 128;
-          x[2 * h + rr] = *reinterpret_cast<const uint32_t*>(p) & mask(ci);
-          x[4 + 2 * h + rr] = *reinterpret_cast<const uint32_t*>(p + kPlane) & mask(ci);
+          const unsigned char* p = s_data + (om[i] & 0xffffffu) + dt * 16 + rr * 128;
+          x[2 * h + rr] = *reinterpret_cast<const uint32_t*>(p) & mask(i);
+          x[4 + 2 * h + rr] = *reinterpret_cast<const uint32_t*>(p + kPlane) & mask(i);
         } else {
           x[2 * h + rr] = 0u;
           x[4 + 2 * h + rr] = 0u;
@@ -843,8 +909,11 @@ struct GatherRegs {
   }
 };
 
+// Step I of the tile (bin fl = I / KS, K-step I % KS) reads register buffer I % 3.  Once its MMAs are committed and those
+// of step I - 1 have completed, buffer (I - 1) % 3 = (I + 2) % 3 takes step I + 2: the registers of step I + 1 were
+// loaded a whole step earlier, so their shared-memory latency is hidden behind the MMAs of two steps, not one.
 template <int EPI, int I>
-__device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& gr, uint32_t (&x)[2][8], const unsigned char* s_data,
+__device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& gr, uint32_t (&x)[3][8], const unsigned char* s_data,
                                              uint64_t d0, int ft, int fr0, int qd, TcClocks& clk) {
   using namespace tc;
   constexpr int KS = tc_gather_spec(EPI).ksteps(), NST = 4 * KS;
@@ -853,32 +922,35 @@ __device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& 
   float(&d)[16] = *reinterpret_cast<float(*)[16]>(acc + 16 * fl);
   // B_{f & 1}, K-step ks (f & 1 = fl & 1: a tile starts on an even bin)
   const uint64_t bh = d0 + (uint64_t)(((fl & 1) * 2 * kB1Plane + ks * 2 * 32 * 16) >> 4), bl = bh + (kB1Plane >> 4);
-  const uint32_t xh[4] = {x[I & 1][0], x[I & 1][1], x[I & 1][2], x[I & 1][3]};
-  const uint32_t xl[4] = {x[I & 1][4], x[I & 1][5], x[I & 1][6], x[I & 1][7]};
+  const uint32_t xh[4] = {x[I % 3][0], x[I % 3][1], x[I % 3][2], x[I % 3][3]};
+  const uint32_t xl[4] = {x[I % 3][4], x[I % 3][5], x[I % 3][6], x[I % 3][7]};
   wgmma_fence();
   wgmma_rs_n32(d, xh, bh, ks ? 1u : 0u);
   wgmma_rs_n32(d, xh, bl, 1u);
   wgmma_rs_n32(d, xl, bh, 1u);
   wgmma_commit();
-  if constexpr (I + 1 < NST) {
+  if constexpr (I + 2 < NST) {
     wgmma_wait<1>();  // the previous step's MMAs are done: its A registers may be refilled
     clk.lap(kClkMma);
-    if constexpr ((I + 1) % KS == 0) gr.setup(4 * ft + (I + 1) / KS, fr0, qd);
-    gr.template load<(I + 1) % KS>(s_data, x[(I + 1) & 1]);
+    // the window offsets follow the bin being LOADED (step I + 2); step I + 1's registers are already in place
+    if constexpr ((I + 2) % KS == 0) gr.setup(4 * ft + (I + 2) / KS, fr0, qd);
+    gr.template load<(I + 2) % KS>(s_data, x[(I + 2) % 3]);
     clk.lap(kClkFull);
-    gather_steps<EPI, I + 1>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
   }
+  if constexpr (I + 1 < NST) gather_steps<EPI, I + 1>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
 }
 
 template <int EPI>
 __device__ __forceinline__ void gather_conv1(float (&acc)[64], const unsigned char* s_data, uint32_t b1, int ft, int fr0, int qd,
                                              TcClocks& clk) {
   using namespace tc;
+  static_assert(tc_gather_spec(EPI).ksteps() >= 2, "the first two K-steps are loaded up front, of the same bin");
   GatherRegs<EPI> gr;
   const uint64_t d0 = make_desc(b1, 32 * 16, 128);
-  uint32_t x[2][8];
+  uint32_t x[3][8];
   gr.setup(4 * ft, fr0, qd);
   gr.template load<0>(s_data, x[0]);
+  gr.template load<1>(s_data, x[1]);
   clk.lap(kClkFull);
   gather_steps<EPI, 0>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
   wgmma_wait<0>();
@@ -1000,13 +1072,6 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     const int slot = warp >> 2, wq = warp & 3, gq = lane >> 2, qd = lane & 3;
     const int tid = threadIdx.x & 127;
     const int fr0 = 16 * wq + gq;  // first of the thread's two fragment rows (the other is fr0 + 8)
-    // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is 2 qd + e (COUT 8) or
-    // 8 (i % 4) + 2 qd + e (COUT 32)
-    float bz[4][2];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[EPI == 0 || EPI == 3 ? 2 * qd + e : 8 * i + 2 * qd + e];
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;  // n_fill: index of the current step's weight fill in the CTA
     const uint32_t a_hi = smem_u32(s_data), a_lo = a_hi + plane_bytes, w_base = smem_u32(s_w);
     const uint32_t* prog = c_prog[slot];
@@ -1127,6 +1192,13 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         const bool first = (g == g0);
         const bool last = (g == g1 - 1) || (ft == a.n_ft - 1);
         const int n_valid = min(a.flt, a.wout - ft * a.flt) * a.cout;  // a multiple of 32 (contour: 64 in the last tile)
+        // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is 2 qd + e (COUT 8) or
+        // 8 (i % 4) + 2 qd + e (COUT 32).  Read here, after the conv1 MMAs, so that it holds no registers during the gather.
+        float bz[4][2];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[EPI == 0 || EPI == 3 ? 2 * qd + e : 8 * i + 2 * qd + e];
         if constexpr (EPI == 0) {
           // contour: 16 bins x 8 channels, bias + ReLU, channels-last rows of 128 contiguous floats
 #pragma unroll

@@ -251,9 +251,14 @@ int bp_debug_tc_plan(int which, const float* w, int32_t* sizes, uint16_t* tiles,
 /* Host-only: the conv1 of the onset (which = 1, w = [32][8][5][5]) or note (which = 2, w = [32][1][7][7]) layer as the
  * kernel computes it, an implicit GEMM with a gathered A operand (csrc/tc_conv.cu, TcGather).  sizes[4] = {K, n_ci, KH,
  * wout}; b1 (may be NULL): the two B matrices, [parity of the output bin 2][plane hi/lo][K / 8][32][8] bf16, row
- * k = 8 (dt * n_ci + ci) + j; starts (may be NULL): [wout][n_ci] first input bin of the 8-bin window of output bin f and
- * channel ci; ranges (may be NULL): [n_ci][2] the input bins [lo, hi) of each channel that hold data (zero elsewhere). */
+ * k = 8 (dt * n_ci + ci) + j (the 8-bin-window form; the kernel's own K order is bp_debug_tc_gather_packed); starts (may
+ * be NULL): [wout][n_ci] first input bin of the window of output bin f and channel ci; ranges (may be NULL): [n_ci][2]
+ * the input bins [lo, hi) of each channel that hold data (zero elsewhere). */
 int bp_debug_tc_gather(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* starts, int32_t* ranges);
+/* Host-only: the same B matrices in the K order the kernel runs (the onset packs its windows to 6 bins).  sizes[1] = {K};
+ * b1 (may be NULL): [2][2][K / 8][32][8] bf16; kmap (may be NULL): [K][3] the (dt, ci, window bin j) of row k, all -1
+ * for K padding.  Window starts and ranges are those of bp_debug_tc_gather. */
+int bp_debug_tc_gather_packed(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* kmap);
 
 /* Host-only: the bf16 hi/lo weight tiles of the fused SECOND convolution of a tensor-core layer (csrc/tc_conv.cu, TcB2):
  * which = 0 contour conv2 (w2 = [1][8][5][5], reference models.py:254-262), 1 onset conv2 ([1][33][3][3], models.py:305-313),
