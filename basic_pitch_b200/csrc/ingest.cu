@@ -74,14 +74,62 @@ __device__ __forceinline__ float to_float<int>(int v) { return (float)v / 214748
 template <>
 __device__ __forceinline__ float to_float<unsigned char>(unsigned char v) { return ((float)v - 128.f) / 128.f; }
 
-// mono sample i of the interleaved PCM: numpy's float32 mean over the channel axis (sequential sum, then / channels)
+// numpy's pairwise_sum of n >= 1 converted values: below 8 a sequential sum from +0, up to 128 eight interleaved
+// accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) then the tail in order
+template <typename T>
+__device__ __forceinline__ float pairwise_block(const T* p, int n) {
+  if (n < 8) {
+    float s = 0.f;
+    for (int c = 0; c < n; ++c) s = __fadd_rn(s, to_float<T>(p[c]));
+    return s;
+  }
+  float r[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) r[j] = to_float<T>(p[j]);
+  int c = 8;
+  for (; c + 8 <= n; c += 8)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], to_float<T>(p[c + j]));
+  float s = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
+                      __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
+  for (; c < n; ++c) s = __fadd_rn(s, to_float<T>(p[c]));
+  return s;
+}
+
+// above 128 numpy splits at n2 = n / 2 - (n / 2) % 8 and adds the two halves' sums; walked here in post-order with an
+// explicit stack.  A split leaves at most n / 2 + 7, so any int count takes at most 24 (65 535 channels, the most a WAV
+// file can have, 9)
+template <typename T>
+__device__ float pairwise_sum(const T* p, int n) {
+  constexpr int kDepth = 32;
+  int right_off[kDepth], right_n[kDepth];
+  float left[kDepth];
+  bool left_done[kDepth];
+  int sp = 0, off = 0;
+  for (;;) {
+    while (n > 128) {  // descend into the left half, remember the right one
+      const int n2 = n / 2 - (n / 2) % 8;
+      right_off[sp] = off + n2, right_n[sp] = n - n2, left_done[sp] = false;
+      ++sp;
+      n = n2;
+    }
+    float v = pairwise_block<T>(p + off, n);
+    while (sp > 0 && left_done[sp - 1]) v = __fadd_rn(left[--sp], v);  // both halves done: combine and climb
+    if (sp == 0) return v;
+    left[sp - 1] = v, left_done[sp - 1] = true;
+    off = right_off[sp - 1], n = right_n[sp - 1];
+  }
+}
+
+// mono sample i of the interleaved PCM: numpy's float32 mean over the channel axis, `x.mean(axis=1, dtype=float32)`:
+// +0 plus the pairwise sum (a frame of -0 gives +0), divided by the integer count in float64 and rounded to float32
+// (the same as a float32 division while the count is exact in float32, i.e. up to 2^24 channels)
 template <typename T>
 __device__ __forceinline__ float mono_sample(const T* pcm, long long i, int channels) {
   const T* p = pcm + i * channels;
   if (channels == 1) return to_float<T>(p[0]);
-  float s = to_float<T>(p[0]);
-  for (int c = 1; c < channels; ++c) s = __fadd_rn(s, to_float<T>(p[c]));
-  return __fdiv_rn(s, (float)channels);
+  const float s = channels <= 128 ? pairwise_block<T>(p, channels) : pairwise_sum<T>(p, channels);
+  return __double2float_rn(__ddiv_rn((double)__fadd_rn(0.f, s), (double)channels));
 }
 
 template <typename T>

@@ -198,8 +198,12 @@ void bp_last_required(int64_t* note_capacity, int64_t* bend_capacity);
 /* Audio ingest — `librosa.load(path, sr=22050, mono=True)` minus the container decode (reference:
  * basic_pitch/inference.py:239): interleaved PCM frames of `channels` channels at `sample_rate` Hz -> mono float32 at
  * 22 050 Hz.  sample_format: 0 float32, 1 int16 (/ 2^15), 2 int32 (/ 2^31; 24-bit WAV left-justified), 3 uint8
- * ((x - 128) / 128).  Channels are averaged in float32; other rates go through a Kaiser-windowed polyphase FIR (pass
- * band 0.913 x Nyquist of the lower rate, 125 dB stop band) applied like scipy.signal.resample_poly.  The output has
+ * ((x - 128) / 128).  Channels are averaged in float32 in NumPy's order (`x.mean(axis=1, dtype=np.float32)`), so at
+ * 22 050 Hz the output is the host loader's (basic_pitch_b200/audio_io.py) bit for bit; other rates go through a
+ * Kaiser-windowed polyphase FIR (pass band 0.913 x Nyquist of the lower rate, 125 dB stop band) applied like
+ * scipy.signal.resample_poly, each output within a per-element float32-accumulation bound of the float64 result
+ * (DESIGN.md §4.4).  Rates needing more than 200 KB of staged input per 256 outputs (ratios beyond ~100:1, e.g.
+ * 2 822 400 Hz) return BP_E_INVALID, as do formats outside 0..3 and channels or sample_rate below 1.  The output has
  * bp_resampled_length(n_frames, sample_rate) = ceil(n_frames * 22050 / sample_rate) samples.
  * _device: PCM and output in device memory, asynchronous on `stream` — the output can feed bp_transcribe_device directly;
  * _host: both in host memory (the PCM crosses PCIe as stored: 2 bytes per sample for 16-bit audio). */

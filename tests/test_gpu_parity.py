@@ -583,56 +583,6 @@ def test_transcribe_files_host_equals_packed_entry_point(model):
 
 
 @pytest.mark.gpu
-def test_device_ingest_matches_host_loader(model, tmp_path):
-    """csrc/ingest.cu (sample conversion + channel mean + polyphase resampler on the GPU, `load_audio_device`) against the
-    host loader (`audio_io.load_audio`: NumPy + scipy.signal.resample_poly in float64) on WAV files of several formats."""
-    from scipy.io import wavfile
-
-    from basic_pitch_b200 import audio_io
-
-    rng = np.random.default_rng(11)
-    cases = [
-        (44100, np.int16, 2, 70001), (48000, np.float32, 1, 50000), (16000, np.uint8, 1, 30011), (22050, np.int16, 2, 9999),
-        (96000, np.int32, 2, 123457), (8000, np.int16, 1, 4000), (11025, np.float32, 3, 2048), (44100, np.int16, 1, 300),
-    ]  # fmt: skip
-    for i, (sr, dt, ch, n) in enumerate(cases):
-        t = np.arange(n) / sr
-        x = 0.4 * np.sin(2 * np.pi * 220.0 * t)[:, None] * np.linspace(1.0, 0.5, ch)[None, :] + 0.05 * rng.standard_normal((n, ch))
-        if dt == np.float32:
-            pcm = x.astype(np.float32)
-        elif dt == np.uint8:
-            pcm = np.clip(np.round(x * 127 + 128), 0, 255).astype(np.uint8)
-        else:
-            pcm = np.clip(np.round(x * (2.0 ** (8 * np.dtype(dt).itemsize - 1) - 1)), -(2.0 ** 31), 2.0 ** 31 - 1).astype(dt)
-        if ch == 1:
-            pcm = pcm[:, 0]
-        path = tmp_path / f"c{i}.wav"
-        wavfile.write(path, sr, pcm)
-        ref, _ = audio_io.load_audio(path)
-        got, sr_out = audio_io.load_audio_device(path, model)
-        assert sr_out == 22050 and got.dtype == np.float32 and got.shape == ref.shape, (sr, dt, ch, got.shape, ref.shape)
-        err = float(np.abs(got - ref).max()) if len(ref) else 0.0
-        assert err < 3e-6, (sr, dt, ch, n, err)  # fp32 accumulation of ~400 taps vs float64
-
-
-@pytest.mark.gpu
-def test_device_ingest_vocadito_44k_vs_golden(model, golden_dir):
-    """The reference's 44.1 kHz test clip through the device ingest and the model against the reference's golden
-    posteriorgrams (reference: tests/test_inference.py:43-70; tolerance = the resampler residual, tests/golden/README.md)."""
-    z = np.load(golden_dir / "vocadito10_pcm44k.npz")
-    pcm, sr = z["pcm"], int(z["sample_rate"])
-    lib = model._lib
-    audio = np.empty(int(lib.bp_resampled_length(len(pcm), sr)), np.float32)
-    lib.bp_load_pcm_host(model.handle, pcm.ctypes.data, 1, len(pcm), 1, sr, audio.ctypes.data)
-    gold = np.load(golden_dir / "vocadito10.npz")
-    assert np.abs(audio - gold["audio22k"]).max() < 3e-6  # the host resampler of the fixture
-    out = model.run_inference_arrays([audio])[0]
-    for k in ("note", "onset", "contour"):
-        assert out[k].shape == gold[f"gold_{k}"].shape
-        assert float(np.abs(out[k] - gold[f"gold_{k}"]).max()) < GOLD_TOL, k
-
-
-@pytest.mark.gpu
 def test_streaming_mode_equals_whole_file(model):
     """Bounded-memory mode: run_inference_stream / predict_stream on a 70 s recording delivered in odd-sized blocks give
     the posteriorgrams of the whole-file call bit for bit, and the same note events."""

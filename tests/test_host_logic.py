@@ -275,20 +275,30 @@ def test_window_audio_file_and_get_audio_input_like_the_reference_tests(golden_d
 
 def test_ingest_filter_and_length_match_scipy():
     """The device resampler (csrc/ingest.cu) designs its Kaiser low-pass itself: same taps as audio_io._resample_filter
-    (scipy.signal.kaiserord + firwin) and the output length of scipy.signal.resample_poly."""
+    (scipy.signal.kaiserord + firwin) and the output length of scipy.signal.resample_poly, at every rate the device
+    ingest tests use (tests/test_gpu_ingest.py), the coprime 44 101 Hz (an 8.27 M-tap filter) included.
+
+    The taps scale as 1 / max(up, down), so the tolerance is also relative to max|h|: the absolute 1e-14 alone would
+    loosen by four orders of magnitude from 11 025 Hz to 44 101 Hz.  The two designs differ by the rounding of
+    sin(pi x) for arguments up to ~90 and of the normalising sum over up to 8.27 M taps: at most 1.8e-13 max|h| (at
+    44 101 Hz) and 3.1e-16 absolute."""
     import scipy.signal
 
     from basic_pitch_b200 import _lib, audio_io
 
     lib = _lib.load()
-    for up, down in ((1, 2), (147, 320), (441, 160), (147, 640)):
+    for sr in (4000, 8000, 11025, 16000, 24000, 32000, 44100, 44101, 48000, 88200, 96000, 192000, 352800, 705600,
+               1411200):
+        g = np.gcd(22050, sr)
+        up, down = 22050 // g, sr // g
         ref = audio_io._resample_filter(up, down)
         n = int(lib.bp_debug_resample_filter(up, down, None, 0))
-        assert n == len(ref)
+        assert n == len(ref), sr
         h = np.zeros(n)
         lib.bp_debug_resample_filter(up, down, h.ctypes.data, n)
-        assert np.abs(h - ref).max() < 1e-14
-    for sr, n in ((44100, 401214), (48000, 12345), (16000, 777), (8000, 1), (22050, 99), (96000, 100001)):
+        assert np.abs(h - ref).max() <= min(1e-14, 1e-12 * np.abs(ref).max()), sr
+    for sr, n in ((44100, 401214), (48000, 12345), (16000, 777), (8000, 1), (22050, 99), (96000, 100001), (44101, 1),
+                  (44101, 88203), (4000, 3), (1411200, 12345)):
         g = np.gcd(22050, sr)
         ref_len = len(scipy.signal.resample_poly(np.zeros(n), 22050 // g, sr // g)) if sr != 22050 else n
         assert int(lib.bp_resampled_length(n, sr)) == ref_len
