@@ -148,7 +148,7 @@ struct bp_model {
     TcConvPlan plan;
     TcConvDev dev{};
     DevBuf<uint16_t> tiles, b1, b2;  // tiles: contour only; b1: onset / note only
-  } tc_contour, tc_onset, tc_note;
+  } tc[3];                           // by layer: 0 contour, 1 onset, 2 note (tc_spec)
   DevBuf<__nv_bfloat16> yhl, chl;
   Lowpass2 lp2{};  // decimation FIR taps, a parameter of every decimation launch
   DevBuf<uint16_t> cqt_wtc;  // three-way bf16 split of the CQT kernel matrix (tensor-core path)
@@ -282,43 +282,40 @@ int derive(bp_model* m, cudaStream_t st) {
   CK(cudaMemcpyAsync(hp.data(), m->d_params, sizeof(float) * ParamLayout::total, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   m->lp2 = lowpass_pairs(hp.data() + ParamLayout::lowpass);
-  const TcConvSpec specs[3] = {tc_contour_spec(), tc_onset_spec(), tc_note_spec()};
-  bp_model::TcLayer* layers[3] = {&m->tc_contour, &m->tc_onset, &m->tc_note};
-  const float* wsrc[3] = {hp.data() + ParamLayout::contour1_w, hp.data() + ParamLayout::onset1_w,
-                          hp.data() + ParamLayout::note1_w};
-  const float* w2src[3] = {hp.data() + ParamLayout::contour2_w, hp.data() + ParamLayout::onset2_w,
-                           hp.data() + ParamLayout::note2_w};
-  const float* b1src[3] = {hp.data() + ParamLayout::contour1_b, hp.data() + ParamLayout::onset1_b,
-                           hp.data() + ParamLayout::note1_b};
-  const float* b2src[3] = {hp.data() + ParamLayout::contour2_b, hp.data() + ParamLayout::onset2_b,
-                           hp.data() + ParamLayout::note2_b};
+  // where each layer's conv1 / conv2 weights and biases sit in the parameter block
+  struct TcParams {
+    int w1, b1, w2, b2;
+  };
+  static constexpr TcParams params[3] = {
+      {ParamLayout::contour1_w, ParamLayout::contour1_b, ParamLayout::contour2_w, ParamLayout::contour2_b},
+      {ParamLayout::onset1_w, ParamLayout::onset1_b, ParamLayout::onset2_w, ParamLayout::onset2_b},
+      {ParamLayout::note1_w, ParamLayout::note1_b, ParamLayout::note2_w, ParamLayout::note2_b}};
   for (int l = 0; l < 3; ++l) {
-    bp_model::TcLayer& L = *layers[l];
-    int n_groups = specs[l].G0;
+    bp_model::TcLayer& L = m->tc[l];
+    const float* w1 = hp.data() + params[l].w1;
     if (l == 0) {  // the contour conv: Toeplitz weight tiles + the MMA program
-      L.plan.build(specs[l], wsrc[l]);
+      L.plan.build(tc_spec(l), w1);
       const TcConvPlan& pl = L.plan;
       if (tc_upload_program(pl, st) != 0)
         return fail(BP_E_INVALID, "tensor-core program does not fit its constant-memory area");
       CK(L.tiles.reserve(pl.tiles.size()));
       CK(cudaMemcpyAsync(L.tiles.p, pl.tiles.data(), pl.tiles.size() * 2, cudaMemcpyHostToDevice, st));
-      n_groups = pl.n_groups;
     } else {  // onset / note: the two B matrices of the gathered conv1
       std::vector<uint16_t> b1;
-      tc_build_b1(l, wsrc[l], b1);
+      tc_build_b1(l, w1, b1);
       CK(L.b1.reserve(b1.size()));
       CK(cudaMemcpyAsync(L.b1.p, b1.data(), b1.size() * 2, cudaMemcpyHostToDevice, st));
     }
     CK(cudaStreamSynchronize(st));
     std::vector<uint16_t> b2;
-    tc_build_b2_full(l, w2src[l], b2);
+    tc_build_b2_full(l, hp.data() + params[l].w2, b2);
     CK(L.b2.reserve(b2.size()));
     CK(cudaMemcpyAsync(L.b2.p, b2.data(), b2.size() * 2, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
-    L.dev = TcConvDev{specs[l], L.tiles.p, L.b1.p, L.b2.p, n_groups, l};
-    std::copy_n(b1src[l], specs[l].COUT, L.dev.bias1);
-    L.dev.bias2 = *b2src[l];
-    if (l == 1) std::copy_n(hp.data() + ParamLayout::onset2_w, 9, L.dev.note_w);  // channel 0: the note input
+    L.dev = TcConvDev{l, L.tiles.p, L.b1.p, L.b2.p};
+    std::copy_n(hp.data() + params[l].b1, tc_spec(l).COUT, L.dev.bias1);
+    L.dev.bias2 = hp[params[l].b2];
+    if (l == 1) std::copy_n(hp.data() + params[l].w2, 9, L.dev.note_w);  // channel 0: the note input
   }
   {
     std::vector<uint16_t> wtc;
@@ -346,12 +343,13 @@ int ensure_forward_ws(bp_model* m, int nb) {
     CK(m->i_onset.reserve(kPitches * fr));
     if (m->path == 1) CK(m->i_contour.reserve((size_t)kContourBins * fr));
   }
-  CK(m->edge.reserve(std::max({tc_edge_floats(tc_contour_spec(), nb), tc_edge_floats(tc_onset_spec(), nb),
-                               tc_edge_floats(tc_note_spec(), nb)})));
+  CK(m->edge.reserve(std::max({tc_edge_floats(tc_spec(0), nb), tc_edge_floats(tc_spec(1), nb),
+                               tc_edge_floats(tc_spec(2), nb)})));
   // split layouts use the row stride of a full chunk whatever the batch size (see launch_conv_tc)
-  CK(m->yhl.reserve((size_t)2 * 40 * 8 * tc_rows_total(m->chunk, tc_contour_spec().rows_per_window)));
+  constexpr TcConvSpec cs = tc_spec(0);
+  CK(m->yhl.reserve((size_t)2 * cs.chunks8 * 8 * tc_rows_total(m->chunk, cs.rows_per_window)));
   {
-    const TcConvSpec ns = tc_note_spec();
+    constexpr TcConvSpec ns = tc_spec(2);
     const size_t need = (size_t)2 * ns.chunks8 * 8 * tc_rows_total(m->chunk, ns.rows_per_window);
     const __nv_bfloat16* before = m->chl.p;
     CK(m->chl.reserve(need));
@@ -419,7 +417,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
     ProfScope ps(m, 3, st);
     for (int s = 0; s < 8; ++s) launch_decimate(m->lp2, audio, desc, chain, s, nb, st);
   }
-  const TcConvSpec cs = tc_contour_spec(), ns = tc_note_spec();
+  constexpr TcConvSpec cs = tc_spec(0), ns = tc_spec(2);
   const int ystride = tc_rows_total(m->chunk, cs.rows_per_window), cstride = tc_rows_total(m->chunk, ns.rows_per_window);
   const long long fr = (long long)m->chunk * kFrames;  // frame stride of the internal raw buffers
   const long long nfr = (long long)nb * kFrames;
@@ -458,7 +456,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
       } else {
         o.act = m->c1.p;  // channels-last activations
       }
-      launch_conv_tc(m->yhl.p, m->tc_contour.dev, o, nb, ystride, m->n_sms, st, /*fuse_next=*/m->path == 1);
+      launch_conv_tc(m->yhl.p, m->tc[0].dev, o, nb, ystride, m->n_sms, st, /*fuse_next=*/m->path == 1);
     }
     {
       ProfScope ps(m, 4, st);
@@ -473,7 +471,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
       o.unwrapped = ud ? u->note : nullptr;
       o.frame_stride = ud ? u->stride : 0;
       o.edge = m->edge.p;
-      launch_conv_tc(m->chl.p, m->tc_note.dev, o, nb, cstride, m->n_sms, st);
+      launch_conv_tc(m->chl.p, m->tc[2].dev, o, nb, cstride, m->n_sms, st);
     }
     {
       ProfScope ps(m, 1, st);
@@ -485,7 +483,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
       o.frame_stride = ud ? u->stride : 0;
       o.note_raw = m->i_note.p;
       o.edge = m->edge.p;
-      launch_conv_tc(m->yhl.p, m->tc_onset.dev, o, nb, ystride, m->n_sms, st);
+      launch_conv_tc(m->yhl.p, m->tc[1].dev, o, nb, ystride, m->n_sms, st);
     }
     if (!ud) {  // raw windows for the caller: internal -> row-major
       launch_pm_to_rows(m->i_note.p, fr, 0, nfr, kPitches, note, st);
@@ -635,7 +633,7 @@ static int model_init(bp_model* m, const std::vector<float>& params, const cudaD
   // M-tiles per SM in every layer (M-tiles advance by 64 - (KH2 - 1) rows: they overlap by the time taps of the fused
   // conv2) -> 184 windows on 132 SMs
   {
-    const TcConvSpec ns = tc_note_spec();
+    constexpr TcConvSpec ns = tc_spec(2);
     m->chunk = std::max(1, 2 * m->n_sms * (128 - (ns.KH2 - 1)) / ns.rows_per_window);
   }
   rc = derive(m, m->stream);
@@ -661,7 +659,7 @@ void bp_model_destroy(bp_model_t* m) {
   m->yhl.release();
   m->chl.release();
   m->cqt_wtc.release();
-  for (bp_model::TcLayer* L : {&m->tc_contour, &m->tc_onset, &m->tc_note}) L->tiles.release(), L->b1.release(), L->b2.release();
+  for (bp_model::TcLayer& L : m->tc) L.tiles.release(), L.b1.release(), L.b2.release();
   if (m->d_params) cudaFree(m->d_params);
   if (m->d_derived) cudaFree(m->d_derived);
   if (m->d_gauss) cudaFree(m->d_gauss);
@@ -1461,7 +1459,7 @@ int bp_debug_tc_plan(int which, const float* w, int32_t* sizes, uint16_t* tiles,
                      int32_t* group_step_off, int32_t* group_ft) {
   if (!w || !sizes || which < 0 || which > 2) return fail(BP_E_INVALID, "bp_debug_tc_plan: bad argument");
   TcConvPlan pl;
-  pl.build(which == 0 ? tc_contour_spec() : which == 1 ? tc_onset_spec() : tc_note_spec(), w);
+  pl.build(tc_spec(which), w);
   sizes[0] = pl.n_tiles;
   sizes[1] = (int32_t)pl.tile_seq.size();
   sizes[2] = pl.n_uses;
@@ -1511,12 +1509,12 @@ int bp_debug_tc_b2(int which, const float* w2, int32_t* sizes, uint16_t* tiles) 
   if (!w2 || !sizes || which < 0 || which > 2) return fail(BP_E_INVALID, "bp_debug_tc_b2: bad argument");
   std::vector<uint16_t> t;
   tc_build_b2(which, w2, t);
-  const int n2 = which == 1 ? 16 : 32;
-  sizes[0] = (int32_t)(t.size() / (2 * 16 * n2));
-  sizes[1] = n2;
-  sizes[2] = which == 0 ? 5 : which == 1 ? 3 : 7;
-  sizes[3] = which == 0 ? 104 : which == 1 ? 32 : 64;
-  sizes[4] = which == 0 ? 5 : which == 1 ? 4 : 8;
+  const TcConvSpec sp = tc_spec(which);
+  sizes[0] = sp.n2_tiles;
+  sizes[1] = sp.n2;
+  sizes[2] = sp.KH2;
+  sizes[3] = sp.width;
+  sizes[4] = sp.js;
   if (tiles) std::memcpy(tiles, t.data(), t.size() * 2);
   return BP_OK;
 }

@@ -362,7 +362,7 @@ void launch_contour2(const float* c1, const CnnWeights& w, float* contour, int n
 }
 void launch_contour2_tc(const float* c1, const CnnWeights& w, float* contour, __nv_bfloat16* chl, int rows_total, int n,
                         cudaStream_t st) {
-  const TcConvSpec sp = tc_note_spec();
+  constexpr TcConvSpec sp = tc_spec(2);  // the note conv reads the contour posteriorgram
   launch1<Contour2CfgN>(NhwcIn<8, 264>{c1}, w.contour2_wT, w.contour2_b, contour, n, st,
                         SplitOut{chl, rows_total, sp.chunks8, sp.rows_per_window, sp.lead_rows});
 }

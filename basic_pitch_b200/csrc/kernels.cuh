@@ -46,18 +46,38 @@ void launch_onset2(const float* note, const float* o1, const CnnWeights& w, floa
 
 
 // ---- tc_conv.cu (tensor-core path of the three wide convolutions, each with its following conv fused) --------
+// The geometry of one layer (layer 0 contour, 1 onset, 2 note): every shape of its kernels, shared-memory layout, host
+// builders and workspaces is derived from this description.
 struct TcConvSpec {
   int KH, KW, SF, PT, PL, COUT, FLT, WOUT;  // taps, frequency stride, pads, channels, bins per 128-column tile, output bins
   int n_ci;                                 // input channels (harmonics of y, or 1 for the contour posteriorgram)
   int shifts[8];                            // frequency shift of every input channel (harmonic stacking)
   int data_bins, chunks8;                   // bins of the input rows and 8-bin chunks of the split layout (even)
   int rows_per_window, lead_rows;           // row layout of the split input: 172 frames + zero rows per window
-  int epi;                                  // 0 contour, 1 onset, 2 note
+  int layer;                                // 0 contour, 1 onset, 2 note
   int KH2, HALO, G0;                        // fused next conv: time taps, frequency halo; tiles of a group are G0 apart
+  // fused next conv as a second contraction (tc_conv.cu): weight tiles, their N, accumulator columns per output offset j,
+  // accumulator columns, columns staged in shared memory at a time (a multiple of 8 and of js: whole output offsets)
+  int n2_tiles, n2, js, width, pass;
+  // gathered conv1 (onset / note, tc_conv.cu): window width in K, and for W = 6 the K slot map
+  int W;
+  int slot[24];
+  __host__ __device__ constexpr int n_ft() const { return (WOUT + FLT - 1) / FLT; }  // frequency tiles
+  __host__ __device__ constexpr int tile_bins() const { return 8 * (chunks8 - 1); }  // bins of a data tile (the last chunk is padding)
+  __host__ __device__ constexpr int ksteps() const { return (KH * n_ci * W + 15) / 16; }  // gathered conv1: K-steps per bin
+  // edge-buffer values per side of a range boundary: the 2 HALO partial sums; the contour also keeps the finished bins
+  // that share the two 8-bin output chunks around the boundary
+  __host__ __device__ constexpr int edge_per_side() const { return 2 * HALO + (layer == 0 ? 8 - HALO : 0); }
 };
-TcConvSpec tc_contour_spec();
-TcConvSpec tc_onset_spec();
-TcConvSpec tc_note_spec();
+// clang-format off
+__host__ __device__ constexpr TcConvSpec tc_spec(int layer) {
+  //                  KH  KW SF PT PL COUT FLT WOUT n_ci shifts                               bins          ch8 rows/win lead layer KH2 HALO G0  n2_tiles n2 js width pass  W
+  return layer == 0 ? TcConvSpec{3, 39, 1, 1, 19, 8, 16, 264, 8, {-36, 0, 36, 57, 72, 84, 93, 101}, kCqtBins,     40, 174, 3, 0, 5, 2, 9,  1, 32, 5, 104, 40, 0, {}}
+       : layer == 1 ? TcConvSpec{5, 5, 3, 2, 1, 32, 4, 88, 8, {-36, 0, 36, 57, 72, 84, 93, 101},   kCqtBins,     40, 174, 3, 1, 3, 1, 12, 2, 16, 4, 32, 32,   6,
+                                 {9, 10, 21, 22, 14, 4, 2, 1, 16, 3, 6, 13, 5, 17, 18, 20, 19, 23, 7, 0, 8, 15, 12, 11}}
+                    : TcConvSpec{7, 7, 3, 3, 2, 32, 4, 88, 1, {0, 0, 0, 0, 0, 0, 0, 0},           kContourBins, 34, 175, 6, 2, 7, 1, 12, 2, 32, 8, 64, 64,   8, {}};
+}
+// clang-format on
 // Host side: weight tiles + the per-group MMA programs of the Toeplitz form.  The kernels run it for the contour conv
 // only; the onset and note convs gather their A operand instead (tc_build_b1), and their plans only serve the tests.
 struct TcConvPlan {
@@ -71,12 +91,10 @@ struct TcConvPlan {
   void build(const TcConvSpec& spec, const float* w /* [COUT][n_ci][KH][KW] */);
 };
 struct TcConvDev {
-  TcConvSpec spec;
+  int layer;  // 0 contour, 1 onset, 2 note (tc_spec)
   const uint16_t* tiles;  // contour: Toeplitz weight tiles (the program is in constant memory)
   const uint16_t* b1;     // onset / note: conv1 B matrices (tc_build_b1)
   const uint16_t* b2;     // conv2 weight matrix of the fused epilogue (tc_build_b2_full)
-  int n_groups;
-  int layer;  // 0 contour, 1 onset, 2 note
   // epilogue values, passed with every launch: conv1 bias (COUT used), conv2 bias, and for the onset layer the conv2
   // weights of its note input channel (models.py:305: concat[note, onset1]) [dt][df]
   float bias1[32];
@@ -84,22 +102,22 @@ struct TcConvDev {
   float note_w[9];
 };
 int tc_upload_program(const TcConvPlan& contour_plan, cudaStream_t st);  // 0 on success
-// conv1 of the onset (epi 1, w = [32][8][5][5]) / note (epi 2, w = [32][1][7][7]) layer as the kernel gathers it: its two
-// B matrices [parity 2][plane hi/lo][K / 8][32][8] bf16, and the geometry of the gather (window start of every output
+// conv1 of the onset (layer 1, w = [32][8][5][5]) / note (layer 2, w = [32][1][7][7]) layer as the kernel gathers it: its
+// two B matrices [parity 2][plane hi/lo][K / 8][32][8] bf16, and the geometry of the gather (window start of every output
 // bin and channel, [wout][n_ci]; the bins [lo, hi) of every channel that hold input, [n_ci][2]).  window8: B in the
 // 8-bin-window form (K rows 8 (dt * n_ci + ci) + j) instead of the K order the kernel uses (kmap).
-void tc_build_b1(int epi, const float* w, std::vector<uint16_t>& out, bool window8 = false);
+void tc_build_b1(int layer, const float* w, std::vector<uint16_t>& out, bool window8 = false);
 struct TcGatherGeom {
   int K, n_ci, KH, wout;  // K of the 8-bin-window form
   int K_packed;           // K the kernel runs
   std::vector<int> starts, ranges;
   std::vector<int> kmap;  // [K_packed][3]: (dt, ci, window bin j) of every row of the kernel's B, -1 for padding
 };
-TcGatherGeom tc_gather_geometry(int epi);
-// bf16 hi/lo weight tiles of the fused second conv (epi: 0 contour, 1 onset, 2 note; w2 = that conv's weights), see TcB2
-void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out);
+TcGatherGeom tc_gather_geometry(int layer);
+// bf16 hi/lo weight tiles of the fused second conv (w2 = that conv's weights), see tc_conv.cu
+void tc_build_b2(int layer, const float* w2, std::vector<uint16_t>& out);
 // the same tiles placed into the K = 128 x N = width conv2 weight matrix the kernel reads (tc_conv.cu)
-void tc_build_b2_full(int epi, const float* w2, std::vector<uint16_t>& out);
+void tc_build_b2_full(int layer, const float* w2, std::vector<uint16_t>& out);
 int tc_rows_total(int n_windows, int rows_per_window);
 size_t tc_edge_floats(const TcConvSpec& spec, int n_windows);  // size of the edge buffer of a fused layer
 int tc_setup();  // 0 on success
@@ -113,7 +131,7 @@ struct UnwrapDesc {
   int pad;
 };
 // NormalizedLog + folded BatchNorm of the CQT log-magnitudes straight into the bf16 hi/lo split operand (k-chunk-major
-// row layout of tc_contour_spec() / tc_onset_spec()); `y` itself is left untouched (launch_lognorm makes the fp32 copy).
+// row layout of tc_spec(0) / tc_spec(1)); `y` itself is left untouched (launch_lognorm makes the fp32 copy).
 // rows_stride: row stride of the split layout (>= tc_rows_total(n_windows, ...)); fixed per model so that rows the
 // kernels never write (separators, pads) keep their zeros across batches of different size
 void launch_lognorm_split(const float* y, const unsigned int* minmax, const float* bn, __nv_bfloat16* dst,
@@ -135,14 +153,14 @@ struct TcOut {
   __nv_bfloat16* chl = nullptr;     // contour layer: split operand of the note conv [2][chl_chunks][chl_rows][8]
   int chl_rows = 0, chl_chunks = 0, chl_rpw = 0, chl_lead = 0;
   float* edge = nullptr;            // >= tc_edge_floats(spec, n_windows) floats of scratch
-  float* act = nullptr;             // EPI 0 (path 2): channels-last activations [B][172][WOUT][COUT]
+  float* act = nullptr;             // unfused contour (path 2): channels-last activations [B][172][WOUT][COUT]
 };
 // fuse_next (contour layer only; the other two always fuse): also compute the following conv in the epilogue instead
 // of storing the channels-last activations
 void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& out, int n_windows, int rows_stride,
                     int n_sms, cudaStream_t st, bool fuse_next = false);
 // contour conv2 on the channels-last output of the tensor-core contour conv; also emits the bf16 hi/lo split of the
-// contour posteriorgram in the layout of tc_note_spec()
+// contour posteriorgram in the layout of tc_spec(2)
 void launch_contour2_tc(const float* c1_nhwc, const CnnWeights& w, float* contour, __nv_bfloat16* chl, int rows_total,
                         int n_windows, cudaStream_t st);
 

@@ -7,12 +7,13 @@
 // conv + ReLU, reference: basic_pitch/models.py:295-304) of the deployed graph, and the harmonic stacking in
 // front of them (reference: basic_pitch/nn.py:69-88), which is folded into the weight operand and never
 // materialised; node 238/239 (note conv1 + ReLU, models.py:270-279) reads the contour posteriorgram instead.
-// One kernel template, three specs (TcConvSpec).  The epilogue (EPI 1 / 2 / 3 = onset / note / contour) also computes
-// the FOLLOWING single-output convolution (onset conv2 models.py:305-313, note conv2 :282-290, contour conv2 :254-262)
+// One kernel template, instantiated per layer (0 contour, 1 onset, 2 note) and per epilogue; every shape comes from the
+// layer's description tc_spec (kernels.cuh).  The fused epilogue (all three layers) also computes the FOLLOWING
+// single-output convolution (onset conv2 models.py:305-313, note conv2 :282-290, contour conv2 :254-262)
 // completely, so neither the 8- / 32-channel activations nor any partial sums of them reach HBM:
 //   * channels and frequency taps are reduced by a SECOND tensor-core contraction whose A operand is bias + ReLU of the
 //     conv1 accumulator, split to bf16 hi/lo straight in the registers (the accumulator fragment of wgmma is the A
-//     register fragment of the next K = 16 step), against a conv2 weight matrix in shared memory (TcB2),
+//     register fragment of the next K = 16 step), against a conv2 weight matrix in shared memory (tc_build_b2_full),
 //   * its sums go through a small shared-memory staging area, where the thread of each tile row adds the time taps of
 //     the rows below it; M-tiles overlap by KH2 - 1 rows, so every frame is complete in exactly one tile.  The thread
 //     of tile row r finishes the output frame r - H (H = KH2 / 2) and adds its taps in the same order whatever its
@@ -21,7 +22,7 @@
 //     order; only where two tile RANGES meet (slot 0 | slot 1, or the group splits of a small batch) the two partial
 //     sums go to a small edge buffer and edge_fix_kernel finishes those 4 (contour) / 2 bins,
 //   * bias, sigmoid (+ the note input channel of the onset conv2, + unwrap inference.py:247-279) and the store.
-// EPI 0 stores the contour activations channels-last (path 2, activation-level tests).
+// The unfused contour epilogue stores the activations channels-last (path 2, activation-level tests).
 //
 // Formulation of the contour conv1 ("Toeplitz along frequency on aligned chunks"; the onset and note conv1 gather instead,
 // see below)
@@ -43,11 +44,11 @@
 // (hi*hi + hi*lo + lo*hi) in fp32, which keeps the posteriorgrams within ~1e-5 of the FP32 path
 // (SURVEY.md Appendix C.4); a single bf16 product would miss the 1e-3 bar.
 //
-// Formulation of the onset and note conv1 (EPI 1 / 2: 5 or 7 frequency taps at stride 3, where a Toeplitz tile would be
+// Formulation of the onset and note conv1 (layers 1 / 2: 5 or 7 frequency taps at stride 3, where a Toeplitz tile would be
 // mostly zeros): an implicit GEMM per output bin f,
 //   D_f[m][co] = sum over K = (dt, ci, j < 8) of x[m + dt][s(f, ci) + j] * B_{f & 1}[(dt, ci, j)][co]      (m64 n32)
 //   s(f, ci)   the even bin at or below the first tap u0 = SF*f - PL + shift_ci, so the taps sit at j = (u0 & 1) + df
-//   B_p        [K = KH * n_ci * 8, padded to 16][32 channels]: the weights at those positions for f & 1 = p (TcGather)
+//   B_p        [K = KH * n_ci * 8, padded to 16][32 channels]: the weights at those positions for f & 1 = p (tc_build_b1)
 // The A operand is GATHERED from the data tile into wgmma A registers: a register holds the bins s + 2 qd, s + 2 qd + 1
 // of one row, one aligned 32-bit shared load, masked to zero where the reference has no input (outside the CQT / the
 // contour posteriorgram, outside the stacked image).  The two B matrices stay resident in shared memory.  The four bins of
@@ -83,6 +84,7 @@ constexpr int kMTile = 64;
 constexpr int kTileBytes = 8192;                                 // weight tile: [plane 2][kchunk 2][128][8] bf16
 constexpr int kMaxSteps = 1024;                                  // program steps per layer (constant memory)
 constexpr int kMaxGroups = 15;
+static_assert(tc_spec(0).G0 <= kMaxGroups, "contour groups in constant memory");
 constexpr int kConsumerWarps = 8;  // two warpgroups, one per accumulator slot
 constexpr int kProducerWarp = 8;   // the first warp of the third warpgroup; its other three warps only hand back registers
 constexpr int kThreads = 32 * kConsumerWarps + 128;
@@ -105,49 +107,26 @@ static_assert(kProducerRegs + 2 * kConsumerRegs <= 3 * 168, "register pool of th
 // With the conv2 accumulator laid out j-major (column j * JS + dt, JS >= KH2) those are a contiguous WINDOW of columns,
 // the same for every step up to its start column: every step multiplies by the same small weight tile
 //   B2[kk][j' * JS + dt] = w2[c(kk)][dt][df(kk, j')]          (N = 32 columns; onset 16)
-// placed at the window's start column (contour 10 ks, note 8 fl, onset 4 fl) of a K = 128 x N = width matrix
-// (tc_build_b2_full), which the MMAs read from shared memory.
-// ------------------------------------------------------------------------------------------------
-struct TcB2 {
-  int n_tiles, n2, kh2, js, width;  // weight tiles, their N, time taps, columns per output offset j, accumulator columns
-  int pass;  // accumulator columns staged in shared memory at a time (a multiple of 8 and of js: whole output offsets)
-};
-__host__ __device__ constexpr TcB2 tc_b2_spec(int epi) {  // epi: 0 / 3 contour, 1 onset, 2 note
-  // contour: 3 passes of 8 output offsets (40 columns), which frees 32 KB of staging for four more weight stages
-  return epi == 1 ? TcB2{2, 16, 3, 4, 32, 32} : epi == 2 ? TcB2{2, 32, 7, 8, 64, 64} : TcB2{1, 32, 5, 5, 104, 40};
-}
-
-// ------------------------------------------------------------------------------------------------
-// The gathered conv1 of the onset (EPI 1) and note (EPI 2) layers, 32 output channels at frequency stride 3 (see the
+// placed at the window's start column (contour 10 ks, note 8 fl, onset 4 fl: js x the step's first bin) of a K = 128 x
+// N = width matrix (tc_build_b2_full), which the MMAs read from shared memory.  The contour stages its sums in 3 passes of
+// 8 output offsets (40 columns), which frees 32 KB of staging for four more weight stages.
+//
+// The gathered conv1 of the onset (layer 1) and note (layer 2), 32 output channels at frequency stride 3 (see the
 // header).  K runs over (time tap dt, channel ci, window bin j < W), padded to whole K = 16 steps (tc_gather_k):
 //   onset: 5 dt x 8 harmonics x 6 = 240 (15 steps, 83 % of the rows hold a tap): the window's first tap is at j = 0 or 1
 //          and KW = 5, so every tap lies in j < 6; k = 48 dt + 2 P + (j & 1) with the slot P of pair (ci, j / 2)
 //   note:  7 dt x 1 x 8 = 56 -> 64 (4 steps): k = 8 (dt * n_ci + ci) + j
+// W = 6: K slot pair P of a time tap (k = 48 dt + 2 P + {0, 1}) -> bin pair 3 ci + jp of window ci (TcConvSpec::slot).
+// Lane qd of a quad loads slot 4 e + qd of register word e; the order keeps the bank conflicts at their minimum (DESIGN §4.1)
 // ------------------------------------------------------------------------------------------------
-struct TcGather {
-  int KH, KW, PL, n_ci;  // time / frequency taps, frequency pad, input channels (frequency stride 3, 32 output channels)
-  int data_bins;         // bins of the input rows (the CQT, or the contour posteriorgram)
-  int tile_bins;         // bins the data tile holds (8 x its chunks)
-  int shifts[8];         // harmonic shift of every input channel
-  int W;                 // window width in K: 8, or 6 where the KW taps fit 6 bins at either parity (onset, KW = 5)
-  // W = 6: K slot pair P of a time tap (k = 48 dt + 2 P + {0, 1}) -> bin pair 3 ci + jp of window ci.  Lane qd of a
-  // quad loads slot 4 e + qd of register word e; the order keeps the bank conflicts at their minimum (DESIGN §4.1)
-  int slot[24];
-  __host__ __device__ constexpr int ksteps() const { return (KH * n_ci * W + 15) / 16; }
-};
-__host__ __device__ constexpr TcGather tc_gather_spec(int epi) {  // epi 1 onset, 2 note (the geometry of tc_*_spec)
-  return epi == 1 ? TcGather{5, 5, 1, 8, kCqtBins, 312, {-36, 0, 36, 57, 72, 84, 93, 101}, 6,
-                             {9, 10, 21, 22, 14, 4, 2, 1, 16, 3, 6, 13, 5, 17, 18, 20, 19, 23, 7, 0, 8, 15, 12, 11}}
-                  : TcGather{7, 7, 2, 1, kContourBins, 264, {0, 0, 0, 0, 0, 0, 0, 0}, 8, {}};
-}
 // row k of B for time tap dt, channel ci, window bin j
-__host__ __device__ constexpr int tc_gather_k(TcGather g, int dt, int ci, int j) {
+__host__ __device__ constexpr int tc_gather_k(TcConvSpec g, int dt, int ci, int j) {
   if (g.W == 8) return 8 * (dt * g.n_ci + ci) + j;
   int P = 0;
   while (g.slot[P] != 3 * ci + j / 2) ++P;
   return g.n_ci * g.W * dt + 2 * P + (j & 1);
 }
-__host__ __device__ constexpr bool tc_gather_slots_ok(TcGather g) {  // W = 6: the slots are a permutation of the pairs
+__host__ __device__ constexpr bool tc_gather_slots_ok(TcConvSpec g) {  // W = 6: the slots are a permutation of the pairs
   if (g.W == 8) return true;
   if (g.W != 6 || g.n_ci != 8) return false;
   for (int p = 0; p < 24; ++p) {
@@ -158,16 +137,18 @@ __host__ __device__ constexpr bool tc_gather_slots_ok(TcGather g) {  // W = 6: t
   return true;
 }
 // W = 6: shift of the channel, and bin pair in its window, that K slot P holds
-__host__ __device__ constexpr int tc_gather_slot_shift(TcGather g, int P) { return g.shifts[g.slot[P] / 3]; }
-__host__ __device__ constexpr int tc_gather_slot_pair(TcGather g, int P) { return g.slot[P] % 3; }
-static_assert(tc_gather_slots_ok(tc_gather_spec(1)) && tc_gather_slots_ok(tc_gather_spec(2)), "K slot map of the gather");
-static_assert(tc_gather_spec(1).ksteps() == 15 && tc_gather_spec(2).ksteps() == 4, "K-steps per output bin");
+__host__ __device__ constexpr int tc_gather_slot_shift(TcConvSpec g, int P) { return g.shifts[g.slot[P] / 3]; }
+__host__ __device__ constexpr int tc_gather_slot_pair(TcConvSpec g, int P) { return g.slot[P] % 3; }
+static_assert(tc_gather_slots_ok(tc_spec(1)) && tc_gather_slots_ok(tc_spec(2)), "K slot map of the gather");
+static_assert(tc_spec(1).ksteps() == 15 && tc_spec(2).ksteps() == 4, "K-steps per output bin");
 // first bin of the 8-bin window of output bin f, channel ci: the even bin at or below its first tap
-__host__ __device__ constexpr int tc_gather_start(TcGather g, int f, int ci) { return (3 * f - g.PL + g.shifts[ci]) & ~1; }
+__host__ __device__ constexpr int tc_gather_start(TcConvSpec g, int f, int ci) {
+  return (g.SF * f - g.PL + g.shifts[ci]) & ~1;
+}
 // the bins u of channel ci that hold input: inside the row (u < data_bins) and inside the stacked image
 // (0 <= u - shift < 264, the zero fill of HarmonicStacking); the gather supplies zero everywhere else
-__host__ __device__ constexpr int tc_gather_lo(TcGather g, int ci) { return g.shifts[ci] > 0 ? g.shifts[ci] : 0; }
-__host__ __device__ constexpr int tc_gather_hi(TcGather g, int ci) {
+__host__ __device__ constexpr int tc_gather_lo(TcConvSpec g, int ci) { return g.shifts[ci] > 0 ? g.shifts[ci] : 0; }
+__host__ __device__ constexpr int tc_gather_hi(TcConvSpec g, int ci) {
   return g.data_bins < kContourBins + g.shifts[ci] ? g.data_bins : kContourBins + g.shifts[ci];
 }
 
@@ -175,7 +156,7 @@ namespace tc {
 // Shared memory is laid out per layer: the data tile; contour: as many weight-tile stages as fit; onset / note: the two
 // conv1 B matrices; for the fused layers the conv2 weight matrix and the staging of the conv2 sums.
 struct TcSmem {
-  int data_bytes;   // [2 planes][chunks][64 + KH - 1 rows][16 B], rounded up to 1 KB
+  int data_bytes;   // [2 planes][chunks8 - 1][64 + KH - 1 rows][16 B], rounded up to 1 KB
   int b1_bytes;     // onset / note conv1 B matrices [parity 2][plane 2][K / 8][32][8] bf16
   int b2_bytes;     // conv2 weight matrix [2 planes][128][width] bf16
   int p_bytes;      // conv2 sums [2 slots][64 rows][pass + 1] fp32
@@ -186,22 +167,21 @@ struct TcSmem {
 };
 constexpr int kMaxSmem = 232448;  // 227 KB opt-in per CTA
 constexpr int kMaxStages = 12;
-__host__ __device__ constexpr TcSmem tc_smem(int epi) {  // epi: 0 contour (activations), 1 onset, 2 note, 3 contour (fused)
+__host__ __device__ constexpr TcSmem tc_smem(int layer, bool fused) {
   TcSmem s{};
-  const int chunks = epi == 2 ? 33 : 39, rows = kMTile + (epi == 1 ? 4 : epi == 2 ? 6 : 2);
-  const TcB2 b2 = tc_b2_spec(epi);
-  const bool gather = epi == 1 || epi == 2;
-  s.data_bytes = (2 * chunks * rows * 16 + 1023) / 1024 * 1024;
-  s.b1_bytes = gather ? 2 * 2 * 16 * tc_gather_spec(epi).ksteps() * 32 * 2 : 0;
-  s.b2_bytes = epi == 0 ? 0 : 2 * 128 * b2.width * 2;
-  s.p_bytes = epi == 0 ? 0 : 2 * 64 * (b2.pass + 1) * 4;
+  const TcConvSpec L = tc_spec(layer);
+  const bool gather = layer != 0;
+  s.data_bytes = (2 * (L.chunks8 - 1) * (kMTile + L.KH - 1) * 16 + 1023) / 1024 * 1024;
+  s.b1_bytes = gather ? 2 * 2 * 16 * L.ksteps() * 32 * 2 : 0;
+  s.b2_bytes = fused ? 2 * 128 * L.width * 2 : 0;
+  s.p_bytes = fused ? 2 * 64 * (L.pass + 1) * 4 : 0;
   const int st = (kMaxSmem - 512 - s.data_bytes - s.b1_bytes - s.b2_bytes - s.p_bytes) / kTileBytes;
   s.stages = gather ? 0 : st < kMaxStages ? st : kMaxStages;
   return s;
 }
 // weight stages of the contour layer (DESIGN §4.1): activations, fused
-static_assert(tc_smem(0).stages == 12 && tc_smem(3).stages == 9, "weight-ring depth per layer");
-static_assert(tc_smem(1).total() <= kMaxSmem && tc_smem(2).total() <= kMaxSmem, "onset / note shared memory");
+static_assert(tc_smem(0, false).stages == 12 && tc_smem(0, true).stages == 9, "weight-ring depth per layer");
+static_assert(tc_smem(1, true).total() <= kMaxSmem && tc_smem(2, true).total() <= kMaxSmem, "onset / note shared memory");
 // step word of a slot: [0,14) A start-address offset >> 4, [15] first MMA into that accumulator; kNoUse = the
 // slot's frequency tile does not use this step's weight tile
 constexpr uint32_t kUseFirstAcc = 1u << 15, kNoUse = 0xffffffffu;
@@ -224,11 +204,6 @@ static inline float bf2f(uint16_t h) {
   return f;
 }
 
-//                                      KH KW SF PT PL COUT FLT WOUT n_ci  shifts                              bins ch8 rows/win lead epi KH2 HALO G0
-TcConvSpec tc_contour_spec() { return {3, 39, 1, 1, 19, 8, 16, 264, 8, {-36, 0, 36, 57, 72, 84, 93, 101}, 309, 40, 174, 3, 0, 5, 2, 9}; }
-TcConvSpec tc_onset_spec() { return {5, 5, 3, 2, 1, 32, 4, 88, 8, {-36, 0, 36, 57, 72, 84, 93, 101}, 309, 40, 174, 3, 1, 3, 1, 12}; }
-TcConvSpec tc_note_spec() { return {7, 7, 3, 3, 2, 32, 4, 88, 1, {0, 0, 0, 0, 0, 0, 0, 0}, 264, 34, 175, 6, 2, 7, 1, 12}; }
-
 void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][KW] */) {
   using namespace tc;
   spec = sp;
@@ -238,7 +213,7 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   slot_words[1].clear();
   group_step_off.clear();
   group_ft.clear();
-  const int n_ft = (sp.WOUT + sp.FLT - 1) / sp.FLT;
+  const int n_ft = sp.n_ft();
   const int data_rows = kMTile + sp.KH - 1;
   const int lbo16 = data_rows;  // (rows * 16 B) >> 4
   // K = 16 steps start on 8-bin chunk boundaries (the k-chunk-major layout makes any chunk index a legal
@@ -404,24 +379,20 @@ __constant__ int c_group_step_off[tc::kMaxGroups + 1];
 __constant__ int c_group_ft[2 * tc::kMaxGroups];
 
 // tiles: [tile][plane hi/lo][k-chunk 2][n N2][8] bf16 (canonical K-major no-swizzle: LBO = N2 * 16 B, SBO = 128 B)
-void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
-  const TcB2 sp = tc_b2_spec(epi);
-  const int tile_elems = 2 * 16 * sp.n2;
-  out.assign((size_t)sp.n_tiles * tile_elems, 0);
-  for (int tl = 0; tl < sp.n_tiles; ++tl)
+// Tile tl, row kk holds element k = 16 tl + kk of the conv1 row: bin b = k / COUT of the step, channel c = k % COUT
+// (contour: 2 bins x 8 channels in one tile; onset / note: the 32 channels of one bin in two tiles).
+void tc_build_b2(int layer, const float* w2, std::vector<uint16_t>& out) {
+  const TcConvSpec sp = tc_spec(layer);
+  const int tile_elems = 2 * 16 * sp.n2, KW2 = 2 * sp.HALO + 1;  // time / frequency taps of the conv2: KH2 x KW2
+  out.assign((size_t)sp.n2_tiles * tile_elems, 0);
+  for (int tl = 0; tl < sp.n2_tiles; ++tl)
     for (int kk = 0; kk < 16; ++kk)
       for (int n = 0; n < sp.n2; ++n) {
         const int jp = n / sp.js, dt = n - jp * sp.js;
-        float w = 0.f;
-        if (dt >= sp.kh2) continue;
-        if (epi == 0 || epi == 3) {  // contour conv2 weights [1][8][5][5]; kk = (bin parity) * 8 + channel
-          const int b = kk >> 3, c = kk & 7, df = b + 4 - jp;
-          if (jp < 6 && df >= 0 && df < 5) w = w2[(c * 5 + dt) * 5 + df];
-        } else {
-          const int c = 16 * tl + kk, df = 2 - jp;
-          if (jp < 3) w = epi == 1 ? w2[(1 + c) * 9 + dt * 3 + df]  // onset conv2 [1][33][3][3], channel 0 = the note input
-                                   : w2[c * 21 + dt * 3 + df];      // note conv2 [1][32][7][3]
-        }
+        const int b = (16 * tl + kk) / sp.COUT, c = (16 * tl + kk) % sp.COUT, df = b + 2 * sp.HALO - jp;
+        if (dt >= sp.KH2 || df < 0 || df >= KW2) continue;
+        // conv2 weights [1][channels][KH2][KW2]; the onset conv2 has 33 channels, channel 0 = the note input
+        const float w = w2[((c + (layer == 1 ? 1 : 0)) * sp.KH2 + dt) * KW2 + df];
         const uint16_t hi = f2bf(w), lo = f2bf(w - bf2f(hi));
         const size_t o = (size_t)tl * tile_elems + (size_t)(kk >> 3) * sp.n2 * 8 + (size_t)n * 8 + (kk & 7);
         out[o] = hi;
@@ -430,7 +401,8 @@ void tc_build_b2(int epi, const float* w2, std::vector<uint16_t>& out) {
 }
 
 int tc_upload_program(const TcConvPlan& pl, cudaStream_t st) {
-  if (pl.spec.epi != 0 || (int)pl.tile_seq.size() > tc::kMaxSteps - 1 || pl.n_groups > tc::kMaxGroups) return -1;
+  // the kernel walks the G0 groups of tc_spec(0)
+  if (pl.spec.layer != 0 || (int)pl.tile_seq.size() > tc::kMaxSteps - 1 || pl.n_groups != tc_spec(0).G0) return -1;
   for (int sl = 0; sl < 2; ++sl)
     cudaMemcpyToSymbolAsync(c_prog, pl.slot_words[sl].data(), pl.slot_words[sl].size() * 4, (size_t)sl * tc::kMaxSteps * 4,
                             cudaMemcpyHostToDevice, st);
@@ -441,19 +413,19 @@ int tc_upload_program(const TcConvPlan& pl, cudaStream_t st) {
   return cudaStreamSynchronize(st) == cudaSuccess ? 0 : -1;
 }
 
-// The two conv1 B matrices of the onset / note layer, f even and f odd (TcGather), in the layout the MMAs read:
+// The two conv1 B matrices of the onset / note layer, f even and f odd, in the layout the MMAs read:
 // [parity 2][plane hi/lo][k-chunk K / 8][n 32][8] bf16 (K-major no-swizzle: LBO = 32 * 16 B, SBO = 128 B).
 // B_p[tc_gather_k(dt, ci, j)][co] = W[co][ci][dt][j - o], o = the first tap's offset in its window for f & 1 = p.
 // window8: the same weights in the 8-bin-window form k = 8 (dt * n_ci + ci) + j, whatever W (bp_debug_tc_gather).
-void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<uint16_t>& out, bool window8) {
-  const TcGather g = tc_gather_spec(epi);
+void tc_build_b1(int layer, const float* W /* [32][n_ci][KH][KW] */, std::vector<uint16_t>& out, bool window8) {
+  const TcConvSpec g = tc_spec(layer);
   const int wn = window8 ? 8 : g.W;
   const size_t plane = (size_t)16 * ((g.KH * g.n_ci * wn + 15) / 16) * 32;
   out.assign(4 * plane, 0);
   for (int p = 0; p < 2; ++p)
     for (int dt = 0; dt < g.KH; ++dt)
       for (int ci = 0; ci < g.n_ci; ++ci) {
-        const int o = 3 * p - g.PL + g.shifts[ci] - tc_gather_start(g, p, ci);
+        const int o = g.SF * p - g.PL + g.shifts[ci] - tc_gather_start(g, p, ci);
         for (int j = 0; j < wn; ++j) {
           const int df = j - o, k = window8 ? 8 * (dt * g.n_ci + ci) + j : tc_gather_k(g, dt, ci, j);
           if (df < 0 || df >= g.KW) continue;
@@ -468,8 +440,8 @@ void tc_build_b1(int epi, const float* W /* [32][n_ci][KH][KW] */, std::vector<u
       }
 }
 
-TcGatherGeom tc_gather_geometry(int epi) {
-  const TcGather g = tc_gather_spec(epi);
+TcGatherGeom tc_gather_geometry(int layer) {
+  const TcConvSpec g = tc_spec(layer);
   TcGatherGeom r;
   r.K = 16 * ((g.KH * g.n_ci * 8 + 15) / 16);  // of the 8-bin-window form
   r.K_packed = 16 * g.ksteps();
@@ -483,8 +455,8 @@ TcGatherGeom tc_gather_geometry(int epi) {
   }
   r.n_ci = g.n_ci;
   r.KH = g.KH;
-  r.wout = kPitches;
-  for (int f = 0; f < kPitches; ++f)
+  r.wout = g.WOUT;
+  for (int f = 0; f < g.WOUT; ++f)
     for (int ci = 0; ci < g.n_ci; ++ci) r.starts.push_back(tc_gather_start(g, f, ci));
   for (int ci = 0; ci < g.n_ci; ++ci) {
     r.ranges.push_back(tc_gather_lo(g, ci));
@@ -495,14 +467,15 @@ TcGatherGeom tc_gather_geometry(int epi) {
 
 // The small tiles expanded into the K = 128 x N = width matrix the conv2 MMAs read:
 // [plane hi/lo][k-chunk 16][n width][8] bf16 (K-major no-swizzle: LBO = width * 16 B, SBO = 128 B)
-void tc_build_b2_full(int epi, const float* w2, std::vector<uint16_t>& out) {
-  const TcB2 sp = tc_b2_spec(epi);
+void tc_build_b2_full(int layer, const float* w2, std::vector<uint16_t>& out) {
+  const TcConvSpec sp = tc_spec(layer);
   std::vector<uint16_t> small;
-  tc_build_b2(epi, w2, small);
+  tc_build_b2(layer, w2, small);
   const size_t tile_elems = (size_t)2 * 16 * sp.n2, plane = (size_t)128 * sp.width;
   out.assign(2 * plane, 0);
   for (int ks = 0; ks < 8; ++ks) {
-    const int col0 = (epi == 0 || epi == 3) ? 10 * ks : sp.js * (ks >> 1), tl = (epi == 0 || epi == 3) ? 0 : ks & 1;
+    // step ks starts at bin 16 ks / COUT of the tile; its weight tile repeats every n2_tiles steps
+    const int col0 = sp.js * (16 * ks / sp.COUT), tl = ks % sp.n2_tiles;
     for (int pl = 0; pl < 2; ++pl)
       for (int kk = 0; kk < 16; ++kk)
         for (int n = 0; n < sp.n2; ++n)
@@ -579,7 +552,7 @@ __global__ void lognorm_split_kernel(const float* __restrict__ y, const unsigned
 }
 
 // ------------------------------------------------------------------------------------------------
-// The tensor-core kernel
+// The tensor-core kernel.  The layer's geometry is compile-time (tc_spec); the arguments are what changes per launch.
 // ------------------------------------------------------------------------------------------------
 struct TcArgs {
   CUtensorMap data_map;         // 4-D tensor map of `data`: (8 elements, rows_total, chunks8, 2 planes); box = one data tile
@@ -590,13 +563,13 @@ struct TcArgs {
   const uint16_t* b2;           // conv2 weight matrix (tc_build_b2_full), fused layers
   TcOut o;                      // where the results go (kernels.cuh)
   int edge_rows;                // row stride of o.edge: [edge slot][side 2][KE][edge_rows]
-  int layer;                    // 0 contour, 1 onset, 2 note (cycle accounting)
   int rows_total, n_mtiles, n_windows;
-  int n_groups, n_split;        // an item covers groups [s*n_groups/n_split, (s+1)*n_groups/n_split)
-  int data_rows, row0;          // tile rows (64 + KH - 1); first data row of M-tile 0
+  int n_split;                  // an item covers groups [s*G0/n_split, (s+1)*G0/n_split)
+  int row0;                     // first data row of M-tile 0
+  // = tc_spec(layer).chunks8: a run-time trip count keeps the producer's per-chunk copy loop rolled, which keeps the
+  // contour's producer and MMA-issue loop state in uniform registers (a compile-time count unrolls it and they move out)
+  int chunks8;
   int ms, h2;                   // M-tile stride (64 - 2*h2) and time halo of the fused conv2
-  int chunks8, rows_per_window;
-  int cout, flt, wout, n_ft, g0;
   float bias1[32], bias2, note_w[9];  // the layer's epilogue values (TcConvDev)
 };
 
@@ -681,20 +654,23 @@ struct RowOut {
   float* unw;    // pitch layers: unw_pm + unwrapped frame  ; contour: unw_cm + unwrapped frame * 8      (nullptr: not stored)
   __nv_bfloat16* chl;  // contour: chl + data row * 8
   float* edge;   // edge buffer column of this frame: edge + R (nullptr: row not complete / not live)
-  const float* note_col;  // EPI 1: note_raw_pm + b*172 + t
+  const float* note_col;  // onset: note_raw_pm + b*172 + t
   int t;         // frame inside the window (of the OUTPUT frame this thread finishes)
   bool ok;       // live output frame whose time taps are complete in this M-tile
   int e_lo, e_hi;  // edge slots of this range's start and of the range above its end (-1: none)
 };
 
-// Frequency halo + finish for the onset / note layers (FLT = 4, halo 1): S[j] is the time-complete sum for bin 4 ft - 1 + j.
-template <int EPI>
+// Frequency halo + finish for the onset / note layers (FLT = 4, HALO = 1): S[j] is the time-complete sum for bin
+// FLT ft - HALO + j.
+template <int LAYER>
 __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut& ro, float (&S)[6], float (&carry)[2], int ft,
                                                   bool first, bool last) {
+  constexpr TcConvSpec L = tc_spec(LAYER);
+  static_assert(L.FLT + 2 * L.HALO == 6 && L.HALO == 1, "sums and carry of a pitch tile");
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
-      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * 2 * a.edge_rows;
+      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * L.edge_per_side() * a.edge_rows;
       e[0] = S[0];
       e[a.edge_rows] = S[1];
     }
@@ -702,14 +678,14 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
     S[0] += carry[0];
     S[1] += carry[1];
   }
-  const int jlo = first ? (lower ? 2 : 1) : 0;
-  const int jhi = (ft == a.n_ft - 1) ? 5 : 4;  // the last tile also finishes its top bin (no tile above)
+  const int jlo = first ? (lower ? 2 * L.HALO : L.HALO) : 0;
+  const int jhi = (ft == L.n_ft() - 1) ? L.FLT + L.HALO : L.FLT;  // the last tile also finishes its top bin (no tile above)
   if (ro.ok) {
     float nv[3][6];
-    if constexpr (EPI == 1) {  // note frames t-1 .. t+1, pitches 4 ft - 2 .. 4 ft + 3 (zero outside the image)
+    if constexpr (LAYER == 1) {  // note frames t-1 .. t+1, pitches FLT ft - 2 .. FLT ft + 3 (zero outside the image)
 #pragma unroll
       for (int c = 0; c < 6; ++c) {
-        const int f = 4 * ft - 2 + c;
+        const int f = L.FLT * ft - 2 + c;
         const bool fin = (unsigned)f < (unsigned)kPitches;
         const float* col = ro.note_col + (size_t)f * a.o.raw_rows;
 #pragma unroll
@@ -718,28 +694,28 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
       }
     }
 #pragma unroll
-    for (int j = 0; j < 5; ++j) {
+    for (int j = 0; j < L.FLT + L.HALO; ++j) {
       if (j < jlo || j >= jhi) continue;
-      const int f = 4 * ft - 1 + j;
+      const int f = L.FLT * ft - L.HALO + j;
       float x = S[j] + a.bias2;
-      if constexpr (EPI == 1) {
+      if constexpr (LAYER == 1) {
 #pragma unroll
         for (int r = 0; r < 3; ++r)
 #pragma unroll
           for (int df = 0; df < 3; ++df)
-            if (j + df < 6) x = fmaf(nv[r][j + df], a.note_w[r * 3 + df], x);  // pitch f + df - 1 = 4 ft - 2 + (j + df)
+            if (j + df < 6) x = fmaf(nv[r][j + df], a.note_w[r * 3 + df], x);  // pitch f + df - 1 = FLT ft - 2 + (j + df)
       }
       const float v = sigmoidf_fast(x);
       if (ro.raw) ro.raw[(size_t)f * a.o.raw_rows] = v;
       if (ro.unw) ro.unw[(size_t)f * a.o.frame_stride] = v;
     }
   }
-  carry[0] = S[4];
-  carry[1] = S[5];
-  if (last && ft < a.n_ft - 1 && ro.edge && ro.e_hi >= 0) {
-    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * 2 * a.edge_rows;
-    e[0] = S[4];
-    e[a.edge_rows] = S[5];
+  carry[0] = S[L.FLT];
+  carry[1] = S[L.FLT + 1];
+  if (last && ft < L.n_ft() - 1 && ro.edge && ro.e_hi >= 0) {
+    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * L.edge_per_side() * a.edge_rows;
+    e[0] = S[L.FLT];
+    e[a.edge_rows] = S[L.FLT + 1];
   }
 }
 
@@ -768,10 +744,12 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
   // chunk 2 ft - 1 = the six bins held back from the previous tile + j = 0, 1; chunk 2 ft = j = 2 .. 9; j = 10 .. 15 are
   // held for the next tile.  Where a range starts / ends, the four partial sums AND the six finished bins next to them go
   // to the edge buffer (10 values per side); edge_fix_kernel assembles the two chunks around the boundary.
+  constexpr TcConvSpec L = tc_spec(0);
+  static_assert(L.FLT == 16 && L.HALO == 2 && L.edge_per_side() == 10, "sums, carry and edge values of a contour tile");
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
-      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * 10 * a.edge_rows;
+      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * L.edge_per_side() * a.edge_rows;
 #pragma unroll
       for (int k = 0; k < 4; ++k) e[(size_t)k * a.edge_rows] = S[k];
 #pragma unroll
@@ -798,8 +776,8 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
   for (int k = 0; k < 6; ++k) hold[k] = fin[10 + k];
 #pragma unroll
   for (int k = 0; k < 4; ++k) carry[k] = S[16 + k];
-  if (last && ft < a.n_ft - 1 && ro.edge && ro.e_hi >= 0) {
-    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * 10 * a.edge_rows;
+  if (last && ft < L.n_ft() - 1 && ro.edge && ro.e_hi >= 0) {
+    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * L.edge_per_side() * a.edge_rows;
 #pragma unroll
     for (int k = 0; k < 4; ++k) e[(size_t)k * a.edge_rows] = S[16 + k];
 #pragma unroll
@@ -834,13 +812,13 @@ __device__ __forceinline__ void conv2_mma(float (&p)[NW / 2], const uint32_t (&a
   }
 }
 
-// conv1 of frequency tile ft of the onset / note layer (EPI 1 / 2), gathered (see the header): for each bin f = 4 ft + fl
-// the K-steps of TcGather, three split products m64n32k16 each, into acc[16 fl ..] (= columns 32 fl .. of the m64n128
+// conv1 of frequency tile ft of the onset / note layer (layer 1 / 2), gathered (see the header): for each bin f = FLT ft + fl
+// the K-steps of the layer, three split products m64n32k16 each, into acc[16 fl ..] (= columns 32 fl .. of the m64n128
 // fragment).  The A registers are loaded two steps ahead of the MMAs that read them (three register buffers, gather_steps).
 // Every output sums its steps in the same order whatever the item: a value depends only on f and the layer.
-template <int EPI>
+template <int LAYER>
 struct GatherRegs {
-  static constexpr TcGather G = tc_gather_spec(EPI);
+  static constexpr TcConvSpec G = tc_spec(LAYER);
   static_assert(G.W == 8 || (G.W == 6 && G.n_ci * G.W == 48), "W = 6: a time tap is 3 whole K-steps, 6 register words");
   // per register word (W = 8: per channel; W = 6: per slot group e, lane qd loads slot 4 e + qd): byte offset of the
   // thread's bin pair (row fr0) in the data tile in bits [0, 24), and in bits 24 / 25 whether its first / second bf16
@@ -848,7 +826,7 @@ struct GatherRegs {
   static constexpr int NWD = G.W == 8 ? G.n_ci : 6;
   uint32_t om[NWD];
   __device__ __forceinline__ static uint32_t word(int u, int lo, int hi, int fr0) {
-    const int uc = min(max(u, 0), G.tile_bins - 2);  // a pair outside the tile is masked; read one inside it
+    const int uc = min(max(u, 0), G.tile_bins() - 2);  // a pair outside the tile is masked; read one inside it
     return (uint32_t)((uc >> 3) * ((tc::kMTile + G.KH - 1) * 16) + (uc & 7) * 2 + fr0 * 16) |
            (u >= lo && u < hi ? 1u << 24 : 0u) | (u + 1 >= lo && u + 1 < hi ? 1u << 25 : 0u);
   }
@@ -877,7 +855,7 @@ struct GatherRegs {
                   j2 = tc_gather_slot_pair(G, 4 * E + 2), j3 = tc_gather_slot_pair(G, 4 * E + 3);
     const int sh = qd == 0 ? s0 : qd == 1 ? s1 : qd == 2 ? s2 : s3;
     const int jp = qd == 0 ? j0 : qd == 1 ? j1 : qd == 2 ? j2 : j3;
-    const int u = ((3 * f - G.PL + sh) & ~1) + 2 * jp;  // tc_gather_start + 2 jp
+    const int u = ((G.SF * f - G.PL + sh) & ~1) + 2 * jp;  // tc_gather_start + 2 jp
     om[E] = word(u, sh > 0 ? sh : 0, G.data_bins < kContourBins + sh ? G.data_bins : kContourBins + sh, fr0);
   }
   __device__ __forceinline__ uint32_t mask(int i) const {  // bits 24 / 25 -> 0x0000ffff / 0xffff0000
@@ -888,7 +866,7 @@ struct GatherRegs {
   // (half 1, fr0 + 8).  W = 8: half h is window 2 ks + h; W = 6: time tap ks / 3, word 2 (ks % 3) + h
   template <int KS>
   __device__ __forceinline__ void load(const unsigned char* s_data, uint32_t (&x)[8]) const {
-    constexpr int kPlane = G.tile_bins / 8 * (tc::kMTile + G.KH - 1) * 16;  // bytes of one plane of the data tile
+    constexpr int kPlane = G.tile_bins() / 8 * (tc::kMTile + G.KH - 1) * 16;  // bytes of one plane of the data tile
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       constexpr int NW = G.W == 8 ? G.KH * G.n_ci : 2 * G.ksteps();  // halves holding taps; the rest is K padding
@@ -912,11 +890,11 @@ struct GatherRegs {
 // Step I of the tile (bin fl = I / KS, K-step I % KS) reads register buffer I % 3.  Once its MMAs are committed and those
 // of step I - 1 have completed, buffer (I - 1) % 3 = (I + 2) % 3 takes step I + 2: the registers of step I + 1 were
 // loaded a whole step earlier, so their shared-memory latency is hidden behind the MMAs of two steps, not one.
-template <int EPI, int I>
-__device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& gr, uint32_t (&x)[3][8], const unsigned char* s_data,
+template <int LAYER, int I>
+__device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<LAYER>& gr, uint32_t (&x)[3][8], const unsigned char* s_data,
                                              uint64_t d0, int ft, int fr0, int qd, TcClocks& clk) {
   using namespace tc;
-  constexpr int KS = tc_gather_spec(EPI).ksteps(), NST = 4 * KS;
+  constexpr int FLT = tc_spec(LAYER).FLT, KS = tc_spec(LAYER).ksteps(), NST = FLT * KS;
   constexpr int fl = I / KS, ks = I % KS;
   constexpr uint32_t kB1Plane = 16 * KS * 32 * 2;  // bytes of one B plane
   float(&d)[16] = *reinterpret_cast<float(*)[16]>(acc + 16 * fl);
@@ -933,41 +911,45 @@ __device__ __forceinline__ void gather_steps(float (&acc)[64], GatherRegs<EPI>& 
     wgmma_wait<1>();  // the previous step's MMAs are done: its A registers may be refilled
     clk.lap(kClkMma);
     // the window offsets follow the bin being LOADED (step I + 2); step I + 1's registers are already in place
-    if constexpr ((I + 2) % KS == 0) gr.setup(4 * ft + (I + 2) / KS, fr0, qd);
+    if constexpr ((I + 2) % KS == 0) gr.setup(FLT * ft + (I + 2) / KS, fr0, qd);
     gr.template load<(I + 2) % KS>(s_data, x[(I + 2) % 3]);
     clk.lap(kClkFull);
   }
-  if constexpr (I + 1 < NST) gather_steps<EPI, I + 1>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
+  if constexpr (I + 1 < NST) gather_steps<LAYER, I + 1>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
 }
 
-template <int EPI>
+template <int LAYER>
 __device__ __forceinline__ void gather_conv1(float (&acc)[64], const unsigned char* s_data, uint32_t b1, int ft, int fr0, int qd,
                                              TcClocks& clk) {
   using namespace tc;
-  static_assert(tc_gather_spec(EPI).ksteps() >= 2, "the first two K-steps are loaded up front, of the same bin");
-  GatherRegs<EPI> gr;
+  static_assert(tc_spec(LAYER).ksteps() >= 2, "the first two K-steps are loaded up front, of the same bin");
+  GatherRegs<LAYER> gr;
   const uint64_t d0 = make_desc(b1, 32 * 16, 128);
   uint32_t x[3][8];
-  gr.setup(4 * ft, fr0, qd);
+  gr.setup(tc_spec(LAYER).FLT * ft, fr0, qd);
   gr.template load<0>(s_data, x[0]);
   gr.template load<1>(s_data, x[1]);
   clk.lap(kClkFull);
-  gather_steps<EPI, 0>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
+  gather_steps<LAYER, 0>(acc, gr, x, s_data, d0, ft, fr0, qd, clk);
   wgmma_wait<0>();
   reg_fence(acc);
   clk.lap(kClkMma);
 }
 
-template <int EPI>
+// LAYER: 0 contour, 1 onset, 2 note; FUSED: the epilogue computes the next conv (always for onset / note; the unfused
+// contour stores its channels-last activations)
+template <int LAYER, bool FUSED>
 __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
   using namespace tc;
-  constexpr bool kFused = EPI != 0;
-  constexpr bool kGather = EPI == 1 || EPI == 2;  // onset / note: gathered conv1, no weight ring
-  constexpr TcB2 B2 = tc_b2_spec(EPI);
-  constexpr int NW = B2.width, PC = B2.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
-  static_assert(PC % 8 == 0 && PC % B2.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
+  constexpr TcConvSpec L = tc_spec(LAYER);
+  constexpr bool kFused = FUSED;
+  constexpr bool kGather = LAYER != 0;  // onset / note: gathered conv1, no weight ring
+  static_assert(kFused || !kGather, "the onset and note epilogues always fuse the next conv");
+  constexpr int NW = L.width, PC = L.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
+  static_assert(PC % 8 == 0 && PC % L.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
+  constexpr int kDataRows = kMTile + L.KH - 1, kFt = L.n_ft();
   extern __shared__ __align__(128) unsigned char smem[];
-  constexpr TcSmem SM = tc_smem(EPI);
+  constexpr TcSmem SM = tc_smem(LAYER, FUSED);
   constexpr int kStages = SM.stages;
   static_assert(SM.total() <= kMaxSmem && kStages <= kMaxStages && (kGather || kStages >= 4), "dynamic shared memory per CTA");
   unsigned char* s_data = smem;                    // [2 planes][chunks][data_rows][16 B]
@@ -987,8 +969,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   // Broadcasting the warp index keeps the role branches and the producer loop state in uniform registers.
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const uint32_t lbo = (uint32_t)a.data_rows * 16u;
-  const uint32_t plane_bytes = (uint32_t)(a.chunks8 - 1) * lbo;  // the tile holds chunks 0 .. chunks8 - 2
+  constexpr uint32_t lbo = kDataRows * 16u;
+  constexpr uint32_t plane_bytes = (L.chunks8 - 1) * lbo;  // the tile holds chunks 0 .. chunks8 - 2
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
@@ -1020,10 +1002,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     if constexpr (kFused) bulk_g2s_expect_pred(s_b2, a.b2, (uint32_t)SM.b2_bytes, b2_full, leader);
     if constexpr (kGather) bulk_g2s_expect_pred(s_b1, a.b1, (uint32_t)SM.b1_bytes, b1_full, leader);
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;
-    const size_t plane_elems = (size_t)a.chunks8 * a.rows_total * 8;
+    const size_t plane_elems = (size_t)L.chunks8 * a.rows_total * 8;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       const int mt = it / a.n_split, sp = it % a.n_split;
-      const int g0 = sp * a.n_groups / a.n_split, g1 = (sp + 1) * a.n_groups / a.n_split;
+      const int g0 = sp * L.G0 / a.n_split, g1 = (sp + 1) * L.G0 / a.n_split;
       clk.lap(kClkProdOther);
       mbar_wait_wd(data_empty, ph_d ^ 1, 1);
       clk.lap(kClkDataEmpty);
@@ -1063,7 +1045,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       }
     }
     clk.lap(kClkProdOther);
-    clk.flush(a.layer);
+    clk.flush(LAYER);
   } else {
     setmaxnreg_inc<kConsumerRegs>();
     // ------------------------------ consumers: one warpgroup per accumulator slot ------------------------------
@@ -1080,15 +1062,15 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     if constexpr (kGather) mbar_wait_wd(b1_full, 0, 7);
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       const int mt = it / a.n_split, spl = it % a.n_split;
-      const int g0 = spl * a.n_groups / a.n_split, g1 = (spl + 1) * a.n_groups / a.n_split;
+      const int g0 = spl * L.G0 / a.n_split, g1 = (spl + 1) * L.G0 / a.n_split;
       // conv1 rows of the thread's fragment (relu(conv1) of a row that is not a live frame is the zero padding in time)
       bool live[2];
       int rb[2], rt[2];
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int m = mt * a.ms - a.h2 + fr0 + 8 * rr;  // row of the (window, frame) space: m = b * rows_per_window + t
-        rb[rr] = m >= 0 ? m / a.rows_per_window : 0;
-        rt[rr] = m - rb[rr] * a.rows_per_window;
+        rb[rr] = m >= 0 ? m / L.rows_per_window : 0;
+        rt[rr] = m - rb[rr] * L.rows_per_window;
         live[rr] = m >= 0 && (rb[rr] < a.n_windows) && (rt[rr] < kFrames);
       }
       // Fused layers: threads 0..63 of the group each finish the output frame of one tile row, h2 rows earlier than the
@@ -1100,7 +1082,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       if constexpr (kFused) {
         const int row = tid;
         const int q = mt * a.ms - 2 * a.h2 + row;
-        const int b = q >= 0 ? q / a.rows_per_window : 0, t = q - b * a.rows_per_window;
+        const int b = q >= 0 ? q / L.rows_per_window : 0, t = q - b * L.rows_per_window;
         ro.e_lo = slot * a.n_split + spl;
         ro.e_hi = (spl + 1 < a.n_split) ? slot * a.n_split + spl + 1 : (slot == 0 ? a.n_split : -1);
         ro.ok = row < 64 && row >= 2 * a.h2 && q >= 0 && b < a.n_windows && t < kFrames;
@@ -1113,14 +1095,14 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
             const int tt = t - kOverlapHalf;
             if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
           }
-          if constexpr (EPI == 3) {
+          if constexpr (LAYER == 0) {
             ro.chl = a.o.chl + ((size_t)a.o.chl_lead + (size_t)b * a.o.chl_rpw + t) * 8;
             if (a.o.raw) ro.raw = a.o.raw + ((size_t)b * kFrames + t) * 8;
             if (uf >= 0) ro.unw = a.o.unwrapped + (size_t)uf * 8;
           } else {
             if (a.o.raw) ro.raw = a.o.raw + (size_t)b * kFrames + t;
             if (uf >= 0) ro.unw = a.o.unwrapped + uf;
-            if constexpr (EPI == 1) ro.note_col = a.o.note_raw + (size_t)b * kFrames + t;
+            if constexpr (LAYER == 1) ro.note_col = a.o.note_raw + (size_t)b * kFrames + t;
           }
         }
       }
@@ -1132,8 +1114,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         float acc[64];
         int ft;
         if constexpr (kGather) {
-          ft = g + slot * a.g0 < a.n_ft ? g + slot * a.g0 : -1;
-          if (ft >= 0) gather_conv1<EPI>(acc, s_data, smem_u32(s_b1), ft, fr0, qd, clk);
+          ft = g + slot * L.G0 < kFt ? g + slot * L.G0 : -1;
+          if (ft >= 0) gather_conv1<LAYER>(acc, s_data, smem_u32(s_b1), ft, fr0, qd, clk);
         } else {
           ft = c_group_ft[2 * g + slot];
           const int s0 = c_group_step_off[g], s1 = c_group_step_off[g + 1];
@@ -1190,21 +1172,21 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         if (ft < 0) continue;
         // first / last tile of this slot's ascending range inside the item
         const bool first = (g == g0);
-        const bool last = (g == g1 - 1) || (ft == a.n_ft - 1);
-        const int n_valid = min(a.flt, a.wout - ft * a.flt) * a.cout;  // a multiple of 32 (contour: 64 in the last tile)
-        // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is 2 qd + e (COUT 8) or
-        // 8 (i % 4) + 2 qd + e (COUT 32).  Read here, after the conv1 MMAs, so that it holds no registers during the gather.
+        const bool last = (g == g1 - 1) || (ft == kFt - 1);
+        const int n_valid = min(L.FLT, L.WOUT - ft * L.FLT) * L.COUT;  // a multiple of 32 (contour: 64 in the last tile)
+        // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is (8 i + 2 qd + e) % COUT.
+        // Read here, after the conv1 MMAs, so that it holds no registers during the gather.
         float bz[4][2];
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
-          for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[EPI == 0 || EPI == 3 ? 2 * qd + e : 8 * i + 2 * qd + e];
-        if constexpr (EPI == 0) {
+          for (int e = 0; e < 2; ++e) bz[i][e] = a.bias1[(8 * i + 2 * qd + e) % L.COUT];
+        if constexpr (!kFused) {
           // contour: 16 bins x 8 channels, bias + ReLU, channels-last rows of 128 contiguous floats
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
             if (!live[rr]) continue;
-            float* dst = a.o.act + ((size_t)rb[rr] * kFrames + rt[rr]) * ((size_t)a.wout * a.cout) + (size_t)ft * 128;
+            float* dst = a.o.act + ((size_t)rb[rr] * kFrames + rt[rr]) * ((size_t)L.WOUT * L.COUT) + (size_t)ft * 128;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
               const int col = 8 * i + 2 * qd;
@@ -1233,7 +1215,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
               ah[r] = hu;
               al[r] = *reinterpret_cast<const uint32_t*>(&ll);
             }
-          // P[row][j * JS + dt] = sum over channels and frequency taps for output offset j and time tap dt (TcB2)
+          // P[row][j * JS + dt] = sum over channels and frequency taps for output offset j and time tap dt
           float p[NW / 2];
           wgmma_fence();
           conv2_mma<NW>(p, ah, al, smem_u32(s_b2));
@@ -1243,8 +1225,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
           // time taps: the frame of tile row r takes P_dt from row r - (KH2 - 1 - dt), taps added from the own row down
           // (the same order for every row: a frame's value does not depend on where the M-tile starts).  The sums go
           // through the staging area PC columns (PC / JS output offsets j) at a time.
-          constexpr int KH2 = B2.kh2, JS = B2.js, JP = PC / JS;
-          constexpr int NJ = EPI == 3 ? 20 : 6;
+          constexpr int KH2 = L.KH2, JS = L.js, JP = PC / JS;
+          constexpr int NJ = L.FLT + 2 * L.HALO;  // output bins whose sums the tile holds
           float S[NJ];
 #pragma unroll
           for (int q = 0; q * JP < NJ; ++q) {
@@ -1272,11 +1254,11 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
             }
           }
           if (tid < 64) {
-            if constexpr (EPI == 3) {
+            if constexpr (LAYER == 0) {
               finish_contour_tile(a, ro, S, ft, first, last, carry, hold);
             } else {
               float c2[2] = {carry[0], carry[1]};
-              finish_pitch_tile<EPI>(a, ro, S, c2, ft, first, last);
+              finish_pitch_tile<LAYER>(a, ro, S, c2, ft, first, last);
               carry[0] = c2[0];
               carry[1] = c2[1];
             }
@@ -1286,7 +1268,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       }
     }
     clk.lap(kClkConsOther);
-    clk.flush(a.layer);
+    clk.flush(LAYER);
   }
 }
 
@@ -1299,34 +1281,39 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
 struct EdgeFixArgs {
   TcOut o;
   int edge_rows, n_rows;        // rows of the (window, frame) space covered by the M-tiles
-  int n_edges;                  // 2 * n_split slots: slot e = s * n_split + q starts at tile q * n_groups / n_split + s * G0
-  int n_split, n_groups, g0, n_ft;
-  int layer, wout, rows_per_window, n_windows;
+  int n_edges;                  // 2 * n_split slots: slot e = s * n_split + q starts at tile q * G0 / n_split + s * G0
+  int n_split, n_windows;
   float bias2, note_w[9];  // the layer's conv2 bias; onset: the conv2 weights of the note input channel
 };
 
+// contour: one thread per (frame, edge); pitch layers: per (frame, edge, bin)
+template <int LAYER>
+constexpr int kEdgeThreads = LAYER == 0 ? 1 : 2 * tc_spec(LAYER).HALO;
+
+template <int LAYER>
 __global__ void edge_fix_kernel(const EdgeFixArgs a) {
+  constexpr TcConvSpec L = tc_spec(LAYER);
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int per_edge = a.layer == 0 ? 1 : 2;  // contour: one thread per (frame, edge); pitch layers: per (frame, edge, bin)
+  constexpr int per_edge = kEdgeThreads<LAYER>;
   const long long total = (long long)a.n_rows * a.n_edges * per_edge;
   if (idx >= total) return;
   const int R = (int)(idx % a.n_rows);  // rows fastest: coalesced reads of the edge buffer, coalesced stores
   const int ek = (int)(idx / a.n_rows);
   const int e = ek / per_edge, k = ek - e * per_edge;
-  const int b = R / a.rows_per_window, t = R - b * a.rows_per_window;
+  const int b = R / L.rows_per_window, t = R - b * L.rows_per_window;
   if (b >= a.n_windows || t >= kFrames) return;
   const int es = e / a.n_split, eq = e - es * a.n_split;
-  const int ft_b = eq * a.n_groups / a.n_split + es * a.g0;
-  if (ft_b <= 0 || ft_b >= a.n_ft) return;  // not a boundary between two ranges
+  const int ft_b = eq * L.G0 / a.n_split + es * L.G0;
+  if (ft_b <= 0 || ft_b >= L.n_ft()) return;  // not a boundary between two ranges
   int uf = -1;
   if (a.o.ud) {
     const UnwrapDesc u = a.o.ud[b];
     const int tt = t - kOverlapHalf;
     if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
   }
-  if (a.layer == 0) {
-    const float* lo = a.o.edge + (size_t)(e * 2 + 0) * 10 * a.edge_rows + R;  // from the range that starts at ft_b
-    const float* hi = a.o.edge + (size_t)(e * 2 + 1) * 10 * a.edge_rows + R;  // from the range that ends at ft_b - 1
+  if constexpr (LAYER == 0) {
+    const float* lo = a.o.edge + (size_t)(e * 2 + 0) * L.edge_per_side() * a.edge_rows + R;  // from the range that starts at ft_b
+    const float* hi = a.o.edge + (size_t)(e * 2 + 1) * L.edge_per_side() * a.edge_rows + R;  // from the range that ends at ft_b - 1
     float fx[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q)  // (S + carry) + bias, the order of the in-kernel carry
@@ -1357,10 +1344,10 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
     }
     return;
   }
-  const int f = 4 * ft_b - 1 + k;
-  if (f < 0 || f >= a.wout) return;
-  float x = (a.o.edge[((size_t)(e * 2 + 0) * 2 + k) * a.edge_rows + R] +
-             a.o.edge[((size_t)(e * 2 + 1) * 2 + k) * a.edge_rows + R]) + a.bias2;  // (S + carry) + bias
+  const int f = L.FLT * ft_b - L.HALO + k;
+  if (f < 0 || f >= L.WOUT) return;
+  float x = (a.o.edge[((size_t)(e * 2 + 0) * L.edge_per_side() + k) * a.edge_rows + R] +
+             a.o.edge[((size_t)(e * 2 + 1) * L.edge_per_side() + k) * a.edge_rows + R]) + a.bias2;  // (S + carry) + bias  // (S + carry) + bias
   if (a.o.note_raw) {
 #pragma unroll
     for (int dt = 0; dt < 3; ++dt)
@@ -1382,10 +1369,11 @@ int tc_rows_total(int n_windows, int rows_per_window) {
 }
 
 int tc_setup() {
-  cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::tc_smem(0).total());
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::tc_smem(1).total());
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::tc_smem(2).total());
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::tc_smem(3).total());
+  using namespace tc;
+  cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(0, false).total());
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(1, true).total());
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(2, true).total());
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(0, true).total());
   return e == cudaSuccess ? 0 : -1;
 }
 
@@ -1400,48 +1388,48 @@ void launch_lognorm_split(const float* y, const unsigned int* minmax, const floa
 size_t tc_edge_floats(const TcConvSpec& sp, int n_windows) {
   const int ms = tc::kMTile - (sp.KH2 - 1);
   const int n_mtiles = (n_windows * sp.rows_per_window + ms - 1) / ms;
-  const int per_side = sp.epi == 0 ? 10 : 2;
-  return (size_t)2 * sp.G0 * 2 * per_side * ((size_t)n_mtiles * ms);  // at most 2 * G0 range starts
+  return (size_t)2 * sp.G0 * 2 * sp.edge_per_side() * ((size_t)n_mtiles * ms);  // at most 2 * G0 range starts
+}
+
+// The conv kernel of one layer and, for a fused epilogue, the fix-up of the bins where two tile ranges meet.
+template <int LAYER, bool FUSED>
+static void launch_layer(const TcArgs& a, const EdgeFixArgs& ef, int grid, cudaStream_t st) {
+  conv_tc_kernel<LAYER, FUSED><<<grid, tc::kThreads, tc::tc_smem(LAYER, FUSED).total(), st>>>(a);
+  if (FUSED) {
+    const long long total = (long long)ef.n_rows * ef.n_edges * kEdgeThreads<LAYER>;
+    edge_fix_kernel<LAYER><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ef);
+  }
 }
 
 void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& o, int n_windows, int rows_stride,
                     int n_sms, cudaStream_t st, bool fuse_next) {
-  const TcConvSpec& sp = dev.spec;
-  const bool fused = sp.epi != 0 || fuse_next;
+  const TcConvSpec sp = tc_spec(dev.layer);
+  const bool fused = dev.layer != 0 || fuse_next;
   TcArgs a{};
   a.data = data;
   a.tiles = dev.tiles;
   a.b1 = dev.b1;
   a.b2 = dev.b2;
   a.o = o;
-  a.layer = dev.layer;
   a.rows_total = rows_stride;  // row stride of the split layout (fixed per model, independent of the batch)
   a.h2 = fused ? (sp.KH2 - 1) / 2 : 0;
   a.ms = tc::kMTile - 2 * a.h2;
   a.n_mtiles = (n_windows * sp.rows_per_window + a.ms - 1) / a.ms;
   a.edge_rows = a.n_mtiles * a.ms;
   a.n_windows = n_windows;
-  a.n_groups = dev.n_groups;
   // An item is (M-tile, one of `split` runs of frequency groups).  Pick the split that minimises the number of waves
   // times the work per item, the data-tile load counted as half a group: full chunks run unsplit, partial chunks and
   // small batches spread over all SMs.
   int split = 1;
   double best = 1e30;
-  for (int s = 1; s <= dev.n_groups; ++s) {
+  for (int s = 1; s <= sp.G0; ++s) {  // G0 groups
     const int waves = (a.n_mtiles * s + n_sms - 1) / n_sms;
-    const double cost = waves * ((dev.n_groups + s - 1) / s + 0.5);
+    const double cost = waves * ((sp.G0 + s - 1) / s + 0.5);
     if (cost < best - 1e-9) best = cost, split = s;
   }
   a.n_split = split;
-  a.data_rows = tc::kMTile + sp.KH - 1;
   a.row0 = sp.lead_rows - sp.PT - a.h2;
   a.chunks8 = sp.chunks8;
-  a.rows_per_window = sp.rows_per_window;
-  a.cout = sp.COUT;
-  a.flt = sp.FLT;
-  a.wout = sp.WOUT;
-  a.n_ft = (sp.WOUT + sp.FLT - 1) / sp.FLT;
-  a.g0 = sp.G0;
   std::copy_n(dev.bias1, 32, a.bias1);
   a.bias2 = dev.bias2;
   std::copy_n(dev.note_w, 9, a.note_w);
@@ -1470,7 +1458,7 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
     if (encode && want_tmap) {
       const cuuint64_t dims[4] = {8, (cuuint64_t)rows_stride, (cuuint64_t)sp.chunks8, 2};
       const cuuint64_t strides[3] = {16, (cuuint64_t)rows_stride * 16, (cuuint64_t)sp.chunks8 * rows_stride * 16};
-      const cuuint32_t box[4] = {8, (cuuint32_t)a.data_rows, (cuuint32_t)(sp.chunks8 - 1), 2};
+      const cuuint32_t box[4] = {8, (cuuint32_t)(tc::kMTile + sp.KH - 1), (cuuint32_t)(sp.chunks8 - 1), 2};
       const cuuint32_t estr[4] = {1, 1, 1, 1};
       if (encode(&a.data_map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<__nv_bfloat16*>(data), dims, strides, box, estr,
                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -1478,33 +1466,24 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
         a.use_tmap = 1;
     }
   }
-  if (sp.epi == 0 && fuse_next)
-    conv_tc_kernel<3><<<grid, tc::kThreads, tc::tc_smem(3).total(), st>>>(a);
-  else if (sp.epi == 0)
-    conv_tc_kernel<0><<<grid, tc::kThreads, tc::tc_smem(0).total(), st>>>(a);
-  else if (sp.epi == 1)
-    conv_tc_kernel<1><<<grid, tc::kThreads, tc::tc_smem(1).total(), st>>>(a);
+  // slot s of split q covers tiles [g0(q) + s*G0, g1(q) + s*G0): edge slot s*split + q
+  EdgeFixArgs ef{};
+  ef.o = o;
+  ef.edge_rows = a.edge_rows;
+  ef.n_rows = n_windows * sp.rows_per_window;
+  ef.n_edges = 2 * split;
+  ef.n_split = split;
+  ef.n_windows = n_windows;
+  ef.bias2 = dev.bias2;
+  std::copy_n(dev.note_w, 9, ef.note_w);
+  if (dev.layer == 1)
+    launch_layer<1, true>(a, ef, grid, st);
+  else if (dev.layer == 2)
+    launch_layer<2, true>(a, ef, grid, st);
+  else if (fuse_next)
+    launch_layer<0, true>(a, ef, grid, st);
   else
-    conv_tc_kernel<2><<<grid, tc::kThreads, tc::tc_smem(2).total(), st>>>(a);
-  if (fused) {  // slot s of split q covers tiles [g0(q) + s*G0, g1(q) + s*G0): edge slot s*split + q
-    EdgeFixArgs ef{};
-    ef.o = o;
-    ef.edge_rows = a.edge_rows;
-    ef.n_rows = n_windows * sp.rows_per_window;
-    ef.n_edges = 2 * split;
-    ef.n_split = split;
-    ef.n_groups = dev.n_groups;
-    ef.g0 = sp.G0;
-    ef.n_ft = a.n_ft;
-    ef.layer = sp.epi;  // 0 contour, 1 onset, 2 note
-    ef.wout = sp.WOUT;
-    ef.rows_per_window = sp.rows_per_window;
-    ef.n_windows = n_windows;
-    ef.bias2 = dev.bias2;
-    std::copy_n(dev.note_w, 9, ef.note_w);
-    const long long total = (long long)ef.n_rows * ef.n_edges * (sp.epi == 0 ? 1 : 2);
-    edge_fix_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ef);
-  }
+    launch_layer<0, false>(a, ef, grid, st);
 }
 
 }  // namespace bp

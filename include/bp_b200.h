@@ -253,7 +253,7 @@ int bp_debug_tc_plan(int which, const float* w, int32_t* sizes, uint16_t* tiles,
                      int32_t* group_step_off, int32_t* group_ft);
 
 /* Host-only: the conv1 of the onset (which = 1, w = [32][8][5][5]) or note (which = 2, w = [32][1][7][7]) layer as the
- * kernel computes it, an implicit GEMM with a gathered A operand (csrc/tc_conv.cu, TcGather).  sizes[4] = {K, n_ci, KH,
+ * kernel computes it, an implicit GEMM with a gathered A operand (csrc/tc_conv.cu, tc_build_b1).  sizes[4] = {K, n_ci, KH,
  * wout}; b1 (may be NULL): the two B matrices, [parity of the output bin 2][plane hi/lo][K / 8][32][8] bf16, row
  * k = 8 (dt * n_ci + ci) + j (the 8-bin-window form; the kernel's own K order is bp_debug_tc_gather_packed); starts (may
  * be NULL): [wout][n_ci] first input bin of the window of output bin f and channel ci; ranges (may be NULL): [n_ci][2]
@@ -264,7 +264,7 @@ int bp_debug_tc_gather(int which, const float* w, int32_t* sizes, uint16_t* b1, 
  * for K padding.  Window starts and ranges are those of bp_debug_tc_gather. */
 int bp_debug_tc_gather_packed(int which, const float* w, int32_t* sizes, uint16_t* b1, int32_t* kmap);
 
-/* Host-only: the bf16 hi/lo weight tiles of the fused SECOND convolution of a tensor-core layer (csrc/tc_conv.cu, TcB2):
+/* Host-only: the bf16 hi/lo weight tiles of the fused SECOND convolution of a tensor-core layer (csrc/tc_conv.cu, tc_build_b2):
  * which = 0 contour conv2 (w2 = [1][8][5][5], reference models.py:254-262), 1 onset conv2 ([1][33][3][3], models.py:305-313),
  * 2 note conv2 ([1][32][7][3], models.py:282-290).  sizes[5] = {n_tiles, N, time taps, accumulator columns, columns per output offset}; tiles
  * (may be NULL to query sizes): n_tiles x [plane hi/lo][k-chunk 2][n N][8] bf16. */
