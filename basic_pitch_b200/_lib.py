@@ -24,7 +24,7 @@ EXPORTS = [
     "bp_model_create", "bp_model_destroy", "bp_model_device", "bp_model_param_block", "bp_model_refresh",
     "bp_model_launch_count", "bp_forward_device", "bp_forward_host", "bp_run_inference_device",
     "bp_run_inference_host", "bp_decode_device", "bp_decode_host", "bp_transcribe_host", "bp_transcribe_device",
-    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host",
+    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout",
 ]  # fmt: skip
 
 
@@ -54,6 +54,17 @@ class Notes(C.Structure):
         ("amplitude", C.c_void_p),
         ("bend_off", C.c_void_p),
         ("bends", C.c_void_p),
+    ]
+
+
+class PcmFile(C.Structure):
+    _fields_ = [
+        ("pcm", C.c_void_p),
+        ("n_frames", C.c_int64),
+        ("sample_format", C.c_int32),
+        ("channels", C.c_int32),
+        ("sample_rate", C.c_int32),
+        ("reserved", C.c_int32),
     ]
 
 
@@ -125,6 +136,10 @@ def load() -> C.CDLL:
     lib.bp_resampled_length.restype = i64
     lib.bp_load_pcm_device.argtypes = [vp, vp, i32, i64, i32, i32, vp, vp]
     lib.bp_load_pcm_host.argtypes = [vp, vp, i32, i64, i32, i32, vp]
+    lib.bp_load_pcm_files_device.argtypes = [vp, C.POINTER(PcmFile), i32, vp, vp, vp]
+    lib.bp_transcribe_pcm_files_host.argtypes = [vp, C.POINTER(PcmFile), i32, C.POINTER(DecodeParams), vp, vp, vp, vp, vp,
+                                                 C.POINTER(Notes)]
+    lib.bp_debug_pcm_layout.argtypes = [C.POINTER(PcmFile), i32, vp, vp]
     lib.bp_debug_resample_filter.argtypes = [i32, i32, vp, i64]
     lib.bp_debug_resample_filter.restype = i64
     lib.bp_write_note_files.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, C.c_double, i32]

@@ -1,5 +1,6 @@
 """Audio file -> mono float32 at 22 050 Hz, in front of the hot path: `load_audio` on the host (NumPy / SciPy),
-`load_audio_device` with the conversion, down-mix and resampling on the GPU (csrc/ingest.cu, same filter).
+`load_audio_device` with the conversion, down-mix and resampling on the GPU (csrc/ingest.cu, same filter); `read_pcm` +
+`pcm_descriptors` hand the stored samples of a whole batch of files to the batched ingest (`Model.transcribe_pcm`).
 
 Stands in for `librosa.load(path, sr=22050, mono=True)` (reference: basic_pitch/inference.py:239).
 WAV files are decoded with scipy; other containers need `soundfile` (optional).  Files that are not
@@ -12,7 +13,7 @@ from __future__ import annotations
 
 import pathlib
 from math import gcd
-from typing import Tuple, Union
+from typing import Sequence, Tuple, Union
 
 import numpy as np
 
@@ -73,6 +74,29 @@ def read_pcm(path: Union[str, pathlib.Path]) -> Tuple[np.ndarray, int]:
     except Exception:
         x, sr = read_audio(path)
         return x, sr
+
+
+def pcm_descriptors(items: Sequence[Tuple[np.ndarray, int]]):
+    """Stored samples of a batch of files -> the `bp_pcm_file_t` array the batched ingest takes (`bp_load_pcm_files_device`,
+    `bp_transcribe_pcm_files_host`) plus the arrays it points into, which the caller keeps alive for the call.  An item is
+    (samples, sample_rate) as `read_pcm` returns them: (n,) or (n, channels) float32 / int16 / int32 / uint8; samples
+    that are not C-contiguous are copied.  The library packs the PCM itself, sub-batch by sub-batch."""
+    from . import _lib
+
+    keep = []
+    files = (_lib.PcmFile * max(len(items), 1))()
+    for f, (x, sr) in zip(files, items):
+        x = np.asarray(x)
+        if x.dtype not in _PCM_FORMATS:
+            raise ValueError(f"unsupported sample dtype {x.dtype}: the device ingest takes float32, int16, int32 and uint8")
+        if x.ndim not in (1, 2):
+            raise ValueError(f"samples must be (n,) or (n, channels), got shape {x.shape}")
+        x = np.ascontiguousarray(x)
+        keep.append(x)
+        f.pcm = x.ctypes.data if x.size else None
+        f.n_frames, f.channels = (x.shape[0], 1) if x.ndim == 1 else x.shape
+        f.sample_format, f.sample_rate = _PCM_FORMATS[x.dtype], int(sr)
+    return files, keep
 
 
 def load_audio_device(path: Union[str, pathlib.Path], model) -> Tuple[np.ndarray, int]:

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -167,10 +168,21 @@ struct bp_model {
   // staging for the host entry points
   DevBuf<float> st_audio, st_note, st_onset, st_contour;
   DevBuf<unsigned char> st_pcm;  // bp_load_pcm_host
-  // pinned gather buffers of per-file input (one sub-batch of audio each); the device->host stream of the posteriorgrams
-  // and its events
-  float* gather[3] = {nullptr, nullptr, nullptr};
-  size_t gather_cap = 0;  // floats per buffer
+  // pinned gather buffers of per-file input (one sub-batch each: float32 audio, or the descriptors and stored PCM of
+  // bp_transcribe_pcm_files_host); the device->host stream of the posteriorgrams and its events
+  unsigned char* gather[3] = {nullptr, nullptr, nullptr};
+  size_t gather_cap = 0;  // bytes per buffer
+  // device side of the PCM sub-batches: upload k + 1 fills one buffer while the ingest of k reads the other;
+  // ingest_ev[k] (compute stream, after the ingest of sub-batch k) frees its buffer for sub-batch k + 2
+  DevBuf<unsigned char> pcm_ring[2];
+  std::vector<cudaEvent_t> ingest_ev;
+  // bp_load_pcm_files_device: descriptors in pinned staging and on the device; the events say when the staging has been
+  // read (host may rewrite it) and when the kernel is done with the device copy (a later call may overwrite it)
+  unsigned char* h_ingest = nullptr;
+  size_t h_ingest_cap = 0;
+  DevBuf<unsigned char> d_ingest;
+  cudaEvent_t ingest_copied = nullptr, ingest_done = nullptr;
+  bool ingest_pending = false;
   cudaStream_t d2h_stream = nullptr;
   std::vector<cudaEvent_t> conv_ev;
   // decode workspace
@@ -651,7 +663,8 @@ void bp_model_destroy(bp_model_t* m) {
   m->i_note.release(); m->i_onset.release(); m->i_contour.release(); m->u_note.release(); m->u_onset.release();
   m->u_contour.release();
   m->wdesc.release(); m->udesc.release(); m->st_audio.release(); m->st_note.release(); m->st_onset.release();
-  m->st_contour.release(); m->st_pcm.release(); m->d_frame_off.release(); m->d_slot_off.release(); m->d_note_base.release();
+  m->st_contour.release(); m->st_pcm.release(); m->pcm_ring[0].release(); m->pcm_ring[1].release(); m->d_ingest.release();
+  m->d_frame_off.release(); m->d_slot_off.release(); m->d_note_base.release();
   m->energy.release(); m->d_amp.release(); m->candbits.release(); m->blk_max.release(); m->blk_arg.release(); m->max_onset.release(); m->max_fd.release();
   m->note_count.release(); m->slot_start.release(); m->slot_end.release(); m->slot_pitch.release();
   m->overflow.release(); m->d_note_off.release(); m->d_start.release(); m->d_end.release(); m->d_pitch.release();
@@ -670,9 +683,13 @@ void bp_model_destroy(bp_model_t* m) {
   for (cudaEvent_t e : m->copy_ev) cudaEventDestroy(e);
   if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
   if (m->d2h_stream) cudaStreamDestroy(m->d2h_stream);
-  for (float* b : m->gather)
+  for (unsigned char* b : m->gather)
     if (b) cudaFreeHost(b);
   for (cudaEvent_t e : m->conv_ev) cudaEventDestroy(e);
+  for (cudaEvent_t e : m->ingest_ev) cudaEventDestroy(e);
+  if (m->h_ingest) cudaFreeHost(m->h_ingest);
+  if (m->ingest_copied) cudaEventDestroy(m->ingest_copied);
+  if (m->ingest_done) cudaEventDestroy(m->ingest_done);
   if (m->stream) cudaStreamDestroy(m->stream);
   delete m;
 }
@@ -829,20 +846,26 @@ static int run_inference_internal(bp_model* m, const float* d_audio, const int64
 namespace {
 // Host threads that copy the files of one sub-batch after the other into pinned staging buffers, running ahead of the
 // caller: worker t copies its share of sub-batch k as soon as the caller has released that buffer (`released` counts the
-// sub-batches whose buffer may be overwritten) and reports it in done[k].  The threads live for one call.
+// sub-batches whose buffer may be overwritten) and reports it in done[k].  The threads live for one call.  Files are
+// bytes here: file i is src[i][0 .. len[i]) and lands off[i] - off[first file of its sub-batch] bytes behind the
+// sub-batch's header (float32 audio: no header, off = 4 x the sample offsets; stored PCM: gaps that start every file on a
+// 16-byte boundary).
 struct Gatherer {
-  const float* const* audio;
-  const int64_t* rel;        // [n_files + 1] sample offsets
+  const unsigned char* const* src;
+  const int64_t* off;        // [n_files + 1] non-decreasing byte offsets, off[i] + len[i] <= off[i + 1]
+  const int64_t* len;        // [n_files]
+  const int64_t* head;       // [n_sub] bytes the caller keeps at the front of each sub-batch's buffer
   const int* cut;            // [n_sub + 1] file index where each sub-batch starts
   int n_sub, n_threads;
-  float* const* stage;       // 3 staging buffers
+  unsigned char* const* stage;  // 3 staging buffers
   std::atomic<int> released{0};
   std::vector<std::atomic<int>> done;
   std::vector<std::thread> threads;
   std::atomic<bool> abort{false};
 
-  Gatherer(const float* const* a, const int64_t* r, const int* c, int ns, int nt, float* const* st)
-      : audio(a), rel(r), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
+  Gatherer(const unsigned char* const* s, const int64_t* o, const int64_t* l, const int64_t* h, const int* c, int ns, int nt,
+           unsigned char* const* st)
+      : src(s), off(o), len(l), head(h), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
     for (auto& d : done) d.store(0);
     for (int t = 0; t < n_threads; ++t) threads.emplace_back([this, t] { run(t); });
   }
@@ -860,15 +883,15 @@ struct Gatherer {
           std::this_thread::sleep_for(std::chrono::microseconds(50));  // do not fight the enqueueing thread for cores
       }
       const int f0 = cut[k], f1 = cut[k + 1];
-      const int64_t base = rel[f0], total = rel[f1] - base;
-      float* dst = stage[k % 3];
-      // thread t copies samples [lo, hi) of the sub-batch: whole files where possible, split files otherwise
+      const int64_t base = off[f0], total = off[f1] - base;
+      unsigned char* dst = stage[k % 3] + head[k];
+      // thread t copies bytes [lo, hi) of the sub-batch: whole files where possible, split files otherwise
       const int64_t lo = base + total * t / n_threads, hi = base + total * (t + 1) / n_threads;
       if (hi > lo) {
-        int i = (int)(std::upper_bound(rel + f0, rel + f1 + 1, lo) - rel) - 1;
-        for (; i < f1 && rel[i] < hi; ++i) {
-          const int64_t a = std::max(lo, rel[i]), b = std::min(hi, rel[i + 1]);
-          if (b > a) std::memcpy(dst + (a - base), audio[i] + (a - rel[i]), sizeof(float) * (size_t)(b - a));
+        int i = (int)(std::upper_bound(off + f0, off + f1 + 1, lo) - off) - 1;
+        for (; i < f1 && off[i] < hi; ++i) {
+          const int64_t a = std::max(lo, off[i]), b = std::min(hi, off[i] + len[i]);
+          if (b > a) std::memcpy(dst + (a - base), src[i] + (a - off[i]), (size_t)(b - a));
         }
       }
       done[k].fetch_add(1, std::memory_order_release);
@@ -881,16 +904,29 @@ struct Gatherer {
 };
 
 // A batch of whole files as an entry point received it: packed back to back (`audio`, in device memory if `on_device`,
-// else in host memory) or one host pointer per file (`files`).
+// else in host memory), one host pointer per file (`files`), or one host pointer per file to its stored PCM (`pcm`),
+// which the device ingest turns into the 22 050 Hz signals the other two kinds start from.
 struct Batch {
   const char* api;             // the calling entry point, prefix of every message
   const float* audio;          // packed: the caller's array; describe_batch moves it to the first file's samples
   bool on_device;
   const float* const* files;
-  std::vector<int64_t> rel{};  // [n_files + 1] sample offsets from the first file (describe_batch)
+  const bp_pcm_file_t* pcm = nullptr;
+  std::vector<int64_t> rel{};  // [n_files + 1] sample offsets (22 050 Hz) from the first file (describe_batch)
   int64_t total_frames = 0;    // frames of the posteriorgrams (describe_batch)
+  std::vector<IngestFile> ingest{};  // pcm: each file's resampler, lengths and format (describe_pcm)
+  std::vector<int64_t> pcm_bytes{};  // pcm: each file's stored size
   int n_files() const { return (int)rel.size() - 1; }
+  bool per_file() const { return files || pcm; }  // gathered into pinned staging sub-batch by sub-batch
 };
+
+constexpr int kPcmSampleBytes[4] = {4, 2, 4, 1};
+constexpr int64_t align16(int64_t n) { return (n + 15) & ~(int64_t)15; }
+// The front of a PCM sub-batch of nf files, on the host and on the device: IngestFile [nf], then the CTA prefix
+// int [nf + 1], padded so that the PCM behind it starts on a 16-byte boundary.
+constexpr int64_t ingest_header_bytes(int nf) {
+  return align16((int64_t)nf * (int64_t)sizeof(IngestFile) + ((int64_t)nf + 1) * (int64_t)sizeof(int));
+}
 
 struct Rows {
   float *note, *onset, *contour;
@@ -916,14 +952,85 @@ static int describe_batch(Batch& b, const int64_t* sample_off, const int64_t* n_
   return BP_OK;
 }
 
+// Validates every stored-PCM file of a batch, host arithmetic only: -> each file's resampler geometry, frame counts in
+// and out (`ingest`, pointers unset) and stored bytes.  `device_pcm`: the pointers are dereferenced by the kernel as they
+// are, so they must be aligned to their sample type.
+static int describe_pcm(const std::string& api, const bp_pcm_file_t* files, int32_t n_files, bool device_pcm,
+                        std::vector<IngestFile>& ingest, std::vector<int64_t>& bytes) {
+  ingest.assign(n_files, IngestFile{});
+  bytes.assign(n_files, 0);
+  int64_t ctas = 0;
+  for (int i = 0; i < n_files; ++i) {
+    const bp_pcm_file_t& f = files[i];
+    const std::string who = api + ": file " + std::to_string(i);
+    if (f.n_frames < 0) return fail(BP_E_INVALID, who + " has a negative length");
+    if (f.sample_format < 0 || f.sample_format > 3)
+      return fail(BP_E_INVALID, who + ": sample_format must be 0 (float32), 1 (int16), 2 (int32) or 3 (uint8)");
+    if (f.channels < 1) return fail(BP_E_INVALID, who + ": channels must be >= 1");
+    if (f.sample_rate < 1) return fail(BP_E_INVALID, who + ": sample_rate must be >= 1");
+    if (ingest_geometry(f.sample_format, f.channels, f.sample_rate, ingest[i]) != 0)
+      return fail(BP_E_INVALID, who + ": the ratio of " + std::to_string(f.sample_rate) +
+                                    " Hz to 22 050 Hz is beyond the resampler's shared-memory limit (~100:1)");
+    const int64_t frame_bytes = (int64_t)f.channels * kPcmSampleBytes[f.sample_format];
+    if (f.n_frames > (INT64_MAX >> 16) / frame_bytes) return fail(BP_E_INVALID, who + " is too long");
+    if (f.n_frames > 0 && !f.pcm) return fail(BP_E_INVALID, who + ": null pcm");
+    if (device_pcm && reinterpret_cast<uintptr_t>(f.pcm) % kPcmSampleBytes[f.sample_format] != 0)
+      return fail(BP_E_INVALID, who + ": pcm is not aligned to its sample type");
+    bytes[i] = f.n_frames * frame_bytes;
+    ingest[i].n_in = f.n_frames;
+    ingest[i].n_out = ingest_output_length(f.n_frames, f.sample_rate);
+    ctas += ingest_ctas(ingest[i].n_out);
+    if (ctas > INT_MAX) return fail(BP_E_INVALID, who + ": the batch is too long for one ingest");
+  }
+  return BP_OK;
+}
+
+// The device's polyphase taps for every file (designed and uploaded on the first use of a ratio).
+static int load_ingest_taps(const std::string& api, int device, std::vector<IngestFile>& ingest) {
+  for (IngestFile& f : ingest) {
+    const int rc = ingest_taps(device, f);
+    if (rc) {
+      cudaGetLastError();
+      return fail(rc == -1 ? BP_E_CUDA : BP_E_INVALID, api + ": resampler filter of ratio " + std::to_string(f.up) + "/" +
+                                                           std::to_string(f.down) + " could not be set up");
+    }
+  }
+  return BP_OK;
+}
+
+// Writes the header of a batched ingest (ingest_header_bytes) over files whose pcm / out pointers are set.
+// -> CTAs of the launch; *max_span: the shared memory it needs, in staged inputs.
+static int write_ingest_header(unsigned char* h, const IngestFile* f, int nf, int* max_span) {
+  std::memcpy(h, f, sizeof(IngestFile) * (size_t)nf);
+  int* cta_off = reinterpret_cast<int*>(h + sizeof(IngestFile) * (size_t)nf);
+  cta_off[0] = 0;
+  *max_span = 1;
+  for (int i = 0; i < nf; ++i) {
+    cta_off[i + 1] = cta_off[i] + (int)ingest_ctas(f[i].n_out);
+    if (f[i].n_out > 0) *max_span = std::max(*max_span, f[i].span);
+  }
+  return cta_off[nf];
+}
+
+// The batched ingest over a header in device memory.
+static int launch_ingest_header(bp_model* m, const unsigned char* d_header, int nf, int n_ctas, int max_span, cudaStream_t st) {
+  if (n_ctas == 0) return BP_OK;
+  const int rc = launch_ingest_batch(reinterpret_cast<const IngestFile*>(d_header),
+                                     reinterpret_cast<const int*>(d_header + sizeof(IngestFile) * (size_t)nf), nf, n_ctas,
+                                     max_span, st);
+  if (rc) return fail(BP_E_CUDA, std::string("batched ingest: ") + cudaGetErrorString(cudaGetLastError()));
+  m->launches += 1;
+  return BP_OK;
+}
+
 // Sub-batches of whole files, as the index of each one's first file plus n_files.  Device input is one sub-batch.  On
 // host input the first two hold at most one chunk of windows (their uploads are the ones the kernels cannot hide), the
-// next two at most two and the rest at most four; two for per-file input, whose three pinned staging buffers each hold
-// a whole sub-batch, so that the cap bounds their size.
+// next two at most two and the rest at most four; two for per-file input (float32 or PCM), whose three pinned staging
+// buffers each hold a whole sub-batch, so that the cap bounds their size.
 static std::vector<int> cut_sub_batches(const Batch& b, int64_t chunk) {
   const int n_files = b.n_files();
   if (b.on_device) return {0, n_files};
-  const int64_t cap = b.files ? 2 : 4;
+  const int64_t cap = b.per_file() ? 2 : 4;
   std::vector<int> cut{0};
   int64_t w = 0;
   for (int i = 0; i < n_files; ++i) {
@@ -942,8 +1049,9 @@ static std::vector<int> cut_sub_batches(const Batch& b, int64_t chunk) {
 
 // The whole-file pipeline of every bp_run_inference_* / bp_transcribe_* entry point: windows -> forward -> unwrap ->
 // row-major posteriorgrams in `rows` (device memory; the model's staging when null), sub-batch by sub-batch
-// (cut_sub_batches).  Host input is uploaded on the copy stream ahead of the kernels, and the posteriorgrams of each
-// sub-batch go to `host` (any may be null) on the device->host stream while later ones compute.  Then the decode, if
+// (cut_sub_batches).  Host input is uploaded on the copy stream ahead of the kernels (stored PCM: followed by one batched
+// ingest per sub-batch, which writes its 22 050 Hz signals where the upload of float32 input would have put them), and the
+// posteriorgrams of each sub-batch go to `host` (any may be null) on the device->host stream while later ones compute.  Then the decode, if
 // `params` is given.  Device input only enqueues on `st` (the decode synchronises it); host input returns synchronised.
 static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, const bp_decode_params_t* params,
                      bp_notes_t* notes, int64_t* h_frame_off, cudaStream_t st) {
@@ -969,18 +1077,37 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
     if ((rc = ensure_events(m->conv_ev, n_sub))) return rc;
   }
   int n_threads = 0;
-  if (b.files) {
-    size_t max_sub = 1;
-    for (int k = 0; k < n_sub; ++k) max_sub = std::max<size_t>(max_sub, (size_t)(b.rel[cut[k + 1]] - b.rel[cut[k]]));
+  // per-file input as the gather threads see it: bytes (Gatherer)
+  std::vector<const unsigned char*> src;
+  std::vector<int64_t> off, len, head;
+  if (b.per_file()) {
+    src.resize(n_files);
+    off.assign(n_files + 1, 0);
+    len.resize(n_files);
+    head.assign(n_sub, 0);
+    for (int i = 0; i < n_files; ++i) {
+      src[i] = static_cast<const unsigned char*>(b.pcm ? b.pcm[i].pcm : static_cast<const void*>(b.files[i]));
+      len[i] = b.pcm ? b.pcm_bytes[i] : (int64_t)sizeof(float) * (b.rel[i + 1] - b.rel[i]);
+      off[i + 1] = off[i] + (b.pcm ? align16(len[i]) : len[i]);
+    }
+    size_t max_sub = 1;  // sized by what is staged: PCM bytes can be many times the samples they become
+    for (int k = 0; k < n_sub; ++k) {
+      if (b.pcm) head[k] = ingest_header_bytes(cut[k + 1] - cut[k]);
+      max_sub = std::max<size_t>(max_sub, (size_t)(head[k] + off[cut[k + 1]] - off[cut[k]]));
+    }
     if (max_sub > m->gather_cap) {
-      for (float*& g : m->gather) {
+      for (unsigned char*& g : m->gather) {
         if (g) cudaFreeHost(g);
         g = nullptr;
       }
       m->gather_cap = 0;
       const size_t want = max_sub + max_sub / 8;
-      for (float*& g : m->gather) CK(cudaHostAlloc(&g, want * sizeof(float), cudaHostAllocDefault));
+      for (unsigned char*& g : m->gather) CK(cudaHostAlloc(&g, want, cudaHostAllocDefault));
       m->gather_cap = want;
+    }
+    if (b.pcm) {
+      for (DevBuf<unsigned char>& d : m->pcm_ring) CK(d.reserve(max_sub));
+      if ((rc = ensure_events(m->ingest_ev, n_sub))) return rc;
     }
     n_threads = (int)std::max(1u, std::min(16u, std::thread::hardware_concurrency() > 2 ? std::thread::hardware_concurrency() - 1 : 1u));
   }
@@ -991,8 +1118,8 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
   double t_gather = 0, t_wait = 0, t_launch = 0;
   if (from_host) CK(cudaStreamSynchronize(st));  // st_audio / st_note.. may still be in use by earlier work on the compute stream
   std::unique_ptr<Gatherer> gatherer;
-  if (b.files) {
-    gatherer.reset(new Gatherer(b.files, b.rel.data(), cut.data(), n_sub, n_threads, m->gather));
+  if (b.per_file()) {
+    gatherer.reset(new Gatherer(src.data(), off.data(), len.data(), head.data(), cut.data(), n_sub, n_threads, m->gather));
     gatherer->release_upto(std::min(3, n_sub));  // the three buffers are free: the workers start at once
   }
   h_frame_off[0] = 0;
@@ -1009,11 +1136,29 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
           t_gather += ms_since(t0);
           t0 = now();
         }
-        const float* src = gatherer ? m->gather[k % 3] : b.audio + s0;
-        if (s1 > s0)
-          CK(cudaMemcpyAsync(m->st_audio.p + s0, src, sizeof(float) * (size_t)(s1 - s0), cudaMemcpyHostToDevice, m->copy_stream));
-        CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
-        CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
+        if (b.pcm) {  // descriptors + PCM up in one copy, then the ingest writes st_audio[s0, s1)
+          const int nf = f1 - f0;
+          unsigned char* d_sub = m->pcm_ring[k % 2].p;
+          std::vector<IngestFile> desc(b.ingest.begin() + f0, b.ingest.begin() + f1);
+          for (int i = 0; i < nf; ++i) {
+            desc[i].pcm = d_sub + head[k] + (off[f0 + i] - off[f0]);
+            desc[i].out = m->st_audio.p + b.rel[f0 + i];
+          }
+          int max_span = 1;
+          const int n_ctas = write_ingest_header(m->gather[k % 3], desc.data(), nf, &max_span);
+          if (k >= 2) CK(cudaStreamWaitEvent(m->copy_stream, m->ingest_ev[k - 2], 0));  // the ingest that last read d_sub
+          CK(cudaMemcpyAsync(d_sub, m->gather[k % 3], (size_t)(head[k] + off[f1] - off[f0]), cudaMemcpyHostToDevice, m->copy_stream));
+          CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
+          CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
+          if ((rc = launch_ingest_header(m, d_sub, nf, n_ctas, max_span, st))) return rc;
+          CK(cudaEventRecord(m->ingest_ev[k], st));
+        } else {
+          const void* from = gatherer ? static_cast<const void*>(m->gather[k % 3]) : b.audio + s0;
+          if (s1 > s0)
+            CK(cudaMemcpyAsync(m->st_audio.p + s0, from, sizeof(float) * (size_t)(s1 - s0), cudaMemcpyHostToDevice, m->copy_stream));
+          CK(cudaEventRecord(m->copy_ev[k], m->copy_stream));
+          CK(cudaStreamWaitEvent(st, m->copy_ev[k], 0));
+        }
       }
       const int64_t base = h_frame_off[f0];  // run_inference_internal writes the offsets relative to it
       rc = run_inference_internal(m, from_host ? m->st_audio.p : b.audio, b.rel.data() + f0, f1 - f0, u, base,
@@ -1445,6 +1590,94 @@ int bp_load_pcm_host(bp_model_t* m, const void* h_pcm, int32_t sample_format, in
   if (rc) return rc;
   CK(cudaMemcpyAsync(h_audio, m->st_audio.p, sizeof(float) * (size_t)n_out, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, float* d_audio,
+                             int64_t* h_sample_off, void* stream) {
+  if (!m || !h_sample_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_load_pcm_files_device: bad argument");
+  const std::string api = "bp_load_pcm_files_device";
+  std::vector<IngestFile> desc;
+  std::vector<int64_t> bytes;
+  int rc = describe_pcm(api, files, n_files, true, desc, bytes);
+  if (rc) return rc;
+  int64_t total = 0;
+  for (const IngestFile& f : desc) total += f.n_out;
+  if (total > 0 && !d_audio) return fail(BP_E_INVALID, api + ": null output");
+  h_sample_off[0] = 0;
+  for (int i = 0; i < n_files; ++i) h_sample_off[i + 1] = h_sample_off[i] + desc[i].n_out;
+  if (total == 0) return BP_OK;
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if ((rc = load_ingest_taps(api, m->device, desc))) return rc;
+  for (int i = 0; i < n_files; ++i) {
+    desc[i].pcm = files[i].pcm;
+    desc[i].out = d_audio + h_sample_off[i];
+  }
+  const size_t hb = (size_t)ingest_header_bytes(n_files);
+  if (m->ingest_pending) {  // the previous call's staging has left the host
+    CK(cudaEventSynchronize(m->ingest_copied));
+    m->ingest_pending = false;
+  }
+  if (hb > m->h_ingest_cap) {
+    if (m->h_ingest) cudaFreeHost(m->h_ingest);
+    m->h_ingest = nullptr;
+    m->h_ingest_cap = 0;
+    const size_t cap = std::max<size_t>(hb, 1 << 16);
+    CK(cudaHostAlloc(&m->h_ingest, cap, cudaHostAllocDefault));
+    m->h_ingest_cap = cap;
+  }
+  CK(m->d_ingest.reserve(hb));
+  if (!m->ingest_copied) {
+    CK(cudaEventCreateWithFlags(&m->ingest_copied, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&m->ingest_done, cudaEventDisableTiming));
+  } else {
+    CK(cudaStreamWaitEvent(st, m->ingest_done, 0));  // the previous call's kernel may have run on another stream
+  }
+  int max_span = 1;
+  const int n_ctas = write_ingest_header(m->h_ingest, desc.data(), n_files, &max_span);
+  CK(cudaMemcpyAsync(m->d_ingest.p, m->h_ingest, hb, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(m->ingest_copied, st));
+  m->ingest_pending = true;
+  rc = launch_ingest_header(m, m->d_ingest.p, n_files, n_ctas, max_span, st);
+  CK(cudaEventRecord(m->ingest_done, st));
+  return rc;
+}
+
+int bp_transcribe_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files,
+                                 const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
+                                 int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_transcribe_pcm_files_host: bad argument");
+  int rc = validate_params(params);
+  if (rc) return rc;
+  Batch b{"bp_transcribe_pcm_files_host", nullptr, false, nullptr};
+  b.pcm = files;
+  if ((rc = describe_pcm(b.api, files, n_files, false, b.ingest, b.pcm_bytes))) return rc;
+  b.rel.assign(n_files + 1, 0);
+  for (int i = 0; i < n_files; ++i) {
+    b.rel[i + 1] = b.rel[i] + b.ingest[i].n_out;
+    b.total_frames += bp_num_frames(b.ingest[i].n_out);
+  }
+  if (h_sample_off) std::copy(b.rel.begin(), b.rel.end(), h_sample_off);
+  DeviceGuard g(m->device);
+  if ((rc = load_ingest_taps(b.api, m->device, b.ingest))) return rc;
+  return run_batch(m, b, nullptr, Rows{h_note, h_onset, h_contour}, params, notes, h_frame_off, m->stream);
+}
+
+int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* byte_off, int64_t* sample_off) {
+  if (n_files < 0 || (n_files > 0 && !files) || !byte_off || !sample_off)
+    return fail(BP_E_INVALID, "bp_debug_pcm_layout: bad argument");
+  std::vector<IngestFile> desc;
+  std::vector<int64_t> bytes;
+  const int rc = describe_pcm("bp_debug_pcm_layout", files, n_files, false, desc, bytes);
+  if (rc) return rc;
+  byte_off[0] = sample_off[0] = 0;
+  for (int i = 0; i < n_files; ++i) {
+    byte_off[i + 1] = byte_off[i] + align16(bytes[i]);
+    sample_off[i + 1] = sample_off[i] + desc[i].n_out;
+  }
   return BP_OK;
 }
 

@@ -37,13 +37,21 @@ double bessel_i0(double x) {  // power series, converges quickly for the argumen
   return sum;
 }
 
+constexpr double kStopDb = 125.0;
+
+// taps of the low-pass for the reduced ratio up / down: scipy.signal.kaiserord(125, width), made odd
+int filter_length(int up, int down) {
+  const int m = std::max(up, down);
+  const double pass_edge = 0.913 / m, stop_edge = 1.0 / m, width = stop_edge - pass_edge;
+  return (int)std::ceil((kStopDb - 7.95) / 2.285 / (M_PI * width) + 1.0) | 1;
+}
+
 // scipy.signal.kaiserord(125, width) + firwin(numtaps | 1, cutoff, window=("kaiser", beta)), as audio_io._resample_filter
 std::vector<double> design_filter(int up, int down) {
   const int m = std::max(up, down);
-  const double pass_edge = 0.913 / m, stop_edge = 1.0 / m, width = stop_edge - pass_edge;
-  const double A = 125.0, beta = 0.1102 * (A - 8.7);
-  int numtaps = (int)std::ceil((A - 7.95) / 2.285 / (M_PI * width) + 1.0);
-  numtaps |= 1;
+  const double pass_edge = 0.913 / m, stop_edge = 1.0 / m;
+  const double A = kStopDb, beta = 0.1102 * (A - 8.7);
+  const int numtaps = filter_length(up, down);
   const double cutoff = 0.5 * (pass_edge + stop_edge), alpha = 0.5 * (numtaps - 1);
   std::vector<double> h(numtaps);
   double sum = 0.0;
@@ -132,12 +140,13 @@ __device__ __forceinline__ float mono_sample(const T* pcm, long long i, int chan
   return __double2float_rn(__ddiv_rn((double)__fadd_rn(0.f, s), (double)channels));
 }
 
+// The work of one CTA, shared by both kernels so that a file has the same bits whichever launched it: outputs
+// [cta * 256, cta * 256 + 256) of one file from its inputs staged (converted and down-mixed) in s_x.
 template <typename T>
-__global__ void __launch_bounds__(kOutPerCta) ingest_kernel(const T* __restrict__ pcm, long long n_in, int channels, int up,
-                                                            int down, int half, int taps, const float* __restrict__ hp,
-                                                            float* __restrict__ out, long long n_out, int span) {
-  extern __shared__ float s_x[];
-  const long long k0 = (long long)blockIdx.x * kOutPerCta;
+__device__ __forceinline__ void ingest_cta(const T* __restrict__ pcm, long long n_in, int channels, int up, int down,
+                                           int half, int taps, const float* __restrict__ hp, float* __restrict__ out,
+                                           long long n_out, int span, long long cta, float* s_x) {
+  const long long k0 = cta * kOutPerCta;
   // inputs the CTA's outputs touch: i in [i_lo, i_lo + span)
   const long long i_lo = (k0 * down + half) / up - (taps - 1);
   for (int t = threadIdx.x; t < span; t += kOutPerCta) {
@@ -167,6 +176,42 @@ __global__ void __launch_bounds__(kOutPerCta) ingest_kernel(const T* __restrict_
   out[k] = (a0 + a1) + (a2 + a3);
 }
 
+template <typename T>
+__global__ void __launch_bounds__(kOutPerCta) ingest_kernel(const T* __restrict__ pcm, long long n_in, int channels, int up,
+                                                            int down, int half, int taps, const float* __restrict__ hp,
+                                                            float* __restrict__ out, long long n_out, int span) {
+  extern __shared__ float s_x[];
+  ingest_cta<T>(pcm, n_in, channels, up, down, half, taps, hp, out, n_out, span, blockIdx.x, s_x);
+}
+
+// Many files in one launch: file i owns CTAs [cta_off[i], cta_off[i + 1]) (none when it is empty), each CTA looks its
+// file up and runs that file's format.
+__global__ void __launch_bounds__(kOutPerCta) ingest_batch_kernel(const IngestFile* __restrict__ files,
+                                                                  const int* __restrict__ cta_off, int n_files) {
+  extern __shared__ float s_x[];
+  const int b = blockIdx.x;
+  int lo = 0, hi = n_files;  // cta_off[lo] <= b < cta_off[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (cta_off[mid] <= b)
+      lo = mid;
+    else
+      hi = mid;
+  }
+  const IngestFile f = files[lo];
+  const long long cta = b - cta_off[lo];
+#define BP_INGEST_CTA(T)                                                                                                   \
+  ingest_cta<T>(static_cast<const T*>(f.pcm), f.n_in, f.channels, f.up, f.down, f.half, f.taps, f.hp, f.out, f.n_out,     \
+                f.span, cta, s_x)
+  switch (f.format) {
+    case 0: BP_INGEST_CTA(float); break;
+    case 1: BP_INGEST_CTA(short); break;
+    case 2: BP_INGEST_CTA(int); break;
+    default: BP_INGEST_CTA(unsigned char); break;
+  }
+#undef BP_INGEST_CTA
+}
+
 long long gcd_ll(long long a, long long b) {
   while (b) {
     const long long t = a % b;
@@ -187,49 +232,72 @@ long long ingest_output_length(long long n_frames, int sample_rate) {
   return (n_frames * up + down - 1) / down;
 }
 
+// The resampler of one sample rate without its taps: ratio, filter geometry and the inputs a CTA stages.  Host
+// arithmetic only.  0, or -2 when the format / channel count / rate is unsupported.
+int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f) {
+  if (channels < 1 || sample_rate < 1 || format < 0 || format > 3) return -2;
+  const long long g = gcd_ll(kSampleRate, sample_rate);
+  f.format = format, f.channels = channels;
+  f.up = (int)(kSampleRate / g), f.down = (int)(sample_rate / g);
+  f.half = 0, f.taps = 1;
+  if (f.up != 1 || f.down != 1) {
+    const int L = filter_length(f.up, f.down);
+    f.half = (L - 1) / 2;
+    f.taps = (L + f.up - 1) / f.up;
+  }
+  // staged inputs per CTA: the newest input of the last output minus the oldest of the first, plus one
+  const long long span = ((long long)(kOutPerCta - 1) * f.down + f.up - 1) / f.up + f.taps + 1;
+  if (span * (long long)sizeof(float) > 200 * 1024) return -2;  // rate ratios beyond ~100:1
+  f.span = (int)span;
+  return 0;
+}
+
+// The polyphase taps of f's ratio on `device` (designed and uploaded on first use) into f.hp.  0, -1 CUDA error.
+int ingest_taps(int device, IngestFile& f) {
+  if (device < 0 || device >= 64) return -2;
+  std::lock_guard<std::mutex> lk(g_mu);
+  auto& cache = g_resamplers[device];
+  const long long key = ((long long)f.up << 32) | (unsigned)f.down;
+  auto it = cache.find(key);
+  if (it == cache.end()) {
+    Resampler rs;
+    rs.up = f.up, rs.down = f.down;
+    if (f.up != 1 || f.down != 1) {
+      const int up = f.up;
+      const std::vector<double> h = design_filter(f.up, f.down);
+      const int L = (int)h.size();
+      rs.half = (L - 1) / 2;
+      rs.taps_per_phase = (L + up - 1) / up;
+      std::vector<float> hp((size_t)up * rs.taps_per_phase, 0.f);
+      for (int p = 0; p < up; ++p)
+        for (int j = 0; p + (long long)j * up < L; ++j) hp[(size_t)p * rs.taps_per_phase + j] = (float)(up * h[p + (size_t)j * up]);
+      if (cudaMalloc(&rs.d_hp, hp.size() * sizeof(float)) != cudaSuccess) return -1;
+      if (cudaMemcpy(rs.d_hp, hp.data(), hp.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return -1;
+    } else {
+      rs.taps_per_phase = 1;
+    }
+    it = cache.emplace(key, rs).first;
+  }
+  f.hp = it->second.d_hp;
+  return 0;
+}
+
 // 0 on success; -1 CUDA error, -2 unsupported argument
 int launch_ingest(int device, const void* d_pcm, int format, long long n_frames, int channels, int sample_rate, float* d_out,
                   cudaStream_t st) {
   if (n_frames <= 0) return 0;
-  if (channels < 1 || sample_rate < 1 || format < 0 || format > 3 || device < 0 || device >= 64) return -2;
-  const long long g = gcd_ll(kSampleRate, sample_rate);
-  const int up = (int)(kSampleRate / g), down = (int)(sample_rate / g);
-  Resampler rs;
-  {
-    std::lock_guard<std::mutex> lk(g_mu);
-    auto& cache = g_resamplers[device];
-    const long long key = ((long long)up << 32) | (unsigned)down;
-    auto it = cache.find(key);
-    if (it == cache.end()) {
-      rs.up = up, rs.down = down;
-      if (up != 1 || down != 1) {
-        const std::vector<double> h = design_filter(up, down);
-        const int L = (int)h.size();
-        rs.half = (L - 1) / 2;
-        rs.taps_per_phase = (L + up - 1) / up;
-        std::vector<float> hp((size_t)up * rs.taps_per_phase, 0.f);
-        for (int p = 0; p < up; ++p)
-          for (int j = 0; p + (long long)j * up < L; ++j) hp[(size_t)p * rs.taps_per_phase + j] = (float)(up * h[p + (size_t)j * up]);
-        if (cudaMalloc(&rs.d_hp, hp.size() * sizeof(float)) != cudaSuccess) return -1;
-        if (cudaMemcpy(rs.d_hp, hp.data(), hp.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return -1;
-      } else {
-        rs.taps_per_phase = 1;
-      }
-      it = cache.emplace(key, rs).first;
-    }
-    rs = it->second;
-  }
+  IngestFile f{};
+  int rc = ingest_geometry(format, channels, sample_rate, f);
+  if (rc == 0) rc = ingest_taps(device, f);
+  if (rc) return rc;
   const long long n_out = ingest_output_length(n_frames, sample_rate);
-  // staged inputs per CTA: the newest input of the last output minus the oldest of the first, plus one
-  const int span = (int)(((long long)(kOutPerCta - 1) * down + up - 1) / up + rs.taps_per_phase + 1);
-  const size_t smem = (size_t)span * sizeof(float);
-  if (smem > 200 * 1024) return -2;  // rate ratios beyond ~100:1
+  const size_t smem = (size_t)f.span * sizeof(float);
   const unsigned grid = (unsigned)((n_out + kOutPerCta - 1) / kOutPerCta);
 #define BP_INGEST(T)                                                                                                       \
   do {                                                                                                                     \
     if (smem > 48 * 1024) cudaFuncSetAttribute(ingest_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
-    ingest_kernel<T><<<grid, kOutPerCta, smem, st>>>(static_cast<const T*>(d_pcm), n_frames, channels, rs.up, rs.down,     \
-                                                     rs.half, rs.taps_per_phase, rs.d_hp, d_out, n_out, span);             \
+    ingest_kernel<T><<<grid, kOutPerCta, smem, st>>>(static_cast<const T*>(d_pcm), n_frames, channels, f.up, f.down,       \
+                                                     f.half, f.taps, f.hp, d_out, n_out, f.span);                          \
   } while (0)
   switch (format) {
     case 0: BP_INGEST(float); break;
@@ -238,6 +306,17 @@ int launch_ingest(int device, const void* d_pcm, int format, long long n_frames,
     default: BP_INGEST(unsigned char); break;
   }
 #undef BP_INGEST
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+long long ingest_ctas(long long n_out) { return (n_out + kOutPerCta - 1) / kOutPerCta; }
+
+int launch_ingest_batch(const IngestFile* d_files, const int* d_cta_off, int n_files, int n_ctas, int max_span,
+                        cudaStream_t st) {
+  if (n_ctas <= 0) return 0;
+  const size_t smem = (size_t)max_span * sizeof(float);
+  if (smem > 48 * 1024) cudaFuncSetAttribute(ingest_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  ingest_batch_kernel<<<(unsigned)n_ctas, kOutPerCta, smem, st>>>(d_files, d_cta_off, n_files);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

@@ -187,6 +187,24 @@ long long ingest_output_length(long long n_frames, int sample_rate);
 std::vector<double> ingest_filter(int up, int down);  // host-only: the low-pass design (unit DC gain)
 int launch_ingest(int device, const void* d_pcm, int format, long long n_frames, int channels, int sample_rate, float* d_out,
                   cudaStream_t st);  // 0 ok, -1 CUDA error, -2 unsupported argument
+// One file of a batched ingest, as the kernel reads it: ingest_geometry fills the format, the ratio, the filter geometry
+// and `span` (the inputs a CTA stages), ingest_taps the device's polyphase taps `hp` of that ratio (designed on first
+// use, shared by the device's models); the caller sets pcm / n_in / out / n_out.  Both return 0, -1 (CUDA error) or -2
+// (unsupported), like launch_ingest.
+struct IngestFile {
+  const void* pcm;  // interleaved frames, aligned to their sample type
+  const float* hp;
+  float* out;
+  long long n_in, n_out;
+  int channels, format, up, down, half, taps, span, pad;
+};
+int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f);
+int ingest_taps(int device, IngestFile& f);
+long long ingest_ctas(long long n_out);  // CTAs a file of n_out output samples takes
+// d_files [n_files] and d_cta_off [n_files + 1] (exclusive prefix sum of ingest_ctas) in device memory; max_span: the
+// largest `span` among the files.  One launch; file i gets the bits of launch_ingest on file i alone.
+int launch_ingest_batch(const IngestFile* d_files, const int* d_cta_off, int n_files, int n_ctas, int max_span,
+                        cudaStream_t st);
 
 // ---- decode.cu ----------------------------------------------------------------------------------
 struct DecodeParamsDev {

@@ -6,7 +6,7 @@ module (`Model`, `predict`, `predict_and_save`, `run_inference`, `window_audio_f
 `save_note_events`, `DEFAULT_*`).  What differs is what sits behind `Model`: instead of dispatching
 to TensorFlow / CoreML / TFLite / onnxruntime (reference: inference.py:78-182) there is one runtime —
 the hand-written sm_90a kernels in `csrc/` reached through the C ABI of include/bp_b200.h — and no
-CPU fallback.  Batch entry points (`Model.transcribe_arrays`, `predict_batch`) are additions.
+CPU fallback.  Batch entry points (`Model.transcribe_arrays`, `Model.transcribe_pcm`, `predict_batch`) are additions.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ import numpy as np
 
 from . import ICASSP_2022_MODEL_PATH, _lib, weights
 from . import note_creation as infer
-from .audio_io import load_audio, load_audio_device
+from .audio_io import load_audio, load_audio_device, pcm_descriptors, read_pcm
 from .constants import (
     ANNOTATIONS_FPS,
     AUDIO_N_SAMPLES,
@@ -341,6 +341,38 @@ class Model:
             keep.append(a if (a.dtype == _F32 and a.flags.c_contiguous) else np.ascontiguousarray(a, dtype=_F32))
         ptrs = (C.c_void_p * max(n_files, 1))(*[a.ctypes.data for a in keep])
         lens = np.fromiter((a.shape[0] for a in keep), dtype=np.int64, count=n_files)
+        p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
+                         include_pitch_bends, min_pitch_idx, max_pitch_idx)
+        return self._transcribe(
+            lens, return_model_output, split_notes,
+            lambda note, onset, contour, foff, nt: self._lib.bp_transcribe_files_host(
+                self._h, ptrs, _ptr(lens), n_files, C.byref(p), _ptr(note), _ptr(onset), _ptr(contour), _ptr(foff), C.byref(nt)),
+        )
+
+    def transcribe_pcm(self, items: Sequence[Tuple[np.ndarray, int]], onset_thresh=0.5, frame_thresh=0.3, min_note_len=11,
+                       energy_tol=11, infer_onsets=True, melodia_trick=True, include_pitch_bends=True,
+                       min_pitch_idx=0, max_pitch_idx=88, return_model_output: bool = True, split_notes: bool = True):
+        """`transcribe_arrays` for files given as their stored samples: an item is (samples, sample_rate) as
+        `audio_io.read_pcm` returns them — (n,) or (n, channels), float32 / int16 / int32 / uint8, any rate.  ONE library
+        call (bp_transcribe_pcm_files_host): the samples go up as stored, one batched ingest per sub-batch converts,
+        down-mixes and resamples them on the device, and the forward pass reads the result there.  Same results as
+        `load_audio_device` per file followed by `transcribe_arrays`, same return value."""
+        files, keep = pcm_descriptors(items)
+        n_files = len(keep)
+        lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in files[:n_files]),
+                           dtype=np.int64, count=n_files)
+        p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
+                         include_pitch_bends, min_pitch_idx, max_pitch_idx)
+        return self._transcribe(
+            lens, return_model_output, split_notes,
+            lambda note, onset, contour, foff, nt: self._lib.bp_transcribe_pcm_files_host(
+                self._h, files, n_files, C.byref(p), _ptr(note), _ptr(onset), _ptr(contour), _ptr(foff), None, C.byref(nt)),
+        )
+
+    def _transcribe(self, lens: np.ndarray, return_model_output: bool, split_notes: bool, call):
+        """The part the whole-path calls share: outputs for files of `lens` samples at 22 050 Hz, capacity negotiation
+        around call(note, onset, contour, frame_off, notes), and the per-file views."""
+        n_files = len(lens)
         frames = [int(self._lib.bp_num_frames(int(n))) for n in lens]
         total = sum(frames)
         note = onset = contour = None
@@ -349,13 +381,7 @@ class Model:
             onset = self._pinned.array((total, N_FREQ_BINS_NOTES))
             contour = self._pinned.array((total, N_FREQ_BINS_CONTOURS))
         foff = np.zeros(n_files + 1, np.int64)
-        p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
-                         include_pitch_bends, min_pitch_idx, max_pitch_idx)
-        arrs = self._with_capacity(
-            n_files, total,
-            lambda nt: self._lib.bp_transcribe_files_host(self._h, ptrs, _ptr(lens), n_files, C.byref(p), _ptr(note),
-                                                          _ptr(onset), _ptr(contour), _ptr(foff), C.byref(nt)),
-        )
+        arrs = self._with_capacity(n_files, total, lambda nt: call(note, onset, contour, foff, nt))
         res = self._split_notes(arrs, n_files) if split_notes else arrs
         outs: List[Optional[Dict[str, np.ndarray]]] = [None] * n_files
         if return_model_output:
@@ -632,21 +658,34 @@ def predict_batch(
 ):
     """`predict` for many clips in one device pass (addition; no reference counterpart).
 
-    Items are paths or mono 22 050 Hz float arrays.  Returns a list of
+    Items are paths or mono 22 050 Hz float arrays.  With a path among them the batch goes through
+    `Model.transcribe_pcm`: the files cross to the device once, as the samples they store, and are converted, down-mixed
+    and resampled there.  Returns a list of
     (model_output | None, midi_data | None, note_events) in input order.  The model outputs are views of three
     page-locked arrays shared by the batch.  With lazy=True (default) the note events are `NoteEventList`s and the MIDI
     objects `LazyPrettyMIDI`s: both turn into the reference's Python objects when first read; lazy=False builds
     everything before returning."""
     model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    audios = [a if isinstance(a, np.ndarray) else load_audio_device(a, model)[0] for a in audio]
     min_note_len = int(np.round(minimum_note_length / 1000 * (AUDIO_SAMPLE_RATE / FFT_HOP)))
     lo, hi = infer.frequency_to_column_range(minimum_frequency, maximum_frequency)
-    outs, arrs, frames = model.transcribe_arrays(
-        audios, onset_thresh=onset_threshold, frame_thresh=frame_threshold, min_note_len=min_note_len,
-        melodia_trick=melodia_trick, min_pitch_idx=lo, max_pitch_idx=hi, return_model_output=return_model_output,
-        split_notes=False,
-    )
-    n = len(audios)
+    decode = dict(onset_thresh=onset_threshold, frame_thresh=frame_threshold, min_note_len=min_note_len,
+                  melodia_trick=melodia_trick, min_pitch_idx=lo, max_pitch_idx=hi, return_model_output=return_model_output,
+                  split_notes=False)
+    if all(isinstance(a, np.ndarray) for a in audio):
+        outs, arrs, frames = model.transcribe_arrays(audio, **decode)
+    else:
+        # files go to the device as the samples they store; arrays beside them as float32 mono at 22 050 Hz, which the
+        # ingest copies bit for bit
+        items = []
+        for a in audio:
+            if isinstance(a, np.ndarray):
+                if a.ndim != 1:
+                    raise ValueError("audio must be mono (1-D)")
+                items.append((np.ascontiguousarray(a, dtype=_F32), AUDIO_SAMPLE_RATE))
+            else:
+                items.append(read_pcm(a))
+        outs, arrs, frames = model.transcribe_pcm(items, **decode)
+    n = len(audio)
     events = infer.note_events_batch(arrs, n, include_pitch_bends=True, lazy=lazy)
     if return_model_output and (minimum_frequency is not None or maximum_frequency is not None):
         # the reference zeroes these columns of the returned arrays (note_creation.py:338-341); all files share two arrays

@@ -213,6 +213,45 @@ int bp_load_pcm_device(bp_model_t* m, const void* d_pcm, int32_t sample_format, 
 int bp_load_pcm_host(bp_model_t* m, const void* h_pcm, int32_t sample_format, int64_t n_frames, int32_t channels,
                      int32_t sample_rate, float* h_audio);
 
+/* One file of a batch as stored PCM: interleaved frames, format codes and conversions as bp_load_pcm_*. */
+typedef struct bp_pcm_file {
+  const void* pcm;       /* n_frames x channels samples; may be NULL when n_frames == 0 */
+  int64_t n_frames;
+  int32_t sample_format; /* 0 float32, 1 int16, 2 int32, 3 uint8 */
+  int32_t channels;
+  int32_t sample_rate;
+  int32_t reserved;
+} bp_pcm_file_t;
+
+/* The ingest for a batch of files in one kernel launch — `librosa.load(path, sr=22050, mono=True)` minus the container
+ * decode, which the reference calls once per file (basic_pitch/inference.py:239 inside predict, looped by
+ * predict_and_save :509-604).  Files may differ in format, channel count and sample rate.  File i's signal has exactly
+ * the bits bp_load_pcm_device gives for that file alone, wherever it sits in the batch.
+ * Every file is validated before anything is enqueued: a format outside 0..3, channels or sample_rate below 1, a
+ * negative length, a NULL pcm with frames, or a rate ratio beyond the limit of bp_load_pcm_device return BP_E_INVALID
+ * with the file's index in bp_last_error() and leave the device untouched.  n_files == 0 is a valid empty call.
+ * bp_load_pcm_files_device: files[i].pcm are device pointers aligned to their sample type; the 22 050 Hz signals are
+ *   written back to back into d_audio (sum of bp_resampled_length samples) and their offsets into
+ *   h_sample_off[n_files + 1] (written before the call returns); asynchronous on `stream`.  d_audio and h_sample_off
+ *   feed bp_transcribe_device / bp_run_inference_device directly.
+ * bp_transcribe_pcm_files_host: predict() for a batch of files given as stored PCM in ordinary (pageable) host memory —
+ *   bp_transcribe_files_host with the ingest in front, on the same sub-batch pipeline: per sub-batch the library packs
+ *   the files' PCM (every file starting on a 16-byte boundary) behind their descriptors in pinned staging, uploads that
+ *   while the previous sub-batch computes, and one batched ingest leaves the signals on the device, where the forward
+ *   pass reads them.  Each sample crosses PCIe once, as stored.  The staging (three pinned buffers, two on the device)
+ *   is sized by the largest sub-batch in PCM bytes.  h_sample_off (may be NULL) receives the resampled lengths as
+ *   offsets [n_files + 1]; everything else as bp_transcribe_files_host. */
+int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, float* d_audio,
+                             int64_t* h_sample_off, void* stream);
+int bp_transcribe_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files,
+                                 const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
+                                 int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes);
+/* Host-only (no GPU needed): validates the files as the two calls above do and returns where
+ * bp_transcribe_pcm_files_host would pack them if they formed one sub-batch: file i's PCM at byte_off[i] (a multiple
+ * of 16) from the first file's, byte_off[n_files] the size of the packed PCM; and sample_off[n_files + 1], the offsets
+ * of their 22 050 Hz signals. */
+int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* byte_off, int64_t* sample_off);
+
 /* Batched writers (host threads, no GPU): one Standard MIDI File and / or one note-event CSV per file of a batch, straight
  * from the concatenated note arrays (times already in seconds).  Replaces, for batches, note_events_to_midi (reference:
  * basic_pitch/note_creation.py:222-271, incl. drop_overlapping_pitch_bends :274-286 when multiple_pitch_bends = 0) +
