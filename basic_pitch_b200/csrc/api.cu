@@ -161,6 +161,10 @@ struct bp_model {
   DevBuf<float> i_note, i_onset, i_contour;        // internal raw: pm [88][chunk*172], cm [33][chunk*172][8] (tensor-core paths)
   DevBuf<float> u_note, u_onset, u_contour;        // internal unwrapped posteriorgrams of a call: pm [88][F], cm [33][F][8]
   bool y_is_log = false;  // tensor-core paths: `y` still holds the raw log-magnitudes (bp_debug_activation normalises)
+  // bp_model_set_debug_frontend: the forward copies the raw log-magnitudes aside before they are normalised
+  bool debug_frontend = false;
+  bool ylog_valid = false;  // ylog holds the raw log-magnitudes of the last forward chunk
+  DevBuf<float> ylog;
   DevBuf<unsigned int> minmax;
   DevBuf<float> edge;  // partial sums where two frequency-tile ranges of a fused conv meet (tc_conv.cu)
   DevBuf<WinDesc> wdesc;
@@ -349,6 +353,7 @@ int ensure_forward_ws(bp_model* m, int nb) {
     CK(m->o1.reserve((size_t)nb * 32 * kFrames * kPitches));
   }
   CK(m->minmax.reserve((size_t)nb * 2));
+  if (m->debug_frontend) CK(m->ylog.reserve((size_t)nb * kFrames * kCqtBins));
   if (m->path >= 1) {
     const size_t fr = (size_t)m->chunk * kFrames;
     CK(m->i_note.reserve(kPitches * fr));
@@ -438,15 +443,18 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
     if (m->path >= 1) {
       launch_cqt_tc(audio, desc, chain, m->cqt_wtc.p, m->d_params + ParamLayout::cqt_scale, m->y.p, m->minmax.p, nb,
                     m->n_sms, st);
+      if (m->debug_frontend) CK(cudaMemcpyAsync(m->ylog.p, m->y.p, sizeof(float) * nb * kFrames * kCqtBins, cudaMemcpyDeviceToDevice, st));
       // NormalizedLog + BatchNorm straight into the bf16 hi/lo split the convs read
       launch_lognorm_split(m->y.p, m->minmax.p, m->d_params + ParamLayout::bn, m->yhl.p, cs, nb, ystride, st);
       m->y_is_log = true;
     } else {
       launch_cqt(audio, desc, chain, m->d_derived + DerivedLayout::cqt_wt, m->d_params + ParamLayout::cqt_scale, m->y.p,
                  m->minmax.p, nb, st);
+      if (m->debug_frontend) CK(cudaMemcpyAsync(m->ylog.p, m->y.p, sizeof(float) * nb * kFrames * kCqtBins, cudaMemcpyDeviceToDevice, st));
       launch_lognorm(m->y.p, m->minmax.p, m->d_params + ParamLayout::bn, nb, st);
       m->y_is_log = false;
     }
+    m->ylog_valid = m->debug_frontend;
   }
   int extra = 0;  // launches beyond the fixed sequence
   if (m->path >= 1) {
@@ -1820,6 +1828,75 @@ int bp_debug_activation(bp_model_t* m, int which, float* h_out, int64_t n_window
         for (int f = 0; f < kContourBins; ++f)
           for (int c = 0; c < 8; ++c)
             h_out[((b * 8 + c) * kFrames + t) * kContourBins + f] = tmp[((b * kFrames + t) * kContourBins + f) * 8 + c];
+  }
+  return BP_OK;
+}
+
+int bp_model_set_debug_frontend(bp_model_t* m, int on) {
+  if (!m) return fail(BP_E_INVALID, "bp_model_set_debug_frontend: null model");
+  m->debug_frontend = on != 0;
+  return BP_OK;
+}
+
+int bp_debug_chain_layout(int32_t* offsets, int32_t* lengths, int32_t* stride) {
+  if (!offsets || !lengths || !stride) return fail(BP_E_INVALID, "bp_debug_chain_layout: null argument");
+  for (int o = 0; o <= 8; ++o) {
+    offsets[o] = o ? chain_off(o) : -1;
+    lengths[o] = octave_len(o);
+  }
+  *stride = kChainStride;
+  return BP_OK;
+}
+
+int bp_debug_split_layout(const bp_model_t* m, int32_t* out) {
+  if (!m || !out) return fail(BP_E_INVALID, "bp_debug_split_layout: null argument");
+  constexpr TcConvSpec cs = tc_spec(0);
+  out[0] = tc_rows_total(m->chunk, cs.rows_per_window);
+  out[1] = m->last_forward_n > 0 ? tc_rows_total((int)m->last_forward_n, cs.rows_per_window) : 0;
+  out[2] = cs.lead_rows;
+  out[3] = cs.rows_per_window;
+  out[4] = cs.chunks8;
+  return BP_OK;
+}
+
+int bp_debug_frontend(bp_model_t* m, int which, void* h_out, int64_t n_windows) {
+  if (!m || !h_out) return fail(BP_E_INVALID, "bp_debug_frontend: null argument");
+  if (n_windows <= 0 || n_windows > m->chunk || n_windows > m->last_forward_n)
+    return fail(BP_E_INVALID, "bp_debug_frontend: only valid for the windows of a single-chunk forward call");
+  if (which < 0 || which > 3) return fail(BP_E_INVALID, "bp_debug_frontend: unknown buffer id");
+  DeviceGuard g(m->device);
+  CK(cudaDeviceSynchronize());
+  switch (which) {
+    case 0:
+      CK(cudaMemcpy(h_out, m->chain.p, sizeof(float) * kChainStride * n_windows, cudaMemcpyDeviceToHost));
+      break;
+    case 1: {
+      const float* src = m->last_path >= 1 && m->y_is_log ? m->y.p : m->ylog_valid ? m->ylog.p : nullptr;
+      if (!src)
+        return fail(BP_E_INVALID, "bp_debug_frontend: the raw log-magnitudes of the last forward call are gone (path 0 "
+                                  "normalises them in place, and bp_debug_activation(0) does so on the tensor-core paths): "
+                                  "call bp_model_set_debug_frontend(m, 1) before the forward call");
+      CK(cudaMemcpy(h_out, src, sizeof(float) * kFrames * kCqtBins * n_windows, cudaMemcpyDeviceToHost));
+      break;
+    }
+    case 2: {
+      std::vector<unsigned int> mm((size_t)2 * n_windows);
+      CK(cudaMemcpy(mm.data(), m->minmax.p, sizeof(unsigned int) * mm.size(), cudaMemcpyDeviceToHost));
+      float* out = static_cast<float*>(h_out);
+      for (size_t i = 0; i < mm.size(); ++i) {  // ordered_to_float on the host
+        const uint32_t u = (mm[i] & 0x80000000u) ? (mm[i] & 0x7fffffffu) : ~mm[i];
+        std::memcpy(out + i, &u, 4);
+      }
+      break;
+    }
+    case 3: {
+      if (m->last_path < 1)
+        return fail(BP_E_INVALID, "bp_debug_frontend: the split operand exists only on the tensor-core paths (1 and 2)");
+      constexpr TcConvSpec cs = tc_spec(0);
+      const size_t n = (size_t)2 * cs.chunks8 * 8 * tc_rows_total(m->chunk, cs.rows_per_window);
+      CK(cudaMemcpy(h_out, m->yhl.p, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
+      break;
+    }
   }
   return BP_OK;
 }

@@ -177,6 +177,27 @@ int64_t bp_model_chunk_windows(const bp_model_t* m);
  * single-output convolution reduced in its epilogue (default); 2 = as 1 but the contour convolution stores its
  * 8-channel activations (bp_debug_activation which = 1). */
 int bp_model_set_path(bp_model_t* m, int path);
+/* Front-end buffers of the most recent forward call (same rule as bp_debug_activation: windows 0..n-1 of a call that
+ * fitted in one chunk).  which:
+ *   0 = the decimation chain x_1..x_8, float [n][stride] (bp_debug_chain_layout);
+ *   1 = the raw log-magnitudes 10 log10(P + 1e-10) before normalisation, float [n][172][309]: on the tensor-core paths
+ *       until bp_debug_activation(0) normalises them; otherwise only when bp_model_set_debug_frontend(m, 1) was on
+ *       during the forward call;
+ *   2 = the per-window min / max of the raw log-magnitudes, float [n][2];
+ *   3 = the split operand of the contour / onset convs (paths 1 and 2), bf16 bits [2][chunks8][rows_stride][8] for
+ *       the whole chunk (bp_debug_split_layout).
+ * An id the last call did not produce is an error. */
+int bp_debug_frontend(bp_model_t* m, int which, void* h_out, int64_t n_windows);
+/* on != 0: every later forward call copies the raw log-magnitudes aside before normalising them (one device copy per
+ * chunk, no extra kernel launch); 0 (default): the forward pass is exactly the one without this switch. */
+int bp_model_set_debug_frontend(bp_model_t* m, int on);
+/* Host-only: where x_o (o = 1..8) starts in one window's chain buffer (offsets[0] = -1: x_0 is the window itself), the
+ * length of x_o (o = 0..8), and the floats per window. */
+int bp_debug_chain_layout(int32_t* offsets, int32_t* lengths, int32_t* stride);
+/* The split-operand layout of bp_debug_frontend(3): out[0] rows_stride (rows per plane and chunk of the buffer), out[1]
+ * rows the last forward call wrote, out[2] lead rows, out[3] rows per window (172 frames + zero rows), out[4] chunks8
+ * (8-bin chunks per row).  Row lead + b * rows_per_window + t holds frame t of window b. */
+int bp_debug_split_layout(const bp_model_t* m, int32_t* out);
 
 /* `bp_transcribe_host` for audio that is NOT packed: file i is audio[i][0 .. n_samples[i]) in ordinary (pageable) host
  * memory — what a caller holding one array per file has (reference: basic_pitch/inference.py:509-604, `predict_and_save`

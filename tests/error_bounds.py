@@ -20,9 +20,24 @@ Model of the arithmetic (u = 2^-24, the float32 unit roundoff):
   * a sigmoid: the bound of its logit times the largest slope on [l - B, l + B], plus the error of a fast exp
     ((2 + 1.16 |l|) ulp relative, which moves the logit by the same amount) and the final rounding
 Posteriorgrams are compared in logit space (`logit_check`): a sigmoid output hides logit errors by p (1 - p).
+
+End to end, the front end's bound of `_y` is loose (median 0.67 where y spans 2.5 under the trained weights), so the
+front end is also checked stage by stage, each stage from the float32 input the kernel actually read, taken as exact
+(tests/test_frontend_bounds.py on the CPU, tests/test_gpu_frontend.py on the kernels' own buffers):
+  * decimation stage s: x_{s+1}[n] = sum_k h[k] x_s[2n + k - 127], zero-padded; bound gamma_256 sum |h||x_s|
+    (`decimate_stage`)
+  * octave o of the constant-Q projection from x_o (octave 0: the window with its zero fill): reflect padding of 128,
+    hop 256 >> o, the octave's bins (g = (8 - o) 36 + bin - 15 >= 0), magnitude * cqt_scale, 10 log10(P + 1e-10) on
+    the interval of P (`cqt_octave`).  Path 0 (FMAs): gamma_256 sum |k||x_o|.  Paths 1 / 2: (EPS_CQT3 + 2 K u (1 + 2^-5))
+    sum |k||x_o|, EPS_CQT3 = 4.02 u the three-way split's dropped terms (derived next to the constant)
+  * min / max: exact; normalisation and its bf16 hi / lo split: bit-exact float32 restatements (`lognorm_f32`,
+    `split_operand`)
+The 2 K u accumulation term of the tensor-core projection is as large as the whole error of a two-way split on real
+signals, so the per-element bound cannot tell a two-way from the three-way split; `split_distance` can.
 """
 from __future__ import annotations
 
+import functools
 from typing import Dict
 
 import numpy as np
@@ -68,6 +83,21 @@ def _conv(x, b_x, w, bias, eps, stride=(1, 1), pad=(0, 0, 0, 0)):
     return z, bz
 
 
+def _log_power(re, im, ere, eim):
+    """re, im (scaled by cqt_scale) with bounds ere, eim -> magnitude and its bound, 10 log10(P + 1e-10) and the ends of
+    its interval.  The log is evaluated on the interval of the power, so bins whose power is lost in the error of the
+    projection are bounded by the floor instead of by a first-order term; then the hardware log and the rounding."""
+    mag = np.sqrt(re * re + im * im)
+    bmag = np.sqrt(ere * ere + eim * eim) + 4 * U * mag
+    power = mag * mag
+    bp = 2 * mag * bmag + bmag * bmag + 2 * U * (power + 1e-10)
+    lpw = DB * np.log(power + 1e-10)
+    l_err = DB * np.log(2.0) * (2.0 ** -21 + 2.0 ** -22 * np.abs(np.log2(power + 1e-10))) + 3 * U * np.abs(lpw)
+    l_lo = DB * np.log(np.maximum(power - bp, 0.0) + 1e-10) - l_err
+    l_hi = DB * np.log(power + bp + 1e-10) + l_err
+    return mag, bmag, lpw, l_lo, l_hi
+
+
 def _cqt_bounds(audio: np.ndarray, w: Dict[str, np.ndarray], eps_cqt: float):
     """(B, 43844) -> y after BatchNorm (B, 172, 309) and its bound, plus per-stage diagnostics"""
     x = _t(audio)[:, None, :]
@@ -96,17 +126,8 @@ def _cqt_bounds(audio: np.ndarray, w: Dict[str, np.ndarray], eps_cqt: float):
     im = torch.cat(im_l, 1)[:, -model_ref.N_BINS :] * sc
     ere = torch.cat(ere_l, 1)[:, -model_ref.N_BINS :] * sc
     eim = torch.cat(eim_l, 1)[:, -model_ref.N_BINS :] * sc
-    mag = torch.sqrt(re * re + im * im)
-    bmag = torch.sqrt(ere * ere + eim * eim) + 4 * U * mag
-    mag, bmag = mag.transpose(1, 2).numpy(), bmag.transpose(1, 2).numpy()  # (B, 172, 309)
-    # 10 log10(P + 1e-10) over the interval of the power, so bins whose power is lost in the error of the projection
-    # are bounded by the floor instead of by a first-order term; then the hardware log and the rounding
-    power = mag * mag
-    bp = 2 * mag * bmag + bmag * bmag + 2 * U * (power + 1e-10)
-    lpw = DB * np.log(power + 1e-10)
-    l_err = DB * np.log(2.0) * (2.0 ** -21 + 2.0 ** -22 * np.abs(np.log2(power + 1e-10))) + 3 * U * np.abs(lpw)
-    l_lo = DB * np.log(np.maximum(power - bp, 0.0) + 1e-10) - l_err
-    l_hi = DB * np.log(power + bp + 1e-10) + l_err
+    t = lambda v: v.transpose(1, 2).numpy()  # noqa: E731  (B, 172, 309)
+    mag, bmag, lpw, l_lo, l_hi = _log_power(t(re), t(im), t(ere), t(eim))
     bl = np.maximum(lpw - l_lo, l_hi - lpw)
     # normalisation y = (L - min L) / max(L - min L) per window, evaluated on the interval ends: the min and the max
     # of the window move with the error of the cells that hold them, the numerator with the cell's own
@@ -186,10 +207,13 @@ def forward_bounds(audio: np.ndarray, w: Dict[str, np.ndarray], eps_cqt: float =
 
 
 def ratio(got: np.ndarray, ref: np.ndarray, bound: np.ndarray) -> float:
-    """max |got - ref| / bound over all elements (<= 1: within the bound)"""
+    """max |got - ref| / bound over all elements (<= 1: within the bound; an exact element whose bound is 0, e.g. a
+    decimation stage over silence, counts 0; a NaN anywhere makes the result NaN, which fails `<= 1`)"""
     got = np.asarray(got, np.float64)
     assert got.shape == ref.shape == bound.shape, (got.shape, ref.shape, bound.shape)
-    return float((np.abs(got - ref) / bound).max())
+    err = np.abs(got - ref)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return float(np.where((err == 0) & (bound == 0), 0.0, err / bound).max())
 
 
 def logit_check(p_got: np.ndarray, l_ref: np.ndarray, b_ref: np.ndarray) -> float:
@@ -207,3 +231,152 @@ def logit_check(p_got: np.ndarray, l_ref: np.ndarray, b_ref: np.ndarray) -> floa
     bound = b_ref + _exp_err(l_ref) + 4 * U * (1.0 + 1.0 / (1.0 - pc)) + 4 * U
     r = np.where(ok, np.abs(l_got - l_ref) / bound, 0.0)
     return float(r.max())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Front end stage by stage: each stage from the float32 input the implementation actually read, taken as exact
+# ---------------------------------------------------------------------------------------------------------------------
+# Three-way bf16 split of both operands of the tensor-core CQT (cqt_tc.cu): x = hi + mid + lo + r with hi = rn(x),
+# mid = rn(x - hi), lo = rn(x - hi - mid), rn to bf16 (8-bit significand, unit roundoff 2^-8; both differences are exact
+# in float32).  |x - hi| <= 2^-8 |x|, |mid| <= (1 + 2^-8) 2^-8 |x|, |x - hi - mid| <= 2^-16 |x|,
+# |lo| <= (1 + 2^-8) 2^-16 |x|, |r| <= 2^-24 |x|.  Of the sixteen products of a * w the kernel keeps hi*hi, hi*mid,
+# mid*hi, hi*lo, lo*hi, mid*mid (each exact in float32); what it drops is
+#   r_a w + (a - r_a) r_w                 <= (2 + 2^-24) 2^-24 |a||w|
+#   mid*lo + lo*mid                       <= 2 (1 + 2^-8)^2 2^-24 |a||w|
+#   lo*lo                                 <= (1 + 2^-8)^2 2^-32 |a||w|
+# in all < 4.02 * 2^-24 |a||w|.
+# Accumulation: the six kept products of all 256 taps sum in magnitude to T <= (1 + 2^-7)^2 (1 + 2^-7 + 3 * 2^-16)
+# sum |a||w| < (1 + 2^-5) sum |a||w|.  They reach one accumulator through 96 wgmma updates (4 K-chunks x 4 k-steps x 6
+# products), update i adding 16 exact products P_i to the accumulator d_{i-1}.  One update is modelled as erring by at
+# most c 2u (|d_{i-1}| + sum |P_i|): the truncation of its result to float32 (< 2u relative) plus the truncating
+# alignment of its 17 addends to the largest exponent, c <= 1 + 17 * 2^-g with g guard bits.  To first order the
+# errors add up to c 2u sum_i (|d_{i-1}| + sum |P_i|) <= c 2u (95 T + T) = c 2u 96 T, since every partial sum |d| <= T.
+# The 2 K u T with K = 256 used here therefore covers c <= 256 / 96 = 2.67, i.e. g >= 4 guard bits in the alignment
+# (1 + 17/16 = 2.06).  The alignment width is not documented; it is the one assumption about the hardware in this bound,
+# and the GPU test holds cqt_tc_kernel's output to it (largest err/bound 0.38 on an H100 SXM).
+EPS_CQT3 = 4.02 * U
+ACC_TC = 2 * 256 * U * (1 + 2.0 ** -5)  # truncating MMA accumulation of the 6 * 256 products, per sum |a||w|
+ACC_FMA = 256 * U / (1 - 256 * U)  # gamma_256: 256 FMAs, round to nearest, any order
+
+
+@functools.lru_cache(maxsize=None)
+def chain_layout():
+    """(offsets, lengths, stride) of the decimation chain buffer, from the library (bp_debug_chain_layout):
+    x_o (o >= 1) of window b is chain[b, offsets[o] : offsets[o] + lengths[o]]; lengths[0] is the window."""
+    import ctypes
+
+    from basic_pitch_b200 import _lib
+
+    off, ln, st = np.zeros(9, np.int32), np.zeros(9, np.int32), ctypes.c_int32()
+    _lib.load().bp_debug_chain_layout(off.ctypes.data, ln.ctypes.data, ctypes.byref(st))
+    return tuple(int(v) for v in off), tuple(int(v) for v in ln), int(st.value)
+
+
+def decimate_stage(x: np.ndarray, h: np.ndarray):
+    """x_{s+1}[n] = sum_k h[k] x_s[2n + k - 127], zero-padded, for a (B, len_s) input taken as exact -> value (float64)
+    and bound gamma_256 sum_k |h[k]| |x_s[2n + k - 127]|"""
+    xt = _t(x)[:, None]
+    lp = _t(h)[None, None]
+    n_out = (x.shape[1] - 2) // 2 + 1
+    v = F.conv1d(F.pad(xt, (127, 127)), lp, stride=2)[:, 0, :n_out]
+    m = F.conv1d(F.pad(xt.abs(), (127, 127)), lp.abs(), stride=2)[:, 0, :n_out]
+    return v.numpy(), ACC_FMA * m.numpy()
+
+
+def reflect_index(length: int, shift_lo: int = 0, shift_hi: int = 0) -> np.ndarray:
+    """signal index of padded position p - 128 (p < length + 256) under reflect padding of 128; shift_lo / shift_hi move
+    the reflection at either end (0 = torch / the kernels)"""
+    i = np.arange(-128, length + 128)
+    i = np.where(i < 0, -i - shift_lo, i)
+    return np.where(i >= length, 2 * (length - 1) - i + shift_hi, i)
+
+
+def octave_frames(x: np.ndarray, o: int, index=None) -> np.ndarray:
+    """(B, len_o) -> the (B, 172, 256) operand of octave o: frame t reads the reflect-padded signal at t * hop + k"""
+    hop = 256 >> o
+    idx = reflect_index(x.shape[1]) if index is None else index
+    pos = np.arange(model_ref.N_FRAMES)[:, None] * hop + np.arange(256)[None, :]
+    return np.asarray(x, np.float64)[:, idx[pos]]
+
+
+def octave_bins(o: int):
+    """(first kernel bin, first global bin) of octave o: global bin g = (8 - o) * 36 + bin - 15 for g >= 0"""
+    g0 = (8 - o) * 36 - 15
+    return max(0, -g0), max(0, g0)
+
+
+def cqt_kernel_matrix(w) -> np.ndarray:
+    """(256, 72) float64: columns interleave the real and imaginary kernels of the 36 bins (the sign of the imaginary
+    part does not reach the magnitude)"""
+    k = np.empty((256, 72))
+    k[:, 0::2] = np.asarray(w["cqt_real"], np.float64).T
+    k[:, 1::2] = np.asarray(w["cqt_imag"], np.float64).T
+    return k
+
+
+def cqt_octave(x: np.ndarray, w: Dict[str, np.ndarray], o: int, path: int, proj=None):
+    """Log-magnitudes of octave o from the (B, len_o) float32 signal x_o the kernel read (octave 0: the window with its
+    zero fill), taken as exact: (value, bound), each (B, 172, bins of the octave), and the octave's global bins.
+    path 0: 256 FMAs per column (cqt_kernel); paths 1, 2: the three-way split and the truncating MMA (cqt_tc_kernel).
+    `proj` (B, 172, 72) replaces the float64 projection as the value (a fault or an emulation to score)."""
+    a = octave_frames(x, o)
+    k = cqt_kernel_matrix(w)
+    c = a @ k if proj is None else np.asarray(proj, np.float64)
+    mabs = np.abs(a) @ np.abs(k)
+    e = (ACC_FMA if path == 0 else EPS_CQT3 + ACC_TC) * mabs
+    b0, g0 = octave_bins(o)
+    s = np.asarray(w["cqt_scale"], np.float64)[g0 : g0 + 36 - b0]
+    re, im, ere, eim = c[..., 0::2][..., b0:], c[..., 1::2][..., b0:], e[..., 0::2][..., b0:], e[..., 1::2][..., b0:]
+    _, _, lpw, l_lo, l_hi = _log_power(re * s, im * s, ere * s, eim * s)
+    return lpw, np.maximum(lpw - l_lo, l_hi - lpw), np.arange(g0, g0 + 36 - b0)
+
+
+def bf16_rn(v: np.ndarray) -> np.ndarray:
+    """float32 -> bf16 bits (uint16), round to nearest even (__float2bfloat16_rn for finite values)"""
+    u = np.ascontiguousarray(v, np.float32).view(np.uint32).astype(np.uint64)
+    return ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+
+
+def bf16_value(h: np.ndarray) -> np.ndarray:
+    return (h.astype(np.uint32) << 16).view(np.float32)
+
+
+def split3(v: np.ndarray):
+    """the three bf16 planes of cqt_tc.cu as float32 values: hi, mid, lo"""
+    v = np.asarray(v, np.float32)
+    hi = bf16_value(bf16_rn(v))
+    r1 = v - hi
+    mid = bf16_value(bf16_rn(r1))
+    return hi, mid, bf16_value(bf16_rn(r1 - mid))
+
+
+def lognorm_f32(log: np.ndarray, minmax: np.ndarray, w: Dict[str, np.ndarray]) -> np.ndarray:
+    """lognorm_kernel / lognorm_split_kernel in float32, operation by operation: (L - mn) / (mx - mn) * bn_scale +
+    bn_bias per window, 0 * bn_scale + bn_bias when mx == mn.  log (B, 172, 309), minmax (B, 2) -> exact bits"""
+    f = np.float32
+    log = np.asarray(log, f)
+    mn = np.asarray(minmax[:, 0], f)[:, None, None]
+    mx = (np.asarray(minmax[:, 1], f)[:, None, None] - mn).astype(f)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        q = np.where(mx == 0, f(0), ((log - mn).astype(f) / mx).astype(f)).astype(f)
+    return ((q * f(w["bn_scale"][0])).astype(f) + f(w["bn_bias"][0])).astype(f)
+
+
+def split_operand(y: np.ndarray, rows_total: int, lead: int, rows_per_window: int, chunks8: int) -> np.ndarray:
+    """lognorm_split_kernel's output for normalised windows y (B, 172, 309): bf16 bits [2][chunks8][rows_total][8],
+    hi = rn(v), lo = rn(v - hi); row lead + b * rows_per_window + t holds frame t of window b, everything else is 0"""
+    n = y.shape[0]
+    v = np.zeros((rows_total, chunks8 * 8), np.float32)
+    rows = lead + np.arange(n)[:, None] * rows_per_window + np.arange(model_ref.N_FRAMES)[None, :]
+    v[rows.reshape(-1), : y.shape[2]] = y.reshape(-1, y.shape[2])
+    hi = bf16_rn(v)
+    lo = bf16_rn(v - bf16_value(hi))
+    out = np.stack([hi, lo]).reshape(2, rows_total, chunks8, 8)
+    return np.ascontiguousarray(out.transpose(0, 2, 1, 3))
+
+
+def split_distance(got: np.ndarray, ref3: np.ndarray, ref2: np.ndarray) -> float:
+    """sum |got - ref2| / sum |got - ref3| over an octave's log-magnitudes: how much closer `got` lies to the three-way
+    split (ref3, float64) than to a two-way split (ref2).  The worst-case bound cannot tell the two apart (EPS_CQT3)."""
+    g = np.asarray(got, np.float64)
+    return float(np.abs(g - ref2).sum() / max(np.abs(g - ref3).sum(), 1e-300))
