@@ -120,9 +120,10 @@ __global__ void compact_notes_kernel(const long long* __restrict__ frame_off, co
                                      int* __restrict__ start, int* __restrict__ end, int* __restrict__ pitch,
                                      long long* __restrict__ note_base) {
   const int file = blockIdx.x;
-  const int n = note_off[file + 1] - note_off[file];
-  const long long s0 = slot_off[file];
-  const int d0 = note_off[file];
+  const long long q = (long long)blockIdx.y * gridDim.x + file;  // grid decode: (setting blockIdx.y, file)
+  const int n = note_off[q + 1] - note_off[q];
+  const long long s0 = slot_off[q];
+  const int d0 = note_off[q];
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     start[d0 + i] = s_start[s0 + i];
     end[d0 + i] = s_end[s0 + i];
@@ -199,6 +200,7 @@ struct bp_model {
   DevBuf<unsigned long long> max_fd;
   DevBuf<int> note_count, slot_start, slot_end, slot_pitch, overflow, d_note_off, d_start, d_end, d_pitch, d_bend_off,
       d_bends;
+  DevBuf<unsigned char> grid_tab;  // group and setting tables of a grid-decode chunk (DecodeGridDev)
   int64_t last_forward_n = 0;
   int last_path = 0;
   // optional per-kernel timing (bench.py roofline): CUDA events around one kernel family
@@ -545,14 +547,60 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
   return BP_OK;
 }
 
-int validate_params(const bp_decode_params_t* p) {
-  if (!p) return fail(BP_E_INVALID, "decode params: null");
+// `who` names the parameter set in the message ("decode params[7]" for a setting of a grid decode)
+int validate_params(const bp_decode_params_t* p, const std::string& who = "decode params") {
+  if (!p) return fail(BP_E_INVALID, who + ": null");
   if (!(p->frame_thresh == p->frame_thresh) || !(p->onset_thresh == p->onset_thresh))
-    return fail(BP_E_INVALID, "decode params: NaN threshold");
+    return fail(BP_E_INVALID, who + ": NaN threshold");
   if (p->melodia_trick && p->frame_thresh < 0)
-    return fail(BP_E_INVALID, "decode params: frame_thresh < 0 with melodia_trick never terminates (the reference loops forever)");
-  if (p->energy_tol < 1) return fail(BP_E_INVALID, "decode params: energy_tol must be >= 1");
-  if (p->min_note_len < 0) return fail(BP_E_INVALID, "decode params: min_note_len must be >= 0");
+    return fail(BP_E_INVALID, who + ": frame_thresh < 0 with melodia_trick never terminates (the reference loops forever)");
+  if (p->energy_tol < 1) return fail(BP_E_INVALID, who + ": energy_tol must be >= 1");
+  if (p->min_note_len < 0) return fail(BP_E_INVALID, who + ": min_note_len must be >= 0");
+  return BP_OK;
+}
+
+DecodeParamsDev params_dev(const bp_decode_params_t& p) {
+  DecodeParamsDev dp;
+  dp.onset_thresh = p.onset_thresh;
+  dp.frame_thresh = p.frame_thresh;
+  dp.min_note_len = p.min_note_len;
+  dp.energy_tol = p.energy_tol;
+  dp.infer_onsets = p.infer_onsets;
+  dp.melodia = p.melodia_trick;
+  dp.lo_col = std::max(0, std::min<int>(p.min_pitch_idx, kPitches));
+  dp.hi_col = std::max(0, std::min<int>(p.max_pitch_idx, kPitches));
+  return dp;
+}
+
+// Grid decode: settings per chunk are bounded by this much device workspace (grid_setting_bytes per setting).  A chunk
+// always holds every file of the batch, so one setting of a very large batch may exceed it on its own.
+constexpr long long kDecodeGridChunkBytes = 2LL << 30;
+constexpr long long kDecodeGridMaxChunk = 65535;  // gridDim.y of the sequential kernel
+
+// Device workspace of one setting in a grid-decode chunk (include/bp_b200.h, bp_decode_grid_chunk_params): its E, a
+// candidate bitmap and a prep group's maxima (every setting may be its own group), its block maxima, its first-attempt
+// note slots (start, end, pitch) and note counts.
+long long grid_setting_bytes(long long total_frames, int n_files) {
+  const long long cells = total_frames * kPitches;
+  return 4 * cells + 4 * decode_cand_words(total_frames) + 8LL * kPitches * decode_block_slots(total_frames, n_files) +
+         12 * std::min(cells, 8 * total_frames + 64LL * n_files) + 16LL * n_files + 64;
+}
+
+// Everything bp_decode_grid_* checks before anything is enqueued: arguments, every setting (by index), frame offsets.
+int check_grid_args(const std::string& api, const bp_model* m, const int64_t* h_frame_off, int n_files,
+                    const bp_decode_params_t* params, int n_params, bool* any_bends) {
+  if (!m || !h_frame_off || n_files < 0 || n_params < 0 || (n_params > 0 && !params))
+    return fail(BP_E_INVALID, api + ": bad argument");
+  *any_bends = false;
+  for (int k = 0; k < n_params; ++k) {
+    const int rc = validate_params(params + k, "decode params[" + std::to_string(k) + "]");
+    if (rc) return rc;
+    *any_bends |= params[k].include_pitch_bends != 0;
+  }
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  if (h_frame_off[0] != 0) return fail(BP_E_INVALID, api + ": frame_off[0] must be 0");
+  for (int i = 1; i <= n_files; ++i)
+    if (h_frame_off[i] < h_frame_off[i - 1]) return fail(BP_E_INVALID, api + ": frame offsets must be non-decreasing");
   return BP_OK;
 }
 
@@ -1268,15 +1316,7 @@ int bp_decode_device(bp_model_t* m, const float* d_note, const float* d_onset, c
   if (total_frames > 0 && (!d_note || !d_onset || (params->include_pitch_bends && !d_contour)))
     return fail(BP_E_INVALID, "bp_decode_device: null posteriorgram");
 
-  DecodeParamsDev dp;
-  dp.onset_thresh = params->onset_thresh;
-  dp.frame_thresh = params->frame_thresh;
-  dp.min_note_len = params->min_note_len;
-  dp.energy_tol = params->energy_tol;
-  dp.infer_onsets = params->infer_onsets;
-  dp.melodia = params->melodia_trick;
-  dp.lo_col = std::max(0, std::min<int>(params->min_pitch_idx, kPitches));
-  dp.hi_col = std::max(0, std::min<int>(params->max_pitch_idx, kPitches));
+  const DecodeParamsDev dp = params_dev(*params);
 
   std::vector<long long> foff(n_files + 1), soff(n_files + 1);
   for (int i = 0; i <= n_files; ++i) {
@@ -1501,6 +1541,231 @@ int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, con
     CK(cudaMemcpyAsync(m->st_contour.p, h_contour, sizeof(float) * total * kContourBins, cudaMemcpyHostToDevice, st));
   }
   return bp_decode_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, notes, st);
+}
+
+int64_t bp_decode_grid_chunk_params(int64_t total_frames, int32_t n_files) {
+  const long long per = grid_setting_bytes(std::max<int64_t>(total_frames, 0), std::max<int32_t>(n_files, 0));
+  return std::max(1LL, std::min(kDecodeGridMaxChunk, kDecodeGridChunkBytes / per));
+}
+
+int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                          const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                          bp_notes_t* notes, void* stream) {
+  const std::string api = "bp_decode_grid_device";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (rc) return rc;
+  if (!notes || !notes->note_off || !notes->bend_off) return fail(BP_E_INVALID, api + ": notes arrays missing");
+  g_need_notes = g_need_bends = 0;
+  notes->note_off[0] = 0;
+  notes->bend_off[0] = 0;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long total_frames = foff[n_files];
+  if (total_frames > 0 && (!d_note || !d_onset || (any_bends && !d_contour)))
+    return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long cells = total_frames * kPitches;
+  const long long chunk = bp_decode_grid_chunk_params(total_frames, n_files);
+  DecodeGridDev gd{};
+  gd.n_files = n_files;
+  gd.e_stride = cells;
+  gd.cand_stride = decode_cand_words(total_frames);
+  gd.blk_stride = (long long)kPitches * decode_block_slots(total_frames, n_files);
+  CK(m->d_frame_off.reserve(n_files + 1));
+  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
+
+  long long n_notes = 0, n_bends = 0;  // over the grid so far
+  bool notes_fit = true, bends_fit = true;
+  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
+    const int P = (int)std::min<long long>(chunk, n_params - p0);
+    const long long n_pairs = (long long)P * n_files;  // (setting, file), setting-major
+    // ---- groups: settings sharing a pitch range share the prep; those also sharing infer_onsets and onset_thresh
+    // share the candidates
+    std::vector<DecodeSettingDev> sd(P);
+    std::vector<DecodePrepGroup> prep;
+    std::vector<DecodeCandGroup> cand;
+    std::vector<int> prep_of(P);
+    for (int s = 0; s < P; ++s) {
+      sd[s].p = params_dev(params[p0 + s]);
+      const DecodeParamsDev& q = sd[s].p;
+      int pg = 0;
+      while (pg < (int)prep.size() && (prep[pg].lo != q.lo_col || prep[pg].hi != q.hi_col)) ++pg;
+      if (pg == (int)prep.size()) prep.push_back(DecodePrepGroup{q.lo_col, q.hi_col, 0, 0});
+      ++prep[pg].set_hi;  // count for now
+      prep_of[s] = pg;
+      int cg = 0;
+      while (cg < (int)cand.size() && (cand[cg].prep != pg || cand[cg].infer != q.infer_onsets ||
+                                       !(cand[cg].onset_thresh == q.onset_thresh)))
+        ++cg;
+      if (cg == (int)cand.size()) cand.push_back(DecodeCandGroup{q.onset_thresh, q.lo_col, q.hi_col, q.infer_onsets, pg});
+      sd[s].cand = cg;
+    }
+    const int n_prep = (int)prep.size(), n_cand = (int)cand.size();
+    for (int k = 0, at = 0; k < n_prep; ++k) {
+      const int n = prep[k].set_hi;
+      prep[k].set_lo = prep[k].set_hi = at;
+      at += n;
+    }
+    std::vector<int> sets(P);
+    for (int s = 0; s < P; ++s) sets[prep[prep_of[s]].set_hi++] = s;
+    // one upload of the tables, 16-byte aligned sections
+    auto sec = [](size_t bytes) { return (bytes + 15) / 16 * 16; };
+    const size_t o_cand = sec(sizeof(DecodePrepGroup) * n_prep), o_sets = o_cand + sec(sizeof(DecodeCandGroup) * n_cand),
+                 o_set = o_sets + sec(sizeof(int) * P), tab_bytes = o_set + sizeof(DecodeSettingDev) * P;
+    std::vector<unsigned char> tab(tab_bytes);
+    std::memcpy(tab.data(), prep.data(), sizeof(DecodePrepGroup) * n_prep);
+    std::memcpy(tab.data() + o_cand, cand.data(), sizeof(DecodeCandGroup) * n_cand);
+    std::memcpy(tab.data() + o_sets, sets.data(), sizeof(int) * P);
+    std::memcpy(tab.data() + o_set, sd.data(), sizeof(DecodeSettingDev) * P);
+    CK(m->grid_tab.reserve(tab_bytes));
+    CK(cudaMemcpyAsync(m->grid_tab.p, tab.data(), tab_bytes, cudaMemcpyHostToDevice, st));
+    gd.prep = reinterpret_cast<const DecodePrepGroup*>(m->grid_tab.p);
+    gd.cand = reinterpret_cast<const DecodeCandGroup*>(m->grid_tab.p + o_cand);
+    gd.sets = reinterpret_cast<const int*>(m->grid_tab.p + o_sets);
+    gd.setting = reinterpret_cast<const DecodeSettingDev*>(m->grid_tab.p + o_set);
+
+    CK(m->energy.reserve((size_t)(P * cells) + 1));
+    CK(m->candbits.reserve((size_t)(n_cand * gd.cand_stride)));
+    CK(m->max_onset.reserve((size_t)n_prep * n_files));
+    CK(m->max_fd.reserve((size_t)n_prep * n_files));
+    CK(m->blk_max.reserve((size_t)(P * gd.blk_stride)));
+    CK(m->blk_arg.reserve((size_t)(P * gd.blk_stride)));
+    CK(m->note_count.reserve((size_t)n_pairs));
+    CK(m->d_slot_off.reserve((size_t)n_pairs + 1));
+    CK(m->overflow.reserve(1));
+    // ---- the loops, with today's two-attempt slot sizing per (setting, file): a pair that ran out of its first
+    // allowance gets 88 T slots, and the chunk runs again (the loops consume E)
+    std::vector<long long> soff(n_pairs + 1);
+    std::vector<char> full(n_pairs, 0);
+    std::vector<int> counts(n_pairs);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      soff[0] = 0;
+      for (long long q = 0; q < n_pairs; ++q) {
+        const long long T = foff[q % n_files + 1] - foff[q % n_files];
+        soff[q + 1] = soff[q] + (full[q] ? T * kPitches : std::min<long long>(T * kPitches, 8 * T + 64));
+      }
+      CK(m->slot_start.reserve((size_t)soff[n_pairs] + 1));
+      CK(m->slot_end.reserve((size_t)soff[n_pairs] + 1));
+      CK(m->slot_pitch.reserve((size_t)soff[n_pairs] + 1));
+      CK(cudaMemcpyAsync(m->d_slot_off.p, soff.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
+      DecodeBuffers b;
+      b.frame_off = m->d_frame_off.p;
+      b.energy = m->energy.p;
+      b.candbits = m->candbits.p;
+      b.max_onset = m->max_onset.p;
+      b.max_fd = m->max_fd.p;
+      b.slot_off = m->d_slot_off.p;
+      b.note_count = m->note_count.p;
+      b.note_start = m->slot_start.p;
+      b.note_end = m->slot_end.p;
+      b.note_pitch = m->slot_pitch.p;
+      b.overflow = m->overflow.p;
+      b.blk_max = m->blk_max.p;
+      b.blk_arg = m->blk_arg.p;
+      {
+        ProfScope ps(m, 5, st);
+        launch_decode_grid(d_note, d_onset, b, n_files, total_frames, gd, n_prep, n_cand, P, st);
+      }
+      CKL();
+      m->launches += total_frames > 0 ? 3 : 1;
+      CK(cudaMemcpyAsync(counts.data(), m->note_count.p, sizeof(int) * n_pairs, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      bool overflow = false;
+      for (long long q = 0; q < n_pairs; ++q)
+        if (counts[q] > soff[q + 1] - soff[q]) overflow = full[q] = 1;
+      if (!overflow) break;
+      if (attempt == 1) return fail(BP_E_CUDA, api + ": note slots overflowed at full capacity (internal error)");
+    }
+    // ---- note offsets; past the note capacity only the counting goes on (bp_last_required totals the whole grid)
+    const long long note0 = n_notes;
+    for (long long q = 0; q < n_pairs; ++q) {
+      n_notes += counts[q];
+      if (n_notes > notes->note_capacity) notes_fit = false;
+      if (notes_fit) notes->note_off[p0 * n_files + q + 1] = (int32_t)n_notes;
+    }
+    const long long nc = n_notes - note0;  // notes of this chunk
+    if (!notes_fit || nc == 0) continue;
+    if (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude)
+      return fail(BP_E_INVALID, api + ": notes arrays missing");
+    std::vector<int> noff(n_pairs + 1);  // chunk-relative
+    for (long long q = 0; q <= n_pairs; ++q) noff[q] = (int)(notes->note_off[p0 * n_files + q] - note0);
+    CK(m->d_note_off.reserve((size_t)n_pairs + 1));
+    CK(m->d_start.reserve((size_t)nc));
+    CK(m->d_end.reserve((size_t)nc));
+    CK(m->d_pitch.reserve((size_t)nc));
+    CK(m->d_amp.reserve((size_t)nc));
+    CK(m->d_note_base.reserve((size_t)nc));
+    CK(m->d_bend_off.reserve((size_t)nc + 1));
+    CK(cudaMemcpyAsync(m->d_note_off.p, noff.data(), sizeof(int) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
+    compact_notes_kernel<<<dim3(n_files, P), 128, 0, st>>>(m->d_frame_off.p, m->d_slot_off.p, m->d_note_off.p,
+                                                           m->slot_start.p, m->slot_end.p, m->slot_pitch.p, m->d_start.p,
+                                                           m->d_end.p, m->d_pitch.p, m->d_note_base.p);
+    CKL();
+    m->launches += 1;
+    CK(cudaMemcpyAsync(notes->start_frame + note0, m->d_start.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(notes->end_frame + note0, m->d_end.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(notes->pitch_midi + note0, m->d_pitch.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    // ---- bend offsets: each setting's own include_pitch_bends (without: empty ranges, as bp_decode_device leaves them)
+    const long long bend0 = n_bends;
+    for (int s = 0; s < P; ++s) {
+      const bool with = params[p0 + s].include_pitch_bends != 0;
+      for (long long j = note0 + noff[(long long)s * n_files]; j < note0 + noff[(long long)(s + 1) * n_files]; ++j) {
+        if (with) n_bends += notes->end_frame[j] - notes->start_frame[j];
+        if (n_bends > 0x7fffffffLL) return fail(BP_E_CAPACITY, api + ": more than 2^31 pitch-bend values");
+        notes->bend_off[j + 1] = (int32_t)n_bends;
+      }
+    }
+    if (n_bends > notes->bend_capacity) bends_fit = false;
+    if (!bends_fit) continue;
+    const long long bc = n_bends - bend0;  // bends of this chunk
+    if (bc > 0 && !notes->bends) return fail(BP_E_INVALID, api + ": bends array missing");
+    std::vector<int> boff(nc + 1);
+    for (long long j = 0; j <= nc; ++j) boff[j] = (int)(notes->bend_off[note0 + j] - bend0);
+    CK(m->d_bends.reserve((size_t)bc + 1));
+    CK(cudaMemcpyAsync(m->d_bend_off.p, boff.data(), sizeof(int) * (nc + 1), cudaMemcpyHostToDevice, st));
+    {
+      ProfScope ps(m, 6, st);
+      launch_note_finish(d_note, d_contour, m->d_note_base.p, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_amp.p,
+                         m->d_bend_off.p, m->d_bends.p, (int)nc, bc > 0 ? 1 : 0, m->d_gauss, st);
+    }
+    CKL();
+    m->launches += 1;
+    CK(cudaMemcpyAsync(notes->amplitude + note0, m->d_amp.p, sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
+    if (bc > 0) CK(cudaMemcpyAsync(notes->bends + bend0, m->d_bends.p, sizeof(int) * bc, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  if (!notes_fit)
+    return g_need_notes = n_notes, fail(BP_E_CAPACITY, api + ": note_capacity too small, need " + std::to_string(n_notes));
+  if (!bends_fit)
+    return g_need_bends = n_bends, fail(BP_E_CAPACITY, api + ": bend_capacity too small, need " + std::to_string(n_bends));
+  return BP_OK;
+}
+
+int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                        const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                        bp_notes_t* notes) {
+  bool any_bends = false;
+  const int rc0 = check_grid_args("bp_decode_grid_host", m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (rc0) return rc0;
+  if (n_files == 0 || n_params == 0)
+    return bp_decode_grid_device(m, nullptr, nullptr, nullptr, h_frame_off, n_files, params, n_params, notes, m->stream);
+  DeviceGuard g(m->device);
+  const int64_t total = h_frame_off[n_files];
+  cudaStream_t st = m->stream;
+  const int rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {  // uploaded once for the whole grid
+    if (!h_note || !h_onset || (any_bends && !h_contour)) return fail(BP_E_INVALID, "bp_decode_grid_host: null posteriorgram");
+    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    if (any_bends)
+      CK(cudaMemcpyAsync(m->st_contour.p, h_contour, sizeof(float) * total * kContourBins, cudaMemcpyHostToDevice, st));
+  }
+  return bp_decode_grid_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, n_params,
+                               notes, st);
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,

@@ -18,6 +18,9 @@
 //                        melodia loop with per-column maxima kept in shared memory
 //   note_finish_kernel   one warp per note: amplitude (NumPy pairwise float32 mean) and per-frame pitch-bend
 //                        arg-max in float64
+// The grid decode (bp_decode_grid_*) runs the same three kernels for many parameter sets at once (template kGrid): the
+// prep per distinct pitch range, the candidates per distinct (range, infer_onsets, onset_thresh), the loops per
+// (file, setting) on the setting's own copy of E; blockIdx.y picks the group or setting.
 #include "kernels.cuh"
 
 namespace bp {
@@ -70,12 +73,20 @@ __device__ __forceinline__ double frame_diff3(float a, float m1, float m2) {
   return d < 0.0 ? 0.0 : d;
 }
 
+// kGrid: blockIdx.y is a prep group of g (range, maxima and the E copies of its settings); otherwise lo / hi and one E
+template <bool kGrid>
 __global__ void __launch_bounds__(256) decode_prep_kernel(const float* __restrict__ note, const float* __restrict__ onset,
                                                           const long long* __restrict__ frame_off, int n_files,
                                                           float* __restrict__ energy,
                                                           unsigned int* __restrict__ max_onset,     // [n_files] ordered-uint
                                                           unsigned long long* __restrict__ max_fd,  // [n_files] bits of a double >= 0
-                                                          int lo, int hi) {
+                                                          int lo, int hi, DecodeGridDev g) {
+  if constexpr (kGrid) {
+    lo = g.prep[blockIdx.y].lo;
+    hi = g.prep[blockIdx.y].hi;
+    max_onset += (size_t)blockIdx.y * n_files;
+    max_fd += (size_t)blockIdx.y * n_files;
+  }
   __shared__ float s_n[kTileFrames + 2][kPitches + 1];  // rows g0-2 .. g0+31, pitch range applied
   __shared__ RowInfo s_row[kTileFrames];
   __shared__ unsigned int s_mo[8];
@@ -130,17 +141,38 @@ __global__ void __launch_bounds__(256) decode_prep_kernel(const float* __restric
   // E is column-major per file ([88][T]): lanes = consecutive frames -> contiguous 128-byte runs
   if (lane < nrows) {
     const RowInfo ri = s_row[lane];
-    float* e = energy + ri.base * kPitches + ri.t;
-    for (int f = warp; f < kPitches; f += 8) e[(long long)f * ri.T] = s_n[lane + 2][f];
+    if constexpr (kGrid) {  // every setting of the group gets its own copy: its loops zero it
+      const int j1 = g.prep[blockIdx.y].set_hi;
+      for (int j = g.prep[blockIdx.y].set_lo; j < j1; ++j) {
+        float* e = energy + g.sets[j] * g.e_stride + ri.base * kPitches + ri.t;
+        for (int f = warp; f < kPitches; f += 8) e[(long long)f * ri.T] = s_n[lane + 2][f];
+      }
+    } else {
+      float* e = energy + ri.base * kPitches + ri.t;
+      for (int f = warp; f < kPitches; f += 8) e[(long long)f * ri.T] = s_n[lane + 2][f];
+    }
   }
 }
 
+// kGrid: blockIdx.y is a candidate group of g (its parameters, its prep group's maxima, its own bitmap)
+template <bool kGrid>
 __global__ void __launch_bounds__(256) decode_cand_kernel(const float* __restrict__ note, const float* __restrict__ onset,
                                                           const long long* __restrict__ frame_off, int n_files,
                                                           const unsigned int* __restrict__ max_onset,
                                                           const unsigned long long* __restrict__ max_fd,
                                                           unsigned int* __restrict__ candbits, int lo, int hi, int infer,
-                                                          double onset_thresh, double* __restrict__ onset64_out) {
+                                                          double onset_thresh, double* __restrict__ onset64_out,
+                                                          DecodeGridDev g) {
+  if constexpr (kGrid) {
+    const DecodeCandGroup cg = g.cand[blockIdx.y];
+    lo = cg.lo;
+    hi = cg.hi;
+    infer = cg.infer;
+    onset_thresh = cg.onset_thresh;
+    max_onset += (size_t)cg.prep * n_files;
+    max_fd += (size_t)cg.prep * n_files;
+    candbits += blockIdx.y * g.cand_stride;
+  }
   __shared__ float s_n[kTileFrames + 4][kPitches + 1];  // note rows g0-3 .. g0+32 (inferred onsets only)
   __shared__ double s_v[kTileFrames + 2][kPitches];     // float64 onset value of rows g0-1 .. g0+32
   __shared__ RowInfo s_row[kTileFrames + 2];
@@ -320,12 +352,25 @@ __device__ void refresh_column(const float* col, int T, float* bmax, int* barg, 
   *out_t = bt;
 }
 
+// kGrid: blockIdx.y is a setting of g, with its own parameters, E, block maxima and note slots / count
+// (setting * n_files + file), reading its candidate group's bitmap
+template <bool kGrid>
 __global__ void __launch_bounds__(kSeqThreads) decode_seq_kernel(
     const long long* __restrict__ frame_off, float* __restrict__ energy, const unsigned int* __restrict__ candbits,
     const long long* __restrict__ slot_off, int* __restrict__ note_count, int* __restrict__ note_start,
     int* __restrict__ note_end, int* __restrict__ note_pitch, int* __restrict__ overflow, float* __restrict__ blk_max,
-    int* __restrict__ blk_arg, DecodeParamsDev p) {
+    int* __restrict__ blk_arg, DecodeParamsDev p, DecodeGridDev g) {
   const int file = blockIdx.x;
+  if constexpr (kGrid) {
+    const int s = blockIdx.y;
+    p = g.setting[s].p;
+    energy += s * g.e_stride;
+    candbits += g.setting[s].cand * g.cand_stride;
+    blk_max += s * g.blk_stride;
+    blk_arg += s * g.blk_stride;
+    slot_off += (long long)s * g.n_files;
+    note_count += (long long)s * g.n_files;
+  }
   const long long base = frame_off[file];
   const int T = (int)(frame_off[file + 1] - base);
   const int lane = threadIdx.x & 31;
@@ -505,14 +550,36 @@ void launch_decode_notes(const float* note, const float* onset, const DecodeBuff
   if (cells > 0) {
     const int threads = 256;
     const unsigned int blocks = (unsigned int)((total_frames + kTileFrames - 1) / kTileFrames);
-    decode_prep_kernel<<<blocks, threads, 0, st>>>(note, onset, b.frame_off, n_files, b.energy, b.max_onset, b.max_fd,
-                                                   p.lo_col, p.hi_col);
-    decode_cand_kernel<<<blocks, threads, 0, st>>>(note, onset, b.frame_off, n_files, b.max_onset, b.max_fd,
-                                                    b.candbits, p.lo_col, p.hi_col, p.infer_onsets, p.onset_thresh, nullptr);
+    decode_prep_kernel<false><<<blocks, threads, 0, st>>>(note, onset, b.frame_off, n_files, b.energy, b.max_onset,
+                                                          b.max_fd, p.lo_col, p.hi_col, DecodeGridDev{});
+    decode_cand_kernel<false><<<blocks, threads, 0, st>>>(note, onset, b.frame_off, n_files, b.max_onset, b.max_fd,
+                                                          b.candbits, p.lo_col, p.hi_col, p.infer_onsets, p.onset_thresh,
+                                                          nullptr, DecodeGridDev{});
   }
-  decode_seq_kernel<<<n_files, kSeqThreads, 0, st>>>(b.frame_off, b.energy, b.candbits, b.slot_off, b.note_count,
-                                                     b.note_start, b.note_end, b.note_pitch, b.overflow, b.blk_max,
-                                                     b.blk_arg, p);
+  decode_seq_kernel<false><<<n_files, kSeqThreads, 0, st>>>(b.frame_off, b.energy, b.candbits, b.slot_off, b.note_count,
+                                                            b.note_start, b.note_end, b.note_pitch, b.overflow, b.blk_max,
+                                                            b.blk_arg, p, DecodeGridDev{});
+}
+
+long long decode_cand_words(long long total_frames) { return total_frames * kPitches / 32 + 2; }
+
+// The launches of launch_decode_notes for a chunk of settings: prep once per prep group, candidates once per candidate
+// group, the loops once per (file, setting).  b.max_onset / b.max_fd hold n_prep * n_files entries.
+void launch_decode_grid(const float* note, const float* onset, const DecodeBuffers& b, int n_files,
+                        long long total_frames, const DecodeGridDev& g, int n_prep, int n_cand, int n_settings,
+                        cudaStream_t st) {
+  cudaMemsetAsync(b.max_onset, 0, sizeof(unsigned int) * n_files * n_prep, st);
+  cudaMemsetAsync(b.max_fd, 0, sizeof(unsigned long long) * n_files * n_prep, st);
+  if (total_frames > 0) {
+    const unsigned int blocks = (unsigned int)((total_frames + kTileFrames - 1) / kTileFrames);
+    decode_prep_kernel<true><<<dim3(blocks, n_prep), 256, 0, st>>>(note, onset, b.frame_off, n_files, b.energy,
+                                                                   b.max_onset, b.max_fd, 0, 0, g);
+    decode_cand_kernel<true><<<dim3(blocks, n_cand), 256, 0, st>>>(note, onset, b.frame_off, n_files, b.max_onset,
+                                                                   b.max_fd, b.candbits, 0, 0, 0, 0.0, nullptr, g);
+  }
+  decode_seq_kernel<true><<<dim3(n_files, n_settings), kSeqThreads, 0, st>>>(
+      b.frame_off, b.energy, b.candbits, b.slot_off, b.note_count, b.note_start, b.note_end, b.note_pitch, b.overflow,
+      b.blk_max, b.blk_arg, DecodeParamsDev{}, g);
 }
 
 // float64 inferred onsets of a batch of files (reference: note_creation.py:289-311): the two cell-parallel kernels of the
@@ -523,9 +590,10 @@ void launch_infer_onsets(const float* note, const float* onset, const DecodeBuff
   cudaMemsetAsync(b.max_fd, 0, sizeof(unsigned long long) * n_files, st);
   if (total_frames <= 0) return;
   const unsigned int blocks = (unsigned int)((total_frames + kTileFrames - 1) / kTileFrames);
-  decode_prep_kernel<<<blocks, 256, 0, st>>>(note, onset, b.frame_off, n_files, b.energy, b.max_onset, b.max_fd, 0, kPitches);
-  decode_cand_kernel<<<blocks, 256, 0, st>>>(note, onset, b.frame_off, n_files, b.max_onset, b.max_fd, b.candbits, 0,
-                                             kPitches, 1, 0.0, out64);
+  decode_prep_kernel<false><<<blocks, 256, 0, st>>>(note, onset, b.frame_off, n_files, b.energy, b.max_onset, b.max_fd,
+                                                    0, kPitches, DecodeGridDev{});
+  decode_cand_kernel<false><<<blocks, 256, 0, st>>>(note, onset, b.frame_off, n_files, b.max_onset, b.max_fd, b.candbits,
+                                                    0, kPitches, 1, 0.0, out64, DecodeGridDev{});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -574,7 +642,7 @@ __global__ void note_finish_kernel(const float* __restrict__ note, const float* 
     float s = np_pairwise_sum(note + (base + t0) * kPitches + col, len, kPitches);
     amp[n] = __fdiv_rn(s, (float)len);
   }
-  if (!with_bends) return;
+  if (!with_bends || bend_off[n + 1] == bend_off[n]) return;  // empty: a grid setting without pitch bends
   // reference: note_creation.py:198-218 ; contour bin of the note = 3*(pitch-21)
   const int c = 3 * col;
   const int lo = max(c - 25, 0);

@@ -229,9 +229,39 @@ struct DecodeBuffers {
 long long decode_block_slots(long long total_frames, int n_files);
 void launch_decode_notes(const float* note, const float* onset, const DecodeBuffers& buf, int n_files,
                          long long total_frames, const DecodeParamsDev& p, cudaStream_t st);
+// Grid decode: a chunk of parameter sets ("settings") over one batch.  The cell-parallel kernels run once per group of
+// settings that share their inputs (blockIdx.y = group); the sequential loops once per (file, setting).
+struct DecodePrepGroup {  // a distinct pitch range (lo, hi): constrained frames, per-file max(onsets) / max(frame_diff)
+  int lo, hi;
+  int set_lo, set_hi;     // its settings are grid_sets[set_lo .. set_hi); the prep writes E of each of them
+};
+struct DecodeCandGroup {  // a distinct (lo, hi, infer_onsets, onset_thresh): one candidate bitmap
+  double onset_thresh;
+  int lo, hi, infer, prep;  // prep: its prep group
+};
+struct DecodeSettingDev {
+  DecodeParamsDev p;
+  int cand;  // candidate group
+};
+struct DecodeGridDev {
+  const DecodePrepGroup* prep;
+  const DecodeCandGroup* cand;
+  const int* sets;                  // chunk-local setting indices, grouped by prep group
+  const DecodeSettingDev* setting;  // [settings of the chunk]
+  int n_files;
+  // per-setting / per-group strides of the DecodeBuffers arrays: E, candidate bitmap and block maxima per setting (E,
+  // blocks) or candidate group (bitmap); max_onset / max_fd have n_files entries per prep group; slot_off and note_count
+  // are indexed setting * n_files + file
+  long long e_stride, cand_stride, blk_stride;
+};
+long long decode_cand_words(long long total_frames);  // 32-bit words of one candidate bitmap
+void launch_decode_grid(const float* note, const float* onset, const DecodeBuffers& buf, int n_files,
+                        long long total_frames, const DecodeGridDev& g, int n_prep, int n_cand, int n_settings,
+                        cudaStream_t st);
 void launch_infer_onsets(const float* note, const float* onset, const DecodeBuffers& buf, int n_files, long long total_frames,
                          double* out64 /* [total_frames][88] */, cudaStream_t st);
-// amplitude (NumPy pairwise mean) + pitch bends for compacted notes
+// amplitude (NumPy pairwise mean) + pitch bends for compacted notes; a note whose bend range is empty gets none (the
+// notes of a grid setting without pitch bends)
 void launch_note_finish(const float* note, const float* contour, const long long* note_frame_base /*[n_notes]*/,
                         const int* start, const int* end, const int* pitch, float* amp, const int* bend_off,
                         int* bends, int n_notes, int with_bends, const double* gauss /*[51] device*/,

@@ -251,11 +251,13 @@ class Model:
             })  # fmt: skip
         return out
 
-    def _with_capacity(self, n_files: int, total_frames: int, call):
-        note_cap = max(4096, 2 * total_frames)
-        bend_cap = max(65536, 24 * total_frames)
+    def _with_capacity(self, n_files: int, total_frames: int, call, n_params: int = 1):
+        """call(notes) with capacities grown from bp_last_required; n_params: settings of a grid decode (the note offsets
+        have n_params * n_files + 1 entries, the first guess scales with n_params)."""
+        note_cap = max(4096, 2 * total_frames * n_params)
+        bend_cap = max(65536, 24 * total_frames * n_params)
         for _ in range(3):  # at most: notes too small, then bends too small, then success
-            notes, arrs = self._alloc_notes(n_files, note_cap, bend_cap)
+            notes, arrs = self._alloc_notes(n_files * n_params, note_cap, bend_cap)
             try:
                 call(notes)
                 return arrs
@@ -275,6 +277,20 @@ class Model:
                       min_pitch_idx=0, max_pitch_idx=88) -> List[Dict[str, np.ndarray]]:
         """Posteriorgrams of a batch of files -> note arrays per file (reference: note_creation.py:52-111)."""
         n_files = len(notes)
+        foff, n_all, o_all, c_all = self._cat_posteriorgrams(notes, onsets, contours, include_pitch_bends)
+        p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
+                         include_pitch_bends, min_pitch_idx, max_pitch_idx)
+        arrs = self._with_capacity(
+            n_files, int(foff[-1]),
+            lambda nt: self._lib.bp_decode_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(c_all), _ptr(foff), n_files, C.byref(p), C.byref(nt)),
+        )
+        return self._split_notes(arrs, n_files)
+
+    @staticmethod
+    def _cat_posteriorgrams(notes, onsets, contours, need_contours: bool):
+        """Per-file posteriorgrams -> (frame offsets, note, onset, contour) back to back, as the decode entry points
+        take them."""
+        n_files = len(notes)
         foff = np.zeros(n_files + 1, np.int64)
         for i, a in enumerate(notes):
             if a.shape[1:] != (N_FREQ_BINS_NOTES,) or onsets[i].shape != a.shape:
@@ -284,20 +300,46 @@ class Model:
         cat = lambda xs, w: np.ascontiguousarray(np.concatenate([np.asarray(x, _F32).reshape(-1, w) for x in xs]) if xs else np.zeros((0, w), _F32), dtype=_F32)  # noqa: E731
         n_all, o_all = cat(list(notes), N_FREQ_BINS_NOTES), cat(list(onsets), N_FREQ_BINS_NOTES)
         if contours is None:
-            if include_pitch_bends:
+            if need_contours:
                 raise ValueError("pitch bends need the contour posteriorgram")
             c_all = np.zeros((max(total, 1), N_FREQ_BINS_CONTOURS), _F32)
         else:
             c_all = cat(list(contours), N_FREQ_BINS_CONTOURS)
             if c_all.shape[0] != total:
                 raise ValueError("contour posteriorgrams must have as many frames as note posteriorgrams")
-        p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
-                         include_pitch_bends, min_pitch_idx, max_pitch_idx)
+        return foff, n_all, o_all, c_all
+
+    _DECODE_DEFAULTS = dict(onset_thresh=0.5, frame_thresh=0.3, min_note_len=11, energy_tol=11, infer_onsets=True,
+                            melodia_trick=True, include_pitch_bends=True, min_pitch_idx=0, max_pitch_idx=88)
+
+    def decode_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
+                    contours: Optional[Sequence[np.ndarray]], settings: Sequence[Dict[str, Any]],
+                    split_notes: bool = True):
+        """Posteriorgrams of a batch of files decoded under every setting of a grid in ONE library call
+        (`bp_decode_grid_host`: the posteriorgrams go up once, settings sharing a pitch range share the per-cell work,
+        the greedy loops of all (setting, file) pairs run in parallel).  A setting is a dict of `decode_arrays`' keyword
+        arguments (missing ones take its defaults).  Returns [setting][file] note-array dicts, each what `decode_arrays`
+        gives for that setting; with split_notes=False the concatenated arrays of the call instead (note_off has
+        len(settings) * n_files + 1 entries, setting-major)."""
+        n_files, n_params = len(notes), len(settings)
+        ps = (_lib.DecodeParams * max(n_params, 1))()
+        for k, s in enumerate(settings):
+            unknown = set(s) - set(self._DECODE_DEFAULTS)
+            if unknown:
+                raise TypeError(f"settings[{k}]: unknown decode argument(s) {sorted(unknown)}")
+            ps[k] = self._params(**{**self._DECODE_DEFAULTS, **s})
+        need_contours = any(bool(p.include_pitch_bends) for p in ps[:n_params])
+        foff, n_all, o_all, c_all = self._cat_posteriorgrams(notes, onsets, contours, need_contours)
         arrs = self._with_capacity(
-            n_files, total,
-            lambda nt: self._lib.bp_decode_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(c_all), _ptr(foff), n_files, C.byref(p), C.byref(nt)),
+            n_files, int(foff[-1]),
+            lambda nt: self._lib.bp_decode_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(c_all), _ptr(foff), n_files,
+                                                     ps, n_params, C.byref(nt)),
+            n_params=n_params,
         )
-        return self._split_notes(arrs, n_files)
+        if not split_notes:
+            return arrs
+        flat = self._split_notes(arrs, n_params * n_files)
+        return [flat[k * n_files : (k + 1) * n_files] for k in range(n_params)]
 
     def infer_onsets_array(self, onsets: np.ndarray, frames: np.ndarray) -> np.ndarray:
         """reference: note_creation.py:289-311 `get_infered_onsets` (n_diff = 2) -> float64 (T, 88), on the device."""
@@ -639,6 +681,34 @@ def predict(
                 ],
             }, f)  # fmt: skip
     return model_output, midi_data, note_events
+
+
+def predict_grid(
+    audio: Union[np.ndarray, pathlib.Path, str],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+):
+    """`predict` of one recording under every setting of a grid (addition; no reference counterpart): the model runs
+    once (device ingest of a path, then `bp_run_inference_host`) and all settings are decoded in one
+    `bp_decode_grid_host` call.  `audio` is a path or a mono 22 050 Hz array; a setting is a dict of `predict`'s
+    keyword arguments (onset_threshold, frame_threshold, minimum_note_length in ms, minimum_frequency,
+    maximum_frequency, multiple_pitch_bends, melodia_trick, midi_tempo), missing ones take its defaults.
+
+    Returns (model_output, [(midi_data, note_events) per setting]); each pair equals what `predict` gives for that
+    setting, with the events as `NoteEventList`s and the MIDI objects as `LazyPrettyMIDI`s (`predict_batch(lazy=True)`).
+    The model output is not column-zeroed: the settings may disagree on the frequency range."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    if isinstance(audio, np.ndarray):
+        if audio.ndim != 1:
+            raise ValueError("audio must be mono (1-D)")
+    else:
+        audio, _ = load_audio_device(audio, model)
+    conv = [infer.grid_setting(s, predict_names=True) for s in settings]
+    model_output = model.run_inference_arrays([audio])[0]
+    arrs = model.decode_grid([model_output["note"]], [model_output["onset"]], [model_output["contour"]],
+                             [d for d, _ in conv], split_notes=False)
+    events = infer.note_events_batch(arrs, len(conv), include_pitch_bends=True, lazy=True)
+    return model_output, [(infer.LazyPrettyMIDI(ev, **midi_kw), ev) for (_, midi_kw), ev in zip(conv, events)]
 
 
 def predict_batch(

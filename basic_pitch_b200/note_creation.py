@@ -137,6 +137,64 @@ def model_output_to_notes(
     return note_events_to_midi(events, multiple_pitch_bends, midi_tempo), events
 
 
+_NOTES_SETTING = dict(onset_thresh=None, frame_thresh=None, infer_onsets=True, min_note_len=DEFAULT_MIN_NOTE_LEN,
+                      min_freq=None, max_freq=None, include_pitch_bends=True, multiple_pitch_bends=False,
+                      melodia_trick=True, midi_tempo=120)
+# predict's keyword names (inference.py) -> model_output_to_notes'; minimum_note_length is in milliseconds
+_PREDICT_SETTING = dict(onset_threshold=("onset_thresh", 0.5), frame_threshold=("frame_thresh", 0.3),
+                        minimum_note_length=("min_note_len", 127.7), minimum_frequency=("min_freq", None),
+                        maximum_frequency=("max_freq", None), multiple_pitch_bends=("multiple_pitch_bends", False),
+                        melodia_trick=("melodia_trick", True), midi_tempo=("midi_tempo", 120))
+
+
+def grid_setting(setting: Dict, predict_names: bool = False) -> Tuple[Dict, Dict]:
+    """One setting of a grid decode -> (`Model.decode_arrays` keyword arguments, `note_events_to_midi` keyword arguments),
+    with the arithmetic `model_output_to_notes` (`_decode`) and `predict` apply to the same arguments: Hz limits to the
+    columns `frequency_to_column_range` gives, and with predict_names=True `predict`'s keyword names and defaults
+    (onset_threshold, frame_threshold, minimum_note_length in ms -> frames, minimum_frequency, maximum_frequency,
+    multiple_pitch_bends, melodia_trick, midi_tempo).  Otherwise `model_output_to_notes`' names; onset_thresh and
+    frame_thresh are required as there.  Unknown names raise TypeError."""
+    s = dict(setting)
+    if predict_names:
+        unknown = set(s) - set(_PREDICT_SETTING)
+        if unknown:
+            raise TypeError(f"unknown predict argument(s) {sorted(unknown)}")
+        s = {name: s.get(k, default) for k, (name, default) in _PREDICT_SETTING.items()}
+        s["min_note_len"] = int(np.round(s["min_note_len"] / 1000 * (AUDIO_SAMPLE_RATE / FFT_HOP)))
+    unknown = set(s) - set(_NOTES_SETTING)
+    if unknown:
+        raise TypeError(f"unknown model_output_to_notes argument(s) {sorted(unknown)}")
+    s = {**_NOTES_SETTING, **s}
+    if s["onset_thresh"] is None or s["frame_thresh"] is None:
+        raise TypeError("a setting needs onset_thresh and frame_thresh")
+    lo, hi = frequency_to_column_range(s["min_freq"], s["max_freq"])
+    decode = dict(onset_thresh=s["onset_thresh"], frame_thresh=s["frame_thresh"], min_note_len=s["min_note_len"],
+                  energy_tol=ENERGY_TOLERANCE, infer_onsets=s["infer_onsets"], melodia_trick=s["melodia_trick"],
+                  include_pitch_bends=s["include_pitch_bends"], min_pitch_idx=lo, max_pitch_idx=hi)
+    return decode, dict(multiple_pitch_bends=s["multiple_pitch_bends"], midi_tempo=s["midi_tempo"])
+
+
+def model_output_to_notes_grid(output: Dict[str, np.ndarray], settings: Sequence[Dict], model=None):
+    """`model_output_to_notes(output, **setting)` for every setting of a grid, decoded in one library call
+    (`Model.decode_grid`, `bp_decode_grid_host`).  A setting is a dict of `model_output_to_notes`' keyword arguments
+    (min_freq / max_freq in Hz included).  Returns one (midi, note_events) per setting, each equal to that call's.
+
+    Unlike `model_output_to_notes` (and the reference's `constrain_frequency`), the arrays of `output` are NOT modified:
+    the settings may disagree on the frequency range, so no zeroing of the caller's columns would fit them all."""
+    from .inference import default_model
+
+    mdl = model if model is not None else default_model()
+    conv = [grid_setting(s) for s in settings]
+    contour = output.get("contour")
+    res = mdl.decode_grid([output["note"]], [output["onset"]], None if contour is None else [contour], [d for d, _ in conv])
+    n_frames = output["note"].shape[0]
+    out = []
+    for (d, midi_kw), r in zip(conv, res):
+        events = note_events_from_arrays(r[0], n_frames, d["include_pitch_bends"])
+        out.append((note_events_to_midi(events, **midi_kw), events))
+    return out
+
+
 def note_events_from_arrays(res: Dict[str, np.ndarray], n_frames: int, include_pitch_bends: bool = True) -> List[NoteEvent]:
     """Decode arrays (frames) -> the reference's list of (start_s, end_s, pitch, amplitude, bends)."""
     times = model_frames_to_time(n_frames)
@@ -437,7 +495,7 @@ def get_infered_onsets(onsets, frames, n_diff: int = 2, model=None):
 
 
 __all__ = [
-    "model_output_to_notes", "output_to_notes_polyphonic", "note_events_to_midi", "write_note_files", "sonify_batch",
+    "model_output_to_notes", "model_output_to_notes_grid", "grid_setting", "output_to_notes_polyphonic", "note_events_to_midi", "write_note_files", "sonify_batch",
     "note_events_batch",
     "NoteEventList", "LazyPrettyMIDI", "drop_overlapping_pitch_bends",
     "model_frames_to_time", "constrain_frequency", "midi_pitch_to_contour_bin", "sonify_midi", "sonify_salience",

@@ -140,6 +140,35 @@ int bp_decode_device(bp_model_t* m, const float* d_note, const float* d_onset, c
 int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
                    const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, bp_notes_t* notes);
 
+/* ---- stage 3 under a grid of decode parameters ------------------------------------------------
+ * reference: note_creation.py:52-111 (model_output_to_notes without the MIDI object), called once per parameter set.
+ * One call decodes the batch under each of params[0 .. n_params): every (setting, file) gets exactly the notes
+ * bp_decode_device gives for that setting.  Settings that share a pitch range share the per-cell preparation; those
+ * also sharing infer_onsets and onset_thresh share the onset candidates; the greedy loops run once per (file, setting),
+ * in parallel.
+ * Output layout: notes->note_off has n_params * n_files + 1 entries, parameter-major: the notes of setting p, file i
+ * occupy [note_off[p*n_files+i], note_off[p*n_files+i+1]) in the reference's generation order; bend_off per note as in
+ * bp_decode_device (a setting without include_pitch_bends has empty bend ranges).  Posteriorgrams are not modified.
+ * Every setting is validated before anything is enqueued: a bad one returns BP_E_INVALID naming its index
+ * ("decode params[7]: ...").  BP_E_CAPACITY: bp_last_required gives the capacities of the whole grid.  n_params == 0 or
+ * n_files == 0: BP_OK with note_off[0] = 0.  The settings run in chunks (bp_decode_grid_chunk_params); the kernel
+ * launches of a call depend on the number of chunks, not on n_params.  _device: posteriorgrams in device memory, work
+ * on `stream`, synchronised before returning; _host: host posteriorgrams, uploaded once for all settings (h_contour may
+ * be NULL when no setting has include_pitch_bends). */
+int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                          const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                          int32_t n_params, bp_notes_t* notes, void* stream);
+int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                        const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                        bp_notes_t* notes);
+/* Host-only: settings per chunk of a grid decode over a batch of this shape (>= 1).  A chunk of c settings keeps its
+ * device workspace within 2 GiB, c * W <= 2^31 bytes, unless one setting alone needs more (c = 1), where
+ *   W = 4 C + 4 (C / 32 + 2) + 8 * 88 * (F / 256 + n_files + 1) + 12 min(C, 8 F + 64 n_files) + 16 n_files + 64
+ * bytes, F = total_frames, C = 88 F: per setting its "remaining energy" copy, a candidate bitmap, the block maxima of the
+ * melodia loop, the first allowance of note slots and per-file counters.  A (setting, file) that outgrows its first
+ * allowance of note slots reruns its chunk with 88 T slots for that pair, beyond this budget. */
+int64_t bp_decode_grid_chunk_params(int64_t total_frames, int32_t n_files);
+
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
