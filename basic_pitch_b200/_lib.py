@@ -24,7 +24,7 @@ EXPORTS = [
     "bp_model_create", "bp_model_destroy", "bp_model_device", "bp_model_param_block", "bp_model_refresh",
     "bp_model_launch_count", "bp_forward_device", "bp_forward_host", "bp_run_inference_device",
     "bp_run_inference_host", "bp_decode_device", "bp_decode_host", "bp_transcribe_host", "bp_transcribe_device",
-    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params",
+    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_clocks", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params", "bp_default_score_params", "bp_frame_times", "bp_score_grid_device", "bp_score_grid_host", "bp_score_notes_host",
 ]  # fmt: skip
 
 
@@ -54,6 +54,24 @@ class Notes(C.Structure):
         ("amplitude", C.c_void_p),
         ("bend_off", C.c_void_p),
         ("bends", C.c_void_p),
+    ]
+
+
+class NoteSet(C.Structure):
+    _fields_ = [
+        ("note_off", C.c_void_p),
+        ("onset_s", C.c_void_p),
+        ("offset_s", C.c_void_p),
+        ("log2_hz", C.c_void_p),
+    ]
+
+
+class ScoreParams(C.Structure):
+    _fields_ = [
+        ("onset_tolerance", C.c_double),
+        ("pitch_tolerance", C.c_double),
+        ("offset_ratio", C.c_double),
+        ("offset_min_tolerance", C.c_double),
     ]
 
 
@@ -119,6 +137,14 @@ def load() -> C.CDLL:
     lib.bp_decode_grid_host.argtypes = [vp, vp, vp, vp, vp, i32, C.POINTER(DecodeParams), i32, C.POINTER(Notes)]
     lib.bp_decode_grid_chunk_params.argtypes = [i64, i32]
     lib.bp_decode_grid_chunk_params.restype = i64
+    lib.bp_default_score_params.argtypes = [C.POINTER(ScoreParams)]
+    lib.bp_default_score_params.restype = None
+    lib.bp_frame_times.argtypes = [i64, vp]
+    lib.bp_score_grid_device.argtypes = [vp, vp, vp, vp, i32, C.POINTER(DecodeParams), i32, C.POINTER(NoteSet),
+                                         C.POINTER(ScoreParams), vp, vp, vp]
+    lib.bp_score_grid_host.argtypes = [vp, vp, vp, vp, i32, C.POINTER(DecodeParams), i32, C.POINTER(NoteSet),
+                                       C.POINTER(ScoreParams), vp, vp]
+    lib.bp_score_notes_host.argtypes = [vp, C.POINTER(NoteSet), C.POINTER(NoteSet), i32, C.POINTER(ScoreParams), vp]
     lib.bp_transcribe_host.argtypes = [vp, vp, vp, i32, C.POINTER(DecodeParams), vp, vp, vp, vp, C.POINTER(Notes)]
     lib.bp_transcribe_device.argtypes = [vp, vp, vp, i32, C.POINTER(DecodeParams), vp, C.POINTER(Notes), vp]
     lib.bp_infer_onsets_host.argtypes = [vp, vp, vp, i64, vp]

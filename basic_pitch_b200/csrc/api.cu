@@ -201,6 +201,10 @@ struct bp_model {
   DevBuf<int> note_count, slot_start, slot_end, slot_pitch, overflow, d_note_off, d_start, d_end, d_pitch, d_bend_off,
       d_bends;
   DevBuf<unsigned char> grid_tab;  // group and setting tables of a grid-decode chunk (DecodeGridDev)
+  // scoring (bp_score_*): the call's references, tables and explicit estimates; match workspace; counts of the call
+  DevBuf<unsigned char> score_in;
+  DevBuf<int> score_ws_ref, score_ws_est;
+  DevBuf<long long> score_counts;
   int64_t last_forward_n = 0;
   int last_path = 0;
   // optional per-kernel timing (bench.py roofline): CUDA events around one kernel family
@@ -602,6 +606,231 @@ int check_grid_args(const std::string& api, const bp_model* m, const int64_t* h_
   for (int i = 1; i <= n_files; ++i)
     if (h_frame_off[i] < h_frame_off[i - 1]) return fail(BP_E_INVALID, api + ": frame offsets must be non-decreasing");
   return BP_OK;
+}
+
+// The chunk loop of the grid entry points (bp_decode_grid_*, bp_score_grid_*): per chunk of settings the group tables,
+// the decode kernels with the rerun of pairs that outgrew their first allowance of note slots, then
+// tail(p0, P, counts, soff) with the chunk's notes in the slots: pair q (setting-major, chunk-local) has counts[q] notes
+// from m->slot_*[soff[q]], soff also at m->d_slot_off.  A tail returns BP_OK to go on to the next chunk.
+template <class Tail>
+int decode_grid_chunks(bp_model* m, const std::string& api, const float* d_note, const float* d_onset,
+                       const std::vector<long long>& foff, int n_files, const bp_decode_params_t* params, int n_params,
+                       cudaStream_t st, Tail&& tail) {
+  const long long total_frames = foff[n_files];
+  const long long cells = total_frames * kPitches;
+  const long long chunk = bp_decode_grid_chunk_params(total_frames, n_files);
+  DecodeGridDev gd{};
+  gd.n_files = n_files;
+  gd.e_stride = cells;
+  gd.cand_stride = decode_cand_words(total_frames);
+  gd.blk_stride = (long long)kPitches * decode_block_slots(total_frames, n_files);
+  CK(m->d_frame_off.reserve(n_files + 1));
+  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
+
+  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
+    const int P = (int)std::min<long long>(chunk, n_params - p0);
+    const long long n_pairs = (long long)P * n_files;  // (setting, file), setting-major
+    // ---- groups: settings sharing a pitch range share the prep; those also sharing infer_onsets and onset_thresh
+    // share the candidates
+    std::vector<DecodeSettingDev> sd(P);
+    std::vector<DecodePrepGroup> prep;
+    std::vector<DecodeCandGroup> cand;
+    std::vector<int> prep_of(P);
+    for (int s = 0; s < P; ++s) {
+      sd[s].p = params_dev(params[p0 + s]);
+      const DecodeParamsDev& q = sd[s].p;
+      int pg = 0;
+      while (pg < (int)prep.size() && (prep[pg].lo != q.lo_col || prep[pg].hi != q.hi_col)) ++pg;
+      if (pg == (int)prep.size()) prep.push_back(DecodePrepGroup{q.lo_col, q.hi_col, 0, 0});
+      ++prep[pg].set_hi;  // count for now
+      prep_of[s] = pg;
+      int cg = 0;
+      while (cg < (int)cand.size() && (cand[cg].prep != pg || cand[cg].infer != q.infer_onsets ||
+                                       !(cand[cg].onset_thresh == q.onset_thresh)))
+        ++cg;
+      if (cg == (int)cand.size()) cand.push_back(DecodeCandGroup{q.onset_thresh, q.lo_col, q.hi_col, q.infer_onsets, pg});
+      sd[s].cand = cg;
+    }
+    const int n_prep = (int)prep.size(), n_cand = (int)cand.size();
+    for (int k = 0, at = 0; k < n_prep; ++k) {
+      const int n = prep[k].set_hi;
+      prep[k].set_lo = prep[k].set_hi = at;
+      at += n;
+    }
+    std::vector<int> sets(P);
+    for (int s = 0; s < P; ++s) sets[prep[prep_of[s]].set_hi++] = s;
+    // one upload of the tables, 16-byte aligned sections
+    auto sec = [](size_t bytes) { return (bytes + 15) / 16 * 16; };
+    const size_t o_cand = sec(sizeof(DecodePrepGroup) * n_prep), o_sets = o_cand + sec(sizeof(DecodeCandGroup) * n_cand),
+                 o_set = o_sets + sec(sizeof(int) * P), tab_bytes = o_set + sizeof(DecodeSettingDev) * P;
+    std::vector<unsigned char> tab(tab_bytes);
+    std::memcpy(tab.data(), prep.data(), sizeof(DecodePrepGroup) * n_prep);
+    std::memcpy(tab.data() + o_cand, cand.data(), sizeof(DecodeCandGroup) * n_cand);
+    std::memcpy(tab.data() + o_sets, sets.data(), sizeof(int) * P);
+    std::memcpy(tab.data() + o_set, sd.data(), sizeof(DecodeSettingDev) * P);
+    CK(m->grid_tab.reserve(tab_bytes));
+    CK(cudaMemcpyAsync(m->grid_tab.p, tab.data(), tab_bytes, cudaMemcpyHostToDevice, st));
+    gd.prep = reinterpret_cast<const DecodePrepGroup*>(m->grid_tab.p);
+    gd.cand = reinterpret_cast<const DecodeCandGroup*>(m->grid_tab.p + o_cand);
+    gd.sets = reinterpret_cast<const int*>(m->grid_tab.p + o_sets);
+    gd.setting = reinterpret_cast<const DecodeSettingDev*>(m->grid_tab.p + o_set);
+
+    CK(m->energy.reserve((size_t)(P * cells) + 1));
+    CK(m->candbits.reserve((size_t)(n_cand * gd.cand_stride)));
+    CK(m->max_onset.reserve((size_t)n_prep * n_files));
+    CK(m->max_fd.reserve((size_t)n_prep * n_files));
+    CK(m->blk_max.reserve((size_t)(P * gd.blk_stride)));
+    CK(m->blk_arg.reserve((size_t)(P * gd.blk_stride)));
+    CK(m->note_count.reserve((size_t)n_pairs));
+    CK(m->d_slot_off.reserve((size_t)n_pairs + 1));
+    CK(m->overflow.reserve(1));
+    // ---- the loops, with today's two-attempt slot sizing per (setting, file): a pair that ran out of its first
+    // allowance gets 88 T slots, and the chunk runs again (the loops consume E)
+    std::vector<long long> soff(n_pairs + 1);
+    std::vector<char> full(n_pairs, 0);
+    std::vector<int> counts(n_pairs);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      soff[0] = 0;
+      for (long long q = 0; q < n_pairs; ++q) {
+        const long long T = foff[q % n_files + 1] - foff[q % n_files];
+        soff[q + 1] = soff[q] + (full[q] ? T * kPitches : std::min<long long>(T * kPitches, 8 * T + 64));
+      }
+      CK(m->slot_start.reserve((size_t)soff[n_pairs] + 1));
+      CK(m->slot_end.reserve((size_t)soff[n_pairs] + 1));
+      CK(m->slot_pitch.reserve((size_t)soff[n_pairs] + 1));
+      CK(cudaMemcpyAsync(m->d_slot_off.p, soff.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
+      DecodeBuffers b;
+      b.frame_off = m->d_frame_off.p;
+      b.energy = m->energy.p;
+      b.candbits = m->candbits.p;
+      b.max_onset = m->max_onset.p;
+      b.max_fd = m->max_fd.p;
+      b.slot_off = m->d_slot_off.p;
+      b.note_count = m->note_count.p;
+      b.note_start = m->slot_start.p;
+      b.note_end = m->slot_end.p;
+      b.note_pitch = m->slot_pitch.p;
+      b.overflow = m->overflow.p;
+      b.blk_max = m->blk_max.p;
+      b.blk_arg = m->blk_arg.p;
+      {
+        ProfScope ps(m, 5, st);
+        launch_decode_grid(d_note, d_onset, b, n_files, total_frames, gd, n_prep, n_cand, P, st);
+      }
+      CKL();
+      m->launches += total_frames > 0 ? 3 : 1;
+      CK(cudaMemcpyAsync(counts.data(), m->note_count.p, sizeof(int) * n_pairs, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      bool overflow = false;
+      for (long long q = 0; q < n_pairs; ++q)
+        if (counts[q] > soff[q + 1] - soff[q]) overflow = full[q] = 1;
+      if (!overflow) break;
+      if (attempt == 1) return fail(BP_E_CUDA, api + ": note slots overflowed at full capacity (internal error)");
+    }
+    const int rc = tail(p0, P, counts, soff);
+    if (rc) return rc;
+  }
+  return BP_OK;
+}
+
+// ---- scoring (bp_score_*) ----------------------------------------------------------------------------------------------
+
+int check_score_params(const std::string& api, const bp_score_params_t* sp) {
+  if (!sp) return fail(BP_E_INVALID, api + ": null score params");
+  const double v[4] = {sp->onset_tolerance, sp->pitch_tolerance, sp->offset_ratio, sp->offset_min_tolerance};
+  const char* name[4] = {"onset_tolerance", "pitch_tolerance", "offset_ratio", "offset_min_tolerance"};
+  for (int k = 0; k < 4; ++k)
+    if (!std::isfinite(v[k]) || v[k] < 0)
+      return fail(BP_E_INVALID, api + ": score params: " + name[k] + " must be finite and >= 0");
+  return BP_OK;
+}
+
+ScoreTol score_tol(const bp_score_params_t& sp) {
+  ScoreTol t{};
+  t.onset = sp.onset_tolerance;
+  t.pitch = sp.pitch_tolerance;
+  t.ratio = sp.offset_ratio;
+  t.off_min = sp.offset_min_tolerance;
+  // around(x, 4) <= tol needs x <= tol + 0.5e-4 (+ rounding); the kernel adds a margin relative to the onset
+  t.window = sp.onset_tolerance * (1 + 1e-12) + 1e-4;
+  t.k_buckets = (int)std::min(std::floor((sp.pitch_tolerance + 1e-6) / 100.0) + 1.0, 1073741824.0);
+  return t;
+}
+
+// Validates n sets of notes (`what` "references" / "estimates", set unit "file" / "item"): note_off[0] = 0 and
+// non-decreasing, at most 2^31 - 1 notes per set, every note with finite values, onset >= 0 and offset > onset.
+int check_note_set(const std::string& api, const char* what, const char* unit, const bp_note_set_t* s, int n) {
+  const std::string who = api + ": " + what;
+  if (!s || !s->note_off) return fail(BP_E_INVALID, who + ": null note set");
+  if (s->note_off[0] != 0) return fail(BP_E_INVALID, who + ": note_off[0] must be 0");
+  for (int i = 0; i < n; ++i)
+    if (s->note_off[i + 1] < s->note_off[i] || s->note_off[i + 1] - s->note_off[i] > INT_MAX)
+      return fail(BP_E_INVALID, who + " " + unit + " " + std::to_string(i) + ": bad note_off");
+  if (s->note_off[n] > 0 && (!s->onset_s || !s->offset_s || !s->log2_hz)) return fail(BP_E_INVALID, who + ": null array");
+  for (int i = 0; i < n; ++i)
+    for (long long j = s->note_off[i]; j < s->note_off[i + 1]; ++j) {
+      const double on = s->onset_s[j], off = s->offset_s[j], l2 = s->log2_hz[j];
+      const char* why = !std::isfinite(on) || !std::isfinite(off) ? "non-finite time"
+                        : !std::isfinite(l2)                      ? "non-finite log2_hz"
+                        : on < 0                                  ? "onset < 0"
+                        : off <= on                               ? "offset <= onset"
+                                                                  : nullptr;
+      if (why)
+        return fail(BP_E_INVALID, who + " " + unit + " " + std::to_string(i) + " note " +
+                                      std::to_string(j - s->note_off[i]) + ": " + why);
+    }
+  return BP_OK;
+}
+
+// 16-byte aligned sections of one host->device upload
+struct Pack {
+  std::vector<unsigned char> buf;
+  size_t add(const void* p, size_t bytes) {
+    const size_t at = (buf.size() + 15) / 16 * 16;
+    buf.resize(at + bytes);
+    if (bytes) std::memcpy(buf.data() + at, p, bytes);
+    return at;
+  }
+};
+
+// The references of n sets, sorted by (bucket, onset) within each set, into `pk`; offsets of the sections in `o[5]`
+// (note_off, onset, offset, log2_hz, bucket); the range of buckets into tol.
+void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol) {
+  const long long R = s->note_off[n];
+  std::vector<long long> idx(R);
+  std::vector<int> bucket(R), bsorted(R);
+  std::vector<double> on(R), off(R), l2(R);
+  tol.bucket_lo = 0, tol.bucket_hi = -1;
+  for (long long j = 0; j < R; ++j) {
+    idx[j] = j;
+    bucket[j] = score_bucket(s->log2_hz[j]);
+    if (j == 0 || bucket[j] < tol.bucket_lo) tol.bucket_lo = bucket[j];
+    if (j == 0 || bucket[j] > tol.bucket_hi) tol.bucket_hi = bucket[j];
+  }
+  for (int i = 0; i < n; ++i)
+    std::sort(idx.begin() + s->note_off[i], idx.begin() + s->note_off[i + 1], [&](long long a, long long b) {
+      if (bucket[a] != bucket[b]) return bucket[a] < bucket[b];
+      if (s->onset_s[a] != s->onset_s[b]) return s->onset_s[a] < s->onset_s[b];
+      return a < b;
+    });
+  for (long long j = 0; j < R; ++j) {
+    on[j] = s->onset_s[idx[j]];
+    off[j] = s->offset_s[idx[j]];
+    l2[j] = s->log2_hz[idx[j]];
+    bsorted[j] = bucket[idx[j]];
+  }
+  const std::vector<long long> noff(s->note_off, s->note_off + n + 1);
+  o[0] = pk.add(noff.data(), sizeof(long long) * (n + 1));
+  o[1] = pk.add(on.data(), sizeof(double) * R);
+  o[2] = pk.add(off.data(), sizeof(double) * R);
+  o[3] = pk.add(l2.data(), sizeof(double) * R);
+  o[4] = pk.add(bsorted.data(), sizeof(int) * R);
+}
+
+ScoreRefs refs_at(const unsigned char* d, const size_t* o) {
+  return ScoreRefs{reinterpret_cast<const long long*>(d + o[0]), reinterpret_cast<const double*>(d + o[1]),
+                   reinterpret_cast<const double*>(d + o[2]), reinterpret_cast<const double*>(d + o[3]),
+                   reinterpret_cast<const int*>(d + o[4])};
 }
 
 }  // namespace
@@ -1566,118 +1795,11 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
     return fail(BP_E_INVALID, api + ": null posteriorgram");
   DeviceGuard g(m->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const long long cells = total_frames * kPitches;
-  const long long chunk = bp_decode_grid_chunk_params(total_frames, n_files);
-  DecodeGridDev gd{};
-  gd.n_files = n_files;
-  gd.e_stride = cells;
-  gd.cand_stride = decode_cand_words(total_frames);
-  gd.blk_stride = (long long)kPitches * decode_block_slots(total_frames, n_files);
-  CK(m->d_frame_off.reserve(n_files + 1));
-  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
-
   long long n_notes = 0, n_bends = 0;  // over the grid so far
   bool notes_fit = true, bends_fit = true;
-  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
-    const int P = (int)std::min<long long>(chunk, n_params - p0);
-    const long long n_pairs = (long long)P * n_files;  // (setting, file), setting-major
-    // ---- groups: settings sharing a pitch range share the prep; those also sharing infer_onsets and onset_thresh
-    // share the candidates
-    std::vector<DecodeSettingDev> sd(P);
-    std::vector<DecodePrepGroup> prep;
-    std::vector<DecodeCandGroup> cand;
-    std::vector<int> prep_of(P);
-    for (int s = 0; s < P; ++s) {
-      sd[s].p = params_dev(params[p0 + s]);
-      const DecodeParamsDev& q = sd[s].p;
-      int pg = 0;
-      while (pg < (int)prep.size() && (prep[pg].lo != q.lo_col || prep[pg].hi != q.hi_col)) ++pg;
-      if (pg == (int)prep.size()) prep.push_back(DecodePrepGroup{q.lo_col, q.hi_col, 0, 0});
-      ++prep[pg].set_hi;  // count for now
-      prep_of[s] = pg;
-      int cg = 0;
-      while (cg < (int)cand.size() && (cand[cg].prep != pg || cand[cg].infer != q.infer_onsets ||
-                                       !(cand[cg].onset_thresh == q.onset_thresh)))
-        ++cg;
-      if (cg == (int)cand.size()) cand.push_back(DecodeCandGroup{q.onset_thresh, q.lo_col, q.hi_col, q.infer_onsets, pg});
-      sd[s].cand = cg;
-    }
-    const int n_prep = (int)prep.size(), n_cand = (int)cand.size();
-    for (int k = 0, at = 0; k < n_prep; ++k) {
-      const int n = prep[k].set_hi;
-      prep[k].set_lo = prep[k].set_hi = at;
-      at += n;
-    }
-    std::vector<int> sets(P);
-    for (int s = 0; s < P; ++s) sets[prep[prep_of[s]].set_hi++] = s;
-    // one upload of the tables, 16-byte aligned sections
-    auto sec = [](size_t bytes) { return (bytes + 15) / 16 * 16; };
-    const size_t o_cand = sec(sizeof(DecodePrepGroup) * n_prep), o_sets = o_cand + sec(sizeof(DecodeCandGroup) * n_cand),
-                 o_set = o_sets + sec(sizeof(int) * P), tab_bytes = o_set + sizeof(DecodeSettingDev) * P;
-    std::vector<unsigned char> tab(tab_bytes);
-    std::memcpy(tab.data(), prep.data(), sizeof(DecodePrepGroup) * n_prep);
-    std::memcpy(tab.data() + o_cand, cand.data(), sizeof(DecodeCandGroup) * n_cand);
-    std::memcpy(tab.data() + o_sets, sets.data(), sizeof(int) * P);
-    std::memcpy(tab.data() + o_set, sd.data(), sizeof(DecodeSettingDev) * P);
-    CK(m->grid_tab.reserve(tab_bytes));
-    CK(cudaMemcpyAsync(m->grid_tab.p, tab.data(), tab_bytes, cudaMemcpyHostToDevice, st));
-    gd.prep = reinterpret_cast<const DecodePrepGroup*>(m->grid_tab.p);
-    gd.cand = reinterpret_cast<const DecodeCandGroup*>(m->grid_tab.p + o_cand);
-    gd.sets = reinterpret_cast<const int*>(m->grid_tab.p + o_sets);
-    gd.setting = reinterpret_cast<const DecodeSettingDev*>(m->grid_tab.p + o_set);
-
-    CK(m->energy.reserve((size_t)(P * cells) + 1));
-    CK(m->candbits.reserve((size_t)(n_cand * gd.cand_stride)));
-    CK(m->max_onset.reserve((size_t)n_prep * n_files));
-    CK(m->max_fd.reserve((size_t)n_prep * n_files));
-    CK(m->blk_max.reserve((size_t)(P * gd.blk_stride)));
-    CK(m->blk_arg.reserve((size_t)(P * gd.blk_stride)));
-    CK(m->note_count.reserve((size_t)n_pairs));
-    CK(m->d_slot_off.reserve((size_t)n_pairs + 1));
-    CK(m->overflow.reserve(1));
-    // ---- the loops, with today's two-attempt slot sizing per (setting, file): a pair that ran out of its first
-    // allowance gets 88 T slots, and the chunk runs again (the loops consume E)
-    std::vector<long long> soff(n_pairs + 1);
-    std::vector<char> full(n_pairs, 0);
-    std::vector<int> counts(n_pairs);
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      soff[0] = 0;
-      for (long long q = 0; q < n_pairs; ++q) {
-        const long long T = foff[q % n_files + 1] - foff[q % n_files];
-        soff[q + 1] = soff[q] + (full[q] ? T * kPitches : std::min<long long>(T * kPitches, 8 * T + 64));
-      }
-      CK(m->slot_start.reserve((size_t)soff[n_pairs] + 1));
-      CK(m->slot_end.reserve((size_t)soff[n_pairs] + 1));
-      CK(m->slot_pitch.reserve((size_t)soff[n_pairs] + 1));
-      CK(cudaMemcpyAsync(m->d_slot_off.p, soff.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
-      DecodeBuffers b;
-      b.frame_off = m->d_frame_off.p;
-      b.energy = m->energy.p;
-      b.candbits = m->candbits.p;
-      b.max_onset = m->max_onset.p;
-      b.max_fd = m->max_fd.p;
-      b.slot_off = m->d_slot_off.p;
-      b.note_count = m->note_count.p;
-      b.note_start = m->slot_start.p;
-      b.note_end = m->slot_end.p;
-      b.note_pitch = m->slot_pitch.p;
-      b.overflow = m->overflow.p;
-      b.blk_max = m->blk_max.p;
-      b.blk_arg = m->blk_arg.p;
-      {
-        ProfScope ps(m, 5, st);
-        launch_decode_grid(d_note, d_onset, b, n_files, total_frames, gd, n_prep, n_cand, P, st);
-      }
-      CKL();
-      m->launches += total_frames > 0 ? 3 : 1;
-      CK(cudaMemcpyAsync(counts.data(), m->note_count.p, sizeof(int) * n_pairs, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      bool overflow = false;
-      for (long long q = 0; q < n_pairs; ++q)
-        if (counts[q] > soff[q + 1] - soff[q]) overflow = full[q] = 1;
-      if (!overflow) break;
-      if (attempt == 1) return fail(BP_E_CUDA, api + ": note slots overflowed at full capacity (internal error)");
-    }
+  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>& counts, const std::vector<long long>&) -> int {
+    const long long n_pairs = (long long)P * n_files;
     // ---- note offsets; past the note capacity only the counting goes on (bp_last_required totals the whole grid)
     const long long note0 = n_notes;
     for (long long q = 0; q < n_pairs; ++q) {
@@ -1686,7 +1808,7 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
       if (notes_fit) notes->note_off[p0 * n_files + q + 1] = (int32_t)n_notes;
     }
     const long long nc = n_notes - note0;  // notes of this chunk
-    if (!notes_fit || nc == 0) continue;
+    if (!notes_fit || nc == 0) return BP_OK;
     if (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude)
       return fail(BP_E_INVALID, api + ": notes arrays missing");
     std::vector<int> noff(n_pairs + 1);  // chunk-relative
@@ -1719,7 +1841,7 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
       }
     }
     if (n_bends > notes->bend_capacity) bends_fit = false;
-    if (!bends_fit) continue;
+    if (!bends_fit) return BP_OK;
     const long long bc = n_bends - bend0;  // bends of this chunk
     if (bc > 0 && !notes->bends) return fail(BP_E_INVALID, api + ": bends array missing");
     std::vector<int> boff(nc + 1);
@@ -1736,7 +1858,9 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
     CK(cudaMemcpyAsync(notes->amplitude + note0, m->d_amp.p, sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
     if (bc > 0) CK(cudaMemcpyAsync(notes->bends + bend0, m->d_bends.p, sizeof(int) * bc, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-  }
+    return BP_OK;
+  });
+  if (rc) return rc;
   if (!notes_fit)
     return g_need_notes = n_notes, fail(BP_E_CAPACITY, api + ": note_capacity too small, need " + std::to_string(n_notes));
   if (!bends_fit)
@@ -1766,6 +1890,168 @@ int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset
   }
   return bp_decode_grid_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, n_params,
                                notes, st);
+}
+
+void bp_default_score_params(bp_score_params_t* p) {
+  if (!p) return;
+  p->onset_tolerance = 0.05;
+  p->pitch_tolerance = 50.0;
+  p->offset_ratio = 0.2;
+  p->offset_min_tolerance = 0.05;
+}
+
+int bp_frame_times(int64_t n, double* out) {
+  if (n < 0 || (n > 0 && !out)) return fail(BP_E_INVALID, "bp_frame_times: bad argument");
+  // model_frames_to_time: (FFT_HOP / SR) * (ANNOT_N_FRAMES - AUDIO_N_SAMPLES / FFT_HOP) + MAGIC_ALIGNMENT_OFFSET, then
+  // frame * FFT_HOP / SR - offset * floor(frame / ANNOT_N_FRAMES); every product rounded on its own (volatile: never
+  // contracted into a multiply-add)
+  volatile double hop_s = 256.0 / 22050.0, frac = 172.0 - 43844.0 / 256.0;
+  volatile double prod = hop_s * frac;
+  const double window_offset = prod + 0.0018;
+  for (int64_t i = 0; i < n; ++i) {
+    volatile double shift = window_offset * std::floor((double)i / 172.0);
+    out[i] = (double)(i * 256) / 22050.0 - shift;
+  }
+  return BP_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Everything bp_score_grid_* check before anything is enqueued, in addition to check_grid_args.
+int check_score_grid(const std::string& api, int n_files, int n_params, const bp_note_set_t* refs,
+                     const bp_score_params_t* sp, const double* est_log2_hz, const int64_t* h_counts) {
+  int rc = check_score_params(api, sp);
+  if (rc || n_files == 0 || n_params == 0) return rc;
+  if (!h_counts || !est_log2_hz) return fail(BP_E_INVALID, api + ": bad argument");
+  for (int k = 0; k < 128; ++k)
+    if (!std::isfinite(est_log2_hz[k]))
+      return fail(BP_E_INVALID, api + ": estimate table entry " + std::to_string(k) + ": non-finite log2_hz");
+  return check_note_set(api, "references", "file", refs, n_files);
+}
+
+}  // namespace
+
+extern "C" {
+
+int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts, void* stream) {
+  const std::string api = "bp_score_grid_device";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long total_frames = foff[n_files];
+  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  long long max_t = 0;
+  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
+  // one upload per call: the references, the seconds of every frame a note can start or end on, the log2(Hz) table
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[5];
+  pack_refs(refs, n_files, pk, o_ref, tol);
+  std::vector<double> frame_t(max_t + 1);
+  bp_frame_times(max_t + 1, frame_t.data());
+  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
+  const size_t o_l2 = pk.add(est_log2_hz, sizeof(double) * 128);
+  const long long n_refs = refs->note_off[n_files];
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(m->score_counts.reserve((size_t)n_params * n_files * 4));
+  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
+  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>&, const std::vector<long long>& soff) -> int {
+    const long long n_pairs = (long long)P * n_files;
+    CK(m->score_ws_ref.reserve((size_t)(2 * P * n_refs) + 1));
+    CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs]) + 1));
+    ScoreEst e{};
+    e.off = m->d_slot_off.p;
+    e.count = m->note_count.p;
+    e.start = m->slot_start.p;
+    e.end = m->slot_end.p;
+    e.pitch = m->slot_pitch.p;
+    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
+    e.log2_midi = reinterpret_cast<const double*>(m->score_in.p + o_l2);
+    launch_score_match(sr, e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_files, n_pairs,
+                       m->score_counts.p + 4 * p0 * n_files, st);
+    CKL();
+    m->launches += 1;
+    return BP_OK;
+  });
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_params * n_files, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_score_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                       int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                       const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts) {
+  const std::string api = "bp_score_grid_host";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  DeviceGuard g(m->device);
+  const int64_t total = h_frame_off[n_files];
+  cudaStream_t st = m->stream;
+  rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {  // uploaded once for the whole grid
+    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
+    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+  }
+  return bp_score_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, sp,
+                              est_log2_hz, h_counts, st);
+}
+
+int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
+                        const bp_score_params_t* sp, int64_t* h_counts) {
+  const std::string api = "bp_score_notes_host";
+  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  int rc = check_score_params(api, sp);
+  if (rc || n_items == 0) return rc;
+  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_note_set(api, "estimates", "item", est, n_items);
+  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items);
+  if (rc) return rc;
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[5];
+  pack_refs(refs, n_items, pk, o_ref, tol);
+  const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
+  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
+  const size_t o_eon = pk.add(est->onset_s, sizeof(double) * n_est);
+  const size_t o_eoffs = pk.add(est->offset_s, sizeof(double) * n_est);
+  const size_t o_el2 = pk.add(est->log2_hz, sizeof(double) * n_est);
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(m->score_ws_ref.reserve((size_t)(2 * n_refs) + 1));
+  CK(m->score_ws_est.reserve((size_t)(4 * n_est) + 1));
+  CK(m->score_counts.reserve((size_t)n_items * 4));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = m->score_in.p;
+  ScoreEst e{};
+  e.off = reinterpret_cast<const long long*>(d + o_eoff);
+  e.onset = reinterpret_cast<const double*>(d + o_eon);
+  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
+  e.log2hz = reinterpret_cast<const double*>(d + o_el2);
+  launch_score_match(refs_at(d, o_ref), e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_items,
+                     n_items, m->score_counts.p, st);
+  CKL();
+  m->launches += 1;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_items, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,

@@ -267,6 +267,43 @@ void launch_note_finish(const float* note, const float* contour, const long long
                         int* bends, int n_notes, int with_bends, const double* gauss /*[51] device*/,
                         cudaStream_t st);
 
+// ---- score.cu: note-level match counts (bp_score_*) ----------------------------------------------------------------
+// Nearest semitone (MIDI number) of a pitch given as log2(Hz), clamped to +-1e9 so that bucket differences fit an int.
+// The host buckets the references with it and the kernel the estimates; a hit lies within floor(cents / 100) + 1
+// buckets whichever side of a .5 either note rounds to.
+__host__ __device__ inline int score_bucket(double log2_hz) {
+  const double m = rint(12.0 * (log2_hz - 8.78135971352466) + 69.0);  // log2(440)
+  return (int)fmin(fmax(m, -1e9), 1e9);
+}
+struct ScoreRefs {  // file i's references are [off[i], off[i+1]), sorted by (bucket, onset)
+  const long long* off;
+  const double* onset;
+  const double* offset;
+  const double* log2hz;
+  const int* bucket;
+};
+struct ScoreEst {  // pair q's estimated notes start at off[q]: count[q] decode slots, or off[q+1] - off[q] explicit notes
+  const long long* off;
+  const int* count;                                   // NULL: explicit notes
+  const double *onset, *offset, *log2hz;              // explicit notes (NULL: decode slots)
+  const int *start, *end, *pitch;                     // decode slots: file-relative frames, MIDI number
+  const double *frame_t, *log2_midi;                  // seconds per frame (bp_frame_times), log2(Hz) per MIDI number
+};
+struct ScoreTol {
+  double onset, pitch, ratio, off_min;
+  double window;          // onset half-width of the candidate search beyond the tolerance (rounding margin)
+  int k_buckets;          // floor(pitch / 100) + 1 (with a rounding margin)
+  int bucket_lo, bucket_hi;  // range of the references' buckets: the scan never leaves it
+};
+struct ScoreWork {       // int workspace: 2 per reference and setting, 4 per estimated note
+  int* ref;              // setting s, file f: ref + 2 (s * n_ref_total + off[f])
+  int* est;              // pair q: est + 4 * ScoreEst.off[q]
+  long long n_ref_total;
+};
+// One launch: counts[4 q ..] = {n_ref, n_est, matched without offsets, matched} of pair q = setting * n_files + file.
+void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
+                        long long n_pairs, long long* counts, cudaStream_t st);
+
 // ---- sonify.cu: bp_sonify_notes_host on the given stream of the current device (h_audio == NULL: size query, no CUDA
 // call); adds its kernel launches to *launches ---------------------------------------------------------------------------
 int sonify_notes(cudaStream_t st, long long* launches, int32_t n_files, const int32_t* note_off, const double* start_s,

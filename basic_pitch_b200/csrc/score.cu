@@ -1,0 +1,193 @@
+// Note-level transcription scores on the device: the counts behind mir_eval.transcription (0.7) match_notes +
+// precision_recall_f1_overlap, with and without offsets, for a grid of (setting, file) pairs or a list of items.
+//
+// One thread per pair.  A pair's reference notes are sorted by (nearest semitone, onset) on the host; its estimated notes
+// come either from the grid decode's note slots (frames and MIDI numbers, turned into seconds and log2(Hz) through two
+// tables the host built) or from explicit arrays.  The hit graph is never stored: an estimated note's neighbours are
+// found by scanning the semitone buckets within reach of the pitch tolerance and binary-searching the onset window, and
+// the exact predicates decide.  The maximum matching is a greedy pass followed by one augmenting-path search (Kuhn) per
+// estimated note the greedy pass left free, with an explicit stack in global workspace.
+#include <cuda_runtime.h>
+
+#include <cmath>
+
+#include "kernels.cuh"
+
+namespace bp {
+
+namespace {
+
+constexpr int kScoreThreads = 128;
+
+// np.around(x, 4): multiply, round half to even, divide
+__device__ __forceinline__ double around4(double x) { return __ddiv_rn(rint(__dmul_rn(x, 10000.0)), 10000.0); }
+
+struct EstNote {
+  double on, off, l2;
+  int bucket;
+};
+
+struct PairCtx {
+  // references of the pair's file: [0, n_ref) relative to r0
+  const double* r_on;
+  const double* r_off;
+  const double* r_l2;
+  const int* r_bucket;
+  int n_ref;
+  ScoreTol tol;
+};
+
+__device__ __forceinline__ EstNote est_note(const ScoreEst& e, long long base, int j) {
+  EstNote n;
+  if (e.onset) {
+    n.on = e.onset[base + j];
+    n.off = e.offset[base + j];
+    n.l2 = e.log2hz[base + j];
+  } else {
+    n.on = e.frame_t[e.start[base + j]];
+    n.off = e.frame_t[e.end[base + j]];
+    n.l2 = e.log2_midi[e.pitch[base + j]];
+  }
+  n.bucket = score_bucket(n.l2);
+  return n;
+}
+
+__device__ __forceinline__ bool hit(const PairCtx& c, const EstNote& e, int i, bool with_offset) {
+  const double r_on = c.r_on[i];
+  if (!(around4(fabs(__dsub_rn(r_on, e.on))) <= c.tol.onset)) return false;
+  if (!(fabs(__dmul_rn(1200.0, __dsub_rn(c.r_l2[i], e.l2))) <= c.tol.pitch)) return false;
+  if (!with_offset) return true;
+  const double r_off = c.r_off[i];
+  const double lim = fmax(__dmul_rn(c.tol.ratio, fabs(__dsub_rn(r_off, r_on))), c.tol.off_min);
+  return around4(fabs(__dsub_rn(r_off, e.off))) <= lim;
+}
+
+// first reference at or after (bucket b, onset lo) in (bucket, onset) order
+__device__ __forceinline__ int lower_bound(const PairCtx& c, int b, double lo) {
+  int a = 0, n = c.n_ref;
+  while (n > 0) {
+    const int h = n >> 1, m = a + h;
+    const int bm = c.r_bucket[m];
+    if (bm < b || (bm == b && c.r_on[m] < lo)) {
+      a = m + 1;
+      n -= h + 1;
+    } else {
+      n = h;
+    }
+  }
+  return a;
+}
+
+// Advances the cursor (db, pos) of estimated note e to its next hit: buckets e.bucket - K .. e.bucket + K, within each
+// the references whose onset lies in [e.on - w, e.on + w] (w = onset tolerance + margin).  pos < 0: start of bucket db.
+__device__ __forceinline__ bool next_hit(const PairCtx& c, const EstNote& e, int& db, int& pos, bool with_offset) {
+  const double w = c.tol.window + fabs(e.on) * 1e-12;
+  const double lo = e.on - w, hi = e.on + w;
+  const int db_hi = min(c.tol.k_buckets, c.tol.bucket_hi - e.bucket);
+  if (pos < 0) db = max(db, c.tol.bucket_lo - e.bucket);
+  while (db <= db_hi) {
+    const int b = e.bucket + db;
+    pos = pos < 0 ? lower_bound(c, b, lo) : pos + 1;
+    if (pos < c.n_ref && c.r_bucket[pos] == b && c.r_on[pos] <= hi) {
+      if (hit(c, e, pos, with_offset)) return true;
+      continue;
+    }
+    ++db;
+    pos = -1;
+  }
+  return false;
+}
+
+// Size of a maximum matching of the hit graph.  match_ref / visit: [n_ref]; match_est: [n_est]; stack: [3 n_est].
+__device__ __forceinline__ int max_matching(const PairCtx& c, const ScoreEst& e, long long ebase, int n_est,
+                                            bool with_offset, int* match_ref, int* visit, int* match_est, int* stack) {
+  const int K = c.tol.k_buckets;
+  for (int i = 0; i < c.n_ref; ++i) match_ref[i] = visit[i] = -1;
+  int matched = 0;
+  for (int j = 0; j < n_est; ++j) {  // greedy: the first free hit
+    match_est[j] = -1;
+    const EstNote en = est_note(e, ebase, j);
+    int db = -K, pos = -1;
+    while (next_hit(c, en, db, pos, with_offset))
+      if (match_ref[pos] < 0) {
+        match_ref[pos] = j;
+        match_est[j] = pos;
+        ++matched;
+        break;
+      }
+  }
+  if (matched == c.n_ref) return matched;
+  // augmenting paths from every estimated note still free; a note without one now never gets one later (Kuhn)
+  for (int j = 0; j < n_est; ++j) {
+    if (match_est[j] >= 0) continue;
+    int depth = 1;
+    stack[0] = j, stack[1] = -K, stack[2] = -1;  // frame: estimated note, bucket cursor, reference cursor
+    while (depth > 0) {
+      int* f = stack + 3 * (depth - 1);
+      const EstNote en = est_note(e, ebase, f[0]);
+      int db = f[1], r = f[2];
+      const bool more = next_hit(c, en, db, r, with_offset);
+      f[1] = db, f[2] = r;
+      if (!more) {
+        --depth;
+        continue;
+      }
+      if (visit[r] == j) continue;
+      visit[r] = j;
+      if (match_ref[r] < 0) {  // flip the path: each frame's note takes the reference its cursor stands on
+        for (int k = 0; k < depth; ++k) {
+          const int jj = stack[3 * k], rr = stack[3 * k + 2];
+          match_est[jj] = rr;
+          match_ref[rr] = jj;
+        }
+        ++matched;
+        break;
+      }
+      int* g = stack + 3 * depth++;
+      g[0] = match_ref[r], g[1] = -K, g[2] = -1;
+    }
+    if (matched == c.n_ref) break;
+  }
+  return matched;
+}
+
+// Pair q = setting * n_files + file (chunk-local).  counts[q] = {n_ref, n_est, matched without offsets, matched}.
+__global__ void __launch_bounds__(kScoreThreads) score_match_kernel(ScoreRefs R, ScoreEst E, ScoreTol tol,
+                                                                    ScoreWork W, int n_files, long long n_pairs,
+                                                                    long long* __restrict__ counts) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n_pairs) return;
+  const int file = (int)(q % n_files);
+  const long long s = q / n_files;
+  const long long r0 = R.off[file];
+  PairCtx c;
+  c.r_on = R.onset + r0;
+  c.r_off = R.offset + r0;
+  c.r_l2 = R.log2hz + r0;
+  c.r_bucket = R.bucket + r0;
+  c.n_ref = (int)(R.off[file + 1] - r0);
+  c.tol = tol;
+  const long long ebase = E.off[q];
+  const int n_est = E.count ? E.count[q] : (int)(E.off[q + 1] - ebase);
+  int* rw = W.ref + 2 * (s * W.n_ref_total + r0);
+  int* ew = W.est + 4 * ebase;
+  long long* out = counts + 4 * q;
+  out[0] = c.n_ref;
+  out[1] = n_est;
+  if (c.n_ref == 0 || n_est == 0) {
+    out[2] = out[3] = 0;
+    return;
+  }
+  for (int pass = 0; pass < 2; ++pass)  // hits without, then with the offset test
+    out[2 + pass] = max_matching(c, E, ebase, n_est, pass == 1, rw, rw + c.n_ref, ew, ew + n_est);
+}
+
+}  // namespace
+
+void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
+                        long long n_pairs, long long* counts, cudaStream_t st) {
+  const unsigned int blocks = (unsigned int)((n_pairs + kScoreThreads - 1) / kScoreThreads);
+  score_match_kernel<<<blocks, kScoreThreads, 0, st>>>(R, E, tol, W, n_files, n_pairs, counts);
+}
+
+}  // namespace bp

@@ -20,7 +20,7 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from . import ICASSP_2022_MODEL_PATH, _lib, weights
+from . import ICASSP_2022_MODEL_PATH, _lib, evaluate, weights
 from . import note_creation as infer
 from .audio_io import load_audio, load_audio_device, pcm_descriptors, read_pcm
 from .constants import (
@@ -46,6 +46,12 @@ _F32 = np.float32
 
 def _ptr(a: Optional[np.ndarray]) -> Optional[int]:
     return None if a is None else a.ctypes.data
+
+
+def _cat_rows(xs: List[np.ndarray], w: int) -> np.ndarray:
+    """Per-file (T, w) arrays -> one C-contiguous float32 (sum T, w) array."""
+    cat = np.concatenate([np.asarray(x, _F32).reshape(-1, w) for x in xs]) if xs else np.zeros((0, w), _F32)
+    return np.ascontiguousarray(cat, dtype=_F32)
 
 
 class _PinnedBlock:
@@ -287,24 +293,28 @@ class Model:
         return self._split_notes(arrs, n_files)
 
     @staticmethod
-    def _cat_posteriorgrams(notes, onsets, contours, need_contours: bool):
-        """Per-file posteriorgrams -> (frame offsets, note, onset, contour) back to back, as the decode entry points
-        take them."""
+    def _cat_note_onset(notes, onsets):
+        """Per-file note / onset posteriorgrams -> (frame offsets, note, onset) back to back."""
         n_files = len(notes)
         foff = np.zeros(n_files + 1, np.int64)
         for i, a in enumerate(notes):
             if a.shape[1:] != (N_FREQ_BINS_NOTES,) or onsets[i].shape != a.shape:
                 raise ValueError("note/onset posteriorgrams must be (T, 88) and of equal shape")
             foff[i + 1] = foff[i] + a.shape[0]
+        return foff, _cat_rows(list(notes), N_FREQ_BINS_NOTES), _cat_rows(list(onsets), N_FREQ_BINS_NOTES)
+
+    @staticmethod
+    def _cat_posteriorgrams(notes, onsets, contours, need_contours: bool):
+        """Per-file posteriorgrams -> (frame offsets, note, onset, contour) back to back, as the decode entry points
+        take them."""
+        foff, n_all, o_all = Model._cat_note_onset(notes, onsets)
         total = int(foff[-1])
-        cat = lambda xs, w: np.ascontiguousarray(np.concatenate([np.asarray(x, _F32).reshape(-1, w) for x in xs]) if xs else np.zeros((0, w), _F32), dtype=_F32)  # noqa: E731
-        n_all, o_all = cat(list(notes), N_FREQ_BINS_NOTES), cat(list(onsets), N_FREQ_BINS_NOTES)
         if contours is None:
             if need_contours:
                 raise ValueError("pitch bends need the contour posteriorgram")
             c_all = np.zeros((max(total, 1), N_FREQ_BINS_CONTOURS), _F32)
         else:
-            c_all = cat(list(contours), N_FREQ_BINS_CONTOURS)
+            c_all = _cat_rows(list(contours), N_FREQ_BINS_CONTOURS)
             if c_all.shape[0] != total:
                 raise ValueError("contour posteriorgrams must have as many frames as note posteriorgrams")
         return foff, n_all, o_all, c_all
@@ -322,12 +332,7 @@ class Model:
         gives for that setting; with split_notes=False the concatenated arrays of the call instead (note_off has
         len(settings) * n_files + 1 entries, setting-major)."""
         n_files, n_params = len(notes), len(settings)
-        ps = (_lib.DecodeParams * max(n_params, 1))()
-        for k, s in enumerate(settings):
-            unknown = set(s) - set(self._DECODE_DEFAULTS)
-            if unknown:
-                raise TypeError(f"settings[{k}]: unknown decode argument(s) {sorted(unknown)}")
-            ps[k] = self._params(**{**self._DECODE_DEFAULTS, **s})
+        ps = self._grid_params(settings)
         need_contours = any(bool(p.include_pitch_bends) for p in ps[:n_params])
         foff, n_all, o_all, c_all = self._cat_posteriorgrams(notes, onsets, contours, need_contours)
         arrs = self._with_capacity(
@@ -340,6 +345,79 @@ class Model:
             return arrs
         flat = self._split_notes(arrs, n_params * n_files)
         return [flat[k * n_files : (k + 1) * n_files] for k in range(n_params)]
+
+    def _grid_params(self, settings: Sequence[Dict[str, Any]]):
+        ps = (_lib.DecodeParams * max(len(settings), 1))()
+        for k, s in enumerate(settings):
+            unknown = set(s) - set(self._DECODE_DEFAULTS)
+            if unknown:
+                raise TypeError(f"settings[{k}]: unknown decode argument(s) {sorted(unknown)}")
+            ps[k] = self._params(**{**self._DECODE_DEFAULTS, **s})
+        return ps
+
+    # ------------------------------------------------------------------ note-level scores
+    @staticmethod
+    def _score_params(tolerances: Dict[str, float]) -> _lib.ScoreParams:
+        unknown = set(tolerances) - set(evaluate.TOLERANCES)
+        if unknown:
+            raise TypeError(f"unknown tolerance(s) {sorted(unknown)}")
+        return _lib.ScoreParams(**{k: float(v) for k, v in {**evaluate.TOLERANCES, **tolerances}.items()})
+
+    @staticmethod
+    def _note_set(sets: Sequence[Tuple[np.ndarray, np.ndarray]], what: str):
+        """[(intervals (n, 2) in seconds, pitches (n,) in Hz)] -> (bp_note_set_t, the arrays it points at); log2 of the
+        pitches as np.log2 takes it (a pitch <= 0 gives a non-finite log2, which the library rejects)."""
+        off = np.zeros(len(sets) + 1, np.int64)
+        ivs, hzs = [], []
+        for i, (iv, hz) in enumerate(sets):
+            iv, hz = np.asarray(iv, np.float64), np.asarray(hz, np.float64).reshape(-1)
+            if iv.size == 0:
+                iv = iv.reshape(0, 2)
+            if iv.ndim != 2 or iv.shape[1] != 2 or len(hz) != len(iv):
+                raise ValueError(f"{what}[{i}]: need intervals (n, 2) and pitches (n,), got {iv.shape} and {hz.shape}")
+            off[i + 1] = off[i] + len(iv)
+            ivs.append(iv)
+            hzs.append(hz)
+        iv = np.concatenate(ivs) if ivs else np.zeros((0, 2))
+        with np.errstate(divide="ignore", invalid="ignore"):
+            l2 = np.log2(np.concatenate(hzs) if hzs else np.zeros(0))
+        arrs = (off, np.ascontiguousarray(iv[:, 0]), np.ascontiguousarray(iv[:, 1]), l2)
+        ns = _lib.NoteSet()
+        ns.note_off, ns.onset_s, ns.offset_s, ns.log2_hz = (_ptr(a) for a in arrs)
+        return ns, arrs
+
+    def score_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray], settings: Sequence[Dict[str, Any]],
+                   references: Sequence[Tuple[np.ndarray, np.ndarray]], **tolerances) -> np.ndarray:
+        """Note-level match counts of a batch of files decoded under every setting of a grid, scored against one
+        reference set per file, in ONE library call (`bp_score_grid_host`): the notes never leave the device.
+        A setting is a dict of `decode_arrays`' keyword arguments (include_pitch_bends is ignored); a reference set is
+        (intervals (n, 2) in seconds, pitches (n,) in Hz), mir_eval's convention; tolerances are those of
+        `evaluate.TOLERANCES`.  Returns int64 counts (n_settings, n_files, 4): n_ref, n_est, matched without offsets,
+        matched (`evaluate.note_scores` turns them into precision, recall and F)."""
+        n_files, n_params = len(notes), len(settings)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference sets")
+        ps = self._grid_params(settings)
+        sp = self._score_params(tolerances)
+        refs, keep = self._note_set(references, "references")
+        foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+        counts = np.zeros((n_params, n_files, 4), np.int64)
+        self._lib.bp_score_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params, C.byref(refs),
+                                     C.byref(sp), _ptr(evaluate.EST_LOG2_HZ), _ptr(counts))
+        return counts
+
+    def score_notes(self, estimates: Sequence[Tuple[np.ndarray, np.ndarray]],
+                    references: Sequence[Tuple[np.ndarray, np.ndarray]], **tolerances) -> np.ndarray:
+        """Item i's estimated notes against item i's reference notes (`bp_score_notes_host`, one kernel launch), both
+        as (intervals (n, 2) in seconds, pitches (n,) in Hz).  Returns int64 counts (n_items, 4) as `score_grid`."""
+        if len(estimates) != len(references):
+            raise ValueError(f"{len(estimates)} estimated but {len(references)} reference sets")
+        sp = self._score_params(tolerances)
+        est, keep_e = self._note_set(estimates, "estimates")
+        refs, keep_r = self._note_set(references, "references")
+        counts = np.zeros((len(estimates), 4), np.int64)
+        self._lib.bp_score_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(counts))
+        return counts
 
     def infer_onsets_array(self, onsets: np.ndarray, frames: np.ndarray) -> np.ndarray:
         """reference: note_creation.py:289-311 `get_infered_onsets` (n_diff = 2) -> float64 (T, 88), on the device."""
@@ -709,6 +787,36 @@ def predict_grid(
                              [d for d, _ in conv], split_notes=False)
     events = infer.note_events_batch(arrs, len(conv), include_pitch_bends=True, lazy=True)
     return model_output, [(infer.LazyPrettyMIDI(ev, **midi_kw), ev) for (_, midi_kw), ev in zip(conv, events)]
+
+
+def evaluate_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, np.ndarray]],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    **tolerances,
+):
+    """Note-level scores of a batch of annotated recordings under every setting of a grid (addition; no reference
+    counterpart): the model runs once over the batch, and every (setting, file) is decoded and scored against its
+    file's reference notes on the device in one `bp_score_grid_host` call.  `audio` items are paths (decoded on the host,
+    converted and resampled on the GPU, as in `predict`) or mono 22 050 Hz arrays; `references[i]` is file i's
+    (intervals (n, 2) in seconds, pitches (n,) in Hz); a setting is a dict of `predict`'s keyword arguments (as in
+    `predict_grid`); tolerances as `evaluate.TOLERANCES`.
+
+    Returns (counts (n_settings, n_files, 4), `evaluate.note_scores(counts)`)."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    outs = model.run_inference_arrays(clips)
+    counts = model.score_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references, **tolerances)
+    return counts, evaluate.note_scores(counts)
 
 
 def predict_batch(

@@ -169,6 +169,60 @@ int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset
  * allowance of note slots reruns its chunk with 88 T slots for that pair, beyond this budget. */
 int64_t bp_decode_grid_chunk_params(int64_t total_frames, int32_t n_files);
 
+/* ---- note-level scores of decoded notes against reference notes ------------------------------------------------------
+ * No reference counterpart: the counts behind mir_eval.transcription 0.7 (match_notes + precision_recall_f1_overlap)
+ * with strict=False, with and without offsets.  A reference note i and an estimated note j of the same file match when,
+ * in float64 and in this order of operations,
+ *   onset:  rint(|on_i - on_j| * 10000) / 10000 <= onset_tolerance            (np.around(., 4), round half to even)
+ *   pitch:  |1200 * (log2_hz_i - log2_hz_j)| <= pitch_tolerance               (cents)
+ *   offset: rint(|off_i - off_j| * 10000) / 10000 <= max(offset_ratio * |off_i - on_i|, offset_min_tolerance)
+ * (the offset test in the "with offsets" pass only).  The matched count of a pass is the size of a maximum matching of
+ * that hit graph.  Per (setting, file) or item the result is four counts: {n_ref, n_est, matched without offsets,
+ * matched}; precision, recall and F follow from them (basic_pitch_b200/evaluate.py).
+ * Notes of set i are [note_off[i], note_off[i+1]); note_off[0] must be 0.  Every note needs finite values, onset >= 0
+ * and offset > onset; every tolerance must be finite and >= 0.  Violations return BP_E_INVALID before anything is
+ * enqueued, naming the file or item and the note index ("references file 3 note 17: offset <= onset"). */
+typedef struct bp_note_set {
+  const int64_t* note_off;  /* [n + 1] */
+  const double* onset_s;
+  const double* offset_s;
+  const double* log2_hz;    /* np.log2 of the pitch in Hz */
+} bp_note_set_t;
+
+typedef struct bp_score_params {
+  double onset_tolerance;      /* seconds, default 0.05 */
+  double pitch_tolerance;      /* cents, default 50 */
+  double offset_ratio;         /* default 0.2 */
+  double offset_min_tolerance; /* seconds, default 0.05 */
+} bp_score_params_t;
+void bp_default_score_params(bp_score_params_t* p);
+
+/* Host-only: the seconds of frames 0 .. n-1, the bits model_frames_to_time gives (basic_pitch_b200/note_creation.py;
+ * reference: note_creation.py:346-357). */
+int bp_frame_times(int64_t n, double* out);
+
+/* Grid scoring: bp_decode_grid_* without the contour, and instead of returning the notes, each (setting, file)'s notes
+ * are scored on the device against file i's references (refs: one set per file, uploaded once per call).  An estimated
+ * note (start_frame, end_frame, pitch_midi) has onset / offset bp_frame_times of its frames and log2_hz
+ * est_log2_hz[pitch_midi] (a 128-entry host table, finite).  Amplitudes and pitch bends are not computed
+ * (include_pitch_bends is ignored) and no note crosses to the host.  h_counts [n_params][n_files][4] (host).
+ * Settings are validated, grouped and chunked as in bp_decode_grid_*.  Kernel launches per chunk: those of the grid
+ * decode (3, or 1 when every file is empty; again as many when a pair outgrows its first allowance of note slots and
+ * the chunk reruns) + 1 match kernel, whatever the number of settings in the chunk.  Device workspace beyond the
+ * decode's: 8 bytes per reference and setting of a chunk, 16 bytes per note slot.
+ * _device: posteriorgrams in device memory, work on `stream`, synchronised before returning; _host: host
+ * posteriorgrams, uploaded once. */
+int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* score, const double* est_log2_hz, int64_t* h_counts, void* stream);
+int bp_score_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                       int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                       const bp_score_params_t* score, const double* est_log2_hz, int64_t* h_counts);
+/* Item i's estimated notes (est, explicit) scored against item i's references; h_counts [n_items][4].  One kernel
+ * launch (none for n_items == 0), synchronous. */
+int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
+                        const bp_score_params_t* score, int64_t* h_counts);
+
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
