@@ -2054,6 +2054,273 @@ int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
   return BP_OK;
 }
 
+}  // extern "C"
+
+// ---- frame-level scoring (bp_score_frames_grid_*, bp_score_multipitch_host, bp_multipitch_map) ---------------------
+namespace {
+
+// Validates n multi-pitch series (`what` "references" / "estimates", set unit "file" / "item"): offsets start at 0 and
+// never decrease, at most 2^31 - 1 frames per set and values per frame, times finite, >= 0 and non-decreasing within a
+// set, midi finite, chroma in [0, 12).
+int check_mp_set(const std::string& api, const char* what, const char* unit, const bp_multipitch_set_t* s, int n) {
+  const std::string who = api + ": " + what;
+  if (!s || !s->frame_off) return fail(BP_E_INVALID, who + ": null multipitch set");
+  if (s->frame_off[0] != 0) return fail(BP_E_INVALID, who + ": frame_off[0] must be 0");
+  for (int i = 0; i < n; ++i)
+    if (s->frame_off[i + 1] < s->frame_off[i] || s->frame_off[i + 1] - s->frame_off[i] > INT_MAX)
+      return fail(BP_E_INVALID, who + " " + unit + " " + std::to_string(i) + ": bad frame_off");
+  const long long F = s->frame_off[n];
+  if (F == 0) return BP_OK;
+  if (!s->time_s || !s->value_off) return fail(BP_E_INVALID, who + ": null array");
+  if (s->value_off[0] != 0) return fail(BP_E_INVALID, who + ": value_off[0] must be 0");
+  for (long long j = 0; j < F; ++j)
+    if (s->value_off[j + 1] < s->value_off[j] || s->value_off[j + 1] - s->value_off[j] > INT_MAX) {
+      const long long i = std::upper_bound(s->frame_off, s->frame_off + n + 1, j) - s->frame_off - 1;
+      return fail(BP_E_INVALID, who + " " + unit + " " + std::to_string(i) + " frame " +
+                                    std::to_string(j - s->frame_off[i]) + ": bad value_off");
+    }
+  if (s->value_off[F] > 0 && (!s->midi || !s->chroma)) return fail(BP_E_INVALID, who + ": null array");
+  for (int i = 0; i < n; ++i)
+    for (long long j = s->frame_off[i]; j < s->frame_off[i + 1]; ++j) {
+      const std::string at = who + " " + unit + " " + std::to_string(i) + " frame " + std::to_string(j - s->frame_off[i]);
+      const double t = s->time_s[j];
+      const char* why = !std::isfinite(t)                             ? "non-finite time"
+                        : t < 0                                       ? "time < 0"
+                        : j > s->frame_off[i] && t < s->time_s[j - 1] ? "time decreases"
+                                                                      : nullptr;
+      if (why) return fail(BP_E_INVALID, at + ": " + why);
+      for (long long v = s->value_off[j]; v < s->value_off[j + 1]; ++v) {
+        const double c = s->chroma[v];
+        why = !std::isfinite(s->midi[v]) ? "non-finite midi" : !(c >= 0 && c < 12) ? "chroma outside [0, 12)" : nullptr;
+        if (why) return fail(BP_E_INVALID, at + " value " + std::to_string(v - s->value_off[j]) + ": " + why);
+      }
+    }
+  return BP_OK;
+}
+
+int check_window(const std::string& api, double window) {
+  if (!std::isfinite(window) || window < 0) return fail(BP_E_INVALID, api + ": window must be finite and >= 0");
+  return BP_OK;
+}
+
+// Rule 1 of the metric (include/bp_b200.h): the estimate frame each reference time reads, -1 for none.
+template <class Out>
+void multipitch_map(const double* et, long long ne, const double* rt, long long nr, Out* out) {
+  if (ne == 0) {
+    for (long long k = 0; k < nr; ++k) out[k] = -1;
+    return;
+  }
+  bool same = ne == nr;  // np.allclose(est_t, ref_t): |a - b| <= 1e-8 + 1e-5 |b|, each operation rounded on its own
+  for (long long k = 0; same && k < nr; ++k) {
+    volatile double tol = 1e-5 * std::fabs(rt[k]);
+    same = std::fabs(et[k] - rt[k]) <= 1e-8 + tol;
+  }
+  if (same) {
+    for (long long k = 0; k < nr; ++k) out[k] = (Out)k;
+    return;
+  }
+  // interp1d(kind='nearest'): x_bds = x / 2, x_bds[1:] + x_bds[:-1], searchsorted(side='left'), clip; outside
+  // [x[0], x[-1]] the fill value
+  std::vector<double> bds(ne - 1);
+  for (long long i = 0; i + 1 < ne; ++i) bds[i] = et[i + 1] / 2.0 + et[i] / 2.0;
+  for (long long k = 0; k < nr; ++k) {
+    const double t = rt[k];
+    const long long i = std::lower_bound(bds.begin(), bds.end(), t) - bds.begin();
+    out[k] = t < et[0] || t > et[ne - 1] ? (Out)-1 : (Out)std::min(i, ne - 1);
+  }
+}
+
+// The values of frames [0, F) of s, each frame's sorted by midi (stable): appended to pk; offsets into o[3]
+// (value_off, midi, chroma).
+void pack_mp_values(const bp_multipitch_set_t* s, long long F, Pack& pk, size_t* o) {
+  const long long V = F > 0 ? s->value_off[F] : 0;
+  std::vector<long long> idx(V), voff(F + 1, 0);
+  std::vector<double> mi(V), ch(V);
+  for (long long v = 0; v < V; ++v) idx[v] = v;
+  for (long long j = 0; j < F; ++j) {
+    voff[j + 1] = s->value_off[j + 1];
+    std::stable_sort(idx.begin() + s->value_off[j], idx.begin() + s->value_off[j + 1],
+                     [&](long long a, long long b) { return s->midi[a] < s->midi[b]; });
+  }
+  for (long long v = 0; v < V; ++v) mi[v] = s->midi[idx[v]], ch[v] = s->chroma[idx[v]];
+  o[0] = pk.add(voff.data(), sizeof(long long) * (F + 1));
+  o[1] = pk.add(mi.data(), sizeof(double) * V);
+  o[2] = pk.add(ch.data(), sizeof(double) * V);
+}
+
+// Everything bp_score_frames_grid_* check before anything is enqueued, in addition to check_grid_args.
+int check_frames_grid(const std::string& api, int n_files, int n_params, const bp_multipitch_set_t* refs, double window,
+                      const double* est_midi, const double* est_chroma, const int64_t* h_counts) {
+  int rc = check_window(api, window);
+  if (rc || n_files == 0 || n_params == 0) return rc;
+  if (!h_counts || !est_midi || !est_chroma) return fail(BP_E_INVALID, api + ": bad argument");
+  for (int k = 0; k < 128; ++k) {
+    const std::string at = api + ": estimate table entry " + std::to_string(k);
+    if (!std::isfinite(est_midi[k])) return fail(BP_E_INVALID, at + ": non-finite midi");
+    if (k > 0 && est_midi[k] < est_midi[k - 1]) return fail(BP_E_INVALID, at + ": midi decreases");
+    if (!(est_chroma[k] >= 0 && est_chroma[k] < 12)) return fail(BP_E_INVALID, at + ": chroma outside [0, 12)");
+  }
+  return check_mp_set(api, "references", "file", refs, n_files);
+}
+
+FrameRefs frame_refs_at(const unsigned char* d, size_t o_owner, size_t o_est, const size_t* o_val, long long K) {
+  return FrameRefs{reinterpret_cast<const int*>(d + o_owner), reinterpret_cast<const int*>(d + o_est),
+                   reinterpret_cast<const long long*>(d + o_val[0]), reinterpret_cast<const double*>(d + o_val[1]),
+                   reinterpret_cast<const double*>(d + o_val[2]), K};
+}
+
+}  // namespace
+
+extern "C" {
+
+int bp_multipitch_map(const double* est_t, int64_t n_est, const double* ref_t, int64_t n_ref, int64_t* out) {
+  if (n_est < 0 || n_ref < 0 || (n_est > 0 && !est_t) || (n_ref > 0 && (!ref_t || !out)))
+    return fail(BP_E_INVALID, "bp_multipitch_map: bad argument");
+  for (int64_t i = 0; i < n_est; ++i)
+    if (!std::isfinite(est_t[i]) || (i > 0 && est_t[i] < est_t[i - 1]))
+      return fail(BP_E_INVALID, "bp_multipitch_map: estimate frame " + std::to_string(i) + ": non-finite or decreasing time");
+  for (int64_t k = 0; k < n_ref; ++k)
+    if (!std::isfinite(ref_t[k]))
+      return fail(BP_E_INVALID, "bp_multipitch_map: reference frame " + std::to_string(k) + ": non-finite time");
+  multipitch_map(est_t, n_est, ref_t, n_ref, out);
+  return BP_OK;
+}
+
+int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                                int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                                const bp_multipitch_set_t* refs, double window, const double* est_midi,
+                                const double* est_chroma, int64_t* h_counts, void* stream) {
+  const std::string api = "bp_score_frames_grid_device";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long total_frames = foff[n_files], cells = total_frames * kPitches;
+  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  // one upload per call: per reference frame its file and the file's frame it reads, the sorted values, the tables
+  const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
+  std::vector<int> owner(K), est(K);
+  std::vector<double> et;
+  for (int f = 0; f < n_files; ++f) {
+    const long long T = foff[f + 1] - foff[f], k0 = refs->frame_off[f];
+    et.resize(T);
+    bp_frame_times(T, et.data());
+    multipitch_map(et.data(), T, refs->time_s + k0, refs->frame_off[f + 1] - k0, est.data() + k0);
+    std::fill(owner.begin() + k0, owner.begin() + refs->frame_off[f + 1], f);
+  }
+  Pack pk;
+  const size_t o_owner = pk.add(owner.data(), sizeof(int) * K), o_est = pk.add(est.data(), sizeof(int) * K);
+  size_t o_val[3];
+  pack_mp_values(refs, K, pk, o_val);
+  const size_t o_tm = pk.add(est_midi, sizeof(double) * 128), o_tc = pk.add(est_chroma, sizeof(double) * 128);
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const long long n_counts = (long long)n_params * n_files * kFrameCounts;
+  CK(m->score_counts.reserve((size_t)n_counts));
+  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
+  const FrameRefs R = frame_refs_at(m->score_in.p, o_owner, o_est, o_val, K);
+  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>&, const std::vector<long long>&) -> int {
+    // each setting's E is dead once the loops have run: it becomes that setting's count roll
+    int* roll = reinterpret_cast<int*>(m->energy.p);
+    if (cells > 0) CK(cudaMemsetAsync(roll, 0, sizeof(int) * P * cells, st));
+    launch_frame_roll(m->d_frame_off.p, m->d_slot_off.p, m->note_count.p, m->slot_start.p, m->slot_end.p,
+                      m->slot_pitch.p, n_files, P, roll, cells, st);
+    CKL();
+    CK(m->score_ws_ref.reserve((size_t)(P * frame_ws_stride(V, K)) + 1));
+    FrameEst e{};
+    e.roll = roll;
+    e.roll_stride = cells;
+    e.frame_off = m->d_frame_off.p;
+    e.tab_midi = reinterpret_cast<const double*>(m->score_in.p + o_tm);
+    e.tab_chroma = reinterpret_cast<const double*>(m->score_in.p + o_tc);
+    launch_frame_match(R, e, window, m->score_ws_ref.p, n_files, P, m->score_counts.p + kFrameCounts * p0 * n_files, st);
+    CKL();
+    m->launches += 3;
+    return BP_OK;
+  });
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * n_counts, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                              int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                              const bp_multipitch_set_t* refs, double window, const double* est_midi,
+                              const double* est_chroma, int64_t* h_counts) {
+  const std::string api = "bp_score_frames_grid_host";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  DeviceGuard g(m->device);
+  const int64_t total = h_frame_off[n_files];
+  cudaStream_t st = m->stream;
+  rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {  // uploaded once for the whole grid
+    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
+    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+  }
+  return bp_score_frames_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, window,
+                                     est_midi, est_chroma, h_counts, st);
+}
+
+int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, const bp_multipitch_set_t* refs,
+                             int32_t n_items, double window, int64_t* h_counts) {
+  const std::string api = "bp_score_multipitch_host";
+  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  int rc = check_window(api, window);
+  if (rc || n_items == 0) return rc;
+  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_mp_set(api, "estimates", "item", est, n_items);
+  if (!rc) rc = check_mp_set(api, "references", "item", refs, n_items);
+  if (rc) return rc;
+  const long long K = refs->frame_off[n_items], V = K > 0 ? refs->value_off[K] : 0, FE = est->frame_off[n_items];
+  if (FE > INT_MAX) return fail(BP_E_INVALID, api + ": more than 2^31 - 1 estimate frames");
+  std::vector<int> owner(K), emap(K);
+  for (int i = 0; i < n_items; ++i) {
+    const long long k0 = refs->frame_off[i], e0 = est->frame_off[i];
+    multipitch_map(est->time_s + e0, est->frame_off[i + 1] - e0, refs->time_s + k0, refs->frame_off[i + 1] - k0,
+                   emap.data() + k0);
+    for (long long k = k0; k < refs->frame_off[i + 1]; ++k) {
+      owner[k] = i;
+      if (emap[k] >= 0) emap[k] += (int)e0;  // global estimate frame
+    }
+  }
+  Pack pk;
+  const size_t o_owner = pk.add(owner.data(), sizeof(int) * K), o_est = pk.add(emap.data(), sizeof(int) * K);
+  size_t o_val[3], o_eval[3];
+  pack_mp_values(refs, K, pk, o_val);
+  pack_mp_values(est, FE, pk, o_eval);
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(m->score_ws_ref.reserve((size_t)frame_ws_stride(V, K) + 1));
+  CK(m->score_counts.reserve((size_t)n_items * kFrameCounts));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * kFrameCounts * n_items, st));
+  const unsigned char* d = m->score_in.p;
+  FrameEst e{};
+  e.voff = reinterpret_cast<const long long*>(d + o_eval[0]);
+  e.midi = reinterpret_cast<const double*>(d + o_eval[1]);
+  e.chroma = reinterpret_cast<const double*>(d + o_eval[2]);
+  launch_frame_match(frame_refs_at(d, o_owner, o_est, o_val, K), e, window, m->score_ws_ref.p, n_items, 1,
+                     m->score_counts.p, st);
+  CKL();
+  m->launches += 1;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * kFrameCounts * n_items, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,
                          const bp_decode_params_t* params, int64_t* h_frame_off, bp_notes_t* notes, void* stream) {
   if (!m || !h_sample_off || !h_frame_off || n_files < 0) return fail(BP_E_INVALID, "bp_transcribe_device: bad argument");

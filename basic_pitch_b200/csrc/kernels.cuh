@@ -304,6 +304,39 @@ struct ScoreWork {       // int workspace: 2 per reference and setting, 4 per es
 void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
                         long long n_pairs, long long* counts, cudaStream_t st);
 
+// ---- score_frames.cu: frame-level multi-pitch counts (bp_score_frames_grid_*, bp_score_multipitch_host) -------------
+constexpr int kFrameCounts = 7;  // n_ref, n_est, tp, tp_chroma, sum min, miss, false alarms
+struct FrameRefs {         // the call's K reference frames, back to back over files (grid) or items
+  const int* owner;        // [K] file or item of frame k
+  const int* est_frame;    // [K] the estimate frame it reads (file-relative for the grid, global otherwise), -1: none
+  const long long* voff;   // [K + 1] values of frame k, ascending midi
+  const double *midi, *chroma;
+  long long n_frames;      // K
+};
+struct FrameEst {
+  // grid: the count roll, int [88][T] per file at roll + s * roll_stride + frame_off[f] * 88, and the value tables of
+  // MIDI numbers 0..127 (midi non-decreasing)
+  const int* roll;
+  long long roll_stride;
+  const long long* frame_off;
+  const double *tab_midi, *tab_chroma;
+  // explicit: estimate frame j's values [voff[j], voff[j+1]), ascending midi
+  const long long* voff;
+  const double *midi, *chroma;
+};
+// int workspace of the chroma matching: frame k of chunk-local setting s at ws + s * (4 V + 2 K) + 4 voff[k] + 2 k
+// (V values, K frames): per reference value its mate and visit stamp, and a stack of 2 (n + 1) for its frame's n.
+__host__ __device__ inline long long frame_ws_stride(long long n_values, long long n_frames) { return 4 * n_values + 2 * n_frames; }
+// Count roll of a grid chunk (the decode's dead E, reused): after the memset, +1 / -1 at each note's start / end, then a
+// prefix sum along frames: roll[p][t] = notes of pitch p + 21 with start <= t < end.  Two launches.
+void launch_frame_roll(const long long* frame_off, const long long* slot_off, const int* note_count, const int* start,
+                       const int* end, const int* pitch, int n_files, int n_settings, int* roll, long long roll_stride,
+                       cudaStream_t st);
+// One launch: counts[7 (s * n_owner + owner) ..] += the seven sums of every frame of setting s (n_settings 1 and
+// E.roll == NULL: explicit estimates).  counts must be zeroed by the caller.
+void launch_frame_match(const FrameRefs& R, const FrameEst& E, double window, int* ws, int n_owner, int n_settings,
+                        long long* counts, cudaStream_t st);
+
 // ---- sonify.cu: bp_sonify_notes_host on the given stream of the current device (h_audio == NULL: size query, no CUDA
 // call); adds its kernel launches to *launches ---------------------------------------------------------------------------
 int sonify_notes(cudaStream_t st, long long* launches, int32_t n_files, const int32_t* note_off, const double* start_s,

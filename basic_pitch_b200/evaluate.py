@@ -1,13 +1,18 @@
-"""Note-level transcription scores (addition; no reference counterpart).
+"""Note-level and frame-level transcription scores (addition; no reference counterpart).
 
 The library counts, per (setting, file) or item, the reference notes, the estimated notes and the size of a maximum
 matching with and without the offset test (`Model.score_grid`, `Model.score_notes`, `inference.evaluate_grid`;
 include/bp_b200.h, bp_score_*).  This module turns the counts into the precision, recall and F-measure of
 mir_eval.transcription.precision_recall_f1_overlap (0.7, beta = 1, strict=False), by its formulas.
+
+Frame level: the library sums, per (setting, file) or item, the seven counts of `FRAME_FIELDS` over the reference
+frames (`Model.score_frames_grid`, `Model.score_multipitch`, `inference.evaluate_frames_grid`; include/bp_b200.h,
+bp_score_frames_grid_* / bp_score_multipitch_host).  `frame_scores` turns them into the 14 numbers of
+mir_eval.multipitch.metrics (0.7), bit for bit.
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, List
 
 import numpy as np
 
@@ -20,6 +25,74 @@ TOLERANCES = dict(onset_tolerance=0.05, pitch_tolerance=50.0, offset_ratio=0.2, 
 EST_LOG2_HZ = np.ascontiguousarray(np.log2(440.0 * 2.0 ** ((np.arange(128, dtype=np.float64) - 69.0) / 12.0)))
 
 FIELDS = ("n_ref", "n_est", "matched_no_offset", "matched")
+
+# Frame level: the default window of mir_eval.multipitch.metrics, in semitones
+WINDOW = 0.5
+FRAME_FIELDS = ("n_ref", "n_est", "tp", "tp_chroma", "n_min", "miss", "false_alarm")
+_METRICS = ("precision", "recall", "accuracy", "substitution_error", "miss_error", "false_alarm_error", "total_error")
+
+
+def multipitch_values(hz):
+    """Pitches in Hz -> (midi, chroma) float64 as mir_eval.multipitch sees them: frequencies_to_midi, then
+    midi_to_chroma followed by the np.mod of util._outer_distance_mod_n (chroma in [0, 12)).  A pitch <= 0 gives a
+    non-finite midi, which the library rejects."""
+    hz = np.asarray(hz, np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        midi = 69.0 + 12.0 * np.log2(hz / 440.0)
+        chroma = np.mod(np.mod(midi, 12), 12)
+    return midi, chroma
+
+
+# Values of the MIDI numbers 0..127 as an estimated note's pitch, from the Hz of EST_LOG2_HZ (`note_creation.midi_to_hz`)
+EST_MIDI, EST_CHROMA = (np.ascontiguousarray(a) for a in
+                        multipitch_values(440.0 * 2.0 ** ((np.arange(128, dtype=np.float64) - 69.0) / 12.0)))
+
+
+def notes_to_multipitch(intervals, pitches_hz, times) -> List[np.ndarray]:
+    """Note annotations -> a multi-pitch series at `times` (non-decreasing, seconds): frame t holds the Hz of every note
+    with onset <= t < offset, in note order.  This is how note annotations become frame references, and, at
+    `note_creation.model_frames_to_time`, the estimate series the grid scorer builds from decoded notes."""
+    iv = np.asarray(intervals, np.float64).reshape(-1, 2)
+    hz = np.asarray(pitches_hz, np.float64).reshape(-1)
+    t = np.asarray(times, np.float64).reshape(-1)
+    if len(iv) != len(hz):
+        raise ValueError(f"{len(iv)} intervals but {len(hz)} pitches")
+    lo = np.searchsorted(t, iv[:, 0], side="left")  # first frame at or after the onset
+    hi = np.maximum(np.searchsorted(t, iv[:, 1], side="left"), lo)  # first frame at or after the offset
+    n = hi - lo
+    frame = np.repeat(lo - np.cumsum(n) + n, n) + np.arange(n.sum())
+    note = np.repeat(np.arange(len(hz)), n)
+    if len(t) == 0:
+        return []
+    order = np.argsort(frame, kind="stable")
+    cuts = np.searchsorted(frame[order], np.arange(1, len(t)))
+    return np.split(hz[note[order]], cuts)
+
+
+def frame_scores(counts) -> Dict[str, np.ndarray]:
+    """counts (..., 7) as `Model.score_frames_grid` / `score_multipitch` return them -> dict of float64 arrays of shape
+    counts.shape[:-1]: precision, recall, accuracy, substitution_error, miss_error, false_alarm_error, total_error and
+    the same seven with a "chroma_" prefix, by mir_eval.multipitch's formulas (0 where a denominator is 0; every error
+    is 0 when n_ref is 0).  "mean" holds them averaged over the last axis, as in `note_scores`."""
+    c = np.asarray(counts, np.int64)
+    if c.ndim < 1 or c.shape[-1] != 7:
+        raise ValueError(f"counts must have shape (..., 7), got {c.shape}")
+    n_ref, n_est, tp, tpc, n_min, miss, fa = (c[..., k].astype(np.float64) for k in range(7))
+
+    def div(a, b):
+        return np.where(b > 0, a / np.where(b > 0, b, 1.0), 0.0)
+
+    out: Dict[str, np.ndarray] = {}
+    for prefix, t in (("", tp), ("chroma_", tpc)):
+        vals = (div(t, n_est), div(t, n_ref), div(t, n_est + n_ref - t), div(n_min - t, n_ref), div(miss, n_ref),
+                div(fa, n_ref), div(n_min + miss + fa - t, n_ref))
+        out.update({prefix + k: v for k, v in zip(_METRICS, vals)})
+    if c.ndim >= 2:
+        n = c.shape[-2]
+        out["mean"] = {k: (v.mean(axis=-1) if n else np.zeros(v.shape[:-1])) for k, v in out.items()}
+    else:
+        out["mean"] = {k: (v.mean() if v.size else np.float64(0.0)) for k, v in out.items()}
+    return out
 
 
 def note_scores(counts) -> Dict[str, np.ndarray]:

@@ -419,6 +419,70 @@ class Model:
         self._lib.bp_score_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(counts))
         return counts
 
+    # ------------------------------------------------------------------ frame-level scores
+    @staticmethod
+    def _multipitch_set(series: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]], what: str):
+        """[(times (n,) in seconds, [Hz array per frame])] (mir_eval.multipitch's convention) -> (bp_multipitch_set_t,
+        the arrays it points at), values as `evaluate.multipitch_values` gives them."""
+        f_off = np.zeros(len(series) + 1, np.int64)
+        times, counts, hzs = [], [], []
+        for i, (t, freqs) in enumerate(series):
+            t = np.asarray(t, np.float64).reshape(-1)
+            if len(t) != len(freqs):
+                raise ValueError(f"{what}[{i}]: {len(t)} times but {len(freqs)} frames of frequencies")
+            f_off[i + 1] = f_off[i] + len(t)
+            times.append(t)
+            for fr in freqs:
+                fr = np.asarray(fr, np.float64).reshape(-1)
+                counts.append(len(fr))
+                hzs.append(fr)
+        v_off = np.zeros(len(counts) + 1, np.int64)
+        np.cumsum(counts, out=v_off[1:])
+        midi, chroma = evaluate.multipitch_values(np.concatenate(hzs) if hzs else np.zeros(0))
+        arrs = (f_off, np.ascontiguousarray(np.concatenate(times) if times else np.zeros(0)), v_off,
+                np.ascontiguousarray(midi), np.ascontiguousarray(chroma))
+        ms = _lib.MultipitchSet()
+        ms.frame_off, ms.time_s, ms.value_off, ms.midi, ms.chroma = (_ptr(a) for a in arrs)
+        return ms, arrs
+
+    def score_frames_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
+                          settings: Sequence[Dict[str, Any]], references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
+                          window: float = evaluate.WINDOW) -> np.ndarray:
+        """Frame-level multi-pitch counts of a batch of files decoded under every setting of a grid, scored against one
+        reference series per file, in ONE library call (`bp_score_frames_grid_host`): the notes never leave the device.
+        A setting is a dict of `decode_arrays`' keyword arguments (include_pitch_bends is ignored: bends are not
+        applied); a reference is (times (n,) in seconds, [Hz array per frame]), mir_eval's convention; window in
+        semitones.  The estimate of (setting, file) is the piano roll of its notes at the model frame times.  Returns
+        int64 counts (n_settings, n_files, 7) in the order of `evaluate.FRAME_FIELDS` (`evaluate.frame_scores` turns them
+        into mir_eval.multipitch's metrics)."""
+        n_files, n_params = len(notes), len(settings)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference series")
+        ps = self._grid_params(settings)
+        refs, keep = self._multipitch_set(references, "references")
+        foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+        counts = np.zeros((n_params, n_files, 7), np.int64)
+        self._lib.bp_score_frames_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params,
+                                            C.byref(refs), float(window), _ptr(evaluate.EST_MIDI),
+                                            _ptr(evaluate.EST_CHROMA), _ptr(counts))
+        return counts
+
+    def score_multipitch(self, estimates: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
+                         references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
+                         window: float = evaluate.WINDOW) -> np.ndarray:
+        """Item i's estimate series against item i's reference series (`bp_score_multipitch_host`, one kernel launch),
+        both as (times (n,) in seconds, [Hz array per frame]): mir_eval.multipitch.metrics for arbitrary series, for
+        example `evaluate.notes_to_multipitch` of another system's notes.  Returns int64 counts (n_items, 7) as
+        `score_frames_grid`."""
+        if len(estimates) != len(references):
+            raise ValueError(f"{len(estimates)} estimate but {len(references)} reference series")
+        est, keep_e = self._multipitch_set(estimates, "estimates")
+        refs, keep_r = self._multipitch_set(references, "references")
+        counts = np.zeros((len(estimates), 7), np.int64)
+        self._lib.bp_score_multipitch_host(self._h, C.byref(est), C.byref(refs), len(estimates), float(window),
+                                           _ptr(counts))
+        return counts
+
     def infer_onsets_array(self, onsets: np.ndarray, frames: np.ndarray) -> np.ndarray:
         """reference: note_creation.py:289-311 `get_infered_onsets` (n_diff = 2) -> float64 (T, 88), on the device."""
         o = np.ascontiguousarray(onsets, dtype=_F32)
@@ -817,6 +881,36 @@ def evaluate_grid(
     outs = model.run_inference_arrays(clips)
     counts = model.score_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references, **tolerances)
     return counts, evaluate.note_scores(counts)
+
+
+def evaluate_frames_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    window: float = evaluate.WINDOW,
+):
+    """Frame-level multi-pitch scores of a batch of annotated recordings under every setting of a grid (addition; no
+    reference counterpart): the model runs once over the batch, and every (setting, file) is decoded and scored against
+    its file's reference series on the device in one `bp_score_frames_grid_host` call.  `audio` and `settings` as in
+    `evaluate_grid`; `references[i]` is file i's (times (n,) in seconds, [Hz array per frame]), mir_eval.multipitch's
+    convention (`evaluate.notes_to_multipitch` makes one from note annotations); window in semitones.
+
+    Returns (counts (n_settings, n_files, 7), `evaluate.frame_scores(counts)`)."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    outs = model.run_inference_arrays(clips)
+    counts = model.score_frames_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
+                                     window=window)
+    return counts, evaluate.frame_scores(counts)
 
 
 def predict_batch(

@@ -223,6 +223,68 @@ int bp_score_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
 int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
                         const bp_score_params_t* score, int64_t* h_counts);
 
+/* ---- frame-level multi-pitch scores of decoded notes against reference frames -------------------------------------
+ * No reference counterpart: the sums behind mir_eval.multipitch.metrics 0.7 (window = 0.5 semitones by default).
+ * A series is a time array time[0 .. N) (seconds, non-decreasing) and per frame a multiset of values, each carried as
+ * two float64 numbers computed by the caller: midi = 69 + 12 log2(hz / 440) and chroma = mod(mod(midi, 12), 12), in
+ * [0, 12) (basic_pitch_b200/evaluate.py, multipitch_values).  The library only subtracts, adds, takes absolute values
+ * and compares, in float64, round to nearest, never contracted.
+ *  1. Time base: reference frame k reads estimate frame k when n_est == n_ref and every
+ *     |est_t - ref_t| <= 1e-8 + 1e-5 |ref_t| (np.allclose); otherwise the frame scipy.interpolate.interp1d(est_t,
+ *     arange(n_est), kind='nearest', bounds_error=False, fill_value=n_est) gives at ref_t: bounds x_k / 2 + x_k+1 / 2,
+ *     the number of bounds below ref_t, clipped to n_est - 1; ref_t < est_t[0] or > est_t[n_est - 1] reads an empty
+ *     frame, as does every frame of an empty estimate.  bp_multipitch_map returns this map.
+ *  2. Hits within a frame: plain, r and e hit when fl(e - w) <= r <= fl(e + w) (midi values); chroma, d = |r - e| and
+ *     min(d, fl(12 - d)) <= w (chroma values).
+ *  3. tp_k is the size of a maximum matching of frame k's hit graph; every element of a multiset is a vertex.
+ *  4. Per (setting, file) or item, seven int64 sums over the reference frames k, with R_k, E_k the frame's multisets:
+ *     {n_ref = sum |R_k|, n_est = sum |E_k|, tp = sum tp_k, tp_chroma = sum tp_chroma_k, n_min = sum min(|R_k|, |E_k|),
+ *      miss = sum max(0, |R_k| - |E_k|), fa = sum max(0, |E_k| - |R_k|)}.
+ *     Precision tp / n_est, recall tp / n_ref, accuracy tp / (n_est + n_ref - tp), and the error rates
+ *     (n_min - tp, miss, fa, n_min + miss + fa - tp) / n_ref follow bit for bit in float64 (0 for a zero denominator;
+ *     evaluate.frame_scores); the chroma versions use tp_chroma.
+ * Validation, before anything is enqueued, returns BP_E_INVALID naming the file or item and the frame or value
+ * ("references file 3 frame 17 value 2: chroma outside [0, 12)"): offsets starting at 0 and never decreasing, at most
+ * 2^31 - 1 frames per set and values per frame, times finite, >= 0 and non-decreasing within a set, midi finite, chroma
+ * in [0, 12); window finite and >= 0. */
+typedef struct bp_multipitch_set {
+  const int64_t* frame_off; /* [n + 1]: frames of set i are [frame_off[i], frame_off[i+1]) */
+  const double* time_s;     /* [frames] */
+  const int64_t* value_off; /* [frames + 1]: values of frame j are [value_off[j], value_off[j+1]); value_off[0] == 0 */
+  const double* midi;       /* [values] */
+  const double* chroma;     /* [values] */
+} bp_multipitch_set_t;
+
+/* Host-only: the reference -> estimate frame map of rule 1 (out[k] = -1: empty frame).  est_t must be finite and
+ * non-decreasing, ref_t finite. */
+int bp_multipitch_map(const double* est_t, int64_t n_est, const double* ref_t, int64_t n_ref, int64_t* out);
+
+/* Grid frame scoring: bp_score_grid_* with frame-level counts.  The estimate series of (setting, file) has the file's
+ * T model frames, times bp_frame_times(T); frame t holds one value per decoded note with start_frame <= t < end_frame,
+ * est_midi[pitch_midi] / est_chroma[pitch_midi] (two 128-entry host tables: midi finite and non-decreasing, chroma in
+ * [0, 12)).  Pitch bends are not applied.  That is the piano roll of the note events, sampled at the model frames.
+ * refs: one series per file.  h_counts [n_params][n_files][7] (host), in the order of rule 4.
+ * Settings are validated, grouped, chunked and rerun as in bp_decode_grid_*.  Kernel launches per chunk: those of the
+ * grid decode + 3 (note-count roll scatter, its prefix sum along frames, the match kernel), whatever the number of
+ * settings and files; the roll is zeroed with one memset.  Device workspace beyond the decode's: the roll reuses each
+ * setting's "remaining energy" copy (int [88][T] per file); the chroma matching takes 16 bytes per reference value and 8
+ * per reference frame, per setting of a chunk.
+ * _device: posteriorgrams in device memory, work on `stream`, synchronised before returning; _host: host
+ * posteriorgrams, uploaded once. */
+int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                                int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                                const bp_multipitch_set_t* refs, double window, const double* est_midi,
+                                const double* est_chroma, int64_t* h_counts, void* stream);
+int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                              int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                              const bp_multipitch_set_t* refs, double window, const double* est_midi,
+                              const double* est_chroma, int64_t* h_counts);
+/* Item i's estimate series (est, explicit) scored against item i's reference series; h_counts [n_items][7].  One
+ * kernel launch and one memset (none for n_items == 0), synchronous.  Workspace: 16 bytes per reference value and 8 per
+ * reference frame. */
+int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, const bp_multipitch_set_t* refs,
+                             int32_t n_items, double window, int64_t* h_counts);
+
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
