@@ -55,7 +55,8 @@ struct TcConvSpec {
   int data_bins, chunks8;                   // bins of the input rows and 8-bin chunks of the split layout (even)
   int rows_per_window, lead_rows;           // row layout of the split input: 172 frames + zero rows per window
   int layer;                                // 0 contour, 1 onset, 2 note
-  int KH2, HALO, G0;                        // fused next conv: time taps, frequency halo; tiles of a group are G0 apart
+  int KH2, HALO, G0;                        // fused next conv: time taps, frequency halo; groups of two frequency tiles
+  int PD;                                   // pair distance: the two tiles of a group are PD apart (tc_group_tile)
   // fused next conv as a second contraction (tc_conv.cu): weight tiles, their N, accumulator columns per output offset j,
   // accumulator columns, columns staged in shared memory at a time (a multiple of 8 and of js: whole output offsets)
   int n2_tiles, n2, js, width, pass;
@@ -71,13 +72,56 @@ struct TcConvSpec {
 };
 // clang-format off
 __host__ __device__ constexpr TcConvSpec tc_spec(int layer) {
-  //                  KH  KW SF PT PL COUT FLT WOUT n_ci shifts                               bins          ch8 rows/win lead layer KH2 HALO G0  n2_tiles n2 js width pass  W
-  return layer == 0 ? TcConvSpec{3, 39, 1, 1, 19, 8, 16, 264, 8, {-36, 0, 36, 57, 72, 84, 93, 101}, kCqtBins,     40, 174, 3, 0, 5, 2, 9,  1, 32, 5, 104, 40, 0, {}}
-       : layer == 1 ? TcConvSpec{5, 5, 3, 2, 1, 32, 4, 88, 8, {-36, 0, 36, 57, 72, 84, 93, 101},   kCqtBins,     40, 174, 3, 1, 3, 1, 12, 2, 16, 4, 32, 32,   6,
+  //                  KH  KW SF PT PL COUT FLT WOUT n_ci shifts                               bins          ch8 rows/win lead layer KH2 HALO G0  PD  n2_tiles n2 js width pass  W
+  return layer == 0 ? TcConvSpec{3, 39, 1, 1, 19, 8, 16, 264, 8, {-36, 0, 36, 57, 72, 84, 93, 101}, kCqtBins,     40, 174, 3, 0, 5, 2, 9,  1,  1, 32, 5, 104, 40, 0, {}}
+       : layer == 1 ? TcConvSpec{5, 5, 3, 2, 1, 32, 4, 88, 8, {-36, 0, 36, 57, 72, 84, 93, 101},   kCqtBins,     40, 174, 3, 1, 3, 1, 12, 12, 2, 16, 4, 32, 32,   6,
                                  {9, 10, 21, 22, 14, 4, 2, 1, 16, 3, 6, 13, 5, 17, 18, 20, 19, 23, 7, 0, 8, 15, 12, 11}}
-                    : TcConvSpec{7, 7, 3, 3, 2, 32, 4, 88, 1, {0, 0, 0, 0, 0, 0, 0, 0},           kContourBins, 34, 175, 6, 2, 7, 1, 12, 2, 32, 8, 64, 64,   8, {}};
+                    : TcConvSpec{7, 7, 3, 3, 2, 32, 4, 88, 1, {0, 0, 0, 0, 0, 0, 0, 0},           kContourBins, 34, 175, 6, 2, 7, 1, 12, 12, 2, 32, 8, 64, 64,   8, {}};
 }
 // clang-format on
+// The pairing of frequency tiles into groups, the one rule the planner, the kernels, edge_fix_kernel and the tests read.
+// Group g is position i = g % PD of run g / PD; a run holds 2 PD consecutive tiles, slot 0 the lower PD, slot 1 the upper
+// PD, so the tiles of group g are {2 PD run + i, 2 PD run + PD + i} (-1: past the last tile, or no such group).
+// Contour PD = 1: neighbouring tiles, which read the same weight tiles at A chunks two apart, so the two slots share
+// almost every step of the weight ring.  Onset / note PD = G0: tiles {g, g + G0} (no weight ring to share).
+__host__ __device__ constexpr int tc_group_tile(const TcConvSpec& s, int g, int slot) {
+  if (g < 0 || g >= s.G0) return -1;
+  const int run = g / s.PD, i = g - run * s.PD, ft = 2 * s.PD * run + slot * s.PD + i;
+  return ft < s.n_ft() ? ft : -1;
+}
+// group (slot in bit 0, group << 1) of frequency tile ft: the inverse of tc_group_tile
+__host__ __device__ constexpr int tc_tile_group(const TcConvSpec& s, int ft) {
+  const int run = ft / (2 * s.PD), r = ft - run * 2 * s.PD, slot = r / s.PD;
+  return ((run * s.PD + r - slot * s.PD) << 1) | slot;
+}
+// A slot walks its tiles of an item's groups [g0, g1) in ascending order and carries the frequency halo of the fused
+// conv2 from one tile to the next in registers.  Its tile in group g STARTS a range (no carry from below) where the item
+// starts or where its tile in g - 1 is not the one below; it ENDS a range where the item ends or its tile in g + 1 is not
+// the one above.  Boundary b (between tiles b - 1 and b) goes through the edge buffer iff tile b starts a range, which is
+// the case iff tile b - 1 ends one.
+__host__ __device__ constexpr bool tc_starts_range(const TcConvSpec& s, int g, int slot, bool item_start) {
+  const int ft = tc_group_tile(s, g, slot);
+  return item_start || ft <= 0 || tc_group_tile(s, g - 1, slot) != ft - 1;
+}
+__host__ __device__ constexpr bool tc_ends_range(const TcConvSpec& s, int g, int slot, bool item_end) {
+  return item_end || tc_group_tile(s, g + 1, slot) != tc_group_tile(s, g, slot) + 1;
+}
+// an item of split n (groups [q G0 / n, (q + 1) G0 / n)) starts at group g
+__host__ __device__ constexpr bool tc_item_starts(const TcConvSpec& s, int n_split, int g) {
+  const int q = (g * n_split + s.G0 - 1) / s.G0;  // the least q with q G0 / n >= g
+  return q < n_split && q * s.G0 / n_split == g;
+}
+// every frequency tile belongs to exactly one (group, slot), and tc_tile_group finds it
+__host__ __device__ constexpr bool tc_pairing_ok(const TcConvSpec& s) {
+  for (int ft = 0; ft < s.n_ft(); ++ft) {
+    int n = 0;
+    for (int g = 0; g < s.G0; ++g)
+      for (int slot = 0; slot < 2; ++slot) n += tc_group_tile(s, g, slot) == ft;
+    const int gs = tc_tile_group(s, ft);
+    if (n != 1 || tc_group_tile(s, gs >> 1, gs & 1) != ft) return false;
+  }
+  return true;
+}
 // Host side: weight tiles + the per-group MMA programs of the Toeplitz form.  The kernels run it for the contour conv
 // only; the onset and note convs gather their A operand instead (tc_build_b1), and their plans only serve the tests.
 struct TcConvPlan {

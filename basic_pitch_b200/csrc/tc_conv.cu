@@ -19,8 +19,9 @@
 //     of tile row r finishes the output frame r - H (H = KH2 / 2) and adds its taps in the same order whatever its
 //     position in the tile, so a frame's value does not depend on the batch around it,
 //   * the frequency halo between neighbouring tiles is a register carry: a slot walks its frequency tiles in ascending
-//     order; only where two tile RANGES meet (slot 0 | slot 1, or the group splits of a small batch) the two partial
-//     sums go to a small edge buffer and edge_fix_kernel finishes those 4 (contour) / 2 bins,
+//     order; only where two tile RANGES meet (a slot's next tile is not the one above, or an item of the group split
+//     ends; tc_starts_range) the two partial sums go to a small edge buffer and edge_fix_kernel finishes those
+//     4 (contour) / 2 bins,
 //   * bias, sigmoid (+ the note input channel of the onset conv2, + unwrap inference.py:247-279) and the store.
 // The unfused contour epilogue stores the activations channels-last (path 2, activation-level tests).
 //
@@ -55,8 +56,9 @@
 // a frequency tile go to four m64n32 accumulators that, side by side, are the m64n128 fragment of the Toeplitz form, so
 // the epilogue is the same for all layers.
 //
-// Work decomposition: item = (M-tile of 64 rows, split s of S over the frequency groups); group g = the two
-// frequency tiles {g, g + G0} (two accumulator slots; shared weight tiles where their content is equal).  A CTA (1 per
+// Work decomposition: item = (M-tile of 64 rows, split s of S over the frequency groups); group g = two frequency
+// tiles (tc_group_tile: contour the neighbours {2g, 2g + 1}, onset / note {g, g + G0}), one per accumulator slot; the
+// contour's two slots share a weight tile where their content is equal, at every step but a few.  A CTA (1 per
 // SM, persistent) walks items i = blockIdx.x, +gridDim.x, ...:
 //   warp 8      producer: bulk-copies the (64+KH-1) x 320 bf16 hi/lo data tile (k-chunk-major) once per item and
 //               (contour) streams the weight tiles of each group's program (8 KB each) through a ring of stages;
@@ -85,6 +87,10 @@ constexpr int kTileBytes = 8192;                                 // weight tile:
 constexpr int kMaxSteps = 1024;                                  // program steps per layer (constant memory)
 constexpr int kMaxGroups = 15;
 static_assert(tc_spec(0).G0 <= kMaxGroups, "contour groups in constant memory");
+static_assert(tc_pairing_ok(tc_spec(0)) && tc_pairing_ok(tc_spec(1)) && tc_pairing_ok(tc_spec(2)), "group -> tile map");
+static_assert(tc_spec(0).n_ft() <= 2 * tc_spec(0).G0 && tc_spec(1).n_ft() <= 2 * tc_spec(1).G0 &&
+                  tc_spec(2).n_ft() <= 2 * tc_spec(2).G0,
+              "every tile has a place in the reference pairing of the summation order (TcConvPlan::build)");
 constexpr int kConsumerWarps = 8;  // two warpgroups, one per accumulator slot
 constexpr int kProducerWarp = 8;   // the first warp of the third warpgroup; its other three warps only hand back registers
 constexpr int kThreads = 32 * kConsumerWarps + 128;
@@ -217,10 +223,10 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   const int data_rows = kMTile + sp.KH - 1;
   const int lbo16 = data_rows;  // (rows * 16 B) >> 4
   // K = 16 steps start on 8-bin chunk boundaries (the k-chunk-major layout makes any chunk index a legal
-  // descriptor start), so frequency tiles d apart share weight tiles when SF*FLT*d is a multiple of 8 bins; the two
-  // tiles of a group are G0 apart: slot 0 walks tiles 0 .. G0-1, slot 1 tiles G0 .. n_ft-1, both in ascending order
-  // (the fused epilogue carries the frequency halo of the next conv from tile to tile in registers)
-  const int stride = sp.G0;
+  // descriptor start), so frequency tiles d apart share weight tiles when SF*FLT*d is a multiple of 8 bins.  The two
+  // tiles of a group are the pair tc_group_tile gives (contour: neighbours, which share almost every step); each slot
+  // walks its tiles in ascending order (the fused epilogue carries the frequency halo of the next conv in registers).
+  // (Every tile has a partner t +- G0 in the reference pairing of the summation order below: n_ft <= 2 G0.)
 
   // Weight tiles are de-duplicated by STRUCTURE, not by value: two steps share a tile when every element of the two
   // sums the same weights.  The program (tile ids, their count, which steps of a group's two slots merge) then depends on
@@ -278,20 +284,28 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
     return n_keys++;
   };
 
-  // groups: pairs {g, g + G0} (or singles)
-  group_step_off.push_back(0);
-  n_uses = 0;
-  for (int ft_a = 0; ft_a < stride; ++ft_a) {
-    const int ft_b = ft_a + stride < n_ft ? ft_a + stride : -1;
-    const int fts[2] = {ft_a, ft_b};
-    group_ft.push_back(ft_a);
-    group_ft.push_back(ft_b);
-    struct Use {
+  // The order in which every tile sums its steps is fixed, whatever tile the kernels pair it with: the order of the
+  // reference pairing {t, t + G0} (t < G0).  There, per time tap, the uses of the two tiles are sorted by their offset
+  // relative to the tile, a weight tile both use is one step, and the steps only the lower tile uses come first, then
+  // the shared ones, then those only the upper tile uses.  The order is a function of the geometry alone (not of the
+  // batch, the split or the pairing below), and every tile's fp32 sums stay what they are under that reference pairing.
+  struct Use {
+    int tile;
+    uint32_t w;  // A start offset >> 4: chunk c8, row dt
+  };
+  struct Step {
+    int tile;
+    uint32_t w[2];
+  };
+  std::vector<std::vector<Use>> order(n_ft);
+  for (int t = 0; t < sp.G0; ++t) {
+    const int fts[2] = {t, t + sp.G0 < n_ft ? t + sp.G0 : -1};
+    struct Cand {
       int tile, slot, c8, dt, off;
     };
-    std::vector<Use> uses;
+    std::vector<Cand> uses;
     for (int dt = 0; dt < sp.KH; ++dt) {
-      std::vector<Use> cand;
+      std::vector<Cand> cand;
       for (int slot = 0; slot < 2; ++slot) {
         const int ft = fts[slot];
         if (ft < 0) continue;
@@ -317,46 +331,71 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
                                                        // holds chunks 0 .. chunks8 - 2 (the last one is padding only)
           const int off = 8 * c - sp.SF * sp.FLT * ft;
           const int tile = find_or_add(dt, c, ft, 8 * (c8 - c));
-          if (tile >= 0) cand.push_back(Use{tile, slot, c, dt, off});
+          if (tile >= 0) cand.push_back(Cand{tile, slot, c, dt, off});
           c8 += 2;
         }
       }
-      std::stable_sort(cand.begin(), cand.end(), [](const Use& a, const Use& b) {
+      std::stable_sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) {
         return a.off != b.off ? a.off < b.off : (a.tile != b.tile ? a.tile < b.tile : a.slot < b.slot);
       });
       uses.insert(uses.end(), cand.begin(), cand.end());
     }
-    struct Step {
-      int tile;
-      uint32_t w[2];
-    };
     std::vector<Step> steps;
     size_t i = 0;
     while (i < uses.size()) {
       size_t j = i;
       while (j < uses.size() && uses[j].tile == uses[i].tile && (j == i || uses[j].slot != uses[j - 1].slot)) ++j;
       Step stp{uses[i].tile, {kNoUse, kNoUse}};
-      for (size_t u = i; u < j; ++u) {
-        stp.w[uses[u].slot] = (uint32_t)(uses[u].c8 * lbo16 + uses[u].dt);  // A start offset >> 4: chunk c8, row dt
-        ++n_uses;
-      }
+      for (size_t u = i; u < j; ++u) stp.w[uses[u].slot] = (uint32_t)(uses[u].c8 * lbo16 + uses[u].dt);
       steps.push_back(stp);
       i = j;
     }
-    // Software skew between the two slots of a group: the steps only slot 0 uses come first, then the shared ones, then
-    // those only slot 1 uses.  The slots move through the weight ring independently (a slot skips the steps it does not
-    // use), so slot 0 runs its epilogue while slot 1 works through its own steps, and slot 1 runs its epilogue while
-    // slot 0 starts on the next group's.
     std::stable_sort(steps.begin(), steps.end(), [](const Step& a, const Step& b) {
       auto cls = [](const Step& s) { return s.w[1] == kNoUse ? 0 : (s.w[0] == kNoUse ? 2 : 1); };
       return cls(a) < cls(b);
     });
+    for (const Step& stp : steps)
+      for (int sl = 0; sl < 2; ++sl)
+        if (stp.w[sl] != kNoUse) order[fts[sl]].push_back(Use{stp.tile, stp.w[sl]});
+  }
+
+  // Groups: the pairs of tc_group_tile (or singles).  The two tiles' orders are merged into one step sequence; a step is
+  // shared wherever the longest common subsequence of their weight tiles allows, every other use is a step of one slot
+  // (where either slot's own step could come next, slot 1's does).  Each slot still walks its own tile's order.  (Neighbouring tiles use the same weight tiles at A chunks two apart,
+  // so for the contour almost every step is shared.)
+  group_step_off.push_back(0);
+  n_uses = 0;
+  const std::vector<Use> none;
+  for (int g = 0; g < sp.G0; ++g) {
+    const int fts[2] = {tc_group_tile(sp, g, 0), tc_group_tile(sp, g, 1)};
+    group_ft.push_back(fts[0]);
+    group_ft.push_back(fts[1]);
+    const std::vector<Use>& a = fts[0] >= 0 ? order[fts[0]] : none;
+    const std::vector<Use>& b = fts[1] >= 0 ? order[fts[1]] : none;
+    const size_t na = a.size(), nb = b.size();
+    std::vector<int> lcs((na + 1) * (nb + 1), 0);  // [i][j]: common weight tiles of a[i..] and b[j..]
+    auto L = [&](size_t i, size_t j) -> int& { return lcs[i * (nb + 1) + j]; };
+    for (size_t i = na; i-- > 0;)
+      for (size_t j = nb; j-- > 0;)
+        L(i, j) = a[i].tile == b[j].tile ? 1 + L(i + 1, j + 1) : std::max(L(i + 1, j), L(i, j + 1));
     bool seen[2] = {false, false};
-    for (Step& stp : steps) {
+    for (size_t i = 0, j = 0; i < na || j < nb;) {
+      Step stp{-1, {kNoUse, kNoUse}};
+      if (i < na && j < nb && a[i].tile == b[j].tile) {
+        stp = Step{a[i].tile, {a[i].w, b[j].w}};
+        ++i, ++j;
+      } else if (j == nb || (i < na && L(i + 1, j) > L(i, j + 1))) {  // (a tie: slot 1's step first)
+        stp = Step{a[i].tile, {a[i].w, kNoUse}};
+        ++i;
+      } else {
+        stp = Step{b[j].tile, {kNoUse, b[j].w}};
+        ++j;
+      }
       for (int sl = 0; sl < 2; ++sl)
         if (stp.w[sl] != kNoUse) {
           if (!seen[sl]) stp.w[sl] |= kUseFirstAcc;
           seen[sl] = true;
+          ++n_uses;
         }
       tile_seq.push_back(stp.tile);
       slot_words[0].push_back(stp.w[0]);
@@ -375,8 +414,7 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
 // (The onset and note layers gather their A operand and need no program.)
 __constant__ uint32_t c_prog[2][tc::kMaxSteps];  // [slot][step]
 __constant__ int c_tile_seq[tc::kMaxSteps];       // [step] -> weight tile id
-__constant__ int c_group_step_off[tc::kMaxGroups + 1];
-__constant__ int c_group_ft[2 * tc::kMaxGroups];
+__constant__ int c_group_step_off[tc::kMaxGroups + 1];  // (the tiles of a group are tc_group_tile's)
 
 // tiles: [tile][plane hi/lo][k-chunk 2][n N2][8] bf16 (canonical K-major no-swizzle: LBO = N2 * 16 B, SBO = 128 B)
 // Tile tl, row kk holds element k = 16 tl + kk of the conv1 row: bin b = k / COUT of the step, channel c = k % COUT
@@ -409,7 +447,6 @@ int tc_upload_program(const TcConvPlan& pl, cudaStream_t st) {
   cudaMemcpyToSymbolAsync(c_tile_seq, pl.tile_seq.data(), pl.tile_seq.size() * 4, 0, cudaMemcpyHostToDevice, st);
   cudaMemcpyToSymbolAsync(c_group_step_off, pl.group_step_off.data(), pl.group_step_off.size() * 4, 0,
                           cudaMemcpyHostToDevice, st);
-  cudaMemcpyToSymbolAsync(c_group_ft, pl.group_ft.data(), pl.group_ft.size() * 4, 0, cudaMemcpyHostToDevice, st);
   return cudaStreamSynchronize(st) == cudaSuccess ? 0 : -1;
 }
 
@@ -641,8 +678,8 @@ __device__ __forceinline__ void slot_barrier(int slot) {  // the four warps (one
   asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
 }
 
-// Edge-buffer slot of the tile range that slot `s` of split `q` walks (it starts at tile g0(q) + s * G0): s * n_split + q.
-// The range that ENDS below it is slot s of split q - 1, or, for (s, q) = (1, 0), slot 0 of the last split.
+// The edge buffer has one slot per boundary b between tiles b - 1 and b (slot b - 1), with two sides: side 0 from the
+// range that starts at tile b, side 1 from the range that ends at tile b - 1 (tc_starts_range / tc_ends_range).
 
 // What the thread that finishes one frame knows about where its results go.  The threads of a warp hold consecutive
 // frames, and every layout below has the frame index fastest.
@@ -657,7 +694,6 @@ struct RowOut {
   const float* note_col;  // onset: note_raw_pm + b*172 + t
   int t;         // frame inside the window (of the OUTPUT frame this thread finishes)
   bool ok;       // live output frame whose time taps are complete in this M-tile
-  int e_lo, e_hi;  // edge slots of this range's start and of the range above its end (-1: none)
 };
 
 // Frequency halo + finish for the onset / note layers (FLT = 4, HALO = 1): S[j] is the time-complete sum for bin
@@ -670,7 +706,7 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
-      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * L.edge_per_side() * a.edge_rows;
+      float* e = ro.edge + (size_t)((ft - 1) * 2 + 0) * L.edge_per_side() * a.edge_rows;
       e[0] = S[0];
       e[a.edge_rows] = S[1];
     }
@@ -712,8 +748,8 @@ __device__ __forceinline__ void finish_pitch_tile(const TcArgs& a, const RowOut&
   }
   carry[0] = S[L.FLT];
   carry[1] = S[L.FLT + 1];
-  if (last && ft < L.n_ft() - 1 && ro.edge && ro.e_hi >= 0) {
-    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * L.edge_per_side() * a.edge_rows;
+  if (last && ft < L.n_ft() - 1 && ro.edge) {
+    float* e = ro.edge + (size_t)(ft * 2 + 1) * L.edge_per_side() * a.edge_rows;
     e[0] = S[L.FLT];
     e[a.edge_rows] = S[L.FLT + 1];
   }
@@ -749,7 +785,7 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
   const bool lower = ft > 0;
   if (first) {
     if (lower && ro.edge) {
-      float* e = ro.edge + (size_t)(ro.e_lo * 2 + 0) * L.edge_per_side() * a.edge_rows;
+      float* e = ro.edge + (size_t)((ft - 1) * 2 + 0) * L.edge_per_side() * a.edge_rows;
 #pragma unroll
       for (int k = 0; k < 4; ++k) e[(size_t)k * a.edge_rows] = S[k];
 #pragma unroll
@@ -776,8 +812,8 @@ __device__ __forceinline__ void finish_contour_tile(const TcArgs& a, const RowOu
   for (int k = 0; k < 6; ++k) hold[k] = fin[10 + k];
 #pragma unroll
   for (int k = 0; k < 4; ++k) carry[k] = S[16 + k];
-  if (last && ft < L.n_ft() - 1 && ro.edge && ro.e_hi >= 0) {
-    float* e = ro.edge + (size_t)(ro.e_hi * 2 + 1) * L.edge_per_side() * a.edge_rows;
+  if (last && ft < L.n_ft() - 1 && ro.edge) {
+    float* e = ro.edge + (size_t)(ft * 2 + 1) * L.edge_per_side() * a.edge_rows;
 #pragma unroll
     for (int k = 0; k < 4; ++k) e[(size_t)k * a.edge_rows] = S[16 + k];
 #pragma unroll
@@ -947,7 +983,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   static_assert(kFused || !kGather, "the onset and note epilogues always fuse the next conv");
   constexpr int NW = L.width, PC = L.pass, PS = PC + 1;  // conv2 accumulator columns, staged per pass; staging row pitch
   static_assert(PC % 8 == 0 && PC % L.js == 0, "a staging pass holds whole fragment blocks and whole output offsets");
-  constexpr int kDataRows = kMTile + L.KH - 1, kFt = L.n_ft();
+  constexpr int kDataRows = kMTile + L.KH - 1;
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr TcSmem SM = tc_smem(LAYER, FUSED);
   constexpr int kStages = SM.stages;
@@ -1083,8 +1119,6 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         const int row = tid;
         const int q = mt * a.ms - 2 * a.h2 + row;
         const int b = q >= 0 ? q / L.rows_per_window : 0, t = q - b * L.rows_per_window;
-        ro.e_lo = slot * a.n_split + spl;
-        ro.e_hi = (spl + 1 < a.n_split) ? slot * a.n_split + spl + 1 : (slot == 0 ? a.n_split : -1);
         ro.ok = row < 64 && row >= 2 * a.h2 && q >= 0 && b < a.n_windows && t < kFrames;
         ro.t = t;
         if (ro.ok) {
@@ -1112,12 +1146,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       ph_d ^= 1;
       for (int g = g0; g < g1; ++g) {
         float acc[64];
-        int ft;
+        const int ft = tc_group_tile(L, g, slot);
         if constexpr (kGather) {
-          ft = g + slot * L.G0 < kFt ? g + slot * L.G0 : -1;
           if (ft >= 0) gather_conv1<LAYER>(acc, s_data, smem_u32(s_b1), ft, fr0, qd, clk);
         } else {
-          ft = c_group_ft[2 * g + slot];
           const int s0 = c_group_step_off[g], s1 = c_group_step_off[g + 1];
           int pend = -1;  // stage read by the MMA group still in flight
           uint32_t pend_fill = 0;  // and its fill index
@@ -1171,8 +1203,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
         if (g == g1 - 1 && lane == 0) mbar_arrive(data_empty);  // this warp no longer reads the data tile
         if (ft < 0) continue;
         // first / last tile of this slot's ascending range inside the item
-        const bool first = (g == g0);
-        const bool last = (g == g1 - 1) || (ft == kFt - 1);
+        const bool first = tc_starts_range(L, g, slot, g == g0);
+        const bool last = tc_ends_range(L, g, slot, g == g1 - 1);
         const int n_valid = min(L.FLT, L.WOUT - ft * L.FLT) * L.COUT;  // a multiple of 32 (contour: 64 in the last tile)
         // conv1 bias of the thread's accumulator columns: channel of column 8 i + 2 qd + e is (8 i + 2 qd + e) % COUT.
         // Read here, after the conv1 MMAs, so that it holds no registers during the gather.
@@ -1274,43 +1306,40 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
 
 
 // ------------------------------------------------------------------------------------------------
-// Where two tile ranges meet (frequency tile ft_b = first tile of a range, ft_b > 0) the 2 * HALO bins
-// FLT * ft_b - HALO + k got one partial sum from each side: finish them here.  Pitch layers: 2 bins per frame.  Contour:
-// 4 bins, and with the six finished bins each side left next to them the two 8-bin chunks around the boundary.
+// Where two tile ranges meet (boundary ft_b: tile ft_b starts a range under the launch's split, see tc_starts_range)
+// the 2 * HALO bins FLT * ft_b - HALO + k got one partial sum from each side: finish them here.  Pitch layers: 2 bins
+// per frame.  Contour: 4 bins, and with the six finished bins each side left next to them the two 8-bin chunks around
+// the boundary.
 // ------------------------------------------------------------------------------------------------
 struct EdgeFixArgs {
   TcOut o;
   int edge_rows, n_rows;        // rows of the (window, frame) space covered by the M-tiles
-  int n_edges;                  // 2 * n_split slots: slot e = s * n_split + q starts at tile q * G0 / n_split + s * G0
-  int n_split, n_windows;
+  uint32_t edges;               // bit b: boundary b goes through the edge buffer under the launch's split (tc_edge_mask)
+  int n_windows;
   float bias2, note_w[9];  // the layer's conv2 bias; onset: the conv2 weights of the note input channel
 };
 
-// contour: one thread per (frame, edge); pitch layers: per (frame, edge, bin)
+// The boundaries b = 1 .. n_ft - 1 where a range starts under split n_split (tile b starts a range in its group)
+__host__ __device__ constexpr uint32_t tc_edge_mask(const TcConvSpec& s, int n_split) {
+  uint32_t m = 0;
+  for (int b = 1; b < s.n_ft(); ++b) {
+    const int gs = tc_tile_group(s, b);
+    if (tc_starts_range(s, gs >> 1, gs & 1, tc_item_starts(s, n_split, gs >> 1))) m |= 1u << b;
+  }
+  return m;
+}
+static_assert(tc_spec(0).n_ft() <= 32 && tc_spec(1).n_ft() <= 32 && tc_spec(2).n_ft() <= 32, "boundary mask");
+static_assert(tc_edge_mask(tc_spec(0), 1) == 0x1fffeu && tc_edge_mask(tc_spec(1), 1) == 1u << 12,
+              "contour: every tile a range of its own; onset: the slot boundary only");
+
+// contour: one thread per frame; pitch layers: per (frame, bin); each fixes the boundaries of the mask
 template <int LAYER>
 constexpr int kEdgeThreads = LAYER == 0 ? 1 : 2 * tc_spec(LAYER).HALO;
 
 template <int LAYER>
-__global__ void edge_fix_kernel(const EdgeFixArgs a) {
+__device__ __forceinline__ void edge_fix_boundary(const EdgeFixArgs& a, int ft_b, int R, int b, int t, int uf, int k) {
   constexpr TcConvSpec L = tc_spec(LAYER);
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  constexpr int per_edge = kEdgeThreads<LAYER>;
-  const long long total = (long long)a.n_rows * a.n_edges * per_edge;
-  if (idx >= total) return;
-  const int R = (int)(idx % a.n_rows);  // rows fastest: coalesced reads of the edge buffer, coalesced stores
-  const int ek = (int)(idx / a.n_rows);
-  const int e = ek / per_edge, k = ek - e * per_edge;
-  const int b = R / L.rows_per_window, t = R - b * L.rows_per_window;
-  if (b >= a.n_windows || t >= kFrames) return;
-  const int es = e / a.n_split, eq = e - es * a.n_split;
-  const int ft_b = eq * L.G0 / a.n_split + es * L.G0;
-  if (ft_b <= 0 || ft_b >= L.n_ft()) return;  // not a boundary between two ranges
-  int uf = -1;
-  if (a.o.ud) {
-    const UnwrapDesc u = a.o.ud[b];
-    const int tt = t - kOverlapHalf;
-    if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
-  }
+  const int e = ft_b - 1;  // edge slot of the boundary
   if constexpr (LAYER == 0) {
     const float* lo = a.o.edge + (size_t)(e * 2 + 0) * L.edge_per_side() * a.edge_rows + R;  // from the range that starts at ft_b
     const float* hi = a.o.edge + (size_t)(e * 2 + 1) * L.edge_per_side() * a.edge_rows + R;  // from the range that ends at ft_b - 1
@@ -1347,7 +1376,7 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
   const int f = L.FLT * ft_b - L.HALO + k;
   if (f < 0 || f >= L.WOUT) return;
   float x = (a.o.edge[((size_t)(e * 2 + 0) * L.edge_per_side() + k) * a.edge_rows + R] +
-             a.o.edge[((size_t)(e * 2 + 1) * L.edge_per_side() + k) * a.edge_rows + R]) + a.bias2;  // (S + carry) + bias  // (S + carry) + bias
+             a.o.edge[((size_t)(e * 2 + 1) * L.edge_per_side() + k) * a.edge_rows + R]) + a.bias2;  // (S + carry) + bias
   if (a.o.note_raw) {
 #pragma unroll
     for (int dt = 0; dt < 3; ++dt)
@@ -1361,6 +1390,24 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
   const float v = sigmoidf_fast(x);
   if (a.o.raw) a.o.raw[(size_t)f * a.o.raw_rows + (size_t)b * kFrames + t] = v;
   if (uf >= 0) a.o.unwrapped[(size_t)f * a.o.frame_stride + uf] = v;
+}
+
+template <int LAYER>
+__global__ void edge_fix_kernel(const EdgeFixArgs a) {
+  constexpr TcConvSpec L = tc_spec(LAYER);
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.n_rows * kEdgeThreads<LAYER>) return;
+  const int R = (int)(idx % a.n_rows);  // rows fastest: coalesced reads of the edge buffer, coalesced stores
+  const int k = (int)(idx / a.n_rows);
+  const int b = R / L.rows_per_window, t = R - b * L.rows_per_window;
+  if (b >= a.n_windows || t >= kFrames) return;
+  int uf = -1;
+  if (a.o.ud) {
+    const UnwrapDesc u = a.o.ud[b];
+    const int tt = t - kOverlapHalf;
+    if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
+  }
+  for (uint32_t m = a.edges; m; m &= m - 1) edge_fix_boundary<LAYER>(a, __ffs(m) - 1, R, b, t, uf, k);
 }
 // ------------------------------------------------------------------------------------------------
 int tc_rows_total(int n_windows, int rows_per_window) {
@@ -1388,7 +1435,7 @@ void launch_lognorm_split(const float* y, const unsigned int* minmax, const floa
 size_t tc_edge_floats(const TcConvSpec& sp, int n_windows) {
   const int ms = tc::kMTile - (sp.KH2 - 1);
   const int n_mtiles = (n_windows * sp.rows_per_window + ms - 1) / ms;
-  return (size_t)2 * sp.G0 * 2 * sp.edge_per_side() * ((size_t)n_mtiles * ms);  // at most 2 * G0 range starts
+  return (size_t)(sp.n_ft() - 1) * 2 * sp.edge_per_side() * ((size_t)n_mtiles * ms);  // one slot per tile boundary
 }
 
 // The conv kernel of one layer and, for a fused epilogue, the fix-up of the bins where two tile ranges meet.
@@ -1396,7 +1443,7 @@ template <int LAYER, bool FUSED>
 static void launch_layer(const TcArgs& a, const EdgeFixArgs& ef, int grid, cudaStream_t st) {
   conv_tc_kernel<LAYER, FUSED><<<grid, tc::kThreads, tc::tc_smem(LAYER, FUSED).total(), st>>>(a);
   if (FUSED) {
-    const long long total = (long long)ef.n_rows * ef.n_edges * kEdgeThreads<LAYER>;
+    const long long total = (long long)ef.n_rows * kEdgeThreads<LAYER>;
     edge_fix_kernel<LAYER><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ef);
   }
 }
@@ -1466,13 +1513,11 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
         a.use_tmap = 1;
     }
   }
-  // slot s of split q covers tiles [g0(q) + s*G0, g1(q) + s*G0): edge slot s*split + q
   EdgeFixArgs ef{};
   ef.o = o;
   ef.edge_rows = a.edge_rows;
   ef.n_rows = n_windows * sp.rows_per_window;
-  ef.n_edges = 2 * split;
-  ef.n_split = split;
+  ef.edges = tc_edge_mask(sp, split);  // the conv kernel's own range predicate
   ef.n_windows = n_windows;
   ef.bias2 = dev.bias2;
   std::copy_n(dev.note_w, 9, ef.note_w);
