@@ -2056,7 +2056,8 @@ int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
 
 }  // extern "C"
 
-// ---- frame-level scoring (bp_score_frames_grid_*, bp_score_multipitch_host, bp_multipitch_map) ---------------------
+// ---- frame-level scoring (bp_score_frames_grid_*, bp_score_multipitch_host, bp_multipitch_map,
+// bp_score_salience_grid_*) ----------------------------------------------------------------------------------------------
 namespace {
 
 // Validates n multi-pitch series (`what` "references" / "estimates", set unit "file" / "item"): offsets start at 0 and
@@ -2167,6 +2168,42 @@ FrameRefs frame_refs_at(const unsigned char* d, size_t o_owner, size_t o_est, co
   return FrameRefs{reinterpret_cast<const int*>(d + o_owner), reinterpret_cast<const int*>(d + o_est),
                    reinterpret_cast<const long long*>(d + o_val[0]), reinterpret_cast<const double*>(d + o_val[1]),
                    reinterpret_cast<const double*>(d + o_val[2]), K};
+}
+
+// Salience scoring (bp_score_salience_grid_*): posteriorgram widths up to this many bins; settings per chunk bounded by
+// this much chroma-matching workspace (bp_score_salience_chunk_params).
+constexpr int kMaxSalienceWidth = 1024;
+constexpr long long kSalienceChunkBytes = 2LL << 30;
+
+// Everything bp_score_salience_grid_* check before anything is enqueued (include/bp_b200.h).
+int check_salience_grid(const std::string& api, const bp_model* m, int width, const int64_t* h_frame_off, int n_files,
+                        const bp_salience_params_t* params, int n_params, const bp_multipitch_set_t* refs, double window,
+                        const double* bin_midi, const double* bin_chroma, const int64_t* h_counts) {
+  if (!m || n_files < 0 || n_params < 0 || (n_params > 0 && !params)) return fail(BP_E_INVALID, api + ": bad argument");
+  if (width < 1 || width > kMaxSalienceWidth)
+    return fail(BP_E_INVALID, api + ": width must be in [1, " + std::to_string(kMaxSalienceWidth) + "]");
+  for (int k = 0; k < n_params; ++k) {
+    const bp_salience_params_t& p = params[k];
+    const char* why = !(std::isfinite(p.threshold) && p.threshold > 0)        ? "threshold must be finite and > 0"
+                      : p.peak_pick != 0 && p.peak_pick != 1                  ? "peak_pick must be 0 or 1"
+                      : !(0 <= p.bin_lo && p.bin_lo <= p.bin_hi && p.bin_hi <= width) ? "need 0 <= bin_lo <= bin_hi <= width"
+                                                                              : nullptr;
+    if (why) return fail(BP_E_INVALID, api + ": salience params[" + std::to_string(k) + "]: " + why);
+  }
+  int rc = check_window(api, window);
+  if (rc || n_files == 0 || n_params == 0) return rc;
+  if (!h_frame_off || !h_counts || !bin_midi || !bin_chroma) return fail(BP_E_INVALID, api + ": bad argument");
+  for (int b = 0; b < width; ++b) {
+    const std::string at = api + ": bin table entry " + std::to_string(b);
+    if (!std::isfinite(bin_midi[b])) return fail(BP_E_INVALID, at + ": non-finite midi");
+    if (b > 0 && bin_midi[b] < bin_midi[b - 1]) return fail(BP_E_INVALID, at + ": midi decreases");
+    if (!(bin_chroma[b] >= 0 && bin_chroma[b] < 12)) return fail(BP_E_INVALID, at + ": chroma outside [0, 12)");
+  }
+  if (h_frame_off[0] != 0) return fail(BP_E_INVALID, api + ": frame_off[0] must be 0");
+  for (int i = 0; i < n_files; ++i)
+    if (h_frame_off[i + 1] < h_frame_off[i] || h_frame_off[i + 1] - h_frame_off[i] > INT_MAX)
+      return fail(BP_E_INVALID, api + ": file " + std::to_string(i) + ": bad frame_off");
+  return check_mp_set(api, "references", "file", refs, n_files);
 }
 
 }  // namespace
@@ -2319,6 +2356,95 @@ int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, cons
   CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * kFrameCounts * n_items, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
+}
+
+int64_t bp_score_salience_chunk_params(int64_t n_ref_frames, int64_t n_ref_values) {
+  const long long per = frame_ws_stride(std::max<int64_t>(n_ref_values, 0), std::max<int64_t>(n_ref_frames, 0)) *
+                        (long long)sizeof(int);  // 16 V + 8 K bytes
+  return std::max(1LL, kSalienceChunkBytes / std::max(1LL, per));
+}
+
+int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t width, const int64_t* h_frame_off,
+                                  int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                  const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                  const double* bin_chroma, int64_t* h_counts, void* stream) {
+  const std::string api = "bp_score_salience_grid_device";
+  int rc = check_salience_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma,
+                               h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  if (foff[n_files] > 0 && !d_gram) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  // one upload per call: per reference frame its file and the file's frame it reads, the sorted values, the bin tables
+  // and every setting
+  const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
+  std::vector<int> owner(K), est(K);
+  std::vector<double> et;
+  for (int f = 0; f < n_files; ++f) {
+    const long long T = foff[f + 1] - foff[f], k0 = refs->frame_off[f];
+    et.resize(T);
+    bp_frame_times(T, et.data());
+    multipitch_map(et.data(), T, refs->time_s + k0, refs->frame_off[f + 1] - k0, est.data() + k0);
+    std::fill(owner.begin() + k0, owner.begin() + refs->frame_off[f + 1], f);
+  }
+  std::vector<SalienceSettingDev> sal(n_params);
+  for (int k = 0; k < n_params; ++k)
+    sal[k] = SalienceSettingDev{params[k].threshold, params[k].peak_pick, params[k].bin_lo, params[k].bin_hi, 0};
+  Pack pk;
+  const size_t o_owner = pk.add(owner.data(), sizeof(int) * K), o_est = pk.add(est.data(), sizeof(int) * K);
+  size_t o_val[3];
+  pack_mp_values(refs, K, pk, o_val);
+  const size_t o_tm = pk.add(bin_midi, sizeof(double) * width), o_tc = pk.add(bin_chroma, sizeof(double) * width),
+               o_set = pk.add(sal.data(), sizeof(SalienceSettingDev) * n_params);
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(m->d_frame_off.reserve(n_files + 1));
+  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
+  const long long n_counts = (long long)n_params * n_files * kFrameCounts;
+  CK(m->score_counts.reserve((size_t)n_counts));
+  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
+  const long long chunk = bp_score_salience_chunk_params(K, V);
+  CK(m->score_ws_ref.reserve((size_t)(std::min<long long>(chunk, n_params) * frame_ws_stride(V, K)) + 1));
+  const FrameRefs R = frame_refs_at(m->score_in.p, o_owner, o_est, o_val, K);
+  FrameEst e{};
+  e.gram = d_gram;
+  e.width = width;
+  e.frame_off = m->d_frame_off.p;
+  e.tab_midi = reinterpret_cast<const double*>(m->score_in.p + o_tm);
+  e.tab_chroma = reinterpret_cast<const double*>(m->score_in.p + o_tc);
+  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
+    const int P = (int)std::min<long long>(chunk, n_params - p0);
+    e.salience = reinterpret_cast<const SalienceSettingDev*>(m->score_in.p + o_set) + p0;
+    launch_frame_match(R, e, window, m->score_ws_ref.p, n_files, P, m->score_counts.p + kFrameCounts * p0 * n_files, st);
+    CKL();
+    m->launches += 1;
+  }
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * n_counts, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_score_salience_grid_host(bp_model_t* m, const float* h_gram, int32_t width, const int64_t* h_frame_off,
+                                int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                const double* bin_chroma, int64_t* h_counts) {
+  const std::string api = "bp_score_salience_grid_host";
+  int rc = check_salience_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma,
+                               h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const int64_t total = h_frame_off[n_files];
+  if (total > 0 && !h_gram) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  if (total > 0) {  // uploaded once for the whole grid
+    CK(m->st_contour.reserve((size_t)total * width));
+    CK(cudaMemcpyAsync(m->st_contour.p, h_gram, sizeof(float) * total * width, cudaMemcpyHostToDevice, st));
+  }
+  return bp_score_salience_grid_device(m, m->st_contour.p, width, h_frame_off, n_files, params, n_params, refs, window,
+                                       bin_midi, bin_chroma, h_counts, st);
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,

@@ -348,8 +348,14 @@ struct ScoreWork {       // int workspace: 2 per reference and setting, 4 per es
 void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
                         long long n_pairs, long long* counts, cudaStream_t st);
 
-// ---- score_frames.cu: frame-level multi-pitch counts (bp_score_frames_grid_*, bp_score_multipitch_host) -------------
+// ---- score_frames.cu: frame-level multi-pitch counts (bp_score_frames_grid_*, bp_score_multipitch_host,
+// bp_score_salience_grid_*) -------------------------------------------------------------------------------------------
 constexpr int kFrameCounts = 7;  // n_ref, n_est, tp, tp_chroma, sum min, miss, false alarms
+enum class EstKind { kExplicit, kRoll, kGram };  // where the match kernel's estimate frames come from
+struct SalienceSettingDev {  // bp_salience_params_t, validated
+  double threshold;
+  int peak_pick, bin_lo, bin_hi, reserved;
+};
 struct FrameRefs {         // the call's K reference frames, back to back over files (grid) or items
   const int* owner;        // [K] file or item of frame k
   const int* est_frame;    // [K] the estimate frame it reads (file-relative for the grid, global otherwise), -1: none
@@ -367,6 +373,11 @@ struct FrameEst {
   // explicit: estimate frame j's values [voff[j], voff[j+1]), ascending midi
   const long long* voff;
   const double *midi, *chroma;
+  // gram: the posteriorgram [frame_off[n_owner]][width], row frame_off[f] + t for frame t of file f, chunk-local
+  // setting s at salience[s]; tab_midi / tab_chroma are the width bin tables (midi non-decreasing)
+  const float* gram;
+  const SalienceSettingDev* salience;
+  long long width;
 };
 // int workspace of the chroma matching: frame k of chunk-local setting s at ws + s * (4 V + 2 K) + 4 voff[k] + 2 k
 // (V values, K frames): per reference value its mate and visit stamp, and a stack of 2 (n + 1) for its frame's n.
@@ -376,8 +387,9 @@ __host__ __device__ inline long long frame_ws_stride(long long n_values, long lo
 void launch_frame_roll(const long long* frame_off, const long long* slot_off, const int* note_count, const int* start,
                        const int* end, const int* pitch, int n_files, int n_settings, int* roll, long long roll_stride,
                        cudaStream_t st);
-// One launch: counts[7 (s * n_owner + owner) ..] += the seven sums of every frame of setting s (n_settings 1 and
-// E.roll == NULL: explicit estimates).  counts must be zeroed by the caller.
+// One launch: counts[7 (s * n_owner + owner) ..] += the seven sums of every frame of setting s (E.roll set: roll
+// estimates; else E.salience set: posteriorgram estimates; else explicit estimates, n_settings 1).  counts must be zeroed by
+// the caller.
 void launch_frame_match(const FrameRefs& R, const FrameEst& E, double window, int* ws, int n_owner, int n_settings,
                         long long* counts, cudaStream_t st);
 

@@ -1,12 +1,15 @@
 // Frame-level multi-pitch counts on the device: the sums behind mir_eval.multipitch.metrics (0.7) for a grid of
-// (setting, file) pairs or a list of items (include/bp_b200.h, bp_score_frames_grid_*, bp_score_multipitch_host).
+// (setting, file) pairs or a list of items (include/bp_b200.h, bp_score_frames_grid_*, bp_score_multipitch_host,
+// bp_score_salience_grid_*).
 //
 // Grid estimates come from the grid decode's note slots.  Once the sequential loops have run, each setting's private
 // "remaining energy" copy is dead; it is exactly an int [88][T] per file, so it becomes a note-count roll: zeroed by the
 // host, +1 / -1 scattered at every note's start / end, then a prefix sum along frames.
 // The match kernel runs one thread per (setting, reference frame).  The reference values of a frame are sorted by midi
-// on the host; the estimate frame is either a roll column (88 pitches in ascending order with their multiplicities) or
-// explicit values sorted by midi.  Every sum is an integer, reduced with integer atomics: the result is deterministic.
+// on the host; the estimate frame is a roll column (88 pitches in ascending order with their multiplicities), explicit
+// values sorted by midi, or a posteriorgram row read under a salience setting (bp_score_salience_grid_*: the bins that
+// pass its threshold, peak and range tests, in ascending bin order, each once).  Every sum is an integer, reduced with
+// integer atomics: the result is deterministic.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -77,16 +80,43 @@ __global__ void __launch_bounds__(kRollThreads) roll_scan_kernel(const long long
 
 // ---- matching -----------------------------------------------------------------------------------------------------
 // The estimate frame as groups g = 0 .. n-1 of equal values in ascending midi: the 88 pitches of a roll column with their
-// counts (grid), or single explicit values.
-template <bool kGrid>
+// counts (roll), single explicit values, or the bins bin_lo + g of a posteriorgram row, each counted once when it is an
+// estimate of the frame under the setting (gram).
+template <EstKind kKind>
 struct EstFrame {
-  const int* col;  // grid: roll column at frame t, pitch g at col[g * T]
+  const int* col;  // roll: roll column at frame t, pitch g at col[g * T]
   long long T;
-  const double *midi, *chroma;  // grid: tables indexed by MIDI number; explicit: this frame's values
+  const double *midi, *chroma;  // roll: tables indexed by MIDI number; explicit: this frame's values; gram: bin tables
   int n;
-  __device__ __forceinline__ int count(int g) const { return kGrid ? col[g * T] : 1; }
-  __device__ __forceinline__ double m(int g) const { return kGrid ? midi[g + 21] : midi[g]; }
-  __device__ __forceinline__ double c(int g) const { return kGrid ? chroma[g + 21] : chroma[g]; }
+  const float* row;  // gram: the posteriorgram row of the frame, `width` bins
+  int width, lo;
+  double thresh;
+  bool peak;
+  // include/bp_b200.h, bp_score_salience_grid_*: bin b is an estimate when thresh <= (double) G[b] and, with peak
+  // picking, 1 <= b <= width - 2 and G[b] > both neighbours (float32, the whole row): scipy.signal.argrelmax, then the
+  // threshold.  Ordered comparisons, so a NaN cell is never an estimate and never below a peak.
+  __device__ __forceinline__ int gram_count(int g) const {
+    const int b = lo + g;
+    const float v = row[b];
+    if (!((double)v >= thresh)) return 0;
+    if (!peak) return 1;
+    return b >= 1 && b <= width - 2 && v > row[b - 1] && v > row[b + 1];
+  }
+  __device__ __forceinline__ int count(int g) const {
+    if constexpr (kKind == EstKind::kRoll) return col[g * T];
+    else if constexpr (kKind == EstKind::kGram) return gram_count(g);
+    else return 1;
+  }
+  __device__ __forceinline__ double m(int g) const {
+    if constexpr (kKind == EstKind::kRoll) return midi[g + 21];
+    else if constexpr (kKind == EstKind::kGram) return midi[lo + g];
+    else return midi[g];
+  }
+  __device__ __forceinline__ double c(int g) const {
+    if constexpr (kKind == EstKind::kRoll) return chroma[g + 21];
+    else if constexpr (kKind == EstKind::kGram) return chroma[lo + g];
+    else return chroma[g];
+  }
 };
 
 // Plain pass (util._fast_hit_windows): e hits r when fl(e - w) <= r <= fl(e + w).  Both ends of the windows are
@@ -95,8 +125,8 @@ struct EstFrame {
 // it is the earliest-deadline greedy for points and intervals sorted by both ends.  A reference skipped for lying below
 // one window's lower end lies below every later window, and exchanging the mate of any maximum matching for the
 // smallest free hit in that order never loses an edge.
-template <bool kGrid>
-__device__ __forceinline__ int plain_tp(const EstFrame<kGrid>& E, const double* rm, int n_ref, double w) {
+template <EstKind kKind>
+__device__ __forceinline__ int plain_tp(const EstFrame<kKind>& E, const double* rm, int n_ref, double w) {
   int i = 0, tp = 0;
   for (int g = 0; g < E.n && i < n_ref; ++g) {
     int c = E.count(g);
@@ -119,8 +149,8 @@ __device__ __forceinline__ bool chroma_hit(double r, double e, double w) {
 // lemma for its copies).  Each search marks the references it visits; the explicit stack holds (group, reference
 // cursor) and grows by one per newly visited reference, so it never exceeds n_ref + 1 frames.
 // ws: mate [n_ref] (group of the reference, -1 free), seen [n_ref] (search stamp), stack [2 (n_ref + 1)].
-template <bool kGrid>
-__device__ __forceinline__ int chroma_tp(const EstFrame<kGrid>& E, const double* rc, int n_ref, int n_est, double w,
+template <EstKind kKind>
+__device__ __forceinline__ int chroma_tp(const EstFrame<kKind>& E, const double* rc, int n_ref, int n_est, double w,
                                          int* ws) {
   const int limit = min(n_ref, n_est);
   if (limit == 0) return 0;
@@ -174,7 +204,7 @@ __device__ __forceinline__ int chroma_tp(const EstFrame<kGrid>& E, const double*
 }
 
 // Thread x = s * K + k: reference frame k under chunk-local setting s.
-template <bool kGrid>
+template <EstKind kKind>
 __global__ void __launch_bounds__(kMatchThreads) frame_match_kernel(FrameRefs R, FrameEst E, double w,
                                                                     int* __restrict__ ws, int n_owner,
                                                                     long long n_threads, long long* __restrict__ counts) {
@@ -189,10 +219,10 @@ __global__ void __launch_bounds__(kMatchThreads) frame_match_kernel(FrameRefs R,
     const long long r0 = R.voff[k];
     const int n_ref = (int)(R.voff[k + 1] - r0);
     pair = s * n_owner + owner;
-    EstFrame<kGrid> ef{};
+    EstFrame<kKind> ef{};
     int n_est = 0;
     if (t >= 0) {
-      if constexpr (kGrid) {
+      if constexpr (kKind == EstKind::kRoll) {
         const long long base = E.frame_off[owner];
         ef.T = E.frame_off[owner + 1] - base;
         ef.col = E.roll + s * E.roll_stride + base * kPitches + t;
@@ -201,6 +231,18 @@ __global__ void __launch_bounds__(kMatchThreads) frame_match_kernel(FrameRefs R,
         ef.n = kPitches;
 #pragma unroll 1  // unrolled, ptxas spills
         for (int g = 0; g < kPitches; ++g) n_est += ef.count(g);
+      } else if constexpr (kKind == EstKind::kGram) {
+        const SalienceSettingDev p = E.salience[s];
+        ef.row = E.gram + (E.frame_off[owner] + t) * E.width;
+        ef.width = (int)E.width;
+        ef.lo = p.bin_lo;
+        ef.n = p.bin_hi - p.bin_lo;
+        ef.thresh = p.threshold;
+        ef.peak = p.peak_pick != 0;
+        ef.midi = E.tab_midi;
+        ef.chroma = E.tab_chroma;
+#pragma unroll 1
+        for (int g = 0; g < ef.n; ++g) n_est += ef.count(g);
       } else {
         const long long e0 = E.voff[t];
         ef.midi = E.midi + e0;
@@ -254,9 +296,11 @@ void launch_frame_match(const FrameRefs& R, const FrameEst& E, double window, in
   const long long n = (long long)n_settings * R.n_frames;
   const unsigned int blocks = (unsigned int)std::max(1LL, (n + kMatchThreads - 1) / kMatchThreads);
   if (E.roll)
-    frame_match_kernel<true><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
+    frame_match_kernel<EstKind::kRoll><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
+  else if (E.salience)
+    frame_match_kernel<EstKind::kGram><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
   else
-    frame_match_kernel<false><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
+    frame_match_kernel<EstKind::kExplicit><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
 }
 
 }  // namespace bp

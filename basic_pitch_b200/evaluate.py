@@ -9,12 +9,20 @@ Frame level: the library sums, per (setting, file) or item, the seven counts of 
 frames (`Model.score_frames_grid`, `Model.score_multipitch`, `inference.evaluate_frames_grid`; include/bp_b200.h,
 bp_score_frames_grid_* / bp_score_multipitch_host).  `frame_scores` turns them into the 14 numbers of
 mir_eval.multipitch.metrics (0.7), bit for bit.
+
+Posteriorgrams as multi-f0 estimates: `salience_to_multipitch` reads a contour (or note) posteriorgram under a
+threshold, peak picking and a frequency range as the series those metrics score (include/bp_b200.h,
+bp_score_salience_grid_*); `Model.score_salience_grid` / `inference.evaluate_salience_grid` score a grid of such
+settings on the device.
 """
 from __future__ import annotations
 
-from typing import Dict, List
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
+
+from . import constants
+from .note_creation import model_frames_to_time
 
 # mir_eval.transcription's defaults: onset within 50 ms, pitch within 50 cents, offset within
 # max(0.2 x reference duration, 50 ms)
@@ -67,6 +75,59 @@ def notes_to_multipitch(intervals, pitches_hz, times) -> List[np.ndarray]:
     order = np.argsort(frame, kind="stable")
     cuts = np.searchsorted(frame[order], np.arange(1, len(t)))
     return np.split(hz[note[order]], cuts)
+
+
+_SALIENCE_HZ = {"contour": constants.FREQ_BINS_CONTOURS, "note": constants.FREQ_BINS_NOTES}
+
+
+def salience_bins(kind: str = "contour") -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(hz, midi, chroma) float64 of every bin of the contour (264 bins, a third of a semitone) or note (88 bins)
+    posteriorgram: the reference's target grids constants.FREQ_BINS_CONTOURS / FREQ_BINS_NOTES, with their values as
+    `multipitch_values` gives them."""
+    if kind not in _SALIENCE_HZ:
+        raise ValueError(f"kind must be 'contour' or 'note', got {kind!r}")
+    hz = np.ascontiguousarray(_SALIENCE_HZ[kind], np.float64)
+    midi, chroma = multipitch_values(hz)
+    return hz, np.ascontiguousarray(midi), np.ascontiguousarray(chroma)
+
+
+def salience_bin_range(kind: str, minimum_frequency: Optional[float], maximum_frequency: Optional[float]):
+    """The bins [lo, hi) of a frequency range: lo is the first bin with Hz >= minimum_frequency, hi the first bin with
+    Hz > maximum_frequency (np.searchsorted on the bin table); None leaves that side open.  A range below its lower end
+    is empty (hi = lo)."""
+    hz = salience_bins(kind)[0]
+    lo = 0 if minimum_frequency is None else int(np.searchsorted(hz, float(minimum_frequency), side="left"))
+    hi = len(hz) if maximum_frequency is None else int(np.searchsorted(hz, float(maximum_frequency), side="right"))
+    return lo, max(lo, hi)
+
+
+def salience_to_multipitch(gram, threshold: float, peak_picking: bool = True, minimum_frequency: Optional[float] = None,
+                           maximum_frequency: Optional[float] = None, kind: str = "contour"):
+    """A posteriorgram (T, bins) as a multi-f0 estimate (times (T,), [Hz array per frame]), mir_eval.multipitch's
+    convention: frame t at the model frame time holds, in ascending order, the Hz of every bin b in the frequency range
+    (`salience_bin_range`) with float64(gram[t, b]) >= threshold and, with peak_picking, a local maximum of the whole
+    row in float32 (scipy.signal.argrelmax(gram, axis=1): 1 <= b <= bins - 2 and strictly above both neighbours).
+    NaN cells are never estimates.  This is the host definition of bp_score_salience_grid_* (include/bp_b200.h).
+
+    The threshold is compared in float64 on purpose: NumPy 2 compares a float32 array with a Python float in float32,
+    which answers differently for a threshold between two float32 values."""
+    hz = salience_bins(kind)[0]
+    g = np.asarray(gram, np.float32)
+    if g.ndim != 2 or g.shape[1] != len(hz):
+        raise ValueError(f"a {kind} posteriorgram must be (T, {len(hz)}), got {g.shape}")
+    threshold = float(threshold)
+    if not (np.isfinite(threshold) and threshold > 0):
+        raise ValueError(f"threshold must be finite and > 0, got {threshold}")
+    est = g.astype(np.float64) >= threshold
+    if peak_picking:
+        peak = np.zeros(g.shape, bool)
+        mid = g[:, 1:-1]
+        peak[:, 1:-1] = (mid > g[:, :-2]) & (mid > g[:, 2:])
+        est &= peak
+    lo, hi = salience_bin_range(kind, minimum_frequency, maximum_frequency)
+    est[:, :lo] = False
+    est[:, hi:] = False
+    return model_frames_to_time(g.shape[0]), [hz[np.flatnonzero(row)] for row in est]
 
 
 def frame_scores(counts) -> Dict[str, np.ndarray]:

@@ -483,6 +483,50 @@ class Model:
                                            _ptr(counts))
         return counts
 
+    _SALIENCE_KEYS = ("threshold", "peak_picking", "minimum_frequency", "maximum_frequency")
+
+    @staticmethod
+    def _salience_params(settings: Sequence[Dict[str, Any]], kind: str):
+        """Settings {threshold, peak_picking (default True), minimum_frequency, maximum_frequency (default None)} ->
+        bp_salience_params_t array, the range in bins as `evaluate.salience_bin_range` gives it."""
+        ps = (_lib.SalienceParams * max(len(settings), 1))()
+        for k, s in enumerate(settings):
+            unknown = set(s) - set(Model._SALIENCE_KEYS)
+            if unknown:
+                raise TypeError(f"settings[{k}]: unknown salience argument(s) {sorted(unknown)}")
+            if "threshold" not in s:
+                raise TypeError(f"settings[{k}]: a threshold is required")
+            lo, hi = evaluate.salience_bin_range(kind, s.get("minimum_frequency"), s.get("maximum_frequency"))
+            ps[k] = _lib.SalienceParams(float(s["threshold"]), int(bool(s.get("peak_picking", True))), lo, hi, 0)
+        return ps
+
+    def score_salience_grid(self, grams: Sequence[np.ndarray], settings: Sequence[Dict[str, Any]],
+                            references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]], kind: str = "contour",
+                            window: float = evaluate.WINDOW) -> np.ndarray:
+        """Frame-level multi-pitch counts of a batch of posteriorgrams read as multi-f0 estimates under every setting of
+        a grid, scored against one reference series per file, in ONE library call (`bp_score_salience_grid_host`: the
+        posteriorgrams go up once, no estimate is built on the host).  grams[i] is file i's (T, 264) contour or (T, 88)
+        note posteriorgram (`kind`); a setting is a dict {threshold, peak_picking=True, minimum_frequency=None,
+        maximum_frequency=None} and its estimate is `evaluate.salience_to_multipitch` of the posteriorgram under it; a
+        reference is (times (n,) in seconds, [Hz array per frame]); window in semitones.  Returns int64 counts
+        (n_settings, n_files, 7) in the order of `evaluate.FRAME_FIELDS`."""
+        hz, midi, chroma = evaluate.salience_bins(kind)
+        n_files, n_params, width = len(grams), len(settings), len(hz)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference series")
+        foff = np.zeros(n_files + 1, np.int64)
+        for i, g in enumerate(grams):
+            if np.ndim(g) != 2 or np.shape(g)[1] != width:
+                raise ValueError(f"grams[{i}]: a {kind} posteriorgram must be (T, {width}), got {np.shape(g)}")
+            foff[i + 1] = foff[i] + np.shape(g)[0]
+        ps = self._salience_params(settings, kind)
+        refs, keep = self._multipitch_set(references, "references")
+        g_all = _cat_rows(list(grams), width)
+        counts = np.zeros((n_params, n_files, 7), np.int64)
+        self._lib.bp_score_salience_grid_host(self._h, _ptr(g_all), width, _ptr(foff), n_files, ps, n_params,
+                                              C.byref(refs), float(window), _ptr(midi), _ptr(chroma), _ptr(counts))
+        return counts
+
     def infer_onsets_array(self, onsets: np.ndarray, frames: np.ndarray) -> np.ndarray:
         """reference: note_creation.py:289-311 `get_infered_onsets` (n_diff = 2) -> float64 (T, 88), on the device."""
         o = np.ascontiguousarray(onsets, dtype=_F32)
@@ -910,6 +954,38 @@ def evaluate_frames_grid(
     outs = model.run_inference_arrays(clips)
     counts = model.score_frames_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
                                      window=window)
+    return counts, evaluate.frame_scores(counts)
+
+
+def evaluate_salience_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
+    settings: Sequence[Dict[str, Any]],
+    kind: str = "contour",
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    window: float = evaluate.WINDOW,
+):
+    """Frame-level multi-pitch scores of the model's contour (or note) posteriorgram read as a multi-f0 estimate, for a
+    batch of annotated recordings under every setting of a grid (addition; no reference counterpart): the model runs
+    once over the batch, and every (setting, file) is scored on the device in one `bp_score_salience_grid_host` call.
+    `audio` as in `evaluate_grid`; `references` as in `evaluate_frames_grid`; a setting is a dict {threshold,
+    peak_picking=True, minimum_frequency=None, maximum_frequency=None} (`Model.score_salience_grid`); window in
+    semitones.
+
+    Returns (counts (n_settings, n_files, 7), `evaluate.frame_scores(counts)`)."""
+    if kind not in ("contour", "note"):
+        raise ValueError(f"kind must be 'contour' or 'note', got {kind!r}")
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    outs = model.run_inference_arrays(clips)
+    counts = model.score_salience_grid([o[kind] for o in outs], settings, references, kind=kind, window=window)
     return counts, evaluate.frame_scores(counts)
 
 

@@ -285,6 +285,56 @@ int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h
 int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, const bp_multipitch_set_t* refs,
                              int32_t n_items, double window, int64_t* h_counts);
 
+/* ---- frame-level multi-pitch scores of a posteriorgram read as a multi-f0 estimate ---------------------------------
+ * No reference counterpart: the estimate the reference's training targets define (the contour posteriorgram is trained
+ * against multi-f0 annotations on FREQ_BINS_CONTOURS), scored by rules 1 to 4 above for a grid of settings.
+ * The posteriorgram G has `width` bins per frame, float32 row-major [total_frames][width]; file i is frames
+ * [h_frame_off[i], h_frame_off[i+1]), the layout of bp_run_inference_*.  bin_midi[width] / bin_chroma[width] carry the
+ * value of each bin (host tables: midi finite and non-decreasing, chroma in [0, 12)); basic_pitch_b200/evaluate.py,
+ * salience_bins, passes multipitch_values of constants.FREQ_BINS_CONTOURS or FREQ_BINS_NOTES, the reference's target
+ * grids (not midi_to_hz: the bits differ).
+ * Under a setting, bin b of frame t is an estimate of that frame when
+ *   bin_lo <= b < bin_hi, and
+ *   (double) G[t][b] >= threshold, in float64, and
+ *   with peak_pick: 1 <= b <= width - 2, G[t][b] > G[t][b-1] and G[t][b] > G[t][b+1], in float32 on the whole row
+ *   (not only [bin_lo, bin_hi)).
+ * The peak test is scipy.signal.argrelmax(G, axis=1) (order 1, mode 'clip': the edge bins are never peaks), picked
+ * before the threshold as DeepSalience's pitch_activations_to_mf0 does.  Every comparison is an IEEE ordered comparison:
+ * a NaN cell is never an estimate and never below a peak.  The threshold test is in float64 because NumPy 2 compares a
+ * float32 array with a Python float in float32, which answers differently for a threshold between two float32 values;
+ * the host definition (evaluate.salience_to_multipitch) casts the posteriorgram to float64 first.
+ * The estimate series of (setting, file) has the file's T model frames at bp_frame_times(T); frame t holds its estimate
+ * bins in ascending bin order (ascending midi).  Rules 1 to 4 then apply unchanged.
+ * h_counts [n_params][n_files][7] (host), in the order of rule 4.
+ * Validation, before anything is enqueued, returns BP_E_INVALID naming the index ("salience params[3]: threshold must
+ * be finite and > 0", "bin table entry 17: midi decreases"): 1 <= width <= 1024; every threshold finite and > 0;
+ * peak_pick 0 or 1; 0 <= bin_lo <= bin_hi <= width; the bin tables as above; h_frame_off starting at 0, never
+ * decreasing, at most 2^31 - 1 frames per file; the references and the window as for bp_score_frames_grid_*.
+ * n_files == 0 or n_params == 0: BP_OK, nothing enqueued.  The settings run in chunks (bp_score_salience_chunk_params);
+ * per call one memset of the counts, per chunk one launch of the match kernel, whatever the number of settings and
+ * files: the predicate is evaluated from the posteriorgram row in the kernel, with no per-setting copy.  Device
+ * workspace: the chroma matching's 16 bytes per reference value and 8 per reference frame, per setting of a chunk.
+ * _device: posteriorgram in device memory, work on `stream`, synchronised before returning; _host: host posteriorgram,
+ * uploaded once for all settings. */
+typedef struct bp_salience_params {
+  double threshold;  /* > 0, compared in float64 */
+  int32_t peak_pick; /* 0 or 1 */
+  int32_t bin_lo;    /* estimate bins are [bin_lo, bin_hi) */
+  int32_t bin_hi;
+  int32_t reserved;
+} bp_salience_params_t;
+int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t width, const int64_t* h_frame_off,
+                                  int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                  const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                  const double* bin_chroma, int64_t* h_counts, void* stream);
+int bp_score_salience_grid_host(bp_model_t* m, const float* h_gram, int32_t width, const int64_t* h_frame_off,
+                                int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                const double* bin_chroma, int64_t* h_counts);
+/* Host-only: settings per chunk of bp_score_salience_grid_* for references of this size (>= 1): a chunk of c settings
+ * keeps the chroma matching's workspace within 2 GiB, c = max(1, 2^31 / max(1, 16 n_ref_values + 8 n_ref_frames)). */
+int64_t bp_score_salience_chunk_params(int64_t n_ref_frames, int64_t n_ref_values);
+
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
