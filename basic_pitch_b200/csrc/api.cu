@@ -205,6 +205,9 @@ struct bp_model {
   DevBuf<unsigned char> score_in;
   DevBuf<int> score_ws_ref, score_ws_est;
   DevBuf<long long> score_counts;
+  // matchings (bp_match_*): hits per pair, workspace offsets and workspace, estimate offsets of a grid chunk, matchings
+  DevBuf<long long> match_edges, match_off, match_est_off;
+  DevBuf<int> match_ws, match_out;
   int64_t last_forward_n = 0;
   int last_path = 0;
   // optional per-kernel timing (bench.py roofline): CUDA events around one kernel family
@@ -733,6 +736,90 @@ int decode_grid_chunks(bp_model* m, const std::string& api, const float* d_note,
   return BP_OK;
 }
 
+// Running totals of a grid call that returns its notes (bp_decode_grid_*, bp_match_grid_*) over the chunks so far.
+struct GridNotes {
+  long long n_notes = 0, n_bends = 0;
+  bool notes_fit = true, bends_fit = true;
+};
+
+// The note half of a grid chunk's tail (bp_decode_grid_*, bp_match_grid_*): the note offsets of the chunk's pairs into
+// notes->note_off (past the note capacity only the counting goes on: bp_last_required totals the whole grid), the
+// compaction of their notes into m->d_start / d_end / d_pitch (chunk-relative int offsets at m->d_note_off), their
+// amplitudes and, when `bends`, the pitch bends of the settings with include_pitch_bends, all copied into `notes`.
+int grid_chunk_notes(bp_model* m, const std::string& api, const float* d_note, const float* d_contour,
+                     const bp_decode_params_t* params, bool bends, int n_files, long long p0, int P,
+                     const std::vector<int>& counts, bp_notes_t* notes, GridNotes& g, cudaStream_t st) {
+  const long long n_pairs = (long long)P * n_files;
+  // ---- note offsets; past the note capacity only the counting goes on (bp_last_required totals the whole grid)
+  const long long note0 = g.n_notes;
+  for (long long q = 0; q < n_pairs; ++q) {
+    g.n_notes += counts[q];
+    if (g.n_notes > notes->note_capacity) g.notes_fit = false;
+    if (g.notes_fit) notes->note_off[p0 * n_files + q + 1] = (int32_t)g.n_notes;
+  }
+  const long long nc = g.n_notes - note0;  // notes of this chunk
+  if (!g.notes_fit || nc == 0) return BP_OK;
+  if (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude)
+    return fail(BP_E_INVALID, api + ": notes arrays missing");
+  std::vector<int> noff(n_pairs + 1);  // chunk-relative
+  for (long long q = 0; q <= n_pairs; ++q) noff[q] = (int)(notes->note_off[p0 * n_files + q] - note0);
+  CK(m->d_note_off.reserve((size_t)n_pairs + 1));
+  CK(m->d_start.reserve((size_t)nc));
+  CK(m->d_end.reserve((size_t)nc));
+  CK(m->d_pitch.reserve((size_t)nc));
+  CK(m->d_amp.reserve((size_t)nc));
+  CK(m->d_note_base.reserve((size_t)nc));
+  CK(m->d_bend_off.reserve((size_t)nc + 1));
+  CK(cudaMemcpyAsync(m->d_note_off.p, noff.data(), sizeof(int) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
+  compact_notes_kernel<<<dim3(n_files, P), 128, 0, st>>>(m->d_frame_off.p, m->d_slot_off.p, m->d_note_off.p,
+                                                         m->slot_start.p, m->slot_end.p, m->slot_pitch.p, m->d_start.p,
+                                                         m->d_end.p, m->d_pitch.p, m->d_note_base.p);
+  CKL();
+  m->launches += 1;
+  CK(cudaMemcpyAsync(notes->start_frame + note0, m->d_start.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(notes->end_frame + note0, m->d_end.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(notes->pitch_midi + note0, m->d_pitch.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  // ---- bend offsets: each setting's own include_pitch_bends (without: empty ranges, as bp_decode_device leaves them)
+  const long long bend0 = g.n_bends;
+  for (int s = 0; s < P; ++s) {
+    const bool with = bends && params[p0 + s].include_pitch_bends != 0;
+    for (long long j = note0 + noff[(long long)s * n_files]; j < note0 + noff[(long long)(s + 1) * n_files]; ++j) {
+      if (with) g.n_bends += notes->end_frame[j] - notes->start_frame[j];
+      if (g.n_bends > 0x7fffffffLL) return fail(BP_E_CAPACITY, api + ": more than 2^31 pitch-bend values");
+      notes->bend_off[j + 1] = (int32_t)g.n_bends;
+    }
+  }
+  if (g.n_bends > notes->bend_capacity) g.bends_fit = false;
+  if (!g.bends_fit) return BP_OK;
+  const long long bc = g.n_bends - bend0;  // bends of this chunk
+  if (bc > 0 && !notes->bends) return fail(BP_E_INVALID, api + ": bends array missing");
+  std::vector<int> boff(nc + 1);
+  for (long long j = 0; j <= nc; ++j) boff[j] = (int)(notes->bend_off[note0 + j] - bend0);
+  CK(m->d_bends.reserve((size_t)bc + 1));
+  CK(cudaMemcpyAsync(m->d_bend_off.p, boff.data(), sizeof(int) * (nc + 1), cudaMemcpyHostToDevice, st));
+  {
+    ProfScope ps(m, 6, st);
+    launch_note_finish(d_note, d_contour, m->d_note_base.p, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_amp.p,
+                       m->d_bend_off.p, m->d_bends.p, (int)nc, bc > 0 ? 1 : 0, m->d_gauss, st);
+  }
+  CKL();
+  m->launches += 1;
+  CK(cudaMemcpyAsync(notes->amplitude + note0, m->d_amp.p, sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
+  if (bc > 0) CK(cudaMemcpyAsync(notes->bends + bend0, m->d_bends.p, sizeof(int) * bc, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+// BP_OK, or BP_E_CAPACITY with bp_last_required, once a grid call that returns its notes has run every chunk.
+int grid_notes_result(const std::string& api, const GridNotes& g) {
+  if (!g.notes_fit)
+    return g_need_notes = g.n_notes, fail(BP_E_CAPACITY, api + ": note_capacity too small, need " + std::to_string(g.n_notes));
+  if (!g.bends_fit)
+    return g_need_bends = g.n_bends, fail(BP_E_CAPACITY, api + ": bend_capacity too small, need " + std::to_string(g.n_bends));
+  return BP_OK;
+}
+
 // ---- scoring (bp_score_*) ----------------------------------------------------------------------------------------------
 
 int check_score_params(const std::string& api, const bp_score_params_t* sp) {
@@ -793,8 +880,8 @@ struct Pack {
   }
 };
 
-// The references of n sets, sorted by (bucket, onset) within each set, into `pk`; offsets of the sections in `o[5]`
-// (note_off, onset, offset, log2_hz, bucket); the range of buckets into tol.
+// The references of n sets, sorted by (bucket, onset) within each set, into `pk`; offsets of the sections in `o[6]`
+// (note_off, onset, offset, log2_hz, bucket, index within its set before sorting); the range of buckets into tol.
 void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol) {
   const long long R = s->note_off[n];
   std::vector<long long> idx(R);
@@ -825,12 +912,63 @@ void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol
   o[2] = pk.add(off.data(), sizeof(double) * R);
   o[3] = pk.add(l2.data(), sizeof(double) * R);
   o[4] = pk.add(bsorted.data(), sizeof(int) * R);
+  std::vector<int> orig(R);
+  for (int i = 0; i < n; ++i)
+    for (long long j = s->note_off[i]; j < s->note_off[i + 1]; ++j) orig[j] = (int)(idx[j] - s->note_off[i]);
+  o[5] = pk.add(orig.data(), sizeof(int) * R);
 }
 
 ScoreRefs refs_at(const unsigned char* d, const size_t* o) {
   return ScoreRefs{reinterpret_cast<const long long*>(d + o[0]), reinterpret_cast<const double*>(d + o[1]),
                    reinterpret_cast<const double*>(d + o[2]), reinterpret_cast<const double*>(d + o[3]),
                    reinterpret_cast<const int*>(d + o[4])};
+}
+
+// Matching workspace per launch (include/bp_b200.h, bp_match_grid_*): consecutive pairs share a launch while their
+// workspace stays within this; a pair that needs more runs alone.
+constexpr long long kMatchWorkBytes = 2LL << 30;
+
+// mir_eval's matchings of n_pairs pairs (pair q = setting * n_files + file; its estimates from E, est_off[q] .. est_off[q
+// + 1] on the host, against file q % n_files's references [ref_off[f], ref_off[f + 1]) of sr) into d_match [n_pairs /
+// n_files][2][n_refs] (estimate index or -1): one count launch, then one match launch per range of pairs whose workspace
+// fits kMatchWorkBytes.
+int match_pairs(bp_model* m, const std::string& api, const ScoreRefs& sr, const int* r_orig, const ScoreEst& E,
+                const ScoreTol& tol, int n_files, long long n_pairs, const std::vector<long long>& est_off,
+                const int64_t* ref_off, long long n_refs, int* d_match, cudaStream_t st) {
+  CK(cudaMemsetAsync(d_match, 0xff, sizeof(int) * 2 * (n_pairs / n_files) * n_refs, st));
+  CK(m->match_edges.reserve((size_t)n_pairs));
+  launch_match_count(sr, E, tol, n_files, n_pairs, m->match_edges.p, st);
+  CKL();
+  m->launches += 1;
+  std::vector<long long> edges(n_pairs), off(n_pairs + 1);
+  CK(cudaMemcpyAsync(edges.data(), m->match_edges.p, sizeof(long long) * n_pairs, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  off[0] = 0;
+  for (long long q = 0; q < n_pairs; ++q) {
+    const long long n_est = est_off[q + 1] - est_off[q], n_ref = ref_off[q % n_files + 1] - ref_off[q % n_files];
+    if (edges[q] > INT_MAX)
+      return fail(BP_E_INVALID, api + ": pair " + std::to_string(q) + " (file " + std::to_string(q % n_files) +
+                                    "): more than 2^31 - 1 hits");
+    off[q + 1] = off[q] + (n_est > 0 && n_ref > 0 ? 2 * match_pass_ints(n_est, n_ref, edges[q]) : 0);
+  }
+  std::vector<long long> cut{0};  // ranges [cut[k], cut[k + 1])
+  long long most = 0;
+  for (long long q0 = 0; q0 < n_pairs;) {
+    long long q1 = q0 + 1;
+    while (q1 < n_pairs && 4 * (off[q1 + 1] - off[q0]) <= kMatchWorkBytes) ++q1;
+    most = std::max(most, off[q1] - off[q0]);
+    cut.push_back(q0 = q1);
+  }
+  CK(m->match_off.reserve((size_t)n_pairs + 1));
+  CK(m->match_ws.reserve((size_t)most + 1));
+  CK(cudaMemcpyAsync(m->match_off.p, off.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
+  const MatchWork w{m->match_ws.p, m->match_off.p, m->match_edges.p, r_orig, d_match, n_refs};
+  for (size_t k = 0; k + 1 < cut.size(); ++k) {
+    launch_match(sr, E, tol, w, n_files, cut[k], cut[k + 1], st);
+    CKL();
+    m->launches += 1;
+  }
+  return BP_OK;
 }
 
 }  // namespace
@@ -954,6 +1092,8 @@ void bp_model_destroy(bp_model_t* m) {
   m->note_count.release(); m->slot_start.release(); m->slot_end.release(); m->slot_pitch.release();
   m->overflow.release(); m->d_note_off.release(); m->d_start.release(); m->d_end.release(); m->d_pitch.release();
   m->d_bend_off.release(); m->d_bends.release(); m->d_onset64.release();
+  m->match_edges.release(); m->match_off.release(); m->match_est_off.release(); m->match_ws.release();
+  m->match_out.release();
   m->yhl.release();
   m->chl.release();
   m->cqt_wtc.release();
@@ -1795,77 +1935,13 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
     return fail(BP_E_INVALID, api + ": null posteriorgram");
   DeviceGuard g(m->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  long long n_notes = 0, n_bends = 0;  // over the grid so far
-  bool notes_fit = true, bends_fit = true;
+  GridNotes gn;  // over the grid so far
   rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
                           const std::vector<int>& counts, const std::vector<long long>&) -> int {
-    const long long n_pairs = (long long)P * n_files;
-    // ---- note offsets; past the note capacity only the counting goes on (bp_last_required totals the whole grid)
-    const long long note0 = n_notes;
-    for (long long q = 0; q < n_pairs; ++q) {
-      n_notes += counts[q];
-      if (n_notes > notes->note_capacity) notes_fit = false;
-      if (notes_fit) notes->note_off[p0 * n_files + q + 1] = (int32_t)n_notes;
-    }
-    const long long nc = n_notes - note0;  // notes of this chunk
-    if (!notes_fit || nc == 0) return BP_OK;
-    if (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude)
-      return fail(BP_E_INVALID, api + ": notes arrays missing");
-    std::vector<int> noff(n_pairs + 1);  // chunk-relative
-    for (long long q = 0; q <= n_pairs; ++q) noff[q] = (int)(notes->note_off[p0 * n_files + q] - note0);
-    CK(m->d_note_off.reserve((size_t)n_pairs + 1));
-    CK(m->d_start.reserve((size_t)nc));
-    CK(m->d_end.reserve((size_t)nc));
-    CK(m->d_pitch.reserve((size_t)nc));
-    CK(m->d_amp.reserve((size_t)nc));
-    CK(m->d_note_base.reserve((size_t)nc));
-    CK(m->d_bend_off.reserve((size_t)nc + 1));
-    CK(cudaMemcpyAsync(m->d_note_off.p, noff.data(), sizeof(int) * (n_pairs + 1), cudaMemcpyHostToDevice, st));
-    compact_notes_kernel<<<dim3(n_files, P), 128, 0, st>>>(m->d_frame_off.p, m->d_slot_off.p, m->d_note_off.p,
-                                                           m->slot_start.p, m->slot_end.p, m->slot_pitch.p, m->d_start.p,
-                                                           m->d_end.p, m->d_pitch.p, m->d_note_base.p);
-    CKL();
-    m->launches += 1;
-    CK(cudaMemcpyAsync(notes->start_frame + note0, m->d_start.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(notes->end_frame + note0, m->d_end.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(notes->pitch_midi + note0, m->d_pitch.p, sizeof(int) * nc, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    // ---- bend offsets: each setting's own include_pitch_bends (without: empty ranges, as bp_decode_device leaves them)
-    const long long bend0 = n_bends;
-    for (int s = 0; s < P; ++s) {
-      const bool with = params[p0 + s].include_pitch_bends != 0;
-      for (long long j = note0 + noff[(long long)s * n_files]; j < note0 + noff[(long long)(s + 1) * n_files]; ++j) {
-        if (with) n_bends += notes->end_frame[j] - notes->start_frame[j];
-        if (n_bends > 0x7fffffffLL) return fail(BP_E_CAPACITY, api + ": more than 2^31 pitch-bend values");
-        notes->bend_off[j + 1] = (int32_t)n_bends;
-      }
-    }
-    if (n_bends > notes->bend_capacity) bends_fit = false;
-    if (!bends_fit) return BP_OK;
-    const long long bc = n_bends - bend0;  // bends of this chunk
-    if (bc > 0 && !notes->bends) return fail(BP_E_INVALID, api + ": bends array missing");
-    std::vector<int> boff(nc + 1);
-    for (long long j = 0; j <= nc; ++j) boff[j] = (int)(notes->bend_off[note0 + j] - bend0);
-    CK(m->d_bends.reserve((size_t)bc + 1));
-    CK(cudaMemcpyAsync(m->d_bend_off.p, boff.data(), sizeof(int) * (nc + 1), cudaMemcpyHostToDevice, st));
-    {
-      ProfScope ps(m, 6, st);
-      launch_note_finish(d_note, d_contour, m->d_note_base.p, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_amp.p,
-                         m->d_bend_off.p, m->d_bends.p, (int)nc, bc > 0 ? 1 : 0, m->d_gauss, st);
-    }
-    CKL();
-    m->launches += 1;
-    CK(cudaMemcpyAsync(notes->amplitude + note0, m->d_amp.p, sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
-    if (bc > 0) CK(cudaMemcpyAsync(notes->bends + bend0, m->d_bends.p, sizeof(int) * bc, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return BP_OK;
+    return grid_chunk_notes(m, api, d_note, d_contour, params, true, n_files, p0, P, counts, notes, gn, st);
   });
   if (rc) return rc;
-  if (!notes_fit)
-    return g_need_notes = n_notes, fail(BP_E_CAPACITY, api + ": note_capacity too small, need " + std::to_string(n_notes));
-  if (!bends_fit)
-    return g_need_bends = n_bends, fail(BP_E_CAPACITY, api + ": bend_capacity too small, need " + std::to_string(n_bends));
-  return BP_OK;
+  return grid_notes_result(api, gn);
 }
 
 int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
@@ -1919,9 +1995,9 @@ int bp_frame_times(int64_t n, double* out) {
 
 namespace {
 
-// Everything bp_score_grid_* check before anything is enqueued, in addition to check_grid_args.
+// Everything bp_score_grid_* and bp_match_grid_* check before anything is enqueued, in addition to check_grid_args.
 int check_score_grid(const std::string& api, int n_files, int n_params, const bp_note_set_t* refs,
-                     const bp_score_params_t* sp, const double* est_log2_hz, const int64_t* h_counts) {
+                     const bp_score_params_t* sp, const double* est_log2_hz, const void* h_counts) {
   int rc = check_score_params(api, sp);
   if (rc || n_files == 0 || n_params == 0) return rc;
   if (!h_counts || !est_log2_hz) return fail(BP_E_INVALID, api + ": bad argument");
@@ -1952,7 +2028,7 @@ int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onse
   // one upload per call: the references, the seconds of every frame a note can start or end on, the log2(Hz) table
   ScoreTol tol = score_tol(*sp);
   Pack pk;
-  size_t o_ref[5];
+  size_t o_ref[6];
   pack_refs(refs, n_files, pk, o_ref, tol);
   std::vector<double> frame_t(max_t + 1);
   bp_frame_times(max_t + 1, frame_t.data());
@@ -2025,7 +2101,7 @@ int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
   if (rc) return rc;
   ScoreTol tol = score_tol(*sp);
   Pack pk;
-  size_t o_ref[5];
+  size_t o_ref[6];
   pack_refs(refs, n_items, pk, o_ref, tol);
   const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
   const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
@@ -2050,6 +2126,141 @@ int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
   CKL();
   m->launches += 1;
   CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_items, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match,
+                         void* stream) {
+  const std::string api = "bp_match_grid_device";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_match);
+  if (rc) return rc;
+  if (!notes || !notes->note_off || !notes->bend_off) return fail(BP_E_INVALID, api + ": notes arrays missing");
+  g_need_notes = g_need_bends = 0;
+  notes->note_off[0] = 0;
+  notes->bend_off[0] = 0;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long total_frames = foff[n_files];
+  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  long long max_t = 0;
+  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
+  // one upload per call: the references, the seconds of every frame a note can start or end on, the log2(Hz) table
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[6];
+  pack_refs(refs, n_files, pk, o_ref, tol);
+  std::vector<double> frame_t(max_t + 1);
+  bp_frame_times(max_t + 1, frame_t.data());
+  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
+  const size_t o_l2 = pk.add(est_log2_hz, sizeof(double) * 128);
+  const long long n_refs = refs->note_off[n_files];
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
+  const int* r_orig = reinterpret_cast<const int*>(m->score_in.p + o_ref[5]);
+  GridNotes gn;  // over the grid so far
+  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>& counts, const std::vector<long long>&) -> int {
+    const long long note0 = gn.n_notes, n_pairs = (long long)P * n_files;
+    int rc = grid_chunk_notes(m, api, d_note, nullptr, params, false, n_files, p0, P, counts, notes, gn, st);
+    if (rc || !gn.notes_fit || n_refs == 0) return rc;
+    int32_t* out = h_match + 2 * p0 * n_refs;
+    if (gn.n_notes == note0) {  // no estimated note in this chunk
+      std::fill(out, out + 2 * P * n_refs, -1);
+      return BP_OK;
+    }
+    // the compacted notes: pair q's are [est_off[q], est_off[q + 1]) of m->d_start / d_end / d_pitch
+    std::vector<long long> est_off(n_pairs + 1);
+    for (long long q = 0; q <= n_pairs; ++q) est_off[q] = notes->note_off[p0 * n_files + q] - note0;
+    CK(m->match_est_off.reserve((size_t)n_pairs + 1));
+    CK(cudaMemcpyAsync(m->match_est_off.p, est_off.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice,
+                       st));
+    CK(m->match_out.reserve((size_t)(2 * P * n_refs)));
+    ScoreEst e{};
+    e.off = m->match_est_off.p;
+    e.start = m->d_start.p;
+    e.end = m->d_end.p;
+    e.pitch = m->d_pitch.p;
+    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
+    e.log2_midi = reinterpret_cast<const double*>(m->score_in.p + o_l2);
+    rc = match_pairs(m, api, sr, r_orig, e, tol, n_files, n_pairs, est_off, refs->note_off, n_refs, m->match_out.p, st);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(out, m->match_out.p, sizeof(int) * 2 * P * n_refs, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return BP_OK;
+  });
+  if (rc) return rc;
+  return grid_notes_result(api, gn);
+}
+
+int bp_match_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                       int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                       const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match) {
+  const std::string api = "bp_match_grid_host";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_match);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0)
+    return bp_match_grid_device(m, nullptr, nullptr, h_frame_off, n_files, params, n_params, refs, sp, est_log2_hz,
+                                notes, h_match, m->stream);
+  DeviceGuard g(m->device);
+  const int64_t total = h_frame_off[n_files];
+  cudaStream_t st = m->stream;
+  rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {  // uploaded once for the whole grid
+    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
+    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+  }
+  return bp_match_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, sp,
+                              est_log2_hz, notes, h_match, st);
+}
+
+int bp_match_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
+                        const bp_score_params_t* sp, int32_t* h_match) {
+  const std::string api = "bp_match_notes_host";
+  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  int rc = check_score_params(api, sp);
+  if (rc || n_items == 0) return rc;
+  if (!h_match) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_note_set(api, "estimates", "item", est, n_items);
+  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items);
+  if (rc) return rc;
+  const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
+  if (n_refs == 0) return BP_OK;
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[6];
+  pack_refs(refs, n_items, pk, o_ref, tol);
+  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
+  const size_t o_eon = pk.add(est->onset_s, sizeof(double) * n_est);
+  const size_t o_eoffs = pk.add(est->offset_s, sizeof(double) * n_est);
+  const size_t o_el2 = pk.add(est->log2_hz, sizeof(double) * n_est);
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(m->match_out.reserve((size_t)(2 * n_refs)));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = m->score_in.p;
+  ScoreEst e{};
+  e.off = reinterpret_cast<const long long*>(d + o_eoff);
+  e.onset = reinterpret_cast<const double*>(d + o_eon);
+  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
+  e.log2hz = reinterpret_cast<const double*>(d + o_el2);
+  const std::vector<long long> est_off(est->note_off, est->note_off + n_items + 1);
+  rc = match_pairs(m, api, refs_at(d, o_ref), reinterpret_cast<const int*>(d + o_ref[5]), e, tol, n_items, n_items,
+                   est_off, refs->note_off, n_refs, m->match_out.p, st);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h_match, m->match_out.p, sizeof(int) * 2 * n_refs, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
 }

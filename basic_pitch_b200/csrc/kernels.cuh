@@ -348,6 +348,28 @@ struct ScoreWork {       // int workspace: 2 per reference and setting, 4 per es
 void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
                         long long n_pairs, long long* counts, cudaStream_t st);
 
+// mir_eval's matching pair for pair (bp_match_*).  Int workspace of one (pair, pass) with N estimated notes, R
+// references and M hits without the offset test (the with-offset graph is a subgraph): adjacency offsets and lists,
+// the preds lists (node estimate, next), per reference its list head / tail, preds state, the new_layer order and the
+// unmatched list, the recursion stack (3 per frame, at most R + 1 frames), per estimate pred, key order and two layers.
+__host__ __device__ inline long long match_pass_ints(long long n_est, long long n_ref, long long n_edges) {
+  return 3 * n_edges + 5 * n_est + 8 * n_ref + 8;
+}
+struct MatchWork {
+  int* ws;                 // pair q, pass p: ws + (off[q] - off[q0]) + p * match_pass_ints(..) of pair q
+  const long long* off;    // [n_pairs + 1] int offsets of every pair's workspace (2 passes), chunk-wide
+  const long long* edges;  // [n_pairs] hits without the offset test
+  const int* r_orig;       // [n_ref_total] index of sorted reference k within its set
+  int* match;              // [n_settings][2][n_ref_total]: estimate index or -1, in the caller's reference order
+  long long n_ref_total;
+};
+// One launch: edges[q] = hits without the offset test of pair q = setting * n_files + file.
+void launch_match_count(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, int n_files, long long n_pairs,
+                        long long* edges, cudaStream_t st);
+// One launch: the matchings of pairs [q0, q1), both passes (one thread per pair and pass); W.match must hold -1.
+void launch_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const MatchWork& W, int n_files,
+                  long long q0, long long q1, cudaStream_t st);
+
 // ---- score_frames.cu: frame-level multi-pitch counts (bp_score_frames_grid_*, bp_score_multipitch_host,
 // bp_score_salience_grid_*) -------------------------------------------------------------------------------------------
 constexpr int kFrameCounts = 7;  // n_ref, n_est, tp, tp_chroma, sum min, miss, false alarms

@@ -7,6 +7,9 @@
 // found by scanning the semitone buckets within reach of the pitch tolerance and binary-searching the onset window, and
 // the exact predicates decide.  The maximum matching is a greedy pass followed by one augmenting-path search (Kuhn) per
 // estimated note the greedy pass left free, with an explicit stack in global workspace.
+//
+// The match kernels (bp_match_*) go further: they store each pair's hit graph and reproduce mir_eval's matching itself,
+// pair for pair, for one (pair, pass) per thread.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -182,7 +185,215 @@ __global__ void __launch_bounds__(kScoreThreads) score_match_kernel(ScoreRefs R,
     out[2 + pass] = max_matching(c, E, ebase, n_est, pass == 1, rw, rw + c.n_ref, ew, ew + n_est);
 }
 
+// ---- mir_eval's matching pair for pair (bp_match_*) ------------------------------------------------------------------
+// mir_eval.transcription.match_notes builds G = {estimate: [references it hits]} from the row-major np.where of the hit
+// matrix and runs util._bipartite_match (Hopcroft-Karp, Eppstein's PADS) on it, walking Python dicts in insertion order.
+// The thread below rebuilds G with arrays (lists in ascending reference index, keys ordered by (first reference, j)) and
+// runs the same steps in the same order, with an explicit stack for the recursion; include/bp_b200.h states them.
+
+// file's references, which start at r0 = R.off[file]
+__device__ __forceinline__ PairCtx pair_ctx(const ScoreRefs& R, const ScoreTol& tol, int file, long long r0) {
+  PairCtx c;
+  c.r_on = R.onset + r0;
+  c.r_off = R.offset + r0;
+  c.r_l2 = R.log2hz + r0;
+  c.r_bucket = R.bucket + r0;
+  c.n_ref = (int)(R.off[file + 1] - r0);
+  c.tol = tol;
+  return c;
+}
+
+__global__ void __launch_bounds__(kScoreThreads) match_count_kernel(ScoreRefs R, ScoreEst E, ScoreTol tol, int n_files,
+                                                                    long long n_pairs, long long* __restrict__ edges) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n_pairs) return;
+  const int file = (int)(q % n_files);
+  const long long r0 = R.off[file];
+  const PairCtx c = pair_ctx(R, tol, file, r0);
+  const long long ebase = E.off[q];
+  const int n_est = E.count ? E.count[q] : (int)(E.off[q + 1] - ebase);
+  long long m = 0;
+  for (int j = 0; c.n_ref > 0 && j < n_est; ++j) {
+    const EstNote en = est_note(E, ebase, j);
+    int db = -c.tol.k_buckets, pos = -1;
+    while (next_hit(c, en, db, pos, false)) ++m;
+  }
+  edges[q] = m;
+}
+
+constexpr int kPredUnmatched = -1;  // pred[u] of an estimate of the first layer (the `unmatched` flag value)
+constexpr int kPredAbsent = -2;     // u not in pred
+
+// Thread t of the launch: pair q0 + t / 2, pass t % 2 (0: hits without the offset test, 1: with it).  Every thread
+// walks its own graph serially; a minimum of one CTA per SM lets ptxas keep the layout pointers in registers (89, no
+// spills) instead of spilling them at the 80 it picks for the default occupancy target.
+__global__ void __launch_bounds__(kScoreThreads, 1) match_kernel(ScoreRefs R, ScoreEst E, ScoreTol tol, MatchWork W,
+                                                              int n_files, long long q0, long long q1) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long q = q0 + (t >> 1);
+  if (q >= q1) return;
+  const int pass = (int)(t & 1);
+  const int file = (int)(q % n_files);
+  const long long r0 = R.off[file];
+  const PairCtx c = pair_ctx(R, tol, file, r0);
+  const long long ebase = E.off[q];
+  const int n_est = E.count ? E.count[q] : (int)(E.off[q + 1] - ebase);
+  const int n_ref = c.n_ref;
+  if (n_ref == 0 || n_est == 0) return;
+  const long long M = W.edges[q];
+  int* w = W.ws + (W.off[q] - W.off[q0]) + pass * match_pass_ints(n_est, n_ref, M);
+  int* adj_off = w;                 // [N + 1]
+  int* adj = adj_off + n_est + 1;   // [M]
+  int* node_u = adj + M;            // [M]
+  int* node_nx = node_u + M;        // [M]
+  int* head = node_nx + M;          // [R + 1], first the counts of the key sort
+  int* tail = head + n_ref + 1;     // [R]
+  int* pst = tail + n_ref;          // [R] preds state: 2 phase + 1 in this layer's new_layer, 2 phase + 2 in preds
+  int* order = pst + n_ref;         // [R] new_layer's insertion order
+  int* unm = order + n_ref;         // [R]
+  int* stack = unm + n_ref;         // [3 (R + 1)] frames (reference, next node, estimate taken)
+  int* pred = stack + 3 * (n_ref + 1);  // [N]
+  int* keys = pred + n_est;         // [N]
+  int* lay = keys + n_est;          // [N]
+  int* nxt = lay + n_est;           // [N]
+  int* out = W.match + ((q / n_files) * 2 + pass) * W.n_ref_total + r0;
+  const int* orig = W.r_orig + r0;
+
+  // G: estimate j's references in ascending original index (insertion sort; the scan visits them by (bucket, onset))
+  int k = 0;
+  for (int j = 0; j < n_est; ++j) {
+    adj_off[j] = k;
+    const EstNote en = est_note(E, ebase, j);
+    int db = -c.tol.k_buckets, pos = -1;
+    while (next_hit(c, en, db, pos, pass == 1)) {
+      const int v = orig[pos];
+      int i = k++;
+      for (; i > adj_off[j] && adj[i - 1] > v; --i) adj[i] = adj[i - 1];
+      adj[i] = v;
+    }
+  }
+  adj_off[n_est] = k;
+  // keys: estimates with a hit, by (first reference, j) -- a counting sort on the first reference, stable in j
+  for (int v = 0; v <= n_ref; ++v) head[v] = 0;
+  for (int j = 0; j < n_est; ++j)
+    if (adj_off[j + 1] > adj_off[j]) ++head[adj[adj_off[j]] + 1];
+  for (int v = 1; v <= n_ref; ++v) head[v] += head[v - 1];
+  int n_keys = 0;
+  for (int j = 0; j < n_est; ++j)
+    if (adj_off[j + 1] > adj_off[j]) keys[head[adj[adj_off[j]]]++] = j, ++n_keys;
+  // greedy: each key takes the first reference of its list not yet matched
+  for (int a = 0; a < n_keys; ++a) {
+    const int u = keys[a];
+    for (int e = adj_off[u]; e < adj_off[u + 1]; ++e)
+      if (out[adj[e]] < 0) {
+        out[adj[e]] = u;
+        break;
+      }
+  }
+  for (int v = 0; v < n_ref; ++v) pst[v] = 0;
+  for (int phase = 1;; ++phase) {
+    const int in_new = 2 * phase + 1, in_preds = 2 * phase + 2;
+    for (int a = 0; a < n_keys; ++a) pred[keys[a]] = kPredUnmatched;
+    for (int v = 0; v < n_ref; ++v)
+      if (out[v] >= 0) pred[out[v]] = kPredAbsent;
+    int n_lay = 0;
+    for (int a = 0; a < n_keys; ++a)
+      if (pred[keys[a]] == kPredUnmatched) lay[n_lay++] = keys[a];
+    int n_unm = 0, n_node = 0;
+    // layering: the preds lists of this phase hold at most one node per hit, every estimate being in one layer at most
+    while (n_lay > 0 && n_unm == 0) {
+      int n_order = 0;
+      for (int a = 0; a < n_lay; ++a) {
+        const int u = lay[a];
+        for (int e = adj_off[u]; e < adj_off[u + 1]; ++e) {
+          const int v = adj[e];
+          if (pst[v] == in_preds) continue;
+          if (pst[v] != in_new) {
+            pst[v] = in_new;
+            head[v] = n_node;
+            order[n_order++] = v;
+          } else {
+            node_nx[tail[v]] = n_node;
+          }
+          node_u[n_node] = u;
+          node_nx[n_node] = -1;
+          tail[v] = n_node++;
+        }
+      }
+      n_lay = 0;
+      for (int a = 0; a < n_order; ++a) {
+        const int v = order[a];
+        pst[v] = in_preds;
+        const int u = out[v];
+        if (u >= 0) {
+          nxt[n_lay++] = u;
+          pred[u] = v;
+        } else {
+          unm[n_unm++] = v;
+        }
+      }
+      int* s = lay;
+      lay = nxt;
+      nxt = s;
+    }
+    if (n_unm == 0) break;
+    // recurse(v) for every unmatched v of the last layer; a frame resumes its list where it left it
+    for (int a = 0; a < n_unm; ++a) {
+      const int v0 = unm[a];
+      if (pst[v0] != in_preds) continue;
+      pst[v0] = 0;  // preds.pop(v)
+      stack[0] = v0, stack[1] = head[v0], stack[2] = -1;
+      int depth = 1;
+      while (depth > 0) {
+        int* f = stack + 3 * (depth - 1);
+        int node = f[1], child = -1;
+        bool found = false;
+        while (node >= 0) {
+          const int u = node_u[node];
+          node = node_nx[node];
+          const int pu = pred[u];
+          if (pu == kPredAbsent) continue;
+          pred[u] = kPredAbsent;
+          f[2] = u;
+          if (pu == kPredUnmatched) {
+            found = true;
+            break;
+          }
+          if (pst[pu] == in_preds) {  // recurse(pu); a reference no longer in preds returns False at once
+            child = pu;
+            break;
+          }
+        }
+        f[1] = node;
+        if (found) {  // every frame's reference takes the estimate it stands on
+          for (int d = 0; d < depth; ++d) out[stack[3 * d]] = stack[3 * d + 2];
+          break;
+        }
+        if (child < 0) {
+          --depth;
+          continue;
+        }
+        pst[child] = 0;
+        int* g = stack + 3 * depth++;
+        g[0] = child, g[1] = head[child], g[2] = -1;
+      }
+    }
+  }
+}
+
 }  // namespace
+
+void launch_match_count(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, int n_files, long long n_pairs,
+                        long long* edges, cudaStream_t st) {
+  const unsigned int blocks = (unsigned int)((n_pairs + kScoreThreads - 1) / kScoreThreads);
+  match_count_kernel<<<blocks, kScoreThreads, 0, st>>>(R, E, tol, n_files, n_pairs, edges);
+}
+
+void launch_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const MatchWork& W, int n_files,
+                  long long q0, long long q1, cudaStream_t st) {
+  const unsigned int blocks = (unsigned int)((2 * (q1 - q0) + kScoreThreads - 1) / kScoreThreads);
+  match_kernel<<<blocks, kScoreThreads, 0, st>>>(R, E, tol, W, n_files, q0, q1);
+}
 
 void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
                         long long n_pairs, long long* counts, cudaStream_t st) {

@@ -10,6 +10,11 @@ frames (`Model.score_frames_grid`, `Model.score_multipitch`, `inference.evaluate
 bp_score_frames_grid_* / bp_score_multipitch_host).  `frame_scores` turns them into the 14 numbers of
 mir_eval.multipitch.metrics (0.7), bit for bit.
 
+Matched pairs: the library also returns which estimated note mir_eval's matching pairs with each reference note
+(`Model.match_grid`, `Model.match_notes`; include/bp_b200.h, bp_match_*).  `matching_scores` turns one file's pairs into
+the average overlap ratio and the note scores with velocity (mir_eval.transcription_velocity), with mir_eval's own
+NumPy expressions; `inference.evaluate_velocity_grid` does this for a grid of settings.
+
 Posteriorgrams as multi-f0 estimates: `salience_to_multipitch` reads a contour (or note) posteriorgram under a
 threshold, peak picking and a frequency range as the series those metrics score (include/bp_b200.h,
 bp_score_salience_grid_*); `Model.score_salience_grid` / `inference.evaluate_salience_grid` score a grid of such
@@ -179,4 +184,80 @@ def note_scores(counts) -> Dict[str, np.ndarray]:
         out["mean"] = {k: (v.mean(axis=-1) if n else np.zeros(v.shape[:-1])) for k, v in out.items()}
     else:
         out["mean"] = {k: (v.mean() if v.size else np.float64(0.0)) for k, v in out.items()}
+    return out
+
+
+# Keys of `matching_scores`; each also exists with a "_no_offset" suffix (the pass without the offset test)
+MATCH_FIELDS = ("average_overlap_ratio", "velocity_precision", "velocity_recall", "velocity_f_measure",
+                "velocity_average_overlap_ratio")
+
+
+def note_velocities(amplitude) -> np.ndarray:
+    """The MIDI velocity the library writes for a note of this amplitude (note_events_to_midi, csrc/midi_events.h
+    velocity_of): int(np.round(np.float32(127) * amplitude)), in float32."""
+    return np.round(np.float32(127) * np.asarray(amplitude, np.float32)).astype(np.int64)
+
+
+def check_velocities(velocities, what: str = "velocities") -> np.ndarray:
+    """float64 copy of one file's velocities; ValueError naming the first that is not finite or is < 0 (mir_eval's
+    transcription_velocity.validate rejects them)."""
+    v = np.asarray(velocities, np.float64).reshape(-1)
+    bad = np.flatnonzero(~(np.isfinite(v) & (v >= 0)))
+    if len(bad):
+        raise ValueError(f"{what} note {int(bad[0])}: velocity must be finite and >= 0, got {v[bad[0]]}")
+    return v
+
+
+def _overlap_ratio(ref_iv, est_iv, r, e) -> float:
+    """transcription.average_overlap_ratio over the pairs (r[k], e[k]), in that order; 0 without pairs."""
+    if len(r) == 0:
+        return 0.0
+    a, b = ref_iv[r], est_iv[e]
+    return np.mean((np.minimum(a[:, 1], b[:, 1]) - np.maximum(a[:, 0], b[:, 0])) /
+                   (np.maximum(a[:, 1], b[:, 1]) - np.minimum(a[:, 0], b[:, 0])))
+
+
+def matching_scores(ref_intervals, ref_velocities, est_intervals, est_velocities, match,
+                    velocity_tolerance: float = 0.1) -> Dict[str, np.float64]:
+    """The scores of one file that depend on which pairs mir_eval 0.7 matches, from the library's matchings.
+
+    ref_intervals (n_ref, 2) and est_intervals (n_est, 2) in seconds; velocities finite and >= 0 (an estimated note's is
+    `note_velocities` of its amplitude); match (2, n_ref) as `Model.match_grid` / `match_notes` return it: per reference
+    note the estimate index or -1, row 0 without and row 1 with the offset test.  Returns float64 values for
+    average_overlap_ratio (transcription.precision_recall_f1_overlap's fourth value) and velocity_precision,
+    velocity_recall, velocity_f_measure, velocity_average_overlap_ratio (transcription_velocity.precision_recall_f1_overlap,
+    velocity_tolerance as there), each with offsets and with a "_no_offset" suffix without.
+
+    The velocity step is mir_eval's: reference velocities become (v - min) / max(1, max - min); a least-squares line
+    np.linalg.lstsq([est_v, 1], ref_v) through the matched pairs rescales the estimated ones; a pair is kept when
+    |slope est_v + intercept - ref_v| < velocity_tolerance.  Every value is 0 when either side is empty."""
+    ref_iv = np.asarray(ref_intervals, np.float64).reshape(-1, 2)
+    est_iv = np.asarray(est_intervals, np.float64).reshape(-1, 2)
+    rv = check_velocities(ref_velocities, "references")
+    ev = check_velocities(est_velocities, "estimates")
+    m = np.asarray(match, np.int64).reshape(2, -1)
+    n_ref, n_est = len(rv), len(ev)
+    if len(ref_iv) != n_ref or len(est_iv) != n_est or m.shape[1] != n_ref:
+        raise ValueError(f"{len(ref_iv)} reference intervals, {n_ref} velocities, {m.shape[1]} matches; "
+                         f"{len(est_iv)} estimated intervals, {n_est} velocities")
+    out: Dict[str, np.float64] = {}
+    for suffix, row in (("", m[1]), ("_no_offset", m[0])):
+        r = np.flatnonzero(row >= 0)  # sorted(matching.items()): ascending reference index
+        e = row[r]
+        if len(r) and (e.max() >= n_est):
+            raise ValueError(f"match refers to estimate {int(e.max())} of {n_est}")
+        vals = dict.fromkeys(MATCH_FIELDS, np.float64(0.0))
+        if n_ref and n_est:
+            vals["average_overlap_ratio"] = np.float64(_overlap_ratio(ref_iv, est_iv, r, e))
+            if len(r):
+                v_min, v_max = np.min(rv), np.max(rv)
+                rn = (rv - v_min) / float(max(1, v_max - v_min))
+                slope, intercept = np.linalg.lstsq(np.vstack([ev[e], np.ones(len(e))]).T, rn[r])[0]
+                keep = np.abs(slope * ev[e] + intercept - rn[r]) < velocity_tolerance
+                r, e = r[keep], e[keep]
+            p, rc = float(len(r)) / n_est, float(len(r)) / n_ref
+            vals["velocity_precision"], vals["velocity_recall"] = np.float64(p), np.float64(rc)
+            vals["velocity_f_measure"] = np.float64(0.0 if p == 0 and rc == 0 else 2 * p * rc / (p + rc))
+            vals["velocity_average_overlap_ratio"] = np.float64(_overlap_ratio(ref_iv, est_iv, r, e))
+        out.update({k + suffix: v for k, v in vals.items()})
     return out

@@ -419,6 +419,52 @@ class Model:
         self._lib.bp_score_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(counts))
         return counts
 
+    def match_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray], settings: Sequence[Dict[str, Any]],
+                   references: Sequence[Tuple[np.ndarray, np.ndarray]], **tolerances):
+        """mir_eval 0.7's note matching, pair for pair, of a batch of files decoded under every setting of a grid, in ONE
+        library call (`bp_match_grid_host`).  Arguments as `score_grid` (include_pitch_bends is ignored).
+
+        Returns (res, match): res[setting][file] the note arrays `decode_grid` gives for that setting (amplitudes, no
+        pitch bends); match[setting][file] int32 (2, n_ref): per reference note, in the caller's order, the index of the
+        estimated note in res[setting][file] it is matched to, or -1; row 0 without, row 1 with the offset test.
+        mir_eval's matching depends on the order of the estimate list: here it is the decode's order; `match_notes`
+        takes another.  `evaluate.matching_scores` turns a file's matchings into its overlap and velocity scores."""
+        n_files, n_params = len(notes), len(settings)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference sets")
+        ps = self._grid_params(settings)
+        sp = self._score_params(tolerances)
+        refs, keep = self._note_set(references, "references")
+        foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+        roff = keep[0]
+        h_match = np.full((max(n_params, 1), 2, max(int(roff[-1]), 1)), -1, np.int32)
+        arrs = self._with_capacity(
+            n_files, int(foff[-1]),
+            lambda nt: self._lib.bp_match_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params,
+                                                    C.byref(refs), C.byref(sp), _ptr(evaluate.EST_LOG2_HZ), C.byref(nt),
+                                                    _ptr(h_match)),
+            n_params=n_params,
+        )
+        flat = self._split_notes(arrs, n_params * n_files)
+        res = [flat[k * n_files : (k + 1) * n_files] for k in range(n_params)]
+        match = [[h_match[k, :, roff[i] : roff[i + 1]].copy() for i in range(n_files)] for k in range(n_params)]
+        return res, match
+
+    def match_notes(self, estimates: Sequence[Tuple[np.ndarray, np.ndarray]],
+                    references: Sequence[Tuple[np.ndarray, np.ndarray]], **tolerances) -> List[np.ndarray]:
+        """mir_eval 0.7's note matching of item i's estimated notes, in the order given, against item i's reference
+        notes (`bp_match_notes_host`), both as (intervals (n, 2) in seconds, pitches (n,) in Hz).  Returns per item an
+        int32 (2, n_ref) array as `match_grid`."""
+        if len(estimates) != len(references):
+            raise ValueError(f"{len(estimates)} estimated but {len(references)} reference sets")
+        sp = self._score_params(tolerances)
+        est, keep_e = self._note_set(estimates, "estimates")
+        refs, keep_r = self._note_set(references, "references")
+        roff = keep_r[0]
+        h_match = np.full((2, max(int(roff[-1]), 1)), -1, np.int32)
+        self._lib.bp_match_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(h_match))
+        return [h_match[:, roff[i] : roff[i + 1]].copy() for i in range(len(estimates))]
+
     # ------------------------------------------------------------------ frame-level scores
     @staticmethod
     def _multipitch_set(series: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]], what: str):
@@ -925,6 +971,67 @@ def evaluate_grid(
     outs = model.run_inference_arrays(clips)
     counts = model.score_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references, **tolerances)
     return counts, evaluate.note_scores(counts)
+
+
+def evaluate_velocity_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, np.ndarray, np.ndarray]],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    velocity_tolerance: float = 0.1,
+    **tolerances,
+):
+    """Note-level scores with velocity and overlap of a batch of annotated recordings under every setting of a grid
+    (addition; no reference counterpart): the model runs once over the batch, every (setting, file) is decoded and
+    matched as mir_eval 0.7 matches it on the device in one `bp_match_grid_host` call, and `evaluate.matching_scores`
+    turns each matching into mir_eval's floats on the host.  `audio`, `settings` and tolerances as in `evaluate_grid`;
+    `references[i]` is file i's (intervals (n, 2) in seconds, pitches (n,) in Hz, velocities (n,), finite and >= 0).
+    An estimated note's velocity is the one the MIDI writer gives it (`evaluate.note_velocities`).
+
+    Returns (counts (n_settings, n_files, 4) as `evaluate_grid`, derived from the matchings; scores), scores holding
+    `evaluate.note_scores(counts)` and every key of `evaluate.matching_scores` as (n_settings, n_files) float64 arrays,
+    with "mean" over files as in `note_scores`."""
+    refs = []
+    for i, ref in enumerate(references):
+        if len(ref) != 3:
+            raise ValueError(f"references[{i}]: need (intervals, pitches_hz, velocities)")
+        iv, hz, vel = ref
+        vel = evaluate.check_velocities(vel, f"references[{i}]")
+        if len(vel) != len(np.asarray(hz).reshape(-1)):
+            raise ValueError(f"references[{i}]: {len(vel)} velocities for {len(np.asarray(hz).reshape(-1))} notes")
+        refs.append((iv, hz, vel))
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    outs = model.run_inference_arrays(clips)
+    res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode,
+                                  [(iv, hz) for iv, hz, _ in refs], **tolerances)
+    n_params, n_files = len(settings), len(clips)
+    counts = np.zeros((n_params, n_files, 4), np.int64)
+    keys = [k + s for s in ("", "_no_offset") for k in evaluate.MATCH_FIELDS]
+    extra = {k: np.zeros((n_params, n_files)) for k in keys}
+    for i, o in enumerate(outs):
+        t = infer.model_frames_to_time(o["note"].shape[0] + 1)
+        ref_iv = np.asarray(refs[i][0], np.float64).reshape(-1, 2)
+        for k in range(n_params):
+            r = res[k][i]
+            est_iv = np.stack([t[r["start"]], t[r["end"]]], 1)
+            counts[k, i] = (len(ref_iv), len(r["start"]), (match[k][i][0] >= 0).sum(), (match[k][i][1] >= 0).sum())
+            vals = evaluate.matching_scores(ref_iv, refs[i][2], est_iv, evaluate.note_velocities(r["amp"]), match[k][i],
+                                            velocity_tolerance)
+            for key in keys:
+                extra[key][k, i] = vals[key]
+    scores = evaluate.note_scores(counts)
+    scores.update(extra)
+    scores["mean"].update({k: (v.mean(axis=-1) if n_files else np.zeros(n_params)) for k, v in extra.items()})
+    return counts, scores
 
 
 def evaluate_frames_grid(

@@ -223,6 +223,66 @@ int bp_score_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
 int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
                         const bp_score_params_t* score, int64_t* h_counts);
 
+/* ---- mir_eval's note matching pair for pair ------------------------------------------------------------------------
+ * No reference counterpart: which estimated note mir_eval.transcription 0.7 (match_notes, strict=False) matches to each
+ * reference note, with and without offsets.  The average overlap ratio and the note scores with velocity
+ * (mir_eval.transcription_velocity) depend on these pairs, not only on their number; the host turns them into floats
+ * with mir_eval's own NumPy expressions (basic_pitch_b200/evaluate.py, matching_scores).
+ * Hits are those of bp_score_* above.  With the references and estimates of one (setting, file) or item:
+ *  1. Graph (match_notes): G maps each estimate j with at least one hit to the list of references it hits, in ascending
+ *     reference index; its keys are ordered by (smallest reference index hitting j, then j), the order in which j first
+ *     appears in the row-major np.where of the hit matrix.  Indices are the caller's order within the set (not the
+ *     (bucket, onset) order the library sorts references into), so the matching depends on the order of the estimate
+ *     list: grid estimates are in the order bp_decode_grid_* returns them; callers wanting another order pass explicit
+ *     notes to bp_match_notes_host.
+ *  2. Matching (util._bipartite_match, Hopcroft-Karp), with "for x in d" walking dict d in insertion order:
+ *       matching = {}                                        # reference v -> estimate u
+ *       for u in G: for v in G[u]: if v not in matching: matching[v] = u; break
+ *       loop:
+ *         preds = {}; unmatched = []
+ *         pred = {u: UNMATCHED for u in G}; del pred[matching[v]] for every v in matching
+ *         layer = list(pred)                                 # the free estimates, in key order
+ *         while layer and not unmatched:
+ *           new_layer = {}                                   # v -> [u, ...], insertion-ordered
+ *           for u in layer: for v in G[u]: if v not in preds: new_layer.setdefault(v, []).append(u)
+ *           layer = []
+ *           for v in new_layer:
+ *             preds[v] = new_layer[v]
+ *             if v in matching: layer.append(matching[v]); pred[matching[v]] = v
+ *             else: unmatched.append(v)
+ *         if not unmatched: return matching
+ *         recurse(v): if v in preds: L = preds.pop(v)
+ *                         for u in L: if u in pred: pu = pred.pop(u)
+ *                                         if pu is UNMATCHED or recurse(pu): matching[v] = u; return True
+ *                     return False
+ *         for v in unmatched: recurse(v)
+ *  3. The result is sorted(matching.items()): h_match gives, per reference in the caller's order, the estimate index it
+ *     is matched to or -1.  Its number of matches is the matched count of bp_score_*.
+ * Pass 0 has no offset test (offset_ratio=None), pass 1 has it.  Each (pair, pass) is one device thread that builds its
+ * G (lists by insertion sort, keys by a counting sort on the first reference, stable in j) and runs these steps with
+ * arrays and an explicit stack in place of the recursion.
+ * Kernel launches: one count launch (hits without the offset test per pair, which size the workspace), then one match
+ * launch per range of consecutive pairs whose workspace fits 2 GiB; a pair that needs more runs alone.  Workspace of a
+ * pair with N estimates, R references and M hits without the offset test: 8 (3 M + 5 N + 8 R + 8) bytes (both passes).
+ * No launch for a chunk without estimated notes or a call without references (every entry -1).
+ *
+ * Grid: bp_score_grid_*'s inputs; the notes come back in `notes` exactly as bp_decode_grid_* gives them (amplitudes,
+ * empty bend ranges: include_pitch_bends is ignored; capacities and BP_E_CAPACITY / bp_last_required as there), and
+ * h_match [n_params][2][n_refs_total] (int32, host).  Per chunk: the grid decode's launches, the compaction and
+ * amplitude launches of bp_decode_grid_*, then the count and match launches above.  Settings, references and
+ * tolerances are validated as in bp_score_grid_* before anything is enqueued. */
+int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* score, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match,
+                         void* stream);
+int bp_match_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
+                       int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                       const bp_score_params_t* score, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match);
+/* Item i's estimated notes (est, explicit, in the order given) matched against item i's references; h_match
+ * [2][n_refs_total].  Validation as bp_score_notes_host; synchronous. */
+int bp_match_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
+                        const bp_score_params_t* score, int32_t* h_match);
+
 /* ---- frame-level multi-pitch scores of decoded notes against reference frames -------------------------------------
  * No reference counterpart: the sums behind mir_eval.multipitch.metrics 0.7 (window = 0.5 semitones by default).
  * A series is a time array time[0 .. N) (seconds, non-decreasing) and per frame a multiset of values, each carried as
