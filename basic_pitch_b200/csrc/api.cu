@@ -846,17 +846,20 @@ ScoreTol score_tol(const bp_score_params_t& sp) {
 
 // Validates n sets of notes (`what` "references" / "estimates", set unit "file" / "item"): note_off[0] = 0 and
 // non-decreasing, at most 2^31 - 1 notes per set, every note with finite values, onset >= 0 and offset > onset.
-int check_note_set(const std::string& api, const char* what, const char* unit, const bp_note_set_t* s, int n) {
+// Without `pitched` log2_hz is not read (intervals only).
+int check_note_set(const std::string& api, const char* what, const char* unit, const bp_note_set_t* s, int n,
+                   bool pitched = true) {
   const std::string who = api + ": " + what;
   if (!s || !s->note_off) return fail(BP_E_INVALID, who + ": null note set");
   if (s->note_off[0] != 0) return fail(BP_E_INVALID, who + ": note_off[0] must be 0");
   for (int i = 0; i < n; ++i)
     if (s->note_off[i + 1] < s->note_off[i] || s->note_off[i + 1] - s->note_off[i] > INT_MAX)
       return fail(BP_E_INVALID, who + " " + unit + " " + std::to_string(i) + ": bad note_off");
-  if (s->note_off[n] > 0 && (!s->onset_s || !s->offset_s || !s->log2_hz)) return fail(BP_E_INVALID, who + ": null array");
+  if (s->note_off[n] > 0 && (!s->onset_s || !s->offset_s || (pitched && !s->log2_hz)))
+    return fail(BP_E_INVALID, who + ": null array");
   for (int i = 0; i < n; ++i)
     for (long long j = s->note_off[i]; j < s->note_off[i + 1]; ++j) {
-      const double on = s->onset_s[j], off = s->offset_s[j], l2 = s->log2_hz[j];
+      const double on = s->onset_s[j], off = s->offset_s[j], l2 = pitched ? s->log2_hz[j] : 0.0;
       const char* why = !std::isfinite(on) || !std::isfinite(off) ? "non-finite time"
                         : !std::isfinite(l2)                      ? "non-finite log2_hz"
                         : on < 0                                  ? "onset < 0"
@@ -882,6 +885,7 @@ struct Pack {
 
 // The references of n sets, sorted by (bucket, onset) within each set, into `pk`; offsets of the sections in `o[6]`
 // (note_off, onset, offset, log2_hz, bucket, index within its set before sorting); the range of buckets into tol.
+// Without log2_hz (s->log2_hz NULL) every reference is in bucket 0 with log2_hz 0.
 void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol) {
   const long long R = s->note_off[n];
   std::vector<long long> idx(R);
@@ -890,7 +894,7 @@ void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol
   tol.bucket_lo = 0, tol.bucket_hi = -1;
   for (long long j = 0; j < R; ++j) {
     idx[j] = j;
-    bucket[j] = score_bucket(s->log2_hz[j]);
+    bucket[j] = s->log2_hz ? score_bucket(s->log2_hz[j]) : 0;
     if (j == 0 || bucket[j] < tol.bucket_lo) tol.bucket_lo = bucket[j];
     if (j == 0 || bucket[j] > tol.bucket_hi) tol.bucket_hi = bucket[j];
   }
@@ -903,7 +907,7 @@ void pack_refs(const bp_note_set_t* s, int n, Pack& pk, size_t* o, ScoreTol& tol
   for (long long j = 0; j < R; ++j) {
     on[j] = s->onset_s[idx[j]];
     off[j] = s->offset_s[idx[j]];
-    l2[j] = s->log2_hz[idx[j]];
+    l2[j] = s->log2_hz ? s->log2_hz[idx[j]] : 0.0;
     bsorted[j] = bucket[idx[j]];
   }
   const std::vector<long long> noff(s->note_off, s->note_off + n + 1);
@@ -2007,6 +2011,16 @@ int check_score_grid(const std::string& api, int n_files, int n_params, const bp
   return check_note_set(api, "references", "file", refs, n_files);
 }
 
+// Everything bp_score_onset_offset_grid_* check before anything is enqueued, in addition to check_grid_args: the
+// pitch_tolerance is validated as elsewhere but unused, and the references' log2_hz is not read.
+int check_onset_offset_grid(const std::string& api, int n_files, int n_params, const bp_note_set_t* refs,
+                            const bp_score_params_t* sp, const void* h_counts) {
+  int rc = check_score_params(api, sp);
+  if (rc || n_files == 0 || n_params == 0) return rc;
+  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
+  return check_note_set(api, "references", "file", refs, n_files, false);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2261,6 +2275,135 @@ int bp_match_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
                    est_off, refs->note_off, n_refs, m->match_out.p, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(h_match, m->match_out.p, sizeof(int) * 2 * n_refs, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+// ---- onset-only and offset-only scores (bp_score_onset_offset_*) -------------------------------------------------------
+
+int bp_score_onset_offset_grid_device(bp_model_t* m, const float* d_note, const float* d_onset,
+                                      const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                      int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* sp,
+                                      const double* est_log2_hz, int64_t* h_counts, void* stream) {
+  const std::string api = "bp_score_onset_offset_grid_device";
+  (void)est_log2_hz;  // no pitch test
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_onset_offset_grid(api, n_files, n_params, refs, sp, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long total_frames = foff[n_files];
+  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  long long max_t = 0;
+  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
+  // one upload per call: the references (intervals only) and the seconds of every frame a note can start or end on
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[6];
+  bp_note_set_t r = *refs;
+  r.log2_hz = nullptr;
+  pack_refs(&r, n_files, pk, o_ref, tol);
+  std::vector<double> frame_t(max_t + 1);
+  bp_frame_times(max_t + 1, frame_t.data());
+  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
+  const long long n_refs = refs->note_off[n_files];
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(m->score_counts.reserve((size_t)n_params * n_files * 4));
+  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
+  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>&, const std::vector<long long>& soff) -> int {
+    const long long n_pairs = (long long)P * n_files;
+    CK(m->score_ws_ref.reserve((size_t)(6 * P * n_refs) + 1));
+    CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs] + 2 * n_pairs) + 1));
+    ScoreEst e{};
+    e.off = m->d_slot_off.p;
+    e.count = m->note_count.p;
+    e.start = m->slot_start.p;
+    e.end = m->slot_end.p;
+    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
+    launch_onset_offset(sr, e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_files, n_pairs,
+                        m->score_counts.p + 4 * p0 * n_files, st);
+    CKL();
+    m->launches += 1;
+    return BP_OK;
+  });
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_params * n_files, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_score_onset_offset_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
+                                    const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                    int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* sp,
+                                    const double* est_log2_hz, int64_t* h_counts) {
+  const std::string api = "bp_score_onset_offset_grid_host";
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_onset_offset_grid(api, n_files, n_params, refs, sp, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  DeviceGuard g(m->device);
+  const int64_t total = h_frame_off[n_files];
+  cudaStream_t st = m->stream;
+  rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {  // uploaded once for the whole grid
+    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
+    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+  }
+  return bp_score_onset_offset_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs,
+                                           sp, est_log2_hz, h_counts, st);
+}
+
+int bp_score_onset_offset_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs,
+                                     int32_t n_items, const bp_score_params_t* sp, int64_t* h_counts) {
+  const std::string api = "bp_score_onset_offset_notes_host";
+  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  int rc = check_score_params(api, sp);
+  if (rc || n_items == 0) return rc;
+  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_note_set(api, "estimates", "item", est, n_items, false);
+  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items, false);
+  if (rc) return rc;
+  ScoreTol tol = score_tol(*sp);
+  Pack pk;
+  size_t o_ref[6];
+  bp_note_set_t r = *refs;
+  r.log2_hz = nullptr;
+  pack_refs(&r, n_items, pk, o_ref, tol);
+  // the count does not depend on the order of the estimates: each item's onsets and offsets go up sorted, apart
+  const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
+  std::vector<double> on(est->onset_s, est->onset_s + n_est), off(est->offset_s, est->offset_s + n_est);
+  for (int i = 0; i < n_items; ++i) {
+    std::sort(on.begin() + est->note_off[i], on.begin() + est->note_off[i + 1]);
+    std::sort(off.begin() + est->note_off[i], off.begin() + est->note_off[i + 1]);
+  }
+  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
+  const size_t o_eon = pk.add(on.data(), sizeof(double) * n_est);
+  const size_t o_eoffs = pk.add(off.data(), sizeof(double) * n_est);
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(m->score_ws_ref.reserve((size_t)(6 * n_refs) + 1));
+  CK(m->score_ws_est.reserve((size_t)(4 * n_est + 2 * n_items) + 1));
+  CK(m->score_counts.reserve((size_t)n_items * 4));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = m->score_in.p;
+  ScoreEst e{};
+  e.off = reinterpret_cast<const long long*>(d + o_eoff);
+  e.onset = reinterpret_cast<const double*>(d + o_eon);
+  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
+  launch_onset_offset(refs_at(d, o_ref), e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_items,
+                      n_items, m->score_counts.p, st);
+  CKL();
+  m->launches += 1;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_items, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
 }

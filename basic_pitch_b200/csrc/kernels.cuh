@@ -348,6 +348,14 @@ struct ScoreWork {       // int workspace: 2 per reference and setting, 4 per es
 void launch_score_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
                         long long n_pairs, long long* counts, cudaStream_t st);
 
+// Onset-only and offset-only match counts (bp_score_onset_offset_*): counts[4 q ..] = {n_ref, n_est, onsets matched,
+// offsets matched} of pair q = setting * n_files + file, one thread per (pair, test).  Explicit estimates: E.onset and
+// E.offset each sorted ascending within every item (they are no longer notes); decode slots: E.start / E.end / E.frame_t.
+// Int workspace of one (pair, test) with N estimate slots and R references: sort keys and next-free array 2 N + 1 at
+// W.est + 4 E.off[q] + 2 q, runs and order 3 R at W.ref + 6 (s * n_ref_total + off[f]).
+void launch_onset_offset(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
+                         long long n_pairs, long long* counts, cudaStream_t st);
+
 // mir_eval's matching pair for pair (bp_match_*).  Int workspace of one (pair, pass) with N estimated notes, R
 // references and M hits without the offset test (the with-offset graph is a subgraph): adjacency offsets and lists,
 // the preds lists (node estimate, next), per reference its list head / tail, preds state, the new_layer order and the

@@ -9,7 +9,8 @@
 // estimated note the greedy pass left free, with an explicit stack in global workspace.
 //
 // The match kernels (bp_match_*) go further: they store each pair's hit graph and reproduce mir_eval's matching itself,
-// pair for pair, for one (pair, pass) per thread.
+// pair for pair, for one (pair, pass) per thread.  The onset-only and offset-only counts (bp_score_onset_offset_*) need
+// no pitch: their graphs are convex, and one thread per (pair, test) matches them greedily.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -381,7 +382,125 @@ __global__ void __launch_bounds__(kScoreThreads, 1) match_kernel(ScoreRefs R, Sc
   }
 }
 
+// ---- onset-only and offset-only counts (bp_score_onset_offset_*) -------------------------------------------------------
+// Without the pitch test each test's hit graph is convex: with the estimates in ascending order of the tested time, a
+// reference hits one contiguous run of them, because around4(|fl(t_r - t_e)|) falls and then rises as t_e grows.  Taking
+// the references by ascending run end, each matched to the smallest free estimate of its run, gives a maximum matching.
+
+// Thread t: pair t / 2, test t % 2 (0: onsets, 1: offsets).  The estimates' tested times come sorted per item (explicit
+// notes, sorted on the host) or are sorted here by frame index (decode slots; bp_frame_times is strictly increasing).
+__global__ void __launch_bounds__(kScoreThreads) onset_offset_kernel(ScoreRefs R, ScoreEst E, ScoreTol tol, ScoreWork W,
+                                                                     int n_files, long long n_pairs,
+                                                                     long long* __restrict__ counts) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long q = t >> 1;
+  if (q >= n_pairs) return;
+  const int test = (int)(t & 1);
+  const int file = (int)(q % n_files);
+  const long long s = q / n_files;
+  const long long r0 = R.off[file];
+  const int n_ref = (int)(R.off[file + 1] - r0);
+  const long long ebase = E.off[q];
+  const int n = E.count ? E.count[q] : (int)(E.off[q + 1] - ebase);
+  long long* out = counts + 4 * q;
+  if (test == 0) out[0] = n_ref, out[1] = n;
+  if (n_ref == 0 || n == 0) {
+    out[2 + test] = 0;
+    return;
+  }
+  int* keys = W.est + 4 * ebase + 2 * q + (long long)test * (2LL * n + 1);  // [N] frame of the k-th smallest time
+  int* cnt = keys + n;                                                      // [N + 1] counts of the sort, then next free
+  int* run = W.ref + 6 * (s * W.n_ref_total + r0) + (long long)test * 3 * n_ref;  // [2 R] lo, end (one past hi)
+  int* order = run + 2 * n_ref;                                                   // [R] references by run end
+  const double* est_t = test ? E.offset + ebase : E.onset + ebase;                // explicit notes, sorted
+  const double* r_t = test ? R.offset + r0 : R.onset + r0;
+  if (E.count) {  // heap sort of the slots' frames
+    const int* fr = (test ? E.end : E.start) + ebase;
+    for (int j = 0; j < n; ++j) keys[j] = fr[j];
+    auto sift = [&](int h, int v, int end) {  // v down from h in the max-heap keys[0, end)
+      for (int c = 2 * h + 1; c < end; c = 2 * h + 1) {
+        if (c + 1 < end && keys[c + 1] > keys[c]) ++c;
+        if (keys[c] <= v) break;
+        keys[h] = keys[c];
+        h = c;
+      }
+      keys[h] = v;
+    };
+    for (int i = n / 2 - 1; i >= 0; --i) sift(i, keys[i], n);
+    for (int end = n - 1; end > 0; --end) {
+      const int v = keys[end];
+      keys[end] = keys[0];
+      sift(0, v, end);
+    }
+  }
+  auto time = [&](int j) { return E.count ? E.frame_t[keys[j]] : est_t[j]; };
+  for (int k = 0; k <= n; ++k) cnt[k] = 0;
+  for (int r = 0; r < n_ref; ++r) {
+    const double tr = r_t[r];
+    const double lim =
+        test ? fmax(__dmul_rn(tol.ratio, fabs(__dsub_rn(R.offset[r0 + r], R.onset[r0 + r]))), tol.off_min) : tol.onset;
+    // lo: estimates before the reference that miss it; end: first estimate after it that misses it
+    int a = 0, len = n;
+    while (len > 0) {
+      const int h = len >> 1, m = a + h;
+      const double te = time(m);
+      if (te < tr && !(around4(fabs(__dsub_rn(tr, te))) <= lim)) {
+        a = m + 1;
+        len -= h + 1;
+      } else {
+        len = h;
+      }
+    }
+    const int lo = a;
+    len = n - lo;
+    while (len > 0) {
+      const int h = len >> 1, m = a + h;
+      const double te = time(m);
+      if (!(te > tr && !(around4(fabs(__dsub_rn(tr, te))) <= lim))) {
+        a = m + 1;
+        len -= h + 1;
+      } else {
+        len = h;
+      }
+    }
+    run[2 * r] = lo;
+    run[2 * r + 1] = a;
+    if (lo < a) ++cnt[a];
+  }
+  for (int k = 0, sum = 0; k <= n; ++k) {  // counting sort by run end (in [1, N] for a non-empty run)
+    const int c = cnt[k];
+    cnt[k] = sum;
+    sum += c;
+  }
+  int n_order = 0;
+  for (int r = 0; r < n_ref; ++r)
+    if (run[2 * r] < run[2 * r + 1]) order[cnt[run[2 * r + 1]]++] = r, ++n_order;
+  // greedy: each reference takes the smallest free estimate of its run (next free, path halving; cnt[N] = N: none)
+  int* nf = cnt;
+  for (int k = 0; k <= n; ++k) nf[k] = k;
+  int matched = 0;
+  for (int k = 0; k < n_order; ++k) {
+    const int r = order[k];
+    int x = run[2 * r];
+    while (nf[x] != x) {
+      nf[x] = nf[nf[x]];
+      x = nf[x];
+    }
+    if (x < run[2 * r + 1]) {
+      nf[x] = x + 1;
+      ++matched;
+    }
+  }
+  out[2 + test] = matched;
+}
+
 }  // namespace
+
+void launch_onset_offset(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, const ScoreWork& W, int n_files,
+                         long long n_pairs, long long* counts, cudaStream_t st) {
+  const unsigned int blocks = (unsigned int)((2 * n_pairs + kScoreThreads - 1) / kScoreThreads);
+  onset_offset_kernel<<<blocks, kScoreThreads, 0, st>>>(R, E, tol, W, n_files, n_pairs, counts);
+}
 
 void launch_match_count(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, int n_files, long long n_pairs,
                         long long* edges, cudaStream_t st) {

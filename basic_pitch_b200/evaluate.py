@@ -15,6 +15,12 @@ Matched pairs: the library also returns which estimated note mir_eval's matching
 the average overlap ratio and the note scores with velocity (mir_eval.transcription_velocity), with mir_eval's own
 NumPy expressions; `inference.evaluate_velocity_grid` does this for a grid of settings.
 
+Onsets and offsets alone: the library counts, per (setting, file) or item, the onsets and the offsets matched without
+the pitch test (`Model.score_onset_offset_grid`, `Model.score_onsets_offsets`; include/bp_b200.h,
+bp_score_onset_offset_*); `onset_offset_scores` turns them into mir_eval's onset-only and offset-only scores, and
+`inference.evaluate_transcription_grid` returns every value of mir_eval.transcription.evaluate (`TRANSCRIPTION_KEYS`)
+for a grid of settings.
+
 Posteriorgrams as multi-f0 estimates: `salience_to_multipitch` reads a contour (or note) posteriorgram under a
 threshold, peak picking and a frequency range as the series those metrics score (include/bp_b200.h,
 bp_score_salience_grid_*); `Model.score_salience_grid` / `inference.evaluate_salience_grid` score a grid of such
@@ -184,6 +190,46 @@ def note_scores(counts) -> Dict[str, np.ndarray]:
         out["mean"] = {k: (v.mean(axis=-1) if n else np.zeros(v.shape[:-1])) for k, v in out.items()}
     else:
         out["mean"] = {k: (v.mean() if v.size else np.float64(0.0)) for k, v in out.items()}
+    return out
+
+
+# Columns of `Model.score_onset_offset_grid` / `score_onsets_offsets`
+ONSET_OFFSET_FIELDS = ("n_ref", "n_est", "onset_matched", "offset_matched")
+
+# mir_eval.transcription.evaluate's keys, in its order, and the names the evaluate_* functions give those values
+TRANSCRIPTION_KEYS = {
+    "Precision": "precision",
+    "Recall": "recall",
+    "F-measure": "f_measure",
+    "Average_Overlap_Ratio": "average_overlap_ratio",
+    "Precision_no_offset": "precision_no_offset",
+    "Recall_no_offset": "recall_no_offset",
+    "F-measure_no_offset": "f_measure_no_offset",
+    "Average_Overlap_Ratio_no_offset": "average_overlap_ratio_no_offset",
+    "Onset_Precision": "onset_precision",
+    "Onset_Recall": "onset_recall",
+    "Onset_F-measure": "onset_f_measure",
+    "Offset_Precision": "offset_precision",
+    "Offset_Recall": "offset_recall",
+    "Offset_F-measure": "offset_f_measure",
+}
+
+_ONSET_OFFSET_NAMES = {"precision_no_offset": "onset_precision", "recall_no_offset": "onset_recall",
+                       "f_measure_no_offset": "onset_f_measure", "precision": "offset_precision",
+                       "recall": "offset_recall", "f_measure": "offset_f_measure"}
+
+
+def onset_offset_scores(counts) -> Dict[str, np.ndarray]:
+    """counts (..., 4) as `Model.score_onset_offset_grid` / `score_onsets_offsets` return them -> dict of float64
+    arrays of shape counts.shape[:-1]: onset_precision, onset_recall, onset_f_measure (mir_eval.transcription's
+    onset_precision_recall_f1) and offset_precision, offset_recall, offset_f_measure (offset_precision_recall_f1).
+    The formulas are `note_scores`' on the same four columns (0 when either side is empty); "mean" as there."""
+    c = np.asarray(counts, np.int64)
+    if c.ndim < 1 or c.shape[-1] != 4:
+        raise ValueError(f"counts must have shape (..., 4), got {c.shape}")
+    s = note_scores(c)
+    out = {name: s[k] for k, name in _ONSET_OFFSET_NAMES.items()}
+    out["mean"] = {name: s["mean"][k] for k, name in _ONSET_OFFSET_NAMES.items()}
     return out
 
 

@@ -465,6 +465,61 @@ class Model:
         self._lib.bp_match_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(h_match))
         return [h_match[:, roff[i] : roff[i + 1]].copy() for i in range(len(estimates))]
 
+    @staticmethod
+    def _interval_set(sets: Sequence[np.ndarray], what: str):
+        """[intervals (n, 2) in seconds] -> (bp_note_set_t without pitches, the arrays it points at)."""
+        off = np.zeros(len(sets) + 1, np.int64)
+        ivs = []
+        for i, iv in enumerate(sets):
+            iv = np.asarray(iv, np.float64)
+            if iv.size == 0:
+                iv = iv.reshape(0, 2)
+            if iv.ndim != 2 or iv.shape[1] != 2:
+                raise ValueError(f"{what}[{i}]: need intervals (n, 2), got {iv.shape}")
+            off[i + 1] = off[i] + len(iv)
+            ivs.append(iv)
+        iv = np.concatenate(ivs) if ivs else np.zeros((0, 2))
+        arrs = (off, np.ascontiguousarray(iv[:, 0]), np.ascontiguousarray(iv[:, 1]))
+        ns = _lib.NoteSet()
+        ns.note_off, ns.onset_s, ns.offset_s = (_ptr(a) for a in arrs)
+        return ns, arrs
+
+    def score_onset_offset_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
+                                settings: Sequence[Dict[str, Any]], references: Sequence[np.ndarray],
+                                **tolerances) -> np.ndarray:
+        """Onset-only and offset-only match counts (mir_eval.transcription's match_note_onsets / match_note_offsets;
+        pitch plays no part) of a batch of files decoded under every setting of a grid, in ONE library call
+        (`bp_score_onset_offset_grid_host`): the notes never leave the device.  Settings as `score_grid`;
+        `references[i]` is file i's intervals (n, 2) in seconds; tolerances those of `evaluate.TOLERANCES`
+        (pitch_tolerance is checked and unused).  Returns int64 counts (n_settings, n_files, 4): n_ref, n_est, onsets
+        matched, offsets matched (`evaluate.onset_offset_scores` turns them into precision, recall and F)."""
+        n_files, n_params = len(notes), len(settings)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference sets")
+        ps = self._grid_params(settings)
+        sp = self._score_params(tolerances)
+        refs, keep = self._interval_set(references, "references")
+        foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+        counts = np.zeros((n_params, n_files, 4), np.int64)
+        self._lib.bp_score_onset_offset_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params,
+                                                  C.byref(refs), C.byref(sp), None, _ptr(counts))
+        return counts
+
+    def score_onsets_offsets(self, estimates: Sequence[np.ndarray], references: Sequence[np.ndarray],
+                             **tolerances) -> np.ndarray:
+        """Item i's estimated intervals against item i's reference intervals, (n, 2) in seconds
+        (`bp_score_onset_offset_notes_host`, one kernel launch).  Returns int64 counts (n_items, 4) as
+        `score_onset_offset_grid`."""
+        if len(estimates) != len(references):
+            raise ValueError(f"{len(estimates)} estimated but {len(references)} reference sets")
+        sp = self._score_params(tolerances)
+        est, keep_e = self._interval_set(estimates, "estimates")
+        refs, keep_r = self._interval_set(references, "references")
+        counts = np.zeros((len(estimates), 4), np.int64)
+        self._lib.bp_score_onset_offset_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp),
+                                                   _ptr(counts))
+        return counts
+
     # ------------------------------------------------------------------ frame-level scores
     @staticmethod
     def _multipitch_set(series: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]], what: str):
@@ -1032,6 +1087,64 @@ def evaluate_velocity_grid(
     scores.update(extra)
     scores["mean"].update({k: (v.mean(axis=-1) if n_files else np.zeros(n_params)) for k, v in extra.items()})
     return counts, scores
+
+
+def evaluate_transcription_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, np.ndarray]],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    **tolerances,
+):
+    """Every value of mir_eval.transcription.evaluate (0.7) for a batch of annotated recordings under every setting of a
+    grid (addition; no reference counterpart).  The model runs once over the batch; one `bp_match_grid_host` call
+    decodes every (setting, file) and returns mir_eval's pairs with and without offsets, which give the note scores and
+    both average overlap ratios; one `bp_score_onset_offset_notes_host` call scores the notes that came back for onsets
+    and offsets alone, so the grid is decoded once.  `audio`, `settings` and tolerances as in `evaluate_grid`;
+    `references[i]` is file i's (intervals (n, 2) in seconds, pitches (n,) in Hz).
+
+    Returns (counts, scores): counts int64 (n_settings, n_files, 6) = n_ref, n_est, matched without offsets, matched,
+    onsets matched, offsets matched; scores the 14 values under the names `evaluate.TRANSCRIPTION_KEYS` maps mir_eval's
+    keys to, in its order, as (n_settings, n_files) float64 arrays, with "mean" over files as in `note_scores`."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    outs = model.run_inference_arrays(clips)
+    res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
+                                  **tolerances)
+    n_params, n_files = len(settings), len(clips)
+    ref_ivs = [np.asarray(iv, np.float64).reshape(-1, 2) for iv, _ in references]
+    times = [infer.model_frames_to_time(o["note"].shape[0] + 1) for o in outs]
+    counts = np.zeros((n_params, n_files, 6), np.int64)
+    overlap = {k: np.zeros((n_params, n_files)) for k in ("average_overlap_ratio", "average_overlap_ratio_no_offset")}
+    ests = []
+    for k in range(n_params):
+        for i in range(n_files):
+            r, m = res[k][i], match[k][i]
+            est_iv = np.stack([times[i][r["start"]], times[i][r["end"]]], 1)
+            ests.append(est_iv)
+            counts[k, i, :4] = (len(ref_ivs[i]), len(est_iv), (m[0] >= 0).sum(), (m[1] >= 0).sum())
+            for suffix, row in (("", m[1]), ("_no_offset", m[0])):
+                ref_idx = np.flatnonzero(row >= 0)  # sorted(matching.items()): ascending reference index
+                overlap["average_overlap_ratio" + suffix][k, i] = evaluate._overlap_ratio(ref_ivs[i], est_iv, ref_idx,
+                                                                                           row[ref_idx])
+    onoff = model.score_onsets_offsets(ests, ref_ivs * n_params, **tolerances).reshape(n_params, n_files, 4)
+    counts[..., 4:] = onoff[..., 2:]
+    scores = evaluate.note_scores(counts[..., :4])
+    scores.update(overlap)
+    scores["mean"].update({k: (v.mean(axis=-1) if n_files else np.zeros(n_params)) for k, v in overlap.items()})
+    oo = evaluate.onset_offset_scores(onoff)
+    scores["mean"].update(oo.pop("mean"))
+    scores.update(oo)
+    names = list(evaluate.TRANSCRIPTION_KEYS.values())
+    return counts, {**{k: scores[k] for k in names}, "mean": {k: scores["mean"][k] for k in names}}
 
 
 def evaluate_frames_grid(

@@ -283,6 +283,44 @@ int bp_match_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
 int bp_match_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
                         const bp_score_params_t* score, int32_t* h_match);
 
+/* ---- onset-only and offset-only note scores --------------------------------------------------------------------------
+ * No reference counterpart: the counts behind mir_eval.transcription 0.7's onset_precision_recall_f1 (match_note_onsets)
+ * and offset_precision_recall_f1 (match_note_offsets) with strict=False.  A reference note i and an estimated note j of
+ * the same file or item hit, in float64 and with the operations and order of bp_score_* above, when
+ *   onset test:  rint(|on_i - on_j| * 10000) / 10000 <= onset_tolerance
+ *   offset test: rint(|off_i - off_j| * 10000) / 10000 <= max(offset_ratio * |off_i - on_i|, offset_min_tolerance)
+ * Pitch plays no part.  The matched count of a test is the size of a maximum matching of its hit graph.  Per (setting,
+ * file) or item the result is four int64 counts: {n_ref, n_est, onsets matched, offsets matched}; precision, recall and
+ * F follow from them as for bp_score_* (basic_pitch_b200/evaluate.py, onset_offset_scores).
+ * Inputs are those of bp_score_*, except that the pitches are not read: log2_hz of a note set and est_log2_hz may be
+ * NULL.  pitch_tolerance is validated as elsewhere and then ignored; intervals are validated as in bp_score_* (finite,
+ * onset >= 0, offset > onset, the failing file or item and note named), before anything is enqueued.
+ * Method: with a pair's estimates in ascending order of the tested time, every reference hits one contiguous run of
+ * them (|fl(t_i - t_j)| does not decrease as t_j moves away from t_i, and the rounding is monotone), so the graph is
+ * convex.  One device thread per (pair, test) sorts the tested times (decode slots: a heap sort of the frame indices,
+ * bp_frame_times being strictly increasing; explicit estimates: sorted on the host), finds each reference's run by two
+ * binary searches with the exact predicate, counting-sorts the references by run end and gives each in turn the smallest
+ * free estimate of its run (a next-free array with path halving).  That greedy is exact on a convex graph.  Workspace of
+ * a pair with N estimate slots and R references: 8 (2 N + 3 R + 1) bytes (both tests).
+ *
+ * Grid: bp_score_grid_*'s arguments and h_counts [n_params][n_files][4] (host).  Settings are validated, grouped and
+ * chunked, and slot reruns happen, as in bp_decode_grid_*.  Kernel launches per chunk: those of the grid decode + 1,
+ * whatever the number of settings.  Device workspace beyond the decode's: 24 bytes per reference and setting of a
+ * chunk, 16 bytes per note slot and 8 bytes per (setting, file).  No note crosses to the host.  _device: posteriorgrams
+ * in device memory, work on `stream`, synchronised before returning; _host: host posteriorgrams, uploaded once. */
+int bp_score_onset_offset_grid_device(bp_model_t* m, const float* d_note, const float* d_onset,
+                                      const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                      int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* score,
+                                      const double* est_log2_hz, int64_t* h_counts, void* stream);
+int bp_score_onset_offset_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
+                                    const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                    int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* score,
+                                    const double* est_log2_hz, int64_t* h_counts);
+/* Item i's estimated notes (explicit, in any order: the counts do not depend on it) against item i's references;
+ * h_counts [n_items][4].  One kernel launch (none for n_items == 0), synchronous. */
+int bp_score_onset_offset_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs,
+                                     int32_t n_items, const bp_score_params_t* score, int64_t* h_counts);
+
 /* ---- frame-level multi-pitch scores of decoded notes against reference frames -------------------------------------
  * No reference counterpart: the sums behind mir_eval.multipitch.metrics 0.7 (window = 0.5 semitones by default).
  * A series is a time array time[0 .. N) (seconds, non-decreasing) and per frame a multiset of values, each carried as
