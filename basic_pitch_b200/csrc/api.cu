@@ -3067,6 +3067,39 @@ int bp_debug_tc_clocks(bp_model_t* m, int which, uint64_t* cycles, int reset) {
   return BP_OK;
 }
 
+int bp_debug_tc_schedule(int which, int fused, int n_windows, int n_sms, int32_t* sizes, int32_t* items, uint32_t* edges) {
+  if (!sizes || which < 0 || which > 2 || n_windows < 1 || n_sms < 1)
+    return fail(BP_E_INVALID, "bp_debug_tc_schedule: bad argument");
+  const TcConvSpec sp = tc_spec(which);
+  int ms = 0;
+  const TcSchedule s = tc_schedule(which, fused != 0 || which != 0, n_windows, n_sms, &ms);
+  sizes[0] = s.n_items();
+  sizes[1] = s.grid;
+  sizes[2] = s.n_mtiles;
+  sizes[3] = s.n_full;
+  sizes[4] = s.n_ranges;
+  sizes[5] = ms;
+  sizes[6] = s.n_full * ms;
+  sizes[7] = sp.G0;
+  if (items)
+    for (int it = 0; it < s.n_items(); ++it) s.item(it, sp.G0, items[3 * it], items[3 * it + 1], items[3 * it + 2]);
+  if (edges) {
+    edges[0] = tc_edge_mask(sp, 1u);
+    edges[1] = tc_edge_mask(sp, s.tail_starts());
+  }
+  return BP_OK;
+}
+
+int bp_debug_tc_cta_busy(bp_model_t* m, int which, uint64_t* ns, int n, int reset) {
+  if (!m || (!ns && n) || which < 0 || which > 2 || n < 0 || n > kTcMaxCtas)
+    return fail(BP_E_INVALID, "bp_debug_tc_cta_busy: bad argument");
+  DeviceGuard g(m->device);
+  CK(cudaDeviceSynchronize());
+  if (tc_read_busy(which, reinterpret_cast<unsigned long long*>(ns), n, reset != 0) != 0)
+    return fail(BP_E_INVALID, "bp_debug_tc_cta_busy: the library was built without -DBP_TC_CLOCKS");
+  return BP_OK;
+}
+
 int bp_model_profile(bp_model_t* m, int which) {
   if (!m) return fail(BP_E_INVALID, "bp_model_profile: null model");
   if (which < -1 || which > 6) return fail(BP_E_INVALID, "bp_model_profile: unknown kernel family");

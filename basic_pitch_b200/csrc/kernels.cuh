@@ -106,10 +106,38 @@ __host__ __device__ constexpr bool tc_starts_range(const TcConvSpec& s, int g, i
 __host__ __device__ constexpr bool tc_ends_range(const TcConvSpec& s, int g, int slot, bool item_end) {
   return item_end || tc_group_tile(s, g + 1, slot) != tc_group_tile(s, g, slot) + 1;
 }
-// an item of split n (groups [q G0 / n, (q + 1) G0 / n)) starts at group g
-__host__ __device__ constexpr bool tc_item_starts(const TcConvSpec& s, int n_split, int g) {
-  const int q = (g * n_split + s.G0 - 1) / s.G0;  // the least q with q G0 / n >= g
-  return q < n_split && q * s.G0 / n_split == g;
+// The items of one conv_tc_kernel launch (tc_schedule, tc_conv.cu).  The persistent CTAs walk items it = blockIdx.x,
+// + grid, ...  Items [0, n_full) are the M-tiles 0 .. n_full - 1 whole (all G0 groups); n_full is a multiple of the grid,
+// so every CTA runs the same number of whole M-tiles.  The n_tail M-tiles after them are each cut into n_ranges group
+// ranges [bounds[q], bounds[q + 1]) of balanced cost; tail item j = it - n_full is range q = j / n_tail of M-tile
+// n_full + j % n_tail (range-major, so that the CTAs that take a second tail item take another range).
+struct TcSchedule {
+  int n_mtiles, n_full, n_tail, n_ranges, grid;
+  unsigned char bounds[16];  // n_ranges + 1 group boundaries: 0 = bounds[0] < ... < bounds[n_ranges] = G0
+  __host__ __device__ int n_items() const { return n_full + n_tail * n_ranges; }
+  __host__ __device__ uint32_t tail_starts() const {  // bit g: a tail item starts at group g
+    uint32_t m = 0;
+    for (int q = 0; q < n_ranges; ++q) m |= 1u << bounds[q];
+    return m;
+  }
+  __host__ __device__ void item(int it, int G0, int& mt, int& g0, int& g1) const {
+    if (it < n_full) {
+      mt = it, g0 = 0, g1 = G0;
+      return;
+    }
+    const int j = it - n_full, q = j / n_tail;
+    mt = n_full + (j - q * n_tail), g0 = bounds[q], g1 = bounds[q + 1];
+  }
+};
+// The boundaries b = 1 .. n_ft - 1 that go through the edge buffer in an M-tile whose items start at the groups of
+// `starts` (bit g): those where tile b starts a range.  Whole M-tiles: starts = 1 (group 0 only).
+__host__ __device__ constexpr uint32_t tc_edge_mask(const TcConvSpec& s, uint32_t starts) {
+  uint32_t m = 0;
+  for (int b = 1; b < s.n_ft(); ++b) {
+    const int gs = tc_tile_group(s, b);
+    if (tc_starts_range(s, gs >> 1, gs & 1, (starts >> (gs >> 1)) & 1u)) m |= 1u << b;
+  }
+  return m;
 }
 // every frequency tile belongs to exactly one (group, slot), and tc_tile_group finds it
 __host__ __device__ constexpr bool tc_pairing_ok(const TcConvSpec& s) {
@@ -168,6 +196,10 @@ int tc_setup();  // 0 on success
 // cycle sums by role of one layer's conv_tc_kernel launches (tc::TcClk order), optionally reset; -1 unless the library
 // was built with -DBP_TC_CLOCKS
 int tc_read_clocks(int layer, unsigned long long* out, bool reset);
+// busy time of every CTA (index = blockIdx.x, n entries) of one layer's conv_tc_kernel launches in ns of %globaltimer,
+// summed over the launches, optionally reset; -1 unless built with -DBP_TC_CLOCKS
+constexpr int kTcMaxCtas = 256;
+int tc_read_busy(int layer, unsigned long long* out, int n, bool reset);
 // Where window w's centre frames go in the unwrapped (per-file) posteriorgrams (reference: inference.py:247-279).
 struct UnwrapDesc {
   long long dst_base;  // first output frame this window contributes to
@@ -203,6 +235,9 @@ struct TcOut {
 // of storing the channels-last activations
 void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& out, int n_windows, int rows_stride,
                     int n_sms, cudaStream_t st, bool fuse_next = false);
+// The items launch_conv_tc runs for a batch of n_windows on n_sms SMs (fused: the M-tiles of the fused epilogue,
+// which overlap by KH2 - 1 rows; the onset and note layers always fuse).  ms: frames an M-tile finishes.
+TcSchedule tc_schedule(int layer, bool fused, int n_windows, int n_sms, int* ms = nullptr);
 // contour conv2 on the channels-last output of the tensor-core contour conv; also emits the bf16 hi/lo split of the
 // contour posteriorgram in the layout of tc_spec(2)
 void launch_contour2_tc(const float* c1_nhwc, const CnnWeights& w, float* contour, __nv_bfloat16* chl, int rows_total,

@@ -19,7 +19,7 @@
 //     of tile row r finishes the output frame r - H (H = KH2 / 2) and adds its taps in the same order whatever its
 //     position in the tile, so a frame's value does not depend on the batch around it,
 //   * the frequency halo between neighbouring tiles is a register carry: a slot walks its frequency tiles in ascending
-//     order; only where two tile RANGES meet (a slot's next tile is not the one above, or an item of the group split
+//     order; only where two tile RANGES meet (a slot's next tile is not the one above, or an item's group range
 //     ends; tc_starts_range) the two partial sums go to a small edge buffer and edge_fix_kernel finishes those
 //     4 (contour) / 2 bins,
 //   * bias, sigmoid (+ the note input channel of the onset conv2, + unwrap inference.py:247-279) and the store.
@@ -56,10 +56,11 @@
 // a frequency tile go to four m64n32 accumulators that, side by side, are the m64n128 fragment of the Toeplitz form, so
 // the epilogue is the same for all layers.
 //
-// Work decomposition: item = (M-tile of 64 rows, split s of S over the frequency groups); group g = two frequency
+// Work decomposition: item = (M-tile of 64 rows, range [g0, g1) of the frequency groups); group g = two frequency
 // tiles (tc_group_tile: contour the neighbours {2g, 2g + 1}, onset / note {g, g + G0}), one per accumulator slot; the
 // contour's two slots share a weight tile where their content is equal, at every step but a few.  A CTA (1 per
-// SM, persistent) walks items i = blockIdx.x, +gridDim.x, ...:
+// SM, persistent) walks items i = blockIdx.x, +gridDim.x, ... of the launch's schedule (tc_schedule): whole M-tiles, the
+// same number per CTA, then the remaining M-tiles cut into group ranges of balanced cost:
 //   warp 8      producer: bulk-copies the (64+KH-1) x 320 bf16 hi/lo data tile (k-chunk-major) once per item and
 //               (contour) streams the weight tiles of each group's program (8 KB each) through a ring of stages;
 //               (onset / note) copies the conv1 B matrices once per CTA
@@ -288,7 +289,7 @@ void TcConvPlan::build(const TcConvSpec& sp, const float* W /* [COUT][n_ci][KH][
   // reference pairing {t, t + G0} (t < G0).  There, per time tap, the uses of the two tiles are sorted by their offset
   // relative to the tile, a weight tile both use is one step, and the steps only the lower tile uses come first, then
   // the shared ones, then those only the upper tile uses.  The order is a function of the geometry alone (not of the
-  // batch, the split or the pairing below), and every tile's fp32 sums stay what they are under that reference pairing.
+  // batch, the schedule of items or the pairing below), and every tile's fp32 sums stay what they are under that reference pairing.
   struct Use {
     int tile;
     uint32_t w;  // A start offset >> 4: chunk c8, row dt
@@ -600,8 +601,8 @@ struct TcArgs {
   const uint16_t* b2;           // conv2 weight matrix (tc_build_b2_full), fused layers
   TcOut o;                      // where the results go (kernels.cuh)
   int edge_rows;                // row stride of o.edge: [edge slot][side 2][KE][edge_rows]
-  int rows_total, n_mtiles, n_windows;
-  int n_split;                  // an item covers groups [s*G0/n_split, (s+1)*G0/n_split)
+  int rows_total, n_windows;
+  TcSchedule sch;               // the launch's items: (M-tile, range of frequency groups), see tc_schedule
   int row0;                     // first data row of M-tile 0
   // = tc_spec(layer).chunks8: a run-time trip count keeps the producer's per-chunk copy loop rolled, which keeps the
   // contour's producer and MMA-issue loop state in uniform registers (a compile-time count unrolls it and they move out)
@@ -628,16 +629,31 @@ enum TcClk {
   kNumClk
 };
 }  // namespace tc
+// With the flag the CTA's busy time (%globaltimer from its start to the end of its last consumer warp) also goes to
+// g_tc_busy[layer][blockIdx.x] (tools/tc_balance.py: how evenly a launch's work is spread over the SMs).
 #ifdef BP_TC_CLOCKS
 __device__ unsigned long long g_tc_clocks[3][tc::kNumClk];
+__device__ unsigned long long g_tc_busy[3][kTcMaxCtas];
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
 struct TcClocks {
   // 32-bit sums (a thread's share of one launch stays far below 2^32 cycles) keep the instrumented consumers within
   // their register budget
   uint32_t t, c[tc::kNumClk];
+  unsigned long long t0;
   __device__ __forceinline__ TcClocks() {
     t = (uint32_t)clock();
+    t0 = globaltimer_ns();
 #pragma unroll
     for (int k = 0; k < tc::kNumClk; ++k) c[k] = 0;
+  }
+  // consumers only (named barrier 3 over their 256 threads): the CTA's work ends with the last consumer warp
+  __device__ __forceinline__ void cta_end(int layer) {
+    asm volatile("bar.sync 3, 256;" ::: "memory");
+    if (threadIdx.x == 0 && blockIdx.x < kTcMaxCtas) atomicAdd(&g_tc_busy[layer][blockIdx.x], globaltimer_ns() - t0);
   }
   __device__ __forceinline__ void lap(int k) {
     const uint32_t n = (uint32_t)clock();
@@ -654,8 +670,25 @@ struct TcClocks {
 struct TcClocks {
   __device__ __forceinline__ void lap(int) {}
   __device__ __forceinline__ void flush(int) {}
+  __device__ __forceinline__ void cta_end(int) {}
 };
 #endif
+
+int tc_read_busy(int layer, unsigned long long* out, int n, bool reset) {
+#ifdef BP_TC_CLOCKS
+  if (layer < 0 || layer > 2 || n < 0 || n > kTcMaxCtas) return -1;
+  const size_t row = kTcMaxCtas * sizeof(unsigned long long);
+  if (n && cudaMemcpyFromSymbol(out, g_tc_busy, n * sizeof(unsigned long long), (size_t)layer * row) != cudaSuccess) return -1;
+  if (reset) {
+    static const unsigned long long zero[kTcMaxCtas] = {};
+    if (cudaMemcpyToSymbol(g_tc_busy, zero, row, (size_t)layer * row) != cudaSuccess) return -1;
+  }
+  return 0;
+#else
+  (void)layer, (void)out, (void)n, (void)reset;
+  return -1;
+#endif
+}
 
 int tc_read_clocks(int layer, unsigned long long* out, bool reset) {
 #ifdef BP_TC_CLOCKS
@@ -1022,7 +1055,7 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
   }
   __syncthreads();
 
-  const int n_items = a.n_mtiles * a.n_split;
+  const int n_items = a.sch.n_items();
   TcClocks clk;
 
   if (warp >= kConsumerWarps) {
@@ -1040,8 +1073,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     uint32_t stage = 0, ph_w = 0, ph_d = 0, n_fill = 0;
     const size_t plane_elems = (size_t)L.chunks8 * a.rows_total * 8;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const int mt = it / a.n_split, sp = it % a.n_split;
-      const int g0 = sp * L.G0 / a.n_split, g1 = (sp + 1) * L.G0 / a.n_split;
+      int mt, g0, g1;
+      a.sch.item(it, L.G0, mt, g0, g1);
       clk.lap(kClkProdOther);
       mbar_wait_wd(data_empty, ph_d ^ 1, 1);
       clk.lap(kClkDataEmpty);
@@ -1097,8 +1130,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     if constexpr (kFused) mbar_wait_wd(b2_full, 0, 6);
     if constexpr (kGather) mbar_wait_wd(b1_full, 0, 7);
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const int mt = it / a.n_split, spl = it % a.n_split;
-      const int g0 = spl * L.G0 / a.n_split, g1 = (spl + 1) * L.G0 / a.n_split;
+      int mt, g0, g1;
+      a.sch.item(it, L.G0, mt, g0, g1);
       // conv1 rows of the thread's fragment (relu(conv1) of a row that is not a live frame is the zero padding in time)
       bool live[2];
       int rb[2], rt[2];
@@ -1301,12 +1334,13 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     }
     clk.lap(kClkConsOther);
     clk.flush(LAYER);
+    clk.cta_end(LAYER);
   }
 }
 
 
 // ------------------------------------------------------------------------------------------------
-// Where two tile ranges meet (boundary ft_b: tile ft_b starts a range under the launch's split, see tc_starts_range)
+// Where two tile ranges meet (boundary ft_b: tile ft_b starts a range in the items of an M-tile, see tc_starts_range)
 // the 2 * HALO bins FLT * ft_b - HALO + k got one partial sum from each side: finish them here.  Pitch layers: 2 bins
 // per frame.  Contour: 4 bins, and with the six finished bins each side left next to them the two 8-bin chunks around
 // the boundary.
@@ -1314,23 +1348,18 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
 struct EdgeFixArgs {
   TcOut o;
   int edge_rows, n_rows;        // rows of the (window, frame) space covered by the M-tiles
-  uint32_t edges;               // bit b: boundary b goes through the edge buffer under the launch's split (tc_edge_mask)
+  // bit b: boundary b goes through the edge buffer (tc_edge_mask) in the rows finished by a whole M-tile (rows below
+  // tail_row0) and by a tail M-tile (the rows from tail_row0 on)
+  uint32_t edges_full, edges_tail;
+  int tail_row0;
   int n_windows;
   float bias2, note_w[9];  // the layer's conv2 bias; onset: the conv2 weights of the note input channel
 };
 
-// The boundaries b = 1 .. n_ft - 1 where a range starts under split n_split (tile b starts a range in its group)
-__host__ __device__ constexpr uint32_t tc_edge_mask(const TcConvSpec& s, int n_split) {
-  uint32_t m = 0;
-  for (int b = 1; b < s.n_ft(); ++b) {
-    const int gs = tc_tile_group(s, b);
-    if (tc_starts_range(s, gs >> 1, gs & 1, tc_item_starts(s, n_split, gs >> 1))) m |= 1u << b;
-  }
-  return m;
-}
 static_assert(tc_spec(0).n_ft() <= 32 && tc_spec(1).n_ft() <= 32 && tc_spec(2).n_ft() <= 32, "boundary mask");
-static_assert(tc_edge_mask(tc_spec(0), 1) == 0x1fffeu && tc_edge_mask(tc_spec(1), 1) == 1u << 12,
-              "contour: every tile a range of its own; onset: the slot boundary only");
+static_assert(tc_edge_mask(tc_spec(0), 1u) == 0x1fffeu && tc_edge_mask(tc_spec(1), 1u) == 1u << 12 &&
+                  tc_edge_mask(tc_spec(2), 1u) == 1u << 12,
+              "whole M-tiles: contour: every tile a range of its own; onset / note: the slot boundary only");
 
 // contour: one thread per frame; pitch layers: per (frame, bin); each fixes the boundaries of the mask
 template <int LAYER>
@@ -1407,7 +1436,9 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
     const int tt = t - kOverlapHalf;
     if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
   }
-  for (uint32_t m = a.edges; m; m &= m - 1) edge_fix_boundary<LAYER>(a, __ffs(m) - 1, R, b, t, uf, k);
+  // the mask of the M-tile that finishes row R (tc_schedule: whole M-tiles first, then the tail)
+  for (uint32_t m = R < a.tail_row0 ? a.edges_full : a.edges_tail; m; m &= m - 1)
+    edge_fix_boundary<LAYER>(a, __ffs(m) - 1, R, b, t, uf, k);
 }
 // ------------------------------------------------------------------------------------------------
 int tc_rows_total(int n_windows, int rows_per_window) {
@@ -1438,6 +1469,98 @@ size_t tc_edge_floats(const TcConvSpec& sp, int n_windows) {
   return (size_t)(sp.n_ft() - 1) * 2 * sp.edge_per_side() * ((size_t)n_mtiles * ms);  // one slot per tile boundary
 }
 
+// ------------------------------------------------------------------------------------------------
+// The items of a launch.  Cutting every M-tile into k equal runs of groups, the item order (it / k, it % k) pinned every
+// CTA to one run when k divides the grid (132 = 2 x 2 x 3 x 11), and the runs are not equal work: the launch waited for
+// the CTAs of the heaviest run.  Instead the first n_full = floor(n_mtiles / grid) x grid M-tiles run whole, the same
+// number per CTA, and only the n_tail < grid M-tiles after them (all of a small batch) are cut, into the number of
+// group ranges, with boundaries of balanced estimated cost, that gives the least estimated time of the busiest CTA.
+// Cost of a group, contour: its MMA uses (the slot programs' words) plus kEpiUses per tile for the epilogue; onset /
+// note: its tiles (every tile of a pitch layer is the same gather).  Per item the data-tile load adds kItemUsesContour /
+// kItemTilesPitch.
+// The weights follow the cycle accounting of the contour kernel (DESIGN 4.1): the epilogue takes about as many
+// consumer cycles as 14 MMA uses per tile, the data-tile wait about 20 per item; the ring steps are not counted on
+// their own, since the consumers set the pace (the producer waits for a free stage most of its time).
+// ------------------------------------------------------------------------------------------------
+namespace tc {
+constexpr double kEpiUses = 14.0, kItemUsesContour = 20.0, kItemTilesPitch = 0.25;
+}
+// per-group cost and per-item cost of a layer, in the units above
+static void tc_group_costs(int layer, std::vector<double>& cost, double& item) {
+  using namespace tc;
+  const TcConvSpec sp = tc_spec(layer);
+  cost.assign(sp.G0, 0.0);
+  for (int g = 0; g < sp.G0; ++g)
+    for (int sl = 0; sl < 2; ++sl) cost[g] += tc_group_tile(sp, g, sl) >= 0 ? (layer == 0 ? kEpiUses : 1.0) : 0.0;
+  item = layer == 0 ? kItemUsesContour : kItemTilesPitch;
+  if (layer != 0) return;
+  // the contour program depends on the geometry alone (TcConvPlan::build): plan it once, with any weights
+  static const std::vector<double> uses = [] {
+    const TcConvSpec s = tc_spec(0);
+    std::vector<float> w((size_t)s.COUT * s.n_ci * s.KH * s.KW, 0.f);
+    TcConvPlan pl;
+    pl.build(s, w.data());
+    std::vector<double> u(s.G0, 0.0);
+    for (int g = 0; g < s.G0; ++g)
+      for (int st = pl.group_step_off[g]; st < pl.group_step_off[g + 1]; ++st)
+        for (int sl = 0; sl < 2; ++sl) u[g] += pl.slot_words[sl][st] != kNoUse ? 1.0 : 0.0;
+    return u;
+  }();
+  for (int g = 0; g < sp.G0; ++g) cost[g] += uses[g];
+}
+
+TcSchedule tc_schedule(int layer, bool fused, int n_windows, int n_sms, int* ms_out) {
+  const TcConvSpec sp = tc_spec(layer);
+  const int h2 = fused || layer != 0 ? (sp.KH2 - 1) / 2 : 0;
+  const int ms = tc::kMTile - 2 * h2;
+  if (ms_out) *ms_out = ms;
+  std::vector<double> cost;
+  double item;
+  tc_group_costs(layer, cost, item);
+  const int G = sp.G0;
+  std::vector<double> pre(G + 1, 0.0);
+  for (int g = 0; g < G; ++g) pre[g + 1] = pre[g] + cost[g];
+  TcSchedule s{};
+  s.n_mtiles = (n_windows * sp.rows_per_window + ms - 1) / ms;
+  s.n_full = s.n_mtiles / n_sms * n_sms;
+  s.n_tail = s.n_mtiles - s.n_full;
+  s.n_ranges = 1;
+  s.bounds[0] = 0, s.bounds[1] = (unsigned char)G;
+  if (s.n_tail > 0) {
+    // best[r][g]: the least largest range cost of the groups [g, G) cut into r ranges, cut[r][g] its first range's end
+    std::vector<std::vector<double>> best(G + 1, std::vector<double>(G + 1, 1e300));
+    std::vector<std::vector<int>> cut(G + 1, std::vector<int>(G + 1, G));
+    for (int g = 0; g < G; ++g) best[1][g] = pre[G] - pre[g];
+    for (int r = 2; r <= G; ++r)
+      for (int g = 0; g + r <= G; ++g)
+        for (int e = g + 1; e + r - 1 <= G; ++e) {
+          const double v = std::max(pre[e] - pre[g], best[r - 1][e]);
+          if (v < best[r][g]) best[r][g] = v, cut[r][g] = e;
+        }
+    // every CTA runs n_full / grid whole M-tiles; the tail items j = c, c + grid, ... of CTA c decide the busiest one
+    double best_t = 1e300;
+    for (int r = 1; r <= G; ++r) {
+      unsigned char b[16];
+      b[0] = 0;
+      for (int q = 0; q < r; ++q) b[q + 1] = (unsigned char)(q + 1 < r ? cut[r - q][b[q]] : G);
+      const int n_items = s.n_tail * r, grid = s.n_full ? n_sms : std::min(n_items, n_sms);
+      double worst = 0.0;
+      for (int c = 0; c < grid && c < n_items; ++c) {
+        double t = 0.0;
+        for (int j = c; j < n_items; j += grid) t += pre[b[j / s.n_tail + 1]] - pre[b[j / s.n_tail]] + item;
+        worst = std::max(worst, t);
+      }
+      if (worst < best_t * (1.0 - 1e-9)) {  // (a tie: fewer ranges, fewer items and edges)
+        best_t = worst;
+        s.n_ranges = r;
+        std::copy_n(b, r + 1, s.bounds);
+      }
+    }
+  }
+  s.grid = std::min(s.n_items(), n_sms);
+  return s;
+}
+
 // The conv kernel of one layer and, for a fused epilogue, the fix-up of the bins where two tile ranges meet.
 template <int LAYER, bool FUSED>
 static void launch_layer(const TcArgs& a, const EdgeFixArgs& ef, int grid, cudaStream_t st) {
@@ -1460,28 +1583,17 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   a.o = o;
   a.rows_total = rows_stride;  // row stride of the split layout (fixed per model, independent of the batch)
   a.h2 = fused ? (sp.KH2 - 1) / 2 : 0;
-  a.ms = tc::kMTile - 2 * a.h2;
-  a.n_mtiles = (n_windows * sp.rows_per_window + a.ms - 1) / a.ms;
-  a.edge_rows = a.n_mtiles * a.ms;
+  // An item is (M-tile, range of frequency groups): whole M-tiles, the same number per CTA, then the last M-tiles cut
+  // into group ranges of balanced cost (tc_schedule)
+  a.sch = tc_schedule(dev.layer, fused, n_windows, n_sms, &a.ms);
+  a.edge_rows = a.sch.n_mtiles * a.ms;
   a.n_windows = n_windows;
-  // An item is (M-tile, one of `split` runs of frequency groups).  Pick the split that minimises the number of waves
-  // times the work per item, the data-tile load counted as half a group: full chunks run unsplit, partial chunks and
-  // small batches spread over all SMs.
-  int split = 1;
-  double best = 1e30;
-  for (int s = 1; s <= sp.G0; ++s) {  // G0 groups
-    const int waves = (a.n_mtiles * s + n_sms - 1) / n_sms;
-    const double cost = waves * ((sp.G0 + s - 1) / s + 0.5);
-    if (cost < best - 1e-9) best = cost, split = s;
-  }
-  a.n_split = split;
   a.row0 = sp.lead_rows - sp.PT - a.h2;
   a.chunks8 = sp.chunks8;
   std::copy_n(dev.bias1, 32, a.bias1);
   a.bias2 = dev.bias2;
   std::copy_n(dev.note_w, 9, a.note_w);
-  const int n_items = a.n_mtiles * a.n_split;
-  const int grid = n_items < n_sms ? n_items : n_sms;
+  const int grid = a.sch.grid;
   {
     // tensor map of the split input: dims (innermost first) 8 elements, rows, 8-bin chunks, hi / lo plane
     using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1517,7 +1629,9 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   ef.o = o;
   ef.edge_rows = a.edge_rows;
   ef.n_rows = n_windows * sp.rows_per_window;
-  ef.edges = tc_edge_mask(sp, split);  // the conv kernel's own range predicate
+  ef.edges_full = tc_edge_mask(sp, 1u);  // the conv kernel's own range predicate
+  ef.edges_tail = tc_edge_mask(sp, a.sch.tail_starts());
+  ef.tail_row0 = a.sch.n_full * a.ms;
   ef.n_windows = n_windows;
   ef.bias2 = dev.bias2;
   std::copy_n(dev.note_w, 9, ef.note_w);

@@ -623,6 +623,15 @@ int bp_debug_tc_gather_packed(int which, const float* w, int32_t* sizes, uint16_
  * (may be NULL to query sizes): n_tiles x [plane hi/lo][k-chunk 2][n N][8] bf16. */
 int bp_debug_tc_b2(int which, const float* w2, int32_t* sizes, uint16_t* tiles);
 
+/* Host-only: the items one launch of a tensor-core conv kernel runs for a batch of n_windows on n_sms SMs (csrc/tc_conv.cu,
+ * tc_schedule), which = 0 contour (fused != 0: with its conv2 fused, the forward path 1), 1 onset, 2 note.  CTA c of the
+ * launch runs items c, c + grid, ...  sizes[8] = {n_items, grid, n_mtiles, whole M-tiles (items 0 .. n_full - 1),
+ * group ranges of the other M-tiles, frames an M-tile finishes (ms), first frame row of the cut M-tiles (n_full * ms),
+ * frequency groups}; items (may be NULL): [n_items][3] the item's M-tile and its groups [g0, g1); edges (may be NULL):
+ * [2] bit b = boundary b between frequency tiles b - 1 and b is finished by edge_fix_kernel in the rows of whole M-tiles
+ * (edges[0]) and in the rows of cut M-tiles (edges[1]). */
+int bp_debug_tc_schedule(int which, int fused, int n_windows, int n_sms, int32_t* sizes, int32_t* items, uint32_t* edges);
+
 /* Per-kernel device timing for the roofline line of bench.py: records CUDA events on the launching
  * stream around every launch of one kernel family (0 = contour conv 3x39, 1 = onset conv 5x5,
  * 2 = CQT projection + log-normalise, 3 = decimation chain, 4 = the remaining small convs,
@@ -638,6 +647,10 @@ int bp_model_profile_read(bp_model_t* m, double* total_ms, int64_t* n_intervals,
  * weight stage, issuing / waiting for MMAs, in the epilogue, waiting on the data tile, other; producer waiting on a free
  * stage, waiting on the data tile to be released, other.  reset != 0 zeroes the sums after the copy. */
 int bp_debug_tc_clocks(bp_model_t* m, int which, uint64_t* cycles, int reset);
+/* Busy time of every CTA of the tensor-core conv kernels (tools/tc_balance.py), also only with -DBP_TC_CLOCKS.
+ * Synchronises the device and copies ns[i] = the %globaltimer nanoseconds CTA i (blockIdx.x, i < n <= 256) spent from
+ * its start to the end of its last MMA warp, summed over all launches of layer `which` since the last reset. */
+int bp_debug_tc_cta_busy(bp_model_t* m, int which, uint64_t* ns, int n, int reset);
 
 #ifdef __cplusplus
 }
