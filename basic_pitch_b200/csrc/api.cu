@@ -820,6 +820,39 @@ int grid_notes_result(const std::string& api, const GridNotes& g) {
   return BP_OK;
 }
 
+// The posteriorgrams of a grid call (the salience scorers' one in `contour`), in device memory or, when `host`, in host
+// memory.
+struct Grams {
+  const float *note, *onset, *contour;
+  bool host;
+};
+
+// Uploads a grid call's host posteriorgrams of `total` frames once for the whole grid on m->stream and points `g` at the
+// model's staging; device memory is left where it is.  gram_width 0: the note and onset rows, and the contour rows when
+// `contour`, into the row staging; otherwise the salience posteriorgram, total x gram_width, into st_contour.
+int stage_grams(bp_model* m, int64_t total, Grams& g, bool contour, int gram_width = 0) {
+  if (!g.host) return BP_OK;
+  cudaStream_t st = m->stream;
+  if (gram_width > 0) {
+    if (total > 0) {
+      CK(m->st_contour.reserve((size_t)total * gram_width));
+      CK(cudaMemcpyAsync(m->st_contour.p, g.contour, sizeof(float) * total * gram_width, cudaMemcpyHostToDevice, st));
+    }
+    g = Grams{nullptr, nullptr, m->st_contour.p, false};
+    return BP_OK;
+  }
+  const int rc = reserve_rows(m, total);
+  if (rc) return rc;
+  if (total > 0) {
+    CK(cudaMemcpyAsync(m->st_note.p, g.note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->st_onset.p, g.onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
+    if (contour)
+      CK(cudaMemcpyAsync(m->st_contour.p, g.contour, sizeof(float) * total * kContourBins, cudaMemcpyHostToDevice, st));
+  }
+  g = Grams{m->st_note.p, m->st_onset.p, m->st_contour.p, false};
+  return BP_OK;
+}
+
 // ---- scoring (bp_score_*) ----------------------------------------------------------------------------------------------
 
 int check_score_params(const std::string& api, const bp_score_params_t* sp) {
@@ -926,6 +959,86 @@ ScoreRefs refs_at(const unsigned char* d, const size_t* o) {
   return ScoreRefs{reinterpret_cast<const long long*>(d + o[0]), reinterpret_cast<const double*>(d + o[1]),
                    reinterpret_cast<const double*>(d + o[2]), reinterpret_cast<const double*>(d + o[3]),
                    reinterpret_cast<const int*>(d + o[4])};
+}
+
+// What the note scorers read, uploaded once per call to m->score_in.
+struct NoteRefs {
+  ScoreRefs sr;
+  const int* r_orig;  // each reference's index within its file or item before sorting
+  ScoreTol tol;
+  ScoreEst e;  // the uploaded part of the estimates: a grid's frame_t and log2_midi, or the explicit notes
+  long long n_refs;
+};
+
+// The references of n_files files, the seconds of every frame a note of files of frame offsets foff can start or end
+// on and, unless est_log2_hz is NULL, the log2(Hz) table of the estimates; without it the references are intervals only
+// (their log2_hz is not read).
+int upload_note_refs(bp_model* m, const bp_note_set_t* refs, int n_files, const std::vector<long long>& foff,
+                     const bp_score_params_t& sp, const double* est_log2_hz, NoteRefs& nr, cudaStream_t st) {
+  long long max_t = 0;
+  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
+  nr.tol = score_tol(sp);
+  Pack pk;
+  size_t o_ref[6];
+  bp_note_set_t r = *refs;
+  if (!est_log2_hz) r.log2_hz = nullptr;
+  pack_refs(&r, n_files, pk, o_ref, nr.tol);
+  std::vector<double> frame_t(max_t + 1);
+  bp_frame_times(max_t + 1, frame_t.data());
+  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
+  const size_t o_l2 = est_log2_hz ? pk.add(est_log2_hz, sizeof(double) * 128) : 0;
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = m->score_in.p;
+  nr.sr = refs_at(d, o_ref);
+  nr.r_orig = reinterpret_cast<const int*>(d + o_ref[5]);
+  nr.e = ScoreEst{};
+  nr.e.frame_t = reinterpret_cast<const double*>(d + o_ft);
+  if (est_log2_hz) nr.e.log2_midi = reinterpret_cast<const double*>(d + o_l2);
+  nr.n_refs = refs->note_off[n_files];
+  return BP_OK;
+}
+
+// The prologue of the explicit-notes scorers (bp_score_notes_host, bp_match_notes_host,
+// bp_score_onset_offset_notes_host): arguments and score params, then, unless there are no items, the output and both
+// note sets (intervals only unless `pitched`).
+int check_notes_call(const std::string& api, const bp_model* m, const bp_note_set_t* est, const bp_note_set_t* refs,
+                     int n_items, const bp_score_params_t* sp, const void* out, bool pitched) {
+  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  int rc = check_score_params(api, sp);
+  if (rc || n_items == 0) return rc;
+  if (!out) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_note_set(api, "estimates", "item", est, n_items, pitched);
+  return rc ? rc : check_note_set(api, "references", "item", refs, n_items, pitched);
+}
+
+// One upload of an explicit-notes call (bp_*_notes_host) to m->score_in: the references of n items, then the estimates
+// (note_off, onset, offset and, when `pitched`, log2_hz); without `pitched` both are intervals only.
+int upload_notes(bp_model* m, const bp_note_set_t& est, const bp_note_set_t* refs, int n, const bp_score_params_t& sp,
+                 bool pitched, NoteRefs& nr, cudaStream_t st) {
+  nr.tol = score_tol(sp);
+  Pack pk;
+  size_t o_ref[6], o_est[4];
+  bp_note_set_t r = *refs;
+  if (!pitched) r.log2_hz = nullptr;
+  pack_refs(&r, n, pk, o_ref, nr.tol);
+  const long long n_est = est.note_off[n];
+  o_est[0] = pk.add(est.note_off, sizeof(long long) * (n + 1));
+  o_est[1] = pk.add(est.onset_s, sizeof(double) * n_est);
+  o_est[2] = pk.add(est.offset_s, sizeof(double) * n_est);
+  if (pitched) o_est[3] = pk.add(est.log2_hz, sizeof(double) * n_est);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = m->score_in.p;
+  nr.sr = refs_at(d, o_ref);
+  nr.r_orig = reinterpret_cast<const int*>(d + o_ref[5]);
+  nr.e = ScoreEst{};
+  nr.e.off = reinterpret_cast<const long long*>(d + o_est[0]);
+  nr.e.onset = reinterpret_cast<const double*>(d + o_est[1]);
+  nr.e.offset = reinterpret_cast<const double*>(d + o_est[2]);
+  if (pitched) nr.e.log2hz = reinterpret_cast<const double*>(d + o_est[3]);
+  nr.n_refs = refs->note_off[n];
+  return BP_OK;
 }
 
 // Matching workspace per launch (include/bp_b200.h, bp_match_grid_*): consecutive pairs share a launch while their
@@ -1921,10 +2034,8 @@ int64_t bp_decode_grid_chunk_params(int64_t total_frames, int32_t n_files) {
   return std::max(1LL, std::min(kDecodeGridMaxChunk, kDecodeGridChunkBytes / per));
 }
 
-int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
-                          const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
-                          bp_notes_t* notes, void* stream) {
-  const std::string api = "bp_decode_grid_device";
+static int decode_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
+                       const bp_decode_params_t* params, int32_t n_params, bp_notes_t* notes, cudaStream_t st) {
   bool any_bends = false;
   int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
   if (rc) return rc;
@@ -1935,41 +2046,32 @@ int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_ons
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long total_frames = foff[n_files];
-  if (total_frames > 0 && (!d_note || !d_onset || (any_bends && !d_contour)))
+  if (total_frames > 0 && (!g.note || !g.onset || (any_bends && !g.contour)))
     return fail(BP_E_INVALID, api + ": null posteriorgram");
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DeviceGuard dg(m->device);
+  rc = stage_grams(m, total_frames, g, any_bends);  // uploaded once for the whole grid
+  if (rc) return rc;
   GridNotes gn;  // over the grid so far
-  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+  rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
                           const std::vector<int>& counts, const std::vector<long long>&) -> int {
-    return grid_chunk_notes(m, api, d_note, d_contour, params, true, n_files, p0, P, counts, notes, gn, st);
+    return grid_chunk_notes(m, api, g.note, g.contour, params, true, n_files, p0, P, counts, notes, gn, st);
   });
   if (rc) return rc;
   return grid_notes_result(api, gn);
 }
 
+int bp_decode_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                          const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                          bp_notes_t* notes, void* stream) {
+  return decode_grid("bp_decode_grid_device", m, Grams{d_note, d_onset, d_contour, false}, h_frame_off, n_files, params,
+                     n_params, notes, static_cast<cudaStream_t>(stream));
+}
+
 int bp_decode_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
                         const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
                         bp_notes_t* notes) {
-  bool any_bends = false;
-  const int rc0 = check_grid_args("bp_decode_grid_host", m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (rc0) return rc0;
-  if (n_files == 0 || n_params == 0)
-    return bp_decode_grid_device(m, nullptr, nullptr, nullptr, h_frame_off, n_files, params, n_params, notes, m->stream);
-  DeviceGuard g(m->device);
-  const int64_t total = h_frame_off[n_files];
-  cudaStream_t st = m->stream;
-  const int rc = reserve_rows(m, total);
-  if (rc) return rc;
-  if (total > 0) {  // uploaded once for the whole grid
-    if (!h_note || !h_onset || (any_bends && !h_contour)) return fail(BP_E_INVALID, "bp_decode_grid_host: null posteriorgram");
-    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    if (any_bends)
-      CK(cudaMemcpyAsync(m->st_contour.p, h_contour, sizeof(float) * total * kContourBins, cudaMemcpyHostToDevice, st));
-  }
-  return bp_decode_grid_device(m, m->st_note.p, m->st_onset.p, m->st_contour.p, h_frame_off, n_files, params, n_params,
-                               notes, st);
+  return decode_grid("bp_decode_grid_host", m, Grams{h_note, h_onset, h_contour, true}, h_frame_off, n_files, params,
+                     n_params, notes, m ? m->stream : nullptr);
 }
 
 void bp_default_score_params(bp_score_params_t* p) {
@@ -1999,77 +2101,57 @@ int bp_frame_times(int64_t n, double* out) {
 
 namespace {
 
-// Everything bp_score_grid_* and bp_match_grid_* check before anything is enqueued, in addition to check_grid_args.
+// Everything bp_score_grid_*, bp_match_grid_* and bp_score_onset_offset_grid_* check before anything is enqueued, in
+// addition to check_grid_args.  Without `pitched` (onset-only and offset-only scores) the pitch_tolerance is validated as
+// elsewhere but unused, and neither the estimate table nor the references' log2_hz is read.
 int check_score_grid(const std::string& api, int n_files, int n_params, const bp_note_set_t* refs,
-                     const bp_score_params_t* sp, const double* est_log2_hz, const void* h_counts) {
+                     const bp_score_params_t* sp, const double* est_log2_hz, const void* out, bool pitched) {
   int rc = check_score_params(api, sp);
   if (rc || n_files == 0 || n_params == 0) return rc;
-  if (!h_counts || !est_log2_hz) return fail(BP_E_INVALID, api + ": bad argument");
-  for (int k = 0; k < 128; ++k)
+  if (!out || (pitched && !est_log2_hz)) return fail(BP_E_INVALID, api + ": bad argument");
+  for (int k = 0; pitched && k < 128; ++k)
     if (!std::isfinite(est_log2_hz[k]))
       return fail(BP_E_INVALID, api + ": estimate table entry " + std::to_string(k) + ": non-finite log2_hz");
-  return check_note_set(api, "references", "file", refs, n_files);
-}
-
-// Everything bp_score_onset_offset_grid_* check before anything is enqueued, in addition to check_grid_args: the
-// pitch_tolerance is validated as elsewhere but unused, and the references' log2_hz is not read.
-int check_onset_offset_grid(const std::string& api, int n_files, int n_params, const bp_note_set_t* refs,
-                            const bp_score_params_t* sp, const void* h_counts) {
-  int rc = check_score_params(api, sp);
-  if (rc || n_files == 0 || n_params == 0) return rc;
-  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
-  return check_note_set(api, "references", "file", refs, n_files, false);
+  return check_note_set(api, "references", "file", refs, n_files, pitched);
 }
 
 }  // namespace
 
 extern "C" {
 
-int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
-                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
-                         const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts, void* stream) {
-  const std::string api = "bp_score_grid_device";
+// bp_score_grid_*, and without `pitched` bp_score_onset_offset_grid_* (the references intervals only, no estimate table).
+static int score_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
+                      const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                      const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts, bool pitched,
+                      cudaStream_t st) {
   bool any_bends = false;
   int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_counts);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_counts, pitched);
   if (rc) return rc;
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long total_frames = foff[n_files];
-  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  long long max_t = 0;
-  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
-  // one upload per call: the references, the seconds of every frame a note can start or end on, the log2(Hz) table
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  pack_refs(refs, n_files, pk, o_ref, tol);
-  std::vector<double> frame_t(max_t + 1);
-  bp_frame_times(max_t + 1, frame_t.data());
-  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
-  const size_t o_l2 = pk.add(est_log2_hz, sizeof(double) * 128);
-  const long long n_refs = refs->note_off[n_files];
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  if (total_frames > 0 && (!g.note || !g.onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  NoteRefs nr;
+  rc = stage_grams(m, total_frames, g, false);
+  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, pitched ? est_log2_hz : nullptr, nr, st);
+  if (rc) return rc;
   CK(m->score_counts.reserve((size_t)n_params * n_files * 4));
-  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
-  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+  rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
                           const std::vector<int>&, const std::vector<long long>& soff) -> int {
     const long long n_pairs = (long long)P * n_files;
-    CK(m->score_ws_ref.reserve((size_t)(2 * P * n_refs) + 1));
-    CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs]) + 1));
-    ScoreEst e{};
+    CK(m->score_ws_ref.reserve((size_t)((pitched ? 2 : 6) * P * nr.n_refs) + 1));
+    CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs] + (pitched ? 0 : 2 * n_pairs)) + 1));
+    ScoreEst e = nr.e;
     e.off = m->d_slot_off.p;
     e.count = m->note_count.p;
     e.start = m->slot_start.p;
     e.end = m->slot_end.p;
-    e.pitch = m->slot_pitch.p;
-    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
-    e.log2_midi = reinterpret_cast<const double*>(m->score_in.p + o_l2);
-    launch_score_match(sr, e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_files, n_pairs,
-                       m->score_counts.p + 4 * p0 * n_files, st);
+    if (pitched) e.pitch = m->slot_pitch.p;
+    (pitched ? launch_score_match : launch_onset_offset)(nr.sr, e, nr.tol,
+                                                         ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, nr.n_refs},
+                                                         n_files, n_pairs, m->score_counts.p + 4 * p0 * n_files, st);
     CKL();
     m->launches += 1;
     return BP_OK;
@@ -2080,63 +2162,48 @@ int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onse
   return BP_OK;
 }
 
+int bp_score_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts, void* stream) {
+  return score_grid("bp_score_grid_device", m, Grams{d_note, d_onset, nullptr, false}, h_frame_off, n_files, params,
+                    n_params, refs, sp, est_log2_hz, h_counts, true, static_cast<cudaStream_t>(stream));
+}
+
 int bp_score_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
                        int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
                        const bp_score_params_t* sp, const double* est_log2_hz, int64_t* h_counts) {
-  const std::string api = "bp_score_grid_host";
-  bool any_bends = false;
-  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  DeviceGuard g(m->device);
-  const int64_t total = h_frame_off[n_files];
-  cudaStream_t st = m->stream;
-  rc = reserve_rows(m, total);
-  if (rc) return rc;
-  if (total > 0) {  // uploaded once for the whole grid
-    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
-    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-  }
-  return bp_score_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, sp,
-                              est_log2_hz, h_counts, st);
+  return score_grid("bp_score_grid_host", m, Grams{h_note, h_onset, nullptr, true}, h_frame_off, n_files, params,
+                    n_params, refs, sp, est_log2_hz, h_counts, true, m ? m->stream : nullptr);
 }
 
-int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
-                        const bp_score_params_t* sp, int64_t* h_counts) {
-  const std::string api = "bp_score_notes_host";
-  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
-  int rc = check_score_params(api, sp);
+// bp_score_notes_host, and without `pitched` bp_score_onset_offset_notes_host (intervals only).
+static int score_notes(const std::string& api, bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs,
+                       int32_t n_items, const bp_score_params_t* sp, int64_t* h_counts, bool pitched) {
+  int rc = check_notes_call(api, m, est, refs, n_items, sp, h_counts, pitched);
   if (rc || n_items == 0) return rc;
-  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
-  rc = check_note_set(api, "estimates", "item", est, n_items);
-  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items);
-  if (rc) return rc;
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  pack_refs(refs, n_items, pk, o_ref, tol);
   const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
-  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
-  const size_t o_eon = pk.add(est->onset_s, sizeof(double) * n_est);
-  const size_t o_eoffs = pk.add(est->offset_s, sizeof(double) * n_est);
-  const size_t o_el2 = pk.add(est->log2_hz, sizeof(double) * n_est);
+  bp_note_set_t e = *est;
+  std::vector<double> on, off;
+  if (!pitched) {  // the count does not depend on the order of the estimates: each item's onsets and offsets go up sorted, apart
+    on.assign(est->onset_s, est->onset_s + n_est);
+    off.assign(est->offset_s, est->offset_s + n_est);
+    for (int i = 0; i < n_items; ++i) {
+      std::sort(on.begin() + est->note_off[i], on.begin() + est->note_off[i + 1]);
+      std::sort(off.begin() + est->note_off[i], off.begin() + est->note_off[i + 1]);
+    }
+    e = bp_note_set_t{est->note_off, on.data(), off.data(), nullptr};
+  }
   DeviceGuard g(m->device);
   cudaStream_t st = m->stream;
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(m->score_ws_ref.reserve((size_t)(2 * n_refs) + 1));
-  CK(m->score_ws_est.reserve((size_t)(4 * n_est) + 1));
+  NoteRefs nr;
+  rc = upload_notes(m, e, refs, n_items, *sp, pitched, nr, st);
+  if (rc) return rc;
+  CK(m->score_ws_ref.reserve((size_t)((pitched ? 2 : 6) * n_refs) + 1));
+  CK(m->score_ws_est.reserve((size_t)(4 * n_est + (pitched ? 0 : 2 * n_items)) + 1));
   CK(m->score_counts.reserve((size_t)n_items * 4));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  const unsigned char* d = m->score_in.p;
-  ScoreEst e{};
-  e.off = reinterpret_cast<const long long*>(d + o_eoff);
-  e.onset = reinterpret_cast<const double*>(d + o_eon);
-  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
-  e.log2hz = reinterpret_cast<const double*>(d + o_el2);
-  launch_score_match(refs_at(d, o_ref), e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_items,
-                     n_items, m->score_counts.p, st);
+  (pitched ? launch_score_match : launch_onset_offset)(nr.sr, nr.e, nr.tol,
+                                                       ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_items,
+                                                       n_items, m->score_counts.p, st);
   CKL();
   m->launches += 1;
   CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_items, cudaMemcpyDeviceToHost, st));
@@ -2144,14 +2211,18 @@ int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_s
   return BP_OK;
 }
 
-int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
-                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
-                         const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match,
-                         void* stream) {
-  const std::string api = "bp_match_grid_device";
+int bp_score_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
+                        const bp_score_params_t* sp, int64_t* h_counts) {
+  return score_notes("bp_score_notes_host", m, est, refs, n_items, sp, h_counts, true);
+}
+
+static int match_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
+                      const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                      const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match,
+                      cudaStream_t st) {
   bool any_bends = false;
   int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_match);
+  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_match, true);
   if (rc) return rc;
   if (!notes || !notes->note_off || !notes->bend_off) return fail(BP_E_INVALID, api + ": notes arrays missing");
   g_need_notes = g_need_bends = 0;
@@ -2160,30 +2231,18 @@ int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onse
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long total_frames = foff[n_files];
-  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  long long max_t = 0;
-  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
-  // one upload per call: the references, the seconds of every frame a note can start or end on, the log2(Hz) table
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  pack_refs(refs, n_files, pk, o_ref, tol);
-  std::vector<double> frame_t(max_t + 1);
-  bp_frame_times(max_t + 1, frame_t.data());
-  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
-  const size_t o_l2 = pk.add(est_log2_hz, sizeof(double) * 128);
-  const long long n_refs = refs->note_off[n_files];
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
-  const int* r_orig = reinterpret_cast<const int*>(m->score_in.p + o_ref[5]);
+  if (total_frames > 0 && (!g.note || !g.onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  NoteRefs nr;
+  rc = stage_grams(m, total_frames, g, false);
+  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, est_log2_hz, nr, st);
+  if (rc) return rc;
+  const long long n_refs = nr.n_refs;
   GridNotes gn;  // over the grid so far
-  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+  rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
                           const std::vector<int>& counts, const std::vector<long long>&) -> int {
     const long long note0 = gn.n_notes, n_pairs = (long long)P * n_files;
-    int rc = grid_chunk_notes(m, api, d_note, nullptr, params, false, n_files, p0, P, counts, notes, gn, st);
+    int rc = grid_chunk_notes(m, api, g.note, nullptr, params, false, n_files, p0, P, counts, notes, gn, st);
     if (rc || !gn.notes_fit || n_refs == 0) return rc;
     int32_t* out = h_match + 2 * p0 * n_refs;
     if (gn.n_notes == note0) {  // no estimated note in this chunk
@@ -2197,14 +2256,13 @@ int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onse
     CK(cudaMemcpyAsync(m->match_est_off.p, est_off.data(), sizeof(long long) * (n_pairs + 1), cudaMemcpyHostToDevice,
                        st));
     CK(m->match_out.reserve((size_t)(2 * P * n_refs)));
-    ScoreEst e{};
+    ScoreEst e = nr.e;
     e.off = m->match_est_off.p;
     e.start = m->d_start.p;
     e.end = m->d_end.p;
     e.pitch = m->d_pitch.p;
-    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
-    e.log2_midi = reinterpret_cast<const double*>(m->score_in.p + o_l2);
-    rc = match_pairs(m, api, sr, r_orig, e, tol, n_files, n_pairs, est_off, refs->note_off, n_refs, m->match_out.p, st);
+    rc = match_pairs(m, api, nr.sr, nr.r_orig, e, nr.tol, n_files, n_pairs, est_off, refs->note_off, n_refs,
+                     m->match_out.p, st);
     if (rc) return rc;
     CK(cudaMemcpyAsync(out, m->match_out.p, sizeof(int) * 2 * P * n_refs, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2214,65 +2272,37 @@ int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onse
   return grid_notes_result(api, gn);
 }
 
+int bp_match_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                         int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
+                         const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match,
+                         void* stream) {
+  return match_grid("bp_match_grid_device", m, Grams{d_note, d_onset, nullptr, false}, h_frame_off, n_files, params,
+                    n_params, refs, sp, est_log2_hz, notes, h_match, static_cast<cudaStream_t>(stream));
+}
+
 int bp_match_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
                        int32_t n_files, const bp_decode_params_t* params, int32_t n_params, const bp_note_set_t* refs,
                        const bp_score_params_t* sp, const double* est_log2_hz, bp_notes_t* notes, int32_t* h_match) {
-  const std::string api = "bp_match_grid_host";
-  bool any_bends = false;
-  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_score_grid(api, n_files, n_params, refs, sp, est_log2_hz, h_match);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0)
-    return bp_match_grid_device(m, nullptr, nullptr, h_frame_off, n_files, params, n_params, refs, sp, est_log2_hz,
-                                notes, h_match, m->stream);
-  DeviceGuard g(m->device);
-  const int64_t total = h_frame_off[n_files];
-  cudaStream_t st = m->stream;
-  rc = reserve_rows(m, total);
-  if (rc) return rc;
-  if (total > 0) {  // uploaded once for the whole grid
-    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
-    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-  }
-  return bp_match_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, sp,
-                              est_log2_hz, notes, h_match, st);
+  return match_grid("bp_match_grid_host", m, Grams{h_note, h_onset, nullptr, true}, h_frame_off, n_files, params,
+                    n_params, refs, sp, est_log2_hz, notes, h_match, m ? m->stream : nullptr);
 }
 
 int bp_match_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs, int32_t n_items,
                         const bp_score_params_t* sp, int32_t* h_match) {
   const std::string api = "bp_match_notes_host";
-  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
-  int rc = check_score_params(api, sp);
+  int rc = check_notes_call(api, m, est, refs, n_items, sp, h_match, true);
   if (rc || n_items == 0) return rc;
-  if (!h_match) return fail(BP_E_INVALID, api + ": bad argument");
-  rc = check_note_set(api, "estimates", "item", est, n_items);
-  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items);
-  if (rc) return rc;
-  const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
+  const long long n_refs = refs->note_off[n_items];
   if (n_refs == 0) return BP_OK;
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  pack_refs(refs, n_items, pk, o_ref, tol);
-  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
-  const size_t o_eon = pk.add(est->onset_s, sizeof(double) * n_est);
-  const size_t o_eoffs = pk.add(est->offset_s, sizeof(double) * n_est);
-  const size_t o_el2 = pk.add(est->log2_hz, sizeof(double) * n_est);
   DeviceGuard g(m->device);
   cudaStream_t st = m->stream;
-  CK(m->score_in.reserve(pk.buf.size()));
+  NoteRefs nr;
+  rc = upload_notes(m, *est, refs, n_items, *sp, true, nr, st);
+  if (rc) return rc;
   CK(m->match_out.reserve((size_t)(2 * n_refs)));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  const unsigned char* d = m->score_in.p;
-  ScoreEst e{};
-  e.off = reinterpret_cast<const long long*>(d + o_eoff);
-  e.onset = reinterpret_cast<const double*>(d + o_eon);
-  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
-  e.log2hz = reinterpret_cast<const double*>(d + o_el2);
   const std::vector<long long> est_off(est->note_off, est->note_off + n_items + 1);
-  rc = match_pairs(m, api, refs_at(d, o_ref), reinterpret_cast<const int*>(d + o_ref[5]), e, tol, n_items, n_items,
-                   est_off, refs->note_off, n_refs, m->match_out.p, st);
+  rc = match_pairs(m, api, nr.sr, nr.r_orig, nr.e, nr.tol, n_items, n_items, est_off, refs->note_off, n_refs,
+                   m->match_out.p, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(h_match, m->match_out.p, sizeof(int) * 2 * n_refs, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -2285,127 +2315,21 @@ int bp_score_onset_offset_grid_device(bp_model_t* m, const float* d_note, const 
                                       const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
                                       int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* sp,
                                       const double* est_log2_hz, int64_t* h_counts, void* stream) {
-  const std::string api = "bp_score_onset_offset_grid_device";
-  (void)est_log2_hz;  // no pitch test
-  bool any_bends = false;
-  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_onset_offset_grid(api, n_files, n_params, refs, sp, h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
-  const long long total_frames = foff[n_files];
-  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  long long max_t = 0;
-  for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
-  // one upload per call: the references (intervals only) and the seconds of every frame a note can start or end on
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  bp_note_set_t r = *refs;
-  r.log2_hz = nullptr;
-  pack_refs(&r, n_files, pk, o_ref, tol);
-  std::vector<double> frame_t(max_t + 1);
-  bp_frame_times(max_t + 1, frame_t.data());
-  const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
-  const long long n_refs = refs->note_off[n_files];
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  CK(m->score_counts.reserve((size_t)n_params * n_files * 4));
-  const ScoreRefs sr = refs_at(m->score_in.p, o_ref);
-  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
-                          const std::vector<int>&, const std::vector<long long>& soff) -> int {
-    const long long n_pairs = (long long)P * n_files;
-    CK(m->score_ws_ref.reserve((size_t)(6 * P * n_refs) + 1));
-    CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs] + 2 * n_pairs) + 1));
-    ScoreEst e{};
-    e.off = m->d_slot_off.p;
-    e.count = m->note_count.p;
-    e.start = m->slot_start.p;
-    e.end = m->slot_end.p;
-    e.frame_t = reinterpret_cast<const double*>(m->score_in.p + o_ft);
-    launch_onset_offset(sr, e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_files, n_pairs,
-                        m->score_counts.p + 4 * p0 * n_files, st);
-    CKL();
-    m->launches += 1;
-    return BP_OK;
-  });
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_params * n_files, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return BP_OK;
+  return score_grid("bp_score_onset_offset_grid_device", m, Grams{d_note, d_onset, nullptr, false}, h_frame_off, n_files,
+                    params, n_params, refs, sp, est_log2_hz, h_counts, false, static_cast<cudaStream_t>(stream));
 }
 
 int bp_score_onset_offset_grid_host(bp_model_t* m, const float* h_note, const float* h_onset,
                                     const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
                                     int32_t n_params, const bp_note_set_t* refs, const bp_score_params_t* sp,
                                     const double* est_log2_hz, int64_t* h_counts) {
-  const std::string api = "bp_score_onset_offset_grid_host";
-  bool any_bends = false;
-  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_onset_offset_grid(api, n_files, n_params, refs, sp, h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  DeviceGuard g(m->device);
-  const int64_t total = h_frame_off[n_files];
-  cudaStream_t st = m->stream;
-  rc = reserve_rows(m, total);
-  if (rc) return rc;
-  if (total > 0) {  // uploaded once for the whole grid
-    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
-    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-  }
-  return bp_score_onset_offset_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs,
-                                           sp, est_log2_hz, h_counts, st);
+  return score_grid("bp_score_onset_offset_grid_host", m, Grams{h_note, h_onset, nullptr, true}, h_frame_off, n_files,
+                    params, n_params, refs, sp, est_log2_hz, h_counts, false, m ? m->stream : nullptr);
 }
 
 int bp_score_onset_offset_notes_host(bp_model_t* m, const bp_note_set_t* est, const bp_note_set_t* refs,
                                      int32_t n_items, const bp_score_params_t* sp, int64_t* h_counts) {
-  const std::string api = "bp_score_onset_offset_notes_host";
-  if (!m || n_items < 0) return fail(BP_E_INVALID, api + ": bad argument");
-  int rc = check_score_params(api, sp);
-  if (rc || n_items == 0) return rc;
-  if (!h_counts) return fail(BP_E_INVALID, api + ": bad argument");
-  rc = check_note_set(api, "estimates", "item", est, n_items, false);
-  if (!rc) rc = check_note_set(api, "references", "item", refs, n_items, false);
-  if (rc) return rc;
-  ScoreTol tol = score_tol(*sp);
-  Pack pk;
-  size_t o_ref[6];
-  bp_note_set_t r = *refs;
-  r.log2_hz = nullptr;
-  pack_refs(&r, n_items, pk, o_ref, tol);
-  // the count does not depend on the order of the estimates: each item's onsets and offsets go up sorted, apart
-  const long long n_est = est->note_off[n_items], n_refs = refs->note_off[n_items];
-  std::vector<double> on(est->onset_s, est->onset_s + n_est), off(est->offset_s, est->offset_s + n_est);
-  for (int i = 0; i < n_items; ++i) {
-    std::sort(on.begin() + est->note_off[i], on.begin() + est->note_off[i + 1]);
-    std::sort(off.begin() + est->note_off[i], off.begin() + est->note_off[i + 1]);
-  }
-  const size_t o_eoff = pk.add(est->note_off, sizeof(long long) * (n_items + 1));
-  const size_t o_eon = pk.add(on.data(), sizeof(double) * n_est);
-  const size_t o_eoffs = pk.add(off.data(), sizeof(double) * n_est);
-  DeviceGuard g(m->device);
-  cudaStream_t st = m->stream;
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(m->score_ws_ref.reserve((size_t)(6 * n_refs) + 1));
-  CK(m->score_ws_est.reserve((size_t)(4 * n_est + 2 * n_items) + 1));
-  CK(m->score_counts.reserve((size_t)n_items * 4));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  const unsigned char* d = m->score_in.p;
-  ScoreEst e{};
-  e.off = reinterpret_cast<const long long*>(d + o_eoff);
-  e.onset = reinterpret_cast<const double*>(d + o_eon);
-  e.offset = reinterpret_cast<const double*>(d + o_eoffs);
-  launch_onset_offset(refs_at(d, o_ref), e, tol, ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, n_refs}, n_items,
-                      n_items, m->score_counts.p, st);
-  CKL();
-  m->launches += 1;
-  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * 4 * n_items, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return BP_OK;
+  return score_notes("bp_score_onset_offset_notes_host", m, est, refs, n_items, sp, h_counts, false);
 }
 
 }  // extern "C"
@@ -2503,25 +2427,52 @@ void pack_mp_values(const bp_multipitch_set_t* s, long long F, Pack& pk, size_t*
   o[2] = pk.add(ch.data(), sizeof(double) * V);
 }
 
+// A value table of n MIDI numbers or posteriorgram bins (`what` "estimate table" / "bin table"): midi finite and
+// non-decreasing, chroma in [0, 12).
+int check_value_table(const std::string& api, const char* what, const double* midi, const double* chroma, int n) {
+  for (int k = 0; k < n; ++k) {
+    const std::string at = api + ": " + what + " entry " + std::to_string(k);
+    if (!std::isfinite(midi[k])) return fail(BP_E_INVALID, at + ": non-finite midi");
+    if (k > 0 && midi[k] < midi[k - 1]) return fail(BP_E_INVALID, at + ": midi decreases");
+    if (!(chroma[k] >= 0 && chroma[k] < 12)) return fail(BP_E_INVALID, at + ": chroma outside [0, 12)");
+  }
+  return BP_OK;
+}
+
 // Everything bp_score_frames_grid_* check before anything is enqueued, in addition to check_grid_args.
 int check_frames_grid(const std::string& api, int n_files, int n_params, const bp_multipitch_set_t* refs, double window,
                       const double* est_midi, const double* est_chroma, const int64_t* h_counts) {
   int rc = check_window(api, window);
   if (rc || n_files == 0 || n_params == 0) return rc;
   if (!h_counts || !est_midi || !est_chroma) return fail(BP_E_INVALID, api + ": bad argument");
-  for (int k = 0; k < 128; ++k) {
-    const std::string at = api + ": estimate table entry " + std::to_string(k);
-    if (!std::isfinite(est_midi[k])) return fail(BP_E_INVALID, at + ": non-finite midi");
-    if (k > 0 && est_midi[k] < est_midi[k - 1]) return fail(BP_E_INVALID, at + ": midi decreases");
-    if (!(est_chroma[k] >= 0 && est_chroma[k] < 12)) return fail(BP_E_INVALID, at + ": chroma outside [0, 12)");
-  }
-  return check_mp_set(api, "references", "file", refs, n_files);
+  rc = check_value_table(api, "estimate table", est_midi, est_chroma, 128);
+  return rc ? rc : check_mp_set(api, "references", "file", refs, n_files);
 }
 
 FrameRefs frame_refs_at(const unsigned char* d, size_t o_owner, size_t o_est, const size_t* o_val, long long K) {
   return FrameRefs{reinterpret_cast<const int*>(d + o_owner), reinterpret_cast<const int*>(d + o_est),
                    reinterpret_cast<const long long*>(d + o_val[0]), reinterpret_cast<const double*>(d + o_val[1]),
                    reinterpret_cast<const double*>(d + o_val[2]), K};
+}
+
+// The references of a frame-level grid call into `pk`: per reference frame its file and the frame of that file it reads
+// at the model's frame times (files of frame offsets foff), then the sorted values; offsets of the sections in o[5]
+// (owner, estimate frame, pack_mp_values' three).
+void pack_ref_frames(const bp_multipitch_set_t* refs, const std::vector<long long>& foff, int n_files, Pack& pk,
+                     size_t* o) {
+  const long long K = refs->frame_off[n_files];
+  std::vector<int> owner(K), est(K);
+  std::vector<double> et;
+  for (int f = 0; f < n_files; ++f) {
+    const long long T = foff[f + 1] - foff[f], k0 = refs->frame_off[f];
+    et.resize(T);
+    bp_frame_times(T, et.data());
+    multipitch_map(et.data(), T, refs->time_s + k0, refs->frame_off[f + 1] - k0, est.data() + k0);
+    std::fill(owner.begin() + k0, owner.begin() + refs->frame_off[f + 1], f);
+  }
+  o[0] = pk.add(owner.data(), sizeof(int) * K);
+  o[1] = pk.add(est.data(), sizeof(int) * K);
+  pack_mp_values(refs, K, pk, o + 2);
 }
 
 // Salience scoring (bp_score_salience_grid_*): posteriorgram widths up to this many bins; settings per chunk bounded by
@@ -2547,12 +2498,8 @@ int check_salience_grid(const std::string& api, const bp_model* m, int width, co
   int rc = check_window(api, window);
   if (rc || n_files == 0 || n_params == 0) return rc;
   if (!h_frame_off || !h_counts || !bin_midi || !bin_chroma) return fail(BP_E_INVALID, api + ": bad argument");
-  for (int b = 0; b < width; ++b) {
-    const std::string at = api + ": bin table entry " + std::to_string(b);
-    if (!std::isfinite(bin_midi[b])) return fail(BP_E_INVALID, at + ": non-finite midi");
-    if (b > 0 && bin_midi[b] < bin_midi[b - 1]) return fail(BP_E_INVALID, at + ": midi decreases");
-    if (!(bin_chroma[b] >= 0 && bin_chroma[b] < 12)) return fail(BP_E_INVALID, at + ": chroma outside [0, 12)");
-  }
+  rc = check_value_table(api, "bin table", bin_midi, bin_chroma, width);
+  if (rc) return rc;
   if (h_frame_off[0] != 0) return fail(BP_E_INVALID, api + ": frame_off[0] must be 0");
   for (int i = 0; i < n_files; ++i)
     if (h_frame_off[i + 1] < h_frame_off[i] || h_frame_off[i + 1] - h_frame_off[i] > INT_MAX)
@@ -2577,11 +2524,10 @@ int bp_multipitch_map(const double* est_t, int64_t n_est, const double* ref_t, i
   return BP_OK;
 }
 
-int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
-                                int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
-                                const bp_multipitch_set_t* refs, double window, const double* est_midi,
-                                const double* est_chroma, int64_t* h_counts, void* stream) {
-  const std::string api = "bp_score_frames_grid_device";
+static int score_frames_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
+                             const bp_decode_params_t* params, int32_t n_params, const bp_multipitch_set_t* refs,
+                             double window, const double* est_midi, const double* est_chroma, int64_t* h_counts,
+                             cudaStream_t st) {
   bool any_bends = false;
   int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
   if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts);
@@ -2589,32 +2535,23 @@ int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float*
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long total_frames = foff[n_files], cells = total_frames * kPitches;
-  if (total_frames > 0 && (!d_note || !d_onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  // one upload per call: per reference frame its file and the file's frame it reads, the sorted values, the tables
+  if (total_frames > 0 && (!g.note || !g.onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  rc = stage_grams(m, total_frames, g, false);
+  if (rc) return rc;
+  // one upload per call: the reference frames and the tables
   const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
-  std::vector<int> owner(K), est(K);
-  std::vector<double> et;
-  for (int f = 0; f < n_files; ++f) {
-    const long long T = foff[f + 1] - foff[f], k0 = refs->frame_off[f];
-    et.resize(T);
-    bp_frame_times(T, et.data());
-    multipitch_map(et.data(), T, refs->time_s + k0, refs->frame_off[f + 1] - k0, est.data() + k0);
-    std::fill(owner.begin() + k0, owner.begin() + refs->frame_off[f + 1], f);
-  }
   Pack pk;
-  const size_t o_owner = pk.add(owner.data(), sizeof(int) * K), o_est = pk.add(est.data(), sizeof(int) * K);
-  size_t o_val[3];
-  pack_mp_values(refs, K, pk, o_val);
+  size_t o_ref[5];
+  pack_ref_frames(refs, foff, n_files, pk, o_ref);
   const size_t o_tm = pk.add(est_midi, sizeof(double) * 128), o_tc = pk.add(est_chroma, sizeof(double) * 128);
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   CK(m->score_in.reserve(pk.buf.size()));
   CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
   const long long n_counts = (long long)n_params * n_files * kFrameCounts;
   CK(m->score_counts.reserve((size_t)n_counts));
   CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
-  const FrameRefs R = frame_refs_at(m->score_in.p, o_owner, o_est, o_val, K);
-  rc = decode_grid_chunks(m, api, d_note, d_onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+  const FrameRefs R = frame_refs_at(m->score_in.p, o_ref[0], o_ref[1], o_ref + 2, K);
+  rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
                           const std::vector<int>&, const std::vector<long long>&) -> int {
     // each setting's E is dead once the loops have run: it becomes that setting's count roll
     int* roll = reinterpret_cast<int*>(m->energy.p);
@@ -2640,28 +2577,21 @@ int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float*
   return BP_OK;
 }
 
+int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const int64_t* h_frame_off,
+                                int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                                const bp_multipitch_set_t* refs, double window, const double* est_midi,
+                                const double* est_chroma, int64_t* h_counts, void* stream) {
+  return score_frames_grid("bp_score_frames_grid_device", m, Grams{d_note, d_onset, nullptr, false}, h_frame_off,
+                           n_files, params, n_params, refs, window, est_midi, est_chroma, h_counts,
+                           static_cast<cudaStream_t>(stream));
+}
+
 int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const int64_t* h_frame_off,
                               int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
                               const bp_multipitch_set_t* refs, double window, const double* est_midi,
                               const double* est_chroma, int64_t* h_counts) {
-  const std::string api = "bp_score_frames_grid_host";
-  bool any_bends = false;
-  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  DeviceGuard g(m->device);
-  const int64_t total = h_frame_off[n_files];
-  cudaStream_t st = m->stream;
-  rc = reserve_rows(m, total);
-  if (rc) return rc;
-  if (total > 0) {  // uploaded once for the whole grid
-    if (!h_note || !h_onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
-    CK(cudaMemcpyAsync(m->st_note.p, h_note, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m->st_onset.p, h_onset, sizeof(float) * total * kPitches, cudaMemcpyHostToDevice, st));
-  }
-  return bp_score_frames_grid_device(m, m->st_note.p, m->st_onset.p, h_frame_off, n_files, params, n_params, refs, window,
-                                     est_midi, est_chroma, h_counts, st);
+  return score_frames_grid("bp_score_frames_grid_host", m, Grams{h_note, h_onset, nullptr, true}, h_frame_off, n_files,
+                           params, n_params, refs, window, est_midi, est_chroma, h_counts, m ? m->stream : nullptr);
 }
 
 int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, const bp_multipitch_set_t* refs,
@@ -2718,40 +2648,29 @@ int64_t bp_score_salience_chunk_params(int64_t n_ref_frames, int64_t n_ref_value
   return std::max(1LL, kSalienceChunkBytes / std::max(1LL, per));
 }
 
-int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t width, const int64_t* h_frame_off,
-                                  int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
-                                  const bp_multipitch_set_t* refs, double window, const double* bin_midi,
-                                  const double* bin_chroma, int64_t* h_counts, void* stream) {
-  const std::string api = "bp_score_salience_grid_device";
+static int score_salience_grid(const std::string& api, bp_model_t* m, Grams g, int32_t width,
+                               const int64_t* h_frame_off, int32_t n_files, const bp_salience_params_t* params,
+                               int32_t n_params, const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                               const double* bin_chroma, int64_t* h_counts, cudaStream_t st) {
   int rc = check_salience_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma,
                                h_counts);
   if (rc) return rc;
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
-  if (foff[n_files] > 0 && !d_gram) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  // one upload per call: per reference frame its file and the file's frame it reads, the sorted values, the bin tables
-  // and every setting
+  if (foff[n_files] > 0 && !g.contour) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  rc = stage_grams(m, foff[n_files], g, true, width);
+  if (rc) return rc;
+  // one upload per call: the reference frames, the bin tables and every setting
   const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
-  std::vector<int> owner(K), est(K);
-  std::vector<double> et;
-  for (int f = 0; f < n_files; ++f) {
-    const long long T = foff[f + 1] - foff[f], k0 = refs->frame_off[f];
-    et.resize(T);
-    bp_frame_times(T, et.data());
-    multipitch_map(et.data(), T, refs->time_s + k0, refs->frame_off[f + 1] - k0, est.data() + k0);
-    std::fill(owner.begin() + k0, owner.begin() + refs->frame_off[f + 1], f);
-  }
   std::vector<SalienceSettingDev> sal(n_params);
   for (int k = 0; k < n_params; ++k)
     sal[k] = SalienceSettingDev{params[k].threshold, params[k].peak_pick, params[k].bin_lo, params[k].bin_hi, 0};
   Pack pk;
-  const size_t o_owner = pk.add(owner.data(), sizeof(int) * K), o_est = pk.add(est.data(), sizeof(int) * K);
-  size_t o_val[3];
-  pack_mp_values(refs, K, pk, o_val);
+  size_t o_ref[5];
+  pack_ref_frames(refs, foff, n_files, pk, o_ref);
   const size_t o_tm = pk.add(bin_midi, sizeof(double) * width), o_tc = pk.add(bin_chroma, sizeof(double) * width),
                o_set = pk.add(sal.data(), sizeof(SalienceSettingDev) * n_params);
-  DeviceGuard g(m->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   CK(m->score_in.reserve(pk.buf.size()));
   CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
   CK(m->d_frame_off.reserve(n_files + 1));
@@ -2761,9 +2680,9 @@ int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t wi
   CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
   const long long chunk = bp_score_salience_chunk_params(K, V);
   CK(m->score_ws_ref.reserve((size_t)(std::min<long long>(chunk, n_params) * frame_ws_stride(V, K)) + 1));
-  const FrameRefs R = frame_refs_at(m->score_in.p, o_owner, o_est, o_val, K);
+  const FrameRefs R = frame_refs_at(m->score_in.p, o_ref[0], o_ref[1], o_ref + 2, K);
   FrameEst e{};
-  e.gram = d_gram;
+  e.gram = g.contour;
   e.width = width;
   e.frame_off = m->d_frame_off.p;
   e.tab_midi = reinterpret_cast<const double*>(m->score_in.p + o_tm);
@@ -2780,25 +2699,22 @@ int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t wi
   return BP_OK;
 }
 
+int bp_score_salience_grid_device(bp_model_t* m, const float* d_gram, int32_t width, const int64_t* h_frame_off,
+                                  int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                  const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                  const double* bin_chroma, int64_t* h_counts, void* stream) {
+  return score_salience_grid("bp_score_salience_grid_device", m, Grams{nullptr, nullptr, d_gram, false}, width,
+                             h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma, h_counts,
+                             static_cast<cudaStream_t>(stream));
+}
+
 int bp_score_salience_grid_host(bp_model_t* m, const float* h_gram, int32_t width, const int64_t* h_frame_off,
                                 int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
                                 const bp_multipitch_set_t* refs, double window, const double* bin_midi,
                                 const double* bin_chroma, int64_t* h_counts) {
-  const std::string api = "bp_score_salience_grid_host";
-  int rc = check_salience_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma,
-                               h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  const int64_t total = h_frame_off[n_files];
-  if (total > 0 && !h_gram) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  DeviceGuard g(m->device);
-  cudaStream_t st = m->stream;
-  if (total > 0) {  // uploaded once for the whole grid
-    CK(m->st_contour.reserve((size_t)total * width));
-    CK(cudaMemcpyAsync(m->st_contour.p, h_gram, sizeof(float) * total * width, cudaMemcpyHostToDevice, st));
-  }
-  return bp_score_salience_grid_device(m, m->st_contour.p, width, h_frame_off, n_files, params, n_params, refs, window,
-                                       bin_midi, bin_chroma, h_counts, st);
+  return score_salience_grid("bp_score_salience_grid_host", m, Grams{nullptr, nullptr, h_gram, true}, width,
+                             h_frame_off, n_files, params, n_params, refs, window, bin_midi, bin_chroma, h_counts,
+                             m ? m->stream : nullptr);
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,

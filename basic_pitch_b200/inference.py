@@ -364,27 +364,38 @@ class Model:
         return _lib.ScoreParams(**{k: float(v) for k, v in {**evaluate.TOLERANCES, **tolerances}.items()})
 
     @staticmethod
-    def _note_set(sets: Sequence[Tuple[np.ndarray, np.ndarray]], what: str):
-        """[(intervals (n, 2) in seconds, pitches (n,) in Hz)] -> (bp_note_set_t, the arrays it points at); log2 of the
-        pitches as np.log2 takes it (a pitch <= 0 gives a non-finite log2, which the library rejects)."""
+    def _note_set(sets: Sequence, what: str, pitched: bool = True):
+        """[(intervals (n, 2) in seconds, pitches (n,) in Hz)], or without `pitched` [intervals (n, 2)] ->
+        (bp_note_set_t, the arrays it points at); log2 of the pitches as np.log2 takes it (a pitch <= 0 gives a
+        non-finite log2, which the library rejects)."""
         off = np.zeros(len(sets) + 1, np.int64)
         ivs, hzs = [], []
-        for i, (iv, hz) in enumerate(sets):
-            iv, hz = np.asarray(iv, np.float64), np.asarray(hz, np.float64).reshape(-1)
+        for i, s in enumerate(sets):
+            iv, hz = s if pitched else (s, None)
+            iv = np.asarray(iv, np.float64)
             if iv.size == 0:
                 iv = iv.reshape(0, 2)
-            if iv.ndim != 2 or iv.shape[1] != 2 or len(hz) != len(iv):
-                raise ValueError(f"{what}[{i}]: need intervals (n, 2) and pitches (n,), got {iv.shape} and {hz.shape}")
+            if pitched:
+                hz = np.asarray(hz, np.float64).reshape(-1)
+                if iv.ndim != 2 or iv.shape[1] != 2 or len(hz) != len(iv):
+                    raise ValueError(f"{what}[{i}]: need intervals (n, 2) and pitches (n,), got {iv.shape} and {hz.shape}")
+                hzs.append(hz)
+            elif iv.ndim != 2 or iv.shape[1] != 2:
+                raise ValueError(f"{what}[{i}]: need intervals (n, 2), got {iv.shape}")
             off[i + 1] = off[i] + len(iv)
             ivs.append(iv)
-            hzs.append(hz)
         iv = np.concatenate(ivs) if ivs else np.zeros((0, 2))
-        with np.errstate(divide="ignore", invalid="ignore"):
-            l2 = np.log2(np.concatenate(hzs) if hzs else np.zeros(0))
-        arrs = (off, np.ascontiguousarray(iv[:, 0]), np.ascontiguousarray(iv[:, 1]), l2)
-        ns = _lib.NoteSet()
-        ns.note_off, ns.onset_s, ns.offset_s, ns.log2_hz = (_ptr(a) for a in arrs)
+        arrs = (off, np.ascontiguousarray(iv[:, 0]), np.ascontiguousarray(iv[:, 1]))
+        if pitched:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                arrs += (np.log2(np.concatenate(hzs) if hzs else np.zeros(0)),)
+        ns = _lib.NoteSet(*(_ptr(a) for a in arrs))
         return ns, arrs
+
+    @staticmethod
+    def _interval_set(sets: Sequence[np.ndarray], what: str):
+        """[intervals (n, 2) in seconds] -> (bp_note_set_t without pitches, the arrays it points at)."""
+        return Model._note_set(sets, what, pitched=False)
 
     def score_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray], settings: Sequence[Dict[str, Any]],
                    references: Sequence[Tuple[np.ndarray, np.ndarray]], **tolerances) -> np.ndarray:
@@ -464,25 +475,6 @@ class Model:
         h_match = np.full((2, max(int(roff[-1]), 1)), -1, np.int32)
         self._lib.bp_match_notes_host(self._h, C.byref(est), C.byref(refs), len(estimates), C.byref(sp), _ptr(h_match))
         return [h_match[:, roff[i] : roff[i + 1]].copy() for i in range(len(estimates))]
-
-    @staticmethod
-    def _interval_set(sets: Sequence[np.ndarray], what: str):
-        """[intervals (n, 2) in seconds] -> (bp_note_set_t without pitches, the arrays it points at)."""
-        off = np.zeros(len(sets) + 1, np.int64)
-        ivs = []
-        for i, iv in enumerate(sets):
-            iv = np.asarray(iv, np.float64)
-            if iv.size == 0:
-                iv = iv.reshape(0, 2)
-            if iv.ndim != 2 or iv.shape[1] != 2:
-                raise ValueError(f"{what}[{i}]: need intervals (n, 2), got {iv.shape}")
-            off[i + 1] = off[i] + len(iv)
-            ivs.append(iv)
-        iv = np.concatenate(ivs) if ivs else np.zeros((0, 2))
-        arrs = (off, np.ascontiguousarray(iv[:, 0]), np.ascontiguousarray(iv[:, 1]))
-        ns = _lib.NoteSet()
-        ns.note_off, ns.onset_s, ns.offset_s = (_ptr(a) for a in arrs)
-        return ns, arrs
 
     def score_onset_offset_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
                                 settings: Sequence[Dict[str, Any]], references: Sequence[np.ndarray],
@@ -970,6 +962,35 @@ def predict(
     return model_output, midi_data, note_events
 
 
+def _model_and_clips(audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+                     model_or_model_path: Union[Model, pathlib.Path, str]) -> Tuple[Model, List[np.ndarray]]:
+    """The model, and `audio`'s items as mono 22 050 Hz arrays: arrays as given, paths decoded on the host and converted
+    and resampled on the GPU (`load_audio_device`)."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    clips = []
+    for a in audio:
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            clips.append(a)
+        else:
+            clips.append(load_audio_device(a, model)[0])
+    return model, clips
+
+
+def _match_counts(outs, ref_ivs, res, match):
+    """Of `Model.match_grid`'s (res, match) on the model outputs `outs`: the estimated intervals in seconds
+    [setting][file], and counts (n_settings, n_files, 4) = n_ref, n_est, matched without offsets, matched."""
+    times = [infer.model_frames_to_time(o["note"].shape[0] + 1) for o in outs]
+    counts = np.zeros((len(res), len(outs), 4), np.int64)
+    est_ivs = []
+    for k, per in enumerate(res):
+        est_ivs.append([np.stack([times[i][r["start"]], times[i][r["end"]]], 1) for i, r in enumerate(per)])
+        for i, m in enumerate(match[k]):
+            counts[k, i] = (len(ref_ivs[i]), len(per[i]["start"]), (m[0] >= 0).sum(), (m[1] >= 0).sum())
+    return est_ivs, counts
+
+
 def predict_grid(
     audio: Union[np.ndarray, pathlib.Path, str],
     settings: Sequence[Dict[str, Any]],
@@ -984,12 +1005,7 @@ def predict_grid(
     Returns (model_output, [(midi_data, note_events) per setting]); each pair equals what `predict` gives for that
     setting, with the events as `NoteEventList`s and the MIDI objects as `LazyPrettyMIDI`s (`predict_batch(lazy=True)`).
     The model output is not column-zeroed: the settings may disagree on the frequency range."""
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    if isinstance(audio, np.ndarray):
-        if audio.ndim != 1:
-            raise ValueError("audio must be mono (1-D)")
-    else:
-        audio, _ = load_audio_device(audio, model)
+    model, (audio,) = _model_and_clips([audio], model_or_model_path)
     conv = [infer.grid_setting(s, predict_names=True) for s in settings]
     model_output = model.run_inference_arrays([audio])[0]
     arrs = model.decode_grid([model_output["note"]], [model_output["onset"]], [model_output["contour"]],
@@ -1013,15 +1029,7 @@ def evaluate_grid(
     `predict_grid`); tolerances as `evaluate.TOLERANCES`.
 
     Returns (counts (n_settings, n_files, 4), `evaluate.note_scores(counts)`)."""
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    clips = []
-    for a in audio:
-        if isinstance(a, np.ndarray):
-            if a.ndim != 1:
-                raise ValueError("audio must be mono (1-D)")
-            clips.append(a)
-        else:
-            clips.append(load_audio_device(a, model)[0])
+    model, clips = _model_and_clips(audio, model_or_model_path)
     decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
     outs = model.run_inference_arrays(clips)
     counts = model.score_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references, **tolerances)
@@ -1055,32 +1063,20 @@ def evaluate_velocity_grid(
         if len(vel) != len(np.asarray(hz).reshape(-1)):
             raise ValueError(f"references[{i}]: {len(vel)} velocities for {len(np.asarray(hz).reshape(-1))} notes")
         refs.append((iv, hz, vel))
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    clips = []
-    for a in audio:
-        if isinstance(a, np.ndarray):
-            if a.ndim != 1:
-                raise ValueError("audio must be mono (1-D)")
-            clips.append(a)
-        else:
-            clips.append(load_audio_device(a, model)[0])
+    model, clips = _model_and_clips(audio, model_or_model_path)
     decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
     outs = model.run_inference_arrays(clips)
     res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode,
                                   [(iv, hz) for iv, hz, _ in refs], **tolerances)
     n_params, n_files = len(settings), len(clips)
-    counts = np.zeros((n_params, n_files, 4), np.int64)
+    ref_ivs = [np.asarray(iv, np.float64).reshape(-1, 2) for iv, _, _ in refs]
+    est_ivs, counts = _match_counts(outs, ref_ivs, res, match)
     keys = [k + s for s in ("", "_no_offset") for k in evaluate.MATCH_FIELDS]
     extra = {k: np.zeros((n_params, n_files)) for k in keys}
-    for i, o in enumerate(outs):
-        t = infer.model_frames_to_time(o["note"].shape[0] + 1)
-        ref_iv = np.asarray(refs[i][0], np.float64).reshape(-1, 2)
-        for k in range(n_params):
-            r = res[k][i]
-            est_iv = np.stack([t[r["start"]], t[r["end"]]], 1)
-            counts[k, i] = (len(ref_iv), len(r["start"]), (match[k][i][0] >= 0).sum(), (match[k][i][1] >= 0).sum())
-            vals = evaluate.matching_scores(ref_iv, refs[i][2], est_iv, evaluate.note_velocities(r["amp"]), match[k][i],
-                                            velocity_tolerance)
+    for k in range(n_params):
+        for i in range(n_files):
+            vals = evaluate.matching_scores(ref_ivs[i], refs[i][2], est_ivs[k][i], evaluate.note_velocities(res[k][i]["amp"]),
+                                            match[k][i], velocity_tolerance)
             for key in keys:
                 extra[key][k, i] = vals[key]
     scores = evaluate.note_scores(counts)
@@ -1106,38 +1102,26 @@ def evaluate_transcription_grid(
     Returns (counts, scores): counts int64 (n_settings, n_files, 6) = n_ref, n_est, matched without offsets, matched,
     onsets matched, offsets matched; scores the 14 values under the names `evaluate.TRANSCRIPTION_KEYS` maps mir_eval's
     keys to, in its order, as (n_settings, n_files) float64 arrays, with "mean" over files as in `note_scores`."""
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    clips = []
-    for a in audio:
-        if isinstance(a, np.ndarray):
-            if a.ndim != 1:
-                raise ValueError("audio must be mono (1-D)")
-            clips.append(a)
-        else:
-            clips.append(load_audio_device(a, model)[0])
+    model, clips = _model_and_clips(audio, model_or_model_path)
     decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
     outs = model.run_inference_arrays(clips)
     res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
                                   **tolerances)
     n_params, n_files = len(settings), len(clips)
     ref_ivs = [np.asarray(iv, np.float64).reshape(-1, 2) for iv, _ in references]
-    times = [infer.model_frames_to_time(o["note"].shape[0] + 1) for o in outs]
-    counts = np.zeros((n_params, n_files, 6), np.int64)
+    est_ivs, counts = _match_counts(outs, ref_ivs, res, match)
     overlap = {k: np.zeros((n_params, n_files)) for k in ("average_overlap_ratio", "average_overlap_ratio_no_offset")}
-    ests = []
     for k in range(n_params):
         for i in range(n_files):
-            r, m = res[k][i], match[k][i]
-            est_iv = np.stack([times[i][r["start"]], times[i][r["end"]]], 1)
-            ests.append(est_iv)
-            counts[k, i, :4] = (len(ref_ivs[i]), len(est_iv), (m[0] >= 0).sum(), (m[1] >= 0).sum())
+            m = match[k][i]
             for suffix, row in (("", m[1]), ("_no_offset", m[0])):
                 ref_idx = np.flatnonzero(row >= 0)  # sorted(matching.items()): ascending reference index
-                overlap["average_overlap_ratio" + suffix][k, i] = evaluate._overlap_ratio(ref_ivs[i], est_iv, ref_idx,
-                                                                                           row[ref_idx])
+                overlap["average_overlap_ratio" + suffix][k, i] = evaluate._overlap_ratio(ref_ivs[i], est_ivs[k][i],
+                                                                                           ref_idx, row[ref_idx])
+    ests = [iv for per in est_ivs for iv in per]
     onoff = model.score_onsets_offsets(ests, ref_ivs * n_params, **tolerances).reshape(n_params, n_files, 4)
-    counts[..., 4:] = onoff[..., 2:]
-    scores = evaluate.note_scores(counts[..., :4])
+    scores = evaluate.note_scores(counts)
+    counts = np.concatenate([counts, onoff[..., 2:]], axis=-1)
     scores.update(overlap)
     scores["mean"].update({k: (v.mean(axis=-1) if n_files else np.zeros(n_params)) for k, v in overlap.items()})
     oo = evaluate.onset_offset_scores(onoff)
@@ -1161,15 +1145,7 @@ def evaluate_frames_grid(
     convention (`evaluate.notes_to_multipitch` makes one from note annotations); window in semitones.
 
     Returns (counts (n_settings, n_files, 7), `evaluate.frame_scores(counts)`)."""
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    clips = []
-    for a in audio:
-        if isinstance(a, np.ndarray):
-            if a.ndim != 1:
-                raise ValueError("audio must be mono (1-D)")
-            clips.append(a)
-        else:
-            clips.append(load_audio_device(a, model)[0])
+    model, clips = _model_and_clips(audio, model_or_model_path)
     decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
     outs = model.run_inference_arrays(clips)
     counts = model.score_frames_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
@@ -1195,15 +1171,7 @@ def evaluate_salience_grid(
     Returns (counts (n_settings, n_files, 7), `evaluate.frame_scores(counts)`)."""
     if kind not in ("contour", "note"):
         raise ValueError(f"kind must be 'contour' or 'note', got {kind!r}")
-    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
-    clips = []
-    for a in audio:
-        if isinstance(a, np.ndarray):
-            if a.ndim != 1:
-                raise ValueError("audio must be mono (1-D)")
-            clips.append(a)
-        else:
-            clips.append(load_audio_device(a, model)[0])
+    model, clips = _model_and_clips(audio, model_or_model_path)
     outs = model.run_inference_arrays(clips)
     counts = model.score_salience_grid([o[kind] for o in outs], settings, references, kind=kind, window=window)
     return counts, evaluate.frame_scores(counts)
