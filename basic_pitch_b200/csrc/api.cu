@@ -211,6 +211,7 @@ struct bp_model {
   // melody scoring (bp_score_melody_*): arg-max of every (range, frame) and held cents of every (setting, frame) of a chunk
   DevBuf<MelodyArg> melody_arg;
   DevBuf<double> melody_held;
+  DevBuf<double> melody_raw;  // bp_score_note_melody_grid_*: raw cents of every (setting, frame) of a chunk
   int64_t last_forward_n = 0;
   int last_path = 0;
   // optional per-kernel timing (bench.py roofline): CUDA events around one kernel family
@@ -1214,7 +1215,7 @@ void bp_model_destroy(bp_model_t* m) {
   m->d_bend_off.release(); m->d_bends.release(); m->d_onset64.release();
   m->match_edges.release(); m->match_off.release(); m->match_est_off.release(); m->match_ws.release();
   m->match_out.release();
-  m->melody_arg.release(); m->melody_held.release();
+  m->melody_arg.release(); m->melody_held.release(); m->melody_raw.release();
   m->yhl.release();
   m->chl.release();
   m->cqt_wtc.release();
@@ -2443,14 +2444,30 @@ int check_value_table(const std::string& api, const char* what, const double* mi
   return BP_OK;
 }
 
-// Everything bp_score_frames_grid_* check before anything is enqueued, in addition to check_grid_args.
+// Everything bp_score_frames_grid_* check before anything is enqueued, in addition to check_grid_args; `bent`
+// (bp_score_bent_frames_grid_*): the tables are the 264-entry bin tables.
 int check_frames_grid(const std::string& api, int n_files, int n_params, const bp_multipitch_set_t* refs, double window,
-                      const double* est_midi, const double* est_chroma, const int64_t* h_counts) {
+                      const double* est_midi, const double* est_chroma, const int64_t* h_counts, bool bent) {
   int rc = check_window(api, window);
   if (rc || n_files == 0 || n_params == 0) return rc;
   if (!h_counts || !est_midi || !est_chroma) return fail(BP_E_INVALID, api + ": bad argument");
-  rc = check_value_table(api, "estimate table", est_midi, est_chroma, 128);
+  rc = bent ? check_value_table(api, "bin table", est_midi, est_chroma, kContourBins)
+            : check_value_table(api, "estimate table", est_midi, est_chroma, 128);
   return rc ? rc : check_mp_set(api, "references", "file", refs, n_files);
+}
+
+// The null-posteriorgram rule of the bent grid scorers (bp_score_bent_frames_grid_*, bp_score_note_melody_grid_*), as
+// bp_decode_grid_*: the contour may be NULL only when no setting has include_pitch_bends; the message names the first
+// setting that has.
+int check_bent_grams(const std::string& api, const Grams& g, long long total_frames, const bp_decode_params_t* params,
+                     int n_params) {
+  if (total_frames == 0) return BP_OK;
+  if (!g.note || !g.onset) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  for (int k = 0; !g.contour && k < n_params; ++k)
+    if (params[k].include_pitch_bends)
+      return fail(BP_E_INVALID, api + ": null contour posteriorgram, but decode params[" + std::to_string(k) +
+                                    "] has include_pitch_bends");
+  return BP_OK;
 }
 
 FrameRefs frame_refs_at(const unsigned char* d, size_t o_owner, size_t o_est, const size_t* o_val, long long K) {
@@ -2528,27 +2545,38 @@ int bp_multipitch_map(const double* est_t, int64_t n_est, const double* ref_t, i
   return BP_OK;
 }
 
+// bp_score_frames_grid_* (128-entry estimate tables, no contour) and, with `bent`, bp_score_bent_frames_grid_* (264-entry
+// bin tables, g.contour, each setting's include_pitch_bends).
 static int score_frames_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
                              const bp_decode_params_t* params, int32_t n_params, const bp_multipitch_set_t* refs,
                              double window, const double* est_midi, const double* est_chroma, int64_t* h_counts,
-                             cudaStream_t st) {
+                             bool bent, cudaStream_t st) {
   bool any_bends = false;
   int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
-  if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts);
+  if (!rc) rc = check_frames_grid(api, n_files, n_params, refs, window, est_midi, est_chroma, h_counts, bent);
   if (rc) return rc;
   if (n_files == 0 || n_params == 0) return BP_OK;
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long total_frames = foff[n_files], cells = total_frames * kPitches;
-  if (total_frames > 0 && (!g.note || !g.onset)) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  if (bent) {
+    rc = check_bent_grams(api, g, total_frames, params, n_params);
+    if (rc) return rc;
+  } else if (total_frames > 0 && (!g.note || !g.onset)) {
+    return fail(BP_E_INVALID, api + ": null posteriorgram");
+  }
   DeviceGuard dg(m->device);
-  rc = stage_grams(m, total_frames, g, false);
+  rc = stage_grams(m, total_frames, g, bent && any_bends);
   if (rc) return rc;
-  // one upload per call: the reference frames and the tables
+  // one upload per call: the reference frames, the tables and (bent) every setting's bend flag
   const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
+  const int n_tab = bent ? kContourBins : 128;
   Pack pk;
   size_t o_ref[5];
   pack_ref_frames(refs, foff, n_files, pk, o_ref);
-  const size_t o_tm = pk.add(est_midi, sizeof(double) * 128), o_tc = pk.add(est_chroma, sizeof(double) * 128);
+  const size_t o_tm = pk.add(est_midi, sizeof(double) * n_tab), o_tc = pk.add(est_chroma, sizeof(double) * n_tab);
+  std::vector<int> bend_on(n_params);
+  for (int k = 0; k < n_params; ++k) bend_on[k] = params[k].include_pitch_bends != 0;
+  const size_t o_bend = pk.add(bend_on.data(), sizeof(int) * n_params);
   CK(m->score_in.reserve(pk.buf.size()));
   CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
   const long long n_counts = (long long)n_params * n_files * kFrameCounts;
@@ -2570,6 +2598,11 @@ static int score_frames_grid(const std::string& api, bp_model_t* m, Grams g, con
     e.frame_off = m->d_frame_off.p;
     e.tab_midi = reinterpret_cast<const double*>(m->score_in.p + o_tm);
     e.tab_chroma = reinterpret_cast<const double*>(m->score_in.p + o_tc);
+    if (bent) {
+      e.bend_on = reinterpret_cast<const int*>(m->score_in.p + o_bend) + p0;
+      e.contour = g.contour;
+      e.gauss = m->d_gauss;
+    }
     launch_frame_match(R, e, window, m->score_ws_ref.p, n_files, P, m->score_counts.p + kFrameCounts * p0 * n_files, st);
     CKL();
     m->launches += 3;
@@ -2586,7 +2619,7 @@ int bp_score_frames_grid_device(bp_model_t* m, const float* d_note, const float*
                                 const bp_multipitch_set_t* refs, double window, const double* est_midi,
                                 const double* est_chroma, int64_t* h_counts, void* stream) {
   return score_frames_grid("bp_score_frames_grid_device", m, Grams{d_note, d_onset, nullptr, false}, h_frame_off,
-                           n_files, params, n_params, refs, window, est_midi, est_chroma, h_counts,
+                           n_files, params, n_params, refs, window, est_midi, est_chroma, h_counts, false,
                            static_cast<cudaStream_t>(stream));
 }
 
@@ -2595,7 +2628,26 @@ int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h
                               const bp_multipitch_set_t* refs, double window, const double* est_midi,
                               const double* est_chroma, int64_t* h_counts) {
   return score_frames_grid("bp_score_frames_grid_host", m, Grams{h_note, h_onset, nullptr, true}, h_frame_off, n_files,
-                           params, n_params, refs, window, est_midi, est_chroma, h_counts, m ? m->stream : nullptr);
+                           params, n_params, refs, window, est_midi, est_chroma, h_counts, false,
+                           m ? m->stream : nullptr);
+}
+
+int bp_score_bent_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                                     const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                     int32_t n_params, const bp_multipitch_set_t* refs, double window,
+                                     const double* bin_midi, const double* bin_chroma, int64_t* h_counts, void* stream) {
+  return score_frames_grid("bp_score_bent_frames_grid_device", m, Grams{d_note, d_onset, d_contour, false}, h_frame_off,
+                           n_files, params, n_params, refs, window, bin_midi, bin_chroma, h_counts, true,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int bp_score_bent_frames_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                                   const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                   int32_t n_params, const bp_multipitch_set_t* refs, double window,
+                                   const double* bin_midi, const double* bin_chroma, int64_t* h_counts) {
+  return score_frames_grid("bp_score_bent_frames_grid_host", m, Grams{h_note, h_onset, h_contour, true}, h_frame_off,
+                           n_files, params, n_params, refs, window, bin_midi, bin_chroma, h_counts, true,
+                           m ? m->stream : nullptr);
 }
 
 int bp_score_multipitch_host(bp_model_t* m, const bp_multipitch_set_t* est, const bp_multipitch_set_t* refs,
@@ -2846,6 +2898,31 @@ int check_tolerance(const std::string& api, double tol) {
   return BP_OK;
 }
 
+// A bin cents table of n entries: finite and non-decreasing, and with `positive` > 0 (the note melody tells voiced frames
+// by nonzero cents).
+int check_cent_table(const std::string& api, const double* bin_cent, int n, bool positive) {
+  for (int b = 0; b < n; ++b) {
+    const std::string at = api + ": bin table entry " + std::to_string(b);
+    if (!std::isfinite(bin_cent[b])) return fail(BP_E_INVALID, at + ": non-finite cents");
+    if (b > 0 && bin_cent[b] < bin_cent[b - 1]) return fail(BP_E_INVALID, at + ": cents decrease");
+    if (positive && !(bin_cent[b] > 0)) return fail(BP_E_INVALID, at + ": cents must be > 0");
+  }
+  return BP_OK;
+}
+
+// The reference map of a melody grid call: each file's reference frames against its estimate at the model frame times.
+std::vector<MelodyRef> melody_grid_refs(const bp_melody_set_t* refs, const std::vector<long long>& foff, int n_files) {
+  std::vector<MelodyRef> R;
+  R.reserve(refs->frame_off[n_files] + n_files);
+  std::vector<double> et;
+  for (int f = 0; f < n_files; ++f) {
+    et.resize(foff[f + 1] - foff[f]);
+    bp_frame_times((int64_t)et.size(), et.data());
+    melody_refs(refs, f, et.data(), (long long)et.size(), foff[f], R);
+  }
+  return R;
+}
+
 // Everything bp_score_melody_grid_* check before anything is enqueued (include/bp_b200.h).
 int check_melody_grid(const std::string& api, const bp_model* m, int width, const int64_t* h_frame_off, int n_files,
                       const bp_melody_params_t* params, int n_params, const bp_melody_set_t* refs, double tol,
@@ -2864,11 +2941,8 @@ int check_melody_grid(const std::string& api, const bp_model* m, int width, cons
   int rc = check_tolerance(api, tol);
   if (rc || n_files == 0 || n_params == 0) return rc;
   if (!h_frame_off || !h_counts || !bin_cent) return fail(BP_E_INVALID, api + ": bad argument");
-  for (int b = 0; b < width; ++b) {
-    const std::string at = api + ": bin table entry " + std::to_string(b);
-    if (!std::isfinite(bin_cent[b])) return fail(BP_E_INVALID, at + ": non-finite cents");
-    if (b > 0 && bin_cent[b] < bin_cent[b - 1]) return fail(BP_E_INVALID, at + ": cents decrease");
-  }
+  rc = check_cent_table(api, bin_cent, width, false);
+  if (rc) return rc;
   if (h_frame_off[0] != 0) return fail(BP_E_INVALID, api + ": frame_off[0] must be 0");
   for (int i = 0; i < n_files; ++i)
     if (h_frame_off[i + 1] < h_frame_off[i] || h_frame_off[i + 1] - h_frame_off[i] > INT_MAX)
@@ -2920,15 +2994,7 @@ static int score_melody_grid(const std::string& api, bp_model_t* m, Grams g, int
   const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
   const long long F = foff[n_files];
   if (F > 0 && !g.contour) return fail(BP_E_INVALID, api + ": null posteriorgram");
-  // the reference map: estimates at the model frame times of each file
-  std::vector<MelodyRef> R;
-  R.reserve(refs->frame_off[n_files] + n_files);
-  std::vector<double> et;
-  for (int f = 0; f < n_files; ++f) {
-    et.resize(foff[f + 1] - foff[f]);
-    bp_frame_times((int64_t)et.size(), et.data());
-    melody_refs(refs, f, et.data(), (long long)et.size(), foff[f], R);
-  }
+  const std::vector<MelodyRef> R = melody_grid_refs(refs, foff, n_files);
   const long long K = (long long)R.size();
   // settings in chunks; each chunk's distinct bin ranges, its settings pointing at them
   const long long chunk = bp_score_melody_chunk_params(F);
@@ -3003,6 +3069,88 @@ int bp_score_melody_grid_host(bp_model_t* m, const float* h_gram, int32_t width,
   return score_melody_grid("bp_score_melody_grid_host", m, Grams{nullptr, nullptr, h_gram, true}, width, h_frame_off,
                            n_files, params, n_params, refs, cent_tolerance, bin_cent, h_counts,
                            m ? m->stream : nullptr);
+}
+
+static int score_note_melody_grid(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off,
+                                  int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
+                                  const bp_melody_set_t* refs, double tol, const double* bin_cent, int64_t* h_counts,
+                                  cudaStream_t st) {
+  bool any_bends = false;
+  int rc = check_grid_args(api, m, h_frame_off, n_files, params, n_params, &any_bends);
+  if (!rc) rc = check_tolerance(api, tol);
+  if (rc || n_files == 0 || n_params == 0) return rc;
+  if (!h_counts || !bin_cent) return fail(BP_E_INVALID, api + ": bad argument");
+  rc = check_cent_table(api, bin_cent, kContourBins, true);
+  if (rc) return rc;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long F = foff[n_files], cells = F * kPitches;
+  if (F > INT_MAX) return fail(BP_E_INVALID, api + ": more than 2^31 - 1 frames");
+  rc = check_melody_set(api, "references", "file", refs, n_files, false);
+  if (!rc) rc = check_bent_grams(api, g, F, params, n_params);
+  if (rc) return rc;
+  const std::vector<MelodyRef> R = melody_grid_refs(refs, foff, n_files);
+  const long long K = (long long)R.size();
+  DeviceGuard dg(m->device);
+  rc = stage_grams(m, F, g, any_bends);
+  if (rc) return rc;
+  // one upload per call: the reference frames, the bin table and every setting's bend flag
+  std::vector<int> bend_on(n_params);
+  for (int k = 0; k < n_params; ++k) bend_on[k] = params[k].include_pitch_bends != 0;
+  Pack pk;
+  const size_t o_ref = pk.add(R.data(), sizeof(MelodyRef) * K), o_tab = pk.add(bin_cent, sizeof(double) * kContourBins),
+               o_bend = pk.add(bend_on.data(), sizeof(int) * n_params);
+  CK(m->score_in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const long long n_counts = (long long)n_params * n_files * kMelodyCounts;
+  CK(m->score_counts.reserve((size_t)n_counts));
+  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
+  const long long P_max = std::min<long long>(bp_decode_grid_chunk_params(F, n_files), n_params);
+  CK(m->melody_held.reserve((size_t)(P_max * F) + 1));
+  CK(m->melody_raw.reserve((size_t)(P_max * F) + 1));
+  const unsigned char* d = m->score_in.p;
+  MelodyEst e{};
+  e.bin_cent = reinterpret_cast<const double*>(d + o_tab);
+  e.held = m->melody_held.p;
+  e.raw = m->melody_raw.p;
+  e.n_frames = F;
+  rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
+                          const std::vector<int>&, const std::vector<long long>&) -> int {
+    // each setting's E is dead once the loops have run: it becomes that setting's count roll
+    int* roll = reinterpret_cast<int*>(m->energy.p);
+    if (cells > 0) CK(cudaMemsetAsync(roll, 0, sizeof(int) * P * cells, st));
+    launch_frame_roll(m->d_frame_off.p, m->d_slot_off.p, m->note_count.p, m->slot_start.p, m->slot_end.p,
+                      m->slot_pitch.p, n_files, P, roll, cells, st);
+    CKL();
+    const NoteMelodyEst N{roll, cells, m->d_frame_off.p, g.note, g.contour, m->d_gauss,
+                          reinterpret_cast<const int*>(d + o_bend) + p0};
+    launch_note_melody(N, n_files, reinterpret_cast<const MelodyRef*>(d + o_ref), K, e, tol, P,
+                       m->score_counts.p + kMelodyCounts * p0 * n_files, st);
+    CKL();
+    m->launches += 4;
+    return BP_OK;
+  });
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * n_counts, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+int bp_score_note_melody_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                                     const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                     int32_t n_params, const bp_melody_set_t* refs, double cent_tolerance,
+                                     const double* bin_cent, int64_t* h_counts, void* stream) {
+  return score_note_melody_grid("bp_score_note_melody_grid_device", m, Grams{d_note, d_onset, d_contour, false},
+                                h_frame_off, n_files, params, n_params, refs, cent_tolerance, bin_cent, h_counts,
+                                static_cast<cudaStream_t>(stream));
+}
+
+int bp_score_note_melody_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                                   const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                   int32_t n_params, const bp_melody_set_t* refs, double cent_tolerance,
+                                   const double* bin_cent, int64_t* h_counts) {
+  return score_note_melody_grid("bp_score_note_melody_grid_host", m, Grams{h_note, h_onset, h_contour, true},
+                                h_frame_off, n_files, params, n_params, refs, cent_tolerance, bin_cent, h_counts,
+                                m ? m->stream : nullptr);
 }
 
 int bp_score_melody_host(bp_model_t* m, const bp_melody_set_t* est, const bp_melody_set_t* refs, int32_t n_items,

@@ -643,30 +643,10 @@ __global__ void note_finish_kernel(const float* __restrict__ note, const float* 
     amp[n] = __fdiv_rn(s, (float)len);
   }
   if (!with_bends || bend_off[n + 1] == bend_off[n]) return;  // empty: a grid setting without pitch bends
-  // reference: note_creation.py:198-218 ; contour bin of the note = 3*(pitch-21)
-  const int c = 3 * col;
-  const int lo = max(c - 25, 0);
-  const int hi = min(kContourBins, c + 26);
-  const int g0 = max(0, 25 - c);       // first Gaussian tap used
-  const int shift = 25 - g0;
-  const int width = hi - lo;           // <= 51
   int* out = bends + bend_off[n];
   // one frame per lane (a note has 11 .. a few dozen frames): every lane walks its frame's <= 51 bins in ascending order
   // and keeps the first maximum — np.argmax semantics without any cross-lane reduction
-  for (int t = t0 + lane; t < t1; t += 32) {
-    const float* row = contour + (base + t) * kContourBins + lo;
-    double bv = -INFINITY;  // np.argmax semantics for any input (callers may pass contours < 0)
-    int bi = 0;
-#pragma unroll 4
-    for (int j = 0; j < width; ++j) {
-      const double v = __dmul_rn((double)__ldg(row + j), gauss[g0 + j]);
-      if (v > bv) {
-        bv = v;
-        bi = j;
-      }
-    }
-    out[t - t0] = bi - shift;
-  }
+  for (int t = t0 + lane; t < t1; t += 32) out[t - t0] = pitch_bend_at(contour + (base + t) * kContourBins, col, gauss);
 }
 
 void launch_note_finish(const float* note, const float* contour, const long long* note_base, const int* start,

@@ -345,6 +345,30 @@ void launch_note_finish(const float* note, const float* contour, const long long
                         const int* start, const int* end, const int* pitch, float* amp, const int* bend_off,
                         int* bends, int n_notes, int with_bends, const double* gauss /*[51] device*/,
                         cudaStream_t st);
+// The pitch bend of note column col (MIDI col + 21) at one frame, `row` that frame's 264 contour bins (reference:
+// note_creation.py:198-218, n_bins_tolerance 25): the first arg-max of float64(row[b]) * gauss[b - c + 25] over the
+// bins b of [c - 25, c + 25] inside [0, 264), c = 3 col, as an offset from c.  It depends on (frame, pitch) only, so every
+// note of that pitch sounding at that frame gets the same bend, and c + bend always lies in [0, 263].  The decode
+// (note_finish_kernel) and the bent scorers (score_frames.cu, score_melody.cu) all call this one function.
+__device__ __forceinline__ int pitch_bend_at(const float* __restrict__ row, int col, const double* __restrict__ gauss) {
+  const int c = 3 * col;
+  const int lo = max(c - 25, 0);
+  const int hi = min(kContourBins, c + 26);
+  const int g0 = max(0, 25 - c);  // first Gaussian tap used
+  const int width = hi - lo;      // <= 51
+  row += lo;
+  double bv = -INFINITY;  // np.argmax semantics for any input (callers may pass contours < 0)
+  int bi = 0;
+#pragma unroll 4
+  for (int j = 0; j < width; ++j) {
+    const double v = __dmul_rn((double)__ldg(row + j), gauss[g0 + j]);
+    if (v > bv) {
+      bv = v;
+      bi = j;
+    }
+  }
+  return bi - (25 - g0);
+}
 
 // ---- score.cu: note-level match counts (bp_score_*) ----------------------------------------------------------------
 // Nearest semitone (MIDI number) of a pitch given as log2(Hz), clamped to +-1e9 so that bucket differences fit an int.
@@ -416,7 +440,7 @@ void launch_match(const ScoreRefs& R, const ScoreEst& E, const ScoreTol& tol, co
 // ---- score_frames.cu: frame-level multi-pitch counts (bp_score_frames_grid_*, bp_score_multipitch_host,
 // bp_score_salience_grid_*) -------------------------------------------------------------------------------------------
 constexpr int kFrameCounts = 7;  // n_ref, n_est, tp, tp_chroma, sum min, miss, false alarms
-enum class EstKind { kExplicit, kRoll, kGram };  // where the match kernel's estimate frames come from
+enum class EstKind { kExplicit, kRoll, kGram, kBent };  // where the match kernel's estimate frames come from
 struct SalienceSettingDev {  // bp_salience_params_t, validated
   double threshold;
   int peak_pick, bin_lo, bin_hi, reserved;
@@ -443,6 +467,12 @@ struct FrameEst {
   const float* gram;
   const SalienceSettingDev* salience;
   long long width;
+  // bent (bend_on set): the count roll as above, each sounding pitch p at contour bin k = 3 (p - 21) + its pitch bend
+  // under chunk-local setting s when bend_on[s] (pitch_bend_at on the contour row [frame_off[n_owner]][264] with the 51
+  // Gaussian taps `gauss`), else 3 (p - 21); tab_midi / tab_chroma are then the 264 bin tables (midi non-decreasing)
+  const int* bend_on;
+  const float* contour;
+  const double* gauss;
 };
 // int workspace of the chroma matching: frame k of chunk-local setting s at ws + s * (4 V + 2 K) + 4 voff[k] + 2 k
 // (V values, K frames): per reference value its mate and visit stamp, and a stack of 2 (n + 1) for its frame's n.
@@ -452,8 +482,8 @@ __host__ __device__ inline long long frame_ws_stride(long long n_values, long lo
 void launch_frame_roll(const long long* frame_off, const long long* slot_off, const int* note_count, const int* start,
                        const int* end, const int* pitch, int n_files, int n_settings, int* roll, long long roll_stride,
                        cudaStream_t st);
-// One launch: counts[7 (s * n_owner + owner) ..] += the seven sums of every frame of setting s (E.roll set: roll
-// estimates; else E.salience set: posteriorgram estimates; else explicit estimates, n_settings 1).  counts must be zeroed by
+// One launch: counts[7 (s * n_owner + owner) ..] += the seven sums of every frame of setting s (E.roll and E.bend_on
+// set: bent roll estimates; E.roll alone: roll estimates; else E.salience set: posteriorgram estimates; else explicit estimates, n_settings 1).  counts must be zeroed by
 // the caller.
 void launch_frame_match(const FrameRefs& R, const FrameEst& E, double window, int* ws, int n_owner, int n_settings,
                         long long* counts, cudaStream_t st);
@@ -489,11 +519,27 @@ struct MelodyEst {
   const int* voiced;
   double* held;  // held cents of chunk-local setting s (explicit: 0) at held[s * n_frames + e]
   long long n_frames;
+  double* raw;   // decoded notes: raw cents of chunk-local setting s at raw[s * n_frames + e], voiced where nonzero
+};
+// Decoded notes of a grid chunk read as a melody (bp_score_note_melody_grid_*): the count roll of launch_frame_roll,
+// the note posteriorgram [frame][88] and contour [frame][264] of the call (row-major, global frames), the 51 Gaussian
+// taps of the bends and each chunk-local setting's bend flag.  MelodyEst.bin_cent holds the 264 bin cents (all > 0).
+struct NoteMelodyEst {
+  const int* roll;
+  long long roll_stride;
+  const long long* frame_off;
+  const float *note, *contour;
+  const double* gauss;
+  const int* bend_on;
 };
 // Grid chunk: arg-max, hold scan and counts, three launches whatever the number of settings and files.
 // counts[7 (s * n_files + file) ..] += the seven sums; zeroed by the caller.
 void launch_melody_grid(const float* gram, long long width, const MelodyRange* ranges, int n_ranges,
                         const long long* frame_off, int n_files, const MelodyRef* refs, long long K, const MelodyEst& E,
+                        double tol, int n_settings, long long* counts, cudaStream_t st);
+// Decoded notes of a grid chunk after launch_frame_roll: the per-(setting, file) pick, bend and hold, then the counts,
+// two launches.  counts as launch_melody_grid.
+void launch_note_melody(const NoteMelodyEst& N, int n_files, const MelodyRef* refs, long long K, const MelodyEst& E,
                         double tol, int n_settings, long long* counts, cudaStream_t st);
 // Explicit tracks (E.held filled by the caller): one launch.
 void launch_melody_explicit(const MelodyRef* refs, long long K, const MelodyEst& E, double tol, int n_items,

@@ -10,6 +10,11 @@
 // values sorted by midi, or a posteriorgram row read under a salience setting (bp_score_salience_grid_*: the bins that
 // pass its threshold, peak and range tests, in ascending bin order, each once).  Every sum is an integer, reduced with
 // integer atomics: the result is deterministic.
+// Bent grid estimates (bp_score_bent_frames_grid_*) read the same roll: each sounding pitch of the column becomes one
+// group at its contour bin, 3 (p - 21) plus the pitch's bend at that frame (pitch_bend_at, the decode's own arg-max: the
+// bend depends on (frame, pitch) only, so a pitch's count of notes all share it).  Bends move a pitch by up to 25 bins, so
+// keys of pitches up to 16 semitones apart can cross: the thread insertion-sorts its <= 88 (key, count) groups in a local
+// array of 88 int64 (704 bytes of stack in that instantiation only; no spills) before the unchanged passes.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -85,6 +90,7 @@ __global__ void __launch_bounds__(kRollThreads) roll_scan_kernel(const long long
 template <EstKind kKind>
 struct EstFrame {
   const int* col;  // roll: roll column at frame t, pitch g at col[g * T]
+  const long long* kv;  // bent: group g is key kv[g] >> 32 (a contour bin) with count kv[g] & 0xffffffff, keys ascending
   long long T;
   const double *midi, *chroma;  // roll: tables indexed by MIDI number; explicit: this frame's values; gram: bin tables
   int n;
@@ -104,16 +110,19 @@ struct EstFrame {
   }
   __device__ __forceinline__ int count(int g) const {
     if constexpr (kKind == EstKind::kRoll) return col[g * T];
+    else if constexpr (kKind == EstKind::kBent) return (int)(kv[g] & 0xffffffffLL);
     else if constexpr (kKind == EstKind::kGram) return gram_count(g);
     else return 1;
   }
   __device__ __forceinline__ double m(int g) const {
     if constexpr (kKind == EstKind::kRoll) return midi[g + 21];
+    else if constexpr (kKind == EstKind::kBent) return midi[kv[g] >> 32];
     else if constexpr (kKind == EstKind::kGram) return midi[lo + g];
     else return midi[g];
   }
   __device__ __forceinline__ double c(int g) const {
     if constexpr (kKind == EstKind::kRoll) return chroma[g + 21];
+    else if constexpr (kKind == EstKind::kBent) return chroma[kv[g] >> 32];
     else if constexpr (kKind == EstKind::kGram) return chroma[lo + g];
     else return chroma[g];
   }
@@ -220,6 +229,7 @@ __global__ void __launch_bounds__(kMatchThreads) frame_match_kernel(FrameRefs R,
     const int n_ref = (int)(R.voff[k + 1] - r0);
     pair = s * n_owner + owner;
     EstFrame<kKind> ef{};
+    long long kv[kKind == EstKind::kBent ? kPitches : 1];
     int n_est = 0;
     if (t >= 0) {
       if constexpr (kKind == EstKind::kRoll) {
@@ -231,6 +241,26 @@ __global__ void __launch_bounds__(kMatchThreads) frame_match_kernel(FrameRefs R,
         ef.n = kPitches;
 #pragma unroll 1  // unrolled, ptxas spills
         for (int g = 0; g < kPitches; ++g) n_est += ef.count(g);
+      } else if constexpr (kKind == EstKind::kBent) {
+        const long long base = E.frame_off[owner], T = E.frame_off[owner + 1] - base;
+        const int* col = E.roll + s * E.roll_stride + base * kPitches + t;
+        const float* crow = E.contour + (base + t) * kContourBins;  // read only with bends
+        const bool bend = E.bend_on[s] != 0;
+        int n = 0;
+#pragma unroll 1
+        for (int p = 0; p < kPitches; ++p) {
+          const int c = col[p * T];
+          if (c == 0) continue;
+          const long long key = (long long)(3 * p + (bend ? pitch_bend_at(crow, p, E.gauss) : 0)) << 32 | (unsigned)c;
+          int i = n++;
+          for (; i > 0 && kv[i - 1] > key; --i) kv[i] = kv[i - 1];
+          kv[i] = key;
+          n_est += c;
+        }
+        ef.kv = kv;
+        ef.n = n;
+        ef.midi = E.tab_midi;
+        ef.chroma = E.tab_chroma;
       } else if constexpr (kKind == EstKind::kGram) {
         const SalienceSettingDev p = E.salience[s];
         ef.row = E.gram + (E.frame_off[owner] + t) * E.width;
@@ -295,7 +325,9 @@ void launch_frame_match(const FrameRefs& R, const FrameEst& E, double window, in
                         long long* counts, cudaStream_t st) {
   const long long n = (long long)n_settings * R.n_frames;
   const unsigned int blocks = (unsigned int)std::max(1LL, (n + kMatchThreads - 1) / kMatchThreads);
-  if (E.roll)
+  if (E.roll && E.bend_on)
+    frame_match_kernel<EstKind::kBent><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
+  else if (E.roll)
     frame_match_kernel<EstKind::kRoll><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);
   else if (E.salience)
     frame_match_kernel<EstKind::kGram><<<blocks, kMatchThreads, 0, st>>>(R, E, window, ws, n_owner, n, counts);

@@ -8,6 +8,10 @@
 // of every (distinct bin range, frame), one warp each; the held cents of every (setting, file), one warp scan along the
 // frames; the counts, one thread per (setting, reference frame), reduced with warp-aggregated integer atomics.  Every
 // sum is an integer: the result is deterministic.
+// Decoded notes read as a melody (bp_score_note_melody_grid_*) replace the first two launches by one: a warp per
+// (setting, file) picks each frame's pitch from the grid decode's count roll and the note posteriorgram, bends it with
+// pitch_bend_at (the decode's own arg-max), writes the raw cents and carries the held cents along the file as the hold
+// kernel does; the counts kernel then reads those raw cents.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -49,11 +53,19 @@ __global__ void __launch_bounds__(kMelodyThreads) melody_argmax_kernel(const flo
   if (lane == 0) arg[w] = MelodyArg{best, bin};
 }
 
+// Where the counts read the raw estimate: explicit tracks, the arg-max of a posteriorgram, or decoded notes.
+enum class MelodySrc { kExplicit, kGram, kNotes };
+
 // Raw cents and voicing of estimate frame e (global) under chunk-local setting s: the grid reads the arg-max of the
-// setting's range (include/bp_b200.h, bp_score_melody_grid_*), explicit tracks their arrays.
-template <bool kGrid>
+// setting's range (include/bp_b200.h, bp_score_melody_grid_*), decoded notes the raw cents note_melody_kernel wrote (voiced
+// exactly where nonzero: every bin cents value is > 0), explicit tracks their arrays.
+template <MelodySrc kSrc>
 __device__ __forceinline__ double raw_cent(const MelodyEst& E, long long s, long long e, int& voiced) {
-  if constexpr (kGrid) {
+  if constexpr (kSrc == MelodySrc::kNotes) {
+    const double c = E.raw[s * E.n_frames + e];
+    voiced = c != 0.0;
+    return c;
+  } else if constexpr (kSrc == MelodySrc::kGram) {
     const MelodySettingDev p = E.set[s];
     const MelodyArg a = E.arg[p.range * E.n_frames + e];
     if (a.bin < 0) return voiced = 0, 0.0;
@@ -81,7 +93,7 @@ __global__ void __launch_bounds__(kMelodyThreads) melody_hold_kernel(MelodyEst E
   for (long long t0 = e0; t0 < e1; t0 += 32) {
     const long long e = t0 + lane;
     int v = 0;
-    const double c = e < e1 ? raw_cent<true>(E, s, e, v) : 0.0;
+    const double c = e < e1 ? raw_cent<MelodySrc::kGram>(E, s, e, v) : 0.0;
     const unsigned nz = __ballot_sync(0xffffffffu, c != 0.0) & (0xffffffffu >> (31 - lane));  // lanes <= this one
     const double from = __shfl_sync(0xffffffffu, c, nz ? 31 - __clz(nz) : 0);
     const double h = nz ? from : carry;
@@ -90,9 +102,52 @@ __global__ void __launch_bounds__(kMelodyThreads) melody_hold_kernel(MelodyEst E
   }
 }
 
+// ---- decoded notes --------------------------------------------------------------------------------------------------
+// Warp q = s * n_files + file, one frame per lane: the sounding pitches of the frame are those with a nonzero roll
+// count; the winner has the largest float32 note posteriorgram value, the lowest pitch on a tie, and a NaN loses to every
+// number (a frame whose sounding cells are all NaN takes its lowest sounding pitch).  raw[s][e] = bin_cent[3 (p - 21) +
+// bend] of the winner (its bend under the setting's bend flag), 0 when nothing sounds; held[s][e] as melody_hold_kernel.
+__global__ void __launch_bounds__(kMelodyThreads) note_melody_kernel(NoteMelodyEst N, MelodyEst E, int n_files,
+                                                                     long long n_warps) {
+  const long long q = (long long)blockIdx.x * (kMelodyThreads / 32) + (threadIdx.x >> 5);
+  if (q >= n_warps) return;
+  const int lane = threadIdx.x & 31;
+  const long long s = q / n_files;
+  const int file = (int)(q % n_files);
+  const long long e0 = N.frame_off[file], T = N.frame_off[file + 1] - e0;
+  const int* roll = N.roll + s * N.roll_stride + e0 * kPitches;
+  const bool bend = N.bend_on[s] != 0;
+  double* raw = E.raw + s * E.n_frames + e0;
+  double* held = E.held + s * E.n_frames + e0;
+  double carry = 0.0;
+  for (long long t0 = 0; t0 < T; t0 += 32) {
+    const long long t = t0 + lane;
+    double c = 0.0;
+    if (t < T) {
+      const float* nrow = N.note + (e0 + t) * kPitches;
+      int best = -1;
+      float bv = 0.0f;
+#pragma unroll 1
+      for (int p = 0; p < kPitches; ++p) {
+        if (roll[p * T + t] == 0) continue;
+        const float v = nrow[p];
+        if (best < 0 || v > bv || (bv != bv && v == v)) best = p, bv = v;
+      }
+      if (best >= 0)
+        c = E.bin_cent[3 * best + (bend ? pitch_bend_at(N.contour + (e0 + t) * kContourBins, best, N.gauss) : 0)];
+      raw[t] = c;
+    }
+    const unsigned nz = __ballot_sync(0xffffffffu, c != 0.0) & (0xffffffffu >> (31 - lane));  // lanes <= this one
+    const double from = __shfl_sync(0xffffffffu, c, nz ? 31 - __clz(nz) : 0);
+    const double h = nz ? from : carry;
+    if (t < T) held[t] = h;
+    carry = __shfl_sync(0xffffffffu, h, 31);
+  }
+}
+
 // ---- counts -----------------------------------------------------------------------------------------------------------
 // Thread x = s * K + k: reference frame k under chunk-local setting s.
-template <bool kGrid>
+template <MelodySrc kSrc>
 __global__ void __launch_bounds__(kMelodyThreads) melody_score_kernel(const MelodyRef* __restrict__ R, long long K,
                                                                       MelodyEst E, double tol, int n_owner,
                                                                       long long n_threads, long long* __restrict__ counts) {
@@ -108,7 +163,7 @@ __global__ void __launch_bounds__(kMelodyThreads) melody_score_kernel(const Melo
     int ev = 0;
     double ec = 0.0;
     if (r.zero >= 0) {
-      const double zc = raw_cent<kGrid>(E, s, r.zero, ev);
+      const double zc = raw_cent<kSrc>(E, s, r.zero, ev);
       if (r.flags & 2) {
         ec = zc;  // identical time bases: the raw estimate
       } else if (zc != 0.0) {
@@ -166,14 +221,22 @@ void launch_melody_grid(const float* gram, long long width, const MelodyRange* r
   melody_argmax_kernel<<<blocks_for(n_arg, per), kMelodyThreads, 0, st>>>(gram, width, ranges, std::max(F, 1LL), n_arg,
                                                                            E.arg);
   melody_hold_kernel<<<blocks_for(n_hold, per), kMelodyThreads, 0, st>>>(E, frame_off, n_files, n_hold);
-  melody_score_kernel<true><<<blocks_for(n, kMelodyThreads), kMelodyThreads, 0, st>>>(refs, std::max(K, 1LL), E, tol,
+  melody_score_kernel<MelodySrc::kGram><<<blocks_for(n, kMelodyThreads), kMelodyThreads, 0, st>>>(refs, std::max(K, 1LL), E, tol,
                                                                                      n_files, n, counts);
 }
 
 void launch_melody_explicit(const MelodyRef* refs, long long K, const MelodyEst& E, double tol, int n_items,
                             long long* counts, cudaStream_t st) {
-  melody_score_kernel<false><<<blocks_for(K, kMelodyThreads), kMelodyThreads, 0, st>>>(refs, std::max(K, 1LL), E, tol,
+  melody_score_kernel<MelodySrc::kExplicit><<<blocks_for(K, kMelodyThreads), kMelodyThreads, 0, st>>>(refs, std::max(K, 1LL), E, tol,
                                                                                       n_items, K, counts);
+}
+
+void launch_note_melody(const NoteMelodyEst& N, int n_files, const MelodyRef* refs, long long K, const MelodyEst& E,
+                        double tol, int n_settings, long long* counts, cudaStream_t st) {
+  const long long n_warps = (long long)n_settings * n_files, n = (long long)n_settings * K;
+  note_melody_kernel<<<blocks_for(n_warps, kMelodyThreads / 32), kMelodyThreads, 0, st>>>(N, E, n_files, n_warps);
+  melody_score_kernel<MelodySrc::kNotes><<<blocks_for(n, kMelodyThreads), kMelodyThreads, 0, st>>>(
+      refs, std::max(K, 1LL), E, tol, n_files, n, counts);
 }
 
 }  // namespace bp

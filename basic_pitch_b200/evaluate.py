@@ -31,6 +31,13 @@ and guess_unvoiced as the (times, f0) series mir_eval.melody scores, the arg-max
 for an unvoiced guess; the library counts, per (setting, file) or item, the seven integers of `MELODY_FIELDS`
 (`Model.score_melody_grid`, `Model.score_melody`, `inference.evaluate_melody_grid`; include/bp_b200.h,
 bp_score_melody_*), and `melody_scores` turns them into the five numbers of mir_eval.melody.evaluate (0.7), bit for bit.
+
+Decoded notes with their pitch bends, the output `predict` hands its users: a note of pitch p sounding at frame t takes
+contour bin k = 3 (p - 21) + its bend at t, of Hz `BENT_HZ[k]`.  `note_frames_to_multipitch` reads the notes as a
+multi-f0 series and `note_frames_to_melody` as a single-f0 track; they are the host definitions of
+bp_score_bent_frames_grid_* and bp_score_note_melody_grid_* (`Model.score_frames_grid(contours=...)`,
+`Model.score_note_melody_grid`, `inference.evaluate_frames_grid(pitch_bends=True)`,
+`inference.evaluate_note_melody_grid`), and `bent_bins` gives the tables those take.
 """
 from __future__ import annotations
 
@@ -410,3 +417,82 @@ def melody_scores(counts) -> Dict[str, np.ndarray]:
     else:
         out["mean"] = {k: (v.mean() if v.size else np.float64(0.0)) for k, v in out.items()}
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- bent notes
+# Hz of the 264 contour bins a decoded note with pitch bends reaches: bin k = 3 (pitch - 21) + bend, a third of a
+# semitone apart from MIDI 21.  BENT_HZ[3 c] is bit for bit `note_creation.midi_to_hz(21 + c)`, the Hz behind
+# EST_LOG2_HZ, EST_MIDI and EST_CHROMA, so a note without bends keeps its values; it is not constants.FREQ_BINS_CONTOURS,
+# whose bits differ.
+BENT_HZ = np.ascontiguousarray(440.0 * 2.0 ** ((21.0 + np.arange(264, dtype=np.float64) / 3.0 - 69.0) / 12.0))
+
+
+def bent_bins() -> Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """(hz, midi, chroma, cents) float64 of the 264 keys of `BENT_HZ`: midi and chroma as `multipitch_values` and cents
+    as `melody_values` give them (the tables bp_score_bent_frames_grid_* and bp_score_note_melody_grid_* take)."""
+    midi, chroma = multipitch_values(BENT_HZ)
+    return (BENT_HZ, np.ascontiguousarray(midi), np.ascontiguousarray(chroma),
+            np.ascontiguousarray(melody_values(BENT_HZ)[0]))
+
+
+def _note_frames(start, end, pitch, bends, n_frames):
+    """Every (frame, pitch, key) of a decode's notes (frames [start, end) clipped to [0, n_frames)), note by note:
+    key = 3 (pitch - 21) + the note's bend at that frame (bends[j][t - start[j]]; None or empty: 0)."""
+    s = np.asarray(start, np.int64).reshape(-1)
+    e = np.asarray(end, np.int64).reshape(-1)
+    p = np.asarray(pitch, np.int64).reshape(-1)
+    if not (len(s) == len(e) == len(p)):
+        raise ValueError(f"{len(s)} starts, {len(e)} ends and {len(p)} pitches")
+    if bends is not None and len(bends) != len(s):
+        raise ValueError(f"{len(s)} notes but {len(bends)} bend lists")
+    n = np.maximum(e - s, 0)
+    frame = np.repeat(s - np.cumsum(n) + n, n) + np.arange(n.sum())
+    note = np.repeat(np.arange(len(s)), n)
+    key = 3 * (p[note] - 21)
+    if bends is not None:
+        at = np.concatenate([[0], np.cumsum(n)])
+        for j, b in enumerate(bends):
+            if b is not None and len(b):
+                if len(b) != n[j]:
+                    raise ValueError(f"note {j}: {len(b)} bends for {n[j]} frames")
+                key[at[j]:at[j + 1]] += np.asarray(b, np.int64)
+    if len(key) and (key.min() < 0 or key.max() >= len(BENT_HZ)):
+        raise ValueError("a bent note lies outside the 264 contour bins")
+    keep = (frame >= 0) & (frame < n_frames)
+    return frame[keep], p[note][keep], key[keep]
+
+
+def note_frames_to_multipitch(start, end, pitch, bends, n_frames: int):
+    """A decode's notes with their pitch bends as a multi-f0 estimate (times (n_frames,), [Hz array per frame]),
+    mir_eval.multipitch's convention: frame t holds `BENT_HZ[k]` once for every note sounding at t (start <= t < end),
+    k = 3 (pitch - 21) + the note's bend at t, in ascending order; times are the model frame times.  start / end are
+    frames, pitch MIDI numbers, bends per-note lists as the decode returns them (None or empty for none: bend 0).  With
+    every bend 0 this is `notes_to_multipitch` of the notes at the model frame times.  The host definition of
+    bp_score_bent_frames_grid_* (include/bp_b200.h)."""
+    frame, _, key = _note_frames(start, end, pitch, bends, n_frames)
+    order = np.lexsort((key, frame))
+    cuts = np.searchsorted(frame[order], np.arange(1, n_frames))
+    return model_frames_to_time(n_frames), (np.split(BENT_HZ[key[order]], cuts) if n_frames else [])
+
+
+def note_frames_to_melody(start, end, pitch, bends, note_gram):
+    """A decode's notes with their pitch bends as a single-f0 estimate (times (T,), f0 (T,)), mir_eval.melody's
+    convention, for the note posteriorgram note_gram (T, 88) they were decoded from: frame t holds the f0 of the pitch,
+    among those with a note sounding at t, with the largest float32 note_gram[t, pitch - 21]; the lowest pitch wins a
+    tie and a NaN loses to every number (a frame whose sounding cells are all NaN takes its lowest sounding pitch).  The
+    f0 is +`BENT_HZ[k]`, voiced, k that pitch's bent key at t (a pitch's bend depends on (frame, pitch) only, so its
+    notes agree); 0 where no note sounds, with no unvoiced guess.  Arguments as `note_frames_to_multipitch`.  The host
+    definition of bp_score_note_melody_grid_* (include/bp_b200.h)."""
+    g = np.asarray(note_gram, np.float32)
+    if g.ndim != 2 or g.shape[1] != 88:
+        raise ValueError(f"a note posteriorgram must be (T, 88), got {g.shape}")
+    T = g.shape[0]
+    frame, p, key = _note_frames(start, end, pitch, bends, T)
+    f0 = np.zeros(T)
+    if len(frame):
+        v = g[frame, p - 21].astype(np.float64)
+        nan = np.isnan(v)
+        order = np.lexsort((p, -np.where(nan, 0.0, v), nan, frame))
+        first = order[np.unique(frame[order], return_index=True)[1]]
+        f0[frame[first]] = BENT_HZ[key[first]]
+    return model_frames_to_time(T), f0

@@ -540,24 +540,33 @@ class Model:
 
     def score_frames_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
                           settings: Sequence[Dict[str, Any]], references: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
-                          window: float = evaluate.WINDOW) -> np.ndarray:
+                          window: float = evaluate.WINDOW, contours: Optional[Sequence[np.ndarray]] = None) -> np.ndarray:
         """Frame-level multi-pitch counts of a batch of files decoded under every setting of a grid, scored against one
-        reference series per file, in ONE library call (`bp_score_frames_grid_host`): the notes never leave the device.
-        A setting is a dict of `decode_arrays`' keyword arguments (include_pitch_bends is ignored: bends are not
-        applied); a reference is (times (n,) in seconds, [Hz array per frame]), mir_eval's convention; window in
-        semitones.  The estimate of (setting, file) is the piano roll of its notes at the model frame times.  Returns
-        int64 counts (n_settings, n_files, 7) in the order of `evaluate.FRAME_FIELDS` (`evaluate.frame_scores` turns them
-        into mir_eval.multipitch's metrics)."""
+        reference series per file, in ONE library call: the notes never leave the device.  A setting is a dict of
+        `decode_arrays`' keyword arguments; a reference is (times (n,) in seconds, [Hz array per frame]), mir_eval's
+        convention; window in semitones.  Without contours (`bp_score_frames_grid_host`) include_pitch_bends is ignored
+        and the estimate of (setting, file) is the piano roll of its notes at the model frame times.  With the files'
+        contour posteriorgrams (`bp_score_bent_frames_grid_host`) each setting's include_pitch_bends (default True)
+        applies: the estimate is `evaluate.note_frames_to_multipitch` of its notes and bends, what `predict` returns.
+        Returns int64 counts (n_settings, n_files, 7) in the order of `evaluate.FRAME_FIELDS` (`evaluate.frame_scores`
+        turns them into mir_eval.multipitch's metrics)."""
         n_files, n_params = len(notes), len(settings)
         if len(references) != n_files:
             raise ValueError(f"{n_files} files but {len(references)} reference series")
         ps = self._grid_params(settings)
         refs, keep = self._multipitch_set(references, "references")
-        foff, n_all, o_all = self._cat_note_onset(notes, onsets)
         counts = np.zeros((n_params, n_files, 7), np.int64)
-        self._lib.bp_score_frames_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params,
-                                            C.byref(refs), float(window), _ptr(evaluate.EST_MIDI),
-                                            _ptr(evaluate.EST_CHROMA), _ptr(counts))
+        if contours is None:
+            foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+            self._lib.bp_score_frames_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(foff), n_files, ps, n_params,
+                                                C.byref(refs), float(window), _ptr(evaluate.EST_MIDI),
+                                                _ptr(evaluate.EST_CHROMA), _ptr(counts))
+            return counts
+        foff, n_all, o_all, c_all = self._cat_posteriorgrams(notes, onsets, contours, True)
+        _, midi, chroma, _ = evaluate.bent_bins()
+        self._lib.bp_score_bent_frames_grid_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(c_all), _ptr(foff), n_files, ps,
+                                                 n_params, C.byref(refs), float(window), _ptr(midi), _ptr(chroma),
+                                                 _ptr(counts))
         return counts
 
     def score_multipitch(self, estimates: Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]],
@@ -684,6 +693,31 @@ class Model:
         counts = np.zeros((n_params, n_files, 7), np.int64)
         self._lib.bp_score_melody_grid_host(self._h, _ptr(g_all), width, _ptr(foff), n_files, ps, n_params,
                                             C.byref(refs), float(cent_tolerance), _ptr(cents), _ptr(counts))
+        return counts
+
+    def score_note_melody_grid(self, notes: Sequence[np.ndarray], onsets: Sequence[np.ndarray],
+                               contours: Optional[Sequence[np.ndarray]], settings: Sequence[Dict[str, Any]],
+                               references: Sequence[Tuple[np.ndarray, np.ndarray]],
+                               cent_tolerance: float = evaluate.CENT_TOLERANCE) -> np.ndarray:
+        """Melody counts of a batch of files decoded under every setting of a grid, each (setting, file)'s notes with
+        their pitch bends read as a single-f0 track (`evaluate.note_frames_to_melody`) and scored against one reference
+        f0 track per file, in ONE library call (`bp_score_note_melody_grid_host`): the notes never leave the device.  A
+        setting is a dict of `decode_arrays`' keyword arguments, whose include_pitch_bends (default True) applies;
+        contours may be None only when no setting has bends; a reference is (times (n,) in seconds, f0 (n,) in Hz),
+        mir_eval.melody's convention.  Returns int64 counts (n_settings, n_files, 7) in the order of
+        `evaluate.MELODY_FIELDS` (`evaluate.melody_scores` turns them into mir_eval.melody.evaluate's scores)."""
+        n_files, n_params = len(notes), len(settings)
+        if len(references) != n_files:
+            raise ValueError(f"{n_files} files but {len(references)} reference tracks")
+        ps = self._grid_params(settings)
+        need_contours = any(bool(p.include_pitch_bends) for p in ps[:n_params])
+        refs, keep = self._melody_set(references, "references")
+        foff, n_all, o_all, c_all = self._cat_posteriorgrams(notes, onsets, contours, need_contours)
+        cents = evaluate.bent_bins()[3]
+        counts = np.zeros((n_params, n_files, 7), np.int64)
+        self._lib.bp_score_note_melody_grid_host(self._h, _ptr(n_all), _ptr(o_all), None if contours is None else _ptr(c_all),
+                                                 _ptr(foff), n_files, ps, n_params, C.byref(refs),
+                                                 float(cent_tolerance), _ptr(cents), _ptr(counts))
         return counts
 
     def score_melody(self, estimates: Sequence[Tuple[np.ndarray, np.ndarray]],
@@ -1219,19 +1253,22 @@ def evaluate_frames_grid(
     settings: Sequence[Dict[str, Any]],
     model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
     window: float = evaluate.WINDOW,
+    pitch_bends: bool = False,
 ):
     """Frame-level multi-pitch scores of a batch of annotated recordings under every setting of a grid (addition; no
     reference counterpart): the model runs once over the batch, and every (setting, file) is decoded and scored against
-    its file's reference series on the device in one `bp_score_frames_grid_host` call.  `audio` and `settings` as in
-    `evaluate_grid`; `references[i]` is file i's (times (n,) in seconds, [Hz array per frame]), mir_eval.multipitch's
-    convention (`evaluate.notes_to_multipitch` makes one from note annotations); window in semitones.
+    its file's reference series on the device in one library call.  `audio` and `settings` as in `evaluate_grid`;
+    `references[i]` is file i's (times (n,) in seconds, [Hz array per frame]), mir_eval.multipitch's convention
+    (`evaluate.notes_to_multipitch` makes one from note annotations); window in semitones.  With pitch_bends=False the
+    estimate is the piano roll of the notes (`bp_score_frames_grid_host`); with True it is the notes with their pitch
+    bends, what `predict` returns (`bp_score_bent_frames_grid_host`, `evaluate.note_frames_to_multipitch`).
 
     Returns (counts (n_settings, n_files, 7), `evaluate.frame_scores(counts)`)."""
     model, clips = _model_and_clips(audio, model_or_model_path)
-    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]  # include_pitch_bends: predict's True
     outs = model.run_inference_arrays(clips)
     counts = model.score_frames_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
-                                     window=window)
+                                     window=window, contours=[o["contour"] for o in outs] if pitch_bends else None)
     return counts, evaluate.frame_scores(counts)
 
 
@@ -1281,6 +1318,32 @@ def evaluate_melody_grid(
     outs = model.run_inference_arrays(clips)
     counts = model.score_melody_grid([o[kind] for o in outs], settings, references, kind=kind,
                                      cent_tolerance=cent_tolerance)
+    return counts, evaluate.melody_scores(counts)
+
+
+def evaluate_note_melody_grid(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    references: Sequence[Tuple[np.ndarray, np.ndarray]],
+    settings: Sequence[Dict[str, Any]],
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    pitch_bends: bool = True,
+    cent_tolerance: float = evaluate.CENT_TOLERANCE,
+):
+    """mir_eval.melody's scores of the decoded notes read as a single-f0 track (`evaluate.note_frames_to_melody`: per
+    frame the sounding pitch with the largest note posteriorgram value, with its pitch bend when pitch_bends), for a
+    batch of f0-annotated recordings under every setting of a grid (addition; no reference counterpart): the model runs
+    once over the batch, and every (setting, file) is decoded and scored on the device in one
+    `bp_score_note_melody_grid_host` call.  `audio` and `settings` as in `evaluate_grid`; `references[i]` is file i's
+    (times (n,) in seconds, f0 (n,) in Hz, 0 or negative where unvoiced), mir_eval.melody's convention; cent_tolerance in
+    cents.
+
+    Returns (counts (n_settings, n_files, 7), `evaluate.melody_scores(counts)`)."""
+    model, clips = _model_and_clips(audio, model_or_model_path)
+    decode = [{**infer.grid_setting(s, predict_names=True)[0], "include_pitch_bends": bool(pitch_bends)} for s in settings]
+    outs = model.run_inference_arrays(clips)
+    counts = model.score_note_melody_grid([o["note"] for o in outs], [o["onset"] for o in outs],
+                                          [o["contour"] for o in outs] if pitch_bends else None, decode, references,
+                                          cent_tolerance=cent_tolerance)
     return counts, evaluate.melody_scores(counts)
 
 

@@ -360,7 +360,8 @@ int bp_multipitch_map(const double* est_t, int64_t n_est, const double* ref_t, i
 /* Grid frame scoring: bp_score_grid_* with frame-level counts.  The estimate series of (setting, file) has the file's
  * T model frames, times bp_frame_times(T); frame t holds one value per decoded note with start_frame <= t < end_frame,
  * est_midi[pitch_midi] / est_chroma[pitch_midi] (two 128-entry host tables: midi finite and non-decreasing, chroma in
- * [0, 12)).  Pitch bends are not applied.  That is the piano roll of the note events, sampled at the model frames.
+ * [0, 12)).  Pitch bends are not applied (bp_score_bent_frames_grid_* applies them).  That is the piano roll of the
+ * note events, sampled at the model frames.
  * refs: one series per file.  h_counts [n_params][n_files][7] (host), in the order of rule 4.
  * Settings are validated, grouped, chunked and rerun as in bp_decode_grid_*.  Kernel launches per chunk: those of the
  * grid decode + 3 (note-count roll scatter, its prefix sum along frames, the match kernel), whatever the number of
@@ -377,6 +378,35 @@ int bp_score_frames_grid_host(bp_model_t* m, const float* h_note, const float* h
                               int32_t n_files, const bp_decode_params_t* params, int32_t n_params,
                               const bp_multipitch_set_t* refs, double window, const double* est_midi,
                               const double* est_chroma, int64_t* h_counts);
+/* Grid frame scoring of the bent notes: the series `predict` hands its users, notes with their pitch bends.
+ * Bent value: a decoded note of pitch p sounding at model frame t (start_frame <= t < end_frame) has the contour bin
+ * k = 3 (p - 21) + b, b its pitch bend at t as bp_decode_grid_* returns it (reference: get_pitch_bends,
+ * n_bins_tolerance 25: the arg-max window is clipped to the 264 contour bins, so k lies in [0, 263]); b = 0 under a
+ * setting without include_pitch_bends.  The bend is an arg-max over contour row t around bin 3 (p - 21): it depends on
+ * (file, p, t) only, so notes of one pitch overlapping at t carry the same bend and the count roll of
+ * bp_score_frames_grid_* still describes the estimate.
+ * The estimate series of (setting, file) has the file's T model frames at bp_frame_times(T); frame t holds
+ * bin_midi[k] / bin_chroma[k] once per sounding note (264-entry host tables: midi finite and non-decreasing, chroma in
+ * [0, 12); evaluate.bent_bins passes multipitch_values of evaluate.BENT_HZ, 440 * 2^((21 + k / 3 - 69) / 12), whose
+ * entries 3 c are bit for bit midi_to_hz(21 + c)).  Rules 1 to 4 then apply unchanged; evaluate.note_frames_to_multipitch
+ * is the host definition.  With every setting's bends off the counts equal bp_score_frames_grid_*'s with the matching
+ * 128-entry tables.
+ * Arguments as bp_score_frames_grid_* plus the contour posteriorgram, float32 row-major [total_frames][264], which may
+ * be NULL only when no setting has include_pitch_bends (as for bp_decode_grid_*; the message names the first setting
+ * that has).  Validation as bp_score_frames_grid_*, the tables named "bin table entry k".
+ * Kernel launches per chunk: those of the grid decode + 3 (roll scatter, roll prefix sum, match), whatever the number of
+ * settings and files; per call one memset of the counts, per chunk one of the roll.  The match thread of a frame puts
+ * its sounding pitches' (key, count) groups in ascending key order (bends can move a pitch past others up to 16
+ * semitones away) with an insertion sort in a 704-byte local array.  Device workspace as bp_score_frames_grid_*, plus 4
+ * bytes per setting; chunks as bp_decode_grid_chunk_params. */
+int bp_score_bent_frames_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                                     const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                     int32_t n_params, const bp_multipitch_set_t* refs, double window,
+                                     const double* bin_midi, const double* bin_chroma, int64_t* h_counts, void* stream);
+int bp_score_bent_frames_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                                   const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                   int32_t n_params, const bp_multipitch_set_t* refs, double window,
+                                   const double* bin_midi, const double* bin_chroma, int64_t* h_counts);
 /* Item i's estimate series (est, explicit) scored against item i's reference series; h_counts [n_items][7].  One
  * kernel launch and one memset (none for n_items == 0), synchronous.  Workspace: 16 bytes per reference value and 8 per
  * reference frame. */
@@ -513,6 +543,36 @@ int bp_score_melody_grid_host(bp_model_t* m, const float* h_gram, int32_t width,
  * launch and one memset (none for n_items == 0), synchronous. */
 int bp_score_melody_host(bp_model_t* m, const bp_melody_set_t* est, const bp_melody_set_t* refs, int32_t n_items,
                          double cent_tolerance, int64_t* h_counts);
+/* Grid melody scoring of the bent notes: the decoded notes of every (setting, file), with their pitch bends, read as a
+ * single-f0 track and scored by rules 1 to 4 above.  Frame t of the estimate (time bp_frame_times(T)[t]) holds the f0 of
+ * one sounding pitch: among the pitches p with a note sounding at t, the one with the largest float32 note
+ * posteriorgram value N[t][p - 21], the lowest pitch on a tie; a NaN loses to every number, so a frame whose sounding
+ * cells are all NaN takes its lowest sounding pitch.  Its cents are bin_cent[k], k the bent value of
+ * bp_score_bent_frames_grid_* (the setting's include_pitch_bends applies), voiced.  A frame with no sounding note has
+ * cents 0, unvoiced; there is no unvoiced guess.  evaluate.note_frames_to_melody is the host definition; evaluate.bent_bins
+ * gives the cents of evaluate.BENT_HZ.
+ * Arguments: the grid decode's inputs (posteriorgrams, h_frame_off, settings; the contour as for
+ * bp_score_bent_frames_grid_*), refs one reference track per file, cent_tolerance, bin_cent[264] (host table: finite,
+ * non-decreasing and > 0).  h_counts [n_params][n_files][7] (host) in the order of rule 4 (evaluate.MELODY_FIELDS).
+ * Validation before anything is enqueued: the grid decode's, cent_tolerance, the bin table ("bin table entry 17: cents
+ * must be > 0"), at most 2^31 - 1 frames in all, the references as for bp_score_melody_grid_*.  n_files == 0 or
+ * n_params == 0: BP_OK, nothing enqueued.
+ * Kernel launches per chunk: those of the grid decode + 4 (roll scatter, roll prefix sum, one warp per (setting, file)
+ * that picks, bends and holds every frame, the counts of every (setting, reference frame)); per call one memset of the
+ * counts, per chunk one of the roll.  No note crosses to the host; the counts are integers reduced with integer atomics.
+ * Device workspace beyond the decode's: the roll reuses the decode's "remaining energy" copies; 16 bytes per frame and
+ * setting of a chunk (raw and held cents), at most 1/22 of the decode's own workspace (bp_decode_grid_chunk_params bounds
+ * the chunk), and 48 bytes per reference frame.
+ * _device: posteriorgrams in device memory, work on `stream`, synchronised before returning; _host: host
+ * posteriorgrams, uploaded once. */
+int bp_score_note_melody_grid_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                                     const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                     int32_t n_params, const bp_melody_set_t* refs, double cent_tolerance,
+                                     const double* bin_cent, int64_t* h_counts, void* stream);
+int bp_score_note_melody_grid_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                                   const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params,
+                                   int32_t n_params, const bp_melody_set_t* refs, double cent_tolerance,
+                                   const double* bin_cent, int64_t* h_counts);
 /* Host-only: settings per chunk of bp_score_melody_grid_* for posteriorgrams of this many frames (>= 1): the arg-max
  * and held cents of a chunk of c settings stay within 2 GiB, c = max(1, 2^31 / max(1, 16 total_frames)). */
 int64_t bp_score_melody_chunk_params(int64_t total_frames);
