@@ -212,6 +212,10 @@ struct bp_model {
   DevBuf<MelodyArg> melody_arg;
   DevBuf<double> melody_held;
   DevBuf<double> melody_raw;  // bp_score_note_melody_grid_*: raw cents of every (setting, frame) of a chunk
+  // bp_evaluate_*: each note-derived family's references (pitched notes, intervals, frames, bent frames, f0), live
+  // together for the whole decode loop; the counts of every family of the call
+  DevBuf<unsigned char> eval_in[5];
+  DevBuf<long long> eval_counts;
   int64_t last_forward_n = 0;
   int last_path = 0;
   // optional per-kernel timing (bench.py roofline): CUDA events around one kernel family
@@ -618,14 +622,15 @@ int check_grid_args(const std::string& api, const bp_model* m, const int64_t* h_
 // The chunk loop of the grid entry points (bp_decode_grid_*, bp_score_grid_*): per chunk of settings the group tables,
 // the decode kernels with the rerun of pairs that outgrew their first allowance of note slots, then
 // tail(p0, P, counts, soff) with the chunk's notes in the slots: pair q (setting-major, chunk-local) has counts[q] notes
-// from m->slot_*[soff[q]], soff also at m->d_slot_off.  A tail returns BP_OK to go on to the next chunk.
+// from m->slot_*[soff[q]], soff also at m->d_slot_off.  A tail returns BP_OK to go on to the next chunk.  chunk: settings
+// per chunk, 0 for bp_decode_grid_chunk_params.
 template <class Tail>
 int decode_grid_chunks(bp_model* m, const std::string& api, const float* d_note, const float* d_onset,
                        const std::vector<long long>& foff, int n_files, const bp_decode_params_t* params, int n_params,
-                       cudaStream_t st, Tail&& tail) {
+                       cudaStream_t st, Tail&& tail, long long chunk = 0) {
   const long long total_frames = foff[n_files];
   const long long cells = total_frames * kPitches;
-  const long long chunk = bp_decode_grid_chunk_params(total_frames, n_files);
+  if (chunk <= 0) chunk = bp_decode_grid_chunk_params(total_frames, n_files);
   DecodeGridDev gd{};
   gd.n_files = n_files;
   gd.e_stride = cells;
@@ -976,9 +981,10 @@ struct NoteRefs {
 
 // The references of n_files files, the seconds of every frame a note of files of frame offsets foff can start or end
 // on and, unless est_log2_hz is NULL, the log2(Hz) table of the estimates; without it the references are intervals only
-// (their log2_hz is not read).
+// (their log2_hz is not read).  The upload goes to `in`.
 int upload_note_refs(bp_model* m, const bp_note_set_t* refs, int n_files, const std::vector<long long>& foff,
-                     const bp_score_params_t& sp, const double* est_log2_hz, NoteRefs& nr, cudaStream_t st) {
+                     const bp_score_params_t& sp, const double* est_log2_hz, NoteRefs& nr, DevBuf<unsigned char>& in,
+                     cudaStream_t st) {
   long long max_t = 0;
   for (int i = 0; i < n_files; ++i) max_t = std::max(max_t, foff[i + 1] - foff[i]);
   nr.tol = score_tol(sp);
@@ -991,9 +997,9 @@ int upload_note_refs(bp_model* m, const bp_note_set_t* refs, int n_files, const 
   bp_frame_times(max_t + 1, frame_t.data());
   const size_t o_ft = pk.add(frame_t.data(), sizeof(double) * (max_t + 1));
   const size_t o_l2 = est_log2_hz ? pk.add(est_log2_hz, sizeof(double) * 128) : 0;
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  const unsigned char* d = m->score_in.p;
+  CK(in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  const unsigned char* d = in.p;
   nr.sr = refs_at(d, o_ref);
   nr.r_orig = reinterpret_cast<const int*>(d + o_ref[5]);
   nr.e = ScoreEst{};
@@ -2140,7 +2146,7 @@ static int score_grid(const std::string& api, bp_model_t* m, Grams g, const int6
   DeviceGuard dg(m->device);
   NoteRefs nr;
   rc = stage_grams(m, total_frames, g, false);
-  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, pitched ? est_log2_hz : nullptr, nr, st);
+  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, pitched ? est_log2_hz : nullptr, nr, m->score_in, st);
   if (rc) return rc;
   CK(m->score_counts.reserve((size_t)n_params * n_files * 4));
   rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, params, n_params, st, [&](long long p0, int P,
@@ -2240,7 +2246,7 @@ static int match_grid(const std::string& api, bp_model_t* m, Grams g, const int6
   DeviceGuard dg(m->device);
   NoteRefs nr;
   rc = stage_grams(m, total_frames, g, false);
-  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, est_log2_hz, nr, st);
+  if (!rc) rc = upload_note_refs(m, refs, n_files, foff, *sp, est_log2_hz, nr, m->score_in, st);
   if (rc) return rc;
   const long long n_refs = nr.n_refs;
   GridNotes gn;  // over the grid so far
@@ -2704,6 +2710,46 @@ int64_t bp_score_salience_chunk_params(int64_t n_ref_frames, int64_t n_ref_value
   return std::max(1LL, kSalienceChunkBytes / std::max(1LL, per));
 }
 
+// The work of a validated salience grid on a device posteriorgram: one upload of the reference frames, the bin tables
+// and every setting to `in`, then one match launch per chunk of settings, adding into d_counts [n_params][n_files][7]
+// (zeroed by the caller).
+static int enqueue_salience_grid(bp_model_t* m, const float* gram, int32_t width, const std::vector<long long>& foff,
+                                 int32_t n_files, const bp_salience_params_t* params, int32_t n_params,
+                                 const bp_multipitch_set_t* refs, double window, const double* bin_midi,
+                                 const double* bin_chroma, long long* d_counts, DevBuf<unsigned char>& in,
+                                 cudaStream_t st) {
+  const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
+  std::vector<SalienceSettingDev> sal(n_params);
+  for (int k = 0; k < n_params; ++k)
+    sal[k] = SalienceSettingDev{params[k].threshold, params[k].peak_pick, params[k].bin_lo, params[k].bin_hi, 0};
+  Pack pk;
+  size_t o_ref[5];
+  pack_ref_frames(refs, foff, n_files, pk, o_ref);
+  const size_t o_tm = pk.add(bin_midi, sizeof(double) * width), o_tc = pk.add(bin_chroma, sizeof(double) * width),
+               o_set = pk.add(sal.data(), sizeof(SalienceSettingDev) * n_params);
+  CK(in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(m->d_frame_off.reserve(n_files + 1));
+  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
+  const long long chunk = bp_score_salience_chunk_params(K, V);
+  CK(m->score_ws_ref.reserve((size_t)(std::min<long long>(chunk, n_params) * frame_ws_stride(V, K)) + 1));
+  const FrameRefs R = frame_refs_at(in.p, o_ref[0], o_ref[1], o_ref + 2, K);
+  FrameEst e{};
+  e.gram = gram;
+  e.width = width;
+  e.frame_off = m->d_frame_off.p;
+  e.tab_midi = reinterpret_cast<const double*>(in.p + o_tm);
+  e.tab_chroma = reinterpret_cast<const double*>(in.p + o_tc);
+  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
+    const int P = (int)std::min<long long>(chunk, n_params - p0);
+    e.salience = reinterpret_cast<const SalienceSettingDev*>(in.p + o_set) + p0;
+    launch_frame_match(R, e, window, m->score_ws_ref.p, n_files, P, d_counts + kFrameCounts * p0 * n_files, st);
+    CKL();
+    m->launches += 1;
+  }
+  return BP_OK;
+}
+
 static int score_salience_grid(const std::string& api, bp_model_t* m, Grams g, int32_t width,
                                const int64_t* h_frame_off, int32_t n_files, const bp_salience_params_t* params,
                                int32_t n_params, const bp_multipitch_set_t* refs, double window, const double* bin_midi,
@@ -2717,39 +2763,12 @@ static int score_salience_grid(const std::string& api, bp_model_t* m, Grams g, i
   DeviceGuard dg(m->device);
   rc = stage_grams(m, foff[n_files], g, true, width);
   if (rc) return rc;
-  // one upload per call: the reference frames, the bin tables and every setting
-  const long long K = refs->frame_off[n_files], V = K > 0 ? refs->value_off[K] : 0;
-  std::vector<SalienceSettingDev> sal(n_params);
-  for (int k = 0; k < n_params; ++k)
-    sal[k] = SalienceSettingDev{params[k].threshold, params[k].peak_pick, params[k].bin_lo, params[k].bin_hi, 0};
-  Pack pk;
-  size_t o_ref[5];
-  pack_ref_frames(refs, foff, n_files, pk, o_ref);
-  const size_t o_tm = pk.add(bin_midi, sizeof(double) * width), o_tc = pk.add(bin_chroma, sizeof(double) * width),
-               o_set = pk.add(sal.data(), sizeof(SalienceSettingDev) * n_params);
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
-  CK(m->d_frame_off.reserve(n_files + 1));
-  CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
   const long long n_counts = (long long)n_params * n_files * kFrameCounts;
   CK(m->score_counts.reserve((size_t)n_counts));
   CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
-  const long long chunk = bp_score_salience_chunk_params(K, V);
-  CK(m->score_ws_ref.reserve((size_t)(std::min<long long>(chunk, n_params) * frame_ws_stride(V, K)) + 1));
-  const FrameRefs R = frame_refs_at(m->score_in.p, o_ref[0], o_ref[1], o_ref + 2, K);
-  FrameEst e{};
-  e.gram = g.contour;
-  e.width = width;
-  e.frame_off = m->d_frame_off.p;
-  e.tab_midi = reinterpret_cast<const double*>(m->score_in.p + o_tm);
-  e.tab_chroma = reinterpret_cast<const double*>(m->score_in.p + o_tc);
-  for (long long p0 = 0; p0 < n_params; p0 += chunk) {
-    const int P = (int)std::min<long long>(chunk, n_params - p0);
-    e.salience = reinterpret_cast<const SalienceSettingDev*>(m->score_in.p + o_set) + p0;
-    launch_frame_match(R, e, window, m->score_ws_ref.p, n_files, P, m->score_counts.p + kFrameCounts * p0 * n_files, st);
-    CKL();
-    m->launches += 1;
-  }
+  rc = enqueue_salience_grid(m, g.contour, width, foff, n_files, params, n_params, refs, window, bin_midi, bin_chroma,
+                             m->score_counts.p, m->score_in, st);
+  if (rc) return rc;
   CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * n_counts, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
@@ -2984,16 +3003,14 @@ int64_t bp_score_melody_chunk_params(int64_t total_frames) {
   return std::max(1LL, kMelodyChunkBytes / std::max(1LL, per));
 }
 
-static int score_melody_grid(const std::string& api, bp_model_t* m, Grams g, int32_t width, const int64_t* h_frame_off,
-                             int32_t n_files, const bp_melody_params_t* params, int32_t n_params,
-                             const bp_melody_set_t* refs, double tol, const double* bin_cent, int64_t* h_counts,
-                             cudaStream_t st) {
-  int rc = check_melody_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, tol, bin_cent, h_counts);
-  if (rc) return rc;
-  if (n_files == 0 || n_params == 0) return BP_OK;
-  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+// The work of a validated melody grid on a device posteriorgram: one upload of the reference frames, the bin table,
+// every setting and every chunk's ranges to `in`, then three launches per chunk of settings, adding into d_counts
+// [n_params][n_files][7] (zeroed by the caller).
+static int enqueue_melody_grid(bp_model_t* m, const float* gram, int32_t width, const std::vector<long long>& foff,
+                               int32_t n_files, const bp_melody_params_t* params, int32_t n_params,
+                               const bp_melody_set_t* refs, double tol, const double* bin_cent, long long* d_counts,
+                               DevBuf<unsigned char>& in, cudaStream_t st) {
   const long long F = foff[n_files];
-  if (F > 0 && !g.contour) return fail(BP_E_INVALID, api + ": null posteriorgram");
   const std::vector<MelodyRef> R = melody_grid_refs(refs, foff, n_files);
   const long long K = (long long)R.size();
   // settings in chunks; each chunk's distinct bin ranges, its settings pointing at them
@@ -3014,25 +3031,18 @@ static int score_melody_grid(const std::string& api, bp_model_t* m, Grams g, int
     max_ranges = std::max(max_ranges, (int)(ranges.size() - range_off.back()));
     range_off.push_back((long long)ranges.size());
   }
-  DeviceGuard dg(m->device);
-  rc = stage_grams(m, F, g, true, width);
-  if (rc) return rc;
-  // one upload per call: the reference frames, the bin table, every setting and every chunk's ranges
   Pack pk;
   const size_t o_ref = pk.add(R.data(), sizeof(MelodyRef) * K), o_tab = pk.add(bin_cent, sizeof(double) * width),
                o_set = pk.add(set.data(), sizeof(MelodySettingDev) * n_params),
                o_rng = pk.add(ranges.data(), sizeof(MelodyRange) * ranges.size());
-  CK(m->score_in.reserve(pk.buf.size()));
-  CK(cudaMemcpyAsync(m->score_in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(in.reserve(pk.buf.size()));
+  CK(cudaMemcpyAsync(in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
   CK(m->d_frame_off.reserve(n_files + 1));
   CK(cudaMemcpyAsync(m->d_frame_off.p, foff.data(), sizeof(long long) * (n_files + 1), cudaMemcpyHostToDevice, st));
-  const long long n_counts = (long long)n_params * n_files * kMelodyCounts;
-  CK(m->score_counts.reserve((size_t)n_counts));
-  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
   const long long P_max = std::min<long long>(chunk, n_params);
   CK(m->melody_arg.reserve((size_t)(max_ranges * F) + 1));
   CK(m->melody_held.reserve((size_t)(P_max * F) + 1));
-  const unsigned char* d = m->score_in.p;
+  const unsigned char* d = in.p;
   MelodyEst e{};
   e.arg = m->melody_arg.p;
   e.bin_cent = reinterpret_cast<const double*>(d + o_tab);
@@ -3041,13 +3051,34 @@ static int score_melody_grid(const std::string& api, bp_model_t* m, Grams g, int
   for (long long p0 = 0, c = 0; p0 < n_params; p0 += chunk, ++c) {
     const int P = (int)std::min<long long>(chunk, n_params - p0);
     e.set = reinterpret_cast<const MelodySettingDev*>(d + o_set) + p0;
-    launch_melody_grid(g.contour, width, reinterpret_cast<const MelodyRange*>(d + o_rng) + range_off[c],
+    launch_melody_grid(gram, width, reinterpret_cast<const MelodyRange*>(d + o_rng) + range_off[c],
                        (int)(range_off[c + 1] - range_off[c]), m->d_frame_off.p, n_files,
-                       reinterpret_cast<const MelodyRef*>(d + o_ref), K, e, tol, P,
-                       m->score_counts.p + kMelodyCounts * p0 * n_files, st);
+                       reinterpret_cast<const MelodyRef*>(d + o_ref), K, e, tol, P, d_counts + kMelodyCounts * p0 * n_files,
+                       st);
     CKL();
     m->launches += 3;
   }
+  return BP_OK;
+}
+
+static int score_melody_grid(const std::string& api, bp_model_t* m, Grams g, int32_t width, const int64_t* h_frame_off,
+                             int32_t n_files, const bp_melody_params_t* params, int32_t n_params,
+                             const bp_melody_set_t* refs, double tol, const double* bin_cent, int64_t* h_counts,
+                             cudaStream_t st) {
+  int rc = check_melody_grid(api, m, width, h_frame_off, n_files, params, n_params, refs, tol, bin_cent, h_counts);
+  if (rc) return rc;
+  if (n_files == 0 || n_params == 0) return BP_OK;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  if (foff[n_files] > 0 && !g.contour) return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  rc = stage_grams(m, foff[n_files], g, true, width);
+  if (rc) return rc;
+  const long long n_counts = (long long)n_params * n_files * kMelodyCounts;
+  CK(m->score_counts.reserve((size_t)n_counts));
+  CK(cudaMemsetAsync(m->score_counts.p, 0, sizeof(long long) * n_counts, st));
+  rc = enqueue_melody_grid(m, g.contour, width, foff, n_files, params, n_params, refs, tol, bin_cent, m->score_counts.p,
+                           m->score_in, st);
+  if (rc) return rc;
   CK(cudaMemcpyAsync(h_counts, m->score_counts.p, sizeof(long long) * n_counts, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
@@ -3198,6 +3229,388 @@ int bp_score_melody_host(bp_model_t* m, const bp_melody_set_t* est, const bp_mel
                      st));
   CK(cudaStreamSynchronize(st));
   return BP_OK;
+}
+
+// ---- every family in one pass (bp_evaluate_*) --------------------------------------------------------------------------
+
+// Which families a request asks for (include/bp_b200.h, bp_eval_request_t).
+struct EvalFamilies {
+  bool notes, onoff, pairs, frames, bent, mel, flat, sal, melody;
+  bool decode() const { return notes || onoff || pairs || frames || bent || mel || flat; }
+};
+
+static EvalFamilies eval_families(const bp_eval_request_t& r) {
+  return EvalFamilies{r.notes_counts != nullptr,       r.onset_offset_counts != nullptr,
+                      r.pair_notes || r.pair_match,    r.frames_counts != nullptr,
+                      r.bent_frames_counts != nullptr, r.note_melody_counts != nullptr,
+                      r.flat_note_melody_counts != nullptr, r.salience_counts != nullptr,
+                      r.melody_counts != nullptr};
+}
+
+static int eval_gram_width(int32_t gram) { return gram == 1 ? kPitches : kContourBins; }
+
+int64_t bp_evaluate_chunk_params(int64_t total_frames, int32_t n_files, const bp_eval_request_t* req) {
+  const long long F = std::max<int64_t>(total_frames, 0);
+  const int n = std::max<int32_t>(n_files, 0);
+  long long per = grid_setting_bytes(F, n);
+  if (req && n > 0) {
+    const EvalFamilies f = eval_families(*req);
+    const long long S = std::min(F * kPitches, 8 * F + 64LL * n);
+    const long long R = (f.notes || f.onoff || f.pairs) && req->note_refs ? (long long)req->note_refs->note_off[n] : 0;
+    long long K = 0, V = 0;
+    if ((f.frames || f.bent) && req->mp_refs) {
+      K = req->mp_refs->frame_off[n];
+      V = K > 0 ? req->mp_refs->value_off[K] : 0;
+    }
+    if (f.notes) per += 8 * R + 16 * S;
+    if (f.onoff) per += 24 * R + 16 * S + 8LL * n;
+    if (f.pairs) per += 8 * R + 28 * S;
+    if (f.frames) per += 16 * V + 8 * K;
+    if (f.bent) per += 16 * V + 8 * K + 4;
+    if (f.mel || f.flat) per += 16 * F;
+  }
+  return std::max(1LL, std::min(kDecodeGridMaxChunk, kDecodeGridChunkBytes / per));
+}
+
+// Everything bp_evaluate_* check before anything is enqueued: each requested family with its standalone checks, the
+// message prefixed by the family.  *any_bends: some setting has include_pitch_bends.
+static int check_eval(const std::string& api, const bp_model* m, const int64_t* h_frame_off, int n_files,
+                      const bp_eval_request_t* req, bool* any_bends) {
+  if (!m || !req || n_files < 0 || (n_files > 0 && !h_frame_off)) return fail(BP_E_INVALID, api + ": bad argument");
+  const bp_eval_request_t& r = *req;
+  const EvalFamilies f = eval_families(r);
+  *any_bends = false;
+  int rc = BP_OK;
+  for (int k = 0; f.decode() && r.params && k < r.n_params && !rc; ++k)
+    rc = validate_params(r.params + k, api + ": decode params[" + std::to_string(k) + "]");
+  if (!rc && f.decode()) rc = check_grid_args(api, m, h_frame_off, n_files, r.params, r.n_params, any_bends);
+  const int P = r.n_params;
+  if (!rc && f.notes) rc = check_score_grid(api + ": notes", n_files, P, r.note_refs, r.score, r.est_log2_hz, r.notes_counts, true);
+  if (!rc && f.onoff)
+    rc = check_score_grid(api + ": onset_offset", n_files, P, r.note_refs, r.score, nullptr, r.onset_offset_counts, false);
+  if (!rc && f.pairs) {
+    rc = check_score_grid(api + ": pairs", n_files, P, r.note_refs, r.score, r.est_log2_hz, r.pair_match, true);
+    if (!rc && (!r.pair_notes || !r.pair_notes->note_off || !r.pair_notes->bend_off))
+      rc = fail(BP_E_INVALID, api + ": pairs: notes arrays missing");
+  }
+  if (!rc && f.frames)
+    rc = check_frames_grid(api + ": frames", n_files, P, r.mp_refs, r.window, r.est_midi, r.est_chroma, r.frames_counts, false);
+  if (!rc && f.bent)
+    rc = check_frames_grid(api + ": bent_frames", n_files, P, r.mp_refs, r.window, r.bin_midi, r.bin_chroma,
+                           r.bent_frames_counts, true);
+  for (int k = 0; k < 2 && !rc; ++k) {  // the two note melodies, as bp_score_note_melody_grid_*
+    if (!(k == 0 ? f.mel : f.flat)) continue;
+    const std::string who = api + (k == 0 ? ": note_melody" : ": flat_note_melody");
+    rc = check_tolerance(who, r.cent_tolerance);
+    if (rc || n_files == 0 || P == 0) continue;
+    if (!r.bin_cent) rc = fail(BP_E_INVALID, who + ": bad argument");
+    if (!rc) rc = check_cent_table(who, r.bin_cent, kContourBins, true);
+    if (!rc && h_frame_off[n_files] > INT_MAX) rc = fail(BP_E_INVALID, who + ": more than 2^31 - 1 frames");
+    if (!rc) rc = check_melody_set(who, "references", "file", r.f0_refs, n_files, false);
+  }
+  if (!rc && f.sal)
+    rc = check_salience_grid(api + ": salience", m, eval_gram_width(r.salience_gram), h_frame_off, n_files,
+                             r.salience_params, r.n_salience, r.salience_refs, r.salience_window, r.salience_midi,
+                             r.salience_chroma, r.salience_counts);
+  if (!rc && f.sal && r.salience_gram != 0 && r.salience_gram != 1)
+    rc = fail(BP_E_INVALID, api + ": salience: salience_gram must be 0 (contour) or 1 (note)");
+  if (!rc && f.melody)
+    rc = check_melody_grid(api + ": melody", m, eval_gram_width(r.melody_gram), h_frame_off, n_files, r.melody_params,
+                           r.n_melody, r.melody_refs, r.melody_tolerance, r.melody_cent, r.melody_counts);
+  if (!rc && f.melody && r.melody_gram != 0 && r.melody_gram != 1)
+    rc = fail(BP_E_INVALID, api + ": melody: melody_gram must be 0 (contour) or 1 (note)");
+  return rc;
+}
+
+// Whether a request reads the contour posteriorgram: bent families with a bending setting, or a posteriorgram family on
+// the contour.
+static bool eval_needs_contour(const bp_eval_request_t& r, bool any_bends) {
+  const EvalFamilies f = eval_families(r);
+  return (any_bends && (f.bent || f.mel)) || (f.sal && r.salience_gram == 0) || (f.melody && r.melody_gram == 0);
+}
+
+// The work of a validated request on device posteriorgrams g (the contour may be NULL when eval_needs_contour is
+// false), synchronised before returning.
+static int run_eval(const std::string& api, bp_model_t* m, Grams g, const std::vector<long long>& foff, int32_t n_files,
+                    const bp_eval_request_t& r, cudaStream_t st) {
+  const EvalFamilies f = eval_families(r);
+  const int n_params = f.decode() ? r.n_params : 0;
+  const long long F = foff[n_files], cells = F * kPitches;
+  if (f.pairs) {
+    g_need_notes = g_need_bends = 0;
+    r.pair_notes->note_off[0] = 0;
+    r.pair_notes->bend_off[0] = 0;
+  }
+  // counts of every family, back to back in one buffer zeroed once: notes, onset_offset, frames, bent_frames,
+  // note_melody, flat_note_melody, salience, melody
+  const long long n4 = (long long)n_params * n_files * 4, n7 = (long long)n_params * n_files * 7;
+  const long long sizes[8] = {f.notes ? n4 : 0, f.onoff ? n4 : 0, f.frames ? n7 : 0, f.bent ? n7 : 0,
+                              f.mel ? n7 : 0,   f.flat ? n7 : 0,  f.sal ? (long long)r.n_salience * n_files * 7 : 0,
+                              f.melody ? (long long)r.n_melody * n_files * 7 : 0};
+  int64_t* const outs[8] = {r.notes_counts,       r.onset_offset_counts,     r.frames_counts,   r.bent_frames_counts,
+                            r.note_melody_counts, r.flat_note_melody_counts, r.salience_counts, r.melody_counts};
+  long long at[9] = {0};
+  for (int k = 0; k < 8; ++k) at[k + 1] = at[k] + sizes[k];
+  CK(m->eval_counts.reserve((size_t)at[8] + 1));
+  long long* counts = m->eval_counts.p;
+  if (at[8] > 0) CK(cudaMemsetAsync(counts, 0, sizeof(long long) * at[8], st));
+  // ---- references, once per family
+  const long long chunk = bp_evaluate_chunk_params(F, n_files, &r);
+  NoteRefs nr, nr_iv;
+  int rc = BP_OK;
+  if (n_params > 0 && (f.notes || f.pairs))
+    rc = upload_note_refs(m, r.note_refs, n_files, foff, *r.score, r.est_log2_hz, nr, m->eval_in[0], st);
+  if (!rc && n_params > 0 && f.onoff)
+    rc = upload_note_refs(m, r.note_refs, n_files, foff, *r.score, nullptr, nr_iv, m->eval_in[1], st);
+  if (rc) return rc;
+  FrameRefs fr[2]{};  // frames, bent_frames
+  FrameEst fe[2]{};
+  long long V = 0, K = 0;
+  for (int b = 0; b < 2 && n_params > 0; ++b) {
+    if (!(b == 0 ? f.frames : f.bent)) continue;
+    K = r.mp_refs->frame_off[n_files], V = K > 0 ? r.mp_refs->value_off[K] : 0;
+    const int n_tab = b ? kContourBins : 128;
+    Pack pk;
+    size_t o_ref[5];
+    pack_ref_frames(r.mp_refs, foff, n_files, pk, o_ref);
+    const size_t o_tm = pk.add(b ? r.bin_midi : r.est_midi, sizeof(double) * n_tab),
+                 o_tc = pk.add(b ? r.bin_chroma : r.est_chroma, sizeof(double) * n_tab);
+    std::vector<int> bend_on(n_params);
+    for (int k = 0; k < n_params; ++k) bend_on[k] = r.params[k].include_pitch_bends != 0;
+    const size_t o_bend = pk.add(bend_on.data(), sizeof(int) * n_params);
+    DevBuf<unsigned char>& in = m->eval_in[2 + b];
+    CK(in.reserve(pk.buf.size()));
+    CK(cudaMemcpyAsync(in.p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+    fr[b] = frame_refs_at(in.p, o_ref[0], o_ref[1], o_ref + 2, K);
+    fe[b].roll_stride = cells;
+    fe[b].tab_midi = reinterpret_cast<const double*>(in.p + o_tm);
+    fe[b].tab_chroma = reinterpret_cast<const double*>(in.p + o_tc);
+    if (b) {
+      fe[b].bend_on = reinterpret_cast<const int*>(in.p + o_bend);
+      fe[b].contour = g.contour;
+      fe[b].gauss = m->d_gauss;
+    }
+  }
+  const MelodyRef* mel_ref = nullptr;
+  const double* mel_tab = nullptr;
+  const int* mel_bend[2] = {nullptr, nullptr};  // note_melody: each setting's flag; flat_note_melody: zeros
+  long long mel_K = 0;
+  if (n_params > 0 && (f.mel || f.flat)) {
+    const std::vector<MelodyRef> R = melody_grid_refs(r.f0_refs, foff, n_files);
+    mel_K = (long long)R.size();
+    std::vector<int> bend_on(n_params), zero(n_params, 0);
+    for (int k = 0; k < n_params; ++k) bend_on[k] = r.params[k].include_pitch_bends != 0;
+    Pack pk;
+    const size_t o_ref = pk.add(R.data(), sizeof(MelodyRef) * mel_K),
+                 o_tab = pk.add(r.bin_cent, sizeof(double) * kContourBins),
+                 o_bend = pk.add(bend_on.data(), sizeof(int) * n_params), o_zero = pk.add(zero.data(), sizeof(int) * n_params);
+    CK(m->eval_in[4].reserve(pk.buf.size()));
+    CK(cudaMemcpyAsync(m->eval_in[4].p, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+    const unsigned char* d = m->eval_in[4].p;
+    mel_ref = reinterpret_cast<const MelodyRef*>(d + o_ref);
+    mel_tab = reinterpret_cast<const double*>(d + o_tab);
+    mel_bend[0] = reinterpret_cast<const int*>(d + o_bend);
+    mel_bend[1] = reinterpret_cast<const int*>(d + o_zero);
+    const long long P_max = std::min<long long>(chunk, n_params);
+    CK(m->melody_held.reserve((size_t)(P_max * F) + 1));
+    CK(m->melody_raw.reserve((size_t)(P_max * F) + 1));
+  }
+  // ---- one decode per chunk, then each requested family's tail on its slots, in the order of the header's table.  No
+  // tail writes what a later one reads: the slots, note counts and d_slot_off are only read; the rolls live in the
+  // decode's dead E and are rebuilt by every tail that reads them; the scoring workspaces are private to a launch.
+  GridNotes gn;
+  if (n_params > 0 && n_files > 0)
+    rc = decode_grid_chunks(m, api, g.note, g.onset, foff, n_files, r.params, n_params, st, [&](long long p0, int P,
+                            const std::vector<int>& note_counts, const std::vector<long long>& soff) -> int {
+      const long long n_pairs = (long long)P * n_files;
+      for (int k = 0; k < 2; ++k) {  // notes, onset_offset: bp_score_grid_*'s tail
+        const bool pitched = k == 0;
+        if (!(pitched ? f.notes : f.onoff)) continue;
+        const NoteRefs& q = pitched ? nr : nr_iv;
+        CK(m->score_ws_ref.reserve((size_t)((pitched ? 2 : 6) * P * q.n_refs) + 1));
+        CK(m->score_ws_est.reserve((size_t)(4 * soff[n_pairs] + (pitched ? 0 : 2 * n_pairs)) + 1));
+        ScoreEst e = q.e;
+        e.off = m->d_slot_off.p;
+        e.count = m->note_count.p;
+        e.start = m->slot_start.p;
+        e.end = m->slot_end.p;
+        if (pitched) e.pitch = m->slot_pitch.p;
+        (pitched ? launch_score_match : launch_onset_offset)(q.sr, e, q.tol,
+                                                             ScoreWork{m->score_ws_ref.p, m->score_ws_est.p, q.n_refs},
+                                                             n_files, n_pairs, counts + at[k] + 4 * p0 * n_files, st);
+        CKL();
+        m->launches += 1;
+      }
+      if (f.pairs) {  // bp_match_grid_*'s tail
+        bp_notes_t* notes = r.pair_notes;
+        const long long note0 = gn.n_notes, n_refs = nr.n_refs;
+        int rc = grid_chunk_notes(m, api, g.note, nullptr, r.params, false, n_files, p0, P, note_counts, notes, gn, st);
+        if (rc) return rc;
+        if (gn.notes_fit && n_refs > 0) {
+          int32_t* out = r.pair_match + 2 * p0 * n_refs;
+          if (gn.n_notes == note0) {
+            std::fill(out, out + 2 * P * n_refs, -1);
+          } else {
+            std::vector<long long> est_off(n_pairs + 1);
+            for (long long q = 0; q <= n_pairs; ++q) est_off[q] = notes->note_off[p0 * n_files + q] - note0;
+            CK(m->match_est_off.reserve((size_t)n_pairs + 1));
+            CK(cudaMemcpyAsync(m->match_est_off.p, est_off.data(), sizeof(long long) * (n_pairs + 1),
+                               cudaMemcpyHostToDevice, st));
+            CK(m->match_out.reserve((size_t)(2 * P * n_refs)));
+            ScoreEst e = nr.e;
+            e.off = m->match_est_off.p;
+            e.start = m->d_start.p;
+            e.end = m->d_end.p;
+            e.pitch = m->d_pitch.p;
+            rc = match_pairs(m, api, nr.sr, nr.r_orig, e, nr.tol, n_files, n_pairs, est_off, r.note_refs->note_off,
+                             n_refs, m->match_out.p, st);
+            if (rc) return rc;
+            CK(cudaMemcpyAsync(out, m->match_out.p, sizeof(int) * 2 * P * n_refs, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+          }
+        }
+      }
+      int* roll = reinterpret_cast<int*>(m->energy.p);  // each setting's E is dead once the loops have run
+      auto build_roll = [&]() -> int {
+        if (cells > 0) CK(cudaMemsetAsync(roll, 0, sizeof(int) * P * cells, st));
+        launch_frame_roll(m->d_frame_off.p, m->d_slot_off.p, m->note_count.p, m->slot_start.p, m->slot_end.p,
+                          m->slot_pitch.p, n_files, P, roll, cells, st);
+        CKL();
+        return BP_OK;
+      };
+      for (int b = 0; b < 2; ++b) {  // frames, bent_frames: bp_score_frames_grid_*'s tail
+        if (!(b == 0 ? f.frames : f.bent)) continue;
+        int rc = build_roll();
+        if (rc) return rc;
+        CK(m->score_ws_ref.reserve((size_t)(P * frame_ws_stride(V, K)) + 1));
+        FrameEst e = fe[b];
+        e.roll = roll;
+        e.frame_off = m->d_frame_off.p;
+        if (b) e.bend_on += p0;
+        launch_frame_match(fr[b], e, r.window, m->score_ws_ref.p, n_files, P, counts + at[2 + b] + kFrameCounts * p0 * n_files,
+                           st);
+        CKL();
+        m->launches += 3;
+      }
+      for (int b = 0; b < 2; ++b) {  // note_melody, flat_note_melody: bp_score_note_melody_grid_*'s tail
+        if (!(b == 0 ? f.mel : f.flat)) continue;
+        int rc = build_roll();
+        if (rc) return rc;
+        MelodyEst e{};
+        e.bin_cent = mel_tab;
+        e.held = m->melody_held.p;
+        e.raw = m->melody_raw.p;
+        e.n_frames = F;
+        const NoteMelodyEst N{roll, cells, m->d_frame_off.p, g.note, g.contour, m->d_gauss, mel_bend[b] + p0};
+        launch_note_melody(N, n_files, mel_ref, mel_K, e, r.cent_tolerance, P,
+                           counts + at[4 + b] + kMelodyCounts * p0 * n_files, st);
+        CKL();
+        m->launches += 4;
+      }
+      return BP_OK;
+    }, chunk);
+  if (rc) return rc;
+  // ---- the posteriorgram families, on the posteriorgrams as they are
+  if (f.sal && r.n_salience > 0)
+    rc = enqueue_salience_grid(m, r.salience_gram == 1 ? g.note : g.contour, eval_gram_width(r.salience_gram), foff,
+                               n_files, r.salience_params, r.n_salience, r.salience_refs, r.salience_window,
+                               r.salience_midi, r.salience_chroma, counts + at[6], m->score_in, st);
+  if (!rc && f.melody && r.n_melody > 0)
+    rc = enqueue_melody_grid(m, r.melody_gram == 1 ? g.note : g.contour, eval_gram_width(r.melody_gram), foff, n_files,
+                             r.melody_params, r.n_melody, r.melody_refs, r.melody_tolerance, r.melody_cent,
+                             counts + at[7], m->score_in, st);
+  if (rc) return rc;
+  for (int k = 0; k < 8; ++k)
+    if (sizes[k] > 0) CK(cudaMemcpyAsync(outs[k], counts + at[k], sizeof(long long) * sizes[k], cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return f.pairs ? grid_notes_result(api, gn) : BP_OK;
+}
+
+// bp_evaluate_device / bp_evaluate_host.
+static int evaluate_grams(const std::string& api, bp_model_t* m, Grams g, const int64_t* h_frame_off, int32_t n_files,
+                          const bp_eval_request_t* req, cudaStream_t st) {
+  bool any_bends = false;
+  int rc = check_eval(api, m, h_frame_off, n_files, req, &any_bends);
+  if (rc || n_files == 0) return rc;
+  const std::vector<long long> foff(h_frame_off, h_frame_off + n_files + 1);
+  const long long F = foff[n_files];
+  const bool contour = eval_needs_contour(*req, any_bends);
+  const EvalFamilies f = eval_families(*req);
+  const bool note = f.decode() || (f.sal && req->salience_gram == 1) || (f.melody && req->melody_gram == 1);
+  if (F > 0 && ((note && !g.note) || (f.decode() && !g.onset) || (contour && !g.contour)))
+    return fail(BP_E_INVALID, api + ": null posteriorgram");
+  DeviceGuard dg(m->device);
+  if (g.host && F > 0) {  // uploaded once for every family: the posteriorgrams some family reads
+    rc = reserve_rows(m, F);
+    if (rc) return rc;
+    if (note) CK(cudaMemcpyAsync(m->st_note.p, g.note, sizeof(float) * F * kPitches, cudaMemcpyHostToDevice, st));
+    if (f.decode()) CK(cudaMemcpyAsync(m->st_onset.p, g.onset, sizeof(float) * F * kPitches, cudaMemcpyHostToDevice, st));
+    if (contour)
+      CK(cudaMemcpyAsync(m->st_contour.p, g.contour, sizeof(float) * F * kContourBins, cudaMemcpyHostToDevice, st));
+    g = Grams{note ? m->st_note.p : nullptr, f.decode() ? m->st_onset.p : nullptr, contour ? m->st_contour.p : nullptr,
+              false};
+  }
+  return run_eval(api, m, g, foff, n_files, *req, st);
+}
+
+int bp_evaluate_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                       const int64_t* h_frame_off, int32_t n_files, const bp_eval_request_t* req, void* stream) {
+  return evaluate_grams("bp_evaluate_device", m, Grams{d_note, d_onset, d_contour, false}, h_frame_off, n_files, req,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int bp_evaluate_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                     const int64_t* h_frame_off, int32_t n_files, const bp_eval_request_t* req) {
+  return evaluate_grams("bp_evaluate_host", m, Grams{h_note, h_onset, h_contour, true}, h_frame_off, n_files, req,
+                        m ? m->stream : nullptr);
+}
+
+// bp_evaluate_audio_host / bp_evaluate_pcm_files_host once the batch is described: the request is checked against the
+// batch's frame offsets, the pipeline runs without a decode and leaves the posteriorgrams in the model's staging, where
+// they are scored.
+static int evaluate_batch(bp_model_t* m, Batch& b, const bp_eval_request_t* req, Rows host, int64_t* h_frame_off) {
+  const std::string api = b.api;
+  const int n_files = b.n_files();
+  std::vector<int64_t> frame_off(n_files + 1, 0);
+  for (int i = 0; i < n_files; ++i) frame_off[i + 1] = frame_off[i] + bp_num_frames(b.rel[i + 1] - b.rel[i]);
+  const std::vector<long long> foff(frame_off.begin(), frame_off.end());
+  bool any_bends = false;
+  int rc = check_eval(api, m, frame_off.data(), n_files, req, &any_bends);
+  if (rc) return rc;
+  if (b.pcm && (rc = load_ingest_taps(api, m->device, b.ingest))) return rc;
+  rc = run_batch(m, b, nullptr, host, nullptr, nullptr, h_frame_off, m->stream);
+  if (rc || n_files == 0) return rc;
+  return run_eval(api, m, Grams{m->st_note.p, m->st_onset.p, m->st_contour.p, false}, foff, n_files, *req, m->stream);
+}
+
+int bp_evaluate_audio_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
+                           const bp_eval_request_t* req, float* h_note, float* h_onset, float* h_contour,
+                           int64_t* h_frame_off) {
+  if (!m || !h_sample_off || !h_frame_off || n_files < 0) return fail(BP_E_INVALID, "bp_evaluate_audio_host: bad argument");
+  DeviceGuard g(m->device);
+  Batch b{"bp_evaluate_audio_host", h_audio, false, nullptr};
+  const int rc = describe_batch(b, h_sample_off, nullptr, n_files);
+  if (rc) return rc;
+  return evaluate_batch(m, b, req, Rows{h_note, h_onset, h_contour}, h_frame_off);
+}
+
+int bp_evaluate_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, const bp_eval_request_t* req,
+                               float* h_note, float* h_onset, float* h_contour, int64_t* h_frame_off,
+                               int64_t* h_sample_off) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_evaluate_pcm_files_host: bad argument");
+  Batch b{"bp_evaluate_pcm_files_host", nullptr, false, nullptr};
+  b.pcm = files;
+  int rc = describe_pcm(b.api, files, n_files, false, b.ingest, b.pcm_bytes);
+  if (rc) return rc;
+  b.rel.assign(n_files + 1, 0);
+  for (int i = 0; i < n_files; ++i) {
+    b.rel[i + 1] = b.rel[i] + b.ingest[i].n_out;
+    b.total_frames += bp_num_frames(b.ingest[i].n_out);
+  }
+  if (h_sample_off) std::copy(b.rel.begin(), b.rel.end(), h_sample_off);
+  DeviceGuard g(m->device);
+  return evaluate_batch(m, b, req, Rows{h_note, h_onset, h_contour}, h_frame_off);
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,

@@ -736,6 +736,193 @@ class Model:
                                        _ptr(counts))
         return counts
 
+    # ------------------------------------------------------------------ every family in one pass
+    EVAL_FAMILIES = ("notes", "onset_offset", "pairs", "frames", "bent_frames", "note_melody", "flat_note_melody",
+                     "salience", "melody")
+
+    def _eval_request(self, n_files: int, families: Sequence[str], settings: Sequence[Dict[str, Any]] = (),
+                      note_refs=None, multipitch_refs=None, f0_refs=None, salience: Optional[Dict[str, Any]] = None,
+                      melody: Optional[Dict[str, Any]] = None, window: float = evaluate.WINDOW,
+                      cent_tolerance: float = evaluate.CENT_TOLERANCE, **tolerances):
+        """The bp_eval_request_t of `evaluate` -> (request, the arrays it points at, {family: counts array}); the pairs'
+        notes (`pair_notes`) are set per attempt by the caller.  Inputs as the standalone `score_*` / `match_grid`
+        calls take them; salience / melody are dicts {settings, references, kind="contour"}."""
+        unknown = set(families) - set(self.EVAL_FAMILIES)
+        if unknown:
+            raise ValueError(f"unknown famil(ies) {sorted(unknown)}; choose from {self.EVAL_FAMILIES}")
+        r, keep, out = _lib.EvalRequest(), [], {}
+        n_params = len(settings)
+
+        def need(refs, what):
+            if refs is None:
+                raise ValueError(f"{what} references are required")
+            if len(refs) != n_files:
+                raise ValueError(f"{n_files} files but {len(refs)} {what} references")
+
+        def counts(name, n, width):
+            out[name] = np.zeros((n, n_files, width), np.int64)
+            return _ptr(out[name])
+
+        if {"notes", "onset_offset", "pairs", "frames", "bent_frames", "note_melody", "flat_note_melody"} & set(families):
+            ps = self._grid_params(settings)
+            r.params, r.n_params = C.addressof(ps), n_params
+            keep.append(ps)
+        if {"notes", "onset_offset", "pairs"} & set(families):
+            need(note_refs, "note")
+            sp = self._score_params(tolerances)
+            pitched = [(ref[0], ref[1]) for ref in note_refs]
+            ns, arrs = self._note_set(pitched, "references")
+            keep += [sp, ns, arrs]
+            r.note_refs, r.score, r.est_log2_hz = C.addressof(ns), C.addressof(sp), _ptr(evaluate.EST_LOG2_HZ)
+            if "notes" in families:
+                r.notes_counts = counts("notes", n_params, 4)
+            if "onset_offset" in families:
+                r.onset_offset_counts = counts("onset_offset", n_params, 4)
+            if "pairs" in families:
+                roff = arrs[0]
+                h_match = np.full((max(n_params, 1), 2, max(int(roff[-1]), 1)), -1, np.int32)
+                out["pairs"] = (h_match, roff)
+                r.pair_match = _ptr(h_match)
+        elif tolerances:
+            self._score_params(tolerances)
+        if {"frames", "bent_frames"} & set(families):
+            need(multipitch_refs, "multi-pitch")
+            ms, arrs = self._multipitch_set(multipitch_refs, "references")
+            keep += [ms, arrs]
+            r.mp_refs, r.window = C.addressof(ms), float(window)
+            if "frames" in families:
+                r.est_midi, r.est_chroma = _ptr(evaluate.EST_MIDI), _ptr(evaluate.EST_CHROMA)
+                r.frames_counts = counts("frames", n_params, 7)
+            if "bent_frames" in families:
+                _, midi, chroma, _ = evaluate.bent_bins()
+                keep += [midi, chroma]
+                r.bin_midi, r.bin_chroma = _ptr(midi), _ptr(chroma)
+                r.bent_frames_counts = counts("bent_frames", n_params, 7)
+        if {"note_melody", "flat_note_melody"} & set(families):
+            need(f0_refs, "f0")
+            ms, arrs = self._melody_set(f0_refs, "references")
+            cents = evaluate.bent_bins()[3]
+            keep += [ms, arrs, cents]
+            r.f0_refs, r.cent_tolerance, r.bin_cent = C.addressof(ms), float(cent_tolerance), _ptr(cents)
+            if "note_melody" in families:
+                r.note_melody_counts = counts("note_melody", n_params, 7)
+            if "flat_note_melody" in families:
+                r.flat_note_melody_counts = counts("flat_note_melody", n_params, 7)
+        for name, spec in (("salience", salience), ("melody", melody)):
+            if name not in families:
+                continue
+            if spec is None or "settings" not in spec:
+                raise ValueError(f"{name} needs a dict with its settings and references")
+            kind = spec.get("kind", "contour")
+            if kind not in ("contour", "note"):
+                raise ValueError(f"{name}: kind must be 'contour' or 'note', got {kind!r}")
+            need(spec.get("references"), name)
+            sets = spec["settings"]
+            if name == "salience":
+                ps = self._salience_params(sets, kind)
+                ms, arrs = self._multipitch_set(spec["references"], "references")
+                _, midi, chroma = evaluate.salience_bins(kind)
+                keep += [ps, ms, arrs, midi, chroma]
+                r.salience_params, r.n_salience, r.salience_gram = C.addressof(ps), len(sets), int(kind == "note")
+                r.salience_refs, r.salience_window = C.addressof(ms), float(window)
+                r.salience_midi, r.salience_chroma = _ptr(midi), _ptr(chroma)
+                r.salience_counts = counts("salience", len(sets), 7)
+            else:
+                ps = self._melody_params(sets, kind)
+                ms, arrs = self._melody_set(spec["references"], "references")
+                cents = evaluate.melody_bins(kind)[1]
+                keep += [ps, ms, arrs, cents]
+                r.melody_params, r.n_melody, r.melody_gram = C.addressof(ps), len(sets), int(kind == "note")
+                r.melody_refs, r.melody_tolerance, r.melody_cent = C.addressof(ms), float(cent_tolerance), _ptr(cents)
+                r.melody_counts = counts("melody", len(sets), 7)
+        return r, keep, out
+
+    def evaluate(self, families: Sequence[str], settings: Sequence[Dict[str, Any]] = (), *, grams=None, audio=None,
+                 pcm=None, return_model_output: bool = False, stream: int = 0, **request) -> Dict[str, Any]:
+        """Every requested metric family of a batch in ONE library call (`bp_evaluate_*`): the batch is decoded once per
+        chunk of settings and every note-derived family scores that decode; the posteriorgram families read the
+        posteriorgrams where they are.  Exactly one input:
+          grams  (notes, onsets, contours) lists of per-file host arrays (contours may be None when no family reads
+                 them), or (note, onset, contour, frame_off) with device tensors (anything with data_ptr(); row-major,
+                 work on `stream`) -> bp_evaluate_host / bp_evaluate_device;
+          audio  mono 22 050 Hz float32 arrays -> bp_evaluate_audio_host (the model runs once);
+          pcm    (samples, sample_rate) items as `transcribe_pcm` takes them -> bp_evaluate_pcm_files_host.
+        families: names from EVAL_FAMILIES; settings: the decode grid of the note-derived families (as `score_grid`);
+        request: note_refs, multipitch_refs, f0_refs, salience / melody dicts {settings, references, kind}, window,
+        cent_tolerance and note tolerances, as the standalone calls take them.
+        Returns {family: int64 counts} as the standalone `score_*` calls return them, "pairs" as `match_grid`'s (res,
+        match), and with return_model_output (audio / pcm) "model_output": per-file posteriorgram dicts."""
+        if sum(x is not None for x in (grams, audio, pcm)) != 1:
+            raise ValueError("give exactly one of grams, audio, pcm")
+        device = grams is not None and hasattr(grams[0], "data_ptr")
+        if device:
+            note, onset, contour, foff = grams
+            foff = np.ascontiguousarray(foff, np.int64)
+            n_files = len(foff) - 1
+        elif grams is not None:
+            notes, onsets, contours = grams
+            n_files = len(notes)
+            foff, n_all, o_all = self._cat_note_onset(notes, onsets)
+            c_all = None if contours is None else _cat_rows(list(contours), N_FREQ_BINS_CONTOURS)
+            if c_all is not None and c_all.shape[0] != foff[-1]:
+                raise ValueError("contour posteriorgrams must have as many frames as note posteriorgrams")
+        elif audio is not None:
+            flat, offs = self._pack_audio(audio)
+            n_files = len(audio)
+            lens = np.diff(offs)
+        else:
+            files, keep_pcm = pcm_descriptors(pcm)
+            n_files = len(keep_pcm)
+            lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in files[:n_files]),
+                               dtype=np.int64, count=n_files)
+        req, keep, out = self._eval_request(n_files, families, settings, **request)
+        n_params = len(settings)
+        mo = {}
+        if grams is None:
+            foff = np.zeros(n_files + 1, np.int64)
+            total = int(sum(self._lib.bp_num_frames(int(n)) for n in lens))
+            if return_model_output:
+                mo = {k: np.empty((total, w), _F32) for k, w in (("note", N_FREQ_BINS_NOTES), ("onset", N_FREQ_BINS_NOTES),
+                                                                 ("contour", N_FREQ_BINS_CONTOURS))}
+
+        def call(notes=None):
+            req.pair_notes = C.addressof(notes) if notes is not None else None
+            if device:
+                self._lib.bp_evaluate_device(self._h, note.data_ptr(), onset.data_ptr(),
+                                             None if contour is None else contour.data_ptr(), _ptr(foff), n_files,
+                                             C.byref(req), stream or None)
+            elif grams is not None:
+                self._lib.bp_evaluate_host(self._h, _ptr(n_all), _ptr(o_all), _ptr(c_all), _ptr(foff), n_files, C.byref(req))
+            elif audio is not None:
+                self._lib.bp_evaluate_audio_host(self._h, _ptr(flat), _ptr(offs), n_files, C.byref(req), _ptr(mo.get("note")),
+                                                 _ptr(mo.get("onset")), _ptr(mo.get("contour")), _ptr(foff))
+            else:
+                self._lib.bp_evaluate_pcm_files_host(self._h, files, n_files, C.byref(req), _ptr(mo.get("note")),
+                                                     _ptr(mo.get("onset")), _ptr(mo.get("contour")), _ptr(foff), None)
+
+        if "pairs" in families:
+            total = int(foff[-1]) if grams is not None else total
+            arrs = self._with_capacity(n_files, total, call, n_params=n_params)
+            flat_res = self._split_notes(arrs, n_params * n_files)
+            h_match, roff = out["pairs"]
+            out["pairs"] = ([flat_res[k * n_files : (k + 1) * n_files] for k in range(n_params)],
+                            [[h_match[k, :, roff[i] : roff[i + 1]].copy() for i in range(n_files)] for k in range(n_params)])
+        else:
+            call()
+        if grams is None:
+            out["frame_off"] = foff
+            if return_model_output:
+                fo = foff.tolist()
+                out["model_output"] = [{k: v[a:b] for k, v in mo.items()} for a, b in zip(fo[:-1], fo[1:])]
+        return out
+
+    def evaluate_chunk_params(self, total_frames: int, families: Sequence[str], settings: Sequence[Dict[str, Any]] = (),
+                              **request) -> int:
+        """`bp_evaluate_chunk_params`: settings per decode chunk of `evaluate` over a batch of this many frames."""
+        n_files = max(len(request.get(k) or ()) for k in ("note_refs", "multipitch_refs", "f0_refs"))
+        req, keep, _ = self._eval_request(n_files, families, settings, **request)
+        return int(self._lib.bp_evaluate_chunk_params(int(total_frames), n_files, C.byref(req)))
+
     def infer_onsets_array(self, onsets: np.ndarray, frames: np.ndarray) -> np.ndarray:
         """reference: note_creation.py:289-311 `get_infered_onsets` (n_diff = 2) -> float64 (T, 88), on the device."""
         o = np.ascontiguousarray(onsets, dtype=_F32)
@@ -1094,11 +1281,11 @@ def _model_and_clips(audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
     return model, clips
 
 
-def _match_counts(outs, ref_ivs, res, match):
-    """Of `Model.match_grid`'s (res, match) on the model outputs `outs`: the estimated intervals in seconds
+def _match_counts(n_frames, ref_ivs, res, match):
+    """Of `Model.match_grid`'s (res, match) on files of n_frames model frames: the estimated intervals in seconds
     [setting][file], and counts (n_settings, n_files, 4) = n_ref, n_est, matched without offsets, matched."""
-    times = [infer.model_frames_to_time(o["note"].shape[0] + 1) for o in outs]
-    counts = np.zeros((len(res), len(outs), 4), np.int64)
+    times = [infer.model_frames_to_time(t + 1) for t in n_frames]
+    counts = np.zeros((len(res), len(n_frames), 4), np.int64)
     est_ivs = []
     for k, per in enumerate(res):
         est_ivs.append([np.stack([times[i][r["start"]], times[i][r["end"]]], 1) for i, r in enumerate(per)])
@@ -1170,6 +1357,17 @@ def evaluate_velocity_grid(
     Returns (counts (n_settings, n_files, 4) as `evaluate_grid`, derived from the matchings; scores), scores holding
     `evaluate.note_scores(counts)` and every key of `evaluate.matching_scores` as (n_settings, n_files) float64 arrays,
     with "mean" over files as in `note_scores`."""
+    refs = _velocity_references(references)
+    model, clips = _model_and_clips(audio, model_or_model_path)
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
+    outs = model.run_inference_arrays(clips)
+    res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode,
+                                  [(iv, hz) for iv, hz, _ in refs], **tolerances)
+    return _velocity_scores([o["note"].shape[0] for o in outs], refs, res, match, velocity_tolerance)
+
+
+def _velocity_references(references):
+    """evaluate_velocity_grid's references, checked: [(intervals, pitches_hz, velocities)]."""
     refs = []
     for i, ref in enumerate(references):
         if len(ref) != 3:
@@ -1179,14 +1377,14 @@ def evaluate_velocity_grid(
         if len(vel) != len(np.asarray(hz).reshape(-1)):
             raise ValueError(f"references[{i}]: {len(vel)} velocities for {len(np.asarray(hz).reshape(-1))} notes")
         refs.append((iv, hz, vel))
-    model, clips = _model_and_clips(audio, model_or_model_path)
-    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]
-    outs = model.run_inference_arrays(clips)
-    res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode,
-                                  [(iv, hz) for iv, hz, _ in refs], **tolerances)
-    n_params, n_files = len(settings), len(clips)
+    return refs
+
+
+def _velocity_scores(n_frames, refs, res, match, velocity_tolerance):
+    """evaluate_velocity_grid's return value from the pairs of files of n_frames model frames."""
+    n_params, n_files = len(res), len(n_frames)
     ref_ivs = [np.asarray(iv, np.float64).reshape(-1, 2) for iv, _, _ in refs]
-    est_ivs, counts = _match_counts(outs, ref_ivs, res, match)
+    est_ivs, counts = _match_counts(n_frames, ref_ivs, res, match)
     keys = [k + s for s in ("", "_no_offset") for k in evaluate.MATCH_FIELDS]
     extra = {k: np.zeros((n_params, n_files)) for k in keys}
     for k in range(n_params):
@@ -1223,9 +1421,19 @@ def evaluate_transcription_grid(
     outs = model.run_inference_arrays(clips)
     res, match = model.match_grid([o["note"] for o in outs], [o["onset"] for o in outs], decode, references,
                                   **tolerances)
-    n_params, n_files = len(settings), len(clips)
+    n_frames = [o["note"].shape[0] for o in outs]
     ref_ivs = [np.asarray(iv, np.float64).reshape(-1, 2) for iv, _ in references]
-    est_ivs, counts = _match_counts(outs, ref_ivs, res, match)
+    est_ivs, _ = _match_counts(n_frames, ref_ivs, res, match)
+    ests = [iv for per in est_ivs for iv in per]
+    onoff = model.score_onsets_offsets(ests, ref_ivs * len(res), **tolerances).reshape(len(res), len(outs), 4)
+    return _transcription_scores(n_frames, ref_ivs, res, match, onoff)
+
+
+def _transcription_scores(n_frames, ref_ivs, res, match, onoff):
+    """evaluate_transcription_grid's return value from the pairs and the onset / offset counts of files of n_frames
+    model frames."""
+    n_params, n_files = len(res), len(n_frames)
+    est_ivs, counts = _match_counts(n_frames, ref_ivs, res, match)
     overlap = {k: np.zeros((n_params, n_files)) for k in ("average_overlap_ratio", "average_overlap_ratio_no_offset")}
     for k in range(n_params):
         for i in range(n_files):
@@ -1234,8 +1442,6 @@ def evaluate_transcription_grid(
                 ref_idx = np.flatnonzero(row >= 0)  # sorted(matching.items()): ascending reference index
                 overlap["average_overlap_ratio" + suffix][k, i] = evaluate._overlap_ratio(ref_ivs[i], est_ivs[k][i],
                                                                                            ref_idx, row[ref_idx])
-    ests = [iv for per in est_ivs for iv in per]
-    onoff = model.score_onsets_offsets(ests, ref_ivs * n_params, **tolerances).reshape(n_params, n_files, 4)
     scores = evaluate.note_scores(counts)
     counts = np.concatenate([counts, onoff[..., 2:]], axis=-1)
     scores.update(overlap)
@@ -1345,6 +1551,105 @@ def evaluate_note_melody_grid(
                                           [o["contour"] for o in outs] if pitch_bends else None, decode, references,
                                           cent_tolerance=cent_tolerance)
     return counts, evaluate.melody_scores(counts)
+
+
+EVALUATE_FAMILIES = ("notes", "transcription", "velocity", "frames", "bent_frames", "note_melody", "flat_note_melody",
+                     "salience", "melody")
+
+
+def evaluate_all(
+    audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
+    settings: Sequence[Dict[str, Any]],
+    notes: Optional[Sequence[Tuple[np.ndarray, ...]]] = None,
+    multipitch: Optional[Sequence[Tuple[np.ndarray, Sequence[np.ndarray]]]] = None,
+    f0: Optional[Sequence[Tuple[np.ndarray, np.ndarray]]] = None,
+    salience: Optional[Dict[str, Any]] = None,
+    melody: Optional[Dict[str, Any]] = None,
+    families: Optional[Sequence[str]] = None,
+    return_model_output: bool = False,
+    model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+    window: float = evaluate.WINDOW,
+    cent_tolerance: float = evaluate.CENT_TOLERANCE,
+    velocity_tolerance: float = 0.1,
+    **tolerances,
+):
+    """Several metric families of a batch of annotated recordings under one grid of settings, in one device pass
+    (addition; no reference counterpart): the batch is ingested and run through the model once, its posteriorgrams stay
+    on the device, each chunk of settings is decoded once and every note-derived family scores that decode
+    (`Model.evaluate`, `bp_evaluate_*`).  Items follow `predict_batch`: with any path the batch goes through the
+    stored-PCM pipeline, otherwise the packed arrays.
+
+    A family stands for one existing call, and its value equals that call's return value bit for bit:
+      notes            evaluate_grid(audio, notes, settings)
+      transcription    evaluate_transcription_grid(audio, notes, settings)
+      velocity         evaluate_velocity_grid(audio, notes, settings, velocity_tolerance=...); notes with velocities
+      frames           evaluate_frames_grid(audio, multipitch, settings, pitch_bends=False)
+      bent_frames      evaluate_frames_grid(audio, multipitch, settings, pitch_bends=True)
+      note_melody      evaluate_note_melody_grid(audio, f0, settings, pitch_bends=True)
+      flat_note_melody evaluate_note_melody_grid(audio, f0, settings, pitch_bends=False)
+      salience         evaluate_salience_grid(audio, refs, salience["settings"], kind=salience.get("kind", "contour"))
+      melody           evaluate_melody_grid(audio, refs, melody["settings"], kind=melody.get("kind", "contour"))
+    with the tolerances given here (window, cent_tolerance, note tolerances as `evaluate.TOLERANCES`).  salience /
+    melody are dicts {settings, kind="contour", references}; their references default to `multipitch` / `f0`.
+    families=None selects every family whose references are given (velocity when the note references carry
+    velocities).  Returns {family: (counts, scores)}, plus "model_output" (per-file posteriorgram dicts) when asked."""
+    salience = None if salience is None else {"references": multipitch, **salience}
+    melody = None if melody is None else {"references": f0, **melody}
+    if families is None:
+        families = [f for f, given in (
+            ("notes", notes), ("transcription", notes), ("velocity", notes and all(len(r) == 3 for r in notes)),
+            ("frames", multipitch), ("bent_frames", multipitch), ("note_melody", f0), ("flat_note_melody", f0),
+            ("salience", salience and salience.get("references")), ("melody", melody and melody.get("references")),
+        ) if given is not None and given is not False]  # fmt: skip
+    unknown = set(families) - set(EVALUATE_FAMILIES)
+    if unknown:
+        raise ValueError(f"unknown famil(ies) {sorted(unknown)}; choose from {EVALUATE_FAMILIES}")
+    fam = set(families)
+    refs = _velocity_references(notes) if "velocity" in fam else None
+    lib_fams = [f for f in ("notes", "frames", "bent_frames", "note_melody", "flat_note_melody", "salience", "melody")
+                if f in fam]
+    if "transcription" in fam:
+        lib_fams.append("onset_offset")
+    if fam & {"transcription", "velocity"}:
+        lib_fams.append("pairs")
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    decode = [infer.grid_setting(s, predict_names=True)[0] for s in settings]  # include_pitch_bends: predict's True
+    request = dict(note_refs=notes, multipitch_refs=multipitch, f0_refs=f0, salience=salience, melody=melody,
+                   window=window, cent_tolerance=cent_tolerance, **tolerances)
+    if all(isinstance(a, np.ndarray) for a in audio):
+        for a in audio:
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+        out = model.evaluate(lib_fams, decode, audio=[np.ascontiguousarray(a, dtype=_F32) for a in audio],
+                             return_model_output=return_model_output, **request)
+    else:
+        items = []
+        for a in audio:
+            if isinstance(a, np.ndarray):
+                if a.ndim != 1:
+                    raise ValueError("audio must be mono (1-D)")
+                items.append((np.ascontiguousarray(a, dtype=_F32), AUDIO_SAMPLE_RATE))
+            else:
+                items.append(read_pcm(a))
+        out = model.evaluate(lib_fams, decode, pcm=items, return_model_output=return_model_output, **request)
+    n_frames = np.diff(out["frame_off"]).tolist()
+    result: Dict[str, Any] = {}
+    if "notes" in fam:
+        result["notes"] = (out["notes"], evaluate.note_scores(out["notes"]))
+    if "transcription" in fam:
+        ref_ivs = [np.asarray(r[0], np.float64).reshape(-1, 2) for r in notes]
+        result["transcription"] = _transcription_scores(n_frames, ref_ivs, *out["pairs"], out["onset_offset"])
+    if "velocity" in fam:
+        result["velocity"] = _velocity_scores(n_frames, refs, *out["pairs"], velocity_tolerance)
+    for f in ("frames", "bent_frames", "salience"):
+        if f in fam:
+            result[f] = (out[f], evaluate.frame_scores(out[f]))
+    for f in ("note_melody", "flat_note_melody", "melody"):
+        if f in fam:
+            result[f] = (out[f], evaluate.melody_scores(out[f]))
+    if return_model_output:
+        result["model_output"] = out["model_output"]
+    return result
 
 
 def predict_batch(

@@ -577,6 +577,102 @@ int bp_score_note_melody_grid_host(bp_model_t* m, const float* h_note, const flo
  * and held cents of a chunk of c settings stay within 2 GiB, c = max(1, 2^31 / max(1, 16 total_frames)). */
 int64_t bp_score_melody_chunk_params(int64_t total_frames);
 
+/* ---- every metric family of a batch under a settings grid, in one device pass --------------------------------------
+ * No reference counterpart.  One request asks for any subset of the grid scorers above over the same batch; each
+ * family's outputs are bit for bit those of its standalone call on the same posteriorgrams.  A family is requested when
+ * its output pointer is non-NULL; its inputs are then those of its standalone entry point:
+ *   notes            notes_counts [n_params][n_files][4]          bp_score_grid_*              (note_refs, score, est_log2_hz)
+ *   onset_offset     onset_offset_counts [n_params][n_files][4]   bp_score_onset_offset_grid_* (note_refs, score)
+ *   pairs            pair_notes + pair_match [n_params][2][R]     bp_match_grid_*              (note_refs, score, est_log2_hz)
+ *   frames           frames_counts [n_params][n_files][7]         bp_score_frames_grid_*       (mp_refs, window, est_midi/chroma)
+ *   bent_frames      bent_frames_counts [n_params][n_files][7]    bp_score_bent_frames_grid_*  (mp_refs, window, bin_midi/chroma)
+ *   note_melody      note_melody_counts [n_params][n_files][7]    bp_score_note_melody_grid_*  (f0_refs, cent_tolerance, bin_cent)
+ *   flat_note_melody flat_note_melody_counts, the same with every setting's include_pitch_bends taken as 0
+ *   salience         salience_counts [n_salience][n_files][7]     bp_score_salience_grid_*     (own settings and references)
+ *   melody           melody_counts [n_melody][n_files][7]         bp_score_melody_grid_*       (own settings and references)
+ * The first seven are note-derived: they share params[0 .. n_params).  salience_gram / melody_gram pick the posteriorgram
+ * the last two read: 0 the contour (264 bins), 1 the note posteriorgram (88 bins).
+ * Order of work: every requested family is validated, with its standalone checks and messages prefixed by its name
+ * ("bp_evaluate_host: frames: references file 3 frame 17 value 2: chroma outside [0, 12)"), before anything is
+ * enqueued; each family's references are uploaded once.  Then one grid-decode chunk loop (chunk size
+ * bp_evaluate_chunk_params) runs the decode once per chunk and, on that chunk's notes, the tail of every requested
+ * note-derived family in the order of the table, each with the launches and workspace of its standalone tail.  Then
+ * the salience and melody chunk loops run on the posteriorgrams as they are.  All counts come back in one copy, with one
+ * synchronisation; the pairs' notes come back per chunk, as in bp_match_grid_* (BP_E_CAPACITY and bp_last_required as
+ * there, after every family has run).
+ * Kernel launches per decode chunk: those of the grid decode (3, or 1 when every file is empty; doubled when the chunk
+ * reruns) + 1 (notes) + 1 (onset_offset) + bp_match_grid_*'s tail (pairs) + 3 (frames) + 3 (bent_frames) + 4
+ * (note_melody) + 4 (flat_note_melody), for the requested families; k note-derived families thus save (k - 1) times the
+ * decode's launches against k standalone calls.  Per salience chunk (bp_score_salience_chunk_params) 1 launch, per
+ * melody chunk (bp_score_melody_chunk_params) 3.
+ * n_files == 0 or no family requested: BP_OK, nothing enqueued.
+ * _device: posteriorgrams (row-major, the layout of bp_run_inference_*) in device memory, work on `stream`, synchronised
+ * before returning; _host: host posteriorgrams, uploaded once (the contour only when a family reads it). */
+typedef struct bp_eval_request {
+  const bp_decode_params_t* params; /* the grid of every note-derived family */
+  int32_t n_params;
+  int32_t reserved0;
+  const bp_note_set_t* note_refs; /* one set per file */
+  const bp_score_params_t* score;
+  const double* est_log2_hz; /* [128] */
+  int64_t* notes_counts;
+  int64_t* onset_offset_counts;
+  bp_notes_t* pair_notes; /* pairs: both non-NULL */
+  int32_t* pair_match;
+  const bp_multipitch_set_t* mp_refs; /* one series per file */
+  double window;
+  const double* est_midi, *est_chroma; /* [128] */
+  int64_t* frames_counts;
+  const double* bin_midi, *bin_chroma; /* [264] */
+  int64_t* bent_frames_counts;
+  const bp_melody_set_t* f0_refs; /* one track per file */
+  double cent_tolerance;
+  const double* bin_cent; /* [264] */
+  int64_t* note_melody_counts;
+  int64_t* flat_note_melody_counts;
+  const bp_salience_params_t* salience_params;
+  int32_t n_salience;
+  int32_t salience_gram;
+  const bp_multipitch_set_t* salience_refs;
+  double salience_window;
+  const double* salience_midi, *salience_chroma; /* [width] */
+  int64_t* salience_counts;
+  const bp_melody_params_t* melody_params;
+  int32_t n_melody;
+  int32_t melody_gram;
+  const bp_melody_set_t* melody_refs;
+  double melody_tolerance;
+  const double* melody_cent; /* [width] */
+  int64_t* melody_counts;
+} bp_eval_request_t;
+typedef struct bp_pcm_file bp_pcm_file_t; /* stored PCM of one file, defined below */
+int bp_evaluate_device(bp_model_t* m, const float* d_note, const float* d_onset, const float* d_contour,
+                       const int64_t* h_frame_off, int32_t n_files, const bp_eval_request_t* req, void* stream);
+int bp_evaluate_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
+                     const int64_t* h_frame_off, int32_t n_files, const bp_eval_request_t* req);
+/* The model's output and the evaluation of a batch in one call: the input of bp_run_inference_host (packed float32
+ * audio) or of bp_transcribe_pcm_files_host (stored PCM).  The batch runs through the whole-file pipeline without a
+ * decode; its posteriorgrams stay in the model's staging, where the request is scored as by bp_evaluate_device.
+ * h_frame_off [n_files + 1] is always written; h_note / h_onset / h_contour (row-major, may be NULL) receive the
+ * posteriorgrams, h_sample_off (PCM, may be NULL) the resampled lengths as offsets.  The request is validated against
+ * the batch's frame offsets before any upload or launch.  Synchronous. */
+int bp_evaluate_audio_host(bp_model_t* m, const float* h_audio, const int64_t* h_sample_off, int32_t n_files,
+                           const bp_eval_request_t* req, float* h_note, float* h_onset, float* h_contour,
+                           int64_t* h_frame_off);
+int bp_evaluate_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, const bp_eval_request_t* req,
+                               float* h_note, float* h_onset, float* h_contour, int64_t* h_frame_off,
+                               int64_t* h_sample_off);
+/* Host-only: settings per decode chunk of bp_evaluate_* over a batch of this shape (>= 1): a chunk of c settings keeps
+ * c * (W + X) <= 2^31 bytes unless c = 1, capped at 65535, where W is the grid decode's per-setting workspace
+ * (bp_decode_grid_chunk_params) and X sums, over the requested note-derived families, with F = total_frames,
+ * S = min(88 F, 8 F + 64 n_files) (a setting's first allowance of note slots), R the reference notes, K the reference
+ * frames and V the reference values of mp_refs:
+ *   notes 8 R + 16 S;  onset_offset 24 R + 16 S + 8 n_files;  pairs 8 R + 28 S;
+ *   frames 16 V + 8 K;  bent_frames 16 V + 8 K + 4;  note_melody and / or flat_note_melody 16 F (shared).
+ * The matching of pairs runs in its own launches of at most 2 GiB (bp_match_grid_*); salience and melody run their
+ * own chunks. */
+int64_t bp_evaluate_chunk_params(int64_t total_frames, int32_t n_files, const bp_eval_request_t* req);
+
 /* ---- the whole path: predict() for a batch of files -------------------------------------------
  * reference: predict (basic_pitch/inference.py:431-506) minus file I/O and the MIDI object:
  * run_inference + model_output_to_notes.  Posteriorgram outputs are optional (pass NULL to keep
