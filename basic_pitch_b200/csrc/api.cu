@@ -4045,3 +4045,342 @@ int bp_debug_frontend(bp_model_t* m, int which, void* h_out, int64_t n_windows) 
 }
 
 }  // extern "C"
+
+// ---- note stream (bp_stream_*) --------------------------------------------------------------------------------------
+// Frames arrive row-major and stay in the held buffers (rows 0 .. n - hb) until the segment that needs them is decoded.
+// Stream frame indices are global (0 = first frame pushed); row = frame - hb.
+struct bp_stream {
+  bp_model* m = nullptr;
+  bp_decode_params_t params{};
+  DecodeParamsDev dp{};
+  long long la = 0, w = 0, after = 0, max_seg = 0;
+  DevBuf<float> note[2], onset[2], contour[2];
+  DevBuf<unsigned char> quiet[2];
+  int cur = 0;                    // which of the two held buffers is live (the other receives the next move)
+  long long hb = 0, n = 0;        // global frame of held row 0; frames pushed so far
+  long long r = 0, a = 0;         // start of the recording or forced part; start of the open segment
+  long long last = -1;            // the frame before the cut-eligible quiet run in progress (kStreamNoRun: none)
+  long long scan_from = 0;        // first frame the cut search has not passed
+  bool ended = false;
+  DevBuf<unsigned int> max_onset, done;
+  DevBuf<unsigned long long> max_fd;
+  DevBuf<long long> scan_out;
+  DevBuf<int> kept;
+  std::vector<int32_t> q_start, q_end, q_pitch, q_bends;  // finished notes not yet taken
+  std::vector<float> q_amp;
+  std::vector<int32_t> q_bend_off{0};
+
+  long long seg_begin(long long at) const { return at == r ? at : at - kStreamCtxBefore; }
+  void release() {
+    for (int k = 0; k < 2; ++k) {
+      note[k].release();
+      onset[k].release();
+      contour[k].release();
+      quiet[k].release();
+    }
+    max_onset.release();
+    done.release();
+    max_fd.release();
+    scan_out.release();
+    kept.release();
+  }
+};
+
+namespace {
+
+// Moves held rows [from - hb, n - hb) to row 0 of the other buffer set, grown to hold `cap` rows, and makes it live.
+int stream_move(bp_stream* s, long long from, long long cap, cudaStream_t st) {
+  const int nx = s->cur ^ 1;
+  CK(s->note[nx].reserve((size_t)cap * kPitches));
+  CK(s->onset[nx].reserve((size_t)cap * kPitches));
+  if (s->params.include_pitch_bends) CK(s->contour[nx].reserve((size_t)cap * kContourBins));
+  CK(s->quiet[nx].reserve((size_t)cap));
+  const long long rows = s->n - from, row0 = from - s->hb;
+  if (rows > 0) {
+    const int c = s->cur;
+    CK(cudaMemcpyAsync(s->note[nx].p, s->note[c].p + row0 * kPitches, sizeof(float) * rows * kPitches,
+                       cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(s->onset[nx].p, s->onset[c].p + row0 * kPitches, sizeof(float) * rows * kPitches,
+                       cudaMemcpyDeviceToDevice, st));
+    if (s->params.include_pitch_bends)
+      CK(cudaMemcpyAsync(s->contour[nx].p, s->contour[c].p + row0 * kContourBins, sizeof(float) * rows * kContourBins,
+                         cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(s->quiet[nx].p, s->quiet[c].p + row0, rows, cudaMemcpyDeviceToDevice, st));
+  }
+  s->cur = nx;
+  s->hb = from;
+  return BP_OK;
+}
+
+// Decodes frames [ds, de) as one file with the stream's running maxima and queues its notes that start in [a, b).
+int stream_decode(bp_stream* s, long long a, long long b, long long ds, long long de, cudaStream_t st) {
+  bp_model* m = s->m;
+  const std::string api = "bp_stream";
+  const long long T = de - ds;
+  if (T <= 0 || b <= a) return BP_OK;
+  if (de > INT_MAX) return fail(BP_E_INVALID, api + ": the stream is longer than 2^31 - 1 frames");
+  const int c = s->cur;
+  const long long row0 = ds - s->hb;
+  const float* note = s->note[c].p;
+  const float* onset = s->onset[c].p;
+  const float* contour = s->contour[c].p;
+  int count = 0;
+  for (int attempt = 0; attempt < 2; ++attempt) {
+    const long long foff[2] = {0, T};
+    const long long soff[2] = {0, attempt == 0 ? std::min<long long>(T * kPitches, 8 * T + 64) : T * kPitches};
+    CK(m->d_frame_off.reserve(2));
+    CK(m->d_slot_off.reserve(2));
+    CK(m->energy.reserve((size_t)T * kPitches + 1));
+    CK(m->candbits.reserve((size_t)decode_cand_words(T)));
+    CK(m->blk_max.reserve((size_t)kPitches * decode_block_slots(T, 1)));
+    CK(m->blk_arg.reserve((size_t)kPitches * decode_block_slots(T, 1)));
+    CK(m->note_count.reserve(1));
+    CK(m->overflow.reserve(1));
+    CK(m->slot_start.reserve((size_t)soff[1] + 1));
+    CK(m->slot_end.reserve((size_t)soff[1] + 1));
+    CK(m->slot_pitch.reserve((size_t)soff[1] + 1));
+    CK(cudaMemcpyAsync(m->d_frame_off.p, foff, sizeof(foff), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m->d_slot_off.p, soff, sizeof(soff), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(m->overflow.p, 0, sizeof(int), st));
+    DecodeBuffers bufs;
+    bufs.frame_off = m->d_frame_off.p;
+    bufs.energy = m->energy.p;
+    bufs.candbits = m->candbits.p;
+    bufs.max_onset = s->max_onset.p;
+    bufs.max_fd = s->max_fd.p;
+    bufs.slot_off = m->d_slot_off.p;
+    bufs.note_count = m->note_count.p;
+    bufs.note_start = m->slot_start.p;
+    bufs.note_end = m->slot_end.p;
+    bufs.note_pitch = m->slot_pitch.p;
+    bufs.overflow = m->overflow.p;
+    bufs.blk_max = m->blk_max.p;
+    bufs.blk_arg = m->blk_arg.p;
+    launch_decode_kernels(note + row0 * kPitches, onset + row0 * kPitches, bufs, 1, T, s->dp, st);
+    CKL();
+    m->launches += 3;
+    int overflow = 0;
+    CK(cudaMemcpyAsync(&count, m->note_count.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&overflow, m->overflow.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (!overflow) break;
+    if (attempt == 1) return fail(BP_E_CUDA, api + ": note slots overflowed at full capacity (internal error)");
+  }
+  if (count == 0) return BP_OK;
+  CK(m->d_start.reserve(count));
+  CK(m->d_end.reserve(count));
+  CK(m->d_pitch.reserve(count));
+  CK(m->d_amp.reserve(count));
+  CK(m->d_note_base.reserve(count));
+  CK(m->d_bend_off.reserve(count + 1));
+  launch_stream_compact(m->note_count.p, m->slot_start.p, m->slot_end.p, m->slot_pitch.p, (int)(a - ds), (int)(b - ds),
+                        (int)ds, -s->hb, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_note_base.p, s->kept.p, st);
+  CKL();
+  m->launches += 1;
+  int kept = 0;
+  CK(cudaMemcpyAsync(&kept, s->kept.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (kept == 0) return BP_OK;
+  const size_t q0 = s->q_start.size();
+  s->q_start.resize(q0 + kept);
+  s->q_end.resize(q0 + kept);
+  s->q_pitch.resize(q0 + kept);
+  s->q_amp.resize(q0 + kept);
+  CK(cudaMemcpyAsync(s->q_start.data() + q0, m->d_start.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(s->q_end.data() + q0, m->d_end.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(s->q_pitch.data() + q0, m->d_pitch.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int with_bends = s->params.include_pitch_bends ? 1 : 0;
+  std::vector<int32_t> boff(kept + 1, 0);
+  for (int j = 0; j < kept; ++j) {
+    const long long nb = boff[j] + (with_bends ? (long long)s->q_end[q0 + j] - s->q_start[q0 + j] : 0);
+    if (nb > 0x7fffffffLL) return fail(BP_E_CAPACITY, api + ": more than 2^31 pitch-bend values in one segment");
+    boff[j + 1] = (int32_t)nb;
+  }
+  CK(m->d_bends.reserve((size_t)boff[kept] + 1));
+  CK(cudaMemcpyAsync(m->d_bend_off.p, boff.data(), sizeof(int) * (kept + 1), cudaMemcpyHostToDevice, st));
+  launch_note_finish(note, contour, m->d_note_base.p, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_amp.p, m->d_bend_off.p,
+                     m->d_bends.p, kept, with_bends, m->d_gauss, st);
+  CKL();
+  m->launches += 1;
+  const size_t b0 = s->q_bends.size();
+  s->q_bends.resize(b0 + boff[kept]);
+  CK(cudaMemcpyAsync(s->q_amp.data() + q0, m->d_amp.p, sizeof(float) * kept, cudaMemcpyDeviceToHost, st));
+  if (boff[kept] > 0)
+    CK(cudaMemcpyAsync(s->q_bends.data() + b0, m->d_bends.p, sizeof(int) * boff[kept], cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int j = 1; j <= kept; ++j) s->q_bend_off.push_back((int32_t)(b0 + boff[j]));
+  return BP_OK;
+}
+
+// One launch of the scan over the held rows from `flag_from` on; *cut = the confirming frame of the first cut at or
+// after s->scan_from, or -1, and *last the state after the last frame (both global).
+int stream_scan(bp_stream* s, long long flag_from, long long* cut, long long* last, cudaStream_t st) {
+  if (flag_from >= s->n && s->scan_from >= s->n) {
+    *cut = -1;
+    *last = s->last;
+    return BP_OK;
+  }
+  const long long hb = s->hb;
+  const long long last_row = s->last == kStreamNoRun ? kStreamNoRun : s->last - hb;
+  launch_stream_scan(s->note[s->cur].p, flag_from - hb, s->n - hb, s->dp.lo_col, s->dp.hi_col, s->dp.frame_thresh,
+                     s->quiet[s->cur].p, s->scan_from - hb, last_row, s->w, s->scan_out.p, s->done.p, st);
+  CKL();
+  s->m->launches += 1;
+  long long out[2];
+  CK(cudaMemcpyAsync(out, s->scan_out.p, sizeof(out), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  *cut = out[0] < 0 ? -1 : out[0] + hb;
+  *last = out[1] == kStreamNoRun ? kStreamNoRun : out[1] + hb;
+  return BP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bp_stream_create(bp_model_t* m, const bp_decode_params_t* params, int64_t max_segment_frames, bp_stream_t** out) {
+  if (!m || !out) return fail(BP_E_INVALID, "bp_stream_create: bad argument");
+  int rc = validate_params(params);
+  if (rc) return rc;
+  if (max_segment_frames < 0) return fail(BP_E_INVALID, "bp_stream_create: max_segment_frames must be >= 0 (0: no forced cut)");
+  DeviceGuard g(m->device);
+  std::unique_ptr<bp_stream> s(new bp_stream);
+  s->m = m;
+  s->params = *params;
+  s->dp = params_dev(*params);
+  s->la = params->energy_tol;
+  s->w = s->la + kStreamCutBefore;
+  s->after = std::max<long long>(1, (long long)params->energy_tol - 2);
+  s->max_seg = max_segment_frames;
+  auto cleanup = [&](int code) {
+    s->release();
+    return code;
+  };
+  if (s->max_onset.reserve(1) || s->max_fd.reserve(1) || s->done.reserve(1) || s->scan_out.reserve(2) || s->kept.reserve(1))
+    return cleanup(fail(BP_E_CUDA, "bp_stream_create: device allocation failed"));
+  cudaStream_t st = m->stream;
+  if (cudaMemsetAsync(s->max_onset.p, 0, sizeof(unsigned int), st) || cudaMemsetAsync(s->max_fd.p, 0, sizeof(unsigned long long), st) ||
+      cudaMemsetAsync(s->done.p, 0, sizeof(unsigned int), st) || cudaStreamSynchronize(st))
+    return cleanup(fail(BP_E_CUDA, std::string("bp_stream_create: ") + cudaGetErrorString(cudaGetLastError())));
+  *out = s.release();
+  return BP_OK;
+}
+
+void bp_stream_destroy(bp_stream_t* s) {
+  if (!s) return;
+  {
+    DeviceGuard g(s->m->device);
+    cudaStreamSynchronize(s->m->stream);
+    s->release();
+  }
+  delete s;
+}
+
+int64_t bp_stream_held_frames(const bp_stream_t* s) { return s ? s->n - s->hb : 0; }
+
+int bp_stream_push_host(bp_stream_t* s, const float* h_note, const float* h_onset, const float* h_contour,
+                        int64_t n_frames) {
+  const std::string api = "bp_stream_push_host";
+  if (!s || n_frames < 0) return fail(BP_E_INVALID, api + ": bad argument");
+  if (s->ended) return fail(BP_E_INVALID, api + ": the stream has ended");
+  if (n_frames > 0 && (!h_note || !h_onset || (s->params.include_pitch_bends && !h_contour)))
+    return fail(BP_E_INVALID, api + ": null posteriorgram");
+  if (n_frames == 0) return BP_OK;
+  if (s->n + n_frames > INT_MAX) return fail(BP_E_INVALID, api + ": the stream is longer than 2^31 - 1 frames");
+  bp_model* m = s->m;
+  DeviceGuard g(m->device);
+  cudaStream_t st = m->stream;
+  const int c0 = s->cur;
+  const long long need = s->n - s->hb + n_frames;
+  if (s->note[c0].cap < (size_t)need * kPitches || s->onset[c0].cap < (size_t)need * kPitches ||
+      (s->params.include_pitch_bends && s->contour[c0].cap < (size_t)need * kContourBins) || s->quiet[c0].cap < (size_t)need) {
+    int rc = stream_move(s, s->hb, need, st);
+    if (rc) return rc;
+  }
+  const int c = s->cur;
+  const long long row = s->n - s->hb;
+  CK(cudaMemcpyAsync(s->note[c].p + row * kPitches, h_note, sizeof(float) * n_frames * kPitches, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s->onset[c].p + row * kPitches, h_onset, sizeof(float) * n_frames * kPitches, cudaMemcpyHostToDevice,
+                     st));
+  if (s->params.include_pitch_bends)
+    CK(cudaMemcpyAsync(s->contour[c].p + row * kContourBins, h_contour, sizeof(float) * n_frames * kContourBins,
+                       cudaMemcpyHostToDevice, st));
+  long long flag_from = s->n;
+  s->n += n_frames;
+  while (true) {
+    long long t = -1, last = 0;
+    int rc = stream_scan(s, flag_from, &t, &last, st);
+    if (rc) return rc;
+    flag_from = s->n;
+    if (t >= 0 && (s->max_seg == 0 || t < s->a + s->max_seg)) {  // a quiet cut
+      const long long cut = t - s->la + 1;
+      rc = stream_decode(s, s->a, cut, s->seg_begin(s->a), cut + s->after, st);
+      if (rc) return rc;
+      s->a = cut;
+      s->last = kStreamNoRun;
+      s->scan_from = t + 1;
+    } else if (s->max_seg > 0 && s->n >= s->a + s->max_seg) {  // a forced cut: the segment ends as a file would
+      const long long f = s->a + s->max_seg;
+      rc = stream_decode(s, s->a, f, s->seg_begin(s->a), f, st);
+      if (rc) return rc;
+      s->r = s->a = f;
+      s->last = f - 1;
+      s->scan_from = f;
+    } else {
+      s->last = last;
+      s->scan_from = s->n;
+      break;
+    }
+  }
+  const long long keep = s->seg_begin(s->a);
+  if (keep > s->hb) return stream_move(s, keep, std::max<long long>(s->n - keep, 1), st);
+  return BP_OK;
+}
+
+int bp_stream_end(bp_stream_t* s) {
+  if (!s) return fail(BP_E_INVALID, "bp_stream_end: bad argument");
+  if (s->ended) return fail(BP_E_INVALID, "bp_stream_end: the stream has ended");
+  DeviceGuard g(s->m->device);
+  s->ended = true;
+  const int rc = stream_decode(s, s->a, s->n, s->seg_begin(s->a), s->n, s->m->stream);
+  if (rc) return rc;
+  s->a = s->hb = s->n;
+  return BP_OK;
+}
+
+int bp_stream_take(bp_stream_t* s, bp_notes_t* notes) {
+  if (!s || !notes || !notes->note_off || !notes->bend_off) return fail(BP_E_INVALID, "bp_stream_take: bad argument");
+  const long long n_notes = (long long)s->q_start.size();
+  const long long n_bends = (long long)s->q_bends.size();
+  g_need_notes = g_need_bends = 0;
+  notes->note_off[0] = 0;
+  notes->bend_off[0] = 0;
+  if (n_notes > notes->note_capacity || n_bends > notes->bend_capacity) {
+    g_need_notes = n_notes > notes->note_capacity ? n_notes : 0;
+    g_need_bends = n_bends > notes->bend_capacity ? n_bends : 0;
+    return fail(BP_E_CAPACITY, "bp_stream_take: capacity too small, need " + std::to_string(n_notes) + " notes and " +
+                                   std::to_string(n_bends) + " pitch-bend values");
+  }
+  if (n_notes > 0 && (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude))
+    return fail(BP_E_INVALID, "bp_stream_take: notes arrays missing");
+  if (n_bends > 0 && !notes->bends) return fail(BP_E_INVALID, "bp_stream_take: bends array missing");
+  notes->note_off[1] = (int32_t)n_notes;
+  if (n_notes > 0) {
+    std::memcpy(notes->start_frame, s->q_start.data(), sizeof(int32_t) * n_notes);
+    std::memcpy(notes->end_frame, s->q_end.data(), sizeof(int32_t) * n_notes);
+    std::memcpy(notes->pitch_midi, s->q_pitch.data(), sizeof(int32_t) * n_notes);
+    std::memcpy(notes->amplitude, s->q_amp.data(), sizeof(float) * n_notes);
+    std::memcpy(notes->bend_off, s->q_bend_off.data(), sizeof(int32_t) * (n_notes + 1));
+  }
+  if (n_bends > 0) std::memcpy(notes->bends, s->q_bends.data(), sizeof(int32_t) * n_bends);
+  s->q_start.clear();
+  s->q_end.clear();
+  s->q_pitch.clear();
+  s->q_amp.clear();
+  s->q_bends.clear();
+  s->q_bend_off.assign(1, 0);
+  return BP_OK;
+}
+
+}  // extern "C"

@@ -544,9 +544,16 @@ __global__ void __launch_bounds__(kSeqThreads) decode_seq_kernel(
 
 void launch_decode_notes(const float* note, const float* onset, const DecodeBuffers& b, int n_files,
                          long long total_frames, const DecodeParamsDev& p, cudaStream_t st) {
-  const long long cells = total_frames * kPitches;
   cudaMemsetAsync(b.max_onset, 0, sizeof(unsigned int) * n_files, st);
   cudaMemsetAsync(b.max_fd, 0, sizeof(unsigned long long) * n_files, st);
+  launch_decode_kernels(note, onset, b, n_files, total_frames, p, st);
+}
+
+// The three launches of launch_decode_notes without the reset of the maxima: the prep folds this batch into whatever
+// b.max_onset / b.max_fd hold (the note stream keeps its running maxima there).
+void launch_decode_kernels(const float* note, const float* onset, const DecodeBuffers& b, int n_files,
+                           long long total_frames, const DecodeParamsDev& p, cudaStream_t st) {
+  const long long cells = total_frames * kPitches;
   if (cells > 0) {
     const int threads = 256;
     const unsigned int blocks = (unsigned int)((total_frames + kTileFrames - 1) / kTileFrames);

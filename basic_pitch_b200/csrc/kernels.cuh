@@ -308,6 +308,23 @@ struct DecodeBuffers {
 long long decode_block_slots(long long total_frames, int n_files);
 void launch_decode_notes(const float* note, const float* onset, const DecodeBuffers& buf, int n_files,
                          long long total_frames, const DecodeParamsDev& p, cudaStream_t st);
+void launch_decode_kernels(const float* note, const float* onset, const DecodeBuffers& buf, int n_files,
+                           long long total_frames, const DecodeParamsDev& p, cudaStream_t st);
+// Note stream (csrc/stream.cu).  Frames are rows of the stream's held buffer.  The scan sets quiet[t] for rows
+// [flag_from, n) (every column of [lo, hi) below frame_thresh), then its last CTA walks rows [from, n): `last` is the row
+// before the cut-eligible quiet run in progress (kStreamNoRun: none), and the first row t with quiet[t] and
+// t - last == w confirms the cut t - energy_tol + 1.  out[0] = that row or -1, out[1] = `last` after row n - 1.
+constexpr long long kStreamNoRun = -(1LL << 60);
+constexpr long long kStreamCutBefore = 3;  // LB: quiet frames before a cut (include/bp_b200.h)
+constexpr long long kStreamCtxBefore = 3;  // decode context before a segment that starts at a cut
+void launch_stream_scan(const float* note, long long flag_from, long long n, int lo, int hi, double frame_thresh,
+                        unsigned char* quiet, long long from, long long last, long long w, long long* out,
+                        unsigned int* done, cudaStream_t st);
+// Keeps, in order, the decoded notes of one segment whose start lies in [keep_lo, keep_hi) (decode-range frames) and
+// writes them with frames offset by `frame0`, note_base[j] = base and *kept = their number.
+void launch_stream_compact(const int* count, const int* s_start, const int* s_end, const int* s_pitch, int keep_lo,
+                           int keep_hi, int frame0, long long base, int* start, int* end, int* pitch, long long* note_base,
+                           int* kept, cudaStream_t st);
 // Grid decode: a chunk of parameter sets ("settings") over one batch.  The cell-parallel kernels run once per group of
 // settings that share their inputs (blockIdx.y = group); the sequential loops once per (file, setting).
 struct DecodePrepGroup {  // a distinct pitch range (lo, hi): constrained frames, per-file max(onsets) / max(frame_diff)

@@ -292,6 +292,18 @@ class Model:
         )
         return self._split_notes(arrs, n_files)
 
+    def note_stream(self, onset_thresh=0.5, frame_thresh=0.3, min_note_len=11, min_freq: Optional[float] = None,
+                    max_freq: Optional[float] = None, melodia_trick=True, include_pitch_bends=True,
+                    max_segment_frames: Optional[int] = None) -> "NoteStream":
+        """A note decode for a recording whose posteriorgrams arrive piecewise (`bp_stream_*`, include/bp_b200.h): the
+        stream cuts at quiet stretches and returns each stretch's notes as soon as the cut after it is known, holding
+        only the frames since the last cut on the device.  Arguments as `note_creation.model_output_to_notes`
+        (infer_onsets on, energy_tol 11); max_segment_frames > 0 also cuts when that many frames passed without a quiet
+        cut, at the price of exactness there (DESIGN.md §4.5)."""
+        lo, hi = infer.frequency_to_column_range(min_freq, max_freq)
+        p = self._params(onset_thresh, frame_thresh, min_note_len, 11, True, melodia_trick, include_pitch_bends, lo, hi)
+        return NoteStream(self, p, max_segment_frames)
+
     @staticmethod
     def _cat_note_onset(notes, onsets):
         """Per-file note / onset posteriorgrams -> (frame offsets, note, onset) back to back."""
@@ -1017,6 +1029,62 @@ class Model:
 _DEFAULT_MODELS: Dict[Tuple[str, int], Model] = {}
 
 
+class NoteStream:
+    """The note decode of one streamed recording (`Model.note_stream`).  `push(note, onset, contour)` takes the next
+    frames ((T, 88), (T, 88), (T, 264) arrays; contour may be None without pitch bends) and `end()` closes the
+    recording; both return the note events that became final, as the reference's (start_s, end_s, pitch, amplitude,
+    bends) tuples with times at their frame index in the whole recording.  `held_frames` is the number of frames the
+    device holds."""
+
+    def __init__(self, model: Model, params: _lib.DecodeParams, max_segment_frames: Optional[int] = None):
+        self._model, self._lib = model, model._lib
+        self._bends = bool(params.include_pitch_bends)
+        self._h = C.c_void_p()
+        self._lib.bp_stream_create(model.handle, C.byref(params), int(max_segment_frames or 0), C.byref(self._h))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h and getattr(self, "_lib", None) is not None:
+            try:
+                self._lib.bp_stream_destroy(h)
+            except Exception:
+                pass
+
+    @property
+    def held_frames(self) -> int:
+        return int(self._lib.bp_stream_held_frames(self._h))
+
+    def push(self, note: np.ndarray, onset: np.ndarray, contour: Optional[np.ndarray]) -> List[infer.NoteEvent]:
+        note = np.ascontiguousarray(note, dtype=_F32).reshape(-1, N_FREQ_BINS_NOTES)
+        onset = np.ascontiguousarray(onset, dtype=_F32).reshape(-1, N_FREQ_BINS_NOTES)
+        if onset.shape != note.shape:
+            raise ValueError("note and onset posteriorgrams must be (T, 88) and of equal shape")
+        if contour is not None:
+            contour = np.ascontiguousarray(contour, dtype=_F32).reshape(-1, N_FREQ_BINS_CONTOURS)
+            if contour.shape[0] != note.shape[0]:
+                raise ValueError("contour posteriorgrams must have as many frames as note posteriorgrams")
+        elif self._bends:
+            raise ValueError("pitch bends need the contour posteriorgram")
+        self._lib.bp_stream_push_host(self._h, _ptr(note), _ptr(onset), _ptr(contour), note.shape[0])
+        return self._take()
+
+    def end(self) -> List[infer.NoteEvent]:
+        self._lib.bp_stream_end(self._h)
+        return self._take()
+
+    def _take(self) -> List[infer.NoteEvent]:
+        arrs = self._model._with_capacity(1, 0, lambda nt: self._lib.bp_stream_take(self._h, C.byref(nt)))
+        n = int(arrs["note_off"][1])
+        start, end = arrs["start"][:n], arrs["end"][:n]
+        t0, t1 = infer.frame_index_to_time(start.astype(np.int64)), infer.frame_index_to_time(end.astype(np.int64))
+        off, flat = arrs["bend_off"], arrs["bends"]
+        return [
+            (t0[j], t1[j], np.int64(arrs["pitch"][j]), np.float32(arrs["amp"][j]),
+             list(flat[off[j] : off[j + 1]].astype(np.int64)) if self._bends else None)
+            for j in range(n)
+        ]  # fmt: skip
+
+
 def default_model(model_path: Union[pathlib.Path, str] = ICASSP_2022_MODEL_PATH, device: Optional[int] = None) -> Model:
     """One shared `Model` per (path, device); what `predict(path)` uses when given a path."""
     dev = _default_device() if device is None else int(device)
@@ -1167,6 +1235,32 @@ def predict_stream(audio_blocks: Iterable[np.ndarray], model_or_model_path: Unio
         melodia_trick=melodia_trick, midi_tempo=midi_tempo, model=model,
     )
     return model_output, midi_data, note_events
+
+
+def predict_stream_notes(audio_blocks: Iterable[np.ndarray],
+                         model_or_model_path: Union["Model", pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+                         onset_threshold: float = DEFAULT_ONSET_THRESHOLD, frame_threshold: float = DEFAULT_FRAME_THRESHOLD,
+                         minimum_note_length: float = DEFAULT_MINIMUM_NOTE_LENGTH_MS,
+                         minimum_frequency: Optional[float] = None, maximum_frequency: Optional[float] = None,
+                         melodia_trick: bool = True, max_segment_seconds: Optional[float] = None,
+                         windows_per_step: int = 64):
+    """`predict`'s note events for a recording delivered block by block, yielded as they become final: a generator of
+    (model_output_part, note_events) per step.  The parts are `run_inference_stream`'s, in order, followed by one part
+    of zero frames that carries the notes of the end of the recording; the events are the reference's
+    (start_s, end_s, pitch, amplitude, bends) tuples with times in the whole recording.  The decode (`Model.note_stream`)
+    holds only the frames since the last quiet stretch on the device, so memory does not grow with the recording.
+    A stretch's notes equal `predict`'s once both of the recording's maxima that the inferred onsets use have arrived
+    (DESIGN.md §4.5); max_segment_seconds also cuts a stretch that grows longer than that, where the notes may differ.
+    The keyword arguments that shape the notes are `predict`'s, with its defaults; the MIDI ones do not apply."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    min_note_len = int(np.round(minimum_note_length / 1000 * (AUDIO_SAMPLE_RATE / FFT_HOP)))
+    max_seg = None if max_segment_seconds is None else max(1, int(np.round(max_segment_seconds * AUDIO_SAMPLE_RATE / FFT_HOP)))
+    stream = model.note_stream(onset_threshold, frame_threshold, min_note_len, minimum_frequency, maximum_frequency,
+                               melodia_trick, True, max_seg)
+    for part in run_inference_stream(audio_blocks, model, windows_per_step):
+        yield part, stream.push(part["note"], part["onset"], part["contour"])
+    widths = {"note": N_FREQ_BINS_NOTES, "onset": N_FREQ_BINS_NOTES, "contour": N_FREQ_BINS_CONTOURS}
+    yield {k: np.zeros((0, w), _F32) for k, w in widths.items()}, stream.end()
 
 
 class OutputExtensions(enum.Enum):

@@ -79,7 +79,11 @@ def constrain_frequency(onsets: np.ndarray, frames: np.ndarray, max_freq: Option
 
 def model_frames_to_time(n_frames: int) -> np.ndarray:
     """reference: note_creation.py:346-357 (librosa.frames_to_time inlined)."""
-    idx = np.arange(n_frames)
+    return frame_index_to_time(np.arange(n_frames))
+
+
+def frame_index_to_time(idx: np.ndarray) -> np.ndarray:
+    """`model_frames_to_time(n)[idx]` for int64 frame indices, element by element (the same float64 values)."""
     original_times = (idx * FFT_HOP).astype(int) / float(AUDIO_SAMPLE_RATE)
     window_numbers = np.floor(idx / ANNOT_N_FRAMES)
     window_offset = (FFT_HOP / AUDIO_SAMPLE_RATE) * (ANNOT_N_FRAMES - (AUDIO_N_SAMPLES / FFT_HOP)) + MAGIC_ALIGNMENT_OFFSET

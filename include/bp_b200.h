@@ -140,6 +140,52 @@ int bp_decode_device(bp_model_t* m, const float* d_note, const float* d_onset, c
 int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, const float* h_contour,
                    const int64_t* h_frame_off, int32_t n_files, const bp_decode_params_t* params, bp_notes_t* notes);
 
+/* ---- stage 3 for a streamed recording -------------------------------------------------------------------------------
+ * reference: model_output_to_notes (note_creation.py:52-111) for a recording whose posteriorgrams arrive piecewise (as
+ * run_inference_stream yields them), decoded as they arrive in bounded device memory.  DESIGN.md §4.5 gives the argument.
+ *   quiet frame  every column of [min_pitch_idx, max_pitch_idx) has a note value strictly below frame_thresh (a value
+ *                equal to it is "on", as in the decode's tracking); columns outside the range count as 0, so
+ *                frame_thresh <= 0 never gives a quiet frame and never cuts.
+ *   cut          at frame c when frames [c - LB, c + LA) are quiet and frame c - LB - 1 is not (or c - LB is the first
+ *                frame of the recording or of a forced part): one cut per quiet run of at least LA + LB frames, with
+ *                LA = energy_tol and LB = 3.  A cut is known once frame c + LA - 1 has been pushed.
+ *   segment      frames [a, b) between two cuts, decoded by the decode kernels as one file over [a - 3, b + A) with
+ *                A = max(1, energy_tol - 2) (no context before the start of the recording or of a forced part); only
+ *                notes that start in [a, b) are kept.  LA and LB are the smallest lengths for which the notes of every
+ *                segment are those of the whole-recording decode that start in it, given that the context is quiet:
+ *                a candidate on the last quiet frame before c scans energy_tol frames (LA); the peak pick at c reads
+ *                frame c - 1, whose inferred onset reads c - 3 (LB); a track whose last loud frame is c - 4 reads up to
+ *                c - 4 + energy_tol, which `i < n_frames - 1` must admit (A); every other read or write of the greedy
+ *                loops stays within energy_tol frames of a loud cell, so no track crosses a cut.
+ *   maxima       segment k infers its onsets with max(onsets) and max(frame_diff) over stream frames [0, e_k), e_k the
+ *                end of its decode range (the running maxima): a segment decoded after both recording-wide maxima have
+ *                arrived has exactly the notes of bp_decode_device on the whole recording; earlier ones may differ.
+ *   forced cut   max_segment_frames = M > 0: when M frames have arrived since the start a of the open segment and no cut
+ *                was known within them, the stream cuts at a + M as at a file boundary (the frames before decode as a
+ *                recording that ends there, those after as one that starts there; the maxima carry over).  Results
+ *                then differ from the whole-recording decode by construction.  M = 0: never.
+ * The device holds the frames from the open segment's decode start on: at most the longest stretch without a cut (or M)
+ * plus 3 frames of context and the frames pushed since the last cut, 1 760 bytes per frame.
+ * bp_stream_create validates params as bp_decode_device does (BP_E_INVALID), and M < 0.  The stream uses its model's
+ * device and stream and must be destroyed before it.
+ * bp_stream_push_host: n_frames consecutive frames, row-major [n_frames][88 | 88 | 264] host arrays (h_contour may be
+ *   NULL when !include_pitch_bends); synchronous.  Launches: one quiet scan, then per segment it closes one more scan
+ *   and the decode's prep, candidate, loop, compaction and note-finish kernels.  BP_E_INVALID after bp_stream_end.
+ * bp_stream_end: the recording has ended; decodes the open segment with the end-of-file rules.  BP_E_INVALID if called
+ *   twice.
+ * bp_stream_take: moves the finished notes out, as bp_decode_device's one file: note_off[0..1], global frame indices,
+ *   segments in time order and within a segment the reference's generation order, amplitudes and pitch bends as
+ *   there.  BP_E_CAPACITY (bp_last_required) leaves them queued.
+ * bp_stream_held_frames: frames held on the device, context included. */
+typedef struct bp_stream bp_stream_t;
+int bp_stream_create(bp_model_t* m, const bp_decode_params_t* params, int64_t max_segment_frames, bp_stream_t** out);
+int bp_stream_push_host(bp_stream_t* s, const float* h_note, const float* h_onset, const float* h_contour,
+                        int64_t n_frames);
+int bp_stream_end(bp_stream_t* s);
+int bp_stream_take(bp_stream_t* s, bp_notes_t* notes);
+int64_t bp_stream_held_frames(const bp_stream_t* s);
+void bp_stream_destroy(bp_stream_t* s);
+
 /* ---- stage 3 under a grid of decode parameters ------------------------------------------------
  * reference: note_creation.py:52-111 (model_output_to_notes without the MIDI object), called once per parameter set.
  * One call decodes the batch under each of params[0 .. n_params): every (setting, file) gets exactly the notes
