@@ -169,8 +169,11 @@ int bp_decode_host(bp_model_t* m, const float* h_note, const float* h_onset, con
  * bp_stream_create validates params as bp_decode_device does (BP_E_INVALID), and M < 0.  The stream uses its model's
  * device and stream and must be destroyed before it.
  * bp_stream_push_host: n_frames consecutive frames, row-major [n_frames][88 | 88 | 264] host arrays (h_contour may be
- *   NULL when !include_pitch_bends); synchronous.  Launches: one quiet scan, then per segment it closes one more scan
- *   and the decode's prep, candidate, loop, compaction and note-finish kernels.  BP_E_INVALID after bp_stream_end.
+ *   NULL when !include_pitch_bends); synchronous.  Launches: one quiet scan (none when n_frames == 0); then per segment
+ *   it closes one more scan unless the cut was confirmed by the last frame pushed, the decode's prep, candidate and loop
+ *   kernels (twice when the segment yields more notes than the first allowance of min(88 T, 8 T + 64) slots, T its
+ *   decode frames), the compaction if the decode found notes, and the note finish if any of them start in the segment.
+ *   BP_E_INVALID after bp_stream_end.
  * bp_stream_end: the recording has ended; decodes the open segment with the end-of-file rules.  BP_E_INVALID if called
  *   twice.
  * bp_stream_take: moves the finished notes out, as bp_decode_device's one file: note_off[0..1], global frame indices,

@@ -109,17 +109,41 @@ def plan(quiet: np.ndarray, energy_tol: int, max_segment_frames: int = 0) -> Lis
             c = t - la + 1
             segs.append((a, c, start(a, r), c + after, r))
             a, last = c, None
+    if m > 0 and n == a + m:  # the last m frames pushed complete a part: the forced cut is known with frame n - 1
+        segs.append((a, n, start(a, r), n, r))
+        r = a = n
     segs.append((a, n, start(a, r), n, r))
     return segs
+
+
+def confirmations(segs, energy_tol: int) -> List[Tuple[int, bool]]:
+    """(confirming frame, forced) of every cut of a plan: frame c + LA - 1 for a quiet cut at c, a + M - 1 for a forced
+    cut at a + M (a forced cut ends its decode range at the cut, a quiet one ctx_after frames later)."""
+    return [(b - 1, True) if e == b else (b + cut_after(energy_tol) - 1, False) for a, b, s, e, r in segs[:-1]]
+
+
+def push_schedule(segs, energy_tol: int, ends) -> Tuple[List[int], List[int]]:
+    """For pushes that end at the stream frames `ends` (cumulative frame counts, nondecreasing; a 0-frame push repeats
+    the previous end): closed_by[k] = the push that returns segment k's notes, the first whose frames include the cut's
+    confirming frame (len(ends): the end of the stream); held[j] = held frames after push j, n_j - (a if a == r else
+    a - 3) for the segment [a, ..) still open then (its decode start)."""
+    conf = [t for t, _ in confirmations(segs, energy_tol)]
+    closed_by = [next((j for j, n in enumerate(ends) if n > t), len(ends)) for t in conf] + [len(ends)]
+    held = []
+    for n in ends:
+        k = next((i for i, t in enumerate(conf) if t >= n), len(conf))
+        held.append(int(n) - segs[k][2])
+    return closed_by, held
 
 
 def stream_notes(output: Dict[str, np.ndarray], onset_thresh: float, frame_thresh: float, infer_onsets_flag: bool = True,
                  min_note_len: int = 11, melodia_trick: bool = True, energy_tol: int = 11, lo_col: int = 0,
                  hi_col: int = 88, include_pitch_bends: bool = True, max_segment_frames: int = 0,
-                 maxima: Optional[Tuple[float, float]] = None):
+                 maxima: Optional[Tuple[float, float]] = None, decoded: Optional[list] = None):
     """The stream's output, one list per segment of (start, end, pitch, amp, bends) frame-indexed notes (global frames)
     in the reference's generation order for that segment, plus the plan.  `maxima` = (max onset, max frame_diff) replaces
-    the running maxima (the whole file's make the decode exact)."""
+    the running maxima (the whole file's make the decode exact).  `decoded`, a list, receives per segment the number of
+    notes its decode range yields before the start filter."""
     note, onset, contour = output["note"], output["onset"], output["contour"]
     n = note.shape[0]
     lo, hi = int(lo_col), int(hi_col)
@@ -130,6 +154,8 @@ def stream_notes(output: Dict[str, np.ndarray], onset_thresh: float, frame_thres
     for a, b, s, e, _r in segs:
         if e <= s:
             out.append([])
+            if decoded is not None:
+                decoded.append(0)
             continue
         if maxima is None:
             mo, mf = oc[:e].max(), fd[:e].max()
@@ -140,6 +166,8 @@ def stream_notes(output: Dict[str, np.ndarray], onset_thresh: float, frame_thres
             local = decode_ref.output_to_notes_polyphonic(
                 np.array(nc[s:e]), np.array(on), onset_thresh, frame_thresh, min_note_len, False, None, None,
                 melodia_trick, energy_tol, lo, hi)  # fmt: skip
+        if decoded is not None:
+            decoded.append(len(local))
         local = [x for x in local if a <= s + x[0] < b]
         if include_pitch_bends:
             wb = decode_ref.pitch_bends(contour[s:e], local)
