@@ -3,8 +3,9 @@
 `to_cent_voicing`, `resample_melody_series` and the five metric functions follow mir_eval.melody.evaluate with its
 default arguments (hop=None, kind='linear', base_frequency=10, cent_tolerance=50, no est_voicing / ref_reward), with
 scipy.interpolate.interp1d doing the interpolation, so SciPy decides every edge case.  `counts` returns the seven
-integers the library's melody scorers return per (setting, file) or item (include/bp_b200.h, bp_score_melody_*), and
-`evaluate` the five floats, in mir_eval's order and under its key names.
+integers the library's melody scorers return per (setting, file) or item (include/bp_b200.h, bp_score_melody_*),
+`counts_cents` the same for series given as cents and voicing (as the library takes them), and `evaluate` the five
+floats, in mir_eval's order and under its key names.
 
 One case mir_eval does not define (it indexes est_time[0]): an estimate of no frames is read as unvoiced, cents 0, at
 every reference frame.
@@ -152,3 +153,26 @@ def counts_resampled(rv, rc, ev, ec, cent_tolerance=50):
 
 def counts(ref_time, ref_freq, est_time, est_freq, cent_tolerance=50):
     return counts_resampled(*to_cent_voicing(ref_time, ref_freq, est_time, est_freq), cent_tolerance)
+
+
+def counts_cents(ref_time, ref_cent, ref_voicing, est_time, est_cent, est_voicing, cent_tolerance=50):
+    """`counts` of series given as cents and voicing (what the library takes, include/bp_b200.h): the steps of
+    `to_cent_voicing` after hz2cents, then `resample_melody_series` and `counts_resampled`."""
+    ref_time, est_time = np.asarray(ref_time, np.float64), np.asarray(est_time, np.float64)
+    ref_cent, est_cent = np.asarray(ref_cent, np.float64), np.asarray(est_cent, np.float64)
+    ref_voicing, est_voicing = np.asarray(ref_voicing, np.float64), np.asarray(est_voicing, np.float64)
+    if len(ref_time) and ref_time[0] > 0:
+        ref_time = np.insert(ref_time, 0, 0)
+        ref_cent = np.insert(ref_cent, 0, ref_cent[0])
+        ref_voicing = np.insert(ref_voicing, 0, ref_voicing[0])
+    if len(est_time) and est_time[0] > 0:
+        est_time = np.insert(est_time, 0, 0)
+        est_cent = np.insert(est_cent, 0, est_cent[0])
+        est_voicing = np.insert(est_voicing, 0, est_voicing[0])
+    if len(est_time) == 0:
+        ev, ec = np.zeros(len(ref_time)), np.zeros(len(ref_time))
+    elif len(ref_time) == 0:
+        ev, ec = np.zeros(0), np.zeros(0)
+    else:
+        ec, ev = resample_melody_series(est_time, est_cent, est_voicing, ref_time)
+    return counts_resampled(ref_voicing, ref_cent, ev, ec, cent_tolerance)
