@@ -4047,20 +4047,66 @@ int bp_debug_frontend(bp_model_t* m, int which, void* h_out, int64_t n_windows) 
 }  // extern "C"
 
 // ---- note stream (bp_stream_*) --------------------------------------------------------------------------------------
+// Where a stream cuts (include/bp_b200.h, DESIGN.md §4.5), shared by bp_stream and the stream group: the open segment,
+// the state of the cut search and the policy "quiet cut, forced cut or wait".  Frame indices are global.
+struct StreamCuts {
+  long long la = 0, after = 0, max_seg = 0;  // LA = energy_tol, context after a quiet cut, M (0: no forced cut)
+  long long r = 0, a = 0;         // start of the recording or forced part; start of the open segment
+  long long last = -1;            // the frame before the cut-eligible quiet run in progress (kStreamNoRun: none)
+  long long scan_from = 0;        // first frame the cut search has not passed
+  struct Seg {
+    long long a, b, ds, de;  // kept frames [a, b), decode range [ds, de)
+  };
+  void init(const bp_decode_params_t& p, long long max_segment_frames) {
+    la = p.energy_tol;
+    after = std::max<long long>(1, (long long)p.energy_tol - 2);
+    max_seg = max_segment_frames;
+  }
+  long long w() const { return la + kStreamCutBefore; }
+  long long seg_begin(long long at) const { return at == r ? at : at - kStreamCtxBefore; }
+  // After a scan of the n frames held so far gave t (the confirming frame of the first cut at or after scan_from, or
+  // -1) and `run` (the run state after frame n - 1): the segment that closes, in *seg, or false when the stream waits
+  // for more frames.  A closed segment moves the search on; the caller scans again from scan_from.
+  bool next(long long n, long long t, long long run, Seg* seg) {
+    if (t >= 0 && (max_seg == 0 || t < a + max_seg)) {  // a quiet cut
+      const long long cut = t - la + 1;
+      *seg = Seg{a, cut, seg_begin(a), cut + after};
+      a = cut;
+      last = kStreamNoRun;
+      scan_from = t + 1;
+      return true;
+    }
+    if (max_seg > 0 && n >= a + max_seg) {  // a forced cut: the segment ends as a file would
+      const long long f = a + max_seg;
+      *seg = Seg{a, f, seg_begin(a), f};
+      r = a = f;
+      last = f - 1;
+      scan_from = f;
+      return true;
+    }
+    last = run;
+    scan_from = n;
+    return false;
+  }
+  // the open segment at the end of the recording
+  Seg end(long long n) {
+    const Seg s{a, n, seg_begin(a), n};
+    a = n;
+    return s;
+  }
+};
+
 // Frames arrive row-major and stay in the held buffers (rows 0 .. n - hb) until the segment that needs them is decoded.
 // Stream frame indices are global (0 = first frame pushed); row = frame - hb.
 struct bp_stream {
   bp_model* m = nullptr;
   bp_decode_params_t params{};
   DecodeParamsDev dp{};
-  long long la = 0, w = 0, after = 0, max_seg = 0;
   DevBuf<float> note[2], onset[2], contour[2];
   DevBuf<unsigned char> quiet[2];
   int cur = 0;                    // which of the two held buffers is live (the other receives the next move)
   long long hb = 0, n = 0;        // global frame of held row 0; frames pushed so far
-  long long r = 0, a = 0;         // start of the recording or forced part; start of the open segment
-  long long last = -1;            // the frame before the cut-eligible quiet run in progress (kStreamNoRun: none)
-  long long scan_from = 0;        // first frame the cut search has not passed
+  StreamCuts cuts;
   bool ended = false;
   DevBuf<unsigned int> max_onset, done;
   DevBuf<unsigned long long> max_fd;
@@ -4070,7 +4116,6 @@ struct bp_stream {
   std::vector<float> q_amp;
   std::vector<int32_t> q_bend_off{0};
 
-  long long seg_begin(long long at) const { return at == r ? at : at - kStreamCtxBefore; }
   void release() {
     for (int k = 0; k < 2; ++k) {
       note[k].release();
@@ -4216,15 +4261,16 @@ int stream_decode(bp_stream* s, long long a, long long b, long long ds, long lon
 // One launch of the scan over the held rows from `flag_from` on; *cut = the confirming frame of the first cut at or
 // after s->scan_from, or -1, and *last the state after the last frame (both global).
 int stream_scan(bp_stream* s, long long flag_from, long long* cut, long long* last, cudaStream_t st) {
-  if (flag_from >= s->n && s->scan_from >= s->n) {
+  const StreamCuts& c = s->cuts;
+  if (flag_from >= s->n && c.scan_from >= s->n) {
     *cut = -1;
-    *last = s->last;
+    *last = c.last;
     return BP_OK;
   }
   const long long hb = s->hb;
-  const long long last_row = s->last == kStreamNoRun ? kStreamNoRun : s->last - hb;
+  const long long last_row = c.last == kStreamNoRun ? kStreamNoRun : c.last - hb;
   launch_stream_scan(s->note[s->cur].p, flag_from - hb, s->n - hb, s->dp.lo_col, s->dp.hi_col, s->dp.frame_thresh,
-                     s->quiet[s->cur].p, s->scan_from - hb, last_row, s->w, s->scan_out.p, s->done.p, st);
+                     s->quiet[s->cur].p, c.scan_from - hb, last_row, c.w(), s->scan_out.p, s->done.p, st);
   CKL();
   s->m->launches += 1;
   long long out[2];
@@ -4249,10 +4295,7 @@ int bp_stream_create(bp_model_t* m, const bp_decode_params_t* params, int64_t ma
   s->m = m;
   s->params = *params;
   s->dp = params_dev(*params);
-  s->la = params->energy_tol;
-  s->w = s->la + kStreamCutBefore;
-  s->after = std::max<long long>(1, (long long)params->energy_tol - 2);
-  s->max_seg = max_segment_frames;
+  s->cuts.init(*params, max_segment_frames);
   auto cleanup = [&](int code) {
     s->release();
     return code;
@@ -4313,27 +4356,12 @@ int bp_stream_push_host(bp_stream_t* s, const float* h_note, const float* h_onse
     int rc = stream_scan(s, flag_from, &t, &last, st);
     if (rc) return rc;
     flag_from = s->n;
-    if (t >= 0 && (s->max_seg == 0 || t < s->a + s->max_seg)) {  // a quiet cut
-      const long long cut = t - s->la + 1;
-      rc = stream_decode(s, s->a, cut, s->seg_begin(s->a), cut + s->after, st);
-      if (rc) return rc;
-      s->a = cut;
-      s->last = kStreamNoRun;
-      s->scan_from = t + 1;
-    } else if (s->max_seg > 0 && s->n >= s->a + s->max_seg) {  // a forced cut: the segment ends as a file would
-      const long long f = s->a + s->max_seg;
-      rc = stream_decode(s, s->a, f, s->seg_begin(s->a), f, st);
-      if (rc) return rc;
-      s->r = s->a = f;
-      s->last = f - 1;
-      s->scan_from = f;
-    } else {
-      s->last = last;
-      s->scan_from = s->n;
-      break;
-    }
+    StreamCuts::Seg seg;
+    if (!s->cuts.next(s->n, t, last, &seg)) break;
+    rc = stream_decode(s, seg.a, seg.b, seg.ds, seg.de, st);
+    if (rc) return rc;
   }
-  const long long keep = s->seg_begin(s->a);
+  const long long keep = s->cuts.seg_begin(s->cuts.a);
   if (keep > s->hb) return stream_move(s, keep, std::max<long long>(s->n - keep, 1), st);
   return BP_OK;
 }
@@ -4343,9 +4371,10 @@ int bp_stream_end(bp_stream_t* s) {
   if (s->ended) return fail(BP_E_INVALID, "bp_stream_end: the stream has ended");
   DeviceGuard g(s->m->device);
   s->ended = true;
-  const int rc = stream_decode(s, s->a, s->n, s->seg_begin(s->a), s->n, s->m->stream);
+  const StreamCuts::Seg seg = s->cuts.end(s->n);
+  const int rc = stream_decode(s, seg.a, seg.b, seg.ds, seg.de, s->m->stream);
   if (rc) return rc;
-  s->a = s->hb = s->n;
+  s->hb = s->n;
   return BP_OK;
 }
 
@@ -4381,6 +4410,793 @@ int bp_stream_take(bp_stream_t* s, bp_notes_t* notes) {
   s->q_bends.clear();
   s->q_bend_off.assign(1, 0);
   return BP_OK;
+}
+
+}  // extern "C"
+
+// ---- stream group (bp_stream_group_*) ------------------------------------------------------------------------------
+// Many streams share one set of arenas.  Audio: each stream's unwindowed tail (samples [tail0, samples) of its
+// recording) sits in its region of the audio arena.  Frames: the rows of frames [hb, written) sit in its region of the
+// note / onset / contour / quiet arenas, frame f at row f + shift (shift = row0 - hb).  A region that runs out of room
+// makes the next push move every live stream's rows into a new arena with twice the room each needs (one copy launch).
+struct GroupStream {
+  int kind = 0;  // 0 nothing pushed yet, 1 audio, 2 posteriorgrams
+  bool ended = false;
+  long long samples = 0, win_done = 0, tail0 = 0;  // audio: samples pushed, windows run, first sample of the tail
+  long long a_beg = 0, a_end = 0, a_off = 0;       // audio region and the arena offset of sample tail0
+  long long f_beg = 0, f_end = 0, row0 = 0;        // frame region and the row of frame hb
+  long long hb = 0, n = 0, written = 0;            // first held frame, frames committed, frames in the arena
+  StreamCuts cuts;
+  std::vector<int32_t> q_start, q_end, q_pitch, q_bends;  // finished notes not yet taken
+  std::vector<float> q_amp;
+  std::vector<int32_t> q_bend_off{0};
+  long long shift() const { return row0 - hb; }
+};
+
+struct bp_stream_group {
+  bp_model* m = nullptr;
+  bp_decode_params_t params{};
+  DecodeParamsDev dp{};
+  long long max_seg = 0;
+  std::vector<GroupStream> s;  // by id
+  DevBuf<float> audio[2];
+  int acur = 0;
+  DevBuf<float> note[2], onset[2], contour[2];
+  DevBuf<unsigned char> quiet[2];
+  int fcur = 0;
+  DevBuf<unsigned int> max_onset, done;  // by id: running maxima; by scan job: the scan's CTA counters
+  DevBuf<unsigned long long> max_fd;
+  DevBuf<long long> scan_out, dst_row;
+  DevBuf<GroupScanJob> jobs;
+  DevBuf<GroupCopySeg> segs;
+  DevBuf<GroupKeep> keep;
+  DevBuf<WinDesc> wd;
+  DevBuf<UnwrapDesc> ud;
+  DevBuf<float> b_note, b_onset, stage;  // the decode batch; uploads and posteriorgram outputs
+  DevBuf<unsigned int> b_max_onset;
+  DevBuf<unsigned long long> b_max_fd;
+  DevBuf<int> note_off;
+  unsigned char* h_stage = nullptr;  // pinned
+  size_t h_stage_cap = 0;
+
+  void release() {
+    for (int k = 0; k < 2; ++k) {
+      audio[k].release();
+      note[k].release();
+      onset[k].release();
+      contour[k].release();
+      quiet[k].release();
+    }
+    for (auto* b : {&b_note, &b_onset, &stage}) b->release();
+    max_onset.release(), done.release(), b_max_onset.release();
+    max_fd.release(), b_max_fd.release();
+    scan_out.release(), dst_row.release();
+    jobs.release(), segs.release(), keep.release(), wd.release(), ud.release(), note_off.release();
+    if (h_stage) cudaFreeHost(h_stage);
+    h_stage = nullptr;
+    h_stage_cap = 0;
+  }
+};
+
+namespace {
+
+template <class T>
+int upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t st) {
+  CK(d.reserve(std::max<size_t>(h.size(), 1)));
+  if (!h.empty()) CK(cudaMemcpyAsync(d.p, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice, st));
+  return BP_OK;
+}
+
+int group_copy(bp_stream_group* g, const std::vector<GroupCopySeg>& segs, const GroupCopyArrays& a, cudaStream_t st) {
+  if (segs.empty()) return BP_OK;
+  int rc = upload(g->segs, segs, st);
+  if (rc) return rc;
+  long long most = 0;
+  for (const GroupCopySeg& x : segs) most = std::max(most, x.rows * a.width[x.arr]);
+  launch_group_copy(g->segs.p, (int)segs.size(), most, a, st);
+  CKL();
+  g->m->launches += 1;
+  return BP_OK;
+}
+
+int stage_host(bp_stream_group* g, size_t bytes) {
+  if (bytes <= g->h_stage_cap) return BP_OK;
+  if (g->h_stage) cudaFreeHost(g->h_stage);
+  g->h_stage = nullptr;
+  g->h_stage_cap = 0;
+  const size_t cap = std::max<size_t>(bytes + bytes / 4, 1 << 20);
+  CK(cudaMallocHost(&g->h_stage, cap));
+  g->h_stage_cap = cap;
+  return BP_OK;
+}
+
+// Makes room for need[id] more frames after each live stream's rows: when some region is too small, every live stream
+// moves to a region of twice what it holds and needs.
+int group_frame_room(bp_stream_group* g, const std::vector<long long>& need, cudaStream_t st) {
+  bool grow = false;
+  for (size_t k = 0; k < g->s.size(); ++k) {
+    const GroupStream& x = g->s[k];
+    if (!x.ended && need[k] > 0 && x.row0 + (x.written - x.hb) + need[k] > x.f_end) grow = true;
+  }
+  if (!grow) return BP_OK;
+  long long total = 0;
+  for (size_t k = 0; k < g->s.size(); ++k)
+    if (!g->s[k].ended) total += 2 * (g->s[k].written - g->s[k].hb + need[k]) + 64;
+  const int nx = g->fcur ^ 1;
+  CK(g->note[nx].reserve((size_t)total * kPitches));
+  CK(g->onset[nx].reserve((size_t)total * kPitches));
+  CK(g->contour[nx].reserve((size_t)total * kContourBins));
+  CK(g->quiet[nx].reserve((size_t)total));
+  const int c = g->fcur;
+  const GroupCopyArrays a{{g->note[c].p, g->onset[c].p, g->contour[c].p, g->quiet[c].p},
+                          {g->note[nx].p, g->onset[nx].p, g->contour[nx].p, g->quiet[nx].p},
+                          {kPitches, kPitches, kContourBins, 1},
+                          {4, 4, 4, 1}};
+  std::vector<GroupCopySeg> segs;
+  long long at = 0;
+  for (size_t k = 0; k < g->s.size(); ++k) {
+    GroupStream& x = g->s[k];
+    if (x.ended) continue;
+    const long long used = x.written - x.hb;
+    for (int arr = 0; arr < 4 && used > 0; ++arr) segs.push_back(GroupCopySeg{x.row0, at, used, arr, 0});
+    x.f_beg = x.row0 = at;
+    x.f_end = at += 2 * (used + need[k]) + 64;
+  }
+  int rc = group_copy(g, segs, a, st);
+  if (rc) return rc;
+  g->fcur = nx;
+  return BP_OK;
+}
+
+// The same for the audio tails.
+int group_audio_room(bp_stream_group* g, const std::vector<long long>& need, cudaStream_t st) {
+  bool grow = false;
+  for (size_t k = 0; k < g->s.size(); ++k) {
+    const GroupStream& x = g->s[k];
+    if (!x.ended && need[k] > 0 && x.a_off + (x.samples - x.tail0) + need[k] > x.a_end) grow = true;
+  }
+  if (!grow) return BP_OK;
+  long long total = 0;
+  for (size_t k = 0; k < g->s.size(); ++k)
+    if (!g->s[k].ended) total += 2 * (g->s[k].samples - g->s[k].tail0 + need[k]) + 256;
+  const int nx = g->acur ^ 1;
+  CK(g->audio[nx].reserve((size_t)total));
+  const GroupCopyArrays a{{g->audio[g->acur].p}, {g->audio[nx].p}, {1}, {4}};
+  std::vector<GroupCopySeg> segs;
+  long long at = 0;
+  for (size_t k = 0; k < g->s.size(); ++k) {
+    GroupStream& x = g->s[k];
+    if (x.ended) continue;
+    const long long used = x.samples - x.tail0;
+    if (used > 0) segs.push_back(GroupCopySeg{x.a_off, at, used, 0, 0});
+    x.a_beg = x.a_off = at;
+    x.a_end = at += 2 * (used + need[k]) + 256;
+  }
+  int rc = group_copy(g, segs, a, st);
+  if (rc) return rc;
+  g->acur = nx;
+  return BP_OK;
+}
+
+// Windows stream x runs when it has `samples` samples (at the end of the recording: all of them, the last zero-padded;
+// none for an empty recording), and the frames it has committed then: run_inference_stream holds back the frames of the
+// newest two windows, which the final trim of unwrap_output can reach, and keeps bp_num_frames(samples) in all.
+long long group_windows(long long samples, bool ending) {
+  if (ending) return samples > 0 ? bp_num_windows(samples) : 0;
+  return samples + kLeadZeros >= kWinSamples ? (samples + kLeadZeros - kWinSamples) / kHopSamples + 1 : 0;
+}
+long long group_committed(long long samples, long long windows, bool ending) {
+  return ending ? bp_num_frames(samples) : std::max<long long>(0, (windows - 2) * kHopFrames);
+}
+
+// Appends the blocks to the tails, runs the windows they complete (all remaining windows when `ending`) through the
+// forward pass into the frame arena and commits the frames run_inference_stream would have yielded by now.
+int group_audio(bp_stream_group* g, const std::vector<int>& ids, const float* const* audio, const int64_t* len,
+                bool ending, cudaStream_t st) {
+  bp_model* m = g->m;
+  std::vector<long long> need(g->s.size(), 0);
+  long long total = 0;
+  for (size_t i = 0; i < ids.size(); ++i) need[ids[i]] = len ? len[i] : 0, total += len ? len[i] : 0;
+  int rc = group_audio_room(g, need, st);
+  if (rc) return rc;
+  if (total > 0) {  // every new sample crosses once: host blocks -> pinned staging -> one copy -> each stream's tail
+    rc = stage_host(g, sizeof(float) * total);
+    if (rc) return rc;
+    CK(g->stage.reserve((size_t)total));
+    std::vector<GroupCopySeg> segs;
+    long long at = 0;
+    for (size_t i = 0; i < ids.size(); ++i) {
+      if (len[i] <= 0) continue;
+      const GroupStream& x = g->s[ids[i]];
+      std::memcpy(g->h_stage + sizeof(float) * at, audio[i], sizeof(float) * len[i]);
+      segs.push_back(GroupCopySeg{at, x.a_off + (x.samples - x.tail0), len[i], 0, 0});
+      at += len[i];
+    }
+    CK(cudaMemcpyAsync(g->stage.p, g->h_stage, sizeof(float) * total, cudaMemcpyHostToDevice, st));
+    rc = group_copy(g, segs, GroupCopyArrays{{g->stage.p}, {g->audio[g->acur].p}, {1}, {4}}, st);
+    if (rc) return rc;
+  }
+  std::fill(need.begin(), need.end(), 0);
+  for (size_t i = 0; i < ids.size(); ++i) {
+    GroupStream& x = g->s[ids[i]];
+    x.samples += len ? len[i] : 0;
+    need[ids[i]] = (group_windows(x.samples, ending) - x.win_done) * kHopFrames;
+  }
+  rc = group_frame_room(g, need, st);
+  if (rc) return rc;
+  std::vector<WinDesc> wd;
+  std::vector<UnwrapDesc> ud;
+  std::vector<long long> dst;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    GroupStream& x = g->s[ids[i]];
+    const long long nw = group_windows(x.samples, ending);
+    for (long long w = x.win_done; w < nw; ++w) {
+      const long long s0 = w * kHopSamples - kLeadZeros;  // window start in the recording (run_inference_internal)
+      WinDesc d;
+      d.base = x.a_off + (s0 - x.tail0);
+      d.lo = (int)std::max<long long>(0, -s0);
+      d.hi = (int)std::max<long long>(d.lo, std::min<long long>(kWinSamples, x.samples - s0));
+      wd.push_back(d);
+      ud.push_back(UnwrapDesc{(long long)(wd.size() - 1) % m->chunk * kHopFrames, kHopFrames, 0});
+      dst.push_back(x.shift() + w * kHopFrames);
+    }
+    x.written += (nw - x.win_done) * kHopFrames;
+    x.win_done = nw;
+    x.n = std::max(x.n, group_committed(x.samples, nw, ending));
+    // samples before the next window's start are not read again
+    const long long keep_from = ending ? x.samples : std::min(x.samples, std::max<long long>(0, nw * kHopSamples - kLeadZeros));
+    x.a_off += keep_from - x.tail0;
+    x.tail0 = keep_from;
+  }
+  const long long nwin = (long long)wd.size();
+  if (nwin == 0) return BP_OK;
+  const int chunk = m->chunk, nbmax = (int)std::min<long long>(nwin, chunk);
+  rc = ensure_forward_ws(m, nbmax);
+  if (rc) return rc;
+  if (m->path == 0) {
+    CK(m->raw_note.reserve((size_t)nbmax * kFrames * kPitches));
+    CK(m->raw_onset.reserve((size_t)nbmax * kFrames * kPitches));
+  }
+  if (m->path != 1) CK(m->raw_contour.reserve((size_t)nbmax * kFrames * kContourBins));
+  const long long stride = (long long)chunk * kHopFrames;
+  CK(m->u_note.reserve((size_t)stride * kPitches));
+  CK(m->u_onset.reserve((size_t)stride * kPitches));
+  CK(m->u_contour.reserve((size_t)stride * kContourBins));
+  if ((rc = upload(g->wd, wd, st)) || (rc = upload(g->ud, ud, st)) || (rc = upload(g->dst_row, dst, st))) return rc;
+  const PostI u{m->u_note.p, m->u_onset.p, m->u_contour.p, stride};
+  const int c = g->fcur;
+  for (long long c0 = 0; c0 < nwin; c0 += chunk) {
+    const int nb = (int)std::min<long long>(chunk, nwin - c0);
+    rc = forward_chunk(m, g->audio[g->acur].p, g->wd.p + c0, nb, m->raw_note.p, m->raw_onset.p, m->raw_contour.p, st,
+                       g->ud.p + c0, &u);
+    if (rc) return rc;
+    launch_group_unwrap(u.note, u.onset, u.contour, stride, g->dst_row.p + c0, nb, g->note[c].p, g->onset[c].p,
+                        g->contour[c].p, true, st);
+    CKL();
+    m->launches += 1;
+  }
+  m->last_forward_n = nbmax == nwin ? nwin : 0;
+  return BP_OK;
+}
+
+// Posteriorgram pushes: frames go to the arena and are committed at once.
+int group_frames(bp_stream_group* g, const std::vector<int>& ids, const float* const* note, const float* const* onset,
+                 const float* const* contour, const int64_t* n_frames, cudaStream_t st) {
+  std::vector<long long> need(g->s.size(), 0);
+  long long total = 0;
+  for (size_t i = 0; i < ids.size(); ++i) need[ids[i]] = n_frames[i], total += n_frames[i];
+  if (total == 0) return BP_OK;
+  int rc = group_frame_room(g, need, st);
+  if (rc) return rc;
+  const size_t row_bytes = sizeof(float) * (2 * kPitches + kContourBins);
+  rc = stage_host(g, row_bytes * total);
+  if (rc) return rc;
+  CK(g->stage.reserve((size_t)total * (2 * kPitches + kContourBins)));
+  float* h = reinterpret_cast<float*>(g->h_stage);
+  float *hn = h, *ho = h + total * kPitches, *hc = h + 2 * total * kPitches;
+  std::vector<GroupCopySeg> segs;
+  long long at = 0;
+  const int c = g->fcur;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    const long long T = n_frames[i];
+    if (T == 0) continue;
+    GroupStream& x = g->s[ids[i]];
+    std::memcpy(hn + at * kPitches, note[i], sizeof(float) * T * kPitches);
+    std::memcpy(ho + at * kPitches, onset[i], sizeof(float) * T * kPitches);
+    const long long row = x.row0 + (x.written - x.hb);
+    segs.push_back(GroupCopySeg{at, row, T, 0, 0});
+    segs.push_back(GroupCopySeg{at, row, T, 1, 0});
+    if (contour && contour[i]) {
+      std::memcpy(hc + at * kContourBins, contour[i], sizeof(float) * T * kContourBins);
+      segs.push_back(GroupCopySeg{at, row, T, 2, 0});
+    }
+    x.written += T;
+    x.n = x.written;
+    at += T;
+  }
+  CK(cudaMemcpyAsync(g->stage.p, h, row_bytes * total, cudaMemcpyHostToDevice, st));
+  const GroupCopyArrays a{{g->stage.p, g->stage.p + total * kPitches, g->stage.p + 2 * total * kPitches},
+                          {g->note[c].p, g->onset[c].p, g->contour[c].p},
+                          {kPitches, kPitches, kContourBins},
+                          {4, 4, 4}};
+  return group_copy(g, segs, a, st);
+}
+
+// One decode round: segment j of `batch` (one per stream) is file j of one decode of the gathered frames.
+int group_decode(bp_stream_group* g, const std::vector<std::pair<int, StreamCuts::Seg>>& batch, cudaStream_t st) {
+  bp_model* m = g->m;
+  const std::string api = "bp_stream_group";
+  const int nf = (int)batch.size();
+  std::vector<long long> foff(nf + 1, 0), soff(nf + 1, 0);
+  std::vector<GroupCopySeg> gather;
+  std::vector<GroupKeep> keep;
+  for (int j = 0; j < nf; ++j) {
+    const GroupStream& x = g->s[batch[j].first];
+    const StreamCuts::Seg& q = batch[j].second;
+    if (q.de > INT_MAX) return fail(BP_E_INVALID, api + ": a stream is longer than 2^31 - 1 frames");
+    const long long T = q.de - q.ds;
+    foff[j + 1] = foff[j] + T;
+    gather.push_back(GroupCopySeg{q.ds + x.shift(), foff[j], T, 0, 0});
+    gather.push_back(GroupCopySeg{q.ds + x.shift(), foff[j], T, 1, 0});
+    gather.push_back(GroupCopySeg{batch[j].first, j, 1, 2, 0});
+    gather.push_back(GroupCopySeg{batch[j].first, j, 1, 3, 0});
+    keep.push_back(GroupKeep{(int)(q.a - q.ds), (int)(q.b - q.ds), (int)q.ds, 0, x.shift()});
+  }
+  const long long total = foff[nf];
+  CK(g->b_note.reserve((size_t)total * kPitches));
+  CK(g->b_onset.reserve((size_t)total * kPitches));
+  CK(g->b_max_onset.reserve(nf));
+  CK(g->b_max_fd.reserve(nf));
+  CK(g->note_off.reserve(nf + 1));
+  int rc = upload(g->keep, keep, st);
+  if (rc) return rc;
+  // the segments' frames and their streams' running maxima (a 64-bit maximum is two 4-byte elements)
+  rc = group_copy(g, gather,
+                  GroupCopyArrays{{g->note[g->fcur].p, g->onset[g->fcur].p, g->max_onset.p, g->max_fd.p},
+                                  {g->b_note.p, g->b_onset.p, g->b_max_onset.p, g->b_max_fd.p},
+                                  {kPitches, kPitches, 1, 2},
+                                  {4, 4, 4, 4}},
+                  st);
+  if (rc) return rc;
+  std::vector<int> noff(nf + 1, 0);
+  for (int attempt = 0; attempt < 2; ++attempt) {
+    for (int j = 0; j < nf; ++j) {  // bp_stream's slot allowance per segment
+      const long long T = foff[j + 1] - foff[j];
+      soff[j + 1] = soff[j] + (attempt == 0 ? std::min<long long>(T * kPitches, 8 * T + 64) : T * kPitches);
+    }
+    if ((rc = upload(m->d_frame_off, foff, st)) || (rc = upload(m->d_slot_off, soff, st))) return rc;
+    CK(m->energy.reserve((size_t)total * kPitches + 1));
+    CK(m->candbits.reserve((size_t)decode_cand_words(total)));
+    CK(m->blk_max.reserve((size_t)kPitches * decode_block_slots(total, nf)));
+    CK(m->blk_arg.reserve((size_t)kPitches * decode_block_slots(total, nf)));
+    CK(m->note_count.reserve(nf));
+    CK(m->overflow.reserve(1));
+    for (auto* b : {&m->slot_start, &m->slot_end, &m->slot_pitch, &m->d_start, &m->d_end, &m->d_pitch})
+      CK(b->reserve((size_t)soff[nf] + 1));
+    CK(m->d_note_base.reserve((size_t)soff[nf] + 1));
+    CK(cudaMemsetAsync(m->overflow.p, 0, sizeof(int), st));
+    DecodeBuffers bufs;
+    bufs.frame_off = m->d_frame_off.p;
+    bufs.energy = m->energy.p;
+    bufs.candbits = m->candbits.p;
+    bufs.max_onset = g->b_max_onset.p;
+    bufs.max_fd = g->b_max_fd.p;
+    bufs.slot_off = m->d_slot_off.p;
+    bufs.note_count = m->note_count.p;
+    bufs.note_start = m->slot_start.p;
+    bufs.note_end = m->slot_end.p;
+    bufs.note_pitch = m->slot_pitch.p;
+    bufs.overflow = m->overflow.p;
+    bufs.blk_max = m->blk_max.p;
+    bufs.blk_arg = m->blk_arg.p;
+    launch_decode_kernels(g->b_note.p, g->b_onset.p, bufs, nf, total, g->dp, st);
+    launch_group_compact(g->keep.p, nf, m->d_slot_off.p, m->note_count.p, m->slot_start.p, m->slot_end.p,
+                         m->slot_pitch.p, m->d_start.p, m->d_end.p, m->d_pitch.p, m->d_note_base.p, g->note_off.p, st);
+    CKL();
+    m->launches += 4;
+    int overflow = 0;
+    CK(cudaMemcpyAsync(&overflow, m->overflow.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(noff.data(), g->note_off.p, sizeof(int) * (nf + 1), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (!overflow) break;
+    if (attempt == 1) return fail(BP_E_CUDA, api + ": note slots overflowed at full capacity (internal error)");
+  }
+  // the maxima back to their streams (the prep folds a segment in idempotently, so a second attempt leaves them as is)
+  std::vector<GroupCopySeg> back;
+  for (int j = 0; j < nf; ++j) {
+    back.push_back(GroupCopySeg{j, batch[j].first, 1, 0, 0});
+    back.push_back(GroupCopySeg{j, batch[j].first, 1, 1, 0});
+  }
+  rc = group_copy(g, back, GroupCopyArrays{{g->b_max_onset.p, g->b_max_fd.p}, {g->max_onset.p, g->max_fd.p}, {1, 2}, {4, 4}},
+                  st);
+  if (rc) return rc;
+  const int kept = noff[nf];
+  if (kept == 0) return BP_OK;
+  std::vector<int32_t> start(kept), end(kept), pitch(kept), bends;
+  std::vector<float> amp(kept);
+  CK(cudaMemcpyAsync(start.data(), m->d_start.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(end.data(), m->d_end.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(pitch.data(), m->d_pitch.p, sizeof(int) * kept, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int with_bends = g->params.include_pitch_bends ? 1 : 0;
+  std::vector<int32_t> boff(kept + 1, 0);
+  for (int k = 0; k < kept; ++k) {
+    const long long nb = boff[k] + (with_bends ? (long long)end[k] - start[k] : 0);
+    if (nb > 0x7fffffffLL) return fail(BP_E_CAPACITY, api + ": more than 2^31 pitch-bend values in one round");
+    boff[k + 1] = (int32_t)nb;
+  }
+  CK(m->d_amp.reserve(kept));
+  CK(m->d_bend_off.reserve(kept + 1));
+  CK(m->d_bends.reserve((size_t)boff[kept] + 1));
+  CK(cudaMemcpyAsync(m->d_bend_off.p, boff.data(), sizeof(int) * (kept + 1), cudaMemcpyHostToDevice, st));
+  launch_note_finish(g->note[g->fcur].p, g->contour[g->fcur].p, m->d_note_base.p, m->d_start.p, m->d_end.p, m->d_pitch.p,
+                     m->d_amp.p, m->d_bend_off.p, m->d_bends.p, kept, with_bends, m->d_gauss, st);
+  CKL();
+  m->launches += 1;
+  bends.resize(boff[kept]);
+  CK(cudaMemcpyAsync(amp.data(), m->d_amp.p, sizeof(float) * kept, cudaMemcpyDeviceToHost, st));
+  if (boff[kept] > 0)
+    CK(cudaMemcpyAsync(bends.data(), m->d_bends.p, sizeof(int) * boff[kept], cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int j = 0; j < nf; ++j) {
+    GroupStream& x = g->s[batch[j].first];
+    for (int k = noff[j]; k < noff[j + 1]; ++k) {
+      x.q_start.push_back(start[k]);
+      x.q_end.push_back(end[k]);
+      x.q_pitch.push_back(pitch[k]);
+      x.q_amp.push_back(amp[k]);
+      x.q_bends.insert(x.q_bends.end(), bends.begin() + boff[k], bends.begin() + boff[k + 1]);
+      x.q_bend_off.push_back((int32_t)x.q_bends.size());
+    }
+  }
+  return BP_OK;
+}
+
+// The scans and decode rounds after the streams `ids` committed frames from flag_from[i] on (`ending`: and ended).
+// Each round scans the streams that may hold a cut in one launch and decodes at most one segment per stream.
+int group_rounds(bp_stream_group* g, const std::vector<int>& ids, const std::vector<long long>& flag_from, bool ending,
+                 cudaStream_t st) {
+  bp_model* m = g->m;
+  std::vector<std::pair<int, long long>> scan;  // (id, first frame whose quiet flag is not set yet)
+  for (size_t i = 0; i < ids.size(); ++i) scan.emplace_back(ids[i], flag_from[i]);
+  std::vector<char> closed(g->s.size(), 0);  // ending: the stream's last segment has been decoded
+  std::vector<long long> out;
+  while (!scan.empty()) {
+    std::vector<GroupScanJob> jobs;
+    std::vector<int> job_of(scan.size(), -1);
+    long long most = 0;
+    for (size_t i = 0; i < scan.size(); ++i) {
+      const GroupStream& x = g->s[scan[i].first];
+      if (scan[i].second >= x.n && x.cuts.scan_from >= x.n) continue;  // nothing to look at (bp_stream: no launch)
+      job_of[i] = (int)jobs.size();
+      jobs.push_back(GroupScanJob{x.shift(), scan[i].second, x.n, x.cuts.scan_from, x.cuts.last});
+      most = std::max(most, x.n - scan[i].second);
+    }
+    if (!jobs.empty()) {
+      int rc = upload(g->jobs, jobs, st);
+      if (rc) return rc;
+      CK(g->scan_out.reserve(2 * jobs.size()));
+      if (g->done.cap < jobs.size()) {  // the CTA counters start at zero and every launch leaves them there
+        CK(g->done.reserve(jobs.size()));
+        CK(cudaMemsetAsync(g->done.p, 0, sizeof(unsigned int) * g->done.cap, st));
+      }
+      launch_group_scan(g->jobs.p, (int)jobs.size(), most, g->note[g->fcur].p, g->dp.lo_col, g->dp.hi_col,
+                        g->dp.frame_thresh, g->quiet[g->fcur].p,
+                        (long long)g->params.energy_tol + kStreamCutBefore, g->scan_out.p, g->done.p, st);
+      CKL();
+      m->launches += 1;
+      out.resize(2 * jobs.size());
+      CK(cudaMemcpyAsync(out.data(), g->scan_out.p, sizeof(long long) * out.size(), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    }
+    std::vector<std::pair<int, StreamCuts::Seg>> batch;
+    std::vector<std::pair<int, long long>> again;
+    for (size_t i = 0; i < scan.size(); ++i) {
+      const int id = scan[i].first;
+      GroupStream& x = g->s[id];
+      const long long t = job_of[i] < 0 ? -1 : out[2 * job_of[i]];
+      const long long run = job_of[i] < 0 ? x.cuts.last : out[2 * job_of[i] + 1];
+      StreamCuts::Seg seg;
+      if (x.cuts.next(x.n, t, run, &seg)) {
+        again.emplace_back(id, x.n);
+      } else if (ending && !closed[id]) {
+        seg = x.cuts.end(x.n);
+        closed[id] = 1;
+      } else {
+        continue;
+      }
+      if (seg.de > seg.ds && seg.b > seg.a) batch.emplace_back(id, seg);
+    }
+    if (!batch.empty()) {
+      int rc = group_decode(g, batch, st);
+      if (rc) return rc;
+    }
+    scan.swap(again);
+  }
+  for (int id : ids) {
+    GroupStream& x = g->s[id];
+    const long long keep = ending ? x.n : x.cuts.seg_begin(x.cuts.a);
+    if (keep > x.hb) {
+      x.row0 += keep - x.hb;
+      x.hb = keep;
+    }
+    if (ending) x.ended = true;
+  }
+  return BP_OK;
+}
+
+// Checks the ids of a call: known, open, each once, and (kind 1 audio, 2 posteriorgrams) not mixing push kinds.
+int group_ids(const bp_stream_group* g, const std::string& api, int32_t n, const int32_t* ids, int kind,
+              std::vector<int>& out) {
+  if (!g || n < 0 || (n > 0 && !ids)) return fail(BP_E_INVALID, api + ": bad argument");
+  if (n > 65535) return fail(BP_E_INVALID, api + ": at most 65 535 streams per call");  // the scan's grid y extent
+  std::vector<char> seen(g->s.size(), 0);
+  out.assign(ids, ids + n);
+  for (int32_t id : out) {
+    if (id < 0 || (size_t)id >= g->s.size()) return fail(BP_E_INVALID, api + ": unknown stream id " + std::to_string(id));
+    if (g->s[id].ended) return fail(BP_E_INVALID, api + ": stream " + std::to_string(id) + " has ended");
+    if (seen[id]) return fail(BP_E_INVALID, api + ": stream " + std::to_string(id) + " listed twice");
+    seen[id] = 1;
+    if (kind && g->s[id].kind && g->s[id].kind != kind)
+      return fail(BP_E_INVALID, api + ": stream " + std::to_string(id) +
+                                    (kind == 1 ? " was given posteriorgrams, not audio" : " was given audio, not posteriorgrams"));
+  }
+  return BP_OK;
+}
+
+// Frames each listed stream commits in a push of n_samples[i] samples (NULL: none) or at its end: offsets [n + 1].
+void group_offsets(const bp_stream_group* g, const std::vector<int>& ids, const int64_t* n_samples, bool ending,
+                   int64_t* off) {
+  off[0] = 0;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    const GroupStream& x = g->s[ids[i]];
+    long long c = x.n;
+    if (x.kind != 2) {
+      const long long smp = x.samples + (n_samples ? n_samples[i] : 0);
+      c = std::max(x.n, group_committed(smp, std::max(x.win_done, group_windows(smp, ending)), ending));
+    }
+    off[i + 1] = off[i] + (c - x.n);
+  }
+}
+
+// Copies the frames [from[i], n) each stream committed to the host arrays at off[i].
+int group_out(bp_stream_group* g, const std::vector<int>& ids, const std::vector<long long>& from, const int64_t* off,
+              float* h_note, float* h_onset, float* h_contour, cudaStream_t st) {
+  const long long total = off[ids.size()];
+  if (total == 0 || (!h_note && !h_onset && !h_contour)) return BP_OK;
+  CK(g->stage.reserve((size_t)total * (2 * kPitches + kContourBins)));
+  float *dn = g->stage.p, *dno = dn + total * kPitches, *dc = dno + total * kPitches;
+  std::vector<GroupCopySeg> segs;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    const GroupStream& x = g->s[ids[i]];
+    const long long rows = off[i + 1] - off[i];
+    if (rows == 0) continue;
+    for (int arr = 0; arr < 3; ++arr) segs.push_back(GroupCopySeg{from[i] + x.shift(), off[i], rows, arr, 0});
+  }
+  const int c = g->fcur;
+  int rc = group_copy(g, segs,
+                      GroupCopyArrays{{g->note[c].p, g->onset[c].p, g->contour[c].p}, {dn, dno, dc},
+                                      {kPitches, kPitches, kContourBins}, {4, 4, 4}},
+                      st);
+  if (rc) return rc;
+  if (h_note) CK(cudaMemcpyAsync(h_note, dn, sizeof(float) * total * kPitches, cudaMemcpyDeviceToHost, st));
+  if (h_onset) CK(cudaMemcpyAsync(h_onset, dno, sizeof(float) * total * kPitches, cudaMemcpyDeviceToHost, st));
+  if (h_contour) CK(cudaMemcpyAsync(h_contour, dc, sizeof(float) * total * kContourBins, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+// An audio push (ending: the streams' end, no new samples).
+int group_audio_step(bp_stream_group* g, const std::string& api, int32_t n, const int32_t* id_arr,
+                     const float* const* audio, const int64_t* n_samples, bool ending, float* h_note, float* h_onset,
+                     float* h_contour, int64_t* h_frame_off) {
+  std::vector<int> ids;
+  int rc = group_ids(g, api, n, id_arr, ending ? 0 : 1, ids);
+  if (rc) return rc;
+  for (int32_t i = 0; i < n && !ending; ++i) {
+    if (!n_samples || n_samples[i] < 0) return fail(BP_E_INVALID, api + ": negative or missing n_samples");
+    if (n_samples[i] > 0 && (!audio || !audio[i])) return fail(BP_E_INVALID, api + ": null audio block");
+  }
+  std::vector<int64_t> off(ids.size() + 1);
+  group_offsets(g, ids, ending ? nullptr : n_samples, ending, off.data());
+  for (size_t i = 0; i < ids.size(); ++i)
+    if (g->s[ids[i]].n + (off[i + 1] - off[i]) > INT_MAX)
+      return fail(BP_E_INVALID, api + ": a stream is longer than 2^31 - 1 frames");
+  if (h_frame_off) std::copy(off.begin(), off.end(), h_frame_off);
+  DeviceGuard dg(g->m->device);
+  cudaStream_t st = g->m->stream;
+  std::vector<int> audio_ids;  // streams whose frames come from the model
+  std::vector<const float*> blocks;
+  std::vector<int64_t> lens;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    GroupStream& x = g->s[ids[i]];
+    if (!ending) x.kind = 1;
+    if (x.kind != 1) continue;
+    audio_ids.push_back(ids[i]);
+    blocks.push_back(ending ? nullptr : audio[i]);
+    lens.push_back(ending ? 0 : n_samples[i]);
+  }
+  std::vector<long long> from;
+  for (int id : ids) from.push_back(g->s[id].n);
+  rc = group_audio(g, audio_ids, blocks.data(), lens.data(), ending, st);
+  if (rc) return rc;
+  rc = group_out(g, ids, from, off.data(), h_note, h_onset, h_contour, st);
+  if (rc) return rc;
+  rc = group_rounds(g, ids, from, ending, st);
+  if (rc) return rc;
+  // a push that commits no frame has not synchronised yet: the next push rewrites the pinned staging this one's
+  // upload reads
+  CK(cudaStreamSynchronize(st));
+  return BP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bp_stream_group_create(bp_model_t* m, const bp_decode_params_t* params, int64_t max_segment_frames,
+                           bp_stream_group_t** out) {
+  if (!m || !out) return fail(BP_E_INVALID, "bp_stream_group_create: bad argument");
+  int rc = validate_params(params);
+  if (rc) return rc;
+  if (max_segment_frames < 0)
+    return fail(BP_E_INVALID, "bp_stream_group_create: max_segment_frames must be >= 0 (0: no forced cut)");
+  bp_stream_group* g = new bp_stream_group;
+  g->m = m;
+  g->params = *params;
+  g->dp = params_dev(*params);
+  g->max_seg = max_segment_frames;
+  *out = g;
+  return BP_OK;
+}
+
+void bp_stream_group_destroy(bp_stream_group_t* g) {
+  if (!g) return;
+  {
+    DeviceGuard dg(g->m->device);
+    cudaStreamSynchronize(g->m->stream);
+    g->release();
+  }
+  delete g;
+}
+
+int bp_stream_group_open(bp_stream_group_t* g, int32_t* id) {
+  if (!g || !id) return fail(BP_E_INVALID, "bp_stream_group_open: bad argument");
+  if (g->s.size() >= (size_t)INT32_MAX) return fail(BP_E_CAPACITY, "bp_stream_group_open: too many streams");
+  DeviceGuard dg(g->m->device);
+  const size_t k = g->s.size();
+  if (g->max_onset.cap <= k || g->max_fd.cap <= k) {  // the running maxima by id; a new stream's start at zero
+    DevBuf<unsigned int> mo;
+    DevBuf<unsigned long long> mf;
+    CK(mo.reserve(k + 1));
+    CK(mf.reserve(k + 1));
+    cudaStream_t st = g->m->stream;
+    if (k > 0) {
+      CK(cudaMemcpyAsync(mo.p, g->max_onset.p, sizeof(unsigned int) * k, cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync(mf.p, g->max_fd.p, sizeof(unsigned long long) * k, cudaMemcpyDeviceToDevice, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    g->max_onset.release();
+    g->max_fd.release();
+    g->max_onset = mo;
+    g->max_fd = mf;
+  }
+  CK(cudaMemsetAsync(g->max_onset.p + k, 0, sizeof(unsigned int), g->m->stream));
+  CK(cudaMemsetAsync(g->max_fd.p + k, 0, sizeof(unsigned long long), g->m->stream));
+  CK(cudaStreamSynchronize(g->m->stream));
+  GroupStream x;
+  x.cuts.init(g->params, g->max_seg);
+  g->s.push_back(std::move(x));
+  *id = (int32_t)k;
+  return BP_OK;
+}
+
+int bp_stream_group_commit_offsets(const bp_stream_group_t* g, int32_t n, const int32_t* ids, const int64_t* n_samples,
+                                   int32_t ending, int64_t* h_frame_off) {
+  const std::string api = "bp_stream_group_commit_offsets";
+  std::vector<int> v;
+  int rc = group_ids(g, api, n, ids, 0, v);
+  if (rc) return rc;
+  if (!h_frame_off) return fail(BP_E_INVALID, api + ": bad argument");
+  for (int32_t i = 0; i < n && !ending; ++i)
+    if (!n_samples || n_samples[i] < 0) return fail(BP_E_INVALID, api + ": negative or missing n_samples");
+  group_offsets(g, v, ending ? nullptr : n_samples, ending != 0, h_frame_off);
+  return BP_OK;
+}
+
+int bp_stream_group_push_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const float* const* audio,
+                              const int64_t* n_samples, float* h_note, float* h_onset, float* h_contour,
+                              int64_t* h_frame_off) {
+  return group_audio_step(g, "bp_stream_group_push_host", n, ids, audio, n_samples, false, h_note, h_onset, h_contour,
+                          h_frame_off);
+}
+
+int bp_stream_group_end(bp_stream_group_t* g, int32_t n, const int32_t* ids, float* h_note, float* h_onset,
+                        float* h_contour, int64_t* h_frame_off) {
+  return group_audio_step(g, "bp_stream_group_end", n, ids, nullptr, nullptr, true, h_note, h_onset, h_contour,
+                          h_frame_off);
+}
+
+int bp_stream_group_push_frames_host(bp_stream_group_t* g, int32_t n, const int32_t* id_arr, const float* const* h_note,
+                                     const float* const* h_onset, const float* const* h_contour,
+                                     const int64_t* n_frames) {
+  const std::string api = "bp_stream_group_push_frames_host";
+  std::vector<int> ids;
+  int rc = group_ids(g, api, n, id_arr, 2, ids);
+  if (rc) return rc;
+  for (int32_t i = 0; i < n; ++i) {
+    if (!n_frames || n_frames[i] < 0) return fail(BP_E_INVALID, api + ": negative or missing n_frames");
+    if (n_frames[i] > 0 && (!h_note || !h_onset || !h_note[i] || !h_onset[i] ||
+                            (g->params.include_pitch_bends && (!h_contour || !h_contour[i]))))
+      return fail(BP_E_INVALID, api + ": null posteriorgram");
+    if (g->s[ids[i]].n + n_frames[i] > INT_MAX) return fail(BP_E_INVALID, api + ": the stream is longer than 2^31 - 1 frames");
+  }
+  DeviceGuard dg(g->m->device);
+  cudaStream_t st = g->m->stream;
+  std::vector<long long> from;
+  for (int id : ids) {
+    from.push_back(g->s[id].n);
+    g->s[id].kind = 2;
+  }
+  rc = group_frames(g, ids, h_note, h_onset, h_contour, n_frames, st);
+  if (rc) return rc;
+  return group_rounds(g, ids, from, false, st);
+}
+
+int bp_stream_group_take(bp_stream_group_t* g, int32_t n, const int32_t* id_arr, bp_notes_t* notes) {
+  const std::string api = "bp_stream_group_take";
+  if (!g || n < 0 || (n > 0 && !id_arr) || !notes || !notes->note_off || !notes->bend_off)
+    return fail(BP_E_INVALID, api + ": bad argument");
+  long long n_notes = 0, n_bends = 0;
+  std::vector<char> seen(g->s.size(), 0);
+  for (int32_t i = 0; i < n; ++i) {  // ended streams may still hold notes
+    const int32_t id = id_arr[i];
+    if (id < 0 || (size_t)id >= g->s.size()) return fail(BP_E_INVALID, api + ": unknown stream id " + std::to_string(id));
+    if (seen[id]) return fail(BP_E_INVALID, api + ": stream " + std::to_string(id) + " listed twice");
+    seen[id] = 1;
+    n_notes += (long long)g->s[id].q_start.size();
+    n_bends += (long long)g->s[id].q_bends.size();
+  }
+  g_need_notes = g_need_bends = 0;
+  notes->note_off[0] = 0;
+  notes->bend_off[0] = 0;
+  if (n_notes > notes->note_capacity || n_bends > notes->bend_capacity) {
+    g_need_notes = n_notes > notes->note_capacity ? n_notes : 0;
+    g_need_bends = n_bends > notes->bend_capacity ? n_bends : 0;
+    return fail(BP_E_CAPACITY, api + ": capacity too small, need " + std::to_string(n_notes) + " notes and " +
+                                   std::to_string(n_bends) + " pitch-bend values");
+  }
+  if (n_notes > 0 && (!notes->start_frame || !notes->end_frame || !notes->pitch_midi || !notes->amplitude))
+    return fail(BP_E_INVALID, api + ": notes arrays missing");
+  if (n_bends > 0 && !notes->bends) return fail(BP_E_INVALID, api + ": bends array missing");
+  long long k = 0, b = 0;
+  for (int32_t i = 0; i < n; ++i) {
+    GroupStream& x = g->s[id_arr[i]];
+    const size_t q = x.q_start.size();
+    if (q > 0) {
+      std::memcpy(notes->start_frame + k, x.q_start.data(), sizeof(int32_t) * q);
+      std::memcpy(notes->end_frame + k, x.q_end.data(), sizeof(int32_t) * q);
+      std::memcpy(notes->pitch_midi + k, x.q_pitch.data(), sizeof(int32_t) * q);
+      std::memcpy(notes->amplitude + k, x.q_amp.data(), sizeof(float) * q);
+      for (size_t j = 1; j <= q; ++j) notes->bend_off[k + j] = (int32_t)(b + x.q_bend_off[j]);
+      if (!x.q_bends.empty()) std::memcpy(notes->bends + b, x.q_bends.data(), sizeof(int32_t) * x.q_bends.size());
+    }
+    k += (long long)q;
+    b += (long long)x.q_bends.size();
+    notes->note_off[i + 1] = (int32_t)k;
+    x.q_start.clear();
+    x.q_end.clear();
+    x.q_pitch.clear();
+    x.q_amp.clear();
+    x.q_bends.clear();
+    x.q_bend_off.assign(1, 0);
+  }
+  return BP_OK;
+}
+
+int64_t bp_stream_group_held_frames(const bp_stream_group_t* g, int32_t id) {
+  if (!g || id < 0 || (size_t)id >= g->s.size()) return 0;
+  return g->s[id].n - g->s[id].hb;
 }
 
 }  // extern "C"

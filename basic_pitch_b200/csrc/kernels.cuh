@@ -325,6 +325,43 @@ void launch_stream_scan(const float* note, long long flag_from, long long n, int
 void launch_stream_compact(const int* count, const int* s_start, const int* s_end, const int* s_pitch, int keep_lo,
                            int keep_hi, int frame0, long long base, int* start, int* end, int* pitch, long long* note_base,
                            int* kept, cudaStream_t st);
+// Stream group (csrc/stream_group.cu).  A copy of rows between arenas: up to four arrays of 4- or 1-byte elements,
+// `width` elements per row; segment k copies rows of array arr.
+struct GroupCopyArrays {
+  const void* src[4];
+  void* dst[4];
+  int width[4];
+  int bytes[4];
+};
+struct GroupCopySeg {
+  long long src_row, dst_row, rows;
+  int arr, pad;
+};
+// max_elems: the most elements (rows x width) any segment copies
+void launch_group_copy(const GroupCopySeg* segs, int n_segs, long long max_elems, const GroupCopyArrays& a,
+                       cudaStream_t st);
+// The 142 kept frames of every window of a forward chunk (unwrapped into pm / cm at frames w * 142 .., frame stride
+// `stride`) to rows dst_row[w] .. of the row-major note / onset (/ contour) arenas.
+void launch_group_unwrap(const float* pm_note, const float* pm_onset, const float* cm, long long stride,
+                         const long long* dst_row, int n_windows, float* note, float* onset, float* contour,
+                         bool with_contour, cudaStream_t st);
+// launch_stream_scan for many streams in one launch (blockIdx.y = job); frames are global, row = frame + shift of the
+// shared arenas `note` / `quiet`; out[2 j], out[2 j + 1] as out[0], out[1] of launch_stream_scan; done[n_jobs].
+struct GroupScanJob {
+  long long shift, flag_from, n, from, last;
+};
+void launch_group_scan(const GroupScanJob* jobs, int n_jobs, long long max_rows, const float* note, int lo, int hi,
+                       double frame_thresh, unsigned char* quiet, long long w, long long* out, unsigned int* done,
+                       cudaStream_t st);
+// launch_stream_compact for a batch of decoded segments (file j of the decode): its notes are written from
+// note_off[j] on, note_off[0 .. n_segs] the running sum of the kept counts.
+struct GroupKeep {
+  int keep_lo, keep_hi, frame0, pad;
+  long long base;
+};
+void launch_group_compact(const GroupKeep* keep, int n_segs, const long long* slot_off, const int* count,
+                          const int* s_start, const int* s_end, const int* s_pitch, int* start, int* end, int* pitch,
+                          long long* note_base, int* note_off, cudaStream_t st);
 // Grid decode: a chunk of parameter sets ("settings") over one batch.  The cell-parallel kernels run once per group of
 // settings that share their inputs (blockIdx.y = group); the sequential loops once per (file, setting).
 struct DecodePrepGroup {  // a distinct pitch range (lo, hi): constrained frames, per-file max(onsets) / max(frame_diff)

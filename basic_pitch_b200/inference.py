@@ -16,7 +16,7 @@ import enum
 import json
 import os
 import pathlib
-from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, Iterable, List, Mapping, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -303,6 +303,15 @@ class Model:
         lo, hi = infer.frequency_to_column_range(min_freq, max_freq)
         p = self._params(onset_thresh, frame_thresh, min_note_len, 11, True, melodia_trick, include_pitch_bends, lo, hi)
         return NoteStream(self, p, max_segment_frames)
+
+    def stream_group(self, onset_thresh=0.5, frame_thresh=0.3, min_note_len=11, min_freq: Optional[float] = None,
+                     max_freq: Optional[float] = None, melodia_trick=True, include_pitch_bends=True,
+                     max_segment_frames: Optional[int] = None) -> "StreamGroup":
+        """Many streamed recordings with one set of note settings (`bp_stream_group_*`, include/bp_b200.h), each push
+        served by one device pass over all of them; arguments as `note_stream`, whose notes every stream's equal."""
+        lo, hi = infer.frequency_to_column_range(min_freq, max_freq)
+        p = self._params(onset_thresh, frame_thresh, min_note_len, 11, True, melodia_trick, include_pitch_bends, lo, hi)
+        return StreamGroup(self, p, max_segment_frames)
 
     @staticmethod
     def _cat_note_onset(notes, onsets):
@@ -1074,15 +1083,121 @@ class NoteStream:
 
     def _take(self) -> List[infer.NoteEvent]:
         arrs = self._model._with_capacity(1, 0, lambda nt: self._lib.bp_stream_take(self._h, C.byref(nt)))
-        n = int(arrs["note_off"][1])
-        start, end = arrs["start"][:n], arrs["end"][:n]
-        t0, t1 = infer.frame_index_to_time(start.astype(np.int64)), infer.frame_index_to_time(end.astype(np.int64))
-        off, flat = arrs["bend_off"], arrs["bends"]
-        return [
-            (t0[j], t1[j], np.int64(arrs["pitch"][j]), np.float32(arrs["amp"][j]),
-             list(flat[off[j] : off[j + 1]].astype(np.int64)) if self._bends else None)
-            for j in range(n)
-        ]  # fmt: skip
+        return _note_events(arrs, 0, int(arrs["note_off"][1]), self._bends)
+
+
+def _note_events(arrs, a: int, b: int, bends: bool) -> List[infer.NoteEvent]:
+    """Notes a .. b of taken note arrays (global frame indices) -> the reference's event tuples."""
+    start, end = arrs["start"][a:b], arrs["end"][a:b]
+    t0, t1 = infer.frame_index_to_time(start.astype(np.int64)), infer.frame_index_to_time(end.astype(np.int64))
+    off, flat = arrs["bend_off"], arrs["bends"]
+    return [
+        (t0[j - a], t1[j - a], np.int64(arrs["pitch"][j]), np.float32(arrs["amp"][j]),
+         list(flat[off[j] : off[j + 1]].astype(np.int64)) if bends else None)
+        for j in range(a, b)
+    ]  # fmt: skip
+
+
+class StreamGroup:
+    """Many streamed recordings decoded together (`Model.stream_group`, `bp_stream_group_*`): each call serves every
+    stream it lists with one device pass — one forward pass over the windows the new audio completes, one quiet scan,
+    and the closed stretches of all streams decoded as one batch per round.  Every stream's notes are those a
+    `NoteStream` (and `predict_stream_notes`) gives for the same recording on its own.
+
+    `open()` adds a stream and returns its id.  `push({id: block})` takes the next mono 22 050 Hz audio block of some
+    streams (any length, 0 included), `push_frames({id: (note, onset, contour)})` posteriorgrams instead (a stream takes
+    one kind only), `end(ids)` closes streams.  Each returns {id: note_events} for the streams it lists, the events that
+    became final; with `with_posteriorgrams` also {id: model_output_part}, the frames each stream committed in that call
+    (concatenated, `run_inference_stream`'s output for the stream's blocks).  `held_frames(id)` is what
+    `NoteStream.held_frames` reports."""
+
+    def __init__(self, model: Model, params: _lib.DecodeParams, max_segment_frames: Optional[int] = None):
+        self._model, self._lib = model, model._lib
+        self._bends = bool(params.include_pitch_bends)
+        self._h = C.c_void_p()
+        self._lib.bp_stream_group_create(model.handle, C.byref(params), int(max_segment_frames or 0), C.byref(self._h))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h and getattr(self, "_lib", None) is not None:
+            try:
+                self._lib.bp_stream_group_destroy(h)
+            except Exception:
+                pass
+
+    def open(self) -> int:
+        i = C.c_int32(0)
+        self._lib.bp_stream_group_open(self._h, C.byref(i))
+        return int(i.value)
+
+    def held_frames(self, stream_id: int) -> int:
+        return int(self._lib.bp_stream_group_held_frames(self._h, int(stream_id)))
+
+    @staticmethod
+    def _ids(ids) -> np.ndarray:
+        return np.ascontiguousarray(np.asarray(list(ids), dtype=np.int64).reshape(-1).astype(np.int32))
+
+    def _call(self, ids: np.ndarray, call, n_samples, with_posteriorgrams: bool):
+        """call(note, onset, contour, frame_off) with output arrays sized by bp_stream_group_commit_offsets."""
+        n = len(ids)
+        off = np.zeros(n + 1, np.int64)
+        outs = [None, None, None]
+        if with_posteriorgrams:
+            self._lib.bp_stream_group_commit_offsets(self._h, n, _ptr(ids), _ptr(n_samples), int(n_samples is None),
+                                                     _ptr(off))
+            total = int(off[-1])
+            outs = [np.empty((total, w), _F32) for w in (N_FREQ_BINS_NOTES, N_FREQ_BINS_NOTES, N_FREQ_BINS_CONTOURS)]
+        call(*(_ptr(o) for o in outs), _ptr(off))
+        events = self._take(ids)
+        if not with_posteriorgrams:
+            return events
+        parts = {int(i): {k: o[off[j] : off[j + 1]] for k, o in zip(("note", "onset", "contour"), outs)}
+                 for j, i in enumerate(ids)}  # fmt: skip
+        return events, parts
+
+    def push(self, blocks: Mapping[int, np.ndarray], with_posteriorgrams: bool = False):
+        ids = self._ids(blocks.keys())
+        audio = [np.ascontiguousarray(np.asarray(b, dtype=_F32).reshape(-1)) for b in blocks.values()]
+        ptrs = (C.c_void_p * max(len(audio), 1))(*[a.ctypes.data for a in audio])
+        lens = np.array([a.shape[0] for a in audio], np.int64)
+        return self._call(
+            ids, lambda no, on, co, off: self._lib.bp_stream_group_push_host(self._h, len(ids), _ptr(ids), ptrs, _ptr(lens),
+                                                                            no, on, co, off),
+            lens, with_posteriorgrams)
+
+    def push_frames(self, frames: Mapping[int, Tuple[np.ndarray, np.ndarray, Optional[np.ndarray]]]):
+        ids = self._ids(frames.keys())
+        keep, rows = [], []
+        for note, onset, contour in frames.values():
+            note = np.ascontiguousarray(note, dtype=_F32).reshape(-1, N_FREQ_BINS_NOTES)
+            onset = np.ascontiguousarray(onset, dtype=_F32).reshape(-1, N_FREQ_BINS_NOTES)
+            if onset.shape != note.shape:
+                raise ValueError("note and onset posteriorgrams must be (T, 88) and of equal shape")
+            if contour is not None:
+                contour = np.ascontiguousarray(contour, dtype=_F32).reshape(-1, N_FREQ_BINS_CONTOURS)
+                if contour.shape[0] != note.shape[0]:
+                    raise ValueError("contour posteriorgrams must have as many frames as note posteriorgrams")
+            elif self._bends:
+                raise ValueError("pitch bends need the contour posteriorgram")
+            keep.append((note, onset, contour))
+            rows.append(note.shape[0])
+        n = max(len(keep), 1)
+        ptrs = [(C.c_void_p * n)(*[_ptr(k[c]) for k in keep]) for c in range(3)]
+        lens = np.array(rows, np.int64)
+        self._lib.bp_stream_group_push_frames_host(self._h, len(ids), _ptr(ids), *ptrs, _ptr(lens))
+        return self._take(ids)
+
+    def end(self, ids: Iterable[int], with_posteriorgrams: bool = False):
+        ids = self._ids(ids)
+        return self._call(ids, lambda no, on, co, off: self._lib.bp_stream_group_end(self._h, len(ids), _ptr(ids), no, on,
+                                                                                    co, off),
+                          None, with_posteriorgrams)
+
+    def _take(self, ids: np.ndarray) -> Dict[int, List[infer.NoteEvent]]:
+        arrs = self._model._with_capacity(
+            len(ids), 0, lambda nt: self._lib.bp_stream_group_take(self._h, len(ids), _ptr(ids), C.byref(nt)))
+        off = arrs["note_off"]
+        return {int(i): _note_events(arrs, int(off[j]), int(off[j + 1]), self._bends) for j, i in enumerate(ids)}
 
 
 def default_model(model_path: Union[pathlib.Path, str] = ICASSP_2022_MODEL_PATH, device: Optional[int] = None) -> Model:
@@ -1261,6 +1376,36 @@ def predict_stream_notes(audio_blocks: Iterable[np.ndarray],
         yield part, stream.push(part["note"], part["onset"], part["contour"])
     widths = {"note": N_FREQ_BINS_NOTES, "onset": N_FREQ_BINS_NOTES, "contour": N_FREQ_BINS_CONTOURS}
     yield {k: np.zeros((0, w), _F32) for k, w in widths.items()}, stream.end()
+
+
+def predict_streams_notes(audio_streams: Sequence[Iterable[np.ndarray]],
+                          model_or_model_path: Union["Model", pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
+                          onset_threshold: float = DEFAULT_ONSET_THRESHOLD, frame_threshold: float = DEFAULT_FRAME_THRESHOLD,
+                          minimum_note_length: float = DEFAULT_MINIMUM_NOTE_LENGTH_MS,
+                          minimum_frequency: Optional[float] = None, maximum_frequency: Optional[float] = None,
+                          melodia_trick: bool = True, max_segment_seconds: Optional[float] = None):
+    """`predict_stream_notes` for many live recordings at once (`Model.stream_group`): each step pulls one block from
+    every iterator that has not ended, pushes them together, ends the recordings whose iterator is exhausted and yields
+    {index: note_events} for the recordings it served.  Every recording's events, concatenated over the steps, equal
+    `predict_stream_notes`' on its blocks alone; the keyword arguments are that function's."""
+    model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
+    min_note_len = int(np.round(minimum_note_length / 1000 * (AUDIO_SAMPLE_RATE / FFT_HOP)))
+    max_seg = None if max_segment_seconds is None else max(1, int(np.round(max_segment_seconds * AUDIO_SAMPLE_RATE / FFT_HOP)))
+    group = model.stream_group(onset_threshold, frame_threshold, min_note_len, minimum_frequency, maximum_frequency,
+                               melodia_trick, True, max_seg)
+    live = {group.open(): (k, iter(it)) for k, it in enumerate(audio_streams)}
+    while live:
+        blocks, done = {}, []
+        for sid, (_, it) in live.items():
+            try:
+                blocks[sid] = next(it)
+            except StopIteration:
+                done.append(sid)
+        events = group.push(blocks) if blocks else {}
+        events.update(group.end(done) if done else {})
+        yield {live[sid][0]: ev for sid, ev in events.items()}
+        for sid in done:
+            del live[sid]
 
 
 class OutputExtensions(enum.Enum):

@@ -189,6 +189,49 @@ int bp_stream_take(bp_stream_t* s, bp_notes_t* notes);
 int64_t bp_stream_held_frames(const bp_stream_t* s);
 void bp_stream_destroy(bp_stream_t* s);
 
+/* ---- many streamed recordings at once (stream group) ----------------------------------------------------------------
+ * A group holds any number of streams with one set of decode params and M, each decoded by exactly the rules of
+ * bp_stream_* above, and serves every stream listed in a call with one device pass: the new samples go up in one copy,
+ * the windows they complete run through one forward pass (one launch chain per bp_model_chunk_windows windows), the
+ * frames stay on the device, one quiet scan covers every stream and the closed segments are decoded in rounds, one
+ * segment per stream per round, as one batch.  A stream's notes are those bp_stream_* gives for the same frames whatever
+ * the push schedule (DESIGN.md §4.6), and the frames of an audio stream are those run_inference_stream yields for its
+ * blocks.  Streams are named by the ids bp_stream_group_open returns; a call lists each at most once.  BP_E_INVALID for
+ * an unknown or ended id, an id listed twice, a negative length, a NULL block of nonzero length, and a stream given
+ * audio after posteriorgrams or the reverse.  The group uses its model's device and stream and must be destroyed before
+ * it; it keeps no model workspace between calls.
+ * bp_stream_group_push_host: the next block of each listed stream, mono float32 at 22 050 Hz (any length, 0 included).
+ *   Frames a stream commits: those of its windows except the newest two (whose frames the final trim of unwrap_output
+ *   can reach), and at its end bp_num_frames(samples) in all.  h_note / h_onset / h_contour (each may be NULL) receive
+ *   the frames each listed stream committed in this call, row-major, stream i's from row h_frame_off[i] on
+ *   (h_frame_off[n + 1], may be NULL; bp_stream_group_commit_offsets gives the same offsets before the call).
+ * bp_stream_group_end: the listed streams have ended: their last windows run (zero-padded), and their open segments are
+ *   decoded with the end-of-file rules; posteriorgram outputs as a push.
+ * bp_stream_group_push_frames_host: posteriorgrams instead of audio, as bp_stream_push_host takes them, n_frames[i]
+ *   rows for stream i (h_contour may be NULL when !include_pitch_bends).
+ * bp_stream_group_commit_offsets: h_frame_off[n + 1] of a push of n_samples[i] samples (ending != 0: of the end).
+ * bp_stream_group_take: moves the finished notes of the listed streams out, stream i's at note_off[i] .. note_off[i + 1]
+ *   (note_off[n + 1]), each as bp_stream_take; ended streams may be listed.  BP_E_CAPACITY (bp_last_required) leaves
+ *   them queued.
+ * bp_stream_group_held_frames: as bp_stream_held_frames (0 for an unknown id). */
+typedef struct bp_stream_group bp_stream_group_t;
+int bp_stream_group_create(bp_model_t* m, const bp_decode_params_t* params, int64_t max_segment_frames,
+                           bp_stream_group_t** out);
+int bp_stream_group_open(bp_stream_group_t* g, int32_t* id);
+int bp_stream_group_commit_offsets(const bp_stream_group_t* g, int32_t n, const int32_t* ids, const int64_t* n_samples,
+                                   int32_t ending, int64_t* h_frame_off);
+int bp_stream_group_push_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const float* const* audio,
+                              const int64_t* n_samples, float* h_note, float* h_onset, float* h_contour,
+                              int64_t* h_frame_off);
+int bp_stream_group_push_frames_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const float* const* h_note,
+                                     const float* const* h_onset, const float* const* h_contour,
+                                     const int64_t* n_frames);
+int bp_stream_group_end(bp_stream_group_t* g, int32_t n, const int32_t* ids, float* h_note, float* h_onset,
+                        float* h_contour, int64_t* h_frame_off);
+int bp_stream_group_take(bp_stream_group_t* g, int32_t n, const int32_t* ids, bp_notes_t* notes);
+int64_t bp_stream_group_held_frames(const bp_stream_group_t* g, int32_t id);
+void bp_stream_group_destroy(bp_stream_group_t* g);
+
 /* ---- stage 3 under a grid of decode parameters ------------------------------------------------
  * reference: note_creation.py:52-111 (model_output_to_notes without the MIDI object), called once per parameter set.
  * One call decodes the batch under each of params[0 .. n_params): every (setting, file) gets exactly the notes
