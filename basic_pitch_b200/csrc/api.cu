@@ -4430,7 +4430,16 @@ struct GroupStream {
   std::vector<int32_t> q_start, q_end, q_pitch, q_bends;  // finished notes not yet taken
   std::vector<float> q_amp;
   std::vector<int32_t> q_bend_off{0};
+  // Opened with bp_stream_group_open_pcm (any capture format but mono float32 at 22 050 Hz): the stream's PCM frames
+  // pushed so far, and the down-mixed inputs [hist_lo, frames) its next outputs read, in hist[hcur].  Plain streams
+  // pushed with bp_stream_group_push_pcm_host use `geo` too: the identity ingest of mono float32 at 22 050 Hz.
+  bool pcm = false;
+  IngestFile geo{};
+  long long frames = 0, hist_lo = 0;
+  DevBuf<float> hist[2];
+  int hcur = 0;
   long long shift() const { return row0 - hb; }
+  long long in_frames() const { return pcm ? frames : samples; }  // inputs of the ingest pushed so far
 };
 
 struct bp_stream_group {
@@ -4453,6 +4462,7 @@ struct bp_stream_group {
   DevBuf<WinDesc> wd;
   DevBuf<UnwrapDesc> ud;
   DevBuf<float> b_note, b_onset, stage;  // the decode batch; uploads and posteriorgram outputs
+  DevBuf<unsigned char> pcm_stage;       // a PCM push: stream ingest descriptors, then the blocks as stored
   DevBuf<unsigned int> b_max_onset;
   DevBuf<unsigned long long> b_max_fd;
   DevBuf<int> note_off;
@@ -4468,6 +4478,8 @@ struct bp_stream_group {
       quiet[k].release();
     }
     for (auto* b : {&b_note, &b_onset, &stage}) b->release();
+    pcm_stage.release();
+    for (GroupStream& x : s) x.hist[0].release(), x.hist[1].release();
     max_onset.release(), done.release(), b_max_onset.release();
     max_fd.release(), b_max_fd.release();
     scan_out.release(), dst_row.release();
@@ -4589,11 +4601,12 @@ long long group_committed(long long samples, long long windows, bool ending) {
   return ending ? bp_num_frames(samples) : std::max<long long>(0, (windows - 2) * kHopFrames);
 }
 
+int group_run(bp_stream_group* g, const std::vector<int>& ids, const int64_t* len, bool ending, cudaStream_t st);
+
 // Appends the blocks to the tails, runs the windows they complete (all remaining windows when `ending`) through the
 // forward pass into the frame arena and commits the frames run_inference_stream would have yielded by now.
 int group_audio(bp_stream_group* g, const std::vector<int>& ids, const float* const* audio, const int64_t* len,
                 bool ending, cudaStream_t st) {
-  bp_model* m = g->m;
   std::vector<long long> need(g->s.size(), 0);
   long long total = 0;
   for (size_t i = 0; i < ids.size(); ++i) need[ids[i]] = len ? len[i] : 0, total += len ? len[i] : 0;
@@ -4616,13 +4629,19 @@ int group_audio(bp_stream_group* g, const std::vector<int>& ids, const float* co
     rc = group_copy(g, segs, GroupCopyArrays{{g->stage.p}, {g->audio[g->acur].p}, {1}, {4}}, st);
     if (rc) return rc;
   }
-  std::fill(need.begin(), need.end(), 0);
+  return group_run(g, ids, len, ending, st);
+}
+
+// After len[i] samples were appended to the tail of stream ids[i] (NULL: none): runs the windows they complete.
+int group_run(bp_stream_group* g, const std::vector<int>& ids, const int64_t* len, bool ending, cudaStream_t st) {
+  bp_model* m = g->m;
+  std::vector<long long> need(g->s.size(), 0);
   for (size_t i = 0; i < ids.size(); ++i) {
     GroupStream& x = g->s[ids[i]];
     x.samples += len ? len[i] : 0;
     need[ids[i]] = (group_windows(x.samples, ending) - x.win_done) * kHopFrames;
   }
-  rc = group_frame_room(g, need, st);
+  int rc = group_frame_room(g, need, st);
   if (rc) return rc;
   std::vector<WinDesc> wd;
   std::vector<UnwrapDesc> ud;
@@ -4677,6 +4696,95 @@ int group_audio(bp_stream_group* g, const std::vector<int>& ids, const float* co
   }
   m->last_forward_n = nbmax == nwin ? nwin : 0;
   return BP_OK;
+}
+
+// The ingest step of each listed stream in a PCM push of frames[i] frames (NULL: none; `ending`: the flush at its end).
+std::vector<PcmStep> group_pcm_steps(const bp_stream_group* g, const std::vector<int>& ids, const int64_t* frames,
+                                     bool ending) {
+  std::vector<PcmStep> step(ids.size());
+  for (size_t i = 0; i < ids.size(); ++i) {
+    const GroupStream& x = g->s[ids[i]];
+    step[i] = pcm_stream_step(x.geo, x.in_frames(), frames ? frames[i] : 0, ending);
+  }
+  return step;
+}
+
+// A PCM push (`ending`: the end of the streams, no new frames): the blocks go up as stored, in one copy behind their
+// descriptors, and one stream ingest launch writes each stream's new final 22 050 Hz samples straight to its tail and
+// its next history to its other history buffer; then the windows run as for a float push.
+int group_pcm(bp_stream_group* g, const std::string& api, const std::vector<int>& ids, const void* const* blocks,
+              const int64_t* frames, bool ending, cudaStream_t st) {
+  const std::vector<PcmStep> step = group_pcm_steps(g, ids, frames, ending);
+  std::vector<int64_t> add(ids.size());
+  std::vector<long long> need(g->s.size(), 0);
+  std::vector<size_t> use;  // the streams the launch serves
+  long long ctas = 0;
+  for (size_t i = 0; i < ids.size(); ++i) {
+    add[i] = step[i].out_hi - step[i].out_lo;
+    need[ids[i]] = add[i];
+    const bool new_hist = step[i].hist_hi > step[i].hist_lo && (frames && frames[i] > 0);
+    if (add[i] > 0 || new_hist) {
+      use.push_back(i);
+      ctas += ingest_ctas(add[i]) + (new_hist ? 1 : 0);
+    }
+  }
+  if (ctas > INT_MAX) return fail(BP_E_INVALID, api + ": the blocks are too long for one ingest");
+  int rc = group_audio_room(g, need, st);
+  if (rc) return rc;
+  if (!use.empty()) {
+    const int nd = (int)use.size();
+    std::vector<int64_t> at(nd);  // descriptors [nd], the CTA prefix [nd + 1], then each block on a 16-byte boundary
+    int64_t bytes = align16((int64_t)nd * (int64_t)sizeof(StreamIngest) + ((int64_t)nd + 1) * (int64_t)sizeof(int));
+    for (int j = 0; j < nd; ++j) {
+      const size_t i = use[j];
+      const IngestFile& f = g->s[ids[i]].geo;
+      at[j] = bytes;
+      if (frames && frames[i] > 0) bytes = align16(bytes + frames[i] * f.channels * kPcmSampleBytes[f.format]);
+    }
+    rc = stage_host(g, (size_t)bytes);
+    if (rc) return rc;
+    CK(g->pcm_stage.reserve((size_t)bytes));
+    std::vector<StreamIngest> d(nd);
+    int max_span = 1;
+    for (int j = 0; j < nd; ++j) {
+      const size_t i = use[j];
+      GroupStream& x = g->s[ids[i]];
+      StreamIngest& e = d[j];
+      e.f = x.geo;
+      const int64_t nb = frames ? frames[i] * x.geo.channels * kPcmSampleBytes[x.geo.format] : 0;
+      if (nb > 0) std::memcpy(g->h_stage + at[j], blocks[i], (size_t)nb);
+      e.f.pcm = g->pcm_stage.p + at[j];
+      e.f.n_in = step[i].hist_hi;
+      e.f.out = g->audio[g->acur].p + x.a_off + (x.samples - x.tail0);
+      e.f.n_out = add[i];
+      e.k0 = step[i].out_lo;
+      e.n_prev = x.in_frames();
+      e.hist_lo = x.hist_lo;
+      e.hist = x.hist[x.hcur].p;
+      e.hist_out = x.hist[x.hcur ^ 1].p;
+      e.new_hist_lo = (frames && frames[i] > 0) ? step[i].hist_lo : step[i].hist_hi;  // no new frames: history kept
+      if (add[i] > 0) max_span = std::max(max_span, e.f.span);
+    }
+    std::memcpy(g->h_stage, d.data(), sizeof(StreamIngest) * (size_t)nd);
+    int* cta_off = reinterpret_cast<int*>(g->h_stage + sizeof(StreamIngest) * (size_t)nd);
+    cta_off[0] = 0;
+    for (int j = 0; j < nd; ++j) cta_off[j + 1] = cta_off[j] + stream_ingest_ctas(d[j]);
+    CK(cudaMemcpyAsync(g->pcm_stage.p, g->h_stage, (size_t)bytes, cudaMemcpyHostToDevice, st));
+    if (launch_stream_ingest(reinterpret_cast<const StreamIngest*>(g->pcm_stage.p),
+                             reinterpret_cast<const int*>(g->pcm_stage.p + sizeof(StreamIngest) * (size_t)nd), nd,
+                             cta_off[nd], max_span, st))
+      return fail(BP_E_CUDA, api + ": stream ingest: " + cudaGetErrorString(cudaGetLastError()));
+    g->m->launches += 1;
+    for (int j = 0; j < nd; ++j)
+      if (d[j].f.n_in > d[j].new_hist_lo) g->s[ids[use[j]]].hcur ^= 1;
+  }
+  for (size_t i = 0; i < ids.size(); ++i) {
+    GroupStream& x = g->s[ids[i]];
+    if (!x.pcm) continue;
+    x.frames = step[i].hist_hi;
+    if (frames && frames[i] > 0) x.hist_lo = step[i].hist_lo;
+  }
+  return group_run(g, ids, add.data(), ending, st);
 }
 
 // Posteriorgram pushes: frames go to the arena and are committed at once.
@@ -4944,7 +5052,8 @@ int group_ids(const bp_stream_group* g, const std::string& api, int32_t n, const
   return BP_OK;
 }
 
-// Frames each listed stream commits in a push of n_samples[i] samples (NULL: none) or at its end: offsets [n + 1].
+// Frames each listed stream commits in a push of n_samples[i] samples (PCM frames for a PCM stream; NULL: none) or at its
+// end: offsets [n + 1].
 void group_offsets(const bp_stream_group* g, const std::vector<int>& ids, const int64_t* n_samples, bool ending,
                    int64_t* off) {
   off[0] = 0;
@@ -4952,7 +5061,8 @@ void group_offsets(const bp_stream_group* g, const std::vector<int>& ids, const 
     const GroupStream& x = g->s[ids[i]];
     long long c = x.n;
     if (x.kind != 2) {
-      const long long smp = x.samples + (n_samples ? n_samples[i] : 0);
+      const long long smp = x.pcm ? pcm_stream_step(x.geo, x.frames, n_samples ? n_samples[i] : 0, ending).out_hi
+                                  : x.samples + (n_samples ? n_samples[i] : 0);
       c = std::max(x.n, group_committed(smp, std::max(x.win_done, group_windows(smp, ending)), ending));
     }
     off[i + 1] = off[i] + (c - x.n);
@@ -4986,17 +5096,27 @@ int group_out(bp_stream_group* g, const std::vector<int>& ids, const std::vector
   return BP_OK;
 }
 
-// An audio push (ending: the streams' end, no new samples).
+// An audio push (ending: the streams' end, no new samples).  pcm_call: the blocks are PCM of each stream's format
+// (bp_stream_group_push_pcm_host), n_samples their frames; otherwise float32 at 22 050 Hz.
 int group_audio_step(bp_stream_group* g, const std::string& api, int32_t n, const int32_t* id_arr,
-                     const float* const* audio, const int64_t* n_samples, bool ending, float* h_note, float* h_onset,
-                     float* h_contour, int64_t* h_frame_off) {
+                     const void* const* audio, const int64_t* n_samples, bool pcm_call, bool ending, float* h_note,
+                     float* h_onset, float* h_contour, int64_t* h_frame_off) {
   std::vector<int> ids;
   int rc = group_ids(g, api, n, id_arr, ending ? 0 : 1, ids);
   if (rc) return rc;
+  bool any_pcm = pcm_call;
   for (int32_t i = 0; i < n && !ending; ++i) {
     if (!n_samples || n_samples[i] < 0) return fail(BP_E_INVALID, api + ": negative or missing n_samples");
     if (n_samples[i] > 0 && (!audio || !audio[i])) return fail(BP_E_INVALID, api + ": null audio block");
+    const GroupStream& x = g->s[ids[i]];
+    if (x.pcm && !pcm_call)
+      return fail(BP_E_INVALID, api + ": stream " + std::to_string(ids[i]) +
+                                    " takes PCM of its own format (bp_stream_group_push_pcm_host), not float32 at 22 050 Hz");
+    const int64_t frame_bytes = (int64_t)x.geo.channels * kPcmSampleBytes[x.geo.format];
+    if (pcm_call && n_samples[i] > (INT64_MAX >> 16) / frame_bytes)
+      return fail(BP_E_INVALID, api + ": the block of stream " + std::to_string(ids[i]) + " is too long");
   }
+  for (size_t i = 0; i < ids.size() && ending; ++i) any_pcm = any_pcm || g->s[ids[i]].pcm;
   std::vector<int64_t> off(ids.size() + 1);
   group_offsets(g, ids, ending ? nullptr : n_samples, ending, off.data());
   for (size_t i = 0; i < ids.size(); ++i)
@@ -5006,7 +5126,7 @@ int group_audio_step(bp_stream_group* g, const std::string& api, int32_t n, cons
   DeviceGuard dg(g->m->device);
   cudaStream_t st = g->m->stream;
   std::vector<int> audio_ids;  // streams whose frames come from the model
-  std::vector<const float*> blocks;
+  std::vector<const void*> blocks;
   std::vector<int64_t> lens;
   for (size_t i = 0; i < ids.size(); ++i) {
     GroupStream& x = g->s[ids[i]];
@@ -5018,7 +5138,10 @@ int group_audio_step(bp_stream_group* g, const std::string& api, int32_t n, cons
   }
   std::vector<long long> from;
   for (int id : ids) from.push_back(g->s[id].n);
-  rc = group_audio(g, audio_ids, blocks.data(), lens.data(), ending, st);
+  if (any_pcm)
+    rc = group_pcm(g, api, audio_ids, blocks.data(), ending ? nullptr : lens.data(), ending, st);
+  else
+    rc = group_audio(g, audio_ids, reinterpret_cast<const float* const*>(blocks.data()), lens.data(), ending, st);
   if (rc) return rc;
   rc = group_out(g, ids, from, off.data(), h_note, h_onset, h_contour, st);
   if (rc) return rc;
@@ -5086,8 +5209,81 @@ int bp_stream_group_open(bp_stream_group_t* g, int32_t* id) {
   CK(cudaStreamSynchronize(g->m->stream));
   GroupStream x;
   x.cuts.init(g->params, g->max_seg);
+  ingest_geometry(0, 1, kSampleRate, x.geo);  // the identity ingest, for PCM pushes that list plain streams
   g->s.push_back(std::move(x));
   *id = (int32_t)k;
+  return BP_OK;
+}
+
+int bp_stream_group_open_pcm(bp_stream_group_t* g, int32_t sample_format, int32_t channels, int32_t sample_rate,
+                             int32_t* id) {
+  const std::string api = "bp_stream_group_open_pcm";
+  if (!g || !id) return fail(BP_E_INVALID, api + ": bad argument");
+  if (sample_format < 0 || sample_format > 3)
+    return fail(BP_E_INVALID, api + ": sample_format must be 0 (float32), 1 (int16), 2 (int32) or 3 (uint8)");
+  if (channels < 1) return fail(BP_E_INVALID, api + ": channels must be >= 1");
+  if (sample_rate < 1) return fail(BP_E_INVALID, api + ": sample_rate must be >= 1");
+  IngestFile f{};
+  if (ingest_geometry(sample_format, channels, sample_rate, f) != 0)
+    return fail(BP_E_INVALID, api + ": the ratio of " + std::to_string(sample_rate) +
+                                  " Hz to 22 050 Hz is beyond the resampler's shared-memory limit (~100:1)");
+  DeviceGuard dg(g->m->device);
+  std::vector<IngestFile> one{f};
+  int rc = load_ingest_taps(api, g->m->device, one);
+  if (rc) return rc;
+  DevBuf<float> hist[2];  // at most taps - 1 held inputs (DESIGN.md §4.6)
+  for (DevBuf<float>& h : hist) {
+    if (h.reserve((size_t)f.taps) != cudaSuccess) {
+      hist[0].release(), hist[1].release();
+      return fail(BP_E_CUDA, api + ": could not allocate the stream's history");
+    }
+  }
+  rc = bp_stream_group_open(g, id);
+  if (rc) {
+    hist[0].release(), hist[1].release();
+    return rc;
+  }
+  GroupStream& x = g->s[*id];
+  x.geo = one[0];
+  x.pcm = !(sample_format == 0 && channels == 1 && sample_rate == kSampleRate);
+  x.kind = 1;
+  x.hist[0] = hist[0], x.hist[1] = hist[1];
+  return BP_OK;
+}
+
+int bp_stream_group_debug_tail(const bp_stream_group_t* g, int32_t id, float* h_out, int64_t capacity,
+                               int64_t* first_sample, int64_t* n) {
+  const std::string api = "bp_stream_group_debug_tail";
+  if (!g || id < 0 || (size_t)id >= g->s.size() || !first_sample || !n) return fail(BP_E_INVALID, api + ": bad argument");
+  const GroupStream& x = g->s[id];
+  *first_sample = x.tail0;
+  *n = x.samples - x.tail0;
+  if (*n > capacity) return fail(BP_E_CAPACITY, api + ": capacity too small, need " + std::to_string(*n) + " samples");
+  if (*n == 0) return BP_OK;
+  if (!h_out) return fail(BP_E_INVALID, api + ": bad argument");
+  DeviceGuard dg(g->m->device);
+  CK(cudaMemcpyAsync(h_out, g->audio[g->acur].p + x.a_off, sizeof(float) * (size_t)*n, cudaMemcpyDeviceToHost,
+                     g->m->stream));
+  CK(cudaStreamSynchronize(g->m->stream));
+  return BP_OK;
+}
+
+int bp_debug_pcm_stream_plan(int32_t sample_format, int32_t channels, int32_t sample_rate, int32_t n_pushes,
+                             const int64_t* frames, int32_t ending, int64_t* out_lo, int64_t* out_hi, int64_t* hist_lo,
+                             int64_t* hist_hi) {
+  const std::string api = "bp_debug_pcm_stream_plan";
+  IngestFile f{};
+  if (n_pushes < 0 || (n_pushes > 0 && !frames) || !out_lo || !out_hi || !hist_lo || !hist_hi ||
+      ingest_geometry(sample_format, channels, sample_rate, f) != 0)
+    return fail(BP_E_INVALID, api + ": bad argument");
+  long long n = 0;
+  for (int32_t p = 0; p <= n_pushes; ++p) {
+    if (p == n_pushes && !ending) break;
+    if (p < n_pushes && frames[p] < 0) return fail(BP_E_INVALID, api + ": negative block length");
+    const PcmStep s = pcm_stream_step(f, n, p < n_pushes ? frames[p] : 0, p == n_pushes);
+    out_lo[p] = s.out_lo, out_hi[p] = s.out_hi, hist_lo[p] = s.hist_lo, hist_hi[p] = s.hist_hi;
+    n = s.hist_hi;
+  }
   return BP_OK;
 }
 
@@ -5107,13 +5303,20 @@ int bp_stream_group_commit_offsets(const bp_stream_group_t* g, int32_t n, const 
 int bp_stream_group_push_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const float* const* audio,
                               const int64_t* n_samples, float* h_note, float* h_onset, float* h_contour,
                               int64_t* h_frame_off) {
-  return group_audio_step(g, "bp_stream_group_push_host", n, ids, audio, n_samples, false, h_note, h_onset, h_contour,
-                          h_frame_off);
+  return group_audio_step(g, "bp_stream_group_push_host", n, ids, reinterpret_cast<const void* const*>(audio), n_samples,
+                          false, false, h_note, h_onset, h_contour, h_frame_off);
+}
+
+int bp_stream_group_push_pcm_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const void* const* pcm,
+                                  const int64_t* n_frames, float* h_note, float* h_onset, float* h_contour,
+                                  int64_t* h_frame_off) {
+  return group_audio_step(g, "bp_stream_group_push_pcm_host", n, ids, pcm, n_frames, true, false, h_note, h_onset,
+                          h_contour, h_frame_off);
 }
 
 int bp_stream_group_end(bp_stream_group_t* g, int32_t n, const int32_t* ids, float* h_note, float* h_onset,
                         float* h_contour, int64_t* h_frame_off) {
-  return group_audio_step(g, "bp_stream_group_end", n, ids, nullptr, nullptr, true, h_note, h_onset, h_contour,
+  return group_audio_step(g, "bp_stream_group_end", n, ids, nullptr, nullptr, false, true, h_note, h_onset, h_contour,
                           h_frame_off);
 }
 

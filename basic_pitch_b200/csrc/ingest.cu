@@ -140,8 +140,29 @@ __device__ __forceinline__ float mono_sample(const T* pcm, long long i, int chan
   return __double2float_rn(__ddiv_rn((double)__fadd_rn(0.f, s), (double)channels));
 }
 
-// The work of one CTA, shared by both kernels so that a file has the same bits whichever launched it: outputs
-// [cta * 256, cta * 256 + 256) of one file from its inputs staged (converted and down-mixed) in s_x.
+// Output k of a resampled signal (up, down not both 1) from inputs staged in s_x, s_x[t] = x[i_lo + t]: the one dot
+// product of every ingest kernel, so that an output has the same bits whichever kernel computed it and wherever its
+// inputs were staged from.
+__device__ __forceinline__ float resample_output(const float* s_x, long long i_lo, long long k, int up, int down,
+                                                 int half, int taps, const float* __restrict__ hp) {
+  const long long t0 = k * down + half;
+  const int p = (int)(t0 % up);
+  const int newest = (int)(t0 / up - i_lo);  // index of x[i_max] in the staged span
+  const float* h = hp + (size_t)p * taps;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;  // four partial sums: shorter dependency chains, smaller rounding error
+  int j = 0;
+  for (; j + 4 <= taps; j += 4) {
+    a0 = fmaf(__ldg(h + j), s_x[newest - j], a0);
+    a1 = fmaf(__ldg(h + j + 1), s_x[newest - j - 1], a1);
+    a2 = fmaf(__ldg(h + j + 2), s_x[newest - j - 2], a2);
+    a3 = fmaf(__ldg(h + j + 3), s_x[newest - j - 3], a3);
+  }
+  for (; j < taps; ++j) a0 = fmaf(__ldg(h + j), s_x[newest - j], a0);
+  return (a0 + a1) + (a2 + a3);
+}
+
+// The work of one CTA, shared by both whole-file kernels so that a file has the same bits whichever launched it:
+// outputs [cta * 256, cta * 256 + 256) of one file from its inputs staged (converted and down-mixed) in s_x.
 template <typename T>
 __device__ __forceinline__ void ingest_cta(const T* __restrict__ pcm, long long n_in, int channels, int up, int down,
                                            int half, int taps, const float* __restrict__ hp, float* __restrict__ out,
@@ -160,20 +181,7 @@ __device__ __forceinline__ void ingest_cta(const T* __restrict__ pcm, long long 
     out[k] = s_x[(int)(k - i_lo)];
     return;
   }
-  const long long t0 = k * down + half;
-  const int p = (int)(t0 % up);
-  const int newest = (int)(t0 / up - i_lo);  // index of x[i_max] in the staged span
-  const float* h = hp + (size_t)p * taps;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;  // four partial sums: shorter dependency chains, smaller rounding error
-  int j = 0;
-  for (; j + 4 <= taps; j += 4) {
-    a0 = fmaf(__ldg(h + j), s_x[newest - j], a0);
-    a1 = fmaf(__ldg(h + j + 1), s_x[newest - j - 1], a1);
-    a2 = fmaf(__ldg(h + j + 2), s_x[newest - j - 2], a2);
-    a3 = fmaf(__ldg(h + j + 3), s_x[newest - j - 3], a3);
-  }
-  for (; j < taps; ++j) a0 = fmaf(__ldg(h + j), s_x[newest - j], a0);
-  out[k] = (a0 + a1) + (a2 + a3);
+  out[k] = resample_output(s_x, i_lo, k, up, down, half, taps, hp);
 }
 
 template <typename T>
@@ -211,6 +219,61 @@ __global__ void __launch_bounds__(kOutPerCta) ingest_batch_kernel(const IngestFi
   }
 #undef BP_INGEST_CTA
 }
+
+// Input i of a live stream in the push `d` describes: zero before the recording, the held history below n_prev, the new
+// block (converted and down-mixed as the whole-file kernels do it) below n_in, zero from there (read only at the end).
+template <typename T>
+__device__ __forceinline__ float stream_input(const StreamIngest& d, long long i) {
+  if (i < d.hist_lo) return 0.f;  // i < 0: no output reads an input before the history otherwise
+  if (i < d.n_prev) return d.hist[i - d.hist_lo];
+  if (i < d.f.n_in) return mono_sample<T>(static_cast<const T*>(d.f.pcm), i - d.n_prev, d.f.channels);
+  return 0.f;
+}
+
+// CTA `cta` of one stream's push: outputs [k0 + 256 cta, k0 + 256 cta + 256) of the push, or, as the stream's last CTA,
+// the history it keeps for the next push, into the other history buffer (the output CTAs still read this one).
+template <typename T>
+__device__ __forceinline__ void stream_ingest_cta(const StreamIngest& d, long long cta, float* s_x) {
+  const IngestFile& f = d.f;
+  const long long out_ctas = (f.n_out + kOutPerCta - 1) / kOutPerCta;
+  if (cta == out_ctas) {
+    for (long long i = d.new_hist_lo + threadIdx.x; i < f.n_in; i += kOutPerCta)
+      d.hist_out[i - d.new_hist_lo] = stream_input<T>(d, i);
+    return;
+  }
+  const long long k0 = d.k0 + cta * kOutPerCta;
+  const long long i_lo = (k0 * f.down + f.half) / f.up - (f.taps - 1);  // as ingest_cta, from this CTA's first output
+  for (int t = threadIdx.x; t < f.span; t += kOutPerCta) s_x[t] = stream_input<T>(d, i_lo + t);
+  __syncthreads();
+  const long long k = k0 + threadIdx.x;
+  if (k >= d.k0 + f.n_out) return;
+  f.out[k - d.k0] = (f.up == 1 && f.down == 1) ? s_x[(int)(k - i_lo)] : resample_output(s_x, i_lo, k, f.up, f.down, f.half, f.taps, f.hp);
+}
+
+// One push of many live streams: stream i owns CTAs [cta_off[i], cta_off[i + 1]).
+__global__ void __launch_bounds__(kOutPerCta) stream_ingest_kernel(const StreamIngest* __restrict__ streams,
+                                                                   const int* __restrict__ cta_off, int n_streams) {
+  extern __shared__ float s_x[];
+  const int b = blockIdx.x;
+  int lo = 0, hi = n_streams;  // cta_off[lo] <= b < cta_off[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (cta_off[mid] <= b)
+      lo = mid;
+    else
+      hi = mid;
+  }
+  const StreamIngest& d = streams[lo];
+  const long long cta = b - cta_off[lo];
+  switch (d.f.format) {
+    case 0: stream_ingest_cta<float>(d, cta, s_x); break;
+    case 1: stream_ingest_cta<short>(d, cta, s_x); break;
+    case 2: stream_ingest_cta<int>(d, cta, s_x); break;
+    default: stream_ingest_cta<unsigned char>(d, cta, s_x); break;
+  }
+}
+
+long long ceil_div_ll(long long a, long long b) { return a >= 0 ? (a + b - 1) / b : -((-a) / b); }
 
 long long gcd_ll(long long a, long long b) {
   while (b) {
@@ -317,6 +380,33 @@ int launch_ingest_batch(const IngestFile* d_files, const int* d_cta_off, int n_f
   const size_t smem = (size_t)max_span * sizeof(float);
   if (smem > 48 * 1024) cudaFuncSetAttribute(ingest_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   ingest_batch_kernel<<<(unsigned)n_ctas, kOutPerCta, smem, st>>>(d_files, d_cta_off, n_files);
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// Output k reads inputs i_max(k) - T + 1 .. i_max(k), i_max(k) = floor((k down + half) / up); after n frames the outputs
+// k < F(n) = max(0, ceil((n up - half) / down)) read only inputs that have arrived.
+PcmStep pcm_stream_step(const IngestFile& f, long long n, long long add, bool ending) {
+  const auto final_outputs = [&](long long frames) {
+    return std::max(0LL, ceil_div_ll(frames * f.up - f.half, f.down));
+  };
+  PcmStep s;
+  s.out_lo = final_outputs(n);
+  s.out_hi = ending ? ceil_div_ll((n + add) * f.up, f.down) : final_outputs(n + add);
+  s.hist_hi = n + add;
+  s.hist_lo = ending ? s.hist_hi : std::min(s.hist_hi, std::max(0LL, (s.out_hi * f.down + f.half) / f.up - (f.taps - 1)));
+  return s;
+}
+
+int stream_ingest_ctas(const StreamIngest& d) {
+  return (int)ingest_ctas(d.f.n_out) + (d.f.n_in > d.new_hist_lo ? 1 : 0);
+}
+
+int launch_stream_ingest(const StreamIngest* d_streams, const int* d_cta_off, int n_streams, int n_ctas, int max_span,
+                         cudaStream_t st) {
+  if (n_ctas <= 0) return 0;
+  const size_t smem = (size_t)max_span * sizeof(float);
+  if (smem > 48 * 1024) cudaFuncSetAttribute(stream_ingest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  stream_ingest_kernel<<<(unsigned)n_ctas, kOutPerCta, smem, st>>>(d_streams, d_cta_off, n_streams);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

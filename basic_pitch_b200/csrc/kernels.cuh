@@ -284,6 +284,25 @@ long long ingest_ctas(long long n_out);  // CTAs a file of n_out output samples 
 // largest `span` among the files.  One launch; file i gets the bits of launch_ingest on file i alone.
 int launch_ingest_batch(const IngestFile* d_files, const int* d_cta_off, int n_files, int n_ctas, int max_span,
                         cudaStream_t st);
+// A live PCM stream (bp_stream_group_open_pcm, include/bp_b200.h): a push of `add` frames to a stream of n frames makes
+// outputs [out_lo, out_hi) final (ending: and every output left) and leaves the inputs [hist_lo, hist_hi) held.
+struct PcmStep {
+  long long out_lo, out_hi, hist_lo, hist_hi;
+};
+PcmStep pcm_stream_step(const IngestFile& f, long long n, long long add, bool ending);
+// One stream's push as the stream ingest kernel reads it.  Input i: 0 below hist_lo (i.e. below 0), hist[i - hist_lo]
+// below n_prev, mono frame i - n_prev of the new block f.pcm below f.n_in, 0 from there.  Outputs [k0, k0 + f.n_out) go
+// to f.out[0 ..] with the bits of the whole-file ingest; inputs [new_hist_lo, f.n_in) to hist_out (not hist).
+struct StreamIngest {
+  IngestFile f;
+  const float* hist;
+  float* hist_out;
+  long long k0, n_prev, hist_lo, new_hist_lo;
+};
+int stream_ingest_ctas(const StreamIngest& d);  // the output CTAs, plus one for the history when it keeps any
+// d_streams [n] and d_cta_off [n + 1] (exclusive prefix sum of stream_ingest_ctas) in device memory.  One launch.
+int launch_stream_ingest(const StreamIngest* d_streams, const int* d_cta_off, int n_streams, int n_ctas, int max_span,
+                         cudaStream_t st);
 
 // ---- decode.cu ----------------------------------------------------------------------------------
 struct DecodeParamsDev {

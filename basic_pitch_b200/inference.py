@@ -13,6 +13,7 @@ from __future__ import annotations
 import csv
 import ctypes as C
 import enum
+import itertools
 import json
 import os
 import pathlib
@@ -1098,6 +1099,29 @@ def _note_events(arrs, a: int, b: int, bends: bool) -> List[infer.NoteEvent]:
     ]  # fmt: skip
 
 
+def _pcm_block(block, dtype: np.dtype, channels: int) -> np.ndarray:
+    """A PCM stream's block as the library takes it: C-contiguous (n, channels) of the stream's dtype.  (n,) stands for
+    (n, 1).  ValueError for any other dtype, channel count or shape."""
+    b = np.asarray(block)
+    if b.dtype != dtype:
+        raise ValueError(f"a block of this PCM stream must be {dtype}, got {b.dtype}")
+    if b.ndim == 1 and channels == 1:
+        b = b.reshape(-1, 1)
+    if b.ndim != 2 or b.shape[1] != channels:
+        raise ValueError(f"a block of this {channels}-channel PCM stream must be (n, {channels})"
+                         + (" or (n,)" if channels == 1 else "") + f", got shape {b.shape}")
+    return np.ascontiguousarray(b)
+
+
+def _pcm_format(dtype) -> int:
+    from .audio_io import _PCM_FORMATS
+
+    dt = np.dtype(dtype)
+    if dt not in _PCM_FORMATS:
+        raise ValueError(f"PCM dtype must be float32, int16, int32 or uint8, got {dt}")
+    return _PCM_FORMATS[dt]
+
+
 class StreamGroup:
     """Many streamed recordings decoded together (`Model.stream_group`, `bp_stream_group_*`): each call serves every
     stream it lists with one device pass — one forward pass over the windows the new audio completes, one quiet scan,
@@ -1109,10 +1133,16 @@ class StreamGroup:
     one kind only), `end(ids)` closes streams.  Each returns {id: note_events} for the streams it lists, the events that
     became final; with `with_posteriorgrams` also {id: model_output_part}, the frames each stream committed in that call
     (concatenated, `run_inference_stream`'s output for the stream's blocks).  `held_frames(id)` is what
-    `NoteStream.held_frames` reports."""
+    `NoteStream.held_frames` reports.
+
+    `open_pcm(sample_rate, channels, dtype)` adds a stream that takes its blocks as captured: (n,) or (n, channels)
+    arrays of that dtype (float32, int16, int32 or uint8, as `audio_io.read_pcm` returns them) at that rate, resampled
+    on the device with state carried across pushes, so that its signal is `bp_load_pcm_host` of the whole recording
+    whatever the blocks (DESIGN.md §4.6)."""
 
     def __init__(self, model: Model, params: _lib.DecodeParams, max_segment_frames: Optional[int] = None):
         self._model, self._lib = model, model._lib
+        self._pcm: Dict[int, Tuple[np.dtype, int]] = {}  # PCM stream id -> (dtype, channels)
         self._bends = bool(params.include_pitch_bends)
         self._h = C.c_void_p()
         self._lib.bp_stream_group_create(model.handle, C.byref(params), int(max_segment_frames or 0), C.byref(self._h))
@@ -1128,6 +1158,13 @@ class StreamGroup:
     def open(self) -> int:
         i = C.c_int32(0)
         self._lib.bp_stream_group_open(self._h, C.byref(i))
+        return int(i.value)
+
+    def open_pcm(self, sample_rate: int, channels: int, dtype) -> int:
+        fmt = _pcm_format(dtype)
+        i = C.c_int32(0)
+        self._lib.bp_stream_group_open_pcm(self._h, fmt, int(channels), int(sample_rate), C.byref(i))
+        self._pcm[int(i.value)] = (np.dtype(dtype), int(channels))
         return int(i.value)
 
     def held_frames(self, stream_id: int) -> int:
@@ -1157,13 +1194,28 @@ class StreamGroup:
 
     def push(self, blocks: Mapping[int, np.ndarray], with_posteriorgrams: bool = False):
         ids = self._ids(blocks.keys())
-        audio = [np.ascontiguousarray(np.asarray(b, dtype=_F32).reshape(-1)) for b in blocks.values()]
+        pcm = any(int(i) in self._pcm for i in ids)
+        audio = [_pcm_block(b, *self._pcm[int(i)]) if int(i) in self._pcm
+                 else np.ascontiguousarray(np.asarray(b, dtype=_F32).reshape(-1)) for i, b in zip(ids, blocks.values())]
         ptrs = (C.c_void_p * max(len(audio), 1))(*[a.ctypes.data for a in audio])
-        lens = np.array([a.shape[0] for a in audio], np.int64)
-        return self._call(
-            ids, lambda no, on, co, off: self._lib.bp_stream_group_push_host(self._h, len(ids), _ptr(ids), ptrs, _ptr(lens),
-                                                                            no, on, co, off),
-            lens, with_posteriorgrams)
+        lens = np.array([a.shape[0] for a in audio], np.int64)  # PCM frames of a PCM stream
+        push = self._lib.bp_stream_group_push_pcm_host if pcm else self._lib.bp_stream_group_push_host
+        return self._call(ids, lambda no, on, co, off: push(self._h, len(ids), _ptr(ids), ptrs, _ptr(lens), no, on, co, off),
+                          lens, with_posteriorgrams)
+
+    def debug_tail(self, stream_id: int) -> Tuple[int, np.ndarray]:
+        """(first sample, samples) of the stream's held 22 050 Hz tail (`bp_stream_group_debug_tail`)."""
+        first, n = C.c_int64(0), C.c_int64(0)
+        try:
+            self._lib.bp_stream_group_debug_tail(self._h, int(stream_id), None, 0, C.byref(first), C.byref(n))
+            return int(first.value), np.zeros(0, _F32)
+        except _lib.BpError as e:
+            if e.code != _lib.BP_E_CAPACITY:
+                raise
+        out = np.empty(int(n.value), _F32)
+        self._lib.bp_stream_group_debug_tail(self._h, int(stream_id), _ptr(out), out.shape[0], C.byref(first),
+                                             C.byref(n))
+        return int(first.value), out
 
     def push_frames(self, frames: Mapping[int, Tuple[np.ndarray, np.ndarray, Optional[np.ndarray]]]):
         ids = self._ids(frames.keys())
@@ -1383,17 +1435,40 @@ def predict_streams_notes(audio_streams: Sequence[Iterable[np.ndarray]],
                           onset_threshold: float = DEFAULT_ONSET_THRESHOLD, frame_threshold: float = DEFAULT_FRAME_THRESHOLD,
                           minimum_note_length: float = DEFAULT_MINIMUM_NOTE_LENGTH_MS,
                           minimum_frequency: Optional[float] = None, maximum_frequency: Optional[float] = None,
-                          melodia_trick: bool = True, max_segment_seconds: Optional[float] = None):
+                          melodia_trick: bool = True, max_segment_seconds: Optional[float] = None,
+                          sample_rates: Optional[Sequence[Optional[int]]] = None):
     """`predict_stream_notes` for many live recordings at once (`Model.stream_group`): each step pulls one block from
     every iterator that has not ended, pushes them together, ends the recordings whose iterator is exhausted and yields
     {index: note_events} for the recordings it served.  Every recording's events, concatenated over the steps, equal
-    `predict_stream_notes`' on its blocks alone; the keyword arguments are that function's."""
+    `predict_stream_notes`' on its blocks alone; the keyword arguments are that function's.
+
+    sample_rates[i] (None: every recording's blocks are mono float32 at 22 050 Hz) is None for such a recording, or the
+    capture rate of recording i, whose blocks are then PCM as captured: (n,) or (n, channels) float32, int16, int32 or
+    uint8.  Its first block fixes the dtype and the channel count (a later block that differs raises ValueError), and
+    its events are `predict_stream_notes`' on `bp_load_pcm_host` of the whole recording, however it was cut."""
     model = model_or_model_path if isinstance(model_or_model_path, Model) else default_model(model_or_model_path)
     min_note_len = int(np.round(minimum_note_length / 1000 * (AUDIO_SAMPLE_RATE / FFT_HOP)))
     max_seg = None if max_segment_seconds is None else max(1, int(np.round(max_segment_seconds * AUDIO_SAMPLE_RATE / FFT_HOP)))
     group = model.stream_group(onset_threshold, frame_threshold, min_note_len, minimum_frequency, maximum_frequency,
                                melodia_trick, True, max_seg)
-    live = {group.open(): (k, iter(it)) for k, it in enumerate(audio_streams)}
+    rates = list(sample_rates) if sample_rates is not None else [None] * len(audio_streams)
+    if len(rates) != len(audio_streams):
+        raise ValueError("sample_rates must give one entry per recording")
+    live = {}
+    for k, it in enumerate(audio_streams):
+        it = iter(it)
+        if rates[k] is None:
+            live[group.open()] = (k, it)
+            continue
+        try:  # the first block fixes the stream's format
+            first = np.asarray(next(it))
+        except StopIteration:
+            live[group.open()] = (k, it)  # an empty recording
+            continue
+        channels = 1 if first.ndim == 1 else (first.shape[1] if first.ndim == 2 else 0)
+        if channels < 1:
+            raise ValueError(f"recording {k}: PCM blocks must be (n,) or (n, channels), got shape {first.shape}")
+        live[group.open_pcm(int(rates[k]), channels, first.dtype)] = (k, itertools.chain([first], it))
     while live:
         blocks, done = {}, []
         for sid, (_, it) in live.items():

@@ -200,7 +200,8 @@ void bp_stream_destroy(bp_stream_t* s);
  * an unknown or ended id, an id listed twice, a negative length, a NULL block of nonzero length, and a stream given
  * audio after posteriorgrams or the reverse.  The group uses its model's device and stream and must be destroyed before
  * it; it keeps no model workspace between calls.
- * bp_stream_group_push_host: the next block of each listed stream, mono float32 at 22 050 Hz (any length, 0 included).
+ * bp_stream_group_push_host: the next block of each listed stream, mono float32 at 22 050 Hz (any length, 0 included;
+ *   PCM streams below take bp_stream_group_push_pcm_host).
  *   Frames a stream commits: those of its windows except the newest two (whose frames the final trim of unwrap_output
  *   can reach), and at its end bp_num_frames(samples) in all.  h_note / h_onset / h_contour (each may be NULL) receive
  *   the frames each listed stream committed in this call, row-major, stream i's from row h_frame_off[i] on
@@ -213,7 +214,38 @@ void bp_stream_destroy(bp_stream_t* s);
  * bp_stream_group_take: moves the finished notes of the listed streams out, stream i's at note_off[i] .. note_off[i + 1]
  *   (note_off[n + 1]), each as bp_stream_take; ended streams may be listed.  BP_E_CAPACITY (bp_last_required) leaves
  *   them queued.
- * bp_stream_group_held_frames: as bp_stream_held_frames (0 for an unknown id). */
+ * bp_stream_group_held_frames: as bp_stream_held_frames (0 for an unknown id).
+ *
+ * PCM streams: live input at its capture rate and format (DESIGN.md §4.6).
+ * bp_stream_group_open_pcm: a stream whose blocks are interleaved PCM of `channels` channels at `sample_rate` Hz, format
+ *   codes and conversions as bp_load_pcm_* (0 float32, 1 int16, 2 int32, 3 uint8), validated as bp_pcm_file_t is
+ *   (BP_E_INVALID for a format outside 0..3, channels or sample_rate below 1, or a ratio beyond ~100:1; the group stays
+ *   usable).  With the reduced ratio up / down = (22050 / g) / (sample_rate / g), the filter's half = (L - 1) / 2 and T
+ *   taps per phase (bp_load_pcm_*'s resampler), output k reads inputs i_max(k) - T + 1 .. i_max(k), i_max(k) =
+ *   floor((k down + half) / up), inputs below 0 and (once the recording has ended) at or past its end being zero:
+ *     final outputs  after n frames exactly the outputs k < F(n) = max(0, ceil((n up - half) / down)) are final (every
+ *                    input they read has arrived); same rate: F(n) = n;
+ *     end            bp_stream_group_end emits the rest, F(n) .. ceil(n up / down), zero-filled as the whole-file ingest;
+ *     history        between pushes the device keeps only the down-mixed inputs [i_max(F(n)) - T + 1, n), at most T - 1
+ *                    floats;
+ *     bit-identity   every output is computed by the whole-file ingest's arithmetic, so for every block schedule the
+ *                    stream's 22 050 Hz signal is bp_load_pcm_host(whole recording) bit for bit, its frames are
+ *                    run_inference_stream's on that signal and its notes predict_stream_notes'.
+ *   A stream opened as mono float32 at 22 050 Hz is a plain stream.
+ * bp_stream_group_push_pcm_host: the next block of each listed stream, n_frames[i] PCM frames (0 allowed) of that
+ *   stream's format; plain streams may be listed with float32 22 050 Hz blocks (n_frames their samples).  The blocks
+ *   are packed behind their descriptors in pinned staging, each on a 16-byte boundary, and go up in one copy as stored;
+ *   one stream ingest launch (none when no listed stream has frames) writes every stream's new final samples straight
+ *   to its tail, in place of the float push's append copy.  The rest, outputs included, is bp_stream_group_push_host.
+ *   bp_stream_group_end flushes ending PCM streams with one ingest launch before their last windows run.  For a PCM
+ *   stream n_samples of bp_stream_group_commit_offsets counts PCM frames.  BP_E_INVALID (before anything is enqueued)
+ *   for bp_stream_group_push_host on a PCM stream, this call on a posteriorgram stream, a NULL block with frames, a
+ *   negative length and a block whose byte count overflows.
+ * bp_stream_group_debug_tail: copies the stream's held 22 050 Hz tail, samples [*first_sample, *first_sample + *n) of
+ *   its signal, to h_out (BP_E_CAPACITY when capacity < *n, which is still set).
+ * bp_debug_pcm_stream_plan: host-only (no GPU).  For a stream of that format pushed frames[0 .. n_pushes) (and ended when
+ *   `ending`: one more entry), per push the outputs it makes final [out_lo, out_hi) and the inputs it holds afterwards
+ *   [hist_lo, hist_hi), from the function the push itself uses. */
 typedef struct bp_stream_group bp_stream_group_t;
 int bp_stream_group_create(bp_model_t* m, const bp_decode_params_t* params, int64_t max_segment_frames,
                            bp_stream_group_t** out);
@@ -231,6 +263,16 @@ int bp_stream_group_end(bp_stream_group_t* g, int32_t n, const int32_t* ids, flo
 int bp_stream_group_take(bp_stream_group_t* g, int32_t n, const int32_t* ids, bp_notes_t* notes);
 int64_t bp_stream_group_held_frames(const bp_stream_group_t* g, int32_t id);
 void bp_stream_group_destroy(bp_stream_group_t* g);
+int bp_stream_group_open_pcm(bp_stream_group_t* g, int32_t sample_format, int32_t channels, int32_t sample_rate,
+                             int32_t* id);
+int bp_stream_group_push_pcm_host(bp_stream_group_t* g, int32_t n, const int32_t* ids, const void* const* pcm,
+                                  const int64_t* n_frames, float* h_note, float* h_onset, float* h_contour,
+                                  int64_t* h_frame_off);
+int bp_stream_group_debug_tail(const bp_stream_group_t* g, int32_t id, float* h_out, int64_t capacity,
+                               int64_t* first_sample, int64_t* n);
+int bp_debug_pcm_stream_plan(int32_t sample_format, int32_t channels, int32_t sample_rate, int32_t n_pushes,
+                             const int64_t* frames, int32_t ending, int64_t* out_lo, int64_t* out_hi, int64_t* hist_lo,
+                             int64_t* hist_hi);
 
 /* ---- stage 3 under a grid of decode parameters ------------------------------------------------
  * reference: note_creation.py:52-111 (model_output_to_notes without the MIDI object), called once per parameter set.
