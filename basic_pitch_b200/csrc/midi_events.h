@@ -53,7 +53,10 @@ inline void drop_overlapping_pitch_bends(std::vector<Ev>& ev) {
     }
 }
 
-inline int velocity_of(float amp) { return (int)std::nearbyintf(127.0f * amp); }  // int(np.round(127 * np.float32))
+// int(np.round(127 * np.float32(amp))) kept as the rounded float32 product (half to even): an exact integer whenever it
+// is finite, of any size (2e7 gives 2 540 000 000).  NaN or +-inf where Python's int() raises; velocity_ok tells.
+inline float velocity_of(float amp) { return std::nearbyintf(127.0f * amp); }
+inline bool velocity_ok(float amp) { return std::isfinite(velocity_of(amp)); }
 
 // Instruments in order of first use: one per pitch with multiple_pitch_bends, else a single one (the defaultdict of
 // note_creation.py:255-261).  events[k] lists the indices of instrument k's notes in event order.

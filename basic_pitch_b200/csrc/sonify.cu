@@ -127,7 +127,7 @@ FilePlan plan_file(std::vector<Ev> ev, bool multiple_pitch_bends, int sample_rat
       n.a = a, n.b = b;
       n.fade = std::min(fade_max, (b - a) / 2);
       n.inv_fade = n.fade > 0 ? 1.0 / (double)n.fade : 0.0;
-      n.vscale = (double)velocity_of(e.amp) / 127.0;  // velocity not clamped, like Note.velocity
+      n.vscale = (double)velocity_of(e.amp) / 127.0;  // velocity not clamped, like Note.velocity: int / float
       Span s{(int)p.notes.size(), (int)p.segs.size(), 0};
       p.notes.push_back(n);
       // segments: the bend active at sample a, then one per later switch sample inside [a, b); events sharing a
@@ -295,6 +295,10 @@ int sonify_notes(cudaStream_t st, long long* launches, int32_t n_files, const in
   for (int j = n0; j < n1; ++j)
     if (!(start_s[j] >= 0.0 && end_s[j] >= 0.0 && start_s[j] < t_max && end_s[j] < t_max))
       return sonify_fail(BP_E_INVALID, "bp_sonify_notes_host: note times must be finite, >= 0 and below 2^53 samples");
+  // velocities Python's int() refuses: a NaN amplitude, or one whose float32 product with 127 overflows
+  for (int j = n0; j < n1; ++j)
+    if (!velocity_ok(amplitude[j]))
+      return sonify_fail(BP_E_INVALID, "bp_sonify_notes_host: 127 * amplitude must be finite in float32");
 
   const bool sizes_only = h_audio == nullptr;
   std::vector<FilePlan> plans(n_files);

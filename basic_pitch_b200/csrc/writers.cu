@@ -75,7 +75,8 @@ std::string midi_bytes(std::vector<bp::Ev> ev, bool multiple_pitch_bends, double
     msgs.push_back({0, 0, {(unsigned char)(0xC0 | ch), (unsigned char)(program & 0x7F), 0}, 2});
     for (int i : inst.events[idx]) {
       const bp::Ev& e = ev[i];
-      const int vel = std::max(0, std::min(127, bp::velocity_of(e.amp)));
+      const float v = bp::velocity_of(e.amp);
+      const int vel = v <= 0.0f ? 0 : v >= 127.0f ? 127 : (int)v;  // max(0, min(127, velocity))
       msgs.push_back({tick_of(e.start), 2, {(unsigned char)(0x90 | ch), (unsigned char)(e.pitch & 0x7F), (unsigned char)vel}, 3});
       msgs.push_back({tick_of(e.end), 1, {(unsigned char)(0x90 | ch), (unsigned char)(e.pitch & 0x7F), 0}, 3});
     }
@@ -137,7 +138,7 @@ void put_float_repr(std::string& out, double x) {
 
 std::string csv_bytes(const std::vector<bp::Ev>& ev) {
   std::string out = "start_time_s,end_time_s,pitch_midi,velocity,pitch_bend\r\n";
-  char buf[32];
+  char buf[48];
   for (const bp::Ev& e : ev) {
     put_float_repr(out, e.start);
     out.push_back(',');
@@ -145,7 +146,9 @@ std::string csv_bytes(const std::vector<bp::Ev>& ev) {
     out.push_back(',');
     out.append(buf, std::to_chars(buf, buf + sizeof(buf), e.pitch).ptr);
     out.push_back(',');
-    out.append(buf, std::to_chars(buf, buf + sizeof(buf), bp::velocity_of(e.amp)).ptr);
+    // int(velocity): the exact digits of the integral float, which may have up to 39 of them; no "-0"
+    const float v = bp::velocity_of(e.amp);
+    out.append(buf, std::to_chars(buf, buf + sizeof(buf), v == 0.0f ? 0.0 : (double)v, std::chars_format::fixed, 0).ptr);
     for (int b = 0; b < e.n_bends; ++b) {
       out.push_back(',');
       out.append(buf, std::to_chars(buf, buf + sizeof(buf), e.bends[b]).ptr);
@@ -170,6 +173,11 @@ extern "C" int bp_write_note_files(int32_t n_files, const char* const* midi_path
                                    const int32_t* bends, int32_t multiple_pitch_bends, double midi_tempo, int32_t n_threads) {
   if (n_files < 0 || !note_off || (n_files > 0 && (!start_s || !end_s || !pitch_midi || !amplitude)) || !(midi_tempo > 0))
     return bp::writer_fail(BP_E_INVALID, "bp_write_note_files: bad argument");
+  // velocities Python's int() refuses (NaN, or 127 * amplitude overflowing float32): refused before any file is written
+  const int32_t j0 = n_files > 0 ? note_off[0] : 0, j1 = n_files > 0 ? note_off[n_files] : 0;
+  for (int32_t j = j0; j < j1; ++j)
+    if (!bp::velocity_ok(amplitude[j]))
+      return bp::writer_fail(BP_E_INVALID, "bp_write_note_files: 127 * amplitude must be finite in float32");
   if (n_threads <= 0) n_threads = (int)std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
   n_threads = std::max(1, std::min(n_threads, n_files));
   std::vector<int> failed(n_threads, -1);

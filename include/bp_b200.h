@@ -945,7 +945,10 @@ int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* by
  * basic_pitch/note_creation.py:222-271, incl. drop_overlapping_pitch_bends :274-286 when multiple_pitch_bends = 0) +
  * PrettyMIDI.write (inference.py:574-584) and save_note_events (inference.py:409-428).  File i owns notes
  * [note_off[i], note_off[i+1]); note j owns bends [bend_off[j], bend_off[j+1]) (bend_off may be NULL: no bends).
- * midi_paths / csv_paths: arrays of n_files paths (the array or single entries may be NULL = skip).  n_threads <= 0: auto. */
+ * midi_paths / csv_paths: arrays of n_files paths (the array or single entries may be NULL = skip).  n_threads <= 0: auto.
+ * A note's velocity is int(np.round(127 * amplitude)) of the float32 product, an exact integer of any size: the CSV
+ * prints all its digits, the MIDI file clamps it to 0..127.  An amplitude that is NaN or whose product is +-inf (where
+ * Python's int() raises) is BP_E_INVALID, before any file is written. */
 int bp_write_note_files(int32_t n_files, const char* const* midi_paths, const char* const* csv_paths,
                         const int32_t* note_off, const double* start_s, const double* end_s, const int32_t* pitch_midi,
                         const float* amplitude, const int32_t* bend_off, const int32_t* bends,
@@ -958,9 +961,11 @@ int bp_write_note_files(int32_t n_files, const char* const* midi_paths, const ch
  * bp_write_note_files (times in seconds, finite and >= 0; bend_off may be NULL).  h_sample_off[n_files + 1] is always
  * written: file i's samples are h_audio[h_sample_off[i] .. h_sample_off[i+1]), none for a file without notes.
  * h_audio == NULL is a size query (host only, no device work); otherwise `capacity` (in samples) must hold them all
- * (BP_E_CAPACITY).  sample_rate <= 0 or malformed offsets: BP_E_INVALID.  Synchronous on the model's device; the
- * device buffers are sized per call (about 8 bytes per output sample), and a file is never split, so one very long
- * file is one unit of work.  Samples match the stand-in except for the rounding of the phase (DESIGN.md §4.4). */
+ * (BP_E_CAPACITY).  sample_rate <= 0 or malformed offsets: BP_E_INVALID.  Each note is scaled by velocity / 127.0,
+ * the velocity being int(np.round(127 * amplitude)) of the float32 product, unclamped and exact at any size; an
+ * amplitude that is NaN or whose product is +-inf is BP_E_INVALID, with no device work.  Synchronous on the model's
+ * device; the device buffers are sized per call (about 8 bytes per output sample), and a file is never split, so one
+ * very long file is one unit of work.  Samples match the stand-in except for the rounding of the phase (DESIGN.md §4.4). */
 int bp_sonify_notes_host(bp_model_t* m, int32_t n_files, const int32_t* note_off, const double* start_s,
                          const double* end_s, const int32_t* pitch_midi, const float* amplitude, const int32_t* bend_off,
                          const int32_t* bends, int32_t multiple_pitch_bends, int32_t sample_rate, int64_t* h_sample_off,

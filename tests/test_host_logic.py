@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 
 from oracle import decode_ref
+from tests import sonifysets
 
 
 def test_weight_blob_roundtrip_and_dsp_constants(weights_np):
@@ -332,6 +333,13 @@ def test_batched_writers_are_byte_identical_to_the_python_path(tmp_path, multi, 
                 amp=rng.random(n).astype(np.float32), bend_off=boff, bends=rng.integers(-40, 40, boff[-1]).astype(np.int32))
     arrs["pitch"][5:7] = 60
     arrs["amp"][5:7] = 0.5
+    # velocities past int32, negative, zero and above 127 (the CSV prints every digit of int(np.round(127 * amp)), the
+    # MIDI file clamps it to 0..127), the float32 ties of np.round (half to even) and amplitudes whose velocity would
+    # differ with the product taken in float64
+    odd = [2e7, -3e9, 1e30, -1e30, 3e38 / 127, 0.0, -0.0, -0.5, 1.7, 1e-30]
+    odd += sonifysets.tie_amplitudes()[::9].tolist() + sonifysets.f64_disagreements(3).tolist()
+    assert n >= 40 + len(odd)
+    arrs["amp"][40 : 40 + len(odd)] = np.array(odd, np.float32)
     lazy = nc.note_events_batch(arrs, n_files)
     eager = nc.note_events_batch(arrs, n_files, lazy=False)
     for tag, events in (("lazy", lazy), ("eager", eager)):
@@ -347,6 +355,26 @@ def test_batched_writers_are_byte_identical_to_the_python_path(tmp_path, multi, 
             else:
                 assert not (tmp_path / f"{tag}{i}.mid").exists()
             assert cp[i].read_bytes() == (tmp_path / "ref.csv").read_bytes(), (tag, i)
+
+
+@pytest.mark.parametrize("amp", [np.nan, -np.nan, np.inf, -np.inf, 3e38, -3e38, np.finfo(np.float32).max])
+def test_batched_writers_refuse_velocities_python_refuses(tmp_path, amp):
+    """An amplitude whose velocity int(np.round(127 * amp)) Python cannot form (NaN, or a float32 product that
+    overflows to +-inf): bp_write_note_files is BP_E_INVALID before it writes any file, as the Python path raises."""
+    from basic_pitch_b200 import _lib
+    from basic_pitch_b200 import inference as inf
+    from basic_pitch_b200 import note_creation as nc
+
+    events = [[(0.1, 0.5, 60, np.float32(0.5), [1, 2])], [(0.2, 0.4, 61, np.float32(amp), None)]]
+    with pytest.raises((ValueError, OverflowError)), np.errstate(over="ignore", invalid="ignore"):
+        inf.save_note_events(events[1], tmp_path / "ref.csv")
+    paths = [[tmp_path / f"f{i}.{ext}" for i in range(2)] for ext in ("mid", "csv")]
+    with pytest.raises(_lib.BpError) as e:
+        nc.write_note_files(events, *paths, n_threads=1)
+    assert e.value.code == _lib.BP_E_INVALID
+    assert not any(p.exists() for ps in paths for p in ps)
+    nc.write_note_files(events[:1], [paths[0][0]], [paths[1][0]])  # the library stays usable
+    assert paths[0][0].exists() and paths[1][0].exists()
 
 
 def test_note_event_list_behaves_like_the_list():
