@@ -18,13 +18,14 @@ BP_E_INVALID = -1
 BP_E_CUDA = -2
 BP_E_CAPACITY = -3
 BP_E_NOMEM = -4
+BP_E_IO = -5
 
 EXPORTS = [
     "bp_version", "bp_last_error", "bp_default_decode_params", "bp_num_windows", "bp_num_frames",
     "bp_model_create", "bp_model_destroy", "bp_model_device", "bp_model_param_block", "bp_model_refresh",
     "bp_model_launch_count", "bp_forward_device", "bp_forward_host", "bp_run_inference_device",
     "bp_run_inference_host", "bp_decode_device", "bp_decode_host", "bp_transcribe_host", "bp_transcribe_device",
-    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_schedule", "bp_debug_tc_clocks", "bp_debug_tc_cta_busy", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params", "bp_default_score_params", "bp_frame_times", "bp_score_grid_device", "bp_score_grid_host", "bp_score_notes_host", "bp_multipitch_map", "bp_score_frames_grid_device", "bp_score_frames_grid_host", "bp_score_multipitch_host", "bp_score_salience_grid_device", "bp_score_salience_grid_host", "bp_score_salience_chunk_params", "bp_match_grid_device", "bp_match_grid_host", "bp_match_notes_host", "bp_score_onset_offset_grid_device", "bp_score_onset_offset_grid_host", "bp_score_onset_offset_notes_host", "bp_melody_map", "bp_score_melody_grid_device", "bp_score_melody_grid_host", "bp_score_melody_host", "bp_score_melody_chunk_params", "bp_score_bent_frames_grid_device", "bp_score_bent_frames_grid_host", "bp_score_note_melody_grid_device", "bp_score_note_melody_grid_host", "bp_evaluate_device", "bp_evaluate_host", "bp_evaluate_audio_host", "bp_evaluate_pcm_files_host", "bp_evaluate_chunk_params", "bp_stream_create", "bp_stream_push_host", "bp_stream_end", "bp_stream_take", "bp_stream_held_frames", "bp_stream_destroy", "bp_stream_group_create", "bp_stream_group_open", "bp_stream_group_commit_offsets", "bp_stream_group_push_host", "bp_stream_group_push_frames_host", "bp_stream_group_end", "bp_stream_group_take", "bp_stream_group_held_frames", "bp_stream_group_destroy", "bp_stream_group_open_pcm", "bp_stream_group_push_pcm_host", "bp_stream_group_debug_tail", "bp_debug_pcm_stream_plan",
+    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_schedule", "bp_debug_tc_clocks", "bp_debug_tc_cta_busy", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params", "bp_default_score_params", "bp_frame_times", "bp_score_grid_device", "bp_score_grid_host", "bp_score_notes_host", "bp_multipitch_map", "bp_score_frames_grid_device", "bp_score_frames_grid_host", "bp_score_multipitch_host", "bp_score_salience_grid_device", "bp_score_salience_grid_host", "bp_score_salience_chunk_params", "bp_match_grid_device", "bp_match_grid_host", "bp_match_notes_host", "bp_score_onset_offset_grid_device", "bp_score_onset_offset_grid_host", "bp_score_onset_offset_notes_host", "bp_melody_map", "bp_score_melody_grid_device", "bp_score_melody_grid_host", "bp_score_melody_host", "bp_score_melody_chunk_params", "bp_score_bent_frames_grid_device", "bp_score_bent_frames_grid_host", "bp_score_note_melody_grid_device", "bp_score_note_melody_grid_host", "bp_evaluate_device", "bp_evaluate_host", "bp_evaluate_audio_host", "bp_evaluate_pcm_files_host", "bp_evaluate_chunk_params", "bp_stream_create", "bp_stream_push_host", "bp_stream_end", "bp_stream_take", "bp_stream_held_frames", "bp_stream_destroy", "bp_stream_group_create", "bp_stream_group_open", "bp_stream_group_commit_offsets", "bp_stream_group_push_host", "bp_stream_group_push_frames_host", "bp_stream_group_end", "bp_stream_group_take", "bp_stream_group_held_frames", "bp_stream_group_destroy", "bp_stream_group_open_pcm", "bp_stream_group_push_pcm_host", "bp_stream_group_debug_tail", "bp_debug_pcm_stream_plan", "bp_probe_wav_files", "bp_transcribe_pcm_sources_host", "bp_evaluate_pcm_sources_host", "bp_load_pcm_sources_device", "bp_debug_pcm_sources_layout",
 ]  # fmt: skip
 
 
@@ -125,6 +126,16 @@ class PcmFile(C.Structure):
     ]
 
 
+class PcmSource(C.Structure):
+    """bp_pcm_source_t: stored PCM in memory (path None) or bytes [data_offset, ...) of a file."""
+
+    _fields_ = [
+        ("pcm", PcmFile),
+        ("path", C.c_char_p),
+        ("data_offset", C.c_int64),
+    ]
+
+
 class EvalRequest(C.Structure):
     """bp_eval_request_t: one block per metric family, a NULL output meaning "not requested"."""
 
@@ -174,6 +185,10 @@ class BpError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libbp_b200 error {code}: {msg}")
         self.code = code
+
+
+class BpIOError(BpError, OSError):
+    """BP_E_IO: a file the library was reading could not be read (the message names it)."""
 
 
 _lib: Optional[C.CDLL] = None
@@ -328,6 +343,12 @@ def load() -> C.CDLL:
     lib.bp_transcribe_pcm_files_host.argtypes = [vp, C.POINTER(PcmFile), i32, C.POINTER(DecodeParams), vp, vp, vp, vp, vp,
                                                  C.POINTER(Notes)]
     lib.bp_debug_pcm_layout.argtypes = [C.POINTER(PcmFile), i32, vp, vp]
+    lib.bp_probe_wav_files.argtypes = [vp, i32, C.POINTER(PcmSource), vp]
+    lib.bp_transcribe_pcm_sources_host.argtypes = [vp, C.POINTER(PcmSource), i32, C.POINTER(DecodeParams), vp, vp, vp, vp,
+                                                   vp, C.POINTER(Notes)]
+    lib.bp_evaluate_pcm_sources_host.argtypes = [vp, C.POINTER(PcmSource), i32, C.POINTER(EvalRequest), vp, vp, vp, vp, vp]
+    lib.bp_load_pcm_sources_device.argtypes = [vp, C.POINTER(PcmSource), i32, vp, vp, vp]
+    lib.bp_debug_pcm_sources_layout.argtypes = [C.POINTER(PcmSource), i32, vp, vp]
     lib.bp_debug_resample_filter.argtypes = [i32, i32, vp, i64]
     lib.bp_debug_resample_filter.restype = i64
     lib.bp_write_note_files.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, C.c_double, i32]
@@ -344,5 +365,6 @@ def load() -> C.CDLL:
 
 def _check(result, func, args):
     if result != BP_OK:
-        raise BpError(result, load().bp_last_error().decode(errors="replace"))
+        msg = load().bp_last_error().decode(errors="replace")
+        raise (BpIOError if result == BP_E_IO else BpError)(result, msg)
     return result

@@ -1,6 +1,7 @@
 """Audio file -> mono float32 at 22 050 Hz, in front of the hot path: `load_audio` on the host (NumPy / SciPy),
 `load_audio_device` with the conversion, down-mix and resampling on the GPU (csrc/ingest.cu, same filter); `read_pcm` +
-`pcm_descriptors` hand the stored samples of a whole batch of files to the batched ingest (`Model.transcribe_pcm`).
+`pcm_descriptors` hand the stored samples of a whole batch of files to the batched ingest (`Model.transcribe_pcm`), and
+`probe_wav` finds the WAV files whose samples the library reads itself (`WavRegion`).
 
 Stands in for `librosa.load(path, sr=22050, mono=True)` (reference: basic_pitch/inference.py:239).
 WAV files are decoded with scipy; other containers need `soundfile` (optional).  Files that are not
@@ -11,9 +12,13 @@ resampler is NOT parity-pinned against librosa/soxr (neither is available offlin
 """
 from __future__ import annotations
 
+import os
 import pathlib
+from dataclasses import dataclass
 from math import gcd
-from typing import Sequence, Tuple, Union
+from typing import List, Optional, Sequence, Tuple, Union
+
+import ctypes as C
 
 import numpy as np
 
@@ -97,6 +102,69 @@ def pcm_descriptors(items: Sequence[Tuple[np.ndarray, int]]):
         f.n_frames, f.channels = (x.shape[0], 1) if x.ndim == 1 else x.shape
         f.sample_format, f.sample_rate = _PCM_FORMATS[x.dtype], int(sr)
     return files, keep
+
+
+@dataclass(frozen=True)
+class WavRegion:
+    """The samples of a WAV file as `probe_wav` found them: bytes [data_offset, data_offset + n_frames x channels x
+    bytes per sample) of `path`, interleaved, in library format `sample_format` (0 float32, 1 int16, 2 int32, 3 uint8,
+    4 packed 24-bit, 5 float64).  An item of `Model.transcribe_pcm` / `Model.evaluate(pcm=...)` beside
+    (samples, sample_rate) pairs: the library reads the bytes itself, and they cross PCIe as stored."""
+
+    path: str
+    data_offset: int
+    n_frames: int
+    sample_format: int
+    channels: int
+    sample_rate: int
+
+
+def probe_wav(paths: Sequence[Union[str, pathlib.Path]]) -> Tuple[List[Optional[WavRegion]], List[int]]:
+    """The WAV headers of `paths`, read by the library (`bp_probe_wav_files`, no GPU): (regions, declined), regions[i]
+    the `WavRegion` of an accepted file and None for a declined one, whose indices `declined` lists.  A file is accepted
+    only when its reading is unambiguous and equals `scipy.io.wavfile.read`'s (include/bp_b200.h); a declined file is
+    for `read_pcm`, which gives it the result or the exception it always did."""
+    from . import _lib
+
+    lib = _lib.load()
+    names = [os.fsencode(p) for p in paths]
+    n = len(names)
+    arg = (C.c_char_p * max(n, 1))(*names)
+    out = (_lib.PcmSource * max(n, 1))()
+    accepted = np.zeros(max(n, 1), np.int32)
+    lib.bp_probe_wav_files(arg, n, out, accepted.ctypes.data)
+    regions: List[Optional[WavRegion]] = []
+    for i in range(n):
+        s = out[i]
+        regions.append(WavRegion(os.fsdecode(names[i]), int(s.data_offset), int(s.pcm.n_frames), int(s.pcm.sample_format),
+                                 int(s.pcm.channels), int(s.pcm.sample_rate)) if accepted[i] else None)
+    return regions, [i for i in range(n) if not accepted[i]]
+
+
+def pcm_sources(items: Sequence[Union[Tuple[np.ndarray, int], WavRegion]]):
+    """`pcm_descriptors` for batches that may hold `WavRegion`s: the `bp_pcm_source_t` array of
+    `bp_transcribe_pcm_sources_host` / `bp_evaluate_pcm_sources_host` plus what it points into (kept by the caller for
+    the call).  (samples, sample_rate) items are described as `pcm_descriptors` describes them."""
+    from . import _lib
+
+    n = len(items)
+    sources = (_lib.PcmSource * max(n, 1))()
+    arrays = [it for it in items if not isinstance(it, WavRegion)]
+    files, keep = pcm_descriptors(arrays)
+    keep = list(keep)
+    k = 0
+    for s, it in zip(sources, items):
+        if isinstance(it, WavRegion):
+            name = os.fsencode(it.path)
+            keep.append(name)
+            s.path, s.data_offset = name, it.data_offset
+            s.pcm.pcm = None
+            s.pcm.n_frames, s.pcm.sample_format = it.n_frames, it.sample_format
+            s.pcm.channels, s.pcm.sample_rate = it.channels, it.sample_rate
+        else:
+            s.pcm = files[k]
+            k += 1
+    return sources, keep
 
 
 def load_audio_device(path: Union[str, pathlib.Path], model) -> Tuple[np.ndarray, int]:

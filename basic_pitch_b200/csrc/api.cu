@@ -1,14 +1,18 @@
 // C ABI of the hot path (include/bp_b200.h): model lifetime, workspace, chunked launch sequences.
 #include <cuda_runtime.h>
+#include <fcntl.h>
+#include <unistd.h>
 
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cerrno>
 #include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <memory>
+#include <mutex>
 #include <thread>
 #include <string>
 #include <vector>
@@ -31,6 +35,7 @@ int fail(int code, const std::string& msg) {
 namespace bp {
 int writer_fail(int code, const std::string& msg) { return fail(code, msg); }  // writers.cu reports through bp_last_error
 int sonify_fail(int code, const std::string& msg) { return fail(code, msg); }  // sonify.cu likewise
+int wav_fail(int code, const std::string& msg) { return fail(code, msg); }     // wav.cu likewise
 }
 namespace {
 
@@ -1402,9 +1407,14 @@ namespace {
 // sub-batches whose buffer may be overwritten) and reports it in done[k].  The threads live for one call.  Files are
 // bytes here: file i is src[i][0 .. len[i]) and lands off[i] - off[first file of its sub-batch] bytes behind the
 // sub-batch's header (float32 audio: no header, off = 4 x the sample offsets; stored PCM: gaps that start every file on a
-// 16-byte boundary).
+// 16-byte boundary).  A file with a path (`path[i]`, when `path` is given) is read instead from bytes
+// [file_off[i], file_off[i] + len[i]) of that file with pread, straight into the staging buffer; each thread opens such a
+// file once for its share of it.  A read that fails or comes up short is recorded (error_file(), error_text()) and the
+// sub-batch still counts as done, so that the caller can end the call.
 struct Gatherer {
   const unsigned char* const* src;
+  const char* const* path = nullptr;  // [n_files] or null: file i is read from path[i] when that is not null
+  const int64_t* file_off = nullptr;  // [n_files] byte offset of file i's first sample in path[i]
   const int64_t* off;        // [n_files + 1] non-decreasing byte offsets, off[i] + len[i] <= off[i + 1]
   const int64_t* len;        // [n_files]
   const int64_t* head;       // [n_sub] bytes the caller keeps at the front of each sub-batch's buffer
@@ -1415,10 +1425,13 @@ struct Gatherer {
   std::vector<std::atomic<int>> done;
   std::vector<std::thread> threads;
   std::atomic<bool> abort{false};
+  std::atomic<int> err_file{-1};
+  std::mutex err_mu;
+  std::string err_text;
 
-  Gatherer(const unsigned char* const* s, const int64_t* o, const int64_t* l, const int64_t* h, const int* c, int ns, int nt,
-           unsigned char* const* st)
-      : src(s), off(o), len(l), head(h), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
+  Gatherer(const unsigned char* const* s, const char* const* p, const int64_t* fo, const int64_t* o, const int64_t* l,
+           const int64_t* h, const int* c, int ns, int nt, unsigned char* const* st)
+      : src(s), path(p), file_off(fo), off(o), len(l), head(h), cut(c), n_sub(ns), n_threads(nt), stage(st), done(ns) {
     for (auto& d : done) d.store(0);
     for (int t = 0; t < n_threads; ++t) threads.emplace_back([this, t] { run(t); });
   }
@@ -1444,11 +1457,44 @@ struct Gatherer {
         int i = (int)(std::upper_bound(off + f0, off + f1 + 1, lo) - off) - 1;
         for (; i < f1 && off[i] < hi; ++i) {
           const int64_t a = std::max(lo, off[i]), b = std::min(hi, off[i] + len[i]);
-          if (b > a) std::memcpy(dst + (a - base), src[i] + (a - off[i]), (size_t)(b - a));
+          if (b <= a) continue;
+          if (path && path[i])
+            read_file(i, file_off[i] + (a - off[i]), dst + (a - base), b - a);
+          else
+            std::memcpy(dst + (a - base), src[i] + (a - off[i]), (size_t)(b - a));
         }
       }
       done[k].fetch_add(1, std::memory_order_release);
     }
+  }
+  // bytes [pos, pos + n) of file i's path into dst
+  void read_file(int i, int64_t pos, unsigned char* dst, int64_t n) {
+    const int fd = open(path[i], O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return record(i, std::string("cannot open: ") + std::strerror(errno));
+    while (n > 0) {
+      const ssize_t r = pread(fd, dst, (size_t)std::min<int64_t>(n, 1 << 30), (off_t)pos);
+      if (r < 0 && errno == EINTR) continue;
+      if (r <= 0) {
+        record(i, r == 0 ? "the file ended " + std::to_string(n) + " bytes before its samples did (short read at byte " +
+                               std::to_string(pos) + ")"
+                         : std::string("read failed: ") + std::strerror(errno));
+        break;
+      }
+      dst += r, pos += r, n -= r;
+    }
+    close(fd);
+  }
+  void record(int i, const std::string& what) {
+    std::lock_guard<std::mutex> lk(err_mu);
+    if (err_file.load() < 0 || i < err_file.load()) {
+      err_text = what;
+      err_file.store(i);
+    }
+  }
+  int error_file() const { return err_file.load(); }
+  std::string error_text() {
+    std::lock_guard<std::mutex> lk(err_mu);
+    return err_text;
   }
   void release_upto(int k) { released.store(k, std::memory_order_release); }  // sub-batches < k may be gathered
   void wait(int k) {
@@ -1457,14 +1503,14 @@ struct Gatherer {
 };
 
 // A batch of whole files as an entry point received it: packed back to back (`audio`, in device memory if `on_device`,
-// else in host memory), one host pointer per file (`files`), or one host pointer per file to its stored PCM (`pcm`),
-// which the device ingest turns into the 22 050 Hz signals the other two kinds start from.
+// else in host memory), one host pointer per file (`files`), or per file its stored PCM in host memory or a byte range
+// of a file (`pcm`), which the device ingest turns into the 22 050 Hz signals the other two kinds start from.
 struct Batch {
   const char* api;             // the calling entry point, prefix of every message
   const float* audio;          // packed: the caller's array; describe_batch moves it to the first file's samples
   bool on_device;
   const float* const* files;
-  const bp_pcm_file_t* pcm = nullptr;
+  const bp_pcm_source_t* pcm = nullptr;
   std::vector<int64_t> rel{};  // [n_files + 1] sample offsets (22 050 Hz) from the first file (describe_batch)
   int64_t total_frames = 0;    // frames of the posteriorgrams (describe_batch)
   std::vector<IngestFile> ingest{};  // pcm: each file's resampler, lengths and format (describe_pcm)
@@ -1473,7 +1519,11 @@ struct Batch {
   bool per_file() const { return files || pcm; }  // gathered into pinned staging sub-batch by sub-batch
 };
 
-constexpr int kPcmSampleBytes[4] = {4, 2, 4, 1};
+// bytes per sample and the alignment the device reads a sample at, per format: 0 float32, 1 int16, 2 int32, 3 uint8,
+// 4 packed 24-bit, 5 float64
+constexpr int kPcmSampleBytes[kBatchIngestFormats] = {4, 2, 4, 1, 3, 8};
+constexpr int kPcmSampleAlign[kBatchIngestFormats] = {4, 2, 4, 1, 1, 8};
+constexpr int kPcmFileFormats = 4;  // what a bp_pcm_file_t may hold (0..3); a bp_pcm_source_t may hold all six
 constexpr int64_t align16(int64_t n) { return (n + 15) & ~(int64_t)15; }
 // The front of a PCM sub-batch of nf files, on the host and on the device: IngestFile [nf], then the CTA prefix
 // int [nf + 1], padded so that the PCM behind it starts on a 16-byte boundary.
@@ -1505,29 +1555,38 @@ static int describe_batch(Batch& b, const int64_t* sample_off, const int64_t* n_
   return BP_OK;
 }
 
-// Validates every stored-PCM file of a batch, host arithmetic only: -> each file's resampler geometry, frame counts in
-// and out (`ingest`, pointers unset) and stored bytes.  `device_pcm`: the pointers are dereferenced by the kernel as they
-// are, so they must be aligned to their sample type.
+// Validates every stored-PCM file of a batch (`files`, or the PCM of `sources` when given), host arithmetic only: -> each
+// file's resampler geometry, frame counts in and out (`ingest`, pointers unset) and stored bytes.  Formats
+// 0 .. n_formats - 1 are valid.  `device_pcm`: the pointers are dereferenced by the kernel as they are, so they must be
+// aligned to their sample type.  A source with a path needs no pointer, but a data offset from which its bytes stay
+// below 2^63.
 static int describe_pcm(const std::string& api, const bp_pcm_file_t* files, int32_t n_files, bool device_pcm,
-                        std::vector<IngestFile>& ingest, std::vector<int64_t>& bytes) {
+                        int n_formats, std::vector<IngestFile>& ingest, std::vector<int64_t>& bytes,
+                        const bp_pcm_source_t* sources = nullptr) {
   ingest.assign(n_files, IngestFile{});
   bytes.assign(n_files, 0);
   int64_t ctas = 0;
   for (int i = 0; i < n_files; ++i) {
-    const bp_pcm_file_t& f = files[i];
+    const bp_pcm_file_t& f = sources ? sources[i].pcm : files[i];
+    const char* path = sources ? sources[i].path : nullptr;
     const std::string who = api + ": file " + std::to_string(i);
     if (f.n_frames < 0) return fail(BP_E_INVALID, who + " has a negative length");
-    if (f.sample_format < 0 || f.sample_format > 3)
-      return fail(BP_E_INVALID, who + ": sample_format must be 0 (float32), 1 (int16), 2 (int32) or 3 (uint8)");
+    if (f.sample_format < 0 || f.sample_format >= n_formats)
+      return fail(BP_E_INVALID, who + (n_formats == kPcmFileFormats
+                                           ? ": sample_format must be 0 (float32), 1 (int16), 2 (int32) or 3 (uint8)"
+                                           : ": sample_format must be 0 (float32), 1 (int16), 2 (int32), 3 (uint8), "
+                                             "4 (packed 24-bit) or 5 (float64)"));
     if (f.channels < 1) return fail(BP_E_INVALID, who + ": channels must be >= 1");
     if (f.sample_rate < 1) return fail(BP_E_INVALID, who + ": sample_rate must be >= 1");
-    if (ingest_geometry(f.sample_format, f.channels, f.sample_rate, ingest[i]) != 0)
+    if (ingest_geometry(f.sample_format, f.channels, f.sample_rate, ingest[i], kBatchIngestFormats) != 0)
       return fail(BP_E_INVALID, who + ": the ratio of " + std::to_string(f.sample_rate) +
                                     " Hz to 22 050 Hz is beyond the resampler's shared-memory limit (~100:1)");
     const int64_t frame_bytes = (int64_t)f.channels * kPcmSampleBytes[f.sample_format];
     if (f.n_frames > (INT64_MAX >> 16) / frame_bytes) return fail(BP_E_INVALID, who + " is too long");
-    if (f.n_frames > 0 && !f.pcm) return fail(BP_E_INVALID, who + ": null pcm");
-    if (device_pcm && reinterpret_cast<uintptr_t>(f.pcm) % kPcmSampleBytes[f.sample_format] != 0)
+    if (path && (sources[i].data_offset < 0 || sources[i].data_offset > INT64_MAX - f.n_frames * frame_bytes))
+      return fail(BP_E_INVALID, who + ": data_offset must be >= 0 and leave the samples below 2^63 bytes");
+    if (f.n_frames > 0 && !f.pcm && !path) return fail(BP_E_INVALID, who + ": null pcm");
+    if (device_pcm && reinterpret_cast<uintptr_t>(f.pcm) % kPcmSampleAlign[f.sample_format] != 0)
       return fail(BP_E_INVALID, who + ": pcm is not aligned to its sample type");
     bytes[i] = f.n_frames * frame_bytes;
     ingest[i].n_in = f.n_frames;
@@ -1630,16 +1689,21 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
     if ((rc = ensure_events(m->conv_ev, n_sub))) return rc;
   }
   int n_threads = 0;
-  // per-file input as the gather threads see it: bytes (Gatherer)
+  // per-file input as the gather threads see it: bytes in memory or in a file (Gatherer)
   std::vector<const unsigned char*> src;
-  std::vector<int64_t> off, len, head;
+  std::vector<const char*> path;
+  std::vector<int64_t> off, len, head, file_off;
+  bool any_path = false;
   if (b.per_file()) {
     src.resize(n_files);
     off.assign(n_files + 1, 0);
     len.resize(n_files);
     head.assign(n_sub, 0);
+    path.assign(n_files, nullptr);
+    file_off.assign(n_files, 0);
     for (int i = 0; i < n_files; ++i) {
-      src[i] = static_cast<const unsigned char*>(b.pcm ? b.pcm[i].pcm : static_cast<const void*>(b.files[i]));
+      src[i] = static_cast<const unsigned char*>(b.pcm ? b.pcm[i].pcm.pcm : static_cast<const void*>(b.files[i]));
+      if (b.pcm && b.pcm[i].path) path[i] = b.pcm[i].path, file_off[i] = b.pcm[i].data_offset, any_path = true;
       len[i] = b.pcm ? b.pcm_bytes[i] : (int64_t)sizeof(float) * (b.rel[i + 1] - b.rel[i]);
       off[i + 1] = off[i] + (b.pcm ? align16(len[i]) : len[i]);
     }
@@ -1672,7 +1736,8 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
   if (from_host) CK(cudaStreamSynchronize(st));  // st_audio / st_note.. may still be in use by earlier work on the compute stream
   std::unique_ptr<Gatherer> gatherer;
   if (b.per_file()) {
-    gatherer.reset(new Gatherer(src.data(), off.data(), len.data(), head.data(), cut.data(), n_sub, n_threads, m->gather));
+    gatherer.reset(new Gatherer(src.data(), any_path ? path.data() : nullptr, file_off.data(), off.data(), len.data(),
+                                head.data(), cut.data(), n_sub, n_threads, m->gather));
     gatherer->release_upto(std::min(3, n_sub));  // the three buffers are free: the workers start at once
   }
   h_frame_off[0] = 0;
@@ -1688,6 +1753,15 @@ static int run_batch(bp_model* m, const Batch& b, const Rows* rows, Rows host, c
           gatherer->wait(k);  // sub-batch k is in its staging buffer (gathered while earlier sub-batches were enqueued)
           t_gather += ms_since(t0);
           t0 = now();
+          if (gatherer->error_file() >= 0) {  // a file could not be read: end the threads, let queued work finish
+            const int i = gatherer->error_file();
+            const std::string what = gatherer->error_text();
+            gatherer.reset();
+            CK(cudaStreamSynchronize(st));
+            CK(cudaStreamSynchronize(m->copy_stream));
+            if (m->d2h_stream) CK(cudaStreamSynchronize(m->d2h_stream));
+            return fail(BP_E_IO, std::string(b.api) + ": file " + std::to_string(i) + " (" + path[i] + "): " + what);
+          }
         }
         if (b.pcm) {  // descriptors + PCM up in one copy, then the ingest writes st_audio[s0, s1)
           const int nf = f1 - f0;
@@ -3594,14 +3668,12 @@ int bp_evaluate_audio_host(bp_model_t* m, const float* h_audio, const int64_t* h
   return evaluate_batch(m, b, req, Rows{h_note, h_onset, h_contour}, h_frame_off);
 }
 
-int bp_evaluate_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, const bp_eval_request_t* req,
-                               float* h_note, float* h_onset, float* h_contour, int64_t* h_frame_off,
-                               int64_t* h_sample_off) {
-  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
-    return fail(BP_E_INVALID, "bp_evaluate_pcm_files_host: bad argument");
-  Batch b{"bp_evaluate_pcm_files_host", nullptr, false, nullptr};
-  b.pcm = files;
-  int rc = describe_pcm(b.api, files, n_files, false, b.ingest, b.pcm_bytes);
+// The stored-PCM batch of the _pcm_files_host / _pcm_sources_host entry points: every source validated and the 22 050 Hz
+// lengths of the batch known (h_sample_off, may be null) before anything else happens.
+static int describe_sources(Batch& b, const bp_pcm_source_t* sources, int32_t n_files, int n_formats,
+                            int64_t* h_sample_off) {
+  b.pcm = sources;
+  const int rc = describe_pcm(b.api, nullptr, n_files, false, n_formats, b.ingest, b.pcm_bytes, sources);
   if (rc) return rc;
   b.rel.assign(n_files + 1, 0);
   for (int i = 0; i < n_files; ++i) {
@@ -3609,8 +3681,43 @@ int bp_evaluate_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_
     b.total_frames += bp_num_frames(b.ingest[i].n_out);
   }
   if (h_sample_off) std::copy(b.rel.begin(), b.rel.end(), h_sample_off);
+  return BP_OK;
+}
+
+// bp_pcm_file_t [n] -> the same files as in-memory sources (still validated as bp_pcm_file_t: formats 0..3)
+static std::vector<bp_pcm_source_t> memory_sources(const bp_pcm_file_t* files, int32_t n_files) {
+  std::vector<bp_pcm_source_t> s((size_t)std::max(n_files, 0));
+  for (int i = 0; i < n_files; ++i) s[i] = bp_pcm_source_t{files[i], nullptr, 0};
+  return s;
+}
+
+static int evaluate_sources(const char* api, bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                            int n_formats, const bp_eval_request_t* req, float* h_note, float* h_onset,
+                            float* h_contour, int64_t* h_frame_off, int64_t* h_sample_off) {
+  Batch b{api, nullptr, false, nullptr};
+  const int rc = describe_sources(b, sources, n_files, n_formats, h_sample_off);
+  if (rc) return rc;
   DeviceGuard g(m->device);
   return evaluate_batch(m, b, req, Rows{h_note, h_onset, h_contour}, h_frame_off);
+}
+
+int bp_evaluate_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, const bp_eval_request_t* req,
+                               float* h_note, float* h_onset, float* h_contour, int64_t* h_frame_off,
+                               int64_t* h_sample_off) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_evaluate_pcm_files_host: bad argument");
+  const std::vector<bp_pcm_source_t> s = memory_sources(files, n_files);
+  return evaluate_sources("bp_evaluate_pcm_files_host", m, s.data(), n_files, kPcmFileFormats, req, h_note, h_onset, h_contour,
+                          h_frame_off, h_sample_off);
+}
+
+int bp_evaluate_pcm_sources_host(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                                 const bp_eval_request_t* req, float* h_note, float* h_onset, float* h_contour,
+                                 int64_t* h_frame_off, int64_t* h_sample_off) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !sources))
+    return fail(BP_E_INVALID, "bp_evaluate_pcm_sources_host: bad argument");
+  return evaluate_sources("bp_evaluate_pcm_sources_host", m, sources, n_files, kBatchIngestFormats, req, h_note, h_onset, h_contour,
+                          h_frame_off, h_sample_off);
 }
 
 int bp_transcribe_device(bp_model_t* m, const float* d_audio, const int64_t* h_sample_off, int32_t n_files,
@@ -3711,14 +3818,16 @@ int bp_load_pcm_host(bp_model_t* m, const void* h_pcm, int32_t sample_format, in
   return BP_OK;
 }
 
-int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, float* d_audio,
-                             int64_t* h_sample_off, void* stream) {
-  if (!m || !h_sample_off || n_files < 0 || (n_files > 0 && !files))
-    return fail(BP_E_INVALID, "bp_load_pcm_files_device: bad argument");
-  const std::string api = "bp_load_pcm_files_device";
+// bp_load_pcm_files_device / bp_load_pcm_sources_device: in-memory sources whose pointers are device pointers.
+static int load_pcm_device(const std::string& api, bp_model_t* m, const bp_pcm_source_t* files, int32_t n_files,
+                           int n_formats, float* d_audio, int64_t* h_sample_off, void* stream) {
+  for (int i = 0; i < n_files; ++i)
+    if (files[i].path)
+      return fail(BP_E_INVALID, api + ": file " + std::to_string(i) + " is a file on disk; the device ingest reads "
+                                      "device memory (bp_transcribe_pcm_sources_host reads files)");
   std::vector<IngestFile> desc;
   std::vector<int64_t> bytes;
-  int rc = describe_pcm(api, files, n_files, true, desc, bytes);
+  int rc = describe_pcm(api, nullptr, n_files, true, n_formats, desc, bytes, files);
   if (rc) return rc;
   int64_t total = 0;
   for (const IngestFile& f : desc) total += f.n_out;
@@ -3730,7 +3839,7 @@ int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if ((rc = load_ingest_taps(api, m->device, desc))) return rc;
   for (int i = 0; i < n_files; ++i) {
-    desc[i].pcm = files[i].pcm;
+    desc[i].pcm = files[i].pcm.pcm;
     desc[i].out = d_audio + h_sample_off[i];
   }
   const size_t hb = (size_t)ingest_header_bytes(n_files);
@@ -3763,33 +3872,59 @@ int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t 
   return rc;
 }
 
-int bp_transcribe_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files,
-                                 const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
-                                 int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes) {
-  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
-    return fail(BP_E_INVALID, "bp_transcribe_pcm_files_host: bad argument");
+int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, float* d_audio,
+                             int64_t* h_sample_off, void* stream) {
+  if (!m || !h_sample_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_load_pcm_files_device: bad argument");
+  const std::vector<bp_pcm_source_t> s = memory_sources(files, n_files);
+  return load_pcm_device("bp_load_pcm_files_device", m, s.data(), n_files, kPcmFileFormats, d_audio, h_sample_off,
+                         stream);
+}
+
+int bp_load_pcm_sources_device(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files, float* d_audio,
+                               int64_t* h_sample_off, void* stream) {
+  if (!m || !h_sample_off || n_files < 0 || (n_files > 0 && !sources))
+    return fail(BP_E_INVALID, "bp_load_pcm_sources_device: bad argument");
+  return load_pcm_device("bp_load_pcm_sources_device", m, sources, n_files, kBatchIngestFormats, d_audio,
+                         h_sample_off, stream);
+}
+
+static int transcribe_sources(const char* api, bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                              int n_formats, const bp_decode_params_t* params, float* h_note, float* h_onset,
+                              float* h_contour, int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes) {
   int rc = validate_params(params);
   if (rc) return rc;
-  Batch b{"bp_transcribe_pcm_files_host", nullptr, false, nullptr};
-  b.pcm = files;
-  if ((rc = describe_pcm(b.api, files, n_files, false, b.ingest, b.pcm_bytes))) return rc;
-  b.rel.assign(n_files + 1, 0);
-  for (int i = 0; i < n_files; ++i) {
-    b.rel[i + 1] = b.rel[i] + b.ingest[i].n_out;
-    b.total_frames += bp_num_frames(b.ingest[i].n_out);
-  }
-  if (h_sample_off) std::copy(b.rel.begin(), b.rel.end(), h_sample_off);
+  Batch b{api, nullptr, false, nullptr};
+  if ((rc = describe_sources(b, sources, n_files, n_formats, h_sample_off))) return rc;
   DeviceGuard g(m->device);
   if ((rc = load_ingest_taps(b.api, m->device, b.ingest))) return rc;
   return run_batch(m, b, nullptr, Rows{h_note, h_onset, h_contour}, params, notes, h_frame_off, m->stream);
 }
 
-int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* byte_off, int64_t* sample_off) {
-  if (n_files < 0 || (n_files > 0 && !files) || !byte_off || !sample_off)
-    return fail(BP_E_INVALID, "bp_debug_pcm_layout: bad argument");
+int bp_transcribe_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files,
+                                 const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
+                                 int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !files))
+    return fail(BP_E_INVALID, "bp_transcribe_pcm_files_host: bad argument");
+  const std::vector<bp_pcm_source_t> s = memory_sources(files, n_files);
+  return transcribe_sources("bp_transcribe_pcm_files_host", m, s.data(), n_files, kPcmFileFormats, params, h_note, h_onset, h_contour,
+                            h_frame_off, h_sample_off, notes);
+}
+
+int bp_transcribe_pcm_sources_host(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                                   const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
+                                   int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes) {
+  if (!m || !h_frame_off || n_files < 0 || (n_files > 0 && !sources))
+    return fail(BP_E_INVALID, "bp_transcribe_pcm_sources_host: bad argument");
+  return transcribe_sources("bp_transcribe_pcm_sources_host", m, sources, n_files, kBatchIngestFormats, params, h_note, h_onset, h_contour,
+                            h_frame_off, h_sample_off, notes);
+}
+
+static int pcm_layout(const std::string& api, const bp_pcm_file_t* files, const bp_pcm_source_t* sources,
+                      int32_t n_files, int n_formats, int64_t* byte_off, int64_t* sample_off) {
   std::vector<IngestFile> desc;
   std::vector<int64_t> bytes;
-  const int rc = describe_pcm("bp_debug_pcm_layout", files, n_files, false, desc, bytes);
+  const int rc = describe_pcm(api, files, n_files, false, n_formats, desc, bytes, sources);
   if (rc) return rc;
   byte_off[0] = sample_off[0] = 0;
   for (int i = 0; i < n_files; ++i) {
@@ -3797,6 +3932,20 @@ int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* by
     sample_off[i + 1] = sample_off[i] + desc[i].n_out;
   }
   return BP_OK;
+}
+
+int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* byte_off, int64_t* sample_off) {
+  if (n_files < 0 || (n_files > 0 && !files) || !byte_off || !sample_off)
+    return fail(BP_E_INVALID, "bp_debug_pcm_layout: bad argument");
+  return pcm_layout("bp_debug_pcm_layout", files, nullptr, n_files, kPcmFileFormats, byte_off, sample_off);
+}
+
+int bp_debug_pcm_sources_layout(const bp_pcm_source_t* sources, int32_t n_files, int64_t* byte_off,
+                                int64_t* sample_off) {
+  if (n_files < 0 || (n_files > 0 && !sources) || !byte_off || !sample_off)
+    return fail(BP_E_INVALID, "bp_debug_pcm_sources_layout: bad argument");
+  return pcm_layout("bp_debug_pcm_sources_layout", nullptr, sources, n_files, kBatchIngestFormats, byte_off,
+                    sample_off);
 }
 
 int64_t bp_debug_resample_filter(int32_t up, int32_t down, double* taps, int64_t capacity) {

@@ -81,6 +81,19 @@ template <>
 __device__ __forceinline__ float to_float<int>(int v) { return (float)v / 2147483648.f; }
 template <>
 __device__ __forceinline__ float to_float<unsigned char>(unsigned char v) { return ((float)v - 128.f) / 128.f; }
+// 24-bit WAV as stored: three bytes, little-endian, two's complement, 1-byte aligned.  v / 2^23 equals
+// to_float<int>(v << 8), the value of the left-justified int32 that scipy reads the same sample as.
+struct s24 {
+  unsigned char b[3];
+};
+template <>
+__device__ __forceinline__ float to_float<s24>(s24 v) {
+  const int x = ((int)((unsigned)v.b[0] << 8 | (unsigned)v.b[1] << 16 | (unsigned)v.b[2] << 24)) >> 8;
+  return (float)x / 8388608.f;
+}
+// float64 WAV: rounded to float32 first, as the host's astype(np.float32) does, then format 0's path.
+template <>
+__device__ __forceinline__ float to_float<double>(double v) { return __double2float_rn(v); }
 
 // numpy's pairwise_sum of n >= 1 converted values: below 8 a sequential sum from +0, up to 128 eight interleaved
 // accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) then the tail in order
@@ -193,7 +206,8 @@ __global__ void __launch_bounds__(kOutPerCta) ingest_kernel(const T* __restrict_
 }
 
 // Many files in one launch: file i owns CTAs [cta_off[i], cta_off[i + 1]) (none when it is empty), each CTA looks its
-// file up and runs that file's format.
+// file up and runs that file's format (0..5: the four of ingest_kernel plus packed 24-bit and float64, which only
+// whole files read from WAV files reach).
 __global__ void __launch_bounds__(kOutPerCta) ingest_batch_kernel(const IngestFile* __restrict__ files,
                                                                   const int* __restrict__ cta_off, int n_files) {
   extern __shared__ float s_x[];
@@ -215,7 +229,9 @@ __global__ void __launch_bounds__(kOutPerCta) ingest_batch_kernel(const IngestFi
     case 0: BP_INGEST_CTA(float); break;
     case 1: BP_INGEST_CTA(short); break;
     case 2: BP_INGEST_CTA(int); break;
-    default: BP_INGEST_CTA(unsigned char); break;
+    case 3: BP_INGEST_CTA(unsigned char); break;
+    case 4: BP_INGEST_CTA(s24); break;
+    default: BP_INGEST_CTA(double); break;
   }
 #undef BP_INGEST_CTA
 }
@@ -296,9 +312,9 @@ long long ingest_output_length(long long n_frames, int sample_rate) {
 }
 
 // The resampler of one sample rate without its taps: ratio, filter geometry and the inputs a CTA stages.  Host
-// arithmetic only.  0, or -2 when the format / channel count / rate is unsupported.
-int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f) {
-  if (channels < 1 || sample_rate < 1 || format < 0 || format > 3) return -2;
+// arithmetic only.  0, or -2 when the format (0 .. n_formats - 1) / channel count / rate is unsupported.
+int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f, int n_formats) {
+  if (channels < 1 || sample_rate < 1 || format < 0 || format >= n_formats) return -2;
   const long long g = gcd_ll(kSampleRate, sample_rate);
   f.format = format, f.channels = channels;
   f.up = (int)(kSampleRate / g), f.down = (int)(sample_rate / g);

@@ -277,7 +277,10 @@ struct IngestFile {
   long long n_in, n_out;
   int channels, format, up, down, half, taps, span, pad;
 };
-int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f);
+// Formats 0 float32, 1 int16, 2 int32, 3 uint8 everywhere; 4 packed 24-bit and 5 float64 only in the batched ingest
+// (n_formats = kBatchIngestFormats).
+constexpr int kBatchIngestFormats = 6;
+int ingest_geometry(int format, int channels, int sample_rate, IngestFile& f, int n_formats = 4);
 int ingest_taps(int device, IngestFile& f);
 long long ingest_ctas(long long n_out);  // CTAs a file of n_out output samples takes
 // d_files [n_files] and d_cta_off [n_files + 1] (exclusive prefix sum of ingest_ctas) in device memory; max_span: the

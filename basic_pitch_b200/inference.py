@@ -23,7 +23,7 @@ import numpy as np
 
 from . import ICASSP_2022_MODEL_PATH, _lib, evaluate, weights
 from . import note_creation as infer
-from .audio_io import load_audio, load_audio_device, pcm_descriptors, read_pcm
+from .audio_io import WavRegion, load_audio, load_audio_device, pcm_descriptors, pcm_sources, probe_wav, read_pcm
 from .constants import (
     ANNOTATIONS_FPS,
     AUDIO_N_SAMPLES,
@@ -868,7 +868,8 @@ class Model:
                  them), or (note, onset, contour, frame_off) with device tensors (anything with data_ptr(); row-major,
                  work on `stream`) -> bp_evaluate_host / bp_evaluate_device;
           audio  mono 22 050 Hz float32 arrays -> bp_evaluate_audio_host (the model runs once);
-          pcm    (samples, sample_rate) items as `transcribe_pcm` takes them -> bp_evaluate_pcm_files_host.
+          pcm    (samples, sample_rate) or `WavRegion` items as `transcribe_pcm` takes them -> bp_evaluate_pcm_files_host
+                 (bp_evaluate_pcm_sources_host when a region is among them).
         families: names from EVAL_FAMILIES; settings: the decode grid of the note-derived families (as `score_grid`);
         request: note_refs, multipitch_refs, f0_refs, salience / melody dicts {settings, references, kind}, window,
         cent_tolerance and note tolerances, as the standalone calls take them.
@@ -893,9 +894,16 @@ class Model:
             n_files = len(audio)
             lens = np.diff(offs)
         else:
-            files, keep_pcm = pcm_descriptors(pcm)
-            n_files = len(keep_pcm)
-            lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in files[:n_files]),
+            from_files = any(isinstance(it, WavRegion) for it in pcm)
+            if from_files:
+                files, keep_pcm = pcm_sources(pcm)
+                n_files = len(pcm)
+                descs = [f.pcm for f in files[:n_files]]
+            else:
+                files, keep_pcm = pcm_descriptors(pcm)
+                n_files = len(keep_pcm)
+                descs = files[:n_files]
+            lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in descs),
                                dtype=np.int64, count=n_files)
         req, keep, out = self._eval_request(n_files, families, settings, **request)
         n_params = len(settings)
@@ -919,8 +927,9 @@ class Model:
                 self._lib.bp_evaluate_audio_host(self._h, _ptr(flat), _ptr(offs), n_files, C.byref(req), _ptr(mo.get("note")),
                                                  _ptr(mo.get("onset")), _ptr(mo.get("contour")), _ptr(foff))
             else:
-                self._lib.bp_evaluate_pcm_files_host(self._h, files, n_files, C.byref(req), _ptr(mo.get("note")),
-                                                     _ptr(mo.get("onset")), _ptr(mo.get("contour")), _ptr(foff), None)
+                entry = self._lib.bp_evaluate_pcm_sources_host if from_files else self._lib.bp_evaluate_pcm_files_host
+                entry(self._h, files, n_files, C.byref(req), _ptr(mo.get("note")), _ptr(mo.get("onset")),
+                      _ptr(mo.get("contour")), _ptr(foff), None)
 
         if "pairs" in families:
             total = int(foff[-1]) if grams is not None else total
@@ -999,19 +1008,30 @@ class Model:
                        energy_tol=11, infer_onsets=True, melodia_trick=True, include_pitch_bends=True,
                        min_pitch_idx=0, max_pitch_idx=88, return_model_output: bool = True, split_notes: bool = True):
         """`transcribe_arrays` for files given as their stored samples: an item is (samples, sample_rate) as
-        `audio_io.read_pcm` returns them — (n,) or (n, channels), float32 / int16 / int32 / uint8, any rate.  ONE library
-        call (bp_transcribe_pcm_files_host): the samples go up as stored, one batched ingest per sub-batch converts,
-        down-mixes and resamples them on the device, and the forward pass reads the result there.  Same results as
-        `load_audio_device` per file followed by `transcribe_arrays`, same return value."""
-        files, keep = pcm_descriptors(items)
-        n_files = len(keep)
-        lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in files[:n_files]),
+        `audio_io.read_pcm` returns them — (n,) or (n, channels), float32 / int16 / int32 / uint8, any rate — or a
+        `WavRegion` from `audio_io.probe_wav`, whose samples the library reads from the file itself.  ONE library call
+        (bp_transcribe_pcm_files_host; bp_transcribe_pcm_sources_host when a region is among the items): the samples go
+        up as stored, one batched ingest per sub-batch converts, down-mixes and resamples them on the device, and the
+        forward pass reads the result there.  Same results as `load_audio_device` per file followed by
+        `transcribe_arrays`, same return value.  A region's file that cannot be read during the call raises OSError
+        (`_lib.BpIOError`) naming it."""
+        from_files = any(isinstance(it, WavRegion) for it in items)
+        if from_files:
+            files, keep = pcm_sources(items)
+            n_files = len(items)
+            descs = [f.pcm for f in files[:n_files]]
+        else:
+            files, keep = pcm_descriptors(items)
+            n_files = len(keep)
+            descs = files[:n_files]
+        lens = np.fromiter((self._lib.bp_resampled_length(int(f.n_frames), int(f.sample_rate)) for f in descs),
                            dtype=np.int64, count=n_files)
         p = self._params(onset_thresh, frame_thresh, min_note_len, energy_tol, infer_onsets, melodia_trick,
                          include_pitch_bends, min_pitch_idx, max_pitch_idx)
+        entry = self._lib.bp_transcribe_pcm_sources_host if from_files else self._lib.bp_transcribe_pcm_files_host
         return self._transcribe(
             lens, return_model_output, split_notes,
-            lambda note, onset, contour, foff, nt: self._lib.bp_transcribe_pcm_files_host(
+            lambda note, onset, contour, foff, nt: entry(
                 self._h, files, n_files, C.byref(p), _ptr(note), _ptr(onset), _ptr(contour), _ptr(foff), None, C.byref(nt)),
         )
 
@@ -1937,15 +1957,7 @@ def evaluate_all(
         out = model.evaluate(lib_fams, decode, audio=[np.ascontiguousarray(a, dtype=_F32) for a in audio],
                              return_model_output=return_model_output, **request)
     else:
-        items = []
-        for a in audio:
-            if isinstance(a, np.ndarray):
-                if a.ndim != 1:
-                    raise ValueError("audio must be mono (1-D)")
-                items.append((np.ascontiguousarray(a, dtype=_F32), AUDIO_SAMPLE_RATE))
-            else:
-                items.append(read_pcm(a))
-        out = model.evaluate(lib_fams, decode, pcm=items, return_model_output=return_model_output, **request)
+        out = model.evaluate(lib_fams, decode, pcm=_pcm_items(audio), return_model_output=return_model_output, **request)
     n_frames = np.diff(out["frame_off"]).tolist()
     result: Dict[str, Any] = {}
     if "notes" in fam:
@@ -1966,6 +1978,26 @@ def evaluate_all(
     return result
 
 
+def _pcm_items(audio: Sequence[Union[np.ndarray, pathlib.Path, str]], wav_in_library: bool = True) -> List[Any]:
+    """A batch of paths and arrays as the items of one `Model.transcribe_pcm` / `Model.evaluate(pcm=...)` call: files go
+    to the device as the samples they store, arrays beside them as float32 mono at 22 050 Hz, which the ingest copies
+    bit for bit.  With wav_in_library every path is probed (`audio_io.probe_wav`): an accepted WAV file becomes a
+    `WavRegion`, which the library reads itself; a declined one, and every path without wav_in_library, is read by
+    `read_pcm` as always, with its result or exception."""
+    paths = [i for i, a in enumerate(audio) if not isinstance(a, np.ndarray)]
+    found = probe_wav([audio[i] for i in paths])[0] if wav_in_library else [None] * len(paths)
+    regions = dict(zip(paths, found))
+    items: List[Any] = []
+    for i, a in enumerate(audio):
+        if isinstance(a, np.ndarray):
+            if a.ndim != 1:
+                raise ValueError("audio must be mono (1-D)")
+            items.append((np.ascontiguousarray(a, dtype=_F32), AUDIO_SAMPLE_RATE))
+        else:
+            items.append(regions[i] if regions[i] is not None else read_pcm(a))
+    return items
+
+
 def predict_batch(
     audio: Sequence[Union[np.ndarray, pathlib.Path, str]],
     model_or_model_path: Union[Model, pathlib.Path, str] = ICASSP_2022_MODEL_PATH,
@@ -1980,12 +2012,17 @@ def predict_batch(
     return_model_output: bool = True,
     build_midi: bool = True,
     lazy: bool = True,
+    wav_in_library: bool = False,
 ):
     """`predict` for many clips in one device pass (addition; no reference counterpart).
 
     Items are paths or mono 22 050 Hz float arrays.  With a path among them the batch goes through
     `Model.transcribe_pcm`: the files cross to the device once, as the samples they store, and are converted, down-mixed
-    and resampled there.  Returns a list of
+    and resampled there.  The files are read by `read_pcm` on this thread (`bp_transcribe_pcm_files_host`); with
+    wav_in_library=True (what `predict_and_save` and the CLI use) WAV files the header probe accepts
+    (`audio_io.probe_wav`) are read by the library's gather threads straight into pinned staging, 24-bit and float64
+    ones as stored (`bp_transcribe_pcm_sources_host`), and only declined files by `read_pcm`.  The results are the same
+    bit for bit, in one library call either way.  Returns a list of
     (model_output | None, midi_data | None, note_events) in input order.  The model outputs are views of three
     page-locked arrays shared by the batch.  With lazy=True (default) the note events are `NoteEventList`s and the MIDI
     objects `LazyPrettyMIDI`s: both turn into the reference's Python objects when first read; lazy=False builds
@@ -1999,17 +2036,7 @@ def predict_batch(
     if all(isinstance(a, np.ndarray) for a in audio):
         outs, arrs, frames = model.transcribe_arrays(audio, **decode)
     else:
-        # files go to the device as the samples they store; arrays beside them as float32 mono at 22 050 Hz, which the
-        # ingest copies bit for bit
-        items = []
-        for a in audio:
-            if isinstance(a, np.ndarray):
-                if a.ndim != 1:
-                    raise ValueError("audio must be mono (1-D)")
-                items.append((np.ascontiguousarray(a, dtype=_F32), AUDIO_SAMPLE_RATE))
-            else:
-                items.append(read_pcm(a))
-        outs, arrs, frames = model.transcribe_pcm(items, **decode)
+        outs, arrs, frames = model.transcribe_pcm(_pcm_items(audio, wav_in_library), **decode)
     n = len(audio)
     events = infer.note_events_batch(arrs, n, include_pitch_bends=True, lazy=lazy)
     if return_model_output and (minimum_frequency is not None or maximum_frequency is not None):
@@ -2049,7 +2076,8 @@ def predict_and_save(
     """reference: inference.py:509-604 — same files, names and failure behaviour (print, then re-raise).
 
     Several files without `debug_file` go through the batch path: one device pass per `BATCH_FILES` files
-    (`predict_batch`: GPU ingest, one library call), one `bp_write_note_files` call for their MIDI / CSV files
+    (`predict_batch(wav_in_library=True)`: GPU ingest, one library call, WAV files read by the library), one
+    `bp_write_note_files` call for their MIDI / CSV files
     (csrc/writers.cu) and, for `sonify_midi` with the bundled MIDI stand-in, one `bp_sonify_notes_host` call for their
     WAV samples (csrc/sonify.cu) instead of a Python loop over files and notes."""
 
@@ -2072,7 +2100,8 @@ def predict_and_save(
             for q in chunk:
                 print(f"\nPredicting MIDI for {q}...")
             results = predict_batch([pathlib.Path(q) for q in chunk], model, onset_threshold, frame_threshold, minimum_note_length,
-                                    minimum_frequency, maximum_frequency, multiple_pitch_bends, melodia_trick, midi_tempo)
+                                    minimum_frequency, maximum_frequency, multiple_pitch_bends, melodia_trick, midi_tempo,
+                                    wav_in_library=True)
             # the GPU renders the bundled stand-in's synthesiser; with the real pretty_midi installed, its own synthesiser
             # makes the file, one by one
             gpu_sonify = sonify_midi and infer.pretty_midi is bundled_midi

@@ -30,6 +30,7 @@ extern "C" {
 #define BP_E_CUDA (-2)     /* CUDA runtime error (message carries cudaGetErrorString)  */
 #define BP_E_CAPACITY (-3) /* caller-provided output capacity too small                */
 #define BP_E_NOMEM (-4)
+#define BP_E_IO (-5)       /* a file could not be read during the call (message names it: index and path)   */
 
 /* Geometry of the model (reference: basic_pitch/constants.py:25-47, inference.py:185-191,302-305). */
 #define BP_SAMPLE_RATE 22050
@@ -905,7 +906,7 @@ int bp_load_pcm_host(bp_model_t* m, const void* h_pcm, int32_t sample_format, in
 typedef struct bp_pcm_file {
   const void* pcm;       /* n_frames x channels samples; may be NULL when n_frames == 0 */
   int64_t n_frames;
-  int32_t sample_format; /* 0 float32, 1 int16, 2 int32, 3 uint8 */
+  int32_t sample_format; /* 0 float32, 1 int16, 2 int32, 3 uint8 (a bp_pcm_source_t also takes 4 and 5) */
   int32_t channels;
   int32_t sample_rate;
   int32_t reserved;
@@ -928,17 +929,67 @@ typedef struct bp_pcm_file {
  *   while the previous sub-batch computes, and one batched ingest leaves the signals on the device, where the forward
  *   pass reads them.  Each sample crosses PCIe once, as stored.  The staging (three pinned buffers, two on the device)
  *   is sized by the largest sub-batch in PCM bytes.  h_sample_off (may be NULL) receives the resampled lengths as
- *   offsets [n_files + 1]; everything else as bp_transcribe_files_host. */
+ *   offsets [n_files + 1]; everything else as bp_transcribe_files_host.  The same call as
+ *   bp_transcribe_pcm_sources_host on in-memory sources. */
 int bp_load_pcm_files_device(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files, float* d_audio,
                              int64_t* h_sample_off, void* stream);
 int bp_transcribe_pcm_files_host(bp_model_t* m, const bp_pcm_file_t* files, int32_t n_files,
                                  const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
                                  int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes);
-/* Host-only (no GPU needed): validates the files as the two calls above do and returns where
+
+/* One file of a batch as stored PCM either in memory (path NULL: pcm as bp_pcm_file_t) or in a file: with `path`
+ * non-NULL the n_frames x channels samples are bytes [data_offset, data_offset + size) of that file, as they lie in a
+ * WAV file's data chunk (pcm.pcm is ignored), and the library reads them itself.  pcm.sample_format takes the four
+ * formats of bp_pcm_file_t and two that WAV files bring: 4 packed signed 24-bit little-endian (3 bytes per sample,
+ * 1-byte aligned; v / 2^23, bit for bit format 2 of v << 8) and 5 float64 (8 bytes; rounded to float32, then as
+ * format 0).  Both cross PCIe as stored. */
+typedef struct bp_pcm_source {
+  bp_pcm_file_t pcm;
+  const char* path;    /* NULL: in memory */
+  int64_t data_offset; /* byte offset of the first sample in `path` (>= 0) */
+} bp_pcm_source_t;
+
+/* Host-only (no GPU needed): reads the header of each WAV file and either accepts it (accepted[i] = 1, out[i] the
+ * source that reads its samples: format, channels, rate, frame count, path = paths[i] and the byte offset of the first
+ * sample) or declines it (accepted[i] = 0, out[i] zeroed).  A file is accepted only when its reading is unambiguous and
+ * agrees with scipy.io.wavfile.read (dtype, channels, rate, frames and sample bytes; 24-bit as scipy's int32 >> 8):
+ *   - RIFF ... WAVE; chunks walked as id, little-endian size, body and a pad byte after an odd body, while the
+ *     position is below the RIFF size + 8;
+ *   - exactly one `fmt ` chunk before exactly one `data` chunk; other chunks anywhere are skipped;
+ *   - format tag 1 (PCM; byte rate = rate x block_align), 3 (IEEE float) or 0xFFFE (EXTENSIBLE, cbSize >= 22) with the
+ *     PCM or IEEE-float sub-format GUID; PCM of 8 / 16 / 24 / 32 bits -> formats 3 / 1 / 4 / 2, float of 32 / 64 bits ->
+ *     formats 0 / 5; block_align = channels x bytes per sample, channels >= 1;
+ *   - a sample rate the batched ingest takes;
+ *   - a data size that is a multiple of block_align, with the whole data chunk inside the file.
+ * Everything else is declined: RIFX, RF64 / W64, mu-law / A-law, ADPCM, 64-bit integer PCM, a missing or repeated
+ * chunk, truncation, a path that does not exist or cannot be read.  BP_E_INVALID only for bad arguments (a NULL path). */
+int bp_probe_wav_files(const char* const* paths, int32_t n_files, bp_pcm_source_t* out, int32_t* accepted);
+/* bp_transcribe_pcm_files_host / bp_evaluate_pcm_files_host over sources: in-memory files are gathered as there, and a
+ * file source is read with pread by the same gather threads straight into the pinned staging, each thread opening a
+ * file once for its share of it; files are split across threads as in-memory ones are.  Every source is validated (as
+ * bp_pcm_file_t, plus data_offset >= 0; a file source needs no pcm) and every length is known before any launch.  A
+ * file that cannot be opened, fails to read or ends before its samples do (e.g. it shrank after the probe) returns
+ * BP_E_IO with its index and path in bp_last_error(); the gather threads have ended, queued work has finished, outputs
+ * are unspecified and the model works normally on its next call. */
+int bp_transcribe_pcm_sources_host(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                                   const bp_decode_params_t* params, float* h_note, float* h_onset, float* h_contour,
+                                   int64_t* h_frame_off, int64_t* h_sample_off, bp_notes_t* notes);
+int bp_evaluate_pcm_sources_host(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files,
+                                 const bp_eval_request_t* req, float* h_note, float* h_onset, float* h_contour,
+                                 int64_t* h_frame_off, int64_t* h_sample_off);
+/* bp_load_pcm_files_device for in-memory sources (device pointers, aligned to their sample type: 1 byte for format 4)
+ * with every source format; a source with a path is BP_E_INVALID. */
+int bp_load_pcm_sources_device(bp_model_t* m, const bp_pcm_source_t* sources, int32_t n_files, float* d_audio,
+                               int64_t* h_sample_off, void* stream);
+/* Host-only (no GPU needed): validates the files as bp_load_pcm_files_device / bp_transcribe_pcm_files_host do and
+ * returns where
  * bp_transcribe_pcm_files_host would pack them if they formed one sub-batch: file i's PCM at byte_off[i] (a multiple
  * of 16) from the first file's, byte_off[n_files] the size of the packed PCM; and sample_off[n_files + 1], the offsets
  * of their 22 050 Hz signals. */
 int bp_debug_pcm_layout(const bp_pcm_file_t* files, int32_t n_files, int64_t* byte_off, int64_t* sample_off);
+/* bp_debug_pcm_layout for sources, validated as bp_transcribe_pcm_sources_host validates them (formats 0..5). */
+int bp_debug_pcm_sources_layout(const bp_pcm_source_t* sources, int32_t n_files, int64_t* byte_off,
+                                int64_t* sample_off);
 
 /* Batched writers (host threads, no GPU): one Standard MIDI File and / or one note-event CSV per file of a batch, straight
  * from the concatenated note arrays (times already in seconds).  Replaces, for batches, note_events_to_midi (reference:
