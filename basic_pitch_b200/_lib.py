@@ -25,7 +25,7 @@ EXPORTS = [
     "bp_model_create", "bp_model_destroy", "bp_model_device", "bp_model_param_block", "bp_model_refresh",
     "bp_model_launch_count", "bp_forward_device", "bp_forward_host", "bp_run_inference_device",
     "bp_run_inference_host", "bp_decode_device", "bp_decode_host", "bp_transcribe_host", "bp_transcribe_device",
-    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_schedule", "bp_debug_tc_clocks", "bp_debug_tc_cta_busy", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params", "bp_default_score_params", "bp_frame_times", "bp_score_grid_device", "bp_score_grid_host", "bp_score_notes_host", "bp_multipitch_map", "bp_score_frames_grid_device", "bp_score_frames_grid_host", "bp_score_multipitch_host", "bp_score_salience_grid_device", "bp_score_salience_grid_host", "bp_score_salience_chunk_params", "bp_match_grid_device", "bp_match_grid_host", "bp_match_notes_host", "bp_score_onset_offset_grid_device", "bp_score_onset_offset_grid_host", "bp_score_onset_offset_notes_host", "bp_melody_map", "bp_score_melody_grid_device", "bp_score_melody_grid_host", "bp_score_melody_host", "bp_score_melody_chunk_params", "bp_score_bent_frames_grid_device", "bp_score_bent_frames_grid_host", "bp_score_note_melody_grid_device", "bp_score_note_melody_grid_host", "bp_evaluate_device", "bp_evaluate_host", "bp_evaluate_audio_host", "bp_evaluate_pcm_files_host", "bp_evaluate_chunk_params", "bp_stream_create", "bp_stream_push_host", "bp_stream_end", "bp_stream_take", "bp_stream_held_frames", "bp_stream_destroy", "bp_stream_group_create", "bp_stream_group_open", "bp_stream_group_commit_offsets", "bp_stream_group_push_host", "bp_stream_group_push_frames_host", "bp_stream_group_end", "bp_stream_group_take", "bp_stream_group_held_frames", "bp_stream_group_destroy", "bp_stream_group_open_pcm", "bp_stream_group_push_pcm_host", "bp_stream_group_debug_tail", "bp_debug_pcm_stream_plan", "bp_probe_wav_files", "bp_transcribe_pcm_sources_host", "bp_evaluate_pcm_sources_host", "bp_load_pcm_sources_device", "bp_debug_pcm_sources_layout",
+    "bp_infer_onsets_host", "bp_pitch_bends_host", "bp_debug_activation", "bp_model_chunk_windows", "bp_model_set_path", "bp_model_profile", "bp_model_profile_read", "bp_debug_tc_plan", "bp_debug_tc_gather", "bp_debug_tc_gather_packed", "bp_debug_tc_b2", "bp_debug_tc_schedule", "bp_debug_tc_row_map", "bp_debug_tc_clocks", "bp_debug_tc_cta_busy", "bp_transcribe_files_host", "bp_host_alloc", "bp_host_free", "bp_last_required", "bp_resampled_length", "bp_load_pcm_device", "bp_load_pcm_host", "bp_debug_resample_filter", "bp_write_note_files", "bp_sonify_notes_host", "bp_load_pcm_files_device", "bp_transcribe_pcm_files_host", "bp_debug_pcm_layout", "bp_debug_frontend", "bp_model_set_debug_frontend", "bp_debug_chain_layout", "bp_debug_split_layout", "bp_decode_grid_device", "bp_decode_grid_host", "bp_decode_grid_chunk_params", "bp_default_score_params", "bp_frame_times", "bp_score_grid_device", "bp_score_grid_host", "bp_score_notes_host", "bp_multipitch_map", "bp_score_frames_grid_device", "bp_score_frames_grid_host", "bp_score_multipitch_host", "bp_score_salience_grid_device", "bp_score_salience_grid_host", "bp_score_salience_chunk_params", "bp_match_grid_device", "bp_match_grid_host", "bp_match_notes_host", "bp_score_onset_offset_grid_device", "bp_score_onset_offset_grid_host", "bp_score_onset_offset_notes_host", "bp_melody_map", "bp_score_melody_grid_device", "bp_score_melody_grid_host", "bp_score_melody_host", "bp_score_melody_chunk_params", "bp_score_bent_frames_grid_device", "bp_score_bent_frames_grid_host", "bp_score_note_melody_grid_device", "bp_score_note_melody_grid_host", "bp_evaluate_device", "bp_evaluate_host", "bp_evaluate_audio_host", "bp_evaluate_pcm_files_host", "bp_evaluate_chunk_params", "bp_stream_create", "bp_stream_push_host", "bp_stream_end", "bp_stream_take", "bp_stream_held_frames", "bp_stream_destroy", "bp_stream_group_create", "bp_stream_group_open", "bp_stream_group_commit_offsets", "bp_stream_group_push_host", "bp_stream_group_push_frames_host", "bp_stream_group_end", "bp_stream_group_take", "bp_stream_group_held_frames", "bp_stream_group_destroy", "bp_stream_group_open_pcm", "bp_stream_group_push_pcm_host", "bp_stream_group_debug_tail", "bp_debug_pcm_stream_plan", "bp_probe_wav_files", "bp_transcribe_pcm_sources_host", "bp_evaluate_pcm_sources_host", "bp_load_pcm_sources_device", "bp_debug_pcm_sources_layout",
 ]  # fmt: skip
 
 
@@ -327,6 +327,7 @@ def load() -> C.CDLL:
     lib.bp_debug_tc_b2.argtypes = [C.c_int, vp, vp, vp]
     lib.bp_debug_tc_clocks.argtypes = [vp, C.c_int, vp, C.c_int]
     lib.bp_debug_tc_schedule.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    lib.bp_debug_tc_row_map.argtypes = [C.c_int, C.c_int, vp, C.c_int32, vp, vp]
     lib.bp_debug_tc_cta_busy.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int]
     lib.bp_transcribe_files_host.argtypes = [vp, vp, vp, i32, C.POINTER(DecodeParams), vp, vp, vp, vp, C.POINTER(Notes)]
     lib.bp_host_alloc.argtypes = [sz]

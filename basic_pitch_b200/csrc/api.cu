@@ -110,13 +110,12 @@ __global__ void derive_kernel(const float* __restrict__ P, float* __restrict__ D
   tr(ParamLayout::onset2_w, DerivedLayout::onset2_wT, 1, 297);
 }
 
+// a[0 .. n) and b[0 .. nb), nb >= n
 __global__ void desc_upload_kernel(const int4* __restrict__ a_src, int4* __restrict__ a_dst, const int4* __restrict__ b_src,
-                                   int4* __restrict__ b_dst, int n) {
+                                   int4* __restrict__ b_dst, int n, int nb) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    a_dst[i] = a_src[i];
-    b_dst[i] = b_src[i];
-  }
+  if (i < n) a_dst[i] = a_src[i];
+  if (i < nb) b_dst[i] = b_src[i];
 }
 
 __global__ void compact_notes_kernel(const long long* __restrict__ frame_off, const long long* __restrict__ slot_off,
@@ -160,6 +159,11 @@ struct bp_model {
   Lowpass2 lp2{};  // decimation FIR taps, a parameter of every decimation launch
   DevBuf<uint16_t> cqt_wtc;  // three-way bf16 split of the CQT kernel matrix (tensor-core path)
   size_t chl_zeroed = 0;  // elements of chl known to hold zeros in every row/bin the kernels never write
+  // uniform row maps of a whole chunk, [layer][chunk] (TcRowWin); the trimmed ones come with each call's descriptors
+  DevBuf<TcRowWin> umap;
+  // a trimmed forward wrote the split operands in its own row layout: chl holds rows where the uniform layout keeps
+  // zeros, and yhl is not the uniform split of the last forward
+  bool chl_trimmed = false, split_trimmed = false;
   int64_t launches = 0;
   // forward workspace (chunk windows)
   DevBuf<float> chain, y, c1, n1, o1;
@@ -395,9 +399,52 @@ int ensure_forward_ws(bp_model* m, int nb) {
     if (m->chl.p != before || m->chl_zeroed < m->chl.cap) {  // separator rows / pad bins are never written: zero once
       CK(cudaMemset(m->chl.p, 0, m->chl.cap * sizeof(__nv_bfloat16)));
       m->chl_zeroed = m->chl.cap;
+      m->chl_trimmed = false;
     }
   }
+  if (!m->umap.p) {
+    std::vector<TcRowWin> h((size_t)3 * m->chunk);
+    int lo1, lo2;
+    for (int l = 0; l < 3; ++l) tc_row_map(l, false, nullptr, m->chunk, h.data() + (size_t)l * m->chunk, &lo1, &lo2);
+    CK(m->umap.reserve(h.size()));
+    CK(cudaMemcpy(m->umap.p, h.data(), h.size() * sizeof(TcRowWin), cudaMemcpyHostToDevice));
+  }
   return BP_OK;
+}
+
+// The trimmed row maps of a call's windows (TcRowWin), chunk by chunk: the bases start again at every chunk of `chunk`
+// windows.  out[0 .. n): the contour / onset map (they share the split of y), out[n .. 2 n): the note map; n_rows[2 c],
+// n_rows[2 c + 1]: the rows of those two row spaces in chunk c.
+void build_trim_maps(const UnwrapDesc* ud, long long n, int chunk, TcRowWin* out, std::vector<int>& n_rows) {
+  n_rows.clear();
+  std::vector<int> kept((size_t)chunk);
+  for (long long c0 = 0; c0 < n; c0 += chunk) {
+    const int nb = (int)std::min<long long>(chunk, n - c0);
+    for (int b = 0; b < nb; ++b) kept[b] = ud[c0 + b].rows;
+    int lo1, lo2;
+    n_rows.push_back(tc_row_map(0, true, kept.data(), nb, out + c0, &lo1, &lo2));
+    n_rows.push_back(tc_row_map(2, true, kept.data(), nb, out + n + c0, &lo1, &lo2));
+  }
+}
+
+// The row maps forward_chunk runs a chunk with: trimmed (path 1 with unwrap) or the model's uniform ones.
+struct ChunkRows {
+  TcRows layer[3];
+};
+ChunkRows chunk_rows(const bp_model* m, int nb, const TcRowWin* trim_map, long long trim_stride, const int* trim_rows) {
+  ChunkRows r;
+  for (int l = 0; l < 3; ++l) {
+    TcRows& x = r.layer[l];
+    if (trim_map) {
+      x.map = trim_map + (l == 2 ? trim_stride : 0);
+      x.n_rows = trim_rows[l == 2 ? 1 : 0];
+      tc_row_map(l, true, nullptr, 0, nullptr, &x.lo1, &x.lo2);
+    } else {
+      x.map = m->umap.p + (size_t)l * m->chunk;
+      x.n_rows = tc_row_map(l, false, nullptr, nb, nullptr, &x.lo1, &x.lo2);
+    }
+  }
+  return r;
 }
 
 // Row-major posteriorgram staging of the model (st_note / st_onset / st_contour) for `n_frames` frames.
@@ -448,8 +495,11 @@ struct PostI {
 // With `ud` (bp_run_inference_*): the centre frames of every window go to their unwrapped position in the internal
 // posteriorgrams `u` — straight from the fused epilogues on the tensor-core path, through a layout conversion of the
 // row-major raw windows on the FP32 path; note / onset / contour are then optional row-major scratch.
+// trim_map / trim_rows (path 1 with `ud` only): the chunk's trimmed row maps, the contour / onset map at trim_map and the
+// note map at trim_map + trim_stride, and their rows (build_trim_maps).  Without them every layer computes whole windows.
 int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, float* note, float* onset,
-                  float* contour, cudaStream_t st, const UnwrapDesc* ud = nullptr, const PostI* u = nullptr) {
+                  float* contour, cudaStream_t st, const UnwrapDesc* ud = nullptr, const PostI* u = nullptr,
+                  const TcRowWin* trim_map = nullptr, long long trim_stride = 0, const int* trim_rows = nullptr) {
   float* chain = m->chain.p;
   if (m->profile_which >= 0) m->prof_windows += nb;
   {
@@ -460,6 +510,13 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
   const int ystride = tc_rows_total(m->chunk, cs.rows_per_window), cstride = tc_rows_total(m->chunk, ns.rows_per_window);
   const long long fr = (long long)m->chunk * kFrames;  // frame stride of the internal raw buffers
   const long long nfr = (long long)nb * kFrames;
+  const bool trim = m->path == 1 && ud;  // only the frames the unwrapped posteriorgrams keep
+  if (trim && !trim_map) return fail(BP_E_INVALID, "forward_chunk: unwrapping without row maps");
+  const ChunkRows rows = chunk_rows(m, nb, trim ? trim_map : nullptr, trim_stride, trim_rows);
+  if (m->path >= 1 && !trim && m->chl_trimmed) {  // the uniform note layer reads zeros between its windows
+    CK(cudaMemsetAsync(m->chl.p, 0, m->chl.cap * sizeof(__nv_bfloat16), st));
+    m->chl_trimmed = false;
+  }
   {
     ProfScope ps(m, 2, st);
     if (m->path >= 1) {
@@ -467,7 +524,9 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
                     m->n_sms, st);
       if (m->debug_frontend) CK(cudaMemcpyAsync(m->ylog.p, m->y.p, sizeof(float) * nb * kFrames * kCqtBins, cudaMemcpyDeviceToDevice, st));
       // NormalizedLog + BatchNorm straight into the bf16 hi/lo split the convs read
-      launch_lognorm_split(m->y.p, m->minmax.p, m->d_params + ParamLayout::bn, m->yhl.p, cs, nb, ystride, st);
+      launch_lognorm_split(m->y.p, m->minmax.p, m->d_params + ParamLayout::bn, m->yhl.p, cs, rows.layer[0], nb, ystride,
+                           st);
+      m->split_trimmed = trim;
       m->y_is_log = true;
     } else {
       launch_cqt(audio, desc, chain, m->d_derived + DerivedLayout::cqt_wt, m->d_params + ParamLayout::cqt_scale, m->y.p,
@@ -493,12 +552,13 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
         o.chl = m->chl.p;
         o.chl_rows = cstride;
         o.chl_chunks = ns.chunks8;
-        o.chl_rpw = ns.rows_per_window;
+        o.chl_map = rows.layer[2].map;
         o.chl_lead = ns.lead_rows;
+        m->chl_trimmed = m->chl_trimmed || trim;
       } else {
         o.act = m->c1.p;  // channels-last activations
       }
-      launch_conv_tc(m->yhl.p, m->tc[0].dev, o, nb, ystride, m->n_sms, st, /*fuse_next=*/m->path == 1);
+      launch_conv_tc(m->yhl.p, m->tc[0].dev, o, nb, rows.layer[0], ystride, m->n_sms, st, /*fuse_next=*/m->path == 1);
     }
     {
       ProfScope ps(m, 4, st);
@@ -513,7 +573,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
       o.unwrapped = ud ? u->note : nullptr;
       o.frame_stride = ud ? u->stride : 0;
       o.edge = m->edge.p;
-      launch_conv_tc(m->chl.p, m->tc[2].dev, o, nb, cstride, m->n_sms, st);
+      launch_conv_tc(m->chl.p, m->tc[2].dev, o, nb, rows.layer[2], cstride, m->n_sms, st);
     }
     {
       ProfScope ps(m, 1, st);
@@ -525,7 +585,7 @@ int forward_chunk(bp_model* m, const float* audio, const WinDesc* desc, int nb, 
       o.frame_stride = ud ? u->stride : 0;
       o.note_raw = m->i_note.p;
       o.edge = m->edge.p;
-      launch_conv_tc(m->yhl.p, m->tc[1].dev, o, nb, ystride, m->n_sms, st);
+      launch_conv_tc(m->yhl.p, m->tc[1].dev, o, nb, rows.layer[1], ystride, m->n_sms, st);
     }
     if (!ud) {  // raw windows for the caller: internal -> row-major
       launch_pm_to_rows(m->i_note.p, fr, 0, nfr, kPitches, note, st);
@@ -1359,7 +1419,11 @@ static int run_inference_internal(bp_model* m, const float* d_audio, const int64
   }
   if (m->path != 1) CK(m->raw_contour.reserve((size_t)nbmax * kFrames * kContourBins));
   CK(m->wdesc.reserve(nwin));
-  CK(m->udesc.reserve(nwin));
+  // the unwrap descriptors, then the trimmed row maps of the windows (path 1: build_trim_maps): 16-byte records alike
+  static_assert(sizeof(TcRowWin) == sizeof(UnwrapDesc), "row maps travel with the unwrap descriptors");
+  const bool trim = m->path == 1;
+  const int64_t n_ud = trim ? 3 * nwin : nwin;
+  CK(m->udesc.reserve(n_ud));
   // descriptors go through pinned staging owned by the model, guarded by an event that completes with the copy (not with
   // the kernels queued behind it): no stream synchronisation here, so back-to-back calls (the sub-batches of
   // bp_transcribe_host) keep the GPU queue full
@@ -1367,13 +1431,13 @@ static int run_inference_internal(bp_model* m, const float* d_audio, const int64
     CK(cudaEventSynchronize(m->desc_ev));
     m->desc_pending = false;
   }
-  if ((size_t)nwin > m->h_desc_cap) {
+  if ((size_t)n_ud > m->h_desc_cap) {
     if (m->h_wd) cudaFreeHost(m->h_wd);
     if (m->h_ud) cudaFreeHost(m->h_ud);
     m->h_wd = nullptr;
     m->h_ud = nullptr;
     m->h_desc_cap = 0;
-    const size_t cap = std::max<size_t>((size_t)nwin, 4096);
+    const size_t cap = std::max<size_t>((size_t)n_ud, 4096);
     CK(cudaMallocHost(&m->h_wd, sizeof(WinDesc) * cap));
     CK(cudaMallocHost(&m->h_ud, sizeof(UnwrapDesc) * cap));
     m->h_desc_cap = cap;
@@ -1381,20 +1445,23 @@ static int run_inference_internal(bp_model* m, const float* d_audio, const int64
   if (!m->desc_ev) CK(cudaEventCreateWithFlags(&m->desc_ev, cudaEventDisableTiming));
   std::memcpy(m->h_wd, wd.data(), sizeof(WinDesc) * nwin);
   std::memcpy(m->h_ud, ud.data(), sizeof(UnwrapDesc) * nwin);
+  std::vector<int> trim_rows;
+  if (trim) build_trim_maps(ud.data(), nwin, chunk, reinterpret_cast<TcRowWin*>(m->h_ud + nwin), trim_rows);
   // a kernel reads the pinned (device-mapped) staging directly: a copy-engine transfer would queue behind the audio
   // uploads that bp_transcribe_host has in flight on the copy stream
   static_assert(sizeof(WinDesc) == 16 && sizeof(UnwrapDesc) == 16, "descriptor upload moves 16-byte records");
-  desc_upload_kernel<<<(unsigned)((nwin + 255) / 256), 256, 0, st>>>(
+  desc_upload_kernel<<<(unsigned)((n_ud + 255) / 256), 256, 0, st>>>(
       reinterpret_cast<const int4*>(m->h_wd), reinterpret_cast<int4*>(m->wdesc.p), reinterpret_cast<const int4*>(m->h_ud),
-      reinterpret_cast<int4*>(m->udesc.p), (int)nwin);
+      reinterpret_cast<int4*>(m->udesc.p), (int)nwin, (int)n_ud);
   CKL();
   m->launches += 1;
   CK(cudaEventRecord(m->desc_ev, st));
   m->desc_pending = true;
   for (int64_t c0 = 0; c0 < nwin; c0 += chunk) {
     const int nb = (int)std::min<int64_t>(chunk, nwin - c0);
+    const TcRowWin* maps = reinterpret_cast<const TcRowWin*>(m->udesc.p + nwin);
     rc = forward_chunk(m, d_audio, m->wdesc.p + c0, nb, m->raw_note.p, m->raw_onset.p, m->raw_contour.p, st,
-                       m->udesc.p + c0, &u);
+                       m->udesc.p + c0, &u, trim ? maps + c0 : nullptr, nwin, trim ? trim_rows.data() + 2 * (c0 / chunk) : nullptr);
     if (rc) return rc;
   }
   m->last_forward_n = std::min<int64_t>(nwin, chunk) == nwin ? nwin : 0;
@@ -4028,6 +4095,19 @@ int bp_debug_tc_clocks(bp_model_t* m, int which, uint64_t* cycles, int reset) {
   return BP_OK;
 }
 
+int bp_debug_tc_row_map(int which, int trimmed, const int32_t* kept, int32_t n_windows, int32_t* map, int32_t* info) {
+  if (!info || which < 0 || which > 2 || n_windows < 0 || (n_windows > 0 && ((trimmed && !kept) || !map)))
+    return fail(BP_E_INVALID, "bp_debug_tc_row_map: bad argument");
+  std::vector<TcRowWin> w((size_t)n_windows);
+  info[0] = tc_row_map(which, trimmed != 0, kept, n_windows, w.data(), &info[1], &info[2]);
+  for (int b = 0; b < n_windows; ++b) {
+    map[3 * b] = w[b].base;
+    map[3 * b + 1] = w[b].first;
+    map[3 * b + 2] = w[b].rows;
+  }
+  return BP_OK;
+}
+
 int bp_debug_tc_schedule(int which, int fused, int n_windows, int n_sms, int32_t* sizes, int32_t* items, uint32_t* edges) {
   if (!sizes || which < 0 || which > 2 || n_windows < 1 || n_sms < 1)
     return fail(BP_E_INVALID, "bp_debug_tc_schedule: bad argument");
@@ -4184,6 +4264,9 @@ int bp_debug_frontend(bp_model_t* m, int which, void* h_out, int64_t n_windows) 
     case 3: {
       if (m->last_path < 1)
         return fail(BP_E_INVALID, "bp_debug_frontend: the split operand exists only on the tensor-core paths (1 and 2)");
+      if (m->split_trimmed)
+        return fail(BP_E_INVALID, "bp_debug_frontend: the last forward wrote the split operand in its trimmed row layout "
+                                  "(path 1 with unwrap); the uniform layout comes from bp_forward_*");
       constexpr TcConvSpec cs = tc_spec(0);
       const size_t n = (size_t)2 * cs.chunks8 * 8 * tc_rows_total(m->chunk, cs.rows_per_window);
       CK(cudaMemcpy(h_out, m->yhl.p, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
@@ -4830,13 +4913,21 @@ int group_run(bp_stream_group* g, const std::vector<int>& ids, const int64_t* le
   CK(m->u_note.reserve((size_t)stride * kPitches));
   CK(m->u_onset.reserve((size_t)stride * kPitches));
   CK(m->u_contour.reserve((size_t)stride * kContourBins));
+  // path 1: the trimmed row maps of the windows go behind the unwrap descriptors, in the same copy (build_trim_maps)
+  const bool trim = m->path == 1;
+  std::vector<int> trim_rows;
+  if (trim) {
+    ud.resize(3 * nwin);
+    build_trim_maps(ud.data(), nwin, chunk, reinterpret_cast<TcRowWin*>(ud.data() + nwin), trim_rows);
+  }
   if ((rc = upload(g->wd, wd, st)) || (rc = upload(g->ud, ud, st)) || (rc = upload(g->dst_row, dst, st))) return rc;
   const PostI u{m->u_note.p, m->u_onset.p, m->u_contour.p, stride};
   const int c = g->fcur;
   for (long long c0 = 0; c0 < nwin; c0 += chunk) {
     const int nb = (int)std::min<long long>(chunk, nwin - c0);
+    const TcRowWin* maps = reinterpret_cast<const TcRowWin*>(g->ud.p + nwin);
     rc = forward_chunk(m, g->audio[g->acur].p, g->wd.p + c0, nb, m->raw_note.p, m->raw_onset.p, m->raw_contour.p, st,
-                       g->ud.p + c0, &u);
+                       g->ud.p + c0, &u, trim ? maps + c0 : nullptr, nwin, trim ? trim_rows.data() + 2 * (c0 / chunk) : nullptr);
     if (rc) return rc;
     launch_group_unwrap(u.note, u.onset, u.contour, stride, g->dst_row.p + c0, nb, g->note[c].p, g->onset[c].p,
                         g->contour[c].p, true, st);

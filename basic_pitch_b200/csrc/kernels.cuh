@@ -191,6 +191,7 @@ void tc_build_b2(int layer, const float* w2, std::vector<uint16_t>& out);
 // the same tiles placed into the K = 128 x N = width conv2 weight matrix the kernel reads (tc_conv.cu)
 void tc_build_b2_full(int layer, const float* w2, std::vector<uint16_t>& out);
 int tc_rows_total(int n_windows, int rows_per_window);
+int tc_rows_used(int n_rows);  // split rows a launch over n_rows rows of a row space reads (lead + rows + the last M-tile)
 size_t tc_edge_floats(const TcConvSpec& spec, int n_windows);  // size of the edge buffer of a fused layer
 int tc_setup();  // 0 on success
 // cycle sums by role of one layer's conv_tc_kernel launches (tc::TcClk order), optionally reset; -1 unless the library
@@ -206,12 +207,35 @@ struct UnwrapDesc {
   int rows;            // how many of its 142 centre frames are kept (may be <= 0)
   int pad;
 };
+// The row space of a tensor-core layer (DESIGN §4.1): window b of a launch holds the input rows [base, base + rows) of
+// the layer's split operand (row lead + base + i of the buffer = frame first + i of the window); the layer's conv1 rows
+// and output frames have the same indices.  Conv1 row / output frame i of a window is live iff lo1 / lo2 <= i < rows -
+// lo1 / lo2; a live row reads only rows of its own window, every other row is computed and dropped.
+//   uniform (every forward without unwrap, path 2, the debug hooks): base = b * rows_per_window, first 0, rows 172,
+//     lo1 = lo2 = 0: whole windows, the zero rows between them are the "same" padding in time;
+//   trimmed (path 1 with unwrap): only the frames the kept centre frames [15, 15 + r) depend on, back to back: window b
+//     holds frames [15 - M, 15 + r + M) (M = tc_trim_margin), none if r <= 0.
+struct TcRowWin {
+  int base, first, rows, pad;
+};
+struct TcRows {
+  const TcRowWin* map = nullptr;  // device, [n_windows]
+  int n_rows = 0;                 // rows the M-tiles cover (uniform: n_windows * rows_per_window)
+  int lo1 = 0, lo2 = 0;
+};
+// trimmed row maps: input frames kept on each side of the centre frames by the split layout a layer reads (contour and
+// onset share the split of y: 10; note: 7), and output frames each side that later layers read (contour 7, onset 0, note 1)
+__host__ __device__ constexpr int tc_trim_margin(int layer) { return layer == 2 ? 7 : 10; }
+__host__ __device__ constexpr int tc_trim_out(int layer) { return layer == 0 ? 7 : layer == 1 ? 0 : 1; }
+// the map of n windows into out[n] (out may be null); kept[b]: the centre frames window b keeps (UnwrapDesc::rows),
+// unused when uniform.  Returns the rows of the row space and sets the live margins.
+int tc_row_map(int layer, bool trimmed, const int* kept, int n, TcRowWin* out, int* lo1, int* lo2);
 // NormalizedLog + folded BatchNorm of the CQT log-magnitudes straight into the bf16 hi/lo split operand (k-chunk-major
 // row layout of tc_spec(0) / tc_spec(1)); `y` itself is left untouched (launch_lognorm makes the fp32 copy).
-// rows_stride: row stride of the split layout (>= tc_rows_total(n_windows, ...)); fixed per model so that rows the
-// kernels never write (separators, pads) keep their zeros across batches of different size
+// rows_stride: row stride of the split layout (>= tc_rows_used(rows.n_rows)), fixed per model.  Every row of
+// [0, tc_rows_used(rows.n_rows)) is written: frame first + i of window b at row lead + base + i, zero in every other row.
 void launch_lognorm_split(const float* y, const unsigned int* minmax, const float* bn, __nv_bfloat16* dst,
-                          const TcConvSpec& spec, int n_windows, int rows_stride, cudaStream_t st);
+                          const TcConvSpec& spec, const TcRows& rows, int n_windows, int rows_stride, cudaStream_t st);
 // Outputs of a fused layer.  Device-internal posteriorgram layouts have the FRAME index fastest, so that the epilogue
 // threads (one frame each, 32 consecutive frames per warp) store coalesced, and so that the decode kernels read coalesced:
 //   note / onset   pitch-major   pm[pitch][frame]                 frame stride = number of frames the buffer holds
@@ -227,16 +251,19 @@ struct TcOut {
   const UnwrapDesc* ud = nullptr;
   const float* note_raw = nullptr;  // onset layer: the raw pitch-major note posteriorgram (input channel 0 of its conv2)
   __nv_bfloat16* chl = nullptr;     // contour layer: split operand of the note conv [2][chl_chunks][chl_rows][8]
-  int chl_rows = 0, chl_chunks = 0, chl_rpw = 0, chl_lead = 0;
+  const TcRowWin* chl_map = nullptr;  // the note layer's row map: frame t of window b goes to row chl_lead + base + t - first
+  int chl_rows = 0, chl_chunks = 0, chl_lead = 0;
   float* edge = nullptr;            // >= tc_edge_floats(spec, n_windows) floats of scratch
   float* act = nullptr;             // unfused contour (path 2): channels-last activations [B][172][WOUT][COUT]
 };
 // fuse_next (contour layer only; the other two always fuse): also compute the following conv in the epilogue instead
-// of storing the channels-last activations
-void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& out, int n_windows, int rows_stride,
-                    int n_sms, cudaStream_t st, bool fuse_next = false);
-// The items launch_conv_tc runs for a batch of n_windows on n_sms SMs (fused: the M-tiles of the fused epilogue,
-// which overlap by KH2 - 1 rows; the onset and note layers always fuse).  ms: frames an M-tile finishes.
+// of storing the channels-last activations.  rows: the layer's row space (TcRowWin); nothing is launched without rows.
+void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& out, int n_windows, const TcRows& rows,
+                    int rows_stride, int n_sms, cudaStream_t st, bool fuse_next = false);
+// The items launch_conv_tc runs over n_rows rows of a layer's row space on n_sms SMs (fused: the M-tiles of the fused
+// epilogue, which overlap by KH2 - 1 rows; the onset and note layers always fuse).  ms: frames an M-tile finishes.
+TcSchedule tc_schedule_rows(int layer, bool fused, int n_rows, int n_sms, int* ms = nullptr);
+// the same for n_windows whole windows (the uniform row map)
 TcSchedule tc_schedule(int layer, bool fused, int n_windows, int n_sms, int* ms = nullptr);
 // contour conv2 on the channels-last output of the tensor-core contour conv; also emits the bf16 hi/lo split of the
 // contour posteriorgram in the layout of tc_spec(2)

@@ -27,7 +27,8 @@
 //
 // Formulation of the contour conv1 ("Toeplitz along frequency on aligned chunks"; the onset and note conv1 gather instead,
 // see below)
-//   rows  m = b*174 + t            time frames of all windows of the chunk, two zero rows between windows
+//   rows  m                        the layer's row space (TcRowWin, kernels.cuh): whole windows of 172 frames with two
+//                                  zero rows between them (m = b*174 + t), or only the frames the unwrap keeps need
 //   D[m][(fl,co)] (+)= A[m+dt][8c .. 8c+15] x T(dt,off)[16][(fl,co)]
 //     A      the normalised CQT y itself (NOT the 8-channel stack), rows shifted by the time tap dt; K = 16 bins that
 //            start on an 8-bin chunk of the k-chunk-major layout
@@ -524,7 +525,8 @@ void tc_build_b2_full(int layer, const float* w2, std::vector<uint16_t>& out) {
 
 // ------------------------------------------------------------------------------------------------
 // fp32 rows -> bf16 hi/lo planes in the k-chunk-major row layout the MMA reads:
-//   dst[plane][q8 (chunks8)][row d (rows_total)][8],  d = lead + b*rows_per_window + t, every other row zero.
+//   dst[plane][q8 (chunks8)][row d (rows_total)][8],  d = lead + base + i for frame first + i of window b (the layer's
+//   row map, TcRowWin), every other row zero.
 // lognorm_split_kernel: the log-magnitude of the CQT kernel -> NormalizedLog (reference: layers/signal.py:177-183:
 //   (L - min) / (max - min), 0 when max == min) + folded BatchNorm (models.py:188-189) as the split operand of the
 //   contour / onset convs (309 bins -> 40 chunks).  (The fp32 copy is only produced on request: launch_lognorm.)
@@ -542,9 +544,22 @@ __device__ __forceinline__ void store_split8(const float (&v)[8], __nv_bfloat16*
   *reinterpret_cast<uint4*>(dst + plane + off) = *reinterpret_cast<const uint4*>(lo);
 }
 
+// The window of row m of a layer's row space (TcRowWin): the last b with map[b].base <= m (0 for m < 0).  The row is one
+// of the window's own rows iff 0 <= m - base < rows.
+__device__ __forceinline__ int tc_row_window(const TcRowWin* __restrict__ map, int n_windows, int m) {
+  int lo = 0, hi = n_windows;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(&map[mid].base) <= m) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
 __global__ void lognorm_split_kernel(const float* __restrict__ y, const unsigned int* __restrict__ minmax,
-                                     const float* __restrict__ bn, __nv_bfloat16* __restrict__ dst, int n_windows,
-                                     int rows_used, int rows_total /* stride */, int chunks8, int rows_per_window, int lead) {
+                                     const float* __restrict__ bn, __nv_bfloat16* __restrict__ dst,
+                                     const TcRowWin* __restrict__ map, int n_windows, int rows_used,
+                                     int rows_total /* stride */, int chunks8, int lead) {
   // one (row, pair of chunks q8, q8 + chunks8 / 2) per thread: the two 32-byte loads are independent (the kernel is bound by
   // load latency, not bandwidth); rows fastest, so the 16-byte stores of a warp are contiguous
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -560,8 +575,10 @@ __global__ void lognorm_split_kernel(const float* __restrict__ y, const unsigned
     for (int j = 0; j < 8; ++j) v[h][j] = 0.f;
   const int m = d - lead;
   if (m >= 0) {
-    const int b = m / rows_per_window, t = m - b * rows_per_window;
-    if (b < n_windows && t < kFrames) {
+    const int b = tc_row_window(map, n_windows, m);
+    const TcRowWin w = map[b];
+    const int i = m - w.base, t = w.first + i;
+    if (i < w.rows) {
       const float bn_scale = __ldg(bn), bn_bias = __ldg(bn + 1);
       const float mn = ordered_to_float(minmax[2 * b]);
       const float mx = __fsub_rn(ordered_to_float(minmax[2 * b + 1]), mn);
@@ -602,7 +619,9 @@ struct TcArgs {
   TcOut o;                      // where the results go (kernels.cuh)
   int edge_rows;                // row stride of o.edge: [edge slot][side 2][KE][edge_rows]
   int rows_total, n_windows;
-  TcSchedule sch;               // the launch's items: (M-tile, range of frequency groups), see tc_schedule
+  const TcRowWin* map;          // the layer's row map (TcRowWin) and its live margins
+  int lo1, lo2;
+  TcSchedule sch;             // the launch's items: (M-tile, range of frequency groups), see tc_schedule
   int row0;                     // first data row of M-tile 0
   // = tc_spec(layer).chunks8: a run-time trip count keeps the producer's per-chunk copy loop rolled, which keeps the
   // contour's producer and MMA-issue loop state in uniform registers (a compile-time count unrolls it and they move out)
@@ -1132,15 +1151,17 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       int mt, g0, g1;
       a.sch.item(it, L.G0, mt, g0, g1);
-      // conv1 rows of the thread's fragment (relu(conv1) of a row that is not a live frame is the zero padding in time)
+      // conv1 rows of the thread's fragment (relu(conv1) of a row that is not live is the zero padding in time)
       bool live[2];
       int rb[2], rt[2];
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
-        const int m = mt * a.ms - a.h2 + fr0 + 8 * rr;  // row of the (window, frame) space: m = b * rows_per_window + t
-        rb[rr] = m >= 0 ? m / L.rows_per_window : 0;
-        rt[rr] = m - rb[rr] * L.rows_per_window;
-        live[rr] = m >= 0 && (rb[rr] < a.n_windows) && (rt[rr] < kFrames);
+        const int m = mt * a.ms - a.h2 + fr0 + 8 * rr;  // row of the layer's row space (TcRowWin)
+        rb[rr] = tc_row_window(a.map, a.n_windows, m);
+        const TcRowWin w = a.map[rb[rr]];
+        const int i = m - w.base;
+        rt[rr] = w.first + i;
+        live[rr] = i >= a.lo1 && i < w.rows - a.lo1;
       }
       // Fused layers: threads 0..63 of the group each finish the output frame of one tile row, h2 rows earlier than the
       // conv1 row (all time taps of the fused conv2 then lie at or below the row); rows < 2 h2 are finished by the
@@ -1151,8 +1172,10 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
       if constexpr (kFused) {
         const int row = tid;
         const int q = mt * a.ms - 2 * a.h2 + row;
-        const int b = q >= 0 ? q / L.rows_per_window : 0, t = q - b * L.rows_per_window;
-        ro.ok = row < 64 && row >= 2 * a.h2 && q >= 0 && b < a.n_windows && t < kFrames;
+        const int b = tc_row_window(a.map, a.n_windows, q);
+        const TcRowWin w = a.map[b];
+        const int i = q - w.base, t = w.first + i;
+        ro.ok = row < 64 && row >= 2 * a.h2 && i >= a.lo2 && i < w.rows - a.lo2;
         ro.t = t;
         if (ro.ok) {
           ro.edge = a.o.edge + q;
@@ -1163,7 +1186,8 @@ __global__ void __launch_bounds__(tc::kThreads, 1) conv_tc_kernel(const __grid_c
             if ((unsigned)tt < (unsigned)max(u.rows, 0)) uf = (int)(u.dst_base + tt);
           }
           if constexpr (LAYER == 0) {
-            ro.chl = a.o.chl + ((size_t)a.o.chl_lead + (size_t)b * a.o.chl_rpw + t) * 8;
+            const TcRowWin nw = a.o.chl_map[b];
+            ro.chl = a.o.chl + ((size_t)a.o.chl_lead + nw.base + (t - nw.first)) * 8;
             if (a.o.raw) ro.raw = a.o.raw + ((size_t)b * kFrames + t) * 8;
             if (uf >= 0) ro.unw = a.o.unwrapped + (size_t)uf * 8;
           } else {
@@ -1353,6 +1377,8 @@ struct EdgeFixArgs {
   uint32_t edges_full, edges_tail;
   int tail_row0;
   int n_windows;
+  const TcRowWin* map;  // the layer's row map and its live output margin
+  int lo2;
   float bias2, note_w[9];  // the layer's conv2 bias; onset: the conv2 weights of the note input channel
 };
 
@@ -1383,7 +1409,8 @@ __device__ __forceinline__ void edge_fix_boundary(const EdgeFixArgs& a, int ft_b
       vb[2 + q] = lo[(size_t)(4 + q) * a.edge_rows];  // bins 16 ft_b + 2 .. + 7
     }
     va[6] = fx[0], va[7] = fx[1], vb[0] = fx[2], vb[1] = fx[3];
-    __nv_bfloat16* chl = a.o.chl + ((size_t)a.o.chl_lead + (size_t)b * a.o.chl_rpw + t) * 8;
+    const TcRowWin nw = a.o.chl_map[b];
+    __nv_bfloat16* chl = a.o.chl + ((size_t)a.o.chl_lead + nw.base + (t - nw.first)) * 8;
     const size_t plane = (size_t)a.o.chl_chunks * a.o.chl_rows * 8;
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
@@ -1423,13 +1450,14 @@ __device__ __forceinline__ void edge_fix_boundary(const EdgeFixArgs& a, int ft_b
 
 template <int LAYER>
 __global__ void edge_fix_kernel(const EdgeFixArgs a) {
-  constexpr TcConvSpec L = tc_spec(LAYER);
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)a.n_rows * kEdgeThreads<LAYER>) return;
   const int R = (int)(idx % a.n_rows);  // rows fastest: coalesced reads of the edge buffer, coalesced stores
   const int k = (int)(idx / a.n_rows);
-  const int b = R / L.rows_per_window, t = R - b * L.rows_per_window;
-  if (b >= a.n_windows || t >= kFrames) return;
+  const int b = tc_row_window(a.map, a.n_windows, R);
+  const TcRowWin w = a.map[b];
+  const int i = R - w.base, t = w.first + i;
+  if (i < a.lo2 || i >= w.rows - a.lo2) return;  // the rows the conv kernel finishes (ro.ok)
   int uf = -1;
   if (a.o.ud) {
     const UnwrapDesc u = a.o.ud[b];
@@ -1441,9 +1469,29 @@ __global__ void edge_fix_kernel(const EdgeFixArgs a) {
     edge_fix_boundary<LAYER>(a, __ffs(m) - 1, R, b, t, uf, k);
 }
 // ------------------------------------------------------------------------------------------------
-int tc_rows_total(int n_windows, int rows_per_window) {
+int tc_rows_used(int n_rows) {
   // lead rows + the rows of the windows + what the last (overlapping) M-tile and its time taps may touch
-  return n_windows * rows_per_window + tc::kMTile + 16;
+  return n_rows + tc::kMTile + 16;
+}
+int tc_rows_total(int n_windows, int rows_per_window) { return tc_rows_used(n_windows * rows_per_window); }
+
+int tc_row_map(int layer, bool trimmed, const int* kept, int n, TcRowWin* out, int* lo1, int* lo2) {
+  const TcConvSpec sp = tc_spec(layer);
+  const int M = tc_trim_margin(layer), h2 = (sp.KH2 - 1) / 2;
+  int base = 0;
+  for (int b = 0; b < n; ++b) {
+    if (!trimmed) {
+      if (out) out[b] = TcRowWin{b * sp.rows_per_window, 0, kFrames, 0};
+      continue;
+    }
+    const int r = std::min(kept[b], kFrames - 2 * kOverlapHalf);
+    const int rows = r > 0 ? r + 2 * M : 0;
+    if (out) out[b] = TcRowWin{base, kOverlapHalf - M, rows, 0};
+    base += rows;
+  }
+  *lo2 = trimmed ? M - tc_trim_out(layer) : 0;
+  *lo1 = trimmed ? *lo2 - h2 : 0;
+  return trimmed ? base : n * sp.rows_per_window;
 }
 
 int tc_setup() {
@@ -1456,14 +1504,14 @@ int tc_setup() {
 }
 
 void launch_lognorm_split(const float* y, const unsigned int* minmax, const float* bn, __nv_bfloat16* dst,
-                          const TcConvSpec& sp, int n_windows, int rows_stride, cudaStream_t st) {
-  const int rows_used = tc_rows_total(n_windows, sp.rows_per_window);  // <= rows_stride
+                          const TcConvSpec& sp, const TcRows& rows, int n_windows, int rows_stride, cudaStream_t st) {
+  const int rows_used = tc_rows_used(rows.n_rows);  // <= rows_stride
   const long long cells = (long long)rows_used * (sp.chunks8 / 2);  // a thread converts two chunks of a row
-  lognorm_split_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(y, minmax, bn, dst, n_windows, rows_used, rows_stride,
-                                                                       sp.chunks8, sp.rows_per_window, sp.lead_rows);
+  lognorm_split_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(y, minmax, bn, dst, rows.map, n_windows, rows_used,
+                                                                       rows_stride, sp.chunks8, sp.lead_rows);
 }
 
-size_t tc_edge_floats(const TcConvSpec& sp, int n_windows) {
+size_t tc_edge_floats(const TcConvSpec& sp, int n_windows) {  // (a trimmed row map has fewer rows than the uniform one)
   const int ms = tc::kMTile - (sp.KH2 - 1);
   const int n_mtiles = (n_windows * sp.rows_per_window + ms - 1) / ms;
   return (size_t)(sp.n_ft() - 1) * 2 * sp.edge_per_side() * ((size_t)n_mtiles * ms);  // one slot per tile boundary
@@ -1510,6 +1558,10 @@ static void tc_group_costs(int layer, std::vector<double>& cost, double& item) {
 }
 
 TcSchedule tc_schedule(int layer, bool fused, int n_windows, int n_sms, int* ms_out) {
+  return tc_schedule_rows(layer, fused, n_windows * tc_spec(layer).rows_per_window, n_sms, ms_out);
+}
+
+TcSchedule tc_schedule_rows(int layer, bool fused, int n_rows, int n_sms, int* ms_out) {
   const TcConvSpec sp = tc_spec(layer);
   const int h2 = fused || layer != 0 ? (sp.KH2 - 1) / 2 : 0;
   const int ms = tc::kMTile - 2 * h2;
@@ -1521,7 +1573,7 @@ TcSchedule tc_schedule(int layer, bool fused, int n_windows, int n_sms, int* ms_
   std::vector<double> pre(G + 1, 0.0);
   for (int g = 0; g < G; ++g) pre[g + 1] = pre[g] + cost[g];
   TcSchedule s{};
-  s.n_mtiles = (n_windows * sp.rows_per_window + ms - 1) / ms;
+  s.n_mtiles = (n_rows + ms - 1) / ms;
   s.n_full = s.n_mtiles / n_sms * n_sms;
   s.n_tail = s.n_mtiles - s.n_full;
   s.n_ranges = 1;
@@ -1571,10 +1623,11 @@ static void launch_layer(const TcArgs& a, const EdgeFixArgs& ef, int grid, cudaS
   }
 }
 
-void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& o, int n_windows, int rows_stride,
-                    int n_sms, cudaStream_t st, bool fuse_next) {
+void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut& o, int n_windows, const TcRows& rows,
+                    int rows_stride, int n_sms, cudaStream_t st, bool fuse_next) {
   const TcConvSpec sp = tc_spec(dev.layer);
   const bool fused = dev.layer != 0 || fuse_next;
+  if (rows.n_rows <= 0) return;  // (trimmed: no window keeps a frame)
   TcArgs a{};
   a.data = data;
   a.tiles = dev.tiles;
@@ -1585,9 +1638,12 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   a.h2 = fused ? (sp.KH2 - 1) / 2 : 0;
   // An item is (M-tile, range of frequency groups): whole M-tiles, the same number per CTA, then the last M-tiles cut
   // into group ranges of balanced cost (tc_schedule)
-  a.sch = tc_schedule(dev.layer, fused, n_windows, n_sms, &a.ms);
+  a.sch = tc_schedule_rows(dev.layer, fused, rows.n_rows, n_sms, &a.ms);
   a.edge_rows = a.sch.n_mtiles * a.ms;
   a.n_windows = n_windows;
+  a.map = rows.map;
+  a.lo1 = rows.lo1;
+  a.lo2 = rows.lo2;
   a.row0 = sp.lead_rows - sp.PT - a.h2;
   a.chunks8 = sp.chunks8;
   std::copy_n(dev.bias1, 32, a.bias1);
@@ -1628,7 +1684,9 @@ void launch_conv_tc(const __nv_bfloat16* data, const TcConvDev& dev, const TcOut
   EdgeFixArgs ef{};
   ef.o = o;
   ef.edge_rows = a.edge_rows;
-  ef.n_rows = n_windows * sp.rows_per_window;
+  ef.n_rows = rows.n_rows;
+  ef.map = rows.map;
+  ef.lo2 = rows.lo2;
   ef.edges_full = tc_edge_mask(sp, 1u);  // the conv kernel's own range predicate
   ef.edges_tail = tc_edge_mask(sp, a.sch.tail_starts());
   ef.tail_row0 = a.sch.n_full * a.ms;

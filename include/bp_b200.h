@@ -1062,6 +1062,14 @@ int bp_debug_tc_b2(int which, const float* w2, int32_t* sizes, uint16_t* tiles);
  * (edges[0]) and in the rows of cut M-tiles (edges[1]). */
 int bp_debug_tc_schedule(int which, int fused, int n_windows, int n_sms, int32_t* sizes, int32_t* items, uint32_t* edges);
 
+/* Host-only: the row map of a tensor-core layer for n_windows windows (csrc/tc_conv.cu, tc_row_map), which = 0 contour,
+ * 1 onset, 2 note.  trimmed = 0: the uniform map of whole windows (bp_forward_*); else the trimmed map the unwrapping
+ * entry points run on path 1, kept[b] = the centre frames window b keeps (<= 0: none).  map (may be NULL when
+ * n_windows = 0): [n_windows][3] = {base, first, rows}: input rows [base, base + rows) of the layer's row space hold
+ * frames first .. first + rows - 1 of window b; info[3] = {rows of the row space, lo1, lo2}: conv1 row / output frame i
+ * of a window is computed for use iff lo1 / lo2 <= i < rows - lo1 / lo2. */
+int bp_debug_tc_row_map(int which, int trimmed, const int32_t* kept, int32_t n_windows, int32_t* map, int32_t* info);
+
 /* Per-kernel device timing for the roofline line of bench.py: records CUDA events on the launching
  * stream around every launch of one kernel family (0 = contour conv 3x39, 1 = onset conv 5x5,
  * 2 = CQT projection + log-normalise, 3 = decimation chain, 4 = the remaining small convs,
